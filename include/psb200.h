@@ -125,6 +125,12 @@ typedef struct psb_model {
 	float* xyz_gradient_accum;/* [P,1] or NULL */
 	float* denom;             /* [P,1] or NULL */
 	int* exist_since_iter;    /* [P] int32 or NULL (GaussianModel::exist_since_iter_; only the densify / prune / insert entry points move it) */
+	unsigned char* adam_live; /* [P] bytes or NULL: "the moments of this row may be non-zero". Contract: adam_live[i] == 0 implies that all
+	                             118 moment floats of row i are exactly zero (a 1 may stand for zero moments too). psb_trainer_step then
+	                             reads and updates nothing of a row whose byte is 0 and that no gradient reaches (Adam is an exact no-op on
+	                             it), and sets the byte of every row it updates with a non-zero gradient. Anything else that writes moments
+	                             must leave the contract intact or be followed by psb_adam_live_rebuild. NULL: the moments themselves are
+	                             read to find such rows. Every other entry point ignores the field. */
 } psb_model;
 
 typedef struct psb_camera {
@@ -158,6 +164,9 @@ int psb_trainer_render(psb_trainer* t, int P, int M, const psb_model* model, con
 int psb_trainer_step(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
                      const float* background, const float* gt_image, const float* mask, const psb_step* step,
                      float* out_color, int* radii, void* stream);
+/* model->adam_live[i] = 1 if any of the 118 moments of row i is non-zero, else 0: one pass over the moments. Restores the
+ * psb_model.adam_live contract after moments were written by anything but psb_trainer_step. Asynchronous on `stream`. */
+int psb_adam_live_rebuild(int P, const psb_model* model, void* stream);
 
 /* Data-parallel halves of the same iteration: psb_trainer_backward writes the gradients w.r.t. the RAW
  * parameters into grads[0..5] (shapes of psb_model.param; every row written, zeros for invisible Gaussians)

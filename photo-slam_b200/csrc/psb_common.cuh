@@ -286,5 +286,14 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
 	             "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
 	             : "memory");
 }
+// 4-byte asynchronous copy global -> shared (SASS LDGSTS): no register staging; complete (for the issuing thread) after cp_async_wait_all
+__device__ __forceinline__ void cp_async4(void* smem_dst, const void* gmem_src)
+{
+	asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all()
+{
+	asm volatile("cp.async.wait_all;" ::: "memory");
+}
 
 }  // namespace psb

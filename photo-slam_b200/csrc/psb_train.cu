@@ -38,6 +38,8 @@ struct AdamCoef { float beta1, beta2, eps, inv_bc1, inv_bc2_sqrt; };
 constexpr int MODE_GRADS = 0;  // dense gradients of the raw parameters -> `grads` (NCCL data-parallel path / tests)
 constexpr int MODE_ADAM = 1;   // fused single-GPU step: parameters and moments updated in place
 constexpr int MODE_PUSH = 2;   // NVLink data-parallel step: 80-byte gradient records pushed into the owner rank's inbox
+constexpr int MODE_ADAM_LIVE = 3;  // MODE_ADAM with the caller's per-row live byte (psb_model.adam_live): rows that are neither live nor
+                                   // reached by a gradient are not read beyond that byte and the visibility word
 
 // torch::optim::Adam single-tensor update (LibTorch adam.cpp): exp_avg.mul_(b1).add_(g, 1-b1);
 // exp_avg_sq.mul_(b2).addcmul_(g, g, 1-b2); denom = exp_avg_sq.sqrt()/sqrt(bc2) + eps; p.addcdiv_(exp_avg, denom, -lr/bc1).
@@ -61,16 +63,27 @@ __device__ __forceinline__ void adam1(float& p, float& m, float& v, float g, flo
 // frest_stream_kernel expands them. The f_rest parameter rows the SH backward has to READ (view-direction term of
 // dL/dxyz) arrive by one TMA bulk copy per block; each thread walks its own row in shared memory (row stride 45 words:
 // bank-conflict free).
+//
+// MODE_ADAM_LIVE (contract of psb_model.adam_live: byte 0 => all 118 moments of the row are zero) reads per row first the live
+// byte and the visibility word, then only what the row needs: visible rows their screen-space sums, render meta word and
+// densification statistics; live rows (and rows whose sums are non-zero) their 14 small parameters and, for live rows, their 28
+// moments (a row reached for the first time starts from the zero moments the contract guarantees). The f_rest rows are staged
+// only for rows with non-zero sums — the only rows whose view-direction term of dL/dxyz can be non-zero — each warp copying its
+// own rows with 4-byte async copies into a compacted region of s_p (one coalesced 180-byte run per row; the whole-block TMA copy
+// would move every row, since nearly every block holds some live row). Seed rows are written, and updated by
+// frest_stream_kernel, only for rows that are live after this step; the live byte is set for every row that received a gradient.
 template <int MODE>
 __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(int first, int P, TrainTensors t, Camera cam, GeomState geom, float4* __restrict__ sink,
                                                             StepHyper h, GradSegments grads, DensifyStats st,
                                                             const uint32_t* __restrict__ counters, uint32_t capacity, float4* __restrict__ seeds,
-                                                            DpPush dp)
+                                                            DpPush dp, unsigned char* __restrict__ adam_live)
 {
-	constexpr bool ADAM = MODE == MODE_ADAM;
-	__shared__ __align__(128) float s_p[TB * REST];  // f_rest parameter rows of this block (TMA destination)
+	constexpr bool LIVE = MODE == MODE_ADAM_LIVE;
+	constexpr bool ADAM = MODE == MODE_ADAM || LIVE;
+	__shared__ __align__(128) float s_p[TB * REST];  // f_rest parameter rows of this block (TMA destination; LIVE: compacted per warp)
 	__shared__ __align__(16) float s_w[TB][SEED];    // seed rows of this block (copied out 128-bit coalesced at the end)
 	__shared__ __align__(8) uint64_t s_bar;
+	__shared__ bool s_live[LIVE ? TB : 1];           // LIVE: the row is live after this step (its seed row is written)
 
 	// A binning arena that turned out too small leaves the tile lists incomplete. Fused step: no-op (the host sees the
 	// same counter, grows the arena and repeats the step). Data-parallel modes: this view contributes a ZERO gradient to
@@ -86,14 +99,14 @@ __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(
 	const int rem_floats = (int)(row_bytes & 15u) / 4;
 	const size_t goff = (size_t)base * REST;
 
-	if (tid == 0) {
+	if (!LIVE && tid == 0) {
 		mbar_init(&s_bar, 1);
 		mbar_fence_init();
 		mbar_arrive_expect_tx(&s_bar, bulk_bytes);
 		bulk_g2s(s_p, t.p[2] + goff, bulk_bytes, &s_bar);
 		for (int i = 0; i < rem_floats; i++) s_p[bulk_bytes / 4 + i] = t.p[2][goff + bulk_bytes / 4 + i];  // < 16 trailing bytes (last block)
 	}
-	__syncthreads();  // the mbarrier must be initialised before any other thread waits on it
+	if (!LIVE) __syncthreads();  // the mbarrier must be initialised before any other thread waits on it
 
 	const int idx = base + tid;
 	const bool valid = idx < P;
@@ -116,29 +129,78 @@ __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(
 	float m3[3][3], v3[3][3], mo = 0.f, vo = 0.f;
 	float4 mr = make_float4(0, 0, 0, 0), vr = mr;
 	float st_rad = 0.f, st_acc = 0.f, st_den = 0.f;
-	if (valid) {
-		if (ADAM) {
-			const int tsel[3] = {0, 1, 4};
+	bool was_live = false, staged = false;  // LIVE: live byte before this step | f_rest row staged (non-zero sums)
+	int rest_slot = tid;                    // this row's f_rest row in s_p
+	float4 s0 = make_float4(0, 0, 0, 0), s1 = s0, s2 = s0;
+	uint32_t meta = 0;
+	auto load_moments = [&]() {
+		const int tsel[3] = {0, 1, 4};
 #pragma unroll
-			for (int a = 0; a < 3; a++)
+		for (int a = 0; a < 3; a++)
 #pragma unroll
-				for (int c = 0; c < 3; c++) { m3[a][c] = t.m[tsel[a]][3 * idx + c]; v3[a][c] = t.v[tsel[a]][3 * idx + c]; }
-			mo = t.m[3][idx]; vo = t.v[3][idx];
-			mr = reinterpret_cast<const float4*>(t.m[5])[idx]; vr = reinterpret_cast<const float4*>(t.v[5])[idx];
-		}
-		if (st.enabled) { st_rad = st.max_radii2D[idx]; st_acc = st.xyz_gradient_accum[idx]; st_den = st.denom[idx]; }
-		const uint32_t tt = geom.tile_info[idx].z;
-		const float4 s0 = sink[3 * idx], s1 = sink[3 * idx + 1], s2 = sink[3 * idx + 2];
-		const uint32_t meta = __float_as_uint(geom.rec[idx].q2.w);
+			for (int c = 0; c < 3; c++) { m3[a][c] = t.m[tsel[a]][3 * idx + c]; v3[a][c] = t.v[tsel[a]][3 * idx + c]; }
+		mo = t.m[3][idx]; vo = t.v[3][idx];
+		mr = reinterpret_cast<const float4*>(t.m[5])[idx]; vr = reinterpret_cast<const float4*>(t.v[5])[idx];
+	};
+	auto load_params = [&]() {
 #pragma unroll
 		for (int c = 0; c < 3; c++) { sp_xyz[c] = t.p[0][3 * idx + c]; sp_dc[c] = t.p[1][3 * idx + c]; sp_sc[c] = t.p[4][3 * idx + c]; }
 		sp_op = t.p[3][idx];
 		sp_rot = reinterpret_cast<const float4*>(t.p[5])[idx];
-		visible = tt != 0 && !overflow;
-		// ready for the next iteration (rows nothing was added to — culled or hidden Gaussians — are zero already: not rewritten)
-		const bool sink_dirty = s0.x != 0.f || s0.y != 0.f || s0.w != 0.f || s1.x != 0.f || s1.z != 0.f || s1.w != 0.f || s2.x != 0.f || s2.y != 0.f || s2.z != 0.f;
-		if (sink_dirty) { const float4 z = make_float4(0, 0, 0, 0); sink[3 * idx] = z; sink[3 * idx + 1] = z; sink[3 * idx + 2] = z; }
-		if (visible) {
+	};
+	if (LIVE) {
+#pragma unroll
+		for (int a = 0; a < 3; a++)
+#pragma unroll
+			for (int c = 0; c < 3; c++) { m3[a][c] = 0.f; v3[a][c] = 0.f; }
+		if (valid) {
+			was_live = adam_live[idx] != 0;
+			visible = geom.tile_info[idx].z != 0;  // (an overflowing step has returned above)
+			if (was_live) load_params();  // (the moments are loaded after the backward: fewer registers held across it)
+			if (visible) {
+				if (st.enabled) { st_rad = st.max_radii2D[idx]; st_acc = st.xyz_gradient_accum[idx]; st_den = st.denom[idx]; }
+				s0 = sink[3 * idx]; s1 = sink[3 * idx + 1]; s2 = sink[3 * idx + 2];
+				meta = __float_as_uint(geom.rec[idx].q2.w);
+				// only visible rows were added to; the others are zero since the last step
+				staged = s0.x != 0.f || s0.y != 0.f || s0.w != 0.f || s1.x != 0.f || s1.z != 0.f || s1.w != 0.f || s2.x != 0.f || s2.y != 0.f || s2.z != 0.f;
+				if (staged) { const float4 z = make_float4(0, 0, 0, 0); sink[3 * idx] = z; sink[3 * idx + 1] = z; sink[3 * idx + 2] = z; }
+				if (staged && !was_live) load_params();  // first gradient of this row: its moments are zero by contract, not read
+				if (st.enabled) {  // (here: fewer registers held across the backward)
+					st.max_radii2D[idx] = fmaxf(st_rad, (float)rec_radius(meta));
+					st.xyz_gradient_accum[idx] = st_acc + sqrtf(s0.x * s0.x + s0.y * s0.y);
+					st.denom[idx] = st_den + 1.0f;
+				}
+			}
+		}
+		// f_rest rows of the rows with non-zero sums -> this warp's 32-row region of s_p, compacted; the copies land while the
+		// geometry backward below runs
+		const int lane = tid & 31, wbase = tid & ~31;
+		const uint32_t ball = __ballot_sync(0xffffffffu, staged);
+		uint32_t b = ball;
+		for (int r = wbase; b != 0u; r++, b &= b - 1u) {
+			const float* src = t.p[2] + (size_t)(base + wbase + __ffs(b) - 1) * REST;
+			float* dst = s_p + r * REST;
+			cp_async4(dst + lane, src + lane);
+			if (lane < REST - 32) cp_async4(dst + 32 + lane, src + 32 + lane);
+		}
+		rest_slot = wbase + __popc(ball & ((1u << lane) - 1u));
+	}
+	if (valid) {
+		uint32_t tt = 0;
+		if (!LIVE) {
+			if (ADAM) load_moments();
+			if (st.enabled) { st_rad = st.max_radii2D[idx]; st_acc = st.xyz_gradient_accum[idx]; st_den = st.denom[idx]; }
+			tt = geom.tile_info[idx].z;
+			s0 = sink[3 * idx]; s1 = sink[3 * idx + 1]; s2 = sink[3 * idx + 2];
+			meta = __float_as_uint(geom.rec[idx].q2.w);
+			load_params();
+			visible = tt != 0 && !overflow;
+			// ready for the next iteration (rows nothing was added to — culled or hidden Gaussians — are zero already: not rewritten)
+			const bool sink_dirty = s0.x != 0.f || s0.y != 0.f || s0.w != 0.f || s1.x != 0.f || s1.z != 0.f || s1.w != 0.f || s2.x != 0.f || s2.y != 0.f || s2.z != 0.f;
+			if (sink_dirty) { const float4 z = make_float4(0, 0, 0, 0); sink[3 * idx] = z; sink[3 * idx + 1] = z; sink[3 * idx + 2] = z; }
+		}
+		// LIVE: a visible row with zero sums has zero gradients (and may not have its parameters loaded): statistics only
+		if (visible && (!LIVE || staged)) {
 			// sink row: [0,1] mean2D.xy | [3,4,6] conic.xyw | [7] opacity | [8,9,10] rgb
 			const float2 dL_dmean2D = make_float2(s0.x, s0.y);
 			const float3 dL_dconic = make_float3(s0.w, s1.x, s1.z);
@@ -166,26 +228,32 @@ __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(
 			const float qd = q.x * dL_drot.x + q.y * dL_drot.y + q.z * dL_drot.z + q.w * dL_drot.w;
 			g_rot = make_float4((dL_drot.x - q.x * qd) / qn, (dL_drot.y - q.y * qd) / qn, (dL_drot.z - q.z * qd) / qn, (dL_drot.w - q.w * qd) / qn);
 			g_opac = dL_dopacity * sig * (1.0f - sig);
-			if (st.enabled) {
-				st.max_radii2D[idx] = fmaxf(st_rad, (float)rec_radius(meta));
-				st.xyz_gradient_accum[idx] = st_acc + sqrtf(dL_dmean2D.x * dL_dmean2D.x + dL_dmean2D.y * dL_dmean2D.y);
-				st.denom[idx] = st_den + 1.0f;
-			}
+		}
+		// every visible row counts, hidden ones included (the reference's denom counts them too)
+		if (!LIVE && visible && st.enabled) {
+			st.max_radii2D[idx] = fmaxf(st_rad, (float)rec_radius(meta));
+			st.xyz_gradient_accum[idx] = st_acc + sqrtf(s0.x * s0.x + s0.y * s0.y);
+			st.denom[idx] = st_den + 1.0f;
 		}
 	}
 
-	mbar_wait(&s_bar, 0);  // f_rest rows have landed
-	__syncthreads();       // (also publishes thread 0's trailing plain stores)
+	if (LIVE) {
+		cp_async_wait_all();  // this thread's copies have landed ...
+		__syncwarp();         // ... and every lane's: each warp reads only its own region of s_p
+	} else {
+		mbar_wait(&s_bar, 0);  // f_rest rows have landed
+		__syncthreads();       // (also publishes thread 0's trailing plain stores)
+	}
 
 	// ---- phase 1b: SH backward seeds; the view-direction term completes dL/dxyz
 	float3 g_dc = make_float3(0, 0, 0);
 	{
-		const float* rp = s_p + tid * REST;
+		const float* rp = s_p + rest_slot * REST;
 		float w[16];
 #pragma unroll
 		for (int k = 0; k < 16; k++) w[k] = 0.f;
 		float gm[3] = {0.f, 0.f, 0.f};
-		if (visible) {
+		if (LIVE ? staged : visible) {
 			const float3 campos = make_float3(cam.campos[0], cam.campos[1], cam.campos[2]);
 			const float3 sh_dmean = sh_backward_t(
 				h.D, mean, campos, clamp_bits, dL_dcolor,
@@ -223,7 +291,16 @@ __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(
 	if (valid) {
 		// a zero gradient on zero moments is an exact no-op of Adam (see frest_stream_kernel): hidden / never-reached Gaussians are not rewritten
 		bool idle = false;
-		if (ADAM) {
+		if (LIVE) {
+			// the f_rest gradient is w_k * masked dL/dRGB: zero unless one of gm (in the seed row) is non-zero
+			const bool gnz = g_xyz.x != 0.f || g_xyz.y != 0.f || g_xyz.z != 0.f || g_dc.x != 0.f || g_dc.y != 0.f || g_dc.z != 0.f || g_scale.x != 0.f ||
+			                 g_scale.y != 0.f || g_scale.z != 0.f || g_opac != 0.f || g_rot.x != 0.f || g_rot.y != 0.f || g_rot.z != 0.f || g_rot.w != 0.f ||
+			                 s_w[tid][16] != 0.f || s_w[tid][17] != 0.f || s_w[tid][18] != 0.f;
+			if (gnz && !was_live) adam_live[idx] = 1;
+			idle = !(gnz || was_live);
+			s_live[tid] = !idle;
+			if (was_live) load_moments();
+		} else if (ADAM) {
 			bool nz = g_xyz.x != 0.f || g_xyz.y != 0.f || g_xyz.z != 0.f || g_dc.x != 0.f || g_dc.y != 0.f || g_dc.z != 0.f || g_scale.x != 0.f ||
 			          g_scale.y != 0.f || g_scale.z != 0.f || g_opac != 0.f || g_rot.x != 0.f || g_rot.y != 0.f || g_rot.z != 0.f || g_rot.w != 0.f ||
 			          mo != 0.f || vo != 0.f || mr.x != 0.f || mr.y != 0.f || mr.z != 0.f || mr.w != 0.f || vr.x != 0.f || vr.y != 0.f || vr.z != 0.f || vr.w != 0.f;
@@ -269,7 +346,8 @@ __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(
 		// seed rows of this block -> global, 128-bit coalesced
 		const float4* src = reinterpret_cast<const float4*>(&s_w[0][0]);
 		float4* dst = seeds + (size_t)base * (SEED / 4);
-		for (int i = tid; i < rows * (SEED / 4); i += TB) dst[i] = src[i];
+		for (int i = tid; i < rows * (SEED / 4); i += TB)
+			if (!LIVE || s_live[i / (SEED / 4)]) dst[i] = src[i];  // (LIVE: frest_stream_kernel reads no seed row of a row that is not live)
 		return;
 	}
 	// MODE_PUSH: the block's records go straight into the inbox of the rank that owns this 128-Gaussian chunk (remote
@@ -308,23 +386,31 @@ __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(
 
 // Adam over the f_rest rows of Gaussians [first, P) (ADAM) or their gradient written out
 // (!ADAM), one float4 per thread. The gradient of element (row, k, ch) is seed[row][k-1] * seed[row][16+ch].
+// ADAM with `live` (psb_model.adam_live, as left by gaussian_backward_kernel<MODE_ADAM_LIVE>): a row whose byte is 0 has zero
+// moments and no gradient (and no seed row written in this step): its elements are a no-op, the thread reads nothing else for them.
 template <bool ADAM>
 __global__ void __launch_bounds__(256) frest_stream_kernel(uint32_t e_first, uint32_t e_end, float* __restrict__ p, float* __restrict__ m, float* __restrict__ v,
                                                            float* __restrict__ gout, const float* __restrict__ seeds, float lr_eff, AdamCoef ac,
-                                                           const uint32_t* __restrict__ counters, uint32_t capacity)
+                                                           const uint32_t* __restrict__ counters, uint32_t capacity, const unsigned char* __restrict__ live)
 {
 	if (ADAM && counters[0] > capacity) return;  // overflowing fused step: no-op (see gaussian_backward_kernel; !ADAM: the seeds are zero)
 	const uint32_t e = e_first + 4u * (blockIdx.x * 256u + threadIdx.x);
 	if (e >= e_end) return;
 	uint32_t row = e / REST;
 	int c = (int)(e - row * REST);
+	bool lv = true, lv_next = true;  // the float4 covers one row or the end of one and the start of the next
+	if (ADAM && live) {
+		lv = live[row] != 0;
+		lv_next = live[min(e + 3u, e_end - 1u) / REST] != 0;
+		if (!lv && !lv_next) return;
+	}
 	const float* sd = seeds + (size_t)row * SEED;
 	float g[4];
 #pragma unroll
 	for (int j = 0; j < 4; j++) {
 		const int k = c / 3, ch = c - 3 * k;
-		g[j] = sd[k] * sd[16 + ch];
-		if (++c == REST) { c = 0; sd += SEED; }
+		g[j] = lv ? sd[k] * sd[16 + ch] : 0.f;
+		if (++c == REST) { c = 0; sd += SEED; lv = lv_next; }
 	}
 	if (e + 4 <= e_end) {
 		if (ADAM) {
@@ -348,6 +434,23 @@ __global__ void __launch_bounds__(256) frest_stream_kernel(uint32_t e_first, uin
 			else gout[e + j] = g[j];
 		}
 	}
+}
+
+// live[i] = any of the 118 moments of row i is non-zero (psb_adam_live_rebuild: repairs psb_model.adam_live after the moments were
+// written by anything other than the fused step). One thread per row; not on the per-iteration path.
+__global__ void __launch_bounds__(256) adam_live_rebuild_kernel(int P, TrainTensors t, unsigned char* __restrict__ live)
+{
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= P) return;
+	const int width[6] = {3, 3, REST, 1, 3, 4};
+	bool nz = false;
+#pragma unroll
+	for (int q = 0; q < 6; q++) {
+		const float* m = t.m[q] + (size_t)i * width[q];
+		const float* v = t.v[q] + (size_t)i * width[q];
+		for (int k = 0; k < width[q]; k++) nz = nz || m[k] != 0.f || v[k] != 0.f;
+	}
+	live[i] = nz ? 1 : 0;
 }
 
 // Plain Adam over one flat tensor (data-parallel path, after the gradient all-reduce). 128-bit accesses.
@@ -649,7 +752,7 @@ __global__ void wait_flags_kernel(const uint32_t* flags, int world, uint32_t epo
 
 int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, float* seeds,
                           const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
-                          cudaStream_t stream, cudaEvent_t between)
+                          cudaStream_t stream, cudaEvent_t between, unsigned char* adam_live)
 {
 	if (P - first <= 0) return 0;
 	const int grid = cdiv(P - first, TB);
@@ -659,16 +762,26 @@ int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, co
 	if ((size_t)P * REST >= (size_t)UINT32_MAX - 8) { set_error_msg("psb_trainer: too many Gaussians for 32-bit element indices"); return -1; }
 	DpPush nodp;
 	memset(&nodp, 0, sizeof(nodp));
-	if (adam) gaussian_backward_kernel<MODE_ADAM><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp);
-	else gaussian_backward_kernel<MODE_GRADS><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp);
+	unsigned char* live = adam ? adam_live : nullptr;
+	if (live) gaussian_backward_kernel<MODE_ADAM_LIVE><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, live);
+	else if (adam) gaussian_backward_kernel<MODE_ADAM><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, nullptr);
+	else gaussian_backward_kernel<MODE_GRADS><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, nullptr);
 	PSB_LAUNCH_OK();
 	if (between) cudaEventRecord(between, stream);
 	AdamCoef ac;
 	ac.beta1 = h.beta1; ac.beta2 = h.beta2; ac.eps = h.eps; ac.inv_bc1 = h.inv_bc1; ac.inv_bc2_sqrt = 1.0f / h.bc2_sqrt;
 	const uint32_t e0 = (uint32_t)first * REST, e1 = (uint32_t)P * REST;
 	const unsigned gridB = (unsigned)(((size_t)(e1 - e0) + 1023) / 1024);
-	if (adam) frest_stream_kernel<true><<<gridB, 256, 0, stream>>>(e0, e1, t.p[2], t.m[2], t.v[2], nullptr, seeds, h.lr[2] * ac.inv_bc1, ac, counters, capacity);
-	else frest_stream_kernel<false><<<gridB, 256, 0, stream>>>(e0, e1, nullptr, nullptr, nullptr, grads.g[2], seeds, 0.f, ac, counters, capacity);
+	if (adam) frest_stream_kernel<true><<<gridB, 256, 0, stream>>>(e0, e1, t.p[2], t.m[2], t.v[2], nullptr, seeds, h.lr[2] * ac.inv_bc1, ac, counters, capacity, live);
+	else frest_stream_kernel<false><<<gridB, 256, 0, stream>>>(e0, e1, nullptr, nullptr, nullptr, grads.g[2], seeds, 0.f, ac, counters, capacity, nullptr);
+	PSB_LAUNCH_OK();
+	return 0;
+}
+
+int launch_adam_live_rebuild(int P, const TrainTensors& t, unsigned char* live, cudaStream_t stream)
+{
+	if (P <= 0) return 0;
+	adam_live_rebuild_kernel<<<cdiv(P, 256), 256, 0, stream>>>(P, t, live);
 	PSB_LAUNCH_OK();
 	return 0;
 }
@@ -680,7 +793,7 @@ int launch_push_backward(int first, int P, const TrainTensors& t, const Camera& 
 	memset(&nog, 0, sizeof(nog));
 	if (P - first > 0) {  // Gaussians [first, P): one pipeline group (first is a multiple of 128 * world)
 		gaussian_backward_kernel<MODE_PUSH><<<cdiv(P - first, TB), TB, 0, stream>>>(first, P, t, cam, geom, reinterpret_cast<float4*>(sink), h, nog, st, counters,
-		                                                                          capacity, nullptr, dp);
+		                                                                          capacity, nullptr, dp, nullptr);
 		PSB_LAUNCH_OK();
 	}
 	if (!dp.fence_in_kernel) {

@@ -69,7 +69,10 @@ int launch_wait_flags(const uint32_t* flags, int world, uint32_t epoch, uint32_t
 // seeds: scratch [P][20] floats (per-Gaussian SH gradient seeds handed from the per-Gaussian kernel to the f_rest stream kernel)
 int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, float* seeds,
                           const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
-                          cudaStream_t stream, cudaEvent_t between = nullptr /* recorded between the two kernels (stage timing) */);
+                          cudaStream_t stream, cudaEvent_t between = nullptr /* recorded between the two kernels (stage timing) */,
+                          unsigned char* adam_live = nullptr /* adam only: psb_model.adam_live, or null (the moments tell idle rows) */);
+// adam_live[i] = any moment of row i non-zero (t.m / t.v: the 12 moment tensors)
+int launch_adam_live_rebuild(int P, const TrainTensors& t, unsigned char* adam_live, cudaStream_t stream);
 int launch_adam(size_t n, float* p, float* m, float* v, const float* g, float lr, const StepHyper& h, float grad_scale, cudaStream_t stream);
 int launch_loss(int H, int W, const float* img, const float* gt, const float* mask, float lambda_dssim, float* dmap, double* sums,
                 float* dL_dimg, cudaStream_t stream);

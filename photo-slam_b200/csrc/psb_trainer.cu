@@ -222,7 +222,7 @@ int step_impl(psb_trainer* t, int P, int M, const psb_model* model, const psb_ca
 	st.max_radii2D = model->max_radii2D; st.xyz_gradient_accum = model->xyz_gradient_accum; st.denom = model->denom;
 	const StepHyper h = to_hyper(step);
 	rc = launch_fused_backward(grads == nullptr, 0, P, tt, cam, geom, t->sink, t->seeds, h, gs, st, geom.counters, (uint32_t)t->capacity, stream,
-	                           (t->profiling && t->ev_ready) ? t->ev[7] : nullptr);
+	                           (t->profiling && t->ev_ready) ? t->ev[7] : nullptr, grads == nullptr ? model->adam_live : nullptr);
 	t->mark(8, stream);
 	t->last_stage = 8;
 	t->ev_recorded = t->profiling && t->ev_ready;
@@ -486,6 +486,16 @@ int psb_trainer_step(psb_trainer* t, int P, int M, const psb_model* model, const
                      const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, void* stream_)
 {
 	return step_impl(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, nullptr, (cudaStream_t)stream_);
+}
+
+int psb_adam_live_rebuild(int P, const psb_model* model, void* stream_)
+{
+	int rc;
+	if ((rc = check_model(P, 16, model, true))) return rc;
+	if (P > 0 && !model->adam_live) { set_error_msg("psb_adam_live_rebuild: model->adam_live is NULL"); return PSB_ERR_ARG; }
+	TrainTensors tt;
+	for (int i = 0; i < 6; i++) { tt.p[i] = model->param[i]; tt.m[i] = model->exp_avg[i]; tt.v[i] = model->exp_avg_sq[i]; }
+	return launch_adam_live_rebuild(P, tt, model->adam_live, (cudaStream_t)stream_);
 }
 
 int psb_trainer_backward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,

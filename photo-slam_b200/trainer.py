@@ -23,7 +23,8 @@ GROUPS = ("xyz", "features_dc", "features_rest", "opacity", "scaling", "rotation
 
 class _Model(C.Structure):
     _fields_ = [("param", C.c_void_p * 6), ("exp_avg", C.c_void_p * 6), ("exp_avg_sq", C.c_void_p * 6),
-                ("max_radii2D", C.c_void_p), ("xyz_gradient_accum", C.c_void_p), ("denom", C.c_void_p), ("exist_since_iter", C.c_void_p)]
+                ("max_radii2D", C.c_void_p), ("xyz_gradient_accum", C.c_void_p), ("denom", C.c_void_p), ("exist_since_iter", C.c_void_p),
+                ("adam_live", C.c_void_p)]
 
 
 class _Camera(C.Structure):
@@ -66,7 +67,9 @@ def _bind():
     L.psb_prune_apply.argtypes = [C.c_int, C.POINTER(_Model), C.POINTER(_Model), C.c_int, vp, C.c_int, vp]
     L.psb_insert_points.argtypes = [C.c_int, C.POINTER(_Model), C.POINTER(_Model), C.c_int, vp, vp, vp, C.c_int, vp]
     L.psb_reset_opacity.argtypes = [C.c_int, vp, vp, vp, vp]
-    for n in ("psb_densify_plan", "psb_densify_apply", "psb_prune_plan", "psb_prune_apply", "psb_insert_points", "psb_reset_opacity"):
+    L.psb_adam_live_rebuild.argtypes = [C.c_int, C.POINTER(_Model), vp]
+    for n in ("psb_densify_plan", "psb_densify_apply", "psb_prune_plan", "psb_prune_apply", "psb_insert_points", "psb_reset_opacity",
+              "psb_adam_live_rebuild"):
         getattr(L, n).restype = C.c_int
     L._trainer_bound = True
     return L
@@ -128,6 +131,10 @@ class GaussianModel:
         self.xyz_gradient_accum_, self.denom_, self.max_radii2D_ = z(P, 1), z(P, 1), z(P)
         self.exp_avg_ = [torch.zeros_like(t) for t in self.tensors()]
         self.exp_avg_sq_ = [torch.zeros_like(t) for t in self.tensors()]
+        # per row: "its moments may be non-zero" (psb_model.adam_live). The fused step keeps it exact; whatever else replaces or
+        # rewrites moments marks it stale and the next fused step rebuilds it from the moments first
+        self.adam_live_ = torch.zeros(P, dtype=torch.uint8, device=self.device)
+        self.adam_live_valid_ = True
         self.step_ = 0
         self.lr_ = [args.position_lr_init * self.spatial_lr_scale_, args.feature_lr, args.feature_lr / 20.0, args.opacity_lr,
                     args.scaling_lr, args.rotation_lr]
@@ -140,9 +147,10 @@ class GaussianModel:
     #     place so device pointers held elsewhere stay valid. Used by bench.py to time every leg on the same iterations.
     def snapshot(self):
         c = lambda ts: [t.clone() for t in ts]
+        live = self._live_tensor()
         return dict(p=c(self.tensors()), m=c(self.exp_avg_), v=c(self.exp_avg_sq_),
                     stats=c([self.xyz_gradient_accum_, self.denom_, self.max_radii2D_]), step=self.step_, lr=list(self.lr_),
-                    sh=self.active_sh_degree_)
+                    sh=self.active_sh_degree_, live=live.clone(), live_valid=self.adam_live_valid_)
 
     def restore(self, snap):
         assert snap["p"][0].shape == self.xyz_.shape, "restore: the model was resized since the snapshot"
@@ -150,6 +158,29 @@ class GaussianModel:
                             snap["p"] + snap["m"] + snap["v"] + snap["stats"]):
             dst.copy_(src)
         self.step_, self.lr_, self.active_sh_degree_ = snap["step"], list(snap["lr"]), snap["sh"]
+        self._live_tensor().copy_(snap["live"])
+        self.adam_live_valid_ = snap["live_valid"]
+
+    def _live_tensor(self):
+        """adam_live_, (re)allocated when the row count changed (its content is then stale)."""
+        if getattr(self, "adam_live_", None) is None or self.adam_live_.size(0) != self.num_points():
+            self.adam_live_ = torch.zeros(self.num_points(), dtype=torch.uint8, device=self.device)
+            self.adam_live_valid_ = False
+        return self.adam_live_
+
+    def invalidateAdamLive(self):
+        """Call after writing moments by any means other than the fused step (the next fused step rebuilds the live bytes)."""
+        self.adam_live_valid_ = False
+
+    def adamLive(self):
+        """adam_live_, rebuilt from the moments (psb_adam_live_rebuild) if it is stale."""
+        live = self._live_tensor()
+        if not self.adam_live_valid_:
+            m = self._cmodel()
+            m.adam_live = live.data_ptr()
+            _lib.check(_bind().psb_adam_live_rebuild(self.num_points(), C.byref(m), torch.cuda.current_stream().cuda_stream), "psb_adam_live_rebuild")
+            self.adam_live_valid_ = True
+        return live
 
     # --- on-disk point cloud (reference GaussianModel::savePly / loadPly / saveSparsePointsPly, gaussian_model.cpp:838-1088)
     def savePly(self, path):
@@ -163,6 +194,7 @@ class GaussianModel:
         t = lambda x: torch.from_numpy(x).to(self.device).contiguous()
         self._set([t(a[k]) for k in ("xyz", "features_dc", "features_rest", "opacity", "scaling", "rotation")])
         self.active_sh_degree_ = self.max_sh_degree_
+        self.invalidateAdamLive()
 
     def setSparsePoints(self, xyz, color):
         """sparse SLAM map points + colours in [0,1] kept for input.ply (reference gaussian_model.cpp: sparse_points_xyz_ / _color_)"""
@@ -239,6 +271,7 @@ class GaussianModel:
         self._set(d["p"])
         self.exp_avg_, self.exp_avg_sq_ = d["m"], d["v"]
         self.xyz_gradient_accum_, self.denom_, self.max_radii2D_, self.exist_since_iter_ = d["accum"], d["denom"], d["max_radii"], d["exist"]
+        self.invalidateAdamLive()   # rows moved: rebuilt from the new moments before the next fused step
 
     def resetOpacity(self):
         """reference gaussian_model.cpp:556-565. NOTE: the reference's misplaced parenthesis makes this
@@ -356,8 +389,11 @@ class GaussianModel:
             self.exp_avg_sq_[i] = torch.zeros_like(self.tensors()[i])
         return num_transformed
 
-    def _cmodel(self, with_state=True):
+    def _cmodel(self, with_state=True, live=None):
+        """live: adam_live_ (valid) for the fused step; every other caller passes NULL."""
         m = _Model()
+        if live is not None:
+            m.adam_live = live.data_ptr()
         for i, t in enumerate(self.tensors()):
             assert t.is_contiguous() and t.dtype == torch.float32
             m.param[i] = t.data_ptr()
@@ -432,7 +468,7 @@ class GaussianTrainer:
         self.iteration += 1
         if densify_stats is None:
             densify_stats = self.iteration < self.opt.densify_until_iter
-        cm, cc, cs = m._cmodel(), _ccamera(cam), self._cstep(densify_stats)
+        cm, cc, cs = m._cmodel(live=m.adamLive()), _ccamera(cam), self._cstep(densify_stats)
         _lib.check(self.L.psb_trainer_step(self.h, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(),
                                            gt_image.data_ptr(), mask.data_ptr() if mask is not None else None, C.byref(cs),
                                            out_color.data_ptr() if out_color is not None else None,
@@ -677,6 +713,7 @@ class DataParallelTrainer(GaussianTrainer):
         self.sync()
         m = self.model
         gather_owned_rows(m.exp_avg_ + m.exp_avg_sq_, self.rank, self.world, self.group)
+        m.invalidateAdamLive()
 
     def rebuild(self):
         """After the model was resized (densify / prune / insertion): new arena, new peer mappings."""
@@ -754,6 +791,7 @@ class DataParallelTrainer(GaussianTrainer):
                     _lib.check(self.L.psb_adam_flat(count * k, p[o:].data_ptr(), a[o:].data_ptr(), b[o:].data_ptr(), blk.data_ptr(), m.lr_[i],
                                                     C.byref(cs), scale, stream), "psb_adam_flat")
         m.step_ += 1
+        m.invalidateAdamLive()   # these steps write moments without maintaining the live bytes (and p2p: only on the owner rank)
         self._last = (cam, gt_image, mask, out_color, radii, densify_stats)
 
     def result(self):
