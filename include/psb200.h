@@ -164,6 +164,32 @@ int psb_trainer_render(psb_trainer* t, int P, int M, const psb_model* model, con
 int psb_trainer_step(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
                      const float* background, const float* gt_image, const float* mask, const psb_step* step,
                      float* out_color, int* radii, void* stream);
+/* ------------------------------------------------------------------------------------------------
+ * Depth. The rendered depth is the un-normalised expected depth D(p) = sum_i z_i alpha_i T_i (z_i = view-space depth of
+ * Gaussian i; alpha, T exactly those of the colour; no background term). Rendering it leaves the colour image, the final
+ * transmittance and the radii bit-identical. The depth loss (RGB-D keyframes) adds lambda_depth * depth_l1 to the loss:
+ *   valid(p) = gt_depth(p) > 0 and, with a mask, mask[0,p] != 0;  depth_l1 = sum_valid |D - G| / max(N_valid, 1)
+ * N_valid is counted on the device (no host synchronisation). The densification statistics include the depth term.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct psb_depth {
+	const float* gt_depth;  /* [H,W] device, metres, <= 0 = no measurement; NULL = no depth loss */
+	float lambda_depth;     /* finite, >= 0; > 0 exactly when gt_depth is given */
+	float* out_depth;       /* [H,W] device or NULL */
+} psb_depth;
+/* psb_trainer_render plus D -> out_depth [H,W] (device; NULL = psb_trainer_render). */
+int psb_trainer_render_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                             const float* background, int sh_degree, float* out_color, int* radii, float* out_depth, void* stream);
+/* psb_trainer_step / psb_trainer_backward with a depth term; depth == NULL is the plain call. PSB_ERR_ARG for a negative or
+ * non-finite lambda_depth, or gt_depth without lambda_depth > 0 (or the reverse). */
+int psb_trainer_step_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                           const float* background, const float* gt_image, const float* mask, const psb_step* step,
+                           float* out_color, int* radii, const psb_depth* depth, void* stream);
+int psb_trainer_backward_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                               const float* background, const float* gt_image, const float* mask, const psb_step* step,
+                               float* out_color, int* radii, float* const* grads, const psb_depth* depth, void* stream);
+/* psb_trainer_result with out4 = {loss, l1, ssim, depth_l1} (depth_l1 = 0 when the last step had no depth term). */
+int psb_trainer_result_depth(psb_trainer* t, float* out4, int* num_rendered, void* stream);
+
 /* model->adam_live[i] = 1 if any of the 118 moments of row i is non-zero, else 0: one pass over the moments. Restores the
  * psb_model.adam_live contract after moments were written by anything but psb_trainer_step. Asynchronous on `stream`. */
 int psb_adam_live_rebuild(int P, const psb_model* model, void* stream);

@@ -49,10 +49,12 @@ int launch_binning(int P, const Camera& cam, const GeomState& geom, BinState& bi
 int launch_scan_binning(int P, const Camera& cam, const GeomState& geom, BinState& bin, const ImgState& img, size_t capacity, bool tight,
                         uint32_t* ovf, uint32_t seq, cudaStream_t stream);
 int launch_render_forward(const Camera& cam, const uint2* ranges, const uint32_t* point_list, const GaussRec* rec, const float* bg,
-                          float* out_color, float* final_T, uint32_t* n_contrib, cudaStream_t stream);
+                          float* out_color, float* final_T, uint32_t* n_contrib, cudaStream_t stream,
+                          float* out_depth = nullptr /* [H,W]: also render the expected depth (depth variant of the kernel) */);
+// dL_ddepth [H,W] (trainer path, packed sink only): depth variant, dL/dz of every Gaussian lands in slot 11 of its sink row
 int launch_render_backward(const Camera& cam, const uint2* ranges, const uint32_t* point_list, const GaussRec* rec, const float* bg,
                            const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, const GradSink& sink,
-                           cudaStream_t stream);
+                           cudaStream_t stream, const float* dL_ddepth = nullptr);
 int launch_preprocess_backward(const GaussIn& in, const Camera& cam, const GeomState& geom, const float* dL_dmean2D, int mean2D_stride,
                                const float* dL_dconic, int conic_stride, const float* dL_dcolor, int color_stride,
                                const GaussGradOut& out, cudaStream_t stream);

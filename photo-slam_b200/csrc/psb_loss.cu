@@ -153,7 +153,51 @@ __global__ void __launch_bounds__(256) loss_bwd_kernel(int H, int W, const float
 	}
 }
 
+// Depth L1, pass 1 (grid-stride, 256 threads): per valid pixel |D - G| and sign(D - G) (-> dL_dD, scaled by pass 2); block sums of
+// |D - G| and of the valid count go to sums[0], sums[1] in double (the count is exact).
+__global__ void __launch_bounds__(256) depth_loss_kernel(int n, const float* __restrict__ D, const float* __restrict__ G, const float* __restrict__ mask,
+                                                         float* __restrict__ dL_dD, double* __restrict__ sums)
+{
+	__shared__ float s_red[8];
+	float acc = 0.f, cnt = 0.f;
+	for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) {
+		const float g = G[i];
+		const bool valid = g > 0.f && (!mask || mask[i] != 0.f);
+		float sgn = 0.f;
+		if (valid) {
+			const float d = D[i] - g;
+			acc += fabsf(d);
+			cnt += 1.f;
+			sgn = (d > 0.f) ? 1.f : ((d < 0.f) ? -1.f : 0.f);
+		}
+		dL_dD[i] = sgn;
+	}
+	const float tacc = block_sum_256(acc, s_red);
+	const float tcnt = block_sum_256(cnt, s_red);
+	if (threadIdx.x == 0) { atomicAdd(&sums[0], (double)tacc); atomicAdd(&sums[1], (double)tcnt); }
+}
+
+// Depth L1, pass 2: dL_dD *= lambda / max(N_valid, 1), N_valid read on the device (no host round trip).
+__global__ void __launch_bounds__(256) depth_grad_scale_kernel(int n, float lambda, const double* __restrict__ sums, float* __restrict__ dL_dD)
+{
+	const float scale = lambda / (float)fmax(sums[1], 1.0);
+	for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) dL_dD[i] *= scale;
+}
+
 }  // namespace
+
+int launch_depth_loss(int H, int W, const float* depth, const float* gt_depth, const float* mask, float lambda_depth, double* sums, float* dL_dD,
+                      cudaStream_t stream)
+{
+	const int n = H * W;
+	const int grid = min(cdiv(n, 256), kNumSMs * 8);
+	PSB_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), stream));
+	depth_loss_kernel<<<grid, 256, 0, stream>>>(n, depth, gt_depth, mask, dL_dD, sums);
+	PSB_LAUNCH_OK();
+	depth_grad_scale_kernel<<<grid, 256, 0, stream>>>(n, lambda_depth, sums, dL_dD);
+	PSB_LAUNCH_OK();
+	return 0;
+}
 
 // sums: device double[2] (zeroed here); after the launch sums[0] = sum|I-G|, sums[1] = sum ssim_map.
 // dmap: device float[9*H*W] scratch. dL_dimg may be null (loss value only).

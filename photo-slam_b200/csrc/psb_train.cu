@@ -40,6 +40,8 @@ constexpr int MODE_ADAM = 1;   // fused single-GPU step: parameters and moments 
 constexpr int MODE_PUSH = 2;   // NVLink data-parallel step: 80-byte gradient records pushed into the owner rank's inbox
 constexpr int MODE_ADAM_LIVE = 3;  // MODE_ADAM with the caller's per-row live byte (psb_model.adam_live): rows that are neither live nor
                                    // reached by a gradient are not read beyond that byte and the visibility word
+constexpr int MODE_DEPTH = 8;      // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE: slot 11 of the sink row holds dL/dz (view-space depth,
+                                   // render_bwd_depth_kernel) and joins dL/dxyz through the view matrix's z row
 
 // torch::optim::Adam single-tensor update (LibTorch adam.cpp): exp_avg.mul_(b1).add_(g, 1-b1);
 // exp_avg_sq.mul_(b2).addcmul_(g, g, 1-b2); denom = exp_avg_sq.sqrt()/sqrt(bc2) + eps; p.addcdiv_(exp_avg, denom, -lr/bc1).
@@ -72,14 +74,19 @@ __device__ __forceinline__ void adam1(float& p, float& m, float& v, float g, flo
 // own rows with 4-byte async copies into a compacted region of s_p (one coalesced 180-byte run per row; the whole-block TMA copy
 // would move every row, since nearly every block holds some live row). Seed rows are written, and updated by
 // frest_stream_kernel, only for rows that are live after this step; the live byte is set for every row that received a gradient.
+//
+// MODE_DEPTH: dL/dxyz += dL/dz (V[2], V[6], V[10]). A row whose only non-zero sum is slot 11 has a gradient (its parameters are loaded and
+// updated, its live byte set) but no SH gradient: the view-direction term depends on dL/dRGB only, so its f_rest row is not staged.
 template <int MODE>
 __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(int first, int P, TrainTensors t, Camera cam, GeomState geom, float4* __restrict__ sink,
                                                             StepHyper h, GradSegments grads, DensifyStats st,
                                                             const uint32_t* __restrict__ counters, uint32_t capacity, float4* __restrict__ seeds,
                                                             DpPush dp, unsigned char* __restrict__ adam_live)
 {
-	constexpr bool LIVE = MODE == MODE_ADAM_LIVE;
-	constexpr bool ADAM = MODE == MODE_ADAM || LIVE;
+	constexpr bool DEPTH = (MODE & MODE_DEPTH) != 0;
+	constexpr int BASE = MODE & ~MODE_DEPTH;
+	constexpr bool LIVE = BASE == MODE_ADAM_LIVE;
+	constexpr bool ADAM = BASE == MODE_ADAM || LIVE;
 	__shared__ __align__(128) float s_p[TB * REST];  // f_rest parameter rows of this block (TMA destination; LIVE: compacted per warp)
 	__shared__ __align__(16) float s_w[TB][SEED];    // seed rows of this block (copied out 128-bit coalesced at the end)
 	__shared__ __align__(8) uint64_t s_bar;
@@ -130,6 +137,7 @@ __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(
 	float4 mr = make_float4(0, 0, 0, 0), vr = mr;
 	float st_rad = 0.f, st_acc = 0.f, st_den = 0.f;
 	bool was_live = false, staged = false;  // LIVE: live byte before this step | f_rest row staged (non-zero sums)
+	bool reached = false;                   // LIVE: staged, or (DEPTH) a non-zero dL/dz
 	int rest_slot = tid;                    // this row's f_rest row in s_p
 	float4 s0 = make_float4(0, 0, 0, 0), s1 = s0, s2 = s0;
 	uint32_t meta = 0;
@@ -163,8 +171,9 @@ __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(
 				meta = __float_as_uint(geom.rec[idx].q2.w);
 				// only visible rows were added to; the others are zero since the last step
 				staged = s0.x != 0.f || s0.y != 0.f || s0.w != 0.f || s1.x != 0.f || s1.z != 0.f || s1.w != 0.f || s2.x != 0.f || s2.y != 0.f || s2.z != 0.f;
-				if (staged) { const float4 z = make_float4(0, 0, 0, 0); sink[3 * idx] = z; sink[3 * idx + 1] = z; sink[3 * idx + 2] = z; }
-				if (staged && !was_live) load_params();  // first gradient of this row: its moments are zero by contract, not read
+				reached = staged || (DEPTH && s2.w != 0.f);
+				if (reached) { const float4 z = make_float4(0, 0, 0, 0); sink[3 * idx] = z; sink[3 * idx + 1] = z; sink[3 * idx + 2] = z; }
+				if (reached && !was_live) load_params();  // first gradient of this row: its moments are zero by contract, not read
 				if (st.enabled) {  // (here: fewer registers held across the backward)
 					st.max_radii2D[idx] = fmaxf(st_rad, (float)rec_radius(meta));
 					st.xyz_gradient_accum[idx] = st_acc + sqrtf(s0.x * s0.x + s0.y * s0.y);
@@ -196,11 +205,12 @@ __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(
 			load_params();
 			visible = tt != 0 && !overflow;
 			// ready for the next iteration (rows nothing was added to — culled or hidden Gaussians — are zero already: not rewritten)
-			const bool sink_dirty = s0.x != 0.f || s0.y != 0.f || s0.w != 0.f || s1.x != 0.f || s1.z != 0.f || s1.w != 0.f || s2.x != 0.f || s2.y != 0.f || s2.z != 0.f;
+			const bool sink_dirty = s0.x != 0.f || s0.y != 0.f || s0.w != 0.f || s1.x != 0.f || s1.z != 0.f || s1.w != 0.f || s2.x != 0.f || s2.y != 0.f || s2.z != 0.f ||
+			                        (DEPTH && s2.w != 0.f);
 			if (sink_dirty) { const float4 z = make_float4(0, 0, 0, 0); sink[3 * idx] = z; sink[3 * idx + 1] = z; sink[3 * idx + 2] = z; }
 		}
 		// LIVE: a visible row with zero sums has zero gradients (and may not have its parameters loaded): statistics only
-		if (visible && (!LIVE || staged)) {
+		if (visible && (!LIVE || reached)) {
 			// sink row: [0,1] mean2D.xy | [3,4,6] conic.xyw | [7] opacity | [8,9,10] rgb
 			const float2 dL_dmean2D = make_float2(s0.x, s0.y);
 			const float3 dL_dconic = make_float3(s0.w, s1.x, s1.z);
@@ -228,6 +238,10 @@ __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(
 			const float qd = q.x * dL_drot.x + q.y * dL_drot.y + q.z * dL_drot.z + q.w * dL_drot.w;
 			g_rot = make_float4((dL_drot.x - q.x * qd) / qn, (dL_drot.y - q.y * qd) / qn, (dL_drot.z - q.z * qd) / qn, (dL_drot.w - q.w * qd) / qn);
 			g_opac = dL_dopacity * sig * (1.0f - sig);
+			if (DEPTH) {  // z = V[2] x + V[6] y + V[10] z + V[14] (column-major view matrix)
+				const float dz = s2.w;
+				g_xyz.x += dz * cam.view[2]; g_xyz.y += dz * cam.view[6]; g_xyz.z += dz * cam.view[10];
+			}
 		}
 		// every visible row counts, hidden ones included (the reference's denom counts them too)
 		if (!LIVE && visible && st.enabled) {
@@ -265,7 +279,7 @@ __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(
 			gm[1] = ((clamp_bits >> 1) & 1u) ? 0.f : dL_dcolor.y;
 			gm[2] = ((clamp_bits >> 2) & 1u) ? 0.f : dL_dcolor.z;
 		}
-		if (MODE != MODE_PUSH) {
+		if (BASE != MODE_PUSH) {
 			const int ncoef = (h.D + 1) * (h.D + 1);
 #pragma unroll
 			for (int k = 1; k < 16; k++) s_w[tid][k - 1] = (k < ncoef) ? w[k] : 0.f;
@@ -332,7 +346,7 @@ __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(
 			}
 			t.p[3][idx] = sp_op; t.m[3][idx] = mo; t.v[3][idx] = vo;
 			reinterpret_cast<float4*>(t.p[5])[idx] = sp_rot; reinterpret_cast<float4*>(t.m[5])[idx] = mr; reinterpret_cast<float4*>(t.v[5])[idx] = vr;
-		} else if (MODE == MODE_GRADS) {
+		} else if (BASE == MODE_GRADS) {
 			grads.g[0][3 * idx] = g_xyz.x; grads.g[0][3 * idx + 1] = g_xyz.y; grads.g[0][3 * idx + 2] = g_xyz.z;
 			grads.g[1][3 * idx] = g_dc.x; grads.g[1][3 * idx + 1] = g_dc.y; grads.g[1][3 * idx + 2] = g_dc.z;
 			grads.g[3][idx] = g_opac;
@@ -342,7 +356,7 @@ __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(
 	}
 	__syncthreads();
 
-	if (MODE != MODE_PUSH) {
+	if (BASE != MODE_PUSH) {
 		// seed rows of this block -> global, 128-bit coalesced
 		const float4* src = reinterpret_cast<const float4*>(&s_w[0][0]);
 		float4* dst = seeds + (size_t)base * (SEED / 4);
@@ -752,7 +766,7 @@ __global__ void wait_flags_kernel(const uint32_t* flags, int world, uint32_t epo
 
 int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, float* seeds,
                           const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
-                          cudaStream_t stream, cudaEvent_t between, unsigned char* adam_live)
+                          cudaStream_t stream, cudaEvent_t between, unsigned char* adam_live, bool depth)
 {
 	if (P - first <= 0) return 0;
 	const int grid = cdiv(P - first, TB);
@@ -763,7 +777,11 @@ int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, co
 	DpPush nodp;
 	memset(&nodp, 0, sizeof(nodp));
 	unsigned char* live = adam ? adam_live : nullptr;
-	if (live) gaussian_backward_kernel<MODE_ADAM_LIVE><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, live);
+	if (depth) {
+		if (live) gaussian_backward_kernel<MODE_ADAM_LIVE | MODE_DEPTH><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, live);
+		else if (adam) gaussian_backward_kernel<MODE_ADAM | MODE_DEPTH><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, nullptr);
+		else gaussian_backward_kernel<MODE_GRADS | MODE_DEPTH><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, nullptr);
+	} else if (live) gaussian_backward_kernel<MODE_ADAM_LIVE><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, live);
 	else if (adam) gaussian_backward_kernel<MODE_ADAM><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, nullptr);
 	else gaussian_backward_kernel<MODE_GRADS><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, nullptr);
 	PSB_LAUNCH_OK();

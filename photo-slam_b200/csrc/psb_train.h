@@ -70,11 +70,16 @@ int launch_wait_flags(const uint32_t* flags, int world, uint32_t epoch, uint32_t
 int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, float* seeds,
                           const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
                           cudaStream_t stream, cudaEvent_t between = nullptr /* recorded between the two kernels (stage timing) */,
-                          unsigned char* adam_live = nullptr /* adam only: psb_model.adam_live, or null (the moments tell idle rows) */);
+                          unsigned char* adam_live = nullptr /* adam only: psb_model.adam_live, or null (the moments tell idle rows) */,
+                          bool depth = false /* the sink rows carry dL/dz in slot 11 (render_bwd_depth_kernel) */);
 // adam_live[i] = any moment of row i non-zero (t.m / t.v: the 12 moment tensors)
 int launch_adam_live_rebuild(int P, const TrainTensors& t, unsigned char* adam_live, cudaStream_t stream);
 int launch_adam(size_t n, float* p, float* m, float* v, const float* g, float lr, const StepHyper& h, float grad_scale, cudaStream_t stream);
 int launch_loss(int H, int W, const float* img, const float* gt, const float* mask, float lambda_dssim, float* dmap, double* sums,
                 float* dL_dimg, cudaStream_t stream);
+// Depth L1 over the valid pixels (gt > 0 and, with a mask, mask[0, p] != 0): sums[0] = sum |D - G|, sums[1] = N_valid (zeroed here);
+// dL_dD [H,W] = lambda * sign(D - G) / max(N_valid, 1) on valid pixels, 0 elsewhere. Two launches, no host synchronisation.
+int launch_depth_loss(int H, int W, const float* depth, const float* gt_depth, const float* mask, float lambda_depth, double* sums, float* dL_dD,
+                      cudaStream_t stream);
 
 }  // namespace psb

@@ -8,6 +8,7 @@
 #include <cmath>
 #include <cstring>
 #include <cstdlib>
+#include <string>
 #include "psb_train.h"
 #include "../../include/psb200.h"
 
@@ -19,8 +20,9 @@ struct psb_trainer {
 	char* bin_chunk = nullptr; size_t bin_bytes = 0; size_t capacity = 0;
 	float* image = nullptr; float* dL_dpix = nullptr; float* dmap = nullptr; size_t pix_alloc = 0;
 	float* sink = nullptr; float* seeds = nullptr; size_t sink_P = 0;
-	double* sums = nullptr;      // device [2]
-	double* h_sums = nullptr;    // pinned [2]
+	float* depth_buf = nullptr; size_t depth_alloc = 0;  // depth loss: [2][H*W] = rendered depth (when the caller passes no out_depth) | dL/dD
+	double* sums = nullptr;      // device [4]: sum |I - G|, sum SSIM | depth loss: sum |D - G|, N_valid
+	double* h_sums = nullptr;    // pinned [4]
 	uint32_t* h_count = nullptr; // pinned [4]: instance count of the last call | sticky overflow record {count, first seq, largest count}
 	uint32_t* ovf = nullptr;     // device [4]: the sticky overflow record (tile_ranges_kernel), collected by psb_trainer_result
 	uint32_t seq = 0;            // sequence number of the last forward pass (render / step / backward) of this context
@@ -28,7 +30,9 @@ struct psb_trainer {
 	cudaEvent_t readback = nullptr;  // recorded once the instance count (and the loss sums) of the last call are in pinned memory
 	int last_P = 0, last_W = 0, last_H = 0;
 	float last_lambda = 0.2f;
+	float last_lambda_depth = 0.f;
 	bool have_loss = false;
+	bool have_depth_loss = false;  // the last step had a depth term (h_sums[2..3] belong to it)
 	// tight instance lists: only the tiles a splat can reach get an instance (see preprocess_fwd_kernel); PSB_TIGHT=0 keeps the
 	// reference's full rectangles (A/B measurements only — images and gradients are the same either way)
 	bool tight = !(getenv("PSB_TIGHT") && atoi(getenv("PSB_TIGHT")) == 0);
@@ -55,7 +59,7 @@ int dev_alloc(T** p, size_t count)
 	return 0;
 }
 
-int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream)
+int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_loss = false)
 {
 	const size_t N = (size_t)W * H;
 	int rc;
@@ -78,6 +82,11 @@ int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream)
 		if ((rc = dev_alloc(&t->dmap, 9 * N))) return rc;
 		t->pix_alloc = N;
 	}
+	if (depth_loss && t->depth_alloc < N) {
+		PSB_CUDA_OK(cudaStreamSynchronize(stream));
+		if ((rc = dev_alloc(&t->depth_buf, 2 * N))) return rc;
+		t->depth_alloc = N;
+	}
 	if (t->sink_P < (size_t)P) {
 		PSB_CUDA_OK(cudaStreamSynchronize(stream));
 		if ((rc = dev_alloc(&t->sink, (size_t)P * 12))) return rc;
@@ -86,8 +95,8 @@ int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream)
 		t->sink_P = (size_t)P;
 	}
 	if (!t->sums) {
-		if ((rc = dev_alloc(&t->sums, 2))) return rc;
-		PSB_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&t->h_sums), 2 * sizeof(double)));
+		if ((rc = dev_alloc(&t->sums, 4))) return rc;
+		PSB_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&t->h_sums), 4 * sizeof(double)));
 		PSB_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&t->h_count), 4 * sizeof(uint32_t)));
 		memset(t->h_count, 0, 4 * sizeof(uint32_t));
 		if ((rc = dev_alloc(&t->ovf, 4))) return rc;
@@ -154,9 +163,25 @@ int check_model(int P, int M, const psb_model* m, bool need_moments)
 	return 0;
 }
 
-// forward from raw parameters into t->image (or out_color)
+// NULL: no depth. Otherwise lambda_depth finite and >= 0, and a target exactly when lambda_depth > 0.
+int check_depth(const psb_depth* d, const char* fn)
+{
+	if (!d) return 0;
+	if (!std::isfinite(d->lambda_depth) || d->lambda_depth < 0.f) {
+		set_error_msg(std::string(fn).append(": lambda_depth must be finite and >= 0").c_str());
+		return PSB_ERR_ARG;
+	}
+	if ((d->gt_depth != nullptr) != (d->lambda_depth > 0.f)) {
+		set_error_msg(std::string(fn).append(": gt_depth and lambda_depth > 0 must be given together").c_str());
+		return PSB_ERR_ARG;
+	}
+	return 0;
+}
+
+// forward from raw parameters into t->image (or out_color); out_depth != NULL: the depth variant also writes the expected depth there
 int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, const psb_camera* camera, const float* background,
-                float* out_color, int* radii, GeomState& geom, BinState& bin, ImgState& img, Camera& cam, cudaStream_t stream)
+                float* out_color, int* radii, GeomState& geom, BinState& bin, ImgState& img, Camera& cam, cudaStream_t stream,
+                float* out_depth = nullptr)
 {
 	int rc;
 	if ((rc = ensure(t, P, camera->width, camera->height, stream))) return rc;
@@ -178,29 +203,42 @@ int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, con
 	PSB_CUDA_OK(cudaEventRecord(t->readback, stream));
 	const int res = make_sort_plan(tile_id_bits(cam.grid_x * cam.grid_y)).npass & 1;
 	rc = launch_render_forward(cam, img.ranges, bin.inst[res], geom.rec, background, out_color ? out_color : t->image, img.final_T,
-	                           img.n_contrib, stream);
+	                           img.n_contrib, stream, out_depth);
 	t->mark(4, stream);
 	return rc;
 }
 
 int step_impl(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, const float* gt_image,
               const float* mask, const psb_step* step, float* out_color, int* radii, float* const* grads, cudaStream_t stream,
-              bool tiles_only = false)
+              bool tiles_only = false, const psb_depth* depth = nullptr)
 {
 	int rc;
 	if (!t || !camera || !step || !background || !gt_image) { set_error_msg("psb_trainer_step: null argument"); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, grads == nullptr && !tiles_only))) return rc;
 	if (step->sh_degree < 0 || step->sh_degree > 3 || step->step < 1) { set_error_msg("psb_trainer_step: sh_degree in 0..3 and step >= 1 required"); return PSB_ERR_ARG; }
+	// depth loss: the depth plane is the caller's out_depth or the context's own; dL/dD lives in the context
+	const bool depth_loss = depth && depth->gt_depth;
+	float* depth_plane = depth ? depth->out_depth : nullptr;
+	float* dL_ddepth = nullptr;
+	if (depth_loss) {
+		if ((rc = ensure(t, P, camera->width, camera->height, stream, true))) return rc;
+		if (!depth_plane) depth_plane = t->depth_buf;
+		dL_ddepth = t->depth_buf + (size_t)camera->width * camera->height;
+	}
 	GeomState geom; BinState bin; ImgState img; Camera cam;
-	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, geom, bin, img, cam, stream))) return rc;
+	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, geom, bin, img, cam, stream, depth_plane))) return rc;
 	const float* image = out_color ? out_color : t->image;
 	if ((rc = launch_loss(cam.H, cam.W, image, gt_image, mask, step->lambda_dssim, t->dmap, t->sums, t->dL_dpix, stream))) return rc;
+	if (depth_loss && (rc = launch_depth_loss(cam.H, cam.W, depth_plane, depth->gt_depth, mask, depth->lambda_depth, t->sums + 2, dL_ddepth, stream)))
+		return rc;
 	// loss sums -> pinned memory right behind the loss kernel, so the host can read the loss of this iteration (and start
 	// enqueueing the next one) while the backward half is still running
-	PSB_CUDA_OK(cudaMemcpyAsync(t->h_sums, t->sums, 2 * sizeof(double), cudaMemcpyDeviceToHost, stream));
+	PSB_CUDA_OK(cudaMemcpyAsync(t->h_sums, t->sums, (depth_loss ? 4 : 2) * sizeof(double), cudaMemcpyDeviceToHost, stream));
 	PSB_CUDA_OK(cudaEventRecord(t->readback, stream));
 	t->last_lambda = step->lambda_dssim;
+	t->last_lambda_depth = depth_loss ? depth->lambda_depth : 0.f;
 	t->have_loss = true;
+	t->have_depth_loss = depth_loss;
 	t->mark(5, stream);
 	if (P == 0) return 0;
 	GradSink sink;
@@ -210,7 +248,8 @@ int step_impl(psb_trainer* t, int P, int M, const psb_model* model, const psb_ca
 	sink.color = t->sink + 8; sink.color_stride = 12;
 	sink.packed = 1;
 	const int res = make_sort_plan(tile_id_bits(cam.grid_x * cam.grid_y)).npass & 1;
-	if ((rc = launch_render_backward(cam, img.ranges, bin.inst[res], geom.rec, background, img.final_T, img.n_contrib, t->dL_dpix, sink, stream))) return rc;
+	if ((rc = launch_render_backward(cam, img.ranges, bin.inst[res], geom.rec, background, img.final_T, img.n_contrib, t->dL_dpix, sink, stream, dL_ddepth)))
+		return rc;
 	t->mark(6, stream);
 	if (tiles_only) return 0;
 	TrainTensors tt;
@@ -222,7 +261,7 @@ int step_impl(psb_trainer* t, int P, int M, const psb_model* model, const psb_ca
 	st.max_radii2D = model->max_radii2D; st.xyz_gradient_accum = model->xyz_gradient_accum; st.denom = model->denom;
 	const StepHyper h = to_hyper(step);
 	rc = launch_fused_backward(grads == nullptr, 0, P, tt, cam, geom, t->sink, t->seeds, h, gs, st, geom.counters, (uint32_t)t->capacity, stream,
-	                           (t->profiling && t->ev_ready) ? t->ev[7] : nullptr, grads == nullptr ? model->adam_live : nullptr);
+	                           (t->profiling && t->ev_ready) ? t->ev[7] : nullptr, grads == nullptr ? model->adam_live : nullptr, depth_loss);
 	t->mark(8, stream);
 	t->last_stage = 8;
 	t->ev_recorded = t->profiling && t->ev_ready;
@@ -462,7 +501,7 @@ int psb_trainer_destroy(psb_trainer* t)
 {
 	if (!t) return 0;
 	cudaFree(t->geom_chunk); cudaFree(t->img_chunk); cudaFree(t->bin_chunk); cudaFree(t->image); cudaFree(t->dL_dpix); cudaFree(t->dmap);
-	cudaFree(t->sink); cudaFree(t->seeds); cudaFree(t->sums); cudaFree(t->ovf);
+	cudaFree(t->sink); cudaFree(t->seeds); cudaFree(t->sums); cudaFree(t->ovf); cudaFree(t->depth_buf);
 	if (t->ev_ready) for (int i = 0; i <= psb_trainer::NSTAGE; i++) cudaEventDestroy(t->ev[i]);
 	if (t->h_sums) cudaFreeHost(t->h_sums);
 	if (t->h_count) cudaFreeHost(t->h_count);
@@ -482,10 +521,30 @@ int psb_trainer_render(psb_trainer* t, int P, int M, const psb_model* model, con
 	return forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, geom, bin, img, cam, (cudaStream_t)stream_);
 }
 
+int psb_trainer_render_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
+                             float* out_color, int* radii, float* out_depth, void* stream_)
+{
+	int rc;
+	if (!t || !camera || !background || !out_color) { set_error_msg("psb_trainer_render_depth: null argument"); return PSB_ERR_ARG; }
+	if ((rc = check_model(P, M, model, false))) return rc;
+	GeomState geom; BinState bin; ImgState img; Camera cam;
+	t->have_loss = false;
+	return forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, geom, bin, img, cam, (cudaStream_t)stream_, out_depth);
+}
+
 int psb_trainer_step(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                      const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, void* stream_)
 {
 	return step_impl(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, nullptr, (cudaStream_t)stream_);
+}
+
+int psb_trainer_step_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                           const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
+                           void* stream_)
+{
+	int rc;
+	if ((rc = check_depth(depth, "psb_trainer_step_depth"))) return rc;
+	return step_impl(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, nullptr, (cudaStream_t)stream_, false, depth);
 }
 
 int psb_adam_live_rebuild(int P, const psb_model* model, void* stream_)
@@ -498,17 +557,26 @@ int psb_adam_live_rebuild(int P, const psb_model* model, void* stream_)
 	return launch_adam_live_rebuild(P, tt, model->adam_live, (cudaStream_t)stream_);
 }
 
-int psb_trainer_backward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
-                         const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, float* const* grads,
-                         void* stream_)
+int psb_trainer_backward_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                               const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, float* const* grads,
+                               const psb_depth* depth, void* stream_)
 {
+	int rc;
+	if ((rc = check_depth(depth, "psb_trainer_backward_depth"))) return rc;
 	if (!grads) { set_error_msg("psb_trainer_backward: grads required"); return PSB_ERR_ARG; }
 	for (int i = 0; i < 6; i++) if (P > 0 && !grads[i]) { set_error_msg("psb_trainer_backward: null gradient segment"); return PSB_ERR_ARG; }
 	if (P > 0 && ((reinterpret_cast<uintptr_t>(grads[2]) | reinterpret_cast<uintptr_t>(grads[5])) & 15)) {
 		set_error_msg("psb_trainer_backward: the features_rest and rotation gradient segments must be 16-byte aligned");
 		return PSB_ERR_ARG;
 	}
-	return step_impl(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, grads, (cudaStream_t)stream_);
+	return step_impl(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, grads, (cudaStream_t)stream_, false, depth);
+}
+
+int psb_trainer_backward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                         const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, float* const* grads,
+                         void* stream_)
+{
+	return psb_trainer_backward_depth(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, grads, nullptr, stream_);
 }
 
 int psb_trainer_backward_begin(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
@@ -565,7 +633,7 @@ int psb_adam_flat(size_t n, float* param, float* exp_avg, float* exp_avg_sq, con
 	return launch_adam(n, param, exp_avg, exp_avg_sq, grad, lr, h, grad_scale, (cudaStream_t)stream_);
 }
 
-int psb_trainer_result(psb_trainer* t, float* out3, int* num_rendered, void* stream_)
+static int result_impl(psb_trainer* t, float* out, bool with_depth, int* num_rendered, void* stream_)
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
 	if (!t || t->geom_P < 0) { set_error_msg("psb_trainer_result: no step has run"); return PSB_ERR_ARG; }
@@ -593,14 +661,27 @@ int psb_trainer_result(psb_trainer* t, float* out3, int* num_rendered, void* str
 		set_error_msg("psb_trainer: binning arena was too small for a view; it has been grown, repeat the call (psb_trainer_overflow_info says which)");
 		return PSB_ERR_RETRY;
 	}
-	if (out3 && t->have_loss) {
+	if (out && t->have_loss) {
 		const double inv_n = 1.0 / (3.0 * (double)t->last_W * (double)t->last_H);
 		const float l1 = (float)(t->h_sums[0] * inv_n), ss = (float)(t->h_sums[1] * inv_n);
-		out3[0] = (1.0f - t->last_lambda) * l1 + t->last_lambda * (1.0f - ss);
-		out3[1] = l1;
-		out3[2] = ss;
+		const float dl1 = t->have_depth_loss ? (float)(t->h_sums[2] / (t->h_sums[3] > 1.0 ? t->h_sums[3] : 1.0)) : 0.f;
+		out[0] = (1.0f - t->last_lambda) * l1 + t->last_lambda * (1.0f - ss);
+		if (t->have_depth_loss) out[0] += t->last_lambda_depth * dl1;
+		out[1] = l1;
+		out[2] = ss;
+		if (with_depth) out[3] = dl1;
 	}
 	return 0;
+}
+
+int psb_trainer_result(psb_trainer* t, float* out3, int* num_rendered, void* stream_)
+{
+	return result_impl(t, out3, false, num_rendered, stream_);
+}
+
+int psb_trainer_result_depth(psb_trainer* t, float* out4, int* num_rendered, void* stream_)
+{
+	return result_impl(t, out4, true, num_rendered, stream_);
 }
 
 // Parity/debug export (tests only): per pixel, the final transmittance and the Gaussian index of the last blended splat

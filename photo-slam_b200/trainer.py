@@ -37,6 +37,20 @@ class _Step(C.Structure):
                 ("lambda_dssim", C.c_float), ("sh_degree", C.c_int), ("update_densify_stats", C.c_int)]
 
 
+class _Depth(C.Structure):
+    _fields_ = [("gt_depth", C.c_void_p), ("lambda_depth", C.c_float), ("out_depth", C.c_void_p)]
+
+
+def _cdepth(gt_depth, lambda_depth, out_depth):
+    """psb_depth for a call, or None when it has no depth argument (the plain C function is called then)."""
+    if gt_depth is None and out_depth is None and not lambda_depth:
+        return None
+    for t in (gt_depth, out_depth):
+        assert t is None or (t.is_contiguous() and t.dtype == torch.float32), "depth planes: contiguous float32 [H,W]"
+    return _Depth(gt_depth.data_ptr() if gt_depth is not None else None, float(lambda_depth),
+                  out_depth.data_ptr() if out_depth is not None else None)
+
+
 class _DensifyCfg(C.Structure):
     _fields_ = [("max_grad", C.c_float), ("min_opacity", C.c_float), ("extent", C.c_float), ("percent_dense", C.c_float), ("max_screen_size", C.c_int),
                 ("seed", C.c_ulonglong), ("offset", C.c_ulonglong)]
@@ -55,9 +69,16 @@ def _bind():
                                        C.POINTER(vp), vp]
     L.psb_adam_update.argtypes = [C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(vp), C.POINTER(_Step), C.c_float, vp]
     L.psb_trainer_result.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int), vp]
+    L.psb_trainer_render_depth.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, C.c_int, vp, vp, vp, vp]
+    L.psb_trainer_step_depth.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp, vp,
+                                         C.POINTER(_Depth), vp]
+    L.psb_trainer_backward_depth.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp, vp,
+                                             C.POINTER(vp), C.POINTER(_Depth), vp]
+    L.psb_trainer_result_depth.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int), vp]
     L.psb_loss.argtypes = [C.c_int, C.c_int, vp, vp, vp, C.c_float, vp, C.POINTER(C.c_float), vp]
     for n in ("psb_trainer_create", "psb_trainer_destroy", "psb_trainer_render", "psb_trainer_step", "psb_trainer_backward",
-              "psb_adam_update", "psb_trainer_result", "psb_loss"):
+              "psb_adam_update", "psb_trainer_result", "psb_loss", "psb_trainer_render_depth", "psb_trainer_step_depth",
+              "psb_trainer_backward_depth", "psb_trainer_result_depth"):
         getattr(L, n).restype = C.c_int
     L.psb_densify_workspace_bytes.argtypes = [C.c_int]
     L.psb_densify_workspace_bytes.restype = C.c_size_t
@@ -447,35 +468,48 @@ class GaussianTrainer:
         s.update_densify_stats = int(densify_stats)
         return s
 
-    def render(self, cam, out=None, radii=None, check=True):
+    def render(self, cam, out=None, radii=None, check=True, out_depth=None):
         """Forward only. check=True waits for the instance count and renders again if the binning arena had to grow (an
-        overflowing render leaves `out` blank); pass check=False to only enqueue (call result() yourself before using `out`)."""
+        overflowing render leaves `out` blank); pass check=False to only enqueue (call result() yourself before using `out`).
+        out_depth: [H,W] float32 tensor that receives the expected depth sum_i z_i alpha_i T_i (psb_trainer_render_depth)."""
         m = self.model
         out = out if out is not None else torch.empty((3, cam["H"], cam["W"]), device=m.device)
         cm, cc = m._cmodel(False), _ccamera(cam)
-        _lib.check(self.L.psb_trainer_render(self.h, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(),
-                                             m.active_sh_degree_, out.data_ptr(), radii.data_ptr() if radii is not None else None,
-                                             torch.cuda.current_stream().cuda_stream), "psb_trainer_render")
-        self._last_render = (cam, out, radii)
+        args = (self.h, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(), m.active_sh_degree_, out.data_ptr(),
+                radii.data_ptr() if radii is not None else None)
+        stream = torch.cuda.current_stream().cuda_stream
+        if out_depth is None:
+            _lib.check(self.L.psb_trainer_render(*args, stream), "psb_trainer_render")
+        else:
+            assert out_depth.is_contiguous() and out_depth.dtype == torch.float32 and out_depth.numel() == cam["H"] * cam["W"]
+            _lib.check(self.L.psb_trainer_render_depth(*args, out_depth.data_ptr(), stream), "psb_trainer_render_depth")
+        self._last_render = (cam, out, radii, out_depth)
         self._last = None
         if check:
             self.result()
         return out
 
-    def trainForOneIteration(self, cam, gt_image, mask=None, out_color=None, radii=None, densify_stats=None):
-        """Enqueues render -> loss -> backward -> Adam on the current stream (no host sync)."""
+    def trainForOneIteration(self, cam, gt_image, mask=None, out_color=None, radii=None, densify_stats=None, gt_depth=None, lambda_depth=0.0,
+                             out_depth=None):
+        """Enqueues render -> loss -> backward -> Adam on the current stream (no host sync).
+        gt_depth: [H,W] float32 target depth in metres (<= 0: no measurement) trained with weight lambda_depth (> 0) as an L1 term
+        over the valid pixels (psb_trainer_step_depth); out_depth: [H,W] float32 tensor that receives the rendered depth."""
         m = self.model
+        depth = _cdepth(gt_depth, lambda_depth, out_depth)
         self.iteration += 1
         if densify_stats is None:
             densify_stats = self.iteration < self.opt.densify_until_iter
         cm, cc, cs = m._cmodel(live=m.adamLive()), _ccamera(cam), self._cstep(densify_stats)
-        _lib.check(self.L.psb_trainer_step(self.h, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(),
-                                           gt_image.data_ptr(), mask.data_ptr() if mask is not None else None, C.byref(cs),
-                                           out_color.data_ptr() if out_color is not None else None,
-                                           radii.data_ptr() if radii is not None else None,
-                                           torch.cuda.current_stream().cuda_stream), "psb_trainer_step")
+        args = (self.h, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(), gt_image.data_ptr(),
+                mask.data_ptr() if mask is not None else None, C.byref(cs), out_color.data_ptr() if out_color is not None else None,
+                radii.data_ptr() if radii is not None else None)
+        stream = torch.cuda.current_stream().cuda_stream
+        if depth is None:
+            _lib.check(self.L.psb_trainer_step(*args, stream), "psb_trainer_step")
+        else:
+            _lib.check(self.L.psb_trainer_step_depth(*args, C.byref(depth), stream), "psb_trainer_step_depth")
         m.step_ += 1
-        self._last = (cam, gt_image, mask, out_color, radii, densify_stats)
+        self._last = (cam, gt_image, mask, out_color, radii, densify_stats, gt_depth, lambda_depth, out_depth)
 
     def _overflow_info(self):
         f, n, cur = C.c_uint(), C.c_uint(), C.c_uint()
@@ -486,9 +520,20 @@ class GaussianTrainer:
     def result(self):
         """Blocks; -> (loss, l1, ssim, num_rendered). Transparently repeats the call if the binning arena had to grow for it.
         The overflow record is sticky on the device: if an EARLIER queued step overflowed (it was a no-op on the model while
-        step_ advanced), this raises instead of silently continuing."""
-        out, n = (C.c_float * 3)(), C.c_int()
-        rc = self.L.psb_trainer_result(self.h, out, C.byref(n), torch.cuda.current_stream().cuda_stream)
+        step_ advanced), this raises instead of silently continuing. The loss includes the depth term of a depth step."""
+        return self._result(False)
+
+    def result_depth(self):
+        """result() with the depth L1 of the last step: -> (loss, l1, ssim, depth_l1, num_rendered); depth_l1 = 0 without a depth target."""
+        return self._result(True)
+
+    def _result(self, with_depth):
+        out, n = (C.c_float * 4)(), C.c_int()
+        stream = torch.cuda.current_stream().cuda_stream
+        if with_depth:
+            rc = self.L.psb_trainer_result_depth(self.h, out, C.byref(n), stream)
+        else:
+            rc = self.L.psb_trainer_result(self.h, out, C.byref(n), stream)
         if rc == -4:
             first, count, cur = self._overflow_info()
             if not (count == 1 and first == cur):
@@ -498,15 +543,17 @@ class GaussianTrainer:
                 raise _lib.PsbError(f"{count} queued call(s) (first: pass {first} of {cur}) overflowed the binning arena and were dropped; the arena has "
                                     "been grown. Collect result() after every step, or render() the view once before queueing steps on it.")
             if getattr(self, "_last", None) is None:  # a render overflowed the arena: render again
-                cam, o, rad = self._last_render
-                self.render(cam, o, rad, check=False)
-                return self.result()
+                cam, o, rad, od = self._last_render
+                self.render(cam, o, rad, check=False, out_depth=od)
+                return self._result(with_depth)
             self.model.step_ -= 1                     # PSB_ERR_RETRY: the step was a no-op
             self.iteration -= 1
-            cam, gt, mask, oc, rad, ds = self._last
-            self.trainForOneIteration(cam, gt, mask, oc, rad, ds)
-            return self.result()
-        _lib.check(rc, "psb_trainer_result")
+            cam, gt, mask, oc, rad, ds, gd, ld, od = self._last
+            self.trainForOneIteration(cam, gt, mask, oc, rad, ds, gt_depth=gd, lambda_depth=ld, out_depth=od)
+            return self._result(with_depth)
+        _lib.check(rc, "psb_trainer_result_depth" if with_depth else "psb_trainer_result")
+        if with_depth:
+            return out[0], out[1], out[2], out[3], n.value
         return out[0], out[1], out[2], n.value
 
     # ------------------------------------------------------------------------------------------------------------
@@ -515,10 +562,10 @@ class GaussianTrainer:
     # GPU still works on iteration i-1, and the loss comes back through psb_trainer_result's early read-back event
     # (recorded right behind the loss kernel), so the host enqueues iteration i+1 under the backward half of i.
     # ------------------------------------------------------------------------------------------------------------
-    def trainHost(self, host_cam, host_gt, mask=None):
+    def trainHost(self, host_cam, host_gt, mask=None, host_depth=None, lambda_depth=0.0):
         """host_cam: dict(viewmatrix, projmatrix, campos: pinned CPU tensors; tanfovx, tanfovy, W, H); host_gt: pinned
-        [3,H,W] CPU tensor. Enqueues this iteration and returns its loss (the GPU may still be in its backward half;
-        flushHost() waits for it)."""
+        [3,H,W] CPU tensor; host_depth: optional pinned [H,W] CPU target depth (metres, <= 0 = none) trained with lambda_depth.
+        Enqueues this iteration and returns its loss (the GPU may still be in its backward half; flushHost() waits for it)."""
         dev = self.model.device
         if not hasattr(self, "_hs"):
             self._copy = torch.cuda.Stream()
@@ -527,16 +574,23 @@ class GaussianTrainer:
                              campos=mk(host_cam["campos"]), ev=torch.cuda.Event(), done=torch.cuda.Event()) for _ in range(2)]
             self._hslot = 0
         slot = self._hs[self._hslot]
+        if host_depth is not None and (slot.get("depth") is None or slot["depth"].shape != host_depth.shape):
+            slot["depth"] = torch.empty(host_depth.shape, dtype=host_depth.dtype, device=dev)   # (the slot is free: see "done" below)
         main = torch.cuda.current_stream()
         with torch.cuda.stream(self._copy):
             self._copy.wait_event(slot["done"])           # the iteration that last used this slot has finished reading it
             slot["gt"].copy_(host_gt, non_blocking=True)
+            if host_depth is not None:
+                slot["depth"].copy_(host_depth, non_blocking=True)
             for k in ("viewmatrix", "projmatrix", "campos"):
                 slot[k].copy_(host_cam[k], non_blocking=True)
             slot["ev"].record(self._copy)
         cam = dict(host_cam, viewmatrix=slot["viewmatrix"], projmatrix=slot["projmatrix"], campos=slot["campos"])
         main.wait_event(slot["ev"])
-        self.trainForOneIteration(cam, slot["gt"], mask)
+        if host_depth is not None:
+            self.trainForOneIteration(cam, slot["gt"], mask, gt_depth=slot["depth"], lambda_depth=lambda_depth)
+        else:
+            self.trainForOneIteration(cam, slot["gt"], mask)
         loss = self.result()[0]                           # waits for the loss scalars only (repeats the step on RETRY)
         slot["done"].record(main)
         self._hslot ^= 1
@@ -698,11 +752,11 @@ class DataParallelTrainer(GaussianTrainer):
     def status(self):
         return self.L.psb_dp_status(self.dp, torch.cuda.current_stream().cuda_stream) if self.mode == "p2p" else 0
 
-    def render(self, cam, out=None, radii=None, check=True):
+    def render(self, cam, out=None, radii=None, check=True, out_depth=None):
         """Forward only, on the complete replica: the owner-side Adam of the last step runs on the context's own stream and the peers
         store their rows asynchronously, so the render is ordered behind both (device-side wait)."""
         self.sync()
-        return super().render(cam, out, radii, check)
+        return super().render(cam, out, radii, check, out_depth)
 
     def gather_moments(self):
         """Every rank receives the Adam moments of all rows (they are only maintained on the owner): call before
@@ -747,8 +801,13 @@ class DataParallelTrainer(GaussianTrainer):
             self.segs = self.grads.segments
         self.flat = self.grads.flat
 
-    def trainForOneIteration(self, cam, gt_image, mask=None, out_color=None, radii=None, densify_stats=None):
+    def trainForOneIteration(self, cam, gt_image, mask=None, out_color=None, radii=None, densify_stats=None, gt_depth=None, lambda_depth=0.0,
+                             out_depth=None):
+        """Depth arguments as in GaussianTrainer; only the non-pipelined "nccl" path takes them (psb_trainer_backward_depth)."""
         m = self.model
+        depth = _cdepth(gt_depth, lambda_depth, out_depth)
+        if depth is not None and (self.mode == "p2p" or self.pipeline):
+            raise ValueError("DataParallelTrainer: depth targets need mode='nccl' without the slab pipeline (pipeline=False)")
         self.iteration += 1
         if densify_stats is None:
             densify_stats = self.iteration < self.opt.densify_until_iter
@@ -764,7 +823,10 @@ class DataParallelTrainer(GaussianTrainer):
         elif not self.pipeline:
             assert self.grads.P == P, "gradient buffer was built for a different model size: call rebuild() after densify/prune"
             ptrs = (C.c_void_p * 6)(*[s.data_ptr() for s in self.segs])
-            _lib.check(self.L.psb_trainer_backward(*args, ptrs, stream), "psb_trainer_backward")
+            if depth is None:
+                _lib.check(self.L.psb_trainer_backward(*args, ptrs, stream), "psb_trainer_backward")
+            else:
+                _lib.check(self.L.psb_trainer_backward_depth(*args, ptrs, C.byref(depth), stream), "psb_trainer_backward_depth")
             scale = self.grads.all_reduce(self.group)   # ONE collective per step: 59 floats per Gaussian
             _lib.check(self.L.psb_adam_update(P, 16, C.byref(cm), ptrs, C.byref(cs), scale, stream), "psb_adam_update")
         else:
@@ -792,19 +854,24 @@ class DataParallelTrainer(GaussianTrainer):
                                                     C.byref(cs), scale, stream), "psb_adam_flat")
         m.step_ += 1
         m.invalidateAdamLive()   # these steps write moments without maintaining the live bytes (and p2p: only on the owner rank)
-        self._last = (cam, gt_image, mask, out_color, radii, densify_stats)
+        self._last = (cam, gt_image, mask, out_color, radii, densify_stats, gt_depth, lambda_depth, out_depth)
 
     def result(self):
         """-> (loss, l1, ssim, num_rendered) of this rank's view. A view whose binning arena overflowed contributed a zero
         gradient to the step (every rank still stepped, replicas identical); it is counted in `dropped_views`, the arena
         has been grown, and the step is NOT repeated (a one-rank retry would desynchronise the group)."""
-        out, n = (C.c_float * 3)(), C.c_int()
-        rc = self.L.psb_trainer_result(self.h, out, C.byref(n), torch.cuda.current_stream().cuda_stream)
+        return self._result(False)
+
+    def _result(self, with_depth):
+        out, n = (C.c_float * 4)(), C.c_int()
+        stream = torch.cuda.current_stream().cuda_stream
+        rc = self.L.psb_trainer_result_depth(self.h, out, C.byref(n), stream) if with_depth else self.L.psb_trainer_result(self.h, out, C.byref(n), stream)
         if rc == -4:
             self.dropped_views += 1
-            return float("nan"), float("nan"), float("nan"), n.value
-        _lib.check(rc, "psb_trainer_result")
-        return out[0], out[1], out[2], n.value
+            nan = float("nan")
+            return (nan, nan, nan, nan, n.value) if with_depth else (nan, nan, nan, n.value)
+        _lib.check(rc, "psb_trainer_result_depth" if with_depth else "psb_trainer_result")
+        return (out[0], out[1], out[2], out[3], n.value) if with_depth else (out[0], out[1], out[2], n.value)
 
     def sync_densify_stats(self):
         """Reduce the rank-local densification statistics (call right before densify/prune)."""
