@@ -214,6 +214,13 @@ int psb_trainer_backward_begin(psb_trainer* t, int P, int M, const psb_model* mo
                                float* out_color, int* radii, void* stream);
 int psb_trainer_backward_slab(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
                               const psb_step* step, int first, int count, float* const* grads, void* stream);
+/* psb_trainer_backward_begin with a depth term (depth == NULL is the plain call; PSB_ERR_ARG as psb_trainer_step_depth). The
+ * context remembers whether the last _begin or _begin_depth carried a depth target, and every _slab that follows takes the
+ * depth term into its gradients; a plain _begin clears that again. _slab keeps its signature, and the caller runs every slab
+ * of a depth _begin before the next _begin, exactly as without depth. */
+int psb_trainer_backward_begin_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                                     const float* background, const float* gt_image, const float* mask, const psb_step* step,
+                                     float* out_color, int* radii, const psb_depth* depth, void* stream);
 /* Same update on one flat range of n floats (any slice of a parameter tensor and the matching slices of its moments and
  * gradient) with an explicit learning rate: lets the caller pipeline chunked all-reduces with the optimizer. */
 int psb_adam_flat(size_t n, float* param, float* exp_avg, float* exp_avg_sq, const float* grad, float lr,
@@ -246,6 +253,13 @@ int psb_dp_params(psb_dp* dp, float** out6);                   /* device address
 int psb_dp_step(psb_trainer* t, psb_dp* dp, int P, int M, const psb_model* model, const psb_camera* camera,
                 const float* background, const float* gt_image, const float* mask, const psb_step* step,
                 float* out_color, int* radii, void* stream);
+/* psb_dp_step with this rank's depth term (depth == NULL is psb_dp_step; PSB_ERR_ARG as psb_trainer_step_depth). dL/dz joins
+ * this rank's xyz gradient before its records are built, so the records and the owner-side Adam are those of psb_dp_step: the
+ * ranks of one step may mix views with and without a depth target. psb_trainer_result_depth reports this rank's depth_l1; a
+ * view that overflows the binning arena contributes a zero gradient, as in psb_dp_step. */
+int psb_dp_step_depth(psb_trainer* t, psb_dp* dp, int P, int M, const psb_model* model, const psb_camera* camera,
+                      const float* background, const float* gt_image, const float* mask, const psb_step* step,
+                      float* out_color, int* radii, const psb_depth* depth, void* stream);
 /* Enqueues a device-side wait until every rank's rows of the last psb_dp_step have landed in this rank's tensors. */
 int psb_dp_sync(psb_dp* dp, void* stream);
 /* 0 = healthy, 1 = a cross-rank wait timed out (PSB_DP_TIMEOUT_MS, default 20 s). Synchronises the stream. */

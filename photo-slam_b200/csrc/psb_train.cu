@@ -40,7 +40,7 @@ constexpr int MODE_ADAM = 1;   // fused single-GPU step: parameters and moments 
 constexpr int MODE_PUSH = 2;   // NVLink data-parallel step: 80-byte gradient records pushed into the owner rank's inbox
 constexpr int MODE_ADAM_LIVE = 3;  // MODE_ADAM with the caller's per-row live byte (psb_model.adam_live): rows that are neither live nor
                                    // reached by a gradient are not read beyond that byte and the visibility word
-constexpr int MODE_DEPTH = 8;      // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE: slot 11 of the sink row holds dL/dz (view-space depth,
+constexpr int MODE_DEPTH = 8;      // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE / MODE_PUSH: slot 11 of the sink row holds dL/dz (view-space depth,
                                    // render_bwd_depth_kernel) and joins dL/dxyz through the view matrix's z row
 
 // torch::optim::Adam single-tensor update (LibTorch adam.cpp): exp_avg.mul_(b1).add_(g, 1-b1);
@@ -805,13 +805,17 @@ int launch_adam_live_rebuild(int P, const TrainTensors& t, unsigned char* live, 
 }
 
 int launch_push_backward(int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, const StepHyper& h,
-                         const DensifyStats& st, const uint32_t* counters, uint32_t capacity, const DpPush& dp, cudaStream_t stream)
+                         const DensifyStats& st, const uint32_t* counters, uint32_t capacity, const DpPush& dp, cudaStream_t stream, bool depth)
 {
 	GradSegments nog;
 	memset(&nog, 0, sizeof(nog));
 	if (P - first > 0) {  // Gaussians [first, P): one pipeline group (first is a multiple of 128 * world)
-		gaussian_backward_kernel<MODE_PUSH><<<cdiv(P - first, TB), TB, 0, stream>>>(first, P, t, cam, geom, reinterpret_cast<float4*>(sink), h, nog, st, counters,
-		                                                                          capacity, nullptr, dp, nullptr);
+		if (depth)
+			gaussian_backward_kernel<MODE_PUSH | MODE_DEPTH><<<cdiv(P - first, TB), TB, 0, stream>>>(first, P, t, cam, geom, reinterpret_cast<float4*>(sink), h, nog, st,
+			                                                                                       counters, capacity, nullptr, dp, nullptr);
+		else
+			gaussian_backward_kernel<MODE_PUSH><<<cdiv(P - first, TB), TB, 0, stream>>>(first, P, t, cam, geom, reinterpret_cast<float4*>(sink), h, nog, st, counters,
+			                                                                          capacity, nullptr, dp, nullptr);
 		PSB_LAUNCH_OK();
 	}
 	if (!dp.fence_in_kernel) {

@@ -60,7 +60,8 @@ struct DpShard {             // what the owner-side Adam kernels need
 	int fence_in_kernel;               // as in DpPush
 };
 int launch_push_backward(int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, const StepHyper& h,
-                         const DensifyStats& st, const uint32_t* counters, uint32_t capacity, const DpPush& dp, cudaStream_t stream);
+                         const DensifyStats& st, const uint32_t* counters, uint32_t capacity, const DpPush& dp, cudaStream_t stream,
+                         bool depth = false /* the sink rows carry dL/dz in slot 11 (render_bwd_depth_kernel) */);
 int launch_shard_adam(const DpShard& d, const TrainTensors& t, const StepHyper& h, float grad_scale, cudaStream_t stream, cudaEvent_t between = nullptr);
 // spins (device side) until flags[0..world) >= epoch (world <= 64 words); after `timeout_ms` writes 1 to *status and gives up
 int launch_wait_flags(const uint32_t* flags, int world, uint32_t epoch, uint32_t* status, cudaStream_t stream);

@@ -33,6 +33,7 @@ struct psb_trainer {
 	float last_lambda_depth = 0.f;
 	bool have_loss = false;
 	bool have_depth_loss = false;  // the last step had a depth term (h_sums[2..3] belong to it)
+	bool slab_depth = false;       // the last psb_trainer_backward_begin* had a depth term: its sink rows carry dL/dz, every _slab must consume slot 11
 	// tight instance lists: only the tiles a splat can reach get an instance (see preprocess_fwd_kernel); PSB_TIGHT=0 keeps the
 	// reference's full rectangles (A/B measurements only — images and gradients are the same either way)
 	bool tight = !(getenv("PSB_TIGHT") && atoi(getenv("PSB_TIGHT")) == 0);
@@ -409,11 +410,13 @@ int psb_dp_status(psb_dp* d, void* stream_)
 	return (int)st;
 }
 
-int psb_dp_step(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
-                const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, void* stream_)
+int psb_dp_step_depth(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                      const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
+                      void* stream_)
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
+	if ((rc = check_depth(depth, "psb_dp_step_depth"))) return rc;
 	if (!d || !d->connected || P != d->P || !model) { set_error_msg("psb_dp_step: context not connected or built for a different P"); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, true))) return rc;
 	for (int i = 0; i < 6; i++)
@@ -426,9 +429,11 @@ int psb_dp_step(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* model,
 	// every rank's updated rows of the previous step must have landed here before this step reads the parameters
 	if (epoch > 1 && P > 0 && (d->world > 1 || d->groups > 1))   // (also orders this step behind the previous step's work on the adam stream)
 		if ((rc = launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_pflag), d->groups * d->world, epoch - 1, d->local + 2, stream))) return rc;
-	// render, loss, tile backward (the 9 screen-space sums per Gaussian)
-	if ((rc = step_impl(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, nullptr, stream, /*tiles_only=*/true))) return rc;
+	// render, loss, tile backward (the 9 screen-space sums per Gaussian; with a depth term also dL/dz in slot 11, which the push
+	// backward below must consume: a plain push backward would leave it in the sink for the next depth step)
+	if ((rc = step_impl(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, nullptr, stream, /*tiles_only=*/true, depth))) return rc;
 	if (P == 0) return 0;
+	const bool depth_loss = depth && depth->gt_depth;
 	char* gc = t->geom_chunk;
 	GeomState geom = GeomState::from_chunk(gc, (size_t)P);
 	const Camera cam = to_camera(camera);
@@ -471,7 +476,7 @@ int psb_dp_step(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* model,
 		DpPush pg = push;
 		for (int j = 0; j < d->world; j++) pg.grad_flag[j] = push.grad_flag[j] + g * d->world;
 		const int first = g * rows_per_group, last = (g + 1) * rows_per_group < P ? (g + 1) * rows_per_group : P;
-		if ((rc = launch_push_backward(first, last, tt, cam, geom, t->sink, h, st, geom.counters, (uint32_t)t->capacity, pg, stream))) return rc;
+		if ((rc = launch_push_backward(first, last, tt, cam, geom, t->sink, h, st, geom.counters, (uint32_t)t->capacity, pg, stream, depth_loss))) return rc;
 	}
 	t->mark(7, stream);
 	t->mark(8, stream);
@@ -488,6 +493,12 @@ int psb_dp_step(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* model,
 	t->last_stage = 9;
 	t->ev_recorded = t->profiling && t->ev_ready;
 	return rc;
+}
+
+int psb_dp_step(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, void* stream_)
+{
+	return psb_dp_step_depth(t, d, P, M, model, camera, background, gt_image, mask, step, out_color, radii, nullptr, stream_);
 }
 
 int psb_trainer_create(psb_trainer** out)
@@ -579,10 +590,22 @@ int psb_trainer_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	return psb_trainer_backward_depth(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, grads, nullptr, stream_);
 }
 
+int psb_trainer_backward_begin_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                                     const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii,
+                                     const psb_depth* depth, void* stream_)
+{
+	int rc;
+	if ((rc = check_depth(depth, "psb_trainer_backward_begin_depth"))) return rc;
+	// set whether or not the call below succeeds: the depth variant of _slab gives the plain result on rows without dL/dz
+	if (t) t->slab_depth = depth && depth->gt_depth;
+	return step_impl(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, nullptr, (cudaStream_t)stream_, /*tiles_only=*/true,
+	                 depth);
+}
+
 int psb_trainer_backward_begin(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                                const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, void* stream_)
 {
-	return step_impl(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, nullptr, (cudaStream_t)stream_, /*tiles_only=*/true);
+	return psb_trainer_backward_begin_depth(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, nullptr, stream_);
 }
 
 int psb_trainer_backward_slab(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const psb_step* step, int first,
@@ -608,7 +631,8 @@ int psb_trainer_backward_slab(psb_trainer* t, int P, int M, const psb_model* mod
 	st.enabled = (step->update_densify_stats && model->max_radii2D && model->xyz_gradient_accum && model->denom) ? 1 : 0;
 	st.max_radii2D = model->max_radii2D; st.xyz_gradient_accum = model->xyz_gradient_accum; st.denom = model->denom;
 	const StepHyper h = to_hyper(step);
-	return launch_fused_backward(false, first, first + count, tt, cam, geom, t->sink, t->seeds, h, gs, st, geom.counters, (uint32_t)t->capacity, (cudaStream_t)stream_);
+	return launch_fused_backward(false, first, first + count, tt, cam, geom, t->sink, t->seeds, h, gs, st, geom.counters, (uint32_t)t->capacity, (cudaStream_t)stream_,
+	                             nullptr, nullptr, t->slab_depth);
 }
 
 int psb_adam_update(int P, int M, const psb_model* model, float* const* grads, const psb_step* step, float grad_scale, void* stream_)

@@ -75,10 +75,14 @@ def _bind():
     L.psb_trainer_backward_depth.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp, vp,
                                              C.POINTER(vp), C.POINTER(_Depth), vp]
     L.psb_trainer_result_depth.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int), vp]
+    L.psb_dp_step_depth.argtypes = [vp, vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp, vp,
+                                    C.POINTER(_Depth), vp]
+    L.psb_trainer_backward_begin_depth.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp,
+                                                   vp, C.POINTER(_Depth), vp]
     L.psb_loss.argtypes = [C.c_int, C.c_int, vp, vp, vp, C.c_float, vp, C.POINTER(C.c_float), vp]
     for n in ("psb_trainer_create", "psb_trainer_destroy", "psb_trainer_render", "psb_trainer_step", "psb_trainer_backward",
               "psb_adam_update", "psb_trainer_result", "psb_loss", "psb_trainer_render_depth", "psb_trainer_step_depth",
-              "psb_trainer_backward_depth", "psb_trainer_result_depth"):
+              "psb_trainer_backward_depth", "psb_trainer_result_depth", "psb_dp_step_depth", "psb_trainer_backward_begin_depth"):
         getattr(L, n).restype = C.c_int
     L.psb_densify_workspace_bytes.argtypes = [C.c_int]
     L.psb_densify_workspace_bytes.restype = C.c_size_t
@@ -803,11 +807,11 @@ class DataParallelTrainer(GaussianTrainer):
 
     def trainForOneIteration(self, cam, gt_image, mask=None, out_color=None, radii=None, densify_stats=None, gt_depth=None, lambda_depth=0.0,
                              out_depth=None):
-        """Depth arguments as in GaussianTrainer; only the non-pipelined "nccl" path takes them (psb_trainer_backward_depth)."""
+        """Depth arguments as in GaussianTrainer, on every path: "p2p" (psb_dp_step_depth), the slab pipeline
+        (psb_trainer_backward_begin_depth) and the flat "nccl" path (psb_trainer_backward_depth). Each rank passes its own view's
+        target or none: ranks with and without a depth term may train in the same step."""
         m = self.model
         depth = _cdepth(gt_depth, lambda_depth, out_depth)
-        if depth is not None and (self.mode == "p2p" or self.pipeline):
-            raise ValueError("DataParallelTrainer: depth targets need mode='nccl' without the slab pipeline (pipeline=False)")
         self.iteration += 1
         if densify_stats is None:
             densify_stats = self.iteration < self.opt.densify_until_iter
@@ -819,7 +823,10 @@ class DataParallelTrainer(GaussianTrainer):
                 mask.data_ptr() if mask is not None else None, C.byref(cs), out_color.data_ptr() if out_color is not None else None,
                 radii.data_ptr() if radii is not None else None)
         if self.mode == "p2p":
-            _lib.check(self.L.psb_dp_step(self.h, self.dp, *args[1:], stream), "psb_dp_step")
+            if depth is None:
+                _lib.check(self.L.psb_dp_step(self.h, self.dp, *args[1:], stream), "psb_dp_step")
+            else:
+                _lib.check(self.L.psb_dp_step_depth(self.h, self.dp, *args[1:], C.byref(depth), stream), "psb_dp_step_depth")
         elif not self.pipeline:
             assert self.grads.P == P, "gradient buffer was built for a different model size: call rebuild() after densify/prune"
             ptrs = (C.c_void_p * 6)(*[s.data_ptr() for s in self.segs])
@@ -832,7 +839,10 @@ class DataParallelTrainer(GaussianTrainer):
         else:
             from .parallel import SIZES
             assert self.grads.P == P, "gradient buffer was built for a different model size: call rebuild() after densify/prune"
-            _lib.check(self.L.psb_trainer_backward_begin(*args, stream), "psb_trainer_backward_begin")
+            if depth is None:
+                _lib.check(self.L.psb_trainer_backward_begin(*args, stream), "psb_trainer_backward_begin")
+            else:
+                _lib.check(self.L.psb_trainer_backward_begin_depth(*args, C.byref(depth), stream), "psb_trainer_backward_begin_depth")
             scale = 1.0 / self.world
             for s, (first, count) in enumerate(self.grads.slabs):
                 ptrs = (C.c_void_p * 6)(*self.grads.kernel_pointers(s))
@@ -859,7 +869,8 @@ class DataParallelTrainer(GaussianTrainer):
     def result(self):
         """-> (loss, l1, ssim, num_rendered) of this rank's view. A view whose binning arena overflowed contributed a zero
         gradient to the step (every rank still stepped, replicas identical); it is counted in `dropped_views`, the arena
-        has been grown, and the step is NOT repeated (a one-rank retry would desynchronise the group)."""
+        has been grown, and the step is NOT repeated (a one-rank retry would desynchronise the group). result_depth() adds this
+        rank's depth_l1; all four terms are NaN for a dropped view."""
         return self._result(False)
 
     def _result(self, with_depth):
