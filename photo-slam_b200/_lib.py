@@ -3,7 +3,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("PSB_LIB") or os.path.join(_HERE, "lib", "libpsb200.so")  # PSB_LIB: A/B experiments only
+LIB_PATH = os.path.join(_HERE, "lib", "libpsb200.so")
 
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_size_t, C.c_void_p)
 

@@ -44,18 +44,6 @@ def build(force=False, verbose=False):
     return LIB
 
 
-def build_variant(name, defines):
-    """A/B experiments only: lib/libpsb200_<name>.so compiled with extra -D flags (select it with PSB_LIB=<path>)."""
-    os.makedirs(LIBDIR, exist_ok=True)
-    out = os.path.join(LIBDIR, f"libpsb200_{name}.so")
-    cmd = ["nvcc", *ARCH, "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-shared", *[f"-D{d}" for d in defines], "-o", out, *sources()]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        sys.stderr.write(r.stdout + r.stderr)
-        raise RuntimeError(f"nvcc failed building {out}")
-    return out
-
-
 TORCH_SRC = os.path.join(HERE, "csrc_torch", "rasterize_points.cpp")
 TORCH_LIB = os.path.join(LIBDIR, "libcuda_rasterizer.so")
 

@@ -355,10 +355,7 @@ __global__ void __launch_bounds__(256) emit_instances_kernel(int P, const uint32
 // one contiguous, coalesced run. counters[0] <- total instance count; instances beyond `capacity` are not written (the
 // step then degrades to a no-op, see psb_trainer.cu).
 constexpr int EM_THREADS = 256, EM_ITEMS = 4, EM_TILE = EM_THREADS * EM_ITEMS;
-#ifndef PSB_EM_STAGE
-#define PSB_EM_STAGE 5120
-#endif
-constexpr int EM_STAGE = PSB_EM_STAGE;  // instances staged per block (40 KB); a block with more writes to global memory directly
+constexpr int EM_STAGE = 5120;  // instances staged per block (40 KB); a block with more writes to global memory directly
 template <bool TIGHT>
 __global__ void __launch_bounds__(EM_THREADS) emit_scan_kernel(int P, const uint32_t* __restrict__ order, const uint4* __restrict__ tile_info,
                                                                uint32_t* __restrict__ tile_key, uint32_t* __restrict__ inst, int grid_x,

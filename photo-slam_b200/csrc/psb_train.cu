@@ -25,10 +25,8 @@ namespace psb {
 
 namespace {
 
-#ifndef PSB_A_MINBLOCKS
-#define PSB_A_MINBLOCKS 5
-#endif
 constexpr int TB = 128;        // Gaussians per block
+constexpr int A_MINBLOCKS = 5; // __launch_bounds__ minimum blocks per SM of gaussian_backward_kernel
 constexpr int REST = 45;       // floats per f_rest row (15 coefficients x 3 channels)
 constexpr int SEED = 20;       // floats per seed row: w_1..w_15 at [0..14], masked dL/dRGB at [16..18]
 
@@ -78,7 +76,7 @@ __device__ __forceinline__ void adam1(float& p, float& m, float& v, float g, flo
 // MODE_DEPTH: dL/dxyz += dL/dz (V[2], V[6], V[10]). A row whose only non-zero sum is slot 11 has a gradient (its parameters are loaded and
 // updated, its live byte set) but no SH gradient: the view-direction term depends on dL/dRGB only, so its f_rest row is not staged.
 template <int MODE>
-__global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(int first, int P, TrainTensors t, Camera cam, GeomState geom, float4* __restrict__ sink,
+__global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int first, int P, TrainTensors t, Camera cam, GeomState geom, float4* __restrict__ sink,
                                                             StepHyper h, GradSegments grads, DensifyStats st,
                                                             const uint32_t* __restrict__ counters, uint32_t capacity, float4* __restrict__ seeds,
                                                             DpPush dp, unsigned char* __restrict__ adam_live)
@@ -375,26 +373,8 @@ __global__ void __launch_bounds__(TB, PSB_A_MINBLOCKS) gaussian_backward_kernel(
 		for (int i = tid; i < rows * (SEED / 4); i += TB) {
 			if (__float_as_uint(s_w[i / (SEED / 4)][19]) == dp.epoch) dst[i] = src[i];
 		}
-		// "all my records of this step have landed". Default: nothing here — dp_signal_kernel, queued right behind this kernel,
-		// publishes the camera centre and raises the flags after ONE system-scope fence (the kernel boundary orders it after every
-		// store of this grid). PSB_DP_SIGNAL=fence: every thread fences its own remote stores, the last block of the grid publishes
-		// (threadFenceReduction pattern) — measured slower: a system-scope fence per block costs microseconds with NVLink stores in flight.
-		if (!dp.fence_in_kernel) return;
-		__threadfence_system();
-		__syncthreads();
-		if (tid == 0) {
-			const uint32_t prev = atomicAdd(dp.done_counter, 1u);
-			if (prev == gridDim.x - 1) {
-				*dp.done_counter = 0u;
-				__threadfence_system();
-				for (int j = 0; j < dp.world; j++) {
-					float* mt = dp.meta[j] + 8 * dp.rank;
-					mt[0] = cam.campos[0]; mt[1] = cam.campos[1]; mt[2] = cam.campos[2]; mt[3] = (float)h.D;
-				}
-				__threadfence_system();
-				for (int j = 0; j < dp.world; j++) *reinterpret_cast<volatile uint32_t*>(dp.grad_flag[j] + dp.rank) = dp.epoch;
-			}
-		}
+		// "all my records of this step have landed": dp_signal_kernel, queued right behind this kernel, publishes the camera centre
+		// and raises the flags after ONE system-scope fence (the kernel boundary orders it after every store of this grid).
 	}
 }
 
@@ -627,41 +607,18 @@ __global__ void __launch_bounds__(TB) shard_adam_small_kernel(DpShard d, TrainTe
 	if (any_live) {
 		const int rows = min(TB, d.P - chunk * TB);
 		const int tsel[5] = {0, 1, 4, 3, 5}, width[5] = {3, 3, 3, 1, 4}, soff[5] = {0, 384, 768, 1152, 1280};
-		if (d.bulk && rows == TB) {
-			// TMA bulk stores (cp.async.bulk shared -> global, 0.5-2 KB each, 5 tensors x world destinations issued back to back by one
-			// thread): the copy engine keeps all of them in flight over NVLink, where per-thread stores are limited by the SM's store queue
-			// (measured: the per-block time of this kernel grew 9x from 1 to 7 remote destinations).
-			asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // this thread's s_out writes -> visible to the async proxy
-			__syncthreads();
-			if (tid == 0) {
-				for (int jj = 0; jj < d.world; jj++) {
-					const int j = d.rotate ? (d.rank + 1 + jj) % d.world : jj;
+		for (int jj = 0; jj < d.world; jj++) {
+			const int j = (d.rank + 1 + jj) % d.world;
 #pragma unroll
-					for (int q = 0; q < 5; q++) {
-						float* gdst = d.param[j][tsel[q]] + (size_t)chunk * TB * width[q];
-						asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_u32(s_out + soff[q])),
-						             "r"((uint32_t)(TB * width[q] * sizeof(float)))
-						             : "memory");
-					}
-				}
-				asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-				asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // writes complete (not only the shared-memory reads) before the block retires
-			}
-		} else {
-			for (int jj = 0; jj < d.world; jj++) {
-				const int j = d.rotate ? (d.rank + 1 + jj) % d.world : jj;
-#pragma unroll
-				for (int q = 0; q < 5; q++) {
-					const int n = rows * width[q];   // floats of this tensor's chunk; the chunk starts 16-byte aligned (128 rows x width x 4 B)
-					float* gdst = d.param[j][tsel[q]] + (size_t)chunk * TB * width[q];
-					const float* ssrc = s_out + soff[q];
-					for (int i = tid; i < n / 4; i += TB) reinterpret_cast<float4*>(gdst)[i] = reinterpret_cast<const float4*>(ssrc)[i];
-					if (tid < (n & 3)) gdst[(n & ~3) + tid] = ssrc[(n & ~3) + tid];
-				}
+			for (int q = 0; q < 5; q++) {
+				const int n = rows * width[q];   // floats of this tensor's chunk; the chunk starts 16-byte aligned (128 rows x width x 4 B)
+				float* gdst = d.param[j][tsel[q]] + (size_t)chunk * TB * width[q];
+				const float* ssrc = s_out + soff[q];
+				for (int i = tid; i < n / 4; i += TB) reinterpret_cast<float4*>(gdst)[i] = reinterpret_cast<const float4*>(ssrc)[i];
+				if (tid < (n & 3)) gdst[(n & ~3) + tid] = ssrc[(n & ~3) + tid];
 			}
 		}
 	}
-	if (d.fence_in_kernel) __threadfence_system();  // this block's remote stores are performed before the kernel can complete
 }
 
 // Adam over the f_rest rows of the owned chunks, one block per chunk (5760 floats), 128-bit accesses; the updated values go
@@ -692,7 +649,7 @@ __global__ void __launch_bounds__(256) shard_adam_frest_kernel(DpShard d, TrainT
 			adam1(pp.w, mm.w, vv.w, gg.w, lr_eff, ac);
 			__stcs(reinterpret_cast<float4*>(m + e), mm); __stcs(reinterpret_cast<float4*>(v + e), vv);
 			for (int jj = 0; jj < d.world; jj++) {
-				const int j = d.rotate ? (d.rank + 1 + jj) % d.world : jj;
+				const int j = (d.rank + 1 + jj) % d.world;
 				*reinterpret_cast<float4*>(d.param[j][2] + e) = pp;
 			}
 		} else {  // < 4 trailing elements (P * 45 not a multiple of 4)
@@ -704,23 +661,13 @@ __global__ void __launch_bounds__(256) shard_adam_frest_kernel(DpShard d, TrainT
 			}
 		}
 	}
-	// "my updated rows have landed everywhere": dp_signal_kernel behind this kernel (default), or the last block of the grid
-	if (!d.fence_in_kernel) return;
-	__threadfence_system();
-	__syncthreads();
-	if (threadIdx.x == 0) {
-		const uint32_t prev = atomicAdd(d.done_counter, 1u);
-		if (prev == gridDim.x - 1) {
-			*d.done_counter = 0u;
-			__threadfence_system();
-			for (int j = 0; j < d.world; j++) *reinterpret_cast<volatile uint32_t*>(d.param_flag[j] + d.rank) = d.epoch;
-		}
-	}
+	// "my updated rows have landed everywhere": dp_signal_kernel behind this kernel
 }
 
 // One warp, queued right behind a data kernel of the data-parallel step: lane j publishes (optionally) this rank's meta row and then
 // raises this rank's epoch word on rank j. Stream order puts it after every store of the data kernel; the single system-scope fence
-// orders those stores (cumulativity) before the flag for an observer on another GPU.
+// orders those stores (cumulativity) before the flag for an observer on another GPU. It replaces a fence in every block of the data
+// kernel because a system-scope fence per block costs microseconds while NVLink stores are in flight.
 struct DpSignal {
 	uint32_t* flag[DP_MAX_WORLD];
 	float* meta[DP_MAX_WORLD];   // null: no meta row
@@ -818,14 +765,12 @@ int launch_push_backward(int first, int P, const TrainTensors& t, const Camera& 
 			                                                                          capacity, nullptr, dp, nullptr);
 		PSB_LAUNCH_OK();
 	}
-	if (!dp.fence_in_kernel) {
-		DpSignal s;
-		memset(&s, 0, sizeof(s));
-		for (int j = 0; j < dp.world; j++) { s.flag[j] = dp.grad_flag[j]; s.meta[j] = dp.meta[j]; }
-		s.campos = cam.campos; s.world = dp.world; s.rank = dp.rank; s.degree = h.D; s.epoch = dp.epoch;
-		dp_signal_kernel<<<1, 32, 0, stream>>>(s);
-		PSB_LAUNCH_OK();
-	}
+	DpSignal s;
+	memset(&s, 0, sizeof(s));
+	for (int j = 0; j < dp.world; j++) { s.flag[j] = dp.grad_flag[j]; s.meta[j] = dp.meta[j]; }
+	s.campos = cam.campos; s.world = dp.world; s.rank = dp.rank; s.degree = h.D; s.epoch = dp.epoch;
+	dp_signal_kernel<<<1, 32, 0, stream>>>(s);
+	PSB_LAUNCH_OK();
 	return 0;
 }
 
@@ -840,14 +785,12 @@ int launch_shard_adam(const DpShard& d, const TrainTensors& t, const StepHyper& 
 		shard_adam_frest_kernel<<<d.nlocal, 256, 0, stream>>>(d, t, h.lr[2] * ac.inv_bc1, ac);
 		PSB_LAUNCH_OK();
 	}
-	if (!d.fence_in_kernel) {
-		DpSignal s;
-		memset(&s, 0, sizeof(s));
-		for (int j = 0; j < d.world; j++) s.flag[j] = d.param_flag[j];
-		s.world = d.world; s.rank = d.rank; s.epoch = d.epoch;
-		dp_signal_kernel<<<1, 32, 0, stream>>>(s);
-		PSB_LAUNCH_OK();
-	}
+	DpSignal s;
+	memset(&s, 0, sizeof(s));
+	for (int j = 0; j < d.world; j++) s.flag[j] = d.param_flag[j];
+	s.world = d.world; s.rank = d.rank; s.epoch = d.epoch;
+	dp_signal_kernel<<<1, 32, 0, stream>>>(s);
+	PSB_LAUNCH_OK();
 	return 0;
 }
 

@@ -39,11 +39,8 @@ struct DpPush {              // what the per-Gaussian backward needs to deliver 
 	float* inbox[DP_MAX_WORLD];        // inbox base of every rank (own included), peer-mapped
 	float* meta[DP_MAX_WORLD];         // [world][8] floats on every rank: row r = camera centre + SH degree of rank r this step
 	uint32_t* grad_flag[DP_MAX_WORLD]; // [world] epoch words on every rank: word r = "rank r's records of this epoch have landed"
-	uint32_t* done_counter;            // local
 	int world, rank, nlocal_max;
 	uint32_t epoch;
-	int fence_in_kernel;               // 1: every block fences its remote stores, the grid's last block raises the flags (PSB_DP_SIGNAL=fence)
-	                                   // 0: a one-block signal kernel behind the data kernel does (stream order + ONE system fence; default)
 };
 struct DpShard {             // what the owner-side Adam kernels need
 	float* param[DP_MAX_WORLD][6];     // the six parameter tensors on every rank (row of `rank` = local)
@@ -51,13 +48,9 @@ struct DpShard {             // what the owner-side Adam kernels need
 	const float* inbox;                // local inbox
 	const float* meta;                 // local meta rows
 	float* g_rest;                     // local scratch [nlocal_max*128][45]: summed f_rest gradient of the owned rows
-	uint32_t* done_counter;            // local
 	int world, rank, nlocal_max, nlocal, P;   // nlocal: owned chunks handled by this launch, starting at local chunk lc_first
 	int lc_first;
-	int bulk;                          // 1 (PSB_DP_BULK=1): the small-parameter chunks leave as TMA bulk stores; 0 (default): per-thread 16-byte stores
-	int rotate;                        // 1: each rank walks the destination ranks starting at rank + 1 (PSB_DP_ROTATE=0: all start at rank 0)
 	uint32_t epoch;
-	int fence_in_kernel;               // as in DpPush
 };
 int launch_push_backward(int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, const StepHyper& h,
                          const DensifyStats& st, const uint32_t* counters, uint32_t capacity, const DpPush& dp, cudaStream_t stream,

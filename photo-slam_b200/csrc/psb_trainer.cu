@@ -281,7 +281,7 @@ struct psb_dp {
 	char* peer[DP_MAX_WORLD] = {};              // arena of every rank in this process' address space (peer[rank] == base)
 	size_t off_param[6] = {}, off_inbox = 0, off_meta = 0, off_gflag = 0, off_pflag = 0, bytes = 0;
 	float* g_rest = nullptr;                    // local scratch
-	uint32_t* local = nullptr;                  // [8]: 0 = backward done-counter, 1 = adam done-counter, 2 = status (1 = a wait timed out)
+	uint32_t* status = nullptr;                 // local word: 1 = a cross-rank wait timed out
 	uint32_t epoch = 0;
 	bool connected = false;
 	cudaIpcMemHandle_t handle;
@@ -321,7 +321,6 @@ int psb_dp_create(psb_dp** out, int rank, int world, int P)
 		// default 1 (no pipelining): the owner-side Adam of group g and the push backward of group g + 1 compete for the same store
 		// path, and the smaller launches lose their tails. Kept selectable for other fabrics.
 		int G = g ? atoi(g) : 1;
-		if (getenv("PSB_DP_SIGNAL") && strcmp(getenv("PSB_DP_SIGNAL"), "fence") == 0) G = 1;   // the in-kernel signalling variant is not pipelined
 		G = G < 1 ? 1 : (G > 8 ? 8 : G);
 		int cpg = (d->nchunks + G - 1) / G;
 		cpg = (cpg + world - 1) / world * world;          // a group holds whole rounds of the chunk -> owner rotation
@@ -332,13 +331,13 @@ int psb_dp_create(psb_dp** out, int rank, int world, int P)
 	cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&d->base), d->bytes);
 	if (e == cudaSuccess) e = cudaMemset(d->base, 0, d->bytes);
 	if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&d->g_rest), ((size_t)d->nlocal_max * 128 * 45 + 64) * sizeof(float));
-	if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&d->local), 8 * sizeof(uint32_t));
-	if (e == cudaSuccess) e = cudaMemset(d->local, 0, 8 * sizeof(uint32_t));
+	if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&d->status), sizeof(uint32_t));
+	if (e == cudaSuccess) e = cudaMemset(d->status, 0, sizeof(uint32_t));
 	if (e == cudaSuccess && world > 1) e = cudaIpcGetMemHandle(&d->handle, d->base);
 	if (e == cudaSuccess && d->groups > 1) e = cudaStreamCreateWithFlags(&d->adam_stream, cudaStreamNonBlocking);
 	if (e != cudaSuccess) {
 		set_error("psb_dp_create", e, __FILE__, __LINE__);
-		cudaFree(d->base); cudaFree(d->g_rest); cudaFree(d->local);
+		cudaFree(d->base); cudaFree(d->g_rest); cudaFree(d->status);
 		delete d;
 		return PSB_ERR_CUDA;
 	}
@@ -385,7 +384,7 @@ int psb_dp_destroy(psb_dp* d)
 	cudaDeviceSynchronize();
 	for (int j = 0; j < d->world; j++)
 		if (j != d->rank && d->peer[j]) cudaIpcCloseMemHandle(d->peer[j]);
-	cudaFree(d->base); cudaFree(d->g_rest); cudaFree(d->local);
+	cudaFree(d->base); cudaFree(d->g_rest); cudaFree(d->status);
 	if (d->adam_stream) cudaStreamDestroy(d->adam_stream);
 	delete d;
 	return 0;
@@ -397,7 +396,7 @@ int psb_dp_sync(psb_dp* d, void* stream_)
 {
 	if (!d) { set_error_msg("psb_dp_sync: null"); return PSB_ERR_ARG; }
 	if (d->epoch == 0 || d->P == 0 || (d->world == 1 && d->groups == 1)) return 0;   // (one rank, one group: everything is on the caller's stream)
-	return launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_pflag), d->groups * d->world, d->epoch, d->local + 2, (cudaStream_t)stream_);
+	return launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_pflag), d->groups * d->world, d->epoch, d->status, (cudaStream_t)stream_);
 }
 
 // 0 = healthy, 1 = a cross-rank wait timed out (a peer never arrived); synchronises the stream
@@ -405,7 +404,7 @@ int psb_dp_status(psb_dp* d, void* stream_)
 {
 	if (!d) { set_error_msg("psb_dp_status: null"); return PSB_ERR_ARG; }
 	uint32_t st = 0;
-	PSB_CUDA_OK(cudaMemcpyAsync(&st, d->local + 2, sizeof(st), cudaMemcpyDeviceToHost, (cudaStream_t)stream_));
+	PSB_CUDA_OK(cudaMemcpyAsync(&st, d->status, sizeof(st), cudaMemcpyDeviceToHost, (cudaStream_t)stream_));
 	PSB_CUDA_OK(cudaStreamSynchronize((cudaStream_t)stream_));
 	return (int)st;
 }
@@ -428,7 +427,7 @@ int psb_dp_step_depth(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* 
 	t->mark(psb_trainer::NSTAGE, stream);
 	// every rank's updated rows of the previous step must have landed here before this step reads the parameters
 	if (epoch > 1 && P > 0 && (d->world > 1 || d->groups > 1))   // (also orders this step behind the previous step's work on the adam stream)
-		if ((rc = launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_pflag), d->groups * d->world, epoch - 1, d->local + 2, stream))) return rc;
+		if ((rc = launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_pflag), d->groups * d->world, epoch - 1, d->status, stream))) return rc;
 	// render, loss, tile backward (the 9 screen-space sums per Gaussian; with a depth term also dL/dz in slot 11, which the push
 	// backward below must consume: a plain push backward would leave it in the sink for the next depth step)
 	if ((rc = step_impl(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, nullptr, stream, /*tiles_only=*/true, depth))) return rc;
@@ -454,19 +453,11 @@ int psb_dp_step_depth(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* 
 		sh.param_flag[j] = reinterpret_cast<uint32_t*>(d->peer[j] + d->off_pflag);
 		for (int i = 0; i < 6; i++) sh.param[j][i] = reinterpret_cast<float*>(d->peer[j] + d->off_param[i]);
 	}
-	push.done_counter = d->local; push.world = d->world; push.rank = d->rank; push.nlocal_max = d->nlocal_max; push.epoch = epoch;
-	static const int fence_in_kernel = (getenv("PSB_DP_SIGNAL") && strcmp(getenv("PSB_DP_SIGNAL"), "fence") == 0) ? 1 : 0;
-	push.fence_in_kernel = fence_in_kernel; sh.fence_in_kernel = fence_in_kernel;
+	push.world = d->world; push.rank = d->rank; push.nlocal_max = d->nlocal_max; push.epoch = epoch;
 	sh.inbox = reinterpret_cast<const float*>(d->base + d->off_inbox);
 	sh.meta = reinterpret_cast<const float*>(d->base + d->off_meta);
-	sh.g_rest = d->g_rest; sh.done_counter = d->local + 1;
+	sh.g_rest = d->g_rest;
 	sh.world = d->world; sh.rank = d->rank; sh.nlocal_max = d->nlocal_max; sh.P = P; sh.epoch = epoch;
-	static const int rotate = (getenv("PSB_DP_ROTATE") && atoi(getenv("PSB_DP_ROTATE")) == 0) ? 0 : 1;
-	sh.rotate = rotate;
-	// TMA bulk stores for the small-parameter chunks: verified over 2 GPUs (same result, same time as per-thread stores); not yet measured
-	// on 8 — the default stays the configuration the 8-GPU numbers in profiles/ were taken with
-	static const int bulk = (getenv("PSB_DP_BULK") && atoi(getenv("PSB_DP_BULK")) != 0) ? 1 : 0;
-	sh.bulk = bulk;
 	// Pipeline over groups of chunks: [main stream] push backward of group g (records go straight into the owners' inboxes) + signal;
 	// [adam stream] wait until every rank's records of group g have landed -> Adam of the owned rows of group g, updated rows stored to
 	// every replica + signal. With one group everything stays on the main stream. Flag word of (group g, rank r) = g * world + r.
@@ -481,7 +472,7 @@ int psb_dp_step_depth(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* 
 	t->mark(7, stream);
 	t->mark(8, stream);
 	for (int g = 0; g < d->groups; g++) {
-		if ((rc = launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_gflag) + g * d->world, d->world, epoch, d->local + 2, as))) return rc;
+		if ((rc = launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_gflag) + g * d->world, d->world, epoch, d->status, as))) return rc;
 		DpShard sg = sh;
 		for (int j = 0; j < d->world; j++) sg.param_flag[j] = sh.param_flag[j] + g * d->world;
 		sg.lc_first = g * (d->chunks_per_group / d->world);
