@@ -80,6 +80,42 @@ int psb_rasterize_backward(int P, int D, int M, int R,
                            float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
                            void* stream);
 
+/*
+ * Depth on the operator path. D(p) = sum_i z_i alpha_i T_i as defined for the trainer below (un-normalised expected depth,
+ * z = view-space depth, alpha and T those of the colour, no background term), rendered over the same full-rectangle
+ * instance lists as psb_rasterize_forward.
+ *
+ * psb_rasterize_forward_depth: psb_rasterize_forward plus out_depth [H,W] (device). out_depth == NULL is psb_rasterize_forward.
+ * Colour, radii, num_rendered and the scratch contents are bit-identical to psb_rasterize_forward's on the same inputs.
+ *
+ * psb_rasterize_backward_depth: psb_rasterize_backward plus dL_ddepth [H,W] (device, or NULL = psb_rasterize_backward) and
+ * dL_dz [P] (caller-allocated, ZERO-INITIALISED, device), which receives dL/dz of every Gaussian. dL/dz is folded into dL_dmean3D,
+ * and dL_dmean2D includes the depth term's screen-space part, so densification statistics taken from it include depth.
+ * PSB_ERR_ARG for dL_ddepth without dL_dz, and for everything psb_rasterize_backward rejects.
+ */
+int psb_rasterize_forward_depth(psb_alloc_fn geometry_buffer, void* geometry_user,
+                                psb_alloc_fn binning_buffer, void* binning_user,
+                                psb_alloc_fn image_buffer, void* image_user,
+                                int P, int D, int M,
+                                const float* background, int width, int height,
+                                const float* means3D, const float* shs, const float* colors_precomp,
+                                const float* opacities, const float* scales, float scale_modifier,
+                                const float* rotations, const float* cov3D_precomp,
+                                const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                                float tan_fovx, float tan_fovy, int prefiltered,
+                                float* out_color, int* radii, float* out_depth, void* stream);
+int psb_rasterize_backward_depth(int P, int D, int M, int R,
+                                 const float* background, int width, int height,
+                                 const float* means3D, const float* shs, const float* colors_precomp,
+                                 const float* scales, float scale_modifier, const float* rotations,
+                                 const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix,
+                                 const float* campos, float tan_fovx, float tan_fovy, const int* radii,
+                                 char* geom_buffer, char* binning_buffer, char* image_buffer,
+                                 const float* dL_dpix,
+                                 float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                                 float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
+                                 const float* dL_ddepth, float* dL_dz, void* stream);
+
 /* Near-plane visibility (view z > 0.2). Replaces CudaRasterizer::Rasterizer::markVisible
  * (cuda_rasterizer/rasterizer.h:24-29, rasterizer_impl.cu:141-153). present: [P] bytes (bool), device. */
 int psb_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,

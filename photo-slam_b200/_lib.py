@@ -37,6 +37,11 @@ def lib():
     L.psb_rasterize_backward.argtypes = [
         C.c_int, C.c_int, C.c_int, C.c_int, fp, C.c_int, C.c_int, fp, fp, fp, fp, C.c_float, fp, fp, fp, fp, fp,
         C.c_float, C.c_float, ip, vp, vp, vp, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, vp]
+    # the _depth variants: the plain argument list plus out_depth, and plus dL_ddepth, dL_dz, before the stream
+    L.psb_rasterize_forward_depth.restype = C.c_int
+    L.psb_rasterize_forward_depth.argtypes = L.psb_rasterize_forward.argtypes[:-1] + [fp, vp]
+    L.psb_rasterize_backward_depth.restype = C.c_int
+    L.psb_rasterize_backward_depth.argtypes = L.psb_rasterize_backward.argtypes[:-1] + [fp, fp, vp]
     L.psb_mark_visible.restype = C.c_int
     L.psb_mark_visible.argtypes = [C.c_int, fp, fp, fp, u8p, vp]
     L.psb_debug_export.restype = C.c_int

@@ -73,6 +73,100 @@ __global__ void export_keys_kernel(int R, const uint32_t* tile_key, const uint32
 	if (values) values[i] = g;
 }
 
+static int arg_error(const char* fn, const char* what)
+{
+	g_last_error = std::string(fn) + ": " + what;
+	return PSB_ERR_ARG;
+}
+
+// Body of psb_rasterize_forward[_depth]; fn names the entry point in error messages. out_depth [H,W] or NULL.
+static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void* geometry_user, psb_alloc_fn binning_buffer, void* binning_user,
+                             psb_alloc_fn image_buffer, void* image_user, int P, int D, int M, const float* background, int width, int height,
+                             const float* means3D, const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
+                             float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
+                             const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered, float* out_color,
+                             int* radii, float* out_depth, void* stream_)
+{
+	(void)prefiltered;  // the reference only uses it for a device-side assert (auxiliary.h:156-160)
+	cudaStream_t stream = (cudaStream_t)stream_;
+	if (P < 0 || width <= 0 || height <= 0 || !geometry_buffer || !binning_buffer || !image_buffer) return arg_error(fn, "bad argument");
+	if (P > 0 && (!means3D || !opacities || !viewmatrix || !projmatrix || !background || !out_color)) return arg_error(fn, "null required pointer");
+	if (P > 0 && ((shs == nullptr) == (colors_precomp == nullptr))) return arg_error(fn, "provide exactly one of shs / colors_precomp");
+	if (P > 0 && (((scales == nullptr) || (rotations == nullptr)) == (cov3D_precomp == nullptr))) return arg_error(fn, "provide exactly one of scales+rotations / cov3D_precomp");
+	if (P > 0 && shs && (M < (D + 1) * (D + 1) || D > 3 || D < 0)) return arg_error(fn, "SH degree / coefficient count mismatch");
+	if (P > 0 && shs && !cam_pos) return arg_error(fn, "cam_pos required with shs");
+	if (width > 65535 * 16 || height > 65535 * 16) return arg_error(fn, "image too large");
+
+	const Camera cam = make_camera(width, height, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy);
+	if ((size_t)cam.grid_x * cam.grid_y >= (1u << 24)) return arg_error(fn, "more than 2^24 tiles");
+
+	char* geom_chunk = geometry_buffer(required_bytes<GeomState>((size_t)P), geometry_user);
+	char* img_chunk = image_buffer(required_bytes<ImgState>((size_t)width * height), image_user);
+	if (!geom_chunk || !img_chunk) return arg_error(fn, "allocator returned null");
+	GeomState geom = GeomState::from_chunk(geom_chunk, (size_t)P);
+	ImgState img = ImgState::from_chunk(img_chunk, (size_t)width * height);
+
+	const GaussIn in = make_input(P, D, M, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp);
+	int rc;
+	if ((rc = launch_preprocess(in, cam, radii, geom, /*raw=*/false, /*tight=*/false, stream))) return rc;
+	if ((rc = launch_depth_sort_and_scan(P, geom, /*scan=*/true, stream))) return rc;
+
+	uint32_t num_rendered = 0;
+	if (P > 0) {
+		PSB_CUDA_OK(cudaMemcpyAsync(&num_rendered, geom.counters, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+		PSB_CUDA_OK(cudaStreamSynchronize(stream));
+	}
+	if (num_rendered >= (1u << 30)) { g_last_error = std::string(fn) + ": more than 2^30 instances"; return PSB_ERR_SIZE; }
+
+	char* bin_chunk = binning_buffer(required_bytes<BinState>((size_t)num_rendered), binning_user);
+	if (!bin_chunk) return arg_error(fn, "allocator returned null");
+	BinState bin = BinState::from_chunk(bin_chunk, (size_t)num_rendered);
+	if ((rc = launch_binning(P, cam, geom, bin, img, (size_t)num_rendered, stream))) return rc;
+
+	const int res = make_sort_plan(tile_id_bits(cam.grid_x * cam.grid_y)).npass & 1;
+	if ((rc = launch_render_forward(cam, img.ranges, bin.inst[res], geom.rec, background, out_color, img.final_T, img.n_contrib, stream, out_depth)))
+		return rc;
+	return (int)num_rendered;
+}
+
+// Body of psb_rasterize_backward[_depth]. dL_ddepth [H,W] or NULL; with it, dL_dz [P] receives dL/dz and the depth variants run.
+static int rasterize_backward(const char* fn, int P, int D, int M, int R, const float* background, int width, int height, const float* means3D,
+                              const float* shs, const float* colors_precomp, const float* scales, float scale_modifier, const float* rotations,
+                              const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix, const float* campos, float tan_fovx,
+                              float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer, const float* dL_dpix,
+                              float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dmean3D, float* dL_dcov3D,
+                              float* dL_dsh, float* dL_dscale, float* dL_drot, const float* dL_ddepth, float* dL_dz, void* stream_)
+{
+	(void)radii;  // visibility is re-derived from the private geometry state (tiles_touched), identical to radii > 0
+	cudaStream_t stream = (cudaStream_t)stream_;
+	if (P == 0) return 0;
+	if (P < 0 || R < 0 || !geom_buffer || !binning_buffer || !image_buffer || !dL_dpix || !dL_dmean2D || !dL_dconic || !dL_dopacity || !dL_dcolor)
+		return arg_error(fn, "bad argument");
+	const Camera cam = make_camera(width, height, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy);
+	GeomState geom = GeomState::from_chunk(geom_buffer, (size_t)P);
+	BinState bin = BinState::from_chunk(binning_buffer, (size_t)R);
+	ImgState img = ImgState::from_chunk(image_buffer, (size_t)width * height);
+	const int res = make_sort_plan(tile_id_bits(cam.grid_x * cam.grid_y)).npass & 1;
+
+	GradSink sink;
+	sink.mean2D = dL_dmean2D; sink.mean2D_stride = 3;
+	sink.conic = dL_dconic; sink.conic_stride = 4;
+	sink.opacity = dL_dopacity; sink.opacity_stride = 1;
+	sink.color = dL_dcolor; sink.color_stride = 3;
+	sink.packed = 0;
+	if (dL_ddepth) { sink.z = dL_dz; sink.z_stride = 1; }
+	int rc;
+	if (R > 0)
+		if ((rc = launch_render_backward(cam, img.ranges, bin.inst[res], geom.rec, background, img.final_T, img.n_contrib, dL_dpix, sink, stream, dL_ddepth)))
+			return rc;
+
+	const GaussIn in = make_input(P, D, M, means3D, shs, colors_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp);
+	GaussGradOut out;
+	out.dL_dmeans3D = dL_dmean3D; out.dL_dcov3D = dL_dcov3D; out.dL_dsh = dL_dsh; out.dL_dscales = dL_dscale; out.dL_drots = dL_drot;
+	if ((rc = launch_preprocess_backward(in, cam, geom, dL_dmean2D, 3, dL_dconic, 4, dL_dcolor, 3, out, stream, dL_ddepth ? dL_dz : nullptr))) return rc;
+	return 0;
+}
+
 }  // namespace psb
 
 using namespace psb;
@@ -91,47 +185,23 @@ int psb_rasterize_forward(psb_alloc_fn geometry_buffer, void* geometry_user, psb
                           const float* means3D, const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
                           float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
                           const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered, float* out_color,
-                          int* radii, void* stream_)
+                          int* radii, void* stream)
 {
-	(void)prefiltered;  // the reference only uses it for a device-side assert (auxiliary.h:156-160)
-	cudaStream_t stream = (cudaStream_t)stream_;
-	if (P < 0 || width <= 0 || height <= 0 || !geometry_buffer || !binning_buffer || !image_buffer) { set_error_msg("psb_rasterize_forward: bad argument"); return PSB_ERR_ARG; }
-	if (P > 0 && (!means3D || !opacities || !viewmatrix || !projmatrix || !background || !out_color)) { set_error_msg("psb_rasterize_forward: null required pointer"); return PSB_ERR_ARG; }
-	if (P > 0 && ((shs == nullptr) == (colors_precomp == nullptr))) { set_error_msg("psb_rasterize_forward: provide exactly one of shs / colors_precomp"); return PSB_ERR_ARG; }
-	if (P > 0 && (((scales == nullptr) || (rotations == nullptr)) == (cov3D_precomp == nullptr))) { set_error_msg("psb_rasterize_forward: provide exactly one of scales+rotations / cov3D_precomp"); return PSB_ERR_ARG; }
-	if (P > 0 && shs && (M < (D + 1) * (D + 1) || D > 3 || D < 0)) { set_error_msg("psb_rasterize_forward: SH degree / coefficient count mismatch"); return PSB_ERR_ARG; }
-	if (P > 0 && shs && !cam_pos) { set_error_msg("psb_rasterize_forward: cam_pos required with shs"); return PSB_ERR_ARG; }
-	if (width > 65535 * 16 || height > 65535 * 16) { set_error_msg("psb_rasterize_forward: image too large"); return PSB_ERR_ARG; }
+	return rasterize_forward("psb_rasterize_forward", geometry_buffer, geometry_user, binning_buffer, binning_user, image_buffer, image_user, P, D, M,
+	                         background, width, height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp,
+	                         viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, nullptr, stream);
+}
 
-	const Camera cam = make_camera(width, height, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy);
-	if ((size_t)cam.grid_x * cam.grid_y >= (1u << 24)) { set_error_msg("psb_rasterize_forward: more than 2^24 tiles"); return PSB_ERR_ARG; }
-
-	char* geom_chunk = geometry_buffer(required_bytes<GeomState>((size_t)P), geometry_user);
-	char* img_chunk = image_buffer(required_bytes<ImgState>((size_t)width * height), image_user);
-	if (!geom_chunk || !img_chunk) { set_error_msg("psb_rasterize_forward: allocator returned null"); return PSB_ERR_ARG; }
-	GeomState geom = GeomState::from_chunk(geom_chunk, (size_t)P);
-	ImgState img = ImgState::from_chunk(img_chunk, (size_t)width * height);
-
-	const GaussIn in = make_input(P, D, M, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp);
-	int rc;
-	if ((rc = launch_preprocess(in, cam, radii, geom, /*raw=*/false, /*tight=*/false, stream))) return rc;
-	if ((rc = launch_depth_sort_and_scan(P, geom, /*scan=*/true, stream))) return rc;
-
-	uint32_t num_rendered = 0;
-	if (P > 0) {
-		PSB_CUDA_OK(cudaMemcpyAsync(&num_rendered, geom.counters, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
-		PSB_CUDA_OK(cudaStreamSynchronize(stream));
-	}
-	if (num_rendered >= (1u << 30)) { set_error_msg("psb_rasterize_forward: more than 2^30 instances"); return PSB_ERR_SIZE; }
-
-	char* bin_chunk = binning_buffer(required_bytes<BinState>((size_t)num_rendered), binning_user);
-	if (!bin_chunk) { set_error_msg("psb_rasterize_forward: allocator returned null"); return PSB_ERR_ARG; }
-	BinState bin = BinState::from_chunk(bin_chunk, (size_t)num_rendered);
-	if ((rc = launch_binning(P, cam, geom, bin, img, (size_t)num_rendered, stream))) return rc;
-
-	const int res = make_sort_plan(tile_id_bits(cam.grid_x * cam.grid_y)).npass & 1;
-	if ((rc = launch_render_forward(cam, img.ranges, bin.inst[res], geom.rec, background, out_color, img.final_T, img.n_contrib, stream))) return rc;
-	return (int)num_rendered;
+int psb_rasterize_forward_depth(psb_alloc_fn geometry_buffer, void* geometry_user, psb_alloc_fn binning_buffer, void* binning_user,
+                                psb_alloc_fn image_buffer, void* image_user, int P, int D, int M, const float* background, int width, int height,
+                                const float* means3D, const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
+                                float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
+                                const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered, float* out_color,
+                                int* radii, float* out_depth, void* stream)
+{
+	return rasterize_forward("psb_rasterize_forward_depth", geometry_buffer, geometry_user, binning_buffer, binning_user, image_buffer, image_user, P,
+	                         D, M, background, width, height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations,
+	                         cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, out_depth, stream);
 }
 
 int psb_rasterize_backward(int P, int D, int M, int R, const float* background, int width, int height, const float* means3D, const float* shs,
@@ -139,36 +209,27 @@ int psb_rasterize_backward(int P, int D, int M, int R, const float* background, 
                            const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix, const float* campos, float tan_fovx,
                            float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer, const float* dL_dpix,
                            float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dmean3D, float* dL_dcov3D,
-                           float* dL_dsh, float* dL_dscale, float* dL_drot, void* stream_)
+                           float* dL_dsh, float* dL_dscale, float* dL_drot, void* stream)
 {
-	(void)radii;  // visibility is re-derived from the private geometry state (tiles_touched), identical to radii > 0
-	cudaStream_t stream = (cudaStream_t)stream_;
-	if (P == 0) return 0;
-	if (P < 0 || R < 0 || !geom_buffer || !binning_buffer || !image_buffer || !dL_dpix || !dL_dmean2D || !dL_dconic || !dL_dopacity || !dL_dcolor) {
-		set_error_msg("psb_rasterize_backward: bad argument");
-		return PSB_ERR_ARG;
-	}
-	const Camera cam = make_camera(width, height, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy);
-	GeomState geom = GeomState::from_chunk(geom_buffer, (size_t)P);
-	BinState bin = BinState::from_chunk(binning_buffer, (size_t)R);
-	ImgState img = ImgState::from_chunk(image_buffer, (size_t)width * height);
-	const int res = make_sort_plan(tile_id_bits(cam.grid_x * cam.grid_y)).npass & 1;
+	return rasterize_backward("psb_rasterize_backward", P, D, M, R, background, width, height, means3D, shs, colors_precomp, scales, scale_modifier,
+	                          rotations, cov3D_precomp, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, radii, geom_buffer, binning_buffer,
+	                          image_buffer, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale,
+	                          dL_drot, nullptr, nullptr, stream);
+}
 
-	GradSink sink;
-	sink.mean2D = dL_dmean2D; sink.mean2D_stride = 3;
-	sink.conic = dL_dconic; sink.conic_stride = 4;
-	sink.opacity = dL_dopacity; sink.opacity_stride = 1;
-	sink.color = dL_dcolor; sink.color_stride = 3;
-	sink.packed = 0;
-	int rc;
-	if (R > 0)
-		if ((rc = launch_render_backward(cam, img.ranges, bin.inst[res], geom.rec, background, img.final_T, img.n_contrib, dL_dpix, sink, stream))) return rc;
-
-	const GaussIn in = make_input(P, D, M, means3D, shs, colors_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp);
-	GaussGradOut out;
-	out.dL_dmeans3D = dL_dmean3D; out.dL_dcov3D = dL_dcov3D; out.dL_dsh = dL_dsh; out.dL_dscales = dL_dscale; out.dL_drots = dL_drot;
-	if ((rc = launch_preprocess_backward(in, cam, geom, dL_dmean2D, 3, dL_dconic, 4, dL_dcolor, 3, out, stream))) return rc;
-	return 0;
+int psb_rasterize_backward_depth(int P, int D, int M, int R, const float* background, int width, int height, const float* means3D,
+                                 const float* shs, const float* colors_precomp, const float* scales, float scale_modifier, const float* rotations,
+                                 const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix, const float* campos, float tan_fovx,
+                                 float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer,
+                                 const float* dL_dpix, float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                                 float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, const float* dL_ddepth,
+                                 float* dL_dz, void* stream)
+{
+	if (dL_ddepth && !dL_dz) return arg_error("psb_rasterize_backward_depth", "dL_ddepth needs a dL_dz array");
+	return rasterize_backward("psb_rasterize_backward_depth", P, D, M, R, background, width, height, means3D, shs, colors_precomp, scales,
+	                          scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, radii, geom_buffer,
+	                          binning_buffer, image_buffer, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh,
+	                          dL_dscale, dL_drot, dL_ddepth, dL_dz, stream);
 }
 
 int psb_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix, unsigned char* present, void* stream_)

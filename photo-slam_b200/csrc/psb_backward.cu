@@ -8,9 +8,13 @@
 
 namespace psb {
 
-__global__ void __launch_bounds__(128) preprocess_bwd_kernel(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
-                                                             int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
-                                                             const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out)
+// DEPTH: dL/dz (view-space depth, render_bwd_depth_kernel's tenth sum) joins dL/dmean3D through the view matrix's z row,
+// z = V[2] x + V[6] y + V[10] z + V[14] (column-major), as in gaussian_backward_kernel<MODE_DEPTH>.
+template <bool DEPTH>
+__device__ __forceinline__ void preprocess_bwd_body(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
+                                                    int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
+                                                    const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out,
+                                                    const float* __restrict__ dL_dz)
 {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	if (idx >= in.P || geom.tile_info[idx].z == 0) return;
@@ -40,6 +44,10 @@ __global__ void __launch_bounds__(128) preprocess_bwd_kernel(GaussIn in, Camera 
 	float4 dL_drot = make_float4(0, 0, 0, 0);
 	float dL_dcov[6];
 	gaussian_backward(in, cam, idx, mean, cov3D, scale, rot, sh_row, clamp_bits, g2, gc, gcol, dsh_row, dL_dmean, dL_dcov, dL_dscale, dL_drot);
+	if (DEPTH) {
+		const float dz = dL_dz[idx];
+		dL_dmean.x += dz * cam.view[2]; dL_dmean.y += dz * cam.view[6]; dL_dmean.z += dz * cam.view[10];
+	}
 
 	if (out.dL_dmeans3D) { out.dL_dmeans3D[3 * idx] = dL_dmean.x; out.dL_dmeans3D[3 * idx + 1] = dL_dmean.y; out.dL_dmeans3D[3 * idx + 2] = dL_dmean.z; }
 	if (out.dL_dcov3D) {
@@ -52,13 +60,32 @@ __global__ void __launch_bounds__(128) preprocess_bwd_kernel(GaussIn in, Camera 
 	}
 }
 
+__global__ void __launch_bounds__(128) preprocess_bwd_kernel(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
+                                                             int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
+                                                             const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out)
+{
+	preprocess_bwd_body<false>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out, nullptr);
+}
+
+__global__ void __launch_bounds__(128) preprocess_bwd_depth_kernel(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
+                                                                   int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
+                                                                   const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out,
+                                                                   const float* __restrict__ dL_dz)
+{
+	preprocess_bwd_body<true>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out, dL_dz);
+}
+
 int launch_preprocess_backward(const GaussIn& in, const Camera& cam, const GeomState& geom, const float* dL_dmean2D, int mean2D_stride,
                                const float* dL_dconic, int conic_stride, const float* dL_dcolor, int color_stride,
-                               const GaussGradOut& out, cudaStream_t stream)
+                               const GaussGradOut& out, cudaStream_t stream, const float* dL_dz)
 {
 	if (in.P == 0) return 0;
-	preprocess_bwd_kernel<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor,
-	                                                           color_stride, out);
+	if (dL_dz)
+		preprocess_bwd_depth_kernel<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor,
+		                                                                 color_stride, out, dL_dz);
+	else
+		preprocess_bwd_kernel<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor,
+		                                                           color_stride, out);
 	PSB_LAUNCH_OK();
 	return 0;
 }

@@ -30,6 +30,7 @@ struct GradSink {
 	float* opacity; int opacity_stride;
 	float* color;   int color_stride;    // rgb at +0..2
 	int packed;                          // != 0: one 16-byte aligned [P][12] row layout (mean2D base), vector reductions
+	float* z = nullptr; int z_stride = 0;  // unpacked sink with a depth gradient: the tenth sum, dL/dz (the packed row keeps it in slot 11)
 };
 
 // Outputs of the per-Gaussian backward (any pointer may be null = not wanted).
@@ -51,12 +52,14 @@ int launch_scan_binning(int P, const Camera& cam, const GeomState& geom, BinStat
 int launch_render_forward(const Camera& cam, const uint2* ranges, const uint32_t* point_list, const GaussRec* rec, const float* bg,
                           float* out_color, float* final_T, uint32_t* n_contrib, cudaStream_t stream,
                           float* out_depth = nullptr /* [H,W]: also render the expected depth (depth variant of the kernel) */);
-// dL_ddepth [H,W] (trainer path, packed sink only): depth variant, dL/dz of every Gaussian lands in slot 11 of its sink row
+// dL_ddepth [H,W]: depth variant, dL/dz of every Gaussian lands in slot 11 of its packed sink row, or at sink.z (unpacked sink;
+// refused without either destination)
 int launch_render_backward(const Camera& cam, const uint2* ranges, const uint32_t* point_list, const GaussRec* rec, const float* bg,
                            const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, const GradSink& sink,
                            cudaStream_t stream, const float* dL_ddepth = nullptr);
+// dL_dz [P] (non-null: depth variant): dL/dmean3D += dL/dz (V[2], V[6], V[10]) for every visible Gaussian
 int launch_preprocess_backward(const GaussIn& in, const Camera& cam, const GeomState& geom, const float* dL_dmean2D, int mean2D_stride,
                                const float* dL_dconic, int conic_stride, const float* dL_dcolor, int color_stride,
-                               const GaussGradOut& out, cudaStream_t stream);
+                               const GaussGradOut& out, cudaStream_t stream, const float* dL_dz = nullptr);
 
 }  // namespace psb

@@ -11,6 +11,7 @@
 // code: no kernels here. The TORCH_LIBRARY block at the end only exists so the Python test-suite can call the
 // C++ entry points (torch.ops.psb200.*).
 #include <functional>
+#include <optional>
 #include <stdexcept>
 #include <tuple>
 #include <vector>
@@ -106,6 +107,86 @@ RasterizeGaussiansBackwardCUDA(const torch::Tensor& background, const torch::Ten
 			dL_dmeans3D.data_ptr<float>(), dL_dcov3D.data_ptr<float>(), M ? dL_dsh.data_ptr<float>() : nullptr, dL_dscales.data_ptr<float>(),
 			dL_drotations.data_ptr<float>(), current_stream());
 		if (rc < 0) { AT_ERROR("psb_rasterize_backward: ", psb_last_error()); }
+	}
+	return std::make_tuple(dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations);
+}
+
+// ---- rendered depth D(p) = sum_i z_i alpha_i T_i (include/psb200.h), which the reference has no symbol for: the two functions
+// above with the depth image added, for a GaussianRasterizerFunction that returns and back-propagates depth (INTEGRATION.md §1)
+std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
+RasterizeGaussiansDepthCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors, const torch::Tensor& opacity,
+                            const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier, const torch::Tensor& cov3D_precomp,
+                            const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
+                            const int image_height, const int image_width, const torch::Tensor& sh, const int degree, const torch::Tensor& campos,
+                            const bool prefiltered)
+{
+	if (means3D.ndimension() != 2 || means3D.size(1) != 3) { AT_ERROR("means3D must have dimensions (num_points, 3)"); }
+	const int P = means3D.size(0);
+	const int H = image_height, W = image_width;
+	auto float_opts = means3D.options().dtype(torch::kFloat32);
+	torch::Tensor out_color = torch::full({3, H, W}, 0.0, float_opts);
+	torch::Tensor out_depth = torch::full({H, W}, 0.0, float_opts);
+	torch::Tensor radii = torch::full({P}, 0, means3D.options().dtype(torch::kInt32));
+	torch::TensorOptions options(torch::kByte);
+	torch::Tensor geomBuffer = torch::empty({0}, options.device(means3D.device()));
+	torch::Tensor binningBuffer = torch::empty({0}, options.device(means3D.device()));
+	torch::Tensor imgBuffer = torch::empty({0}, options.device(means3D.device()));
+	int rendered = 0;
+	if (P != 0) {
+		int M = 0;
+		if (sh.size(0) != 0) M = sh.size(1);
+		const auto bg = background.contiguous(), m3 = means3D.contiguous(), shc = sh.contiguous(), col = colors.contiguous(), op = opacity.contiguous(),
+		           sc = scales.contiguous(), rot = rotations.contiguous(), cov = cov3D_precomp.contiguous(), vm = viewmatrix.contiguous(),
+		           pm = projmatrix.contiguous(), cp = campos.contiguous();
+		rendered = psb_rasterize_forward_depth(resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer, P, degree, M, fptr(bg), W, H,
+		                                       fptr(m3), fptr(shc), fptr(col), fptr(op), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm),
+		                                       fptr(pm), fptr(cp), tan_fovx, tan_fovy, prefiltered ? 1 : 0, out_color.data_ptr<float>(),
+		                                       radii.data_ptr<int>(), out_depth.data_ptr<float>(), current_stream());
+		if (rendered < 0) { AT_ERROR("psb_rasterize_forward_depth: ", psb_last_error()); }
+	}
+	return std::make_tuple(rendered, out_color, out_depth, radii, geomBuffer, binningBuffer, imgBuffer);
+}
+
+// dL_dout_depth [H,W]; an undefined tensor is the plain backward. dL/dz is folded into dL_dmeans3D, and dL_dmeans2D includes the depth term.
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
+RasterizeGaussiansBackwardDepthCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii, const torch::Tensor& colors,
+                                    const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier,
+                                    const torch::Tensor& cov3D_precomp, const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix,
+                                    const float tan_fovx, const float tan_fovy, const torch::Tensor& dL_dout_color,
+                                    const torch::Tensor& dL_dout_depth, const torch::Tensor& sh, const int degree, const torch::Tensor& campos,
+                                    const torch::Tensor& geomBuffer, const int R, const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer)
+{
+	const int P = means3D.size(0);
+	const int H = dL_dout_color.size(1), W = dL_dout_color.size(2);
+	const bool depth = dL_dout_depth.defined() && dL_dout_depth.numel() != 0;
+	if (depth && (dL_dout_depth.ndimension() != 2 || dL_dout_depth.size(0) != H || dL_dout_depth.size(1) != W)) {
+		AT_ERROR("dL_dout_depth must have dimensions (", H, ", ", W, ")");
+	}
+	int M = 0;
+	if (sh.size(0) != 0) M = sh.size(1);
+	torch::Tensor dL_dmeans3D = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_dmeans2D = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_dcolors = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_dconic = torch::zeros({P, 2, 2}, means3D.options());
+	torch::Tensor dL_dopacity = torch::zeros({P, 1}, means3D.options());
+	torch::Tensor dL_dcov3D = torch::zeros({P, 6}, means3D.options());
+	torch::Tensor dL_dsh = torch::zeros({P, M, 3}, means3D.options());
+	torch::Tensor dL_dscales = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_drotations = torch::zeros({P, 4}, means3D.options());
+	torch::Tensor dL_dz = torch::zeros({depth ? P : 0}, means3D.options());
+	if (P != 0) {
+		const auto bg = background.contiguous(), m3 = means3D.contiguous(), shc = sh.contiguous(), col = colors.contiguous(), sc = scales.contiguous(),
+		           rot = rotations.contiguous(), cov = cov3D_precomp.contiguous(), vm = viewmatrix.contiguous(), pm = projmatrix.contiguous(),
+		           cp = campos.contiguous(), dpix = dL_dout_color.contiguous(), rad = radii.contiguous();
+		const torch::Tensor ddep = depth ? dL_dout_depth.contiguous() : torch::Tensor();
+		const int rc = psb_rasterize_backward_depth(
+			P, degree, M, R, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
+			tan_fovx, tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(geomBuffer.contiguous().data_ptr()),
+			reinterpret_cast<char*>(binningBuffer.contiguous().data_ptr()), reinterpret_cast<char*>(imageBuffer.contiguous().data_ptr()), fptr(dpix),
+			dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(), dL_dopacity.data_ptr<float>(), dL_dcolors.data_ptr<float>(),
+			dL_dmeans3D.data_ptr<float>(), dL_dcov3D.data_ptr<float>(), M ? dL_dsh.data_ptr<float>() : nullptr, dL_dscales.data_ptr<float>(),
+			dL_drotations.data_ptr<float>(), depth ? ddep.data_ptr<float>() : nullptr, depth ? dL_dz.data_ptr<float>() : nullptr, current_stream());
+		if (rc < 0) { AT_ERROR("psb_rasterize_backward_depth: ", psb_last_error()); }
 	}
 	return std::make_tuple(dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations);
 }
@@ -282,6 +363,21 @@ std::tuple<T, T, T, T, T, T, T, T> op_bwd(const T& bg, const T& m3, const T& rad
 {
 	return RasterizeGaussiansBackwardCUDA(bg, m3, radii, col, sc, rot, (float)smod, cov, vm, pm, (float)tfx, (float)tfy, dpix, sh, (int)deg, cp, gb, (int)R, bb, ib);
 }
+std::tuple<int64_t, T, T, T, T, T, T> op_fwd_depth(const T& bg, const T& m3, const T& col, const T& op, const T& sc, const T& rot, double smod,
+                                                   const T& cov, const T& vm, const T& pm, double tfx, double tfy, int64_t H, int64_t W, const T& sh,
+                                                   int64_t deg, const T& cp, bool pre)
+{
+	auto r = RasterizeGaussiansDepthCUDA(bg, m3, col, op, sc, rot, (float)smod, cov, vm, pm, (float)tfx, (float)tfy, (int)H, (int)W, sh, (int)deg, cp, pre);
+	return std::make_tuple((int64_t)std::get<0>(r), std::get<1>(r), std::get<2>(r), std::get<3>(r), std::get<4>(r), std::get<5>(r), std::get<6>(r));
+}
+std::tuple<T, T, T, T, T, T, T, T> op_bwd_depth(const T& bg, const T& m3, const T& radii, const T& col, const T& sc, const T& rot, double smod,
+                                                const T& cov, const T& vm, const T& pm, double tfx, double tfy, const T& dpix,
+                                                const std::optional<T>& ddep, const T& sh, int64_t deg, const T& cp, const T& gb, int64_t R, const T& bb,
+                                                const T& ib)
+{
+	return RasterizeGaussiansBackwardDepthCUDA(bg, m3, radii, col, sc, rot, (float)smod, cov, vm, pm, (float)tfx, (float)tfy, dpix, ddep.value_or(T()), sh,
+	                                           (int)deg, cp, gb, (int)R, bb, ib);
+}
 T op_vis(T m3, T vm, T pm) { return markVisible(m3, vm, pm); }
 T op_dist(const T& p) { return distCUDA2(p); }
 T op_xform(T p, T m) { transformPoints(p, m); return p; }
@@ -315,6 +411,8 @@ TORCH_LIBRARY(psb200, m)
 {
 	m.def("rasterize_gaussians", &op_fwd);
 	m.def("rasterize_gaussians_backward", &op_bwd);
+	m.def("rasterize_gaussians_depth", &op_fwd_depth);
+	m.def("rasterize_gaussians_backward_depth", &op_bwd_depth);
 	m.def("mark_visible", &op_vis);
 	m.def("b2_forward", &op_b2_fwd);
 	m.def("dist_cuda2", &op_dist);

@@ -7,6 +7,10 @@ Mirrors, name for name and argument for argument:
   rasterizeGaussians, GaussianRasterizer
       reference include/gaussian_rasterizer.h:25-127, src/gaussian_rasterizer.cpp:28-234
 
+Rendered depth D(p) = sum_i z_i alpha_i T_i (include/psb200.h), which the reference does not have:
+  RasterizeGaussiansDepthCUDA / RasterizeGaussiansBackwardDepthCUDA   the two functions above plus the depth image and its gradient
+  _RasterizeGaussiansDepth, GaussianRasterizer.forward(..., return_depth=True)   autograd through colour and depth
+
 PyTorch is used only for device memory, streams and autograd bookkeeping.
 """
 from dataclasses import dataclass
@@ -48,16 +52,16 @@ class _Scratch:
         return self.tensor.data_ptr()
 
 
-def RasterizeGaussiansCUDA(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
-                           viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos,
-                           prefiltered):
-    """-> (num_rendered, out_color [3,H,W], radii [P] int32, geomBuffer, binningBuffer, imgBuffer)."""
+def _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
+             tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, depth):
+    """RasterizeGaussiansCUDA, and with depth=True also the [H,W] depth image (psb_rasterize_forward_depth)."""
     if means3D.dim() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")  # AT_ERROR in the reference
     L = _lib.lib()
     dev = means3D.device
     P, H, W = means3D.size(0), int(image_height), int(image_width)
     out_color = torch.zeros((3, H, W), dtype=torch.float32, device=dev)
+    out_depth = torch.zeros((H, W), dtype=torch.float32, device=dev) if depth else None
     radii = torch.zeros((P,), dtype=torch.int32, device=dev)
     geom, binning, img = _Scratch(dev), _Scratch(dev), _Scratch(dev)
     rendered = 0
@@ -66,18 +70,39 @@ def RasterizeGaussiansCUDA(background, means3D, colors, opacity, scales, rotatio
         tensors = [_f32c(t) for t in (background, means3D, sh, colors, opacity, scales, rotations, cov3D_precomp,
                                       viewmatrix, projmatrix, campos)]
         bg, m3, shc, col, opa, sca, rot, cov, vm, pm, cp = tensors
-        rendered = _lib.check(L.psb_rasterize_forward(
-            geom.cb, None, binning.cb, None, img.cb, None, P, int(degree), int(M), _ptr(bg), W, H,
-            _ptr(m3), _ptr(shc), _ptr(col), _ptr(opa), _ptr(sca), float(scale_modifier), _ptr(rot), _ptr(cov),
-            _ptr(vm), _ptr(pm), _ptr(cp), float(tan_fovx), float(tan_fovy), int(bool(prefiltered)),
-            out_color.data_ptr(), radii.data_ptr(), _stream()), "psb_rasterize_forward")
-    return rendered, out_color, radii, geom.tensor, binning.tensor, img.tensor
+        args = [geom.cb, None, binning.cb, None, img.cb, None, P, int(degree), int(M), _ptr(bg), W, H,
+                _ptr(m3), _ptr(shc), _ptr(col), _ptr(opa), _ptr(sca), float(scale_modifier), _ptr(rot), _ptr(cov),
+                _ptr(vm), _ptr(pm), _ptr(cp), float(tan_fovx), float(tan_fovy), int(bool(prefiltered)),
+                out_color.data_ptr(), radii.data_ptr()]
+        if depth:
+            rendered = _lib.check(L.psb_rasterize_forward_depth(*args, out_depth.data_ptr(), _stream()), "psb_rasterize_forward_depth")
+        else:
+            rendered = _lib.check(L.psb_rasterize_forward(*args, _stream()), "psb_rasterize_forward")
+    return rendered, out_color, out_depth, radii, geom.tensor, binning.tensor, img.tensor
 
 
-def RasterizeGaussiansBackwardCUDA(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp,
-                                   viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, sh, degree, campos,
-                                   geomBuffer, R, binningBuffer, imageBuffer):
-    """-> (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations)."""
+def RasterizeGaussiansCUDA(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
+                           viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos,
+                           prefiltered):
+    """-> (num_rendered, out_color [3,H,W], radii [P] int32, geomBuffer, binningBuffer, imgBuffer)."""
+    rendered, out_color, _, radii, geom, binning, img = _forward(
+        background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx,
+        tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, depth=False)
+    return rendered, out_color, radii, geom, binning, img
+
+
+def RasterizeGaussiansDepthCUDA(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
+                                viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos,
+                                prefiltered):
+    """RasterizeGaussiansCUDA plus the depth image -> (num_rendered, out_color [3,H,W], out_depth [H,W], radii [P] int32, geomBuffer,
+    binningBuffer, imgBuffer). Colour, radii and buffers are bit-identical to RasterizeGaussiansCUDA's."""
+    return _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
+                    tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, depth=True)
+
+
+def _backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
+              tan_fovx, tan_fovy, dL_dout_color, dL_dout_depth, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer):
+    """RasterizeGaussiansBackwardCUDA, and with a depth gradient psb_rasterize_backward_depth."""
     L = _lib.lib()
     P = means3D.size(0)
     H, W = dL_dout_color.size(1), dL_dout_color.size(2)
@@ -96,14 +121,37 @@ def RasterizeGaussiansBackwardCUDA(background, means3D, radii, colors, scales, r
         tensors = [_f32c(t) for t in (background, means3D, sh, colors, scales, rotations, cov3D_precomp, viewmatrix,
                                       projmatrix, campos, dL_dout_color)]
         bg, m3, shc, col, sca, rot, cov, vm, pm, cp, dpix = tensors
-        _lib.check(L.psb_rasterize_backward(
-            P, int(degree), int(M), int(R), _ptr(bg), W, H, _ptr(m3), _ptr(shc), _ptr(col), _ptr(sca),
-            float(scale_modifier), _ptr(rot), _ptr(cov), _ptr(vm), _ptr(pm), _ptr(cp), float(tan_fovx), float(tan_fovy),
-            _ptr(radii), _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imageBuffer), _ptr(dpix),
-            dL_dmeans2D.data_ptr(), dL_dconic.data_ptr(), dL_dopacity.data_ptr(), dL_dcolors.data_ptr(),
-            dL_dmeans3D.data_ptr(), dL_dcov3D.data_ptr(), _ptr(dL_dsh), dL_dscales.data_ptr(), dL_drotations.data_ptr(),
-            _stream()), "psb_rasterize_backward")
+        args = [P, int(degree), int(M), int(R), _ptr(bg), W, H, _ptr(m3), _ptr(shc), _ptr(col), _ptr(sca),
+                float(scale_modifier), _ptr(rot), _ptr(cov), _ptr(vm), _ptr(pm), _ptr(cp), float(tan_fovx), float(tan_fovy),
+                _ptr(radii), _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imageBuffer), _ptr(dpix),
+                dL_dmeans2D.data_ptr(), dL_dconic.data_ptr(), dL_dopacity.data_ptr(), dL_dcolors.data_ptr(),
+                dL_dmeans3D.data_ptr(), dL_dcov3D.data_ptr(), _ptr(dL_dsh), dL_dscales.data_ptr(), dL_drotations.data_ptr()]
+        if dL_dout_depth is not None:
+            ddep = _f32c(dL_dout_depth)
+            if tuple(ddep.shape) != (H, W):
+                raise RuntimeError(f"dL_dout_depth must have dimensions ({H}, {W})")
+            dL_dz = torch.zeros((P,), **o)      # [P], zero-initialised as the C-ABI requires; folded into dL_dmeans3D there
+            _lib.check(L.psb_rasterize_backward_depth(*args, ddep.data_ptr(), dL_dz.data_ptr(), _stream()), "psb_rasterize_backward_depth")
+        else:
+            _lib.check(L.psb_rasterize_backward(*args, _stream()), "psb_rasterize_backward")
     return dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations
+
+
+def RasterizeGaussiansBackwardCUDA(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp,
+                                   viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, sh, degree, campos,
+                                   geomBuffer, R, binningBuffer, imageBuffer):
+    """-> (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations)."""
+    return _backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
+                     tan_fovx, tan_fovy, dL_dout_color, None, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer)
+
+
+def RasterizeGaussiansBackwardDepthCUDA(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp,
+                                        viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, dL_dout_depth, sh, degree, campos,
+                                        geomBuffer, R, binningBuffer, imageBuffer):
+    """RasterizeGaussiansBackwardCUDA with the gradient of the depth image as well (dL_dout_depth [H,W]; None = the plain backward).
+    dL/dz is folded into dL_dmeans3D, and dL_dmeans2D includes the depth term. Returns the same 8-tuple."""
+    return _backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
+                     tan_fovx, tan_fovy, dL_dout_color, dL_dout_depth, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer)
 
 
 def markVisible(means3D, viewmatrix, projmatrix):
@@ -165,6 +213,42 @@ class _RasterizeGaussians(torch.autograd.Function):
                 g(grad_scales, scales), g(grad_rotations, rotations), g(grad_cov3Ds_precomp, cov3Ds_precomp), None)
 
 
+class _RasterizeGaussiansDepth(torch.autograd.Function):
+    """_RasterizeGaussians with the depth image as a third, differentiable output."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):
+        rs = raster_settings
+        num_rendered, color, depth, radii, geomBuffer, binningBuffer, imgBuffer = RasterizeGaussiansDepthCUDA(
+            rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
+            rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, sh, rs.sh_degree,
+            rs.campos, rs.prefiltered)
+        ctx.raster_settings = rs
+        ctx.num_rendered = num_rendered
+        ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
+                              binningBuffer, imgBuffer)
+        ctx.mark_non_differentiable(radii)
+        ctx.set_materialize_grads(False)    # an output the loss does not use arrives as None, not as a zero image
+        return color, radii, depth
+
+    @staticmethod
+    def backward(ctx, grad_out_color, _grad_radii, grad_out_depth):
+        rs = ctx.raster_settings
+        colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer = ctx.saved_tensors
+        if grad_out_color is None:
+            grad_out_color = torch.zeros((3, rs.image_height, rs.image_width), dtype=torch.float32, device=means3D.device)
+        (grad_means2D, grad_colors_precomp, grad_opacities, grad_means3D, grad_cov3Ds_precomp, grad_sh, grad_scales,
+         grad_rotations) = RasterizeGaussiansBackwardDepthCUDA(
+            rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix,
+            rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_out_color, grad_out_depth, sh, rs.sh_degree, rs.campos, geomBuffer,
+            ctx.num_rendered, binningBuffer, imgBuffer)
+
+        def g(t, ref):
+            return t if (ref is not None and ref.numel() != 0) else None
+        return (grad_means3D, grad_means2D, g(grad_sh, sh), g(grad_colors_precomp, colors_precomp), grad_opacities,
+                g(grad_scales, scales), g(grad_rotations, rotations), g(grad_cov3Ds_precomp, cov3Ds_precomp), None)
+
+
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):
     """reference rasterizeGaussians (include/gaussian_rasterizer.h:77-99)."""
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
@@ -182,7 +266,8 @@ class GaussianRasterizer:
             return markVisible(positions, self.raster_settings.viewmatrix, self.raster_settings.projmatrix)
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
-                cov3D_precomp=None):
+                cov3D_precomp=None, return_depth=False):
+        """-> (color, radii), or (color, radii, depth [H,W]) with return_depth=True (differentiable, as the colour)."""
         has = lambda t: t is not None and t.numel() != 0
         if has(shs) == has(colors_precomp):
             raise RuntimeError("Please provide excatly one of either SHs or precomputed colors!")
@@ -190,6 +275,9 @@ class GaussianRasterizer:
             raise RuntimeError("Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!")
         empty = torch.empty(0, dtype=torch.float32, device=means3D.device)
         e = lambda t: t if has(t) else empty
+        if return_depth:
+            return _RasterizeGaussiansDepth.apply(means3D, means2D, e(shs), e(colors_precomp), opacities, e(scales), e(rotations),
+                                                  e(cov3D_precomp), self.raster_settings)
         return rasterize_gaussians(means3D, means2D, e(shs), e(colors_precomp), opacities, e(scales), e(rotations),
                                    e(cov3D_precomp), self.raster_settings)
 

@@ -7,8 +7,8 @@ EVERY pipeline branch, on top of the psb200 rasterizer operator (rasterizer.Gaus
   default              raw SH rows to the rasterizer                                               (:114-117)
 
 and any SH storage size M = (max_sh_degree + 1)^2 (the operator-level path takes M from the tensor). The result tuple is the
-reference's: (rendered_image, viewspace_points, visibility_filter, radii); gradients flow through torch autograd into the model
-tensors, and viewspace_points.grad[:, :2] feeds addDensificationStats like in the reference.
+reference's: (rendered_image, viewspace_points, visibility_filter, radii), plus the depth image with return_depth=True; gradients
+flow through torch autograd into the model tensors, and viewspace_points.grad[:, :2] feeds addDensificationStats like in the reference.
 
 This is the general, differentiable path. The trainer's hot loop does not come through here: psb_trainer_step / psb_trainer_render fuse
 the default branch (activations, SH gather, loss, backward, Adam) into the kernels; tests/test_renderer_gpu.py checks that both paths draw
@@ -54,9 +54,11 @@ def get_covariance_activation(model, scaling_modifier=1.0):
 
 
 def render(viewpoint_camera, image_height, image_width, pc, pipe=None, bg_color=None, override_color=None, scaling_modifier=1.0,
-           use_override_color=False):
+           use_override_color=False, return_depth=False):
     """viewpoint_camera: dict(viewmatrix, projmatrix, campos: device tensors; tanfovx, tanfovy) — the fields of GaussianKeyframe the
-    reference reads (world_view_transform_, full_proj_transform_, camera_center_, FoVx_/FoVy_ as tangents). pc: trainer.GaussianModel."""
+    reference reads (world_view_transform_, full_proj_transform_, camera_center_, FoVx_/FoVy_ as tangents). pc: trainer.GaussianModel.
+    return_depth=True appends the rendered depth [H,W] (include/psb200.h: sum z alpha T, no background term) to the tuple, in every
+    branch; gradients flow through it like through the image."""
     pipe = pipe or GaussianPipelineParams()
     dev = pc.xyz_.device
     bg_color = bg_color if bg_color is not None else torch.zeros(3, device=dev)
@@ -84,6 +86,10 @@ def render(viewpoint_camera, image_height, image_width, pc, pipe=None, bg_color=
         colors_precomp = torch.clamp_min(sh_utils.eval_sh(pc.active_sh_degree_, shs_view, dir_pp) + 0.5, 0.0)
     else:
         shs = get_features(pc)
+    if return_depth:
+        rendered_image, radii, depth = rasterizer(means3D, means2D, opacity, shs=shs, colors_precomp=colors_precomp, scales=scales,
+                                                  rotations=rotations, cov3D_precomp=cov3D_precomp, return_depth=True)
+        return rendered_image, screenspace_points, radii > 0, radii, depth
     rendered_image, radii = rasterizer(means3D, means2D, opacity, shs=shs, colors_precomp=colors_precomp, scales=scales, rotations=rotations,
                                        cov3D_precomp=cov3D_precomp)
     return rendered_image, screenspace_points, radii > 0, radii

@@ -1,0 +1,108 @@
+"""Cost of rendered depth on the rasterizer operator path (psb_rasterize_forward_depth / psb_rasterize_backward_depth through the B1
+glue), on bench.py's scenes at configs B and D (1200x680).
+
+    python tools/operator_depth_bench.py [--configs B,D] [--calls K] [--warmup W] [--rounds R]
+
+Per config, a plain leg (RasterizeGaussiansCUDA -> RasterizeGaussiansBackwardCUDA) and a depth leg (RasterizeGaussiansDepthCUDA ->
+RasterizeGaussiansBackwardDepthCUDA, with a depth gradient) alternate R times in one process, the order of the two legs alternating
+from round to round. Each leg times K forward and K backward calls with CUDA events (every forward blocks the host once, like the
+reference's, to size the binning scratch). Prints one JSON line with the per-round times, the per-call cost of depth and the spread of
+each leg between rounds, the device name and its power limit; writes nothing."""
+import argparse
+import json
+import os
+import sys
+
+import numpy as np
+import torch
+import torch.nn.functional as F
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "oracle")]
+import bench  # noqa: E402  (its workload: make_inputs)
+
+
+def power_limit_w(index):
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        h = pynvml.nvmlDeviceGetHandleByIndex(index)
+        return pynvml.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
+    except Exception:  # noqa: BLE001
+        return None
+
+
+def run_config(config, a, dev):
+    from photo_slam_b200 import rasterizer as R
+    args = argparse.Namespace(config=config)
+    args.points, args.camera = {"B": (500_000, "replica"), "D": (3_000_000, "replica")}[config]
+    scene, cam, host, c, gt = bench.make_inputs(args, 0, dev)
+    T = lambda k: torch.from_numpy(scene[k]).to(dev)
+    means3D, opac = T("xyz"), torch.sigmoid(T("opacity"))
+    scales, rots = torch.exp(T("scaling")), F.normalize(T("rotation"))
+    shs = torch.cat((T("features_dc"), T("features_rest")), dim=1).contiguous()
+    bg, e = torch.zeros(3, device=dev), torch.empty(0, device=dev)
+    H, W = c["H"], c["W"]
+    fwd_args = (bg, means3D, e, opac, scales, rots, 1.0, e, c["viewmatrix"], c["projmatrix"], c["tanfovx"], c["tanfovy"], H, W, shs, 3, c["campos"],
+                False)
+    gen = torch.Generator(device=dev).manual_seed(1)
+    dpix = torch.randn((3, H, W), device=dev, generator=gen) / (3 * H * W)
+    ddep = torch.randn((H, W), device=dev, generator=gen) / (H * W)
+
+    def leg(depth):
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+        fwd = R.RasterizeGaussiansDepthCUDA if depth else R.RasterizeGaussiansCUDA
+        ev[0].record()
+        for _ in range(a.calls):
+            out = fwd(*fwd_args)
+        ev[1].record()
+        nr, radii, bufs = out[0], out[-4], out[-3:]
+        bwd_args = (bg, means3D, radii, e, scales, rots, 1.0, e, c["viewmatrix"], c["projmatrix"], c["tanfovx"], c["tanfovy"], dpix)
+        tail = (shs, 3, c["campos"], bufs[0], nr, bufs[1], bufs[2])
+        ev[2].record()
+        for _ in range(a.calls):
+            if depth:
+                R.RasterizeGaussiansBackwardDepthCUDA(*bwd_args, ddep, *tail)
+            else:
+                R.RasterizeGaussiansBackwardCUDA(*bwd_args, *tail)
+        ev[3].record()
+        torch.cuda.synchronize()
+        return ev[0].elapsed_time(ev[1]) / a.calls, ev[2].elapsed_time(ev[3]) / a.calls, nr
+
+    for _ in range(a.warmup):
+        leg(False)
+        leg(True)
+    res = {k: dict(forward_ms=[], backward_ms=[]) for k in ("plain", "depth")}
+    for rnd in range(a.rounds):
+        for name in (("plain", "depth") if rnd % 2 == 0 else ("depth", "plain")):
+            f, b, nr = leg(name == "depth")
+            res[name]["forward_ms"].append(f)
+            res[name]["backward_ms"].append(b)
+    out = {"gaussians": args.points, "width": W, "height": H, "num_rendered": int(nr)}
+    for name, r in res.items():
+        out[name] = {k: v for k, v in r.items()}
+        for k in ("forward_ms", "backward_ms"):
+            out[name][k + "_mean"] = float(np.mean(r[k]))
+            out[name][k + "_spread"] = float(np.max(r[k]) - np.min(r[k]))
+    out["depth_cost_ms"] = {k: out["depth"][k + "_mean"] - out["plain"][k + "_mean"] for k in ("forward_ms", "backward_ms")}
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--configs", default="B,D")
+    ap.add_argument("--calls", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--rounds", type=int, default=4)
+    a = ap.parse_args()
+    dev = torch.device("cuda", 0)
+    out = {"device": torch.cuda.get_device_name(dev), "power_limit_w": power_limit_w(0), "calls": a.calls, "rounds": a.rounds,
+           "unit": "ms per call (CUDA events)"}
+    for config in a.configs.split(","):
+        out[config] = run_config(config, a, dev)
+        torch.cuda.empty_cache()
+    print(json.dumps(out), flush=True)
+
+
+if __name__ == "__main__":
+    main()
