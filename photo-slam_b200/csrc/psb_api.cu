@@ -18,19 +18,6 @@ void set_error(const char* what, cudaError_t e, const char* file, int line)
 }
 void set_error_msg(const char* what) { g_last_error = what; }
 
-static Camera make_camera(int width, int height, const float* view, const float* proj, const float* campos, float tan_fovx, float tan_fovy)
-{
-	Camera cam;
-	cam.view = view; cam.proj = proj; cam.campos = campos;
-	cam.tan_fovx = tan_fovx; cam.tan_fovy = tan_fovy;
-	cam.focal_y = height / (2.0f * tan_fovy);
-	cam.focal_x = width / (2.0f * tan_fovx);
-	cam.W = width; cam.H = height;
-	cam.grid_x = (width + PSB_TILE_X - 1) / PSB_TILE_X;
-	cam.grid_y = (height + PSB_TILE_Y - 1) / PSB_TILE_Y;
-	return cam;
-}
-
 static GaussIn make_input(int P, int D, int M, const float* means3D, const float* shs, const float* colors_precomp, const float* opacities,
                           const float* scales, float scale_modifier, const float* rotations, const float* cov3D_precomp)
 {
@@ -123,8 +110,7 @@ static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void*
 	BinState bin = BinState::from_chunk(bin_chunk, (size_t)num_rendered);
 	if ((rc = launch_binning(P, cam, geom, bin, img, (size_t)num_rendered, stream))) return rc;
 
-	const int res = make_sort_plan(tile_id_bits(cam.grid_x * cam.grid_y)).npass & 1;
-	if ((rc = launch_render_forward(cam, img.ranges, bin.inst[res], geom.rec, background, out_color, img.final_T, img.n_contrib, stream, out_depth)))
+	if ((rc = launch_render_forward(cam, img.ranges, bin.inst[sorted_slot(width, height)], geom.rec, background, out_color, img.final_T, img.n_contrib, stream, out_depth)))
 		return rc;
 	return (int)num_rendered;
 }
@@ -146,7 +132,6 @@ static int rasterize_backward(const char* fn, int P, int D, int M, int R, const 
 	GeomState geom = GeomState::from_chunk(geom_buffer, (size_t)P);
 	BinState bin = BinState::from_chunk(binning_buffer, (size_t)R);
 	ImgState img = ImgState::from_chunk(image_buffer, (size_t)width * height);
-	const int res = make_sort_plan(tile_id_bits(cam.grid_x * cam.grid_y)).npass & 1;
 
 	GradSink sink;
 	sink.mean2D = dL_dmean2D; sink.mean2D_stride = 3;
@@ -157,7 +142,7 @@ static int rasterize_backward(const char* fn, int P, int D, int M, int R, const 
 	if (dL_ddepth) { sink.z = dL_dz; sink.z_stride = 1; }
 	int rc;
 	if (R > 0)
-		if ((rc = launch_render_backward(cam, img.ranges, bin.inst[res], geom.rec, background, img.final_T, img.n_contrib, dL_dpix, sink, stream, dL_ddepth)))
+		if ((rc = launch_render_backward(cam, img.ranges, bin.inst[sorted_slot(width, height)], geom.rec, background, img.final_T, img.n_contrib, dL_dpix, sink, stream, dL_ddepth)))
 			return rc;
 
 	const GaussIn in = make_input(P, D, M, means3D, shs, colors_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp);
@@ -248,16 +233,16 @@ int psb_debug_export(int P, int R, int width, int height, char* geom_buffer, cha
 	GeomState geom = GeomState::from_chunk(geom_buffer, (size_t)P);
 	export_geom_kernel<<<cdiv(P, 256), 256, 0, stream>>>(P, geom, depths, means2D, conic_opacity, rgb, clamped, tiles_touched);
 	PSB_LAUNCH_OK();
-	const int gx = (width + PSB_TILE_X - 1) / PSB_TILE_X, gy = (height + PSB_TILE_Y - 1) / PSB_TILE_Y;
 	if (binning_buffer && R > 0 && (keys_sorted || values_sorted)) {
 		BinState bin = BinState::from_chunk(binning_buffer, (size_t)R);
-		const int res = make_sort_plan(tile_id_bits(gx * gy)).npass & 1;
+		const int res = sorted_slot(width, height);
 		export_keys_kernel<<<cdiv(R, 256), 256, 0, stream>>>(R, bin.tile_key[res], bin.inst[res], geom.rec, keys_sorted, values_sorted);
 		PSB_LAUNCH_OK();
 	}
 	if (image_buffer) {
 		ImgState img = ImgState::from_chunk(image_buffer, (size_t)width * height);
-		if (ranges) PSB_CUDA_OK(cudaMemcpyAsync(ranges, img.ranges, (size_t)gx * gy * sizeof(uint2), cudaMemcpyDeviceToDevice, stream));
+		const int2 grid = tile_grid(width, height);
+		if (ranges) PSB_CUDA_OK(cudaMemcpyAsync(ranges, img.ranges, (size_t)grid.x * grid.y * sizeof(uint2), cudaMemcpyDeviceToDevice, stream));
 		if (n_contrib) PSB_CUDA_OK(cudaMemcpyAsync(n_contrib, img.n_contrib, (size_t)width * height * sizeof(uint32_t), cudaMemcpyDeviceToDevice, stream));
 		if (final_T) PSB_CUDA_OK(cudaMemcpyAsync(final_T, img.final_T, (size_t)width * height * sizeof(float), cudaMemcpyDeviceToDevice, stream));
 	}
@@ -278,7 +263,7 @@ int psb_debug_sort_pairs(uint32_t* keys, uint32_t* vals, size_t n, int nbits, vo
 	uint32_t* kk[2] = {keys, k1};
 	uint32_t* vv[2] = {vals, v1};
 	int rc = radix_sort_pairs(kk, vv, false, nullptr, n, plan, scratch, sb, stream);
-	if (rc == 0 && (plan.npass & 1)) {
+	if (rc == 0 && plan.result() == 1) {
 		cudaMemcpyAsync(keys, k1, n * 4, cudaMemcpyDeviceToDevice, stream);
 		cudaMemcpyAsync(vals, v1, n * 4, cudaMemcpyDeviceToDevice, stream);
 	}

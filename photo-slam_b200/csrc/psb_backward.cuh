@@ -20,6 +20,27 @@ __device__ __forceinline__ float3 dnormvdv(float3 v, float3 dv)
 	return o;
 }
 
+// Unit view direction of dir = pos - campos: the direction the SH colour of a Gaussian at pos is evaluated at.
+__device__ __forceinline__ float3 sh_dir(const float3 dir)
+{
+	const float len = sqrtf(dir.x * dir.x + dir.y * dir.y + dir.z * dir.z);
+	return make_float3(dir.x / len, dir.y / len, dir.z / len);
+}
+
+// SH basis weights w_k = dRGB/dsh_k of the unit direction d, k < 16. The NVLink owner rank re-evaluates them from its copy of xyz
+// and the sender's camera centre: both sides go through sh_dir and this function, so the weights agree bit for bit.
+__device__ __forceinline__ void sh_basis(const float3 d, float* w /*[16]*/)
+{
+	const float x = d.x, y = d.y, z = d.z;
+	const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
+	w[0] = kSH_C0;
+	w[1] = -kSH_C1 * y; w[2] = kSH_C1 * z; w[3] = -kSH_C1 * x;
+	w[4] = kSH_C2_0 * xy; w[5] = kSH_C2_1 * yz; w[6] = kSH_C2_2 * (2.f * zz - xx - yy); w[7] = kSH_C2_3 * xz; w[8] = kSH_C2_4 * (xx - yy);
+	w[9] = kSH_C3_0 * y * (3.f * xx - yy); w[10] = kSH_C3_1 * xy * z; w[11] = kSH_C3_2 * y * (4.f * zz - xx - yy);
+	w[12] = kSH_C3_3 * z * (2.f * zz - 3.f * xx - 3.f * yy); w[13] = kSH_C3_4 * x * (4.f * zz - xx - yy); w[14] = kSH_C3_5 * z * (xx - yy);
+	w[15] = kSH_C3_6 * x * (xx - 3.f * yy);
+}
+
 // SH backward for one Gaussian. `get(k, ch)` returns SH coefficient k of channel ch, `put(k, ch, g)` receives
 // dL/dsh[k][ch] (called for the coefficients of the active degree only). All reads happen before the
 // first put, so `put` may update the coefficient in place. Returns the view-direction contribution to dL/dmean.
@@ -28,8 +49,8 @@ __device__ __forceinline__ float3 sh_backward_t(int deg, const float3 pos, const
                                                 const float3 dL_dcolor, Get get, Put put, float* w_out = nullptr)
 {
 	const float3 dir_orig = make_float3(pos.x - campos.x, pos.y - campos.y, pos.z - campos.z);
-	const float len = sqrtf(dir_orig.x * dir_orig.x + dir_orig.y * dir_orig.y + dir_orig.z * dir_orig.z);
-	const float x = dir_orig.x / len, y = dir_orig.y / len, z = dir_orig.z / len;
+	const float3 d = sh_dir(dir_orig);
+	const float x = d.x, y = d.y, z = d.z;
 	float g[3] = {dL_dcolor.x, dL_dcolor.y, dL_dcolor.z};
 #pragma unroll
 	for (int ch = 0; ch < 3; ch++) g[ch] *= ((clamp_bits >> ch) & 1u) ? 0 : 1;
@@ -59,14 +80,8 @@ __device__ __forceinline__ float3 sh_backward_t(int deg, const float3 pos, const
 		}
 	}
 #undef SHC
-	// basis weights dRGB/dsh_k
 	float w[16];
-	w[0] = kSH_C0;
-	w[1] = -kSH_C1 * y; w[2] = kSH_C1 * z; w[3] = -kSH_C1 * x;
-	w[4] = kSH_C2_0 * xy; w[5] = kSH_C2_1 * yz; w[6] = kSH_C2_2 * (2.f * zz - xx - yy); w[7] = kSH_C2_3 * xz; w[8] = kSH_C2_4 * (xx - yy);
-	w[9] = kSH_C3_0 * y * (3.f * xx - yy); w[10] = kSH_C3_1 * xy * z; w[11] = kSH_C3_2 * y * (4.f * zz - xx - yy);
-	w[12] = kSH_C3_3 * z * (2.f * zz - 3.f * xx - 3.f * yy); w[13] = kSH_C3_4 * x * (4.f * zz - xx - yy); w[14] = kSH_C3_5 * z * (xx - yy);
-	w[15] = kSH_C3_6 * x * (xx - 3.f * yy);
+	sh_basis(d, w);
 	if (w_out) {
 #pragma unroll
 		for (int k = 0; k < 16; k++) w_out[k] = w[k];

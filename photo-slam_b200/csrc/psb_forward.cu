@@ -512,8 +512,7 @@ int launch_binning(int P, const Camera& cam, const GeomState& geom, BinState& bi
 	const SortPlan plan = make_sort_plan(tile_id_bits(num_tiles));
 	int rc = radix_sort_pairs(bin.tile_key, bin.inst, false, nullptr, n_host, plan, bin.sort_scratch, bin.sort_scratch_bytes, stream);
 	if (rc) return rc;
-	const int res = plan.npass & 1;
-	tile_ranges_kernel<<<ranges_grid(n_host), 256, 0, stream>>>(nullptr, (uint32_t)n_host, bin.tile_key[res], img.ranges, nullptr, 0u);
+	tile_ranges_kernel<<<ranges_grid(n_host), 256, 0, stream>>>(nullptr, (uint32_t)n_host, bin.tile_key[plan.result()], img.ranges, nullptr, 0u);
 	PSB_LAUNCH_OK();
 	return 0;
 }
@@ -536,8 +535,7 @@ int launch_scan_binning(int P, const Camera& cam, const GeomState& geom, BinStat
 	PSB_LAUNCH_OK();
 	int rc = radix_sort_pairs(bin.tile_key, bin.inst, false, geom.counters, capacity, plan, bin.sort_scratch, bin.sort_scratch_bytes, stream);
 	if (rc) return rc;
-	const int res = plan.npass & 1;
-	tile_ranges_kernel<<<ranges_grid(capacity), 256, 0, stream>>>(geom.counters, (uint32_t)capacity, bin.tile_key[res], img.ranges, ovf, seq);
+	tile_ranges_kernel<<<ranges_grid(capacity), 256, 0, stream>>>(geom.counters, (uint32_t)capacity, bin.tile_key[plan.result()], img.ranges, ovf, seq);
 	PSB_LAUNCH_OK();
 	return 0;
 }

@@ -42,6 +42,30 @@ struct GaussGradOut {
 	float* dL_drots;     // [P,4]
 };
 
+// tiles of an image of width x height pixels in x and y
+inline int2 tile_grid(int width, int height) { return make_int2(cdiv(width, PSB_TILE_X), cdiv(height, PSB_TILE_Y)); }
+
+inline Camera make_camera(int width, int height, const float* view, const float* proj, const float* campos, float tan_fovx, float tan_fovy)
+{
+	Camera cam;
+	cam.view = view; cam.proj = proj; cam.campos = campos;
+	cam.tan_fovx = tan_fovx; cam.tan_fovy = tan_fovy;
+	cam.focal_y = height / (2.0f * tan_fovy);
+	cam.focal_x = width / (2.0f * tan_fovx);
+	cam.W = width; cam.H = height;
+	const int2 grid = tile_grid(width, height);
+	cam.grid_x = grid.x; cam.grid_y = grid.y;
+	return cam;
+}
+
+// The half of a BinState's ping-pong buffers (tile_key / inst) that holds the instance list sorted by tile, for an image of
+// width x height pixels (the plan launch_binning / launch_scan_binning sort with).
+inline int sorted_slot(int width, int height)
+{
+	const int2 grid = tile_grid(width, height);
+	return make_sort_plan(tile_id_bits(grid.x * grid.y)).result();
+}
+
 // tight: instance lists hold only the tiles a splat can reach (trainer path; see preprocess_fwd_kernel) — pass the same flag to launch_scan_binning
 int launch_preprocess(const GaussIn& in, const Camera& cam, int* radii_out, const GeomState& geom, bool raw, bool tight, cudaStream_t stream);
 int launch_mark_visible(int P, const float* means3D, const float* view, uint8_t* present, cudaStream_t stream);

@@ -334,7 +334,7 @@ int psb_dist_cuda2(int P, const float* points, float* mean_dists, void* stream_)
 	PSB_LAUNCH_OK();
 	int rc = radix_sort_pairs(keys, vals, /*iota_vals=*/true, nullptr, (size_t)P, plan, scratch, sb, stream);
 	if (rc == 0) {
-		const uint32_t* order = vals[plan.npass & 1];
+		const uint32_t* order = vals[plan.result()];
 		knn_gather_kernel<<<cdiv(P, 256), 256, 0, stream>>>(P, points, order, sorted);
 		knn_tile_box_kernel<<<nbox, KNN_TILE, 0, stream>>>(P, sorted, boxes);
 		knn_search_kernel<<<nbox, KNN_TILE, 0, stream>>>(P, nbox, sorted, boxes, mean_dists);

@@ -17,6 +17,8 @@ struct SortPlan {
 	int npass;
 	int shift[RS_MAX_PASS];
 	int bits[RS_MAX_PASS];
+	// the ping-pong buffer radix_sort_pairs leaves the sorted keys and values in
+	int result() const { return npass & 1; }
 };
 
 // Digit plan covering key bits [0, nbits): ceil(nbits/8) passes of equal width.
@@ -27,7 +29,7 @@ size_t sort_scratch_bytes(size_t max_n, int npass);
 
 // Sorts (keys, vals) of length n (n = *n_dev if n_dev != nullptr, else n_host; n_host must be an upper
 // bound used to size grids). Buffers ping-pong: pass p reads buffer (p & 1) and writes buffer ((p+1) & 1);
-// the result is in buffer (plan.npass & 1). If vals[0] == nullptr is passed with iota_vals = true the
+// the result is in buffer plan.result(). If vals[0] == nullptr is passed with iota_vals = true the
 // first pass uses the element index as payload.
 int radix_sort_pairs(uint32_t* keys[2], uint32_t* vals[2], bool iota_vals, const uint32_t* n_dev, size_t n_host,
                      const SortPlan& plan, void* scratch, size_t scratch_bytes, cudaStream_t stream);

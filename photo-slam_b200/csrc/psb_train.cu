@@ -30,7 +30,11 @@ constexpr int A_MINBLOCKS = 5; // __launch_bounds__ minimum blocks per SM of gau
 constexpr int REST = 45;       // floats per f_rest row (15 coefficients x 3 channels)
 constexpr int SEED = 20;       // floats per seed row: w_1..w_15 at [0..14], masked dL/dRGB at [16..18]
 
-struct AdamCoef { float beta1, beta2, eps, inv_bc1, inv_bc2_sqrt; };
+struct AdamCoef {
+	float beta1, beta2, eps, inv_bc1, inv_bc2_sqrt;
+	__host__ __device__ explicit AdamCoef(const StepHyper& h)
+		: beta1(h.beta1), beta2(h.beta2), eps(h.eps), inv_bc1(h.inv_bc1), inv_bc2_sqrt(1.0f / h.bc2_sqrt) {}
+};
 
 // gaussian_backward_kernel modes
 constexpr int MODE_GRADS = 0;  // dense gradients of the raw parameters -> `grads` (NCCL data-parallel path / tests)
@@ -52,6 +56,90 @@ __device__ __forceinline__ void adam1(float& p, float& m, float& v, float g, flo
 	const float sq = v > 0.f ? v * rsqrtf(v) : 0.f;
 	const float denom = sq * c.inv_bc2_sqrt + c.eps;
 	p = p - lr_eff * __fdividef(m, denom);
+}
+
+__device__ __forceinline__ void adam4(float4& p, float4& m, float4& v, const float4 g, float lr_eff, const AdamCoef& c)
+{
+	adam1(p.x, m.x, v.x, g.x, lr_eff, c);
+	adam1(p.y, m.y, v.y, g.y, lr_eff, c);
+	adam1(p.z, m.z, v.z, g.z, lr_eff, c);
+	adam1(p.w, m.w, v.w, g.w, lr_eff, c);
+}
+
+// Adam over the 4 elements at p, m, v (16-byte aligned) with gradient g. A zero gradient on zero moments is an exact no-op of Adam
+// (m' = v' = 0, p' = p - lr * 0 / (0 + eps) = p): such elements (Gaussians no view has reached since their moments were created) are
+// neither read beyond their moments nor rewritten, and false is returned. Otherwise the moments are stored back and the new
+// parameters are returned in `pp` for the caller to store.
+__device__ __forceinline__ bool adam4_unless_noop(const float* p, float* m, float* v, const float4 g, float lr_eff, const AdamCoef& c, float4& pp)
+{
+	float4 mm = __ldcs(reinterpret_cast<const float4*>(m)), vv = __ldcs(reinterpret_cast<const float4*>(v));
+	if (g.x == 0.f && g.y == 0.f && g.z == 0.f && g.w == 0.f && mm.x == 0.f && mm.y == 0.f && mm.z == 0.f && mm.w == 0.f &&
+	    vv.x == 0.f && vv.y == 0.f && vv.z == 0.f && vv.w == 0.f) return false;
+	pp = __ldcs(reinterpret_cast<const float4*>(p));
+	adam4(pp, mm, vv, g, lr_eff, c);
+	__stcs(reinterpret_cast<float4*>(m), mm); __stcs(reinterpret_cast<float4*>(v), vv);
+	return true;
+}
+
+// The 14 small parameters of one Gaussian (or their moments, or their gradients), by tensor: xyz 3 (tensor 0) | f_dc 3 (1) |
+// scaling 3 (4) | opacity 1 (3) | rotation 4 (5).
+struct SmallRow {
+	float xyz[3], dc[3], sc[3], op;
+	float4 rot;
+};
+
+__device__ __forceinline__ void load_small(SmallRow& r, float* const* ts, int idx)
+{
+#pragma unroll
+	for (int c = 0; c < 3; c++) { r.xyz[c] = ts[0][3 * idx + c]; r.dc[c] = ts[1][3 * idx + c]; r.sc[c] = ts[4][3 * idx + c]; }
+	r.op = ts[3][idx];
+	r.rot = reinterpret_cast<const float4*>(ts[5])[idx];
+}
+
+__device__ __forceinline__ void store_small(float* const* ts, int idx, const SmallRow& r)
+{
+#pragma unroll
+	for (int c = 0; c < 3; c++) { ts[0][3 * idx + c] = r.xyz[c]; ts[1][3 * idx + c] = r.dc[c]; ts[4][3 * idx + c] = r.sc[c]; }
+	ts[3][idx] = r.op;
+	reinterpret_cast<float4*>(ts[5])[idx] = r.rot;
+}
+
+// any of the 14 values is non-zero
+__device__ __forceinline__ bool any_nonzero(const SmallRow& r)
+{
+	bool nz = false;
+#pragma unroll
+	for (int c = 0; c < 3; c++) nz = nz || r.xyz[c] != 0.f || r.dc[c] != 0.f || r.sc[c] != 0.f;
+	return nz || r.op != 0.f || r.rot.x != 0.f || r.rot.y != 0.f || r.rot.z != 0.f || r.rot.w != 0.f;
+}
+
+// any of the 28 moments is non-zero. (The order of the tests is the one that keeps the spill reloads of the fused Adam modes of
+// gaussian_backward_kernel, which hold the moments across the backward, lowest.)
+__device__ __forceinline__ bool any_nonzero(const SmallRow& m, const SmallRow& v)
+{
+	bool nz = m.op != 0.f || v.op != 0.f || m.rot.x != 0.f || m.rot.y != 0.f || m.rot.z != 0.f || m.rot.w != 0.f || v.rot.x != 0.f || v.rot.y != 0.f ||
+	          v.rot.z != 0.f || v.rot.w != 0.f;
+	const float* m3[3] = {m.xyz, m.dc, m.sc};
+	const float* v3[3] = {v.xyz, v.dc, v.sc};
+#pragma unroll
+	for (int a = 0; a < 3; a++)
+#pragma unroll
+		for (int c = 0; c < 3; c++) nz = nz || m3[a][c] != 0.f || v3[a][c] != 0.f;
+	return nz;
+}
+
+// Adam over the 14 small parameters with the gradient g * gs, each tensor at its own learning rate h.lr[i] / (1 - beta1^t)
+__device__ __forceinline__ void adam_small(SmallRow& p, SmallRow& m, SmallRow& v, const SmallRow& g, float gs, const StepHyper& h, const AdamCoef& ac)
+{
+#pragma unroll
+	for (int c = 0; c < 3; c++) {
+		adam1(p.xyz[c], m.xyz[c], v.xyz[c], g.xyz[c] * gs, h.lr[0] * ac.inv_bc1, ac);
+		adam1(p.dc[c], m.dc[c], v.dc[c], g.dc[c] * gs, h.lr[1] * ac.inv_bc1, ac);
+		adam1(p.sc[c], m.sc[c], v.sc[c], g.sc[c] * gs, h.lr[4] * ac.inv_bc1, ac);
+	}
+	adam1(p.op, m.op, v.op, g.op * gs, h.lr[3] * ac.inv_bc1, ac);
+	const float4 gr = make_float4(g.rot.x * gs, g.rot.y * gs, g.rot.z * gs, g.rot.w * gs);
+	adam4(p.rot, m.rot, v.rot, gr, h.lr[5] * ac.inv_bc1, ac);
 }
 
 // ADAM = true : fused update (parameters and moments of the 14 small parameters updated in place).
@@ -115,8 +203,7 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 
 	const int idx = base + tid;
 	const bool valid = idx < P;
-	AdamCoef ac;
-	ac.beta1 = h.beta1; ac.beta2 = h.beta2; ac.eps = h.eps; ac.inv_bc1 = h.inv_bc1; ac.inv_bc2_sqrt = 1.0f / h.bc2_sqrt;
+	const AdamCoef ac(h);
 
 	// ---- phase 1a: everything that does not need the staged rows
 	bool visible = false;
@@ -128,50 +215,35 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 	uint32_t clamp_bits = 0;
 	// the 14 small parameters (every Gaussian needs them for its Adam update): issued up front, with the
 	// screen-space sums, as one batch of independent loads — a single memory round trip instead of a chain
-	float sp_xyz[3] = {0, 0, 1}, sp_dc[3] = {0, 0, 0}, sp_sc[3] = {0, 0, 0}, sp_op = 0.f;
-	float4 sp_rot = make_float4(1, 0, 0, 0);
+	SmallRow p = {{0, 0, 1}, {0, 0, 0}, {0, 0, 0}, 0.f, make_float4(1, 0, 0, 0)};
 	// ... and their moments (consumed last): loaded here as well so their latency hides behind the whole backward
-	float m3[3][3], v3[3][3], mo = 0.f, vo = 0.f;
-	float4 mr = make_float4(0, 0, 0, 0), vr = mr;
+	SmallRow m, v;
+	if (LIVE) m = v = SmallRow{};  // (a row reached for the first time starts from zero moments)
 	float st_rad = 0.f, st_acc = 0.f, st_den = 0.f;
-	bool was_live = false, staged = false;  // LIVE: live byte before this step | f_rest row staged (non-zero sums)
-	bool reached = false;                   // LIVE: staged, or (DEPTH) a non-zero dL/dz
-	int rest_slot = tid;                    // this row's f_rest row in s_p
+	bool was_live = false;  // LIVE: live byte before this step
+	bool staged = false;    // non-zero screen-space sums (LIVE: the f_rest row is staged)
+	bool reached = false;   // staged, or (DEPTH) a non-zero dL/dz: the sink row was added to and has a gradient
+	int rest_slot = tid;    // this row's f_rest row in s_p
 	float4 s0 = make_float4(0, 0, 0, 0), s1 = s0, s2 = s0;
 	uint32_t meta = 0;
-	auto load_moments = [&]() {
-		const int tsel[3] = {0, 1, 4};
-#pragma unroll
-		for (int a = 0; a < 3; a++)
-#pragma unroll
-			for (int c = 0; c < 3; c++) { m3[a][c] = t.m[tsel[a]][3 * idx + c]; v3[a][c] = t.v[tsel[a]][3 * idx + c]; }
-		mo = t.m[3][idx]; vo = t.v[3][idx];
-		mr = reinterpret_cast<const float4*>(t.m[5])[idx]; vr = reinterpret_cast<const float4*>(t.v[5])[idx];
-	};
-	auto load_params = [&]() {
-#pragma unroll
-		for (int c = 0; c < 3; c++) { sp_xyz[c] = t.p[0][3 * idx + c]; sp_dc[c] = t.p[1][3 * idx + c]; sp_sc[c] = t.p[4][3 * idx + c]; }
-		sp_op = t.p[3][idx];
-		sp_rot = reinterpret_cast<const float4*>(t.p[5])[idx];
+	auto load_moments = [&]() { load_small(m, t.m, idx); load_small(v, t.v, idx); };
+	// rows nothing was added to (culled or hidden Gaussians) are zero since the last step: only the others are re-zeroed for the next one
+	auto take_sink = [&]() {
+		staged = s0.x != 0.f || s0.y != 0.f || s0.w != 0.f || s1.x != 0.f || s1.z != 0.f || s1.w != 0.f || s2.x != 0.f || s2.y != 0.f || s2.z != 0.f;
+		reached = staged || (DEPTH && s2.w != 0.f);
+		if (reached) { const float4 z = make_float4(0, 0, 0, 0); sink[3 * idx] = z; sink[3 * idx + 1] = z; sink[3 * idx + 2] = z; }
 	};
 	if (LIVE) {
-#pragma unroll
-		for (int a = 0; a < 3; a++)
-#pragma unroll
-			for (int c = 0; c < 3; c++) { m3[a][c] = 0.f; v3[a][c] = 0.f; }
 		if (valid) {
 			was_live = adam_live[idx] != 0;
 			visible = geom.tile_info[idx].z != 0;  // (an overflowing step has returned above)
-			if (was_live) load_params();  // (the moments are loaded after the backward: fewer registers held across it)
+			if (was_live) load_small(p, t.p, idx);  // (the moments are loaded after the backward: fewer registers held across it)
 			if (visible) {
 				if (st.enabled) { st_rad = st.max_radii2D[idx]; st_acc = st.xyz_gradient_accum[idx]; st_den = st.denom[idx]; }
 				s0 = sink[3 * idx]; s1 = sink[3 * idx + 1]; s2 = sink[3 * idx + 2];
 				meta = __float_as_uint(geom.rec[idx].q2.w);
-				// only visible rows were added to; the others are zero since the last step
-				staged = s0.x != 0.f || s0.y != 0.f || s0.w != 0.f || s1.x != 0.f || s1.z != 0.f || s1.w != 0.f || s2.x != 0.f || s2.y != 0.f || s2.z != 0.f;
-				reached = staged || (DEPTH && s2.w != 0.f);
-				if (reached) { const float4 z = make_float4(0, 0, 0, 0); sink[3 * idx] = z; sink[3 * idx + 1] = z; sink[3 * idx + 2] = z; }
-				if (reached && !was_live) load_params();  // first gradient of this row: its moments are zero by contract, not read
+				take_sink();  // (only visible rows were added to)
+				if (reached && !was_live) load_small(p, t.p, idx);  // first gradient of this row: its moments are zero by contract, not read
 				if (st.enabled) {  // (here: fewer registers held across the backward)
 					st.max_radii2D[idx] = fmaxf(st_rad, (float)rec_radius(meta));
 					st.xyz_gradient_accum[idx] = st_acc + sqrtf(s0.x * s0.x + s0.y * s0.y);
@@ -200,12 +272,9 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 			tt = geom.tile_info[idx].z;
 			s0 = sink[3 * idx]; s1 = sink[3 * idx + 1]; s2 = sink[3 * idx + 2];
 			meta = __float_as_uint(geom.rec[idx].q2.w);
-			load_params();
+			load_small(p, t.p, idx);
 			visible = tt != 0 && !overflow;
-			// ready for the next iteration (rows nothing was added to — culled or hidden Gaussians — are zero already: not rewritten)
-			const bool sink_dirty = s0.x != 0.f || s0.y != 0.f || s0.w != 0.f || s1.x != 0.f || s1.z != 0.f || s1.w != 0.f || s2.x != 0.f || s2.y != 0.f || s2.z != 0.f ||
-			                        (DEPTH && s2.w != 0.f);
-			if (sink_dirty) { const float4 z = make_float4(0, 0, 0, 0); sink[3 * idx] = z; sink[3 * idx + 1] = z; sink[3 * idx + 2] = z; }
+			take_sink();
 		}
 		// LIVE: a visible row with zero sums has zero gradients (and may not have its parameters loaded): statistics only
 		if (visible && (!LIVE || reached)) {
@@ -214,11 +283,11 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 			const float3 dL_dconic = make_float3(s0.w, s1.x, s1.z);
 			const float dL_dopacity = s1.w;
 			dL_dcolor = make_float3(s2.x, s2.y, s2.z);
-			mean = make_float3(sp_xyz[0], sp_xyz[1], sp_xyz[2]);
-			dc = make_float3(sp_dc[0], sp_dc[1], sp_dc[2]);
-			const float3 sraw = make_float3(sp_sc[0], sp_sc[1], sp_sc[2]);
-			const float4 qraw = sp_rot;
-			const float oraw = sp_op;
+			mean = make_float3(p.xyz[0], p.xyz[1], p.xyz[2]);
+			dc = make_float3(p.dc[0], p.dc[1], p.dc[2]);
+			const float3 sraw = make_float3(p.sc[0], p.sc[1], p.sc[2]);
+			const float4 qraw = p.rot;
+			const float oraw = p.op;
 			clamp_bits = rec_clamp_bits(meta);
 			// activations exactly as in the forward (preprocess_fwd_kernel<RAW>)
 			const float3 s = make_float3(expf(sraw.x), expf(sraw.y), expf(sraw.z));
@@ -259,12 +328,12 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 
 	// ---- phase 1b: SH backward seeds; the view-direction term completes dL/dxyz
 	float3 g_dc = make_float3(0, 0, 0);
+	float gm[3] = {0.f, 0.f, 0.f};  // clamp-masked dL/dRGB: the f_rest gradient is w_k * gm
 	{
 		const float* rp = s_p + rest_slot * REST;
 		float w[16];
 #pragma unroll
 		for (int k = 0; k < 16; k++) w[k] = 0.f;
-		float gm[3] = {0.f, 0.f, 0.f};
 		if (LIVE ? staged : visible) {
 			const float3 campos = make_float3(cam.campos[0], cam.campos[1], cam.campos[2]);
 			const float3 sh_dmean = sh_backward_t(
@@ -282,74 +351,42 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 #pragma unroll
 			for (int k = 1; k < 16; k++) s_w[tid][k - 1] = (k < ncoef) ? w[k] : 0.f;
 			s_w[tid][15] = 0.f; s_w[tid][16] = gm[0]; s_w[tid][17] = gm[1]; s_w[tid][18] = gm[2]; s_w[tid][19] = 0.f;
-		} else {
-			// gradient record of this Gaussian for its owner rank (see DpPush): the SH weights are NOT sent, the owner
-			// re-evaluates w_k(dir) from its bit-identical copy of xyz and this rank's camera centre
-			s_w[tid][0] = g_xyz.x; s_w[tid][1] = g_xyz.y; s_w[tid][2] = g_xyz.z;
-			s_w[tid][3] = g_dc.x; s_w[tid][4] = g_dc.y; s_w[tid][5] = g_dc.z;
-			s_w[tid][6] = g_opac;
-			s_w[tid][7] = g_scale.x; s_w[tid][8] = g_scale.y; s_w[tid][9] = g_scale.z;
-			s_w[tid][10] = g_rot.x; s_w[tid][11] = g_rot.y; s_w[tid][12] = g_rot.z; s_w[tid][13] = g_rot.w;
-			s_w[tid][14] = gm[0]; s_w[tid][15] = gm[1]; s_w[tid][16] = gm[2];
-			s_w[tid][17] = 0.f; s_w[tid][18] = 0.f;
-			// a visible Gaussian hidden behind nearer splats receives no gradient: like an invisible one it sends nothing
-			const bool sends = visible && (g_xyz.x != 0.f || g_xyz.y != 0.f || g_xyz.z != 0.f || g_opac != 0.f || gm[0] != 0.f || gm[1] != 0.f || gm[2] != 0.f ||
-			                               g_scale.x != 0.f || g_scale.y != 0.f || g_scale.z != 0.f || g_rot.x != 0.f || g_rot.y != 0.f || g_rot.z != 0.f || g_rot.w != 0.f);
-			s_w[tid][19] = __uint_as_float(sends ? dp.epoch : 0u);
 		}
+	}
+	const SmallRow g = {{g_xyz.x, g_xyz.y, g_xyz.z}, {g_dc.x, g_dc.y, g_dc.z}, {g_scale.x, g_scale.y, g_scale.z}, g_opac, g_rot};
+	// the row has a gradient: one of its 14 small-parameter gradients, or one of gm (its f_rest gradient), is non-zero
+	const bool gnz = any_nonzero(g) || gm[0] != 0.f || gm[1] != 0.f || gm[2] != 0.f;
+	if (BASE == MODE_PUSH) {
+		// gradient record of this Gaussian for its owner rank (see DpPush): the SH weights are NOT sent, the owner
+		// re-evaluates w_k(dir) from its bit-identical copy of xyz and this rank's camera centre
+		s_w[tid][0] = g_xyz.x; s_w[tid][1] = g_xyz.y; s_w[tid][2] = g_xyz.z;
+		s_w[tid][3] = g_dc.x; s_w[tid][4] = g_dc.y; s_w[tid][5] = g_dc.z;
+		s_w[tid][6] = g_opac;
+		s_w[tid][7] = g_scale.x; s_w[tid][8] = g_scale.y; s_w[tid][9] = g_scale.z;
+		s_w[tid][10] = g_rot.x; s_w[tid][11] = g_rot.y; s_w[tid][12] = g_rot.z; s_w[tid][13] = g_rot.w;
+		s_w[tid][14] = gm[0]; s_w[tid][15] = gm[1]; s_w[tid][16] = gm[2];
+		s_w[tid][17] = 0.f; s_w[tid][18] = 0.f;
+		// a visible Gaussian hidden behind nearer splats receives no gradient: like an invisible one it sends nothing
+		s_w[tid][19] = __uint_as_float(visible && gnz ? dp.epoch : 0u);
 	}
 
 	// ---- the 14 small parameters of this Gaussian
 	if (valid) {
-		// a zero gradient on zero moments is an exact no-op of Adam (see frest_stream_kernel): hidden / never-reached Gaussians are not rewritten
+		// a zero gradient on zero moments is an exact no-op of Adam (see adam4_unless_noop): hidden / never-reached Gaussians are not rewritten
 		bool idle = false;
 		if (LIVE) {
-			// the f_rest gradient is w_k * masked dL/dRGB: zero unless one of gm (in the seed row) is non-zero
-			const bool gnz = g_xyz.x != 0.f || g_xyz.y != 0.f || g_xyz.z != 0.f || g_dc.x != 0.f || g_dc.y != 0.f || g_dc.z != 0.f || g_scale.x != 0.f ||
-			                 g_scale.y != 0.f || g_scale.z != 0.f || g_opac != 0.f || g_rot.x != 0.f || g_rot.y != 0.f || g_rot.z != 0.f || g_rot.w != 0.f ||
-			                 s_w[tid][16] != 0.f || s_w[tid][17] != 0.f || s_w[tid][18] != 0.f;
 			if (gnz && !was_live) adam_live[idx] = 1;
 			idle = !(gnz || was_live);
 			s_live[tid] = !idle;
 			if (was_live) load_moments();
 		} else if (ADAM) {
-			bool nz = g_xyz.x != 0.f || g_xyz.y != 0.f || g_xyz.z != 0.f || g_dc.x != 0.f || g_dc.y != 0.f || g_dc.z != 0.f || g_scale.x != 0.f ||
-			          g_scale.y != 0.f || g_scale.z != 0.f || g_opac != 0.f || g_rot.x != 0.f || g_rot.y != 0.f || g_rot.z != 0.f || g_rot.w != 0.f ||
-			          mo != 0.f || vo != 0.f || mr.x != 0.f || mr.y != 0.f || mr.z != 0.f || mr.w != 0.f || vr.x != 0.f || vr.y != 0.f || vr.z != 0.f || vr.w != 0.f;
-#pragma unroll
-			for (int a = 0; a < 3; a++)
-#pragma unroll
-				for (int c = 0; c < 3; c++) nz = nz || m3[a][c] != 0.f || v3[a][c] != 0.f;
-			idle = !nz;
+			idle = !(any_nonzero(g) || any_nonzero(m, v));
 		}
 		if (ADAM && !idle) {
-			const float gx[3] = {g_xyz.x, g_xyz.y, g_xyz.z}, gd[3] = {g_dc.x, g_dc.y, g_dc.z}, gs[3] = {g_scale.x, g_scale.y, g_scale.z};
-#pragma unroll
-			for (int c = 0; c < 3; c++) {
-				adam1(sp_xyz[c], m3[0][c], v3[0][c], gx[c], h.lr[0] * ac.inv_bc1, ac);
-				adam1(sp_dc[c], m3[1][c], v3[1][c], gd[c], h.lr[1] * ac.inv_bc1, ac);
-				adam1(sp_sc[c], m3[2][c], v3[2][c], gs[c], h.lr[4] * ac.inv_bc1, ac);
-			}
-			adam1(sp_op, mo, vo, g_opac, h.lr[3] * ac.inv_bc1, ac);
-			const float lrr = h.lr[5] * ac.inv_bc1;
-			adam1(sp_rot.x, mr.x, vr.x, g_rot.x, lrr, ac);
-			adam1(sp_rot.y, mr.y, vr.y, g_rot.y, lrr, ac);
-			adam1(sp_rot.z, mr.z, vr.z, g_rot.z, lrr, ac);
-			adam1(sp_rot.w, mr.w, vr.w, g_rot.w, lrr, ac);
-#pragma unroll
-			for (int c = 0; c < 3; c++) {
-				t.p[0][3 * idx + c] = sp_xyz[c]; t.m[0][3 * idx + c] = m3[0][c]; t.v[0][3 * idx + c] = v3[0][c];
-				t.p[1][3 * idx + c] = sp_dc[c]; t.m[1][3 * idx + c] = m3[1][c]; t.v[1][3 * idx + c] = v3[1][c];
-				t.p[4][3 * idx + c] = sp_sc[c]; t.m[4][3 * idx + c] = m3[2][c]; t.v[4][3 * idx + c] = v3[2][c];
-			}
-			t.p[3][idx] = sp_op; t.m[3][idx] = mo; t.v[3][idx] = vo;
-			reinterpret_cast<float4*>(t.p[5])[idx] = sp_rot; reinterpret_cast<float4*>(t.m[5])[idx] = mr; reinterpret_cast<float4*>(t.v[5])[idx] = vr;
+			adam_small(p, m, v, g, 1.f, h, ac);
+			store_small(t.p, idx, p); store_small(t.m, idx, m); store_small(t.v, idx, v);
 		} else if (BASE == MODE_GRADS) {
-			grads.g[0][3 * idx] = g_xyz.x; grads.g[0][3 * idx + 1] = g_xyz.y; grads.g[0][3 * idx + 2] = g_xyz.z;
-			grads.g[1][3 * idx] = g_dc.x; grads.g[1][3 * idx + 1] = g_dc.y; grads.g[1][3 * idx + 2] = g_dc.z;
-			grads.g[3][idx] = g_opac;
-			grads.g[4][3 * idx] = g_scale.x; grads.g[4][3 * idx + 1] = g_scale.y; grads.g[4][3 * idx + 2] = g_scale.z;
-			reinterpret_cast<float4*>(grads.g[5])[idx] = g_rot;
+			store_small(grads.g, idx, g);
 		}
 	}
 	__syncthreads();
@@ -408,17 +445,8 @@ __global__ void __launch_bounds__(256) frest_stream_kernel(uint32_t e_first, uin
 	}
 	if (e + 4 <= e_end) {
 		if (ADAM) {
-			float4 mm = __ldcs(reinterpret_cast<const float4*>(m + e)), vv = __ldcs(reinterpret_cast<const float4*>(v + e));
-			// a zero gradient on zero moments is an exact no-op of Adam (m' = v' = 0, p' = p - lr * 0 / (0 + eps) = p): such elements
-			// (Gaussians no view has reached since their moments were created) are neither re-read nor rewritten
-			if (g[0] == 0.f && g[1] == 0.f && g[2] == 0.f && g[3] == 0.f && mm.x == 0.f && mm.y == 0.f && mm.z == 0.f && mm.w == 0.f &&
-			    vv.x == 0.f && vv.y == 0.f && vv.z == 0.f && vv.w == 0.f) return;
-			float4 pp = __ldcs(reinterpret_cast<const float4*>(p + e));
-			adam1(pp.x, mm.x, vv.x, g[0], lr_eff, ac);
-			adam1(pp.y, mm.y, vv.y, g[1], lr_eff, ac);
-			adam1(pp.z, mm.z, vv.z, g[2], lr_eff, ac);
-			adam1(pp.w, mm.w, vv.w, g[3], lr_eff, ac);
-			__stcs(reinterpret_cast<float4*>(p + e), pp); __stcs(reinterpret_cast<float4*>(m + e), mm); __stcs(reinterpret_cast<float4*>(v + e), vv);
+			float4 pp;
+			if (adam4_unless_noop(p + e, m + e, v + e, make_float4(g[0], g[1], g[2], g[3]), lr_eff, ac, pp)) __stcs(reinterpret_cast<float4*>(p + e), pp);
 		} else {
 			__stcs(reinterpret_cast<float4*>(gout + e), make_float4(g[0], g[1], g[2], g[3]));
 		}
@@ -455,11 +483,7 @@ __global__ void __launch_bounds__(256) adam_kernel(size_t n4, float4* __restrict
 	if (i >= n4) return;
 	float4 pp = p[i], mm = m[i], vv = v[i];
 	const float4 gg = g[i];
-	const float le = lr * c.inv_bc1;
-	adam1(pp.x, mm.x, vv.x, gg.x * grad_scale, le, c);
-	adam1(pp.y, mm.y, vv.y, gg.y * grad_scale, le, c);
-	adam1(pp.z, mm.z, vv.z, gg.z * grad_scale, le, c);
-	adam1(pp.w, mm.w, vv.w, gg.w * grad_scale, le, c);
+	adam4(pp, mm, vv, make_float4(gg.x * grad_scale, gg.y * grad_scale, gg.z * grad_scale, gg.w * grad_scale), lr * c.inv_bc1, c);
 	p[i] = pp; m[i] = mm; v[i] = vv;
 }
 __global__ void adam_tail_kernel(size_t start, size_t n, float* p, float* m, float* v, const float* g, float lr, AdamCoef c, float grad_scale)
@@ -475,23 +499,6 @@ __global__ void adam_tail_kernel(size_t start, size_t n, float* p, float* m, flo
 // owner) and writes the updated parameters into EVERY rank's parameter tensors (remote stores over NVLink): reduce-scatter,
 // sharded optimizer and all-gather without a materialised reduced gradient and without a collective call.
 // ------------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void sh_weights(int deg, const float3 pos, const float3 campos, float* w /*[16]*/)
-{
-	// same expressions as sh_backward_t (psb_backward.cuh): the owner reproduces the source rank's weights bit for bit
-	const float3 d = make_float3(pos.x - campos.x, pos.y - campos.y, pos.z - campos.z);
-	const float len = sqrtf(d.x * d.x + d.y * d.y + d.z * d.z);
-	const float x = d.x / len, y = d.y / len, z = d.z / len;
-	const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-	w[0] = kSH_C0;
-	w[1] = -kSH_C1 * y; w[2] = kSH_C1 * z; w[3] = -kSH_C1 * x;
-	w[4] = kSH_C2_0 * xy; w[5] = kSH_C2_1 * yz; w[6] = kSH_C2_2 * (2.f * zz - xx - yy); w[7] = kSH_C2_3 * xz; w[8] = kSH_C2_4 * (xx - yy);
-	w[9] = kSH_C3_0 * y * (3.f * xx - yy); w[10] = kSH_C3_1 * xy * z; w[11] = kSH_C3_2 * y * (4.f * zz - xx - yy);
-	w[12] = kSH_C3_3 * z * (2.f * zz - 3.f * xx - 3.f * yy); w[13] = kSH_C3_4 * x * (4.f * zz - xx - yy); w[14] = kSH_C3_5 * z * (xx - yy);
-	w[15] = kSH_C3_6 * x * (xx - 3.f * yy);
-	const int ncoef = (deg + 1) * (deg + 1);
-#pragma unroll
-	for (int k = 0; k < 16; k++) if (k >= ncoef) w[k] = 0.f;
-}
 
 // One block per owned chunk, one thread per Gaussian: the 14 small parameters (Adam + all-gather) and the summed f_rest gradient row.
 // The updated small parameters leave through shared memory: each of the five tensors' 128-row chunk is contiguous in every replica, so
@@ -501,23 +508,17 @@ __global__ void __launch_bounds__(TB) shard_adam_small_kernel(DpShard d, TrainTe
 {
 	__shared__ __align__(16) float s_g[TB * REST];
 	__shared__ __align__(16) float s_out[TB * 14];   // [xyz 384 | f_dc 384 | scaling 384 | opacity 128 | rotation 512] in tensor-chunk layout
-	const int tid = threadIdx.x, lc = d.lc_first + blockIdx.x;
+	const int tid = threadIdx.x, lc = blockIdx.x;
 	const int chunk = lc * d.world + d.rank;
 	const int idx = chunk * TB + tid;
 	const bool valid = idx < d.P;
-	AdamCoef ac;
-	ac.beta1 = h.beta1; ac.beta2 = h.beta2; ac.eps = h.eps; ac.inv_bc1 = h.inv_bc1; ac.inv_bc2_sqrt = 1.0f / h.bc2_sqrt;
 
-	float acc[14];
+	SmallRow acc = {};  // summed records
 	float G[REST];
 #pragma unroll
-	for (int i = 0; i < 14; i++) acc[i] = 0.f;
-#pragma unroll
 	for (int i = 0; i < REST; i++) G[i] = 0.f;
-	float sp_xyz[3] = {0, 0, 1}, sp_dc[3] = {0, 0, 0}, sp_sc[3] = {0, 0, 0}, sp_op = 0.f;
-	float4 sp_rot = make_float4(1, 0, 0, 0);
-	float m3[3][3], v3[3][3], mo = 0.f, vo = 0.f;
-	float4 mr = make_float4(0, 0, 0, 0), vr = mr;
+	SmallRow p = {{0, 0, 1}, {0, 0, 0}, {0, 0, 0}, 0.f, make_float4(1, 0, 0, 0)};
+	SmallRow m = {}, v = {};
 	bool live = false;
 	if (valid) {
 		// every rank's epoch word of this row first (independent loads: one round trip instead of one per source)
@@ -527,73 +528,41 @@ __global__ void __launch_bounds__(TB) shard_adam_small_kernel(DpShard d, TrainTe
 			tail[s] = make_float4(0.f, 0.f, 0.f, 0.f);
 			if (s < d.world) tail[s] = (reinterpret_cast<const float4*>(d.inbox) + (((size_t)s * d.nlocal_max + lc) * TB + tid) * (DP_REC / 4))[4];
 		}
-		const int tsel[3] = {0, 1, 4};
-#pragma unroll
-		for (int a = 0; a < 3; a++)
-#pragma unroll
-			for (int c = 0; c < 3; c++) { m3[a][c] = t.m[tsel[a]][3 * idx + c]; v3[a][c] = t.v[tsel[a]][3 * idx + c]; }
-		mo = t.m[3][idx]; vo = t.v[3][idx];
-		mr = reinterpret_cast<const float4*>(t.m[5])[idx]; vr = reinterpret_cast<const float4*>(t.v[5])[idx];
-#pragma unroll
-		for (int c = 0; c < 3; c++) { sp_xyz[c] = t.p[0][3 * idx + c]; sp_dc[c] = t.p[1][3 * idx + c]; sp_sc[c] = t.p[4][3 * idx + c]; }
-		sp_op = t.p[3][idx];
-		sp_rot = reinterpret_cast<const float4*>(t.p[5])[idx];
-		const float3 pos = make_float3(sp_xyz[0], sp_xyz[1], sp_xyz[2]);
+		load_small(m, t.m, idx);
+		load_small(v, t.v, idx);
+		load_small(p, t.p, idx);
+		const float3 pos = make_float3(p.xyz[0], p.xyz[1], p.xyz[2]);
 #pragma unroll
 		for (int s = 0; s < DP_MAX_WORLD; s++) {
 			if (s >= d.world || __float_as_uint(tail[s].w) != d.epoch) continue;  // rank s sent nothing for this Gaussian in this step
 			const float4* r = reinterpret_cast<const float4*>(d.inbox) + (((size_t)s * d.nlocal_max + lc) * TB + tid) * (DP_REC / 4);
 			const float4 r0 = r[0], r1 = r[1], r2 = r[2], r3 = r[3];
-			acc[0] += r0.x; acc[1] += r0.y; acc[2] += r0.z; acc[3] += r0.w;
-			acc[4] += r1.x; acc[5] += r1.y; acc[6] += r1.z; acc[7] += r1.w;
-			acc[8] += r2.x; acc[9] += r2.y; acc[10] += r2.z; acc[11] += r2.w;
-			acc[12] += r3.x; acc[13] += r3.y;
+			acc.xyz[0] += r0.x; acc.xyz[1] += r0.y; acc.xyz[2] += r0.z; acc.dc[0] += r0.w;
+			acc.dc[1] += r1.x; acc.dc[2] += r1.y; acc.op += r1.z; acc.sc[0] += r1.w;
+			acc.sc[1] += r2.x; acc.sc[2] += r2.y; acc.rot.x += r2.z; acc.rot.y += r2.w;
+			acc.rot.z += r3.x; acc.rot.w += r3.y;
 			const float gm[3] = {r3.z, r3.w, tail[s].x};
 			const float* mt = d.meta + 8 * s;
+			const int deg = (int)mt[3], ncoef = (deg + 1) * (deg + 1);
 			float w[16];
-			sh_weights((int)mt[3], pos, make_float3(mt[0], mt[1], mt[2]), w);
+			sh_basis(sh_dir(make_float3(pos.x - mt[0], pos.y - mt[1], pos.z - mt[2])), w);
 #pragma unroll
 			for (int k = 1; k < 16; k++)
 #pragma unroll
-				for (int ch = 0; ch < 3; ch++) G[3 * (k - 1) + ch] += w[k] * gm[ch];
+				for (int ch = 0; ch < 3; ch++) G[3 * (k - 1) + ch] += (k < ncoef ? w[k] : 0.f) * gm[ch];
 		}
-		const float gs = grad_scale;
-		const float lx = h.lr[0] * ac.inv_bc1, ld = h.lr[1] * ac.inv_bc1, lo = h.lr[3] * ac.inv_bc1, ls = h.lr[4] * ac.inv_bc1, lrr = h.lr[5] * ac.inv_bc1;
 		// zero gradient on zero moments = an exact no-op of Adam: nothing to update (hidden / never-reached Gaussians)
-		live = mo != 0.f || vo != 0.f || mr.x != 0.f || mr.y != 0.f || mr.z != 0.f || mr.w != 0.f || vr.x != 0.f || vr.y != 0.f || vr.z != 0.f || vr.w != 0.f;
-#pragma unroll
-		for (int i = 0; i < 14; i++) live = live || acc[i] != 0.f;
-#pragma unroll
-		for (int a = 0; a < 3; a++)
-#pragma unroll
-			for (int c = 0; c < 3; c++) live = live || m3[a][c] != 0.f || v3[a][c] != 0.f;
+		live = any_nonzero(m, v) || any_nonzero(acc);
 		if (live) {
-#pragma unroll
-			for (int c = 0; c < 3; c++) {
-				adam1(sp_xyz[c], m3[0][c], v3[0][c], acc[c] * gs, lx, ac);
-				adam1(sp_dc[c], m3[1][c], v3[1][c], acc[3 + c] * gs, ld, ac);
-				adam1(sp_sc[c], m3[2][c], v3[2][c], acc[7 + c] * gs, ls, ac);
-			}
-			adam1(sp_op, mo, vo, acc[6] * gs, lo, ac);
-			adam1(sp_rot.x, mr.x, vr.x, acc[10] * gs, lrr, ac);
-			adam1(sp_rot.y, mr.y, vr.y, acc[11] * gs, lrr, ac);
-			adam1(sp_rot.z, mr.z, vr.z, acc[12] * gs, lrr, ac);
-			adam1(sp_rot.w, mr.w, vr.w, acc[13] * gs, lrr, ac);
-#pragma unroll
-			for (int c = 0; c < 3; c++) {
-				t.m[0][3 * idx + c] = m3[0][c]; t.v[0][3 * idx + c] = v3[0][c];
-				t.m[1][3 * idx + c] = m3[1][c]; t.v[1][3 * idx + c] = v3[1][c];
-				t.m[4][3 * idx + c] = m3[2][c]; t.v[4][3 * idx + c] = v3[2][c];
-			}
-			t.m[3][idx] = mo; t.v[3][idx] = vo;
-			reinterpret_cast<float4*>(t.m[5])[idx] = mr; reinterpret_cast<float4*>(t.v[5])[idx] = vr;
+			adam_small(p, m, v, acc, grad_scale, h, AdamCoef(h));
+			store_small(t.m, idx, m); store_small(t.v, idx, v);
 		}
 	}
 	// the block's (updated or unchanged) small parameters in tensor-chunk layout
 #pragma unroll
-	for (int c = 0; c < 3; c++) { s_out[3 * tid + c] = sp_xyz[c]; s_out[384 + 3 * tid + c] = sp_dc[c]; s_out[768 + 3 * tid + c] = sp_sc[c]; }
-	s_out[1152 + tid] = sp_op;
-	reinterpret_cast<float4*>(s_out + 1280)[tid] = sp_rot;
+	for (int c = 0; c < 3; c++) { s_out[3 * tid + c] = p.xyz[c]; s_out[384 + 3 * tid + c] = p.dc[c]; s_out[768 + 3 * tid + c] = p.sc[c]; }
+	s_out[1152 + tid] = p.op;
+	reinterpret_cast<float4*>(s_out + 1280)[tid] = p.rot;
 	// summed f_rest gradient row -> local scratch (coalesced through shared memory; row stride 45 words is conflict-free)
 #pragma unroll
 	for (int i = 0; i < REST; i++) s_g[tid * REST + i] = G[i] * grad_scale;
@@ -625,7 +594,7 @@ __global__ void __launch_bounds__(TB) shard_adam_small_kernel(DpShard d, TrainTe
 // to every rank. Rows nobody has ever seen (g = m = v = 0) are left alone: their Adam update is exactly zero.
 __global__ void __launch_bounds__(256) shard_adam_frest_kernel(DpShard d, TrainTensors t, float lr_eff, AdamCoef ac)
 {
-	const int lc = d.lc_first + blockIdx.x;
+	const int lc = blockIdx.x;
 	const int chunk = lc * d.world + d.rank;
 	const size_t e0 = (size_t)chunk * (TB * REST);
 	const size_t e_end = (size_t)d.P * REST;
@@ -637,17 +606,8 @@ __global__ void __launch_bounds__(256) shard_adam_frest_kernel(DpShard d, TrainT
 		const size_t e = e0 + 4 * (size_t)i;
 		if (e >= e_end) break;
 		if (e + 4 <= e_end) {
-			const float4 gg = __ldcs(reinterpret_cast<const float4*>(g + 4 * i));
-			float4 mm = __ldcs(reinterpret_cast<const float4*>(m + e)), vv = __ldcs(reinterpret_cast<const float4*>(v + e));
-			const bool idle = gg.x == 0.f && gg.y == 0.f && gg.z == 0.f && gg.w == 0.f && mm.x == 0.f && mm.y == 0.f && mm.z == 0.f && mm.w == 0.f &&
-			                  vv.x == 0.f && vv.y == 0.f && vv.z == 0.f && vv.w == 0.f;
-			if (idle) continue;
-			float4 pp = __ldcs(reinterpret_cast<const float4*>(p + e));
-			adam1(pp.x, mm.x, vv.x, gg.x, lr_eff, ac);
-			adam1(pp.y, mm.y, vv.y, gg.y, lr_eff, ac);
-			adam1(pp.z, mm.z, vv.z, gg.z, lr_eff, ac);
-			adam1(pp.w, mm.w, vv.w, gg.w, lr_eff, ac);
-			__stcs(reinterpret_cast<float4*>(m + e), mm); __stcs(reinterpret_cast<float4*>(v + e), vv);
+			float4 pp;
+			if (!adam4_unless_noop(p + e, m + e, v + e, __ldcs(reinterpret_cast<const float4*>(g + 4 * i)), lr_eff, ac, pp)) continue;
 			for (int jj = 0; jj < d.world; jj++) {
 				const int j = (d.rank + 1 + jj) % d.world;
 				*reinterpret_cast<float4*>(d.param[j][2] + e) = pp;
@@ -698,7 +658,7 @@ __device__ __forceinline__ unsigned long long global_timer_ns()
 // process) must not hang this GPU — after timeout_ns the kernel records the failure and returns.
 __global__ void wait_flags_kernel(const uint32_t* flags, int world, uint32_t epoch, uint32_t* status, unsigned long long timeout_ns)
 {
-	const int lane = threadIdx.x;   // `world` = number of flag words (ranks, or groups x ranks), <= blockDim.x
+	const int lane = threadIdx.x;
 	if (lane >= world) return;
 	const volatile uint32_t* f = flags + lane;
 	const unsigned long long t0 = global_timer_ns();
@@ -709,6 +669,52 @@ __global__ void wait_flags_kernel(const uint32_t* flags, int world, uint32_t epo
 	__threadfence_system();
 }
 
+// The only launch of gaussian_backward_kernel: MODE picked at run time by launch_gaussian_backward.
+template <int MODE, typename... Args>
+void run_gaussian_backward(int first, int P, cudaStream_t stream, Args... args)
+{
+	gaussian_backward_kernel<MODE><<<cdiv(P - first, TB), TB, 0, stream>>>(first, P, args...);
+}
+
+// Gaussians [first, P) in mode `mode` (MODE_GRADS, MODE_ADAM, MODE_ADAM_LIVE or MODE_PUSH, each optionally | MODE_DEPTH)
+int launch_gaussian_backward(int mode, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink,
+                             const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
+                             float* seeds, const DpPush& dp, unsigned char* adam_live, cudaStream_t stream)
+{
+	if (P - first <= 0) return 0;
+	float4* sink4 = reinterpret_cast<float4*>(sink);
+	float4* seeds4 = reinterpret_cast<float4*>(seeds);
+#define PSB_BACKWARD_CASE(M) \
+	case M: run_gaussian_backward<M>(first, P, stream, t, cam, geom, sink4, h, grads, st, counters, capacity, seeds4, dp, adam_live); break
+	switch (mode) {
+		PSB_BACKWARD_CASE(MODE_GRADS);
+		PSB_BACKWARD_CASE(MODE_ADAM);
+		PSB_BACKWARD_CASE(MODE_ADAM_LIVE);
+		PSB_BACKWARD_CASE(MODE_PUSH);
+		PSB_BACKWARD_CASE(MODE_GRADS | MODE_DEPTH);
+		PSB_BACKWARD_CASE(MODE_ADAM | MODE_DEPTH);
+		PSB_BACKWARD_CASE(MODE_ADAM_LIVE | MODE_DEPTH);
+		PSB_BACKWARD_CASE(MODE_PUSH | MODE_DEPTH);
+		default: set_error_msg("launch_gaussian_backward: unknown mode"); return -1;
+	}
+#undef PSB_BACKWARD_CASE
+	PSB_LAUNCH_OK();
+	return 0;
+}
+
+// dp_signal_kernel for `world` ranks: raises this rank's word in flag[j] of every rank j; with meta, first publishes campos and degree
+int launch_signal(uint32_t* const* flag, float* const* meta, const float* campos, int degree, int world, int rank, uint32_t epoch,
+                  cudaStream_t stream)
+{
+	DpSignal s;
+	memset(&s, 0, sizeof(s));
+	for (int j = 0; j < world; j++) { s.flag[j] = flag[j]; s.meta[j] = meta ? meta[j] : nullptr; }
+	s.campos = campos; s.degree = degree; s.world = world; s.rank = rank; s.epoch = epoch;
+	dp_signal_kernel<<<1, 32, 0, stream>>>(s);
+	PSB_LAUNCH_OK();
+	return 0;
+}
+
 }  // namespace
 
 int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, float* seeds,
@@ -716,25 +722,16 @@ int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, co
                           cudaStream_t stream, cudaEvent_t between, unsigned char* adam_live, bool depth)
 {
 	if (P - first <= 0) return 0;
-	const int grid = cdiv(P - first, TB);
-	float4* sd4 = reinterpret_cast<float4*>(seeds);
-	float4* sink4 = reinterpret_cast<float4*>(sink);
 	if (!seeds) { set_error_msg("launch_fused_backward: seed scratch missing"); return -1; }
 	if ((size_t)P * REST >= (size_t)UINT32_MAX - 8) { set_error_msg("psb_trainer: too many Gaussians for 32-bit element indices"); return -1; }
 	DpPush nodp;
 	memset(&nodp, 0, sizeof(nodp));
 	unsigned char* live = adam ? adam_live : nullptr;
-	if (depth) {
-		if (live) gaussian_backward_kernel<MODE_ADAM_LIVE | MODE_DEPTH><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, live);
-		else if (adam) gaussian_backward_kernel<MODE_ADAM | MODE_DEPTH><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, nullptr);
-		else gaussian_backward_kernel<MODE_GRADS | MODE_DEPTH><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, nullptr);
-	} else if (live) gaussian_backward_kernel<MODE_ADAM_LIVE><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, live);
-	else if (adam) gaussian_backward_kernel<MODE_ADAM><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, nullptr);
-	else gaussian_backward_kernel<MODE_GRADS><<<grid, TB, 0, stream>>>(first, P, t, cam, geom, sink4, h, grads, st, counters, capacity, sd4, nodp, nullptr);
-	PSB_LAUNCH_OK();
+	const int mode = (live ? MODE_ADAM_LIVE : adam ? MODE_ADAM : MODE_GRADS) | (depth ? MODE_DEPTH : 0);
+	int rc;
+	if ((rc = launch_gaussian_backward(mode, first, P, t, cam, geom, sink, h, grads, st, counters, capacity, seeds, nodp, live, stream))) return rc;
 	if (between) cudaEventRecord(between, stream);
-	AdamCoef ac;
-	ac.beta1 = h.beta1; ac.beta2 = h.beta2; ac.eps = h.eps; ac.inv_bc1 = h.inv_bc1; ac.inv_bc2_sqrt = 1.0f / h.bc2_sqrt;
+	const AdamCoef ac(h);
 	const uint32_t e0 = (uint32_t)first * REST, e1 = (uint32_t)P * REST;
 	const unsigned gridB = (unsigned)(((size_t)(e1 - e0) + 1023) / 1024);
 	if (adam) frest_stream_kernel<true><<<gridB, 256, 0, stream>>>(e0, e1, t.p[2], t.m[2], t.v[2], nullptr, seeds, h.lr[2] * ac.inv_bc1, ac, counters, capacity, live);
@@ -751,53 +748,34 @@ int launch_adam_live_rebuild(int P, const TrainTensors& t, unsigned char* live, 
 	return 0;
 }
 
-int launch_push_backward(int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, const StepHyper& h,
+int launch_push_backward(int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, const StepHyper& h,
                          const DensifyStats& st, const uint32_t* counters, uint32_t capacity, const DpPush& dp, cudaStream_t stream, bool depth)
 {
-	GradSegments nog;
-	memset(&nog, 0, sizeof(nog));
-	if (P - first > 0) {  // Gaussians [first, P): one pipeline group (first is a multiple of 128 * world)
-		if (depth)
-			gaussian_backward_kernel<MODE_PUSH | MODE_DEPTH><<<cdiv(P - first, TB), TB, 0, stream>>>(first, P, t, cam, geom, reinterpret_cast<float4*>(sink), h, nog, st,
-			                                                                                       counters, capacity, nullptr, dp, nullptr);
-		else
-			gaussian_backward_kernel<MODE_PUSH><<<cdiv(P - first, TB), TB, 0, stream>>>(first, P, t, cam, geom, reinterpret_cast<float4*>(sink), h, nog, st, counters,
-			                                                                          capacity, nullptr, dp, nullptr);
-		PSB_LAUNCH_OK();
-	}
-	DpSignal s;
-	memset(&s, 0, sizeof(s));
-	for (int j = 0; j < dp.world; j++) { s.flag[j] = dp.grad_flag[j]; s.meta[j] = dp.meta[j]; }
-	s.campos = cam.campos; s.world = dp.world; s.rank = dp.rank; s.degree = h.D; s.epoch = dp.epoch;
-	dp_signal_kernel<<<1, 32, 0, stream>>>(s);
-	PSB_LAUNCH_OK();
-	return 0;
+	const GradSegments nog = {};
+	int rc;
+	if ((rc = launch_gaussian_backward(MODE_PUSH | (depth ? MODE_DEPTH : 0), 0, P, t, cam, geom, sink, h, nog, st, counters, capacity, nullptr, dp,
+	                                   nullptr, stream)))
+		return rc;
+	return launch_signal(dp.grad_flag, dp.meta, cam.campos, h.D, dp.world, dp.rank, dp.epoch, stream);
 }
 
 int launch_shard_adam(const DpShard& d, const TrainTensors& t, const StepHyper& h, float grad_scale, cudaStream_t stream, cudaEvent_t between)
 {
-	AdamCoef ac;
-	ac.beta1 = h.beta1; ac.beta2 = h.beta2; ac.eps = h.eps; ac.inv_bc1 = h.inv_bc1; ac.inv_bc2_sqrt = 1.0f / h.bc2_sqrt;
-	if (d.nlocal > 0) {  // owned chunks [lc_first, lc_first + nlocal) of this pipeline group
+	if (d.nlocal > 0) {
+		const AdamCoef ac(h);
 		shard_adam_small_kernel<<<d.nlocal, TB, 0, stream>>>(d, t, h, grad_scale);
 		PSB_LAUNCH_OK();
 		if (between) cudaEventRecord(between, stream);
 		shard_adam_frest_kernel<<<d.nlocal, 256, 0, stream>>>(d, t, h.lr[2] * ac.inv_bc1, ac);
 		PSB_LAUNCH_OK();
 	}
-	DpSignal s;
-	memset(&s, 0, sizeof(s));
-	for (int j = 0; j < d.world; j++) s.flag[j] = d.param_flag[j];
-	s.world = d.world; s.rank = d.rank; s.epoch = d.epoch;
-	dp_signal_kernel<<<1, 32, 0, stream>>>(s);
-	PSB_LAUNCH_OK();
-	return 0;
+	return launch_signal(d.param_flag, nullptr, nullptr, 0, d.world, d.rank, d.epoch, stream);
 }
 
 int launch_wait_flags(const uint32_t* flags, int world, uint32_t epoch, uint32_t* status, cudaStream_t stream)
 {
 	static const unsigned long long timeout_ns = (unsigned long long)(getenv("PSB_DP_TIMEOUT_MS") ? atoll(getenv("PSB_DP_TIMEOUT_MS")) : 20000) * 1000000ull;
-	wait_flags_kernel<<<1, world <= 32 ? 32 : 64, 0, stream>>>(flags, world, epoch, status, timeout_ns);
+	wait_flags_kernel<<<1, 32, 0, stream>>>(flags, world, epoch, status, timeout_ns);
 	PSB_LAUNCH_OK();
 	return 0;
 }
@@ -805,8 +783,7 @@ int launch_wait_flags(const uint32_t* flags, int world, uint32_t epoch, uint32_t
 int launch_adam(size_t n, float* p, float* m, float* v, const float* g, float lr, const StepHyper& h, float grad_scale, cudaStream_t stream)
 {
 	if (n == 0) return 0;
-	AdamCoef c;
-	c.beta1 = h.beta1; c.beta2 = h.beta2; c.eps = h.eps; c.inv_bc1 = h.inv_bc1; c.inv_bc2_sqrt = 1.0f / h.bc2_sqrt;
+	const AdamCoef c(h);
 	const bool aligned = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(m) | reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(g)) & 15) == 0;
 	const size_t n4 = aligned ? n / 4 : 0;
 	if (n4) {

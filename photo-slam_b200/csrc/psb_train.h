@@ -48,15 +48,14 @@ struct DpShard {             // what the owner-side Adam kernels need
 	const float* inbox;                // local inbox
 	const float* meta;                 // local meta rows
 	float* g_rest;                     // local scratch [nlocal_max*128][45]: summed f_rest gradient of the owned rows
-	int world, rank, nlocal_max, nlocal, P;   // nlocal: owned chunks handled by this launch, starting at local chunk lc_first
-	int lc_first;
+	int world, rank, nlocal_max, nlocal, P;   // nlocal: owned chunks of this rank
 	uint32_t epoch;
 };
-int launch_push_backward(int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, const StepHyper& h,
+int launch_push_backward(int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, const StepHyper& h,
                          const DensifyStats& st, const uint32_t* counters, uint32_t capacity, const DpPush& dp, cudaStream_t stream,
                          bool depth = false /* the sink rows carry dL/dz in slot 11 (render_bwd_depth_kernel) */);
 int launch_shard_adam(const DpShard& d, const TrainTensors& t, const StepHyper& h, float grad_scale, cudaStream_t stream, cudaEvent_t between = nullptr);
-// spins (device side) until flags[0..world) >= epoch (world <= 64 words); after `timeout_ms` writes 1 to *status and gives up
+// spins (device side) until flags[0..world) >= epoch (world <= 32 words); after `timeout_ms` writes 1 to *status and gives up
 int launch_wait_flags(const uint32_t* flags, int world, uint32_t epoch, uint32_t* status, cudaStream_t stream);
 
 // Gaussians [first, P) (first must be a multiple of 128 so f_rest chunks stay 16-byte aligned)

@@ -48,6 +48,9 @@ struct psb_trainer {
 	cudaEvent_t ev[NSTAGE + 1] = {};
 	bool ev_ready = false, ev_recorded = false;
 	void mark(int i, cudaStream_t s) { if (profiling && ev_ready) cudaEventRecord(ev[i], s); }
+	cudaEvent_t event(int i) const { return profiling && ev_ready ? ev[i] : nullptr; }
+	// the last boundary of a profiled call: psb_trainer_stage_times reads the stages up to it
+	void end_stages(int last, cudaStream_t s) { mark(last, s); last_stage = last; ev_recorded = profiling && ev_ready; }
 };
 
 namespace {
@@ -118,15 +121,21 @@ int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_
 
 Camera to_camera(const psb_camera* c)
 {
-	Camera cam;
-	cam.view = c->viewmatrix; cam.proj = c->projmatrix; cam.campos = c->campos;
-	cam.tan_fovx = c->tan_fovx; cam.tan_fovy = c->tan_fovy;
-	cam.focal_y = c->height / (2.0f * c->tan_fovy);
-	cam.focal_x = c->width / (2.0f * c->tan_fovx);
-	cam.W = c->width; cam.H = c->height;
-	cam.grid_x = (c->width + PSB_TILE_X - 1) / PSB_TILE_X;
-	cam.grid_y = (c->height + PSB_TILE_Y - 1) / PSB_TILE_Y;
-	return cam;
+	return make_camera(c->width, c->height, c->viewmatrix, c->projmatrix, c->campos, c->tan_fovx, c->tan_fovy);
+}
+
+// the scratch states of the last forward pass of P Gaussians over width x height pixels, carved from the context's arena
+struct Scratch {
+	GeomState geom;
+	ImgState img;
+	BinState bin;
+};
+Scratch carve_scratch(const psb_trainer* t, int P, int width, int height)
+{
+	char* gc = t->geom_chunk;
+	char* ic = t->img_chunk;
+	char* bc = t->bin_chunk;
+	return {GeomState::from_chunk(gc, (size_t)P), ImgState::from_chunk(ic, (size_t)width * height), BinState::from_chunk(bc, t->capacity)};
 }
 
 GaussIn raw_input(int P, int D, int M, const psb_model* m)
@@ -149,6 +158,25 @@ StepHyper to_hyper(const psb_step* s)
 	h.bc2_sqrt = (float)std::sqrt(1.0 - std::pow((double)s->beta2, s->step));
 	h.D = s->sh_degree;
 	return h;
+}
+
+TrainTensors train_tensors(const psb_model* m, bool moments)
+{
+	TrainTensors tt;
+	for (int i = 0; i < 6; i++) {
+		tt.p[i] = m->param[i];
+		tt.m[i] = moments ? m->exp_avg[i] : nullptr;
+		tt.v[i] = moments ? m->exp_avg_sq[i] : nullptr;
+	}
+	return tt;
+}
+
+DensifyStats densify_stats(const psb_model* m, const psb_step* s)
+{
+	DensifyStats st;
+	st.enabled = (s->update_densify_stats && m->max_radii2D && m->xyz_gradient_accum && m->denom) ? 1 : 0;
+	st.max_radii2D = m->max_radii2D; st.xyz_gradient_accum = m->xyz_gradient_accum; st.denom = m->denom;
+	return st;
 }
 
 int check_model(int P, int M, const psb_model* m, bool need_moments)
@@ -179,17 +207,31 @@ int check_depth(const psb_depth* d, const char* fn)
 	return 0;
 }
 
+// Gradient segments of P rows: six non-null pointers, features_rest and rotation 16-byte aligned (written with float4 stores).
+int check_grads(float* const* grads, int P, const char* fn)
+{
+	if (!grads) { set_error_msg(std::string(fn).append(": grads required").c_str()); return PSB_ERR_ARG; }
+	if (P <= 0) return 0;
+	for (int i = 0; i < 6; i++)
+		if (!grads[i]) { set_error_msg(std::string(fn).append(": null gradient segment").c_str()); return PSB_ERR_ARG; }
+	if ((reinterpret_cast<uintptr_t>(grads[2]) | reinterpret_cast<uintptr_t>(grads[5])) & 15) {
+		set_error_msg(std::string(fn).append(": the features_rest and rotation gradient segments must be 16-byte aligned").c_str());
+		return PSB_ERR_ARG;
+	}
+	return 0;
+}
+
 // forward from raw parameters into t->image (or out_color); out_depth != NULL: the depth variant also writes the expected depth there
 int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, const psb_camera* camera, const float* background,
-                float* out_color, int* radii, GeomState& geom, BinState& bin, ImgState& img, Camera& cam, cudaStream_t stream,
-                float* out_depth = nullptr)
+                float* out_color, int* radii, Scratch& sc, Camera& cam, cudaStream_t stream, float* out_depth = nullptr)
 {
 	int rc;
 	if ((rc = ensure(t, P, camera->width, camera->height, stream))) return rc;
 	cam = to_camera(camera);
-	char* gc = t->geom_chunk; geom = GeomState::from_chunk(gc, (size_t)P);
-	char* ic = t->img_chunk; img = ImgState::from_chunk(ic, (size_t)camera->width * camera->height);
-	char* bc = t->bin_chunk; bin = BinState::from_chunk(bc, t->capacity);
+	sc = carve_scratch(t, P, camera->width, camera->height);
+	GeomState& geom = sc.geom;
+	BinState& bin = sc.bin;
+	ImgState& img = sc.img;
 	const GaussIn in = raw_input(P, D, M, model);
 	t->mark(0, stream);
 	if ((rc = launch_preprocess(in, cam, radii, geom, /*raw=*/true, t->tight, stream))) return rc;
@@ -202,20 +244,29 @@ int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, con
 	PSB_CUDA_OK(cudaMemcpyAsync(t->h_count, geom.counters, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
 	PSB_CUDA_OK(cudaMemcpyAsync(t->h_count + 1, t->ovf, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
 	PSB_CUDA_OK(cudaEventRecord(t->readback, stream));
-	const int res = make_sort_plan(tile_id_bits(cam.grid_x * cam.grid_y)).npass & 1;
-	rc = launch_render_forward(cam, img.ranges, bin.inst[res], geom.rec, background, out_color ? out_color : t->image, img.final_T,
+	rc = launch_render_forward(cam, img.ranges, bin.inst[sorted_slot(cam.W, cam.H)], geom.rec, background, out_color ? out_color : t->image, img.final_T,
 	                           img.n_contrib, stream, out_depth);
 	t->mark(4, stream);
 	return rc;
 }
 
-int step_impl(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, const float* gt_image,
-              const float* mask, const psb_step* step, float* out_color, int* radii, float* const* grads, cudaStream_t stream,
-              bool tiles_only = false, const psb_depth* depth = nullptr)
+// What the first half of a training step leaves for its per-Gaussian stage: the sink rows hold the view's screen-space sums
+// (with a depth term also dL/dz in slot 11, which the per-Gaussian kernel that follows must consume).
+struct TileBackward {
+	GeomState geom;
+	Camera cam;
+	bool depth;
+};
+
+// render -> loss (+ depth loss) -> pinned read-back of the loss sums -> tile backward. `moments`: the caller's per-Gaussian stage
+// updates the Adam moments of the model.
+int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                         const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
+                         bool moments, cudaStream_t stream, TileBackward& out)
 {
 	int rc;
 	if (!t || !camera || !step || !background || !gt_image) { set_error_msg("psb_trainer_step: null argument"); return PSB_ERR_ARG; }
-	if ((rc = check_model(P, M, model, grads == nullptr && !tiles_only))) return rc;
+	if ((rc = check_model(P, M, model, moments))) return rc;
 	if (step->sh_degree < 0 || step->sh_degree > 3 || step->step < 1) { set_error_msg("psb_trainer_step: sh_degree in 0..3 and step >= 1 required"); return PSB_ERR_ARG; }
 	// depth loss: the depth plane is the caller's out_depth or the context's own; dL/dD lives in the context
 	const bool depth_loss = depth && depth->gt_depth;
@@ -226,8 +277,9 @@ int step_impl(psb_trainer* t, int P, int M, const psb_model* model, const psb_ca
 		if (!depth_plane) depth_plane = t->depth_buf;
 		dL_ddepth = t->depth_buf + (size_t)camera->width * camera->height;
 	}
-	GeomState geom; BinState bin; ImgState img; Camera cam;
-	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, geom, bin, img, cam, stream, depth_plane))) return rc;
+	Scratch sc;
+	Camera cam;
+	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, sc, cam, stream, depth_plane))) return rc;
 	const float* image = out_color ? out_color : t->image;
 	if ((rc = launch_loss(cam.H, cam.W, image, gt_image, mask, step->lambda_dssim, t->dmap, t->sums, t->dL_dpix, stream))) return rc;
 	if (depth_loss && (rc = launch_depth_loss(cam.H, cam.W, depth_plane, depth->gt_depth, mask, depth->lambda_depth, t->sums + 2, dL_ddepth, stream)))
@@ -248,25 +300,14 @@ int step_impl(psb_trainer* t, int P, int M, const psb_model* model, const psb_ca
 	sink.opacity = t->sink + 7; sink.opacity_stride = 12;
 	sink.color = t->sink + 8; sink.color_stride = 12;
 	sink.packed = 1;
-	const int res = make_sort_plan(tile_id_bits(cam.grid_x * cam.grid_y)).npass & 1;
-	if ((rc = launch_render_backward(cam, img.ranges, bin.inst[res], geom.rec, background, img.final_T, img.n_contrib, t->dL_dpix, sink, stream, dL_ddepth)))
+	if ((rc = launch_render_backward(cam, sc.img.ranges, sc.bin.inst[sorted_slot(cam.W, cam.H)], sc.geom.rec, background, sc.img.final_T, sc.img.n_contrib,
+	                                 t->dL_dpix, sink, stream, dL_ddepth)))
 		return rc;
 	t->mark(6, stream);
-	if (tiles_only) return 0;
-	TrainTensors tt;
-	for (int i = 0; i < 6; i++) { tt.p[i] = model->param[i]; tt.m[i] = model->exp_avg[i]; tt.v[i] = model->exp_avg_sq[i]; }
-	GradSegments gs;
-	for (int i = 0; i < 6; i++) gs.g[i] = grads ? grads[i] : nullptr;
-	DensifyStats st;
-	st.enabled = (step->update_densify_stats && model->max_radii2D && model->xyz_gradient_accum && model->denom) ? 1 : 0;
-	st.max_radii2D = model->max_radii2D; st.xyz_gradient_accum = model->xyz_gradient_accum; st.denom = model->denom;
-	const StepHyper h = to_hyper(step);
-	rc = launch_fused_backward(grads == nullptr, 0, P, tt, cam, geom, t->sink, t->seeds, h, gs, st, geom.counters, (uint32_t)t->capacity, stream,
-	                           (t->profiling && t->ev_ready) ? t->ev[7] : nullptr, grads == nullptr ? model->adam_live : nullptr, depth_loss);
-	t->mark(8, stream);
-	t->last_stage = 8;
-	t->ev_recorded = t->profiling && t->ev_ready;
-	return rc;
+	out.geom = sc.geom;
+	out.cam = cam;
+	out.depth = depth_loss;
+	return 0;
 }
 
 }  // namespace
@@ -285,10 +326,6 @@ struct psb_dp {
 	uint32_t epoch = 0;
 	bool connected = false;
 	cudaIpcMemHandle_t handle;
-	// pipeline: the Gaussians are cut into `groups` contiguous ranges (boundaries at multiples of 128 * world chunks); the owner-side Adam
-	// of group g runs on `adam_stream` as soon as every rank's records of group g have landed, under the push backward of group g + 1
-	int groups = 1, chunks_per_group = 0;
-	cudaStream_t adam_stream = nullptr;
 };
 
 namespace {
@@ -316,25 +353,12 @@ int psb_dp_create(psb_dp** out, int rank, int world, int P)
 	d->nlocal_max = (d->nchunks + world - 1) / world;
 	d->nlocal = d->nchunks > rank ? (d->nchunks - rank + world - 1) / world : 0;
 	dp_layout(d);
-	{
-		const char* g = getenv("PSB_DP_GROUPS");
-		// default 1 (no pipelining): the owner-side Adam of group g and the push backward of group g + 1 compete for the same store
-		// path, and the smaller launches lose their tails. Kept selectable for other fabrics.
-		int G = g ? atoi(g) : 1;
-		G = G < 1 ? 1 : (G > 8 ? 8 : G);
-		int cpg = (d->nchunks + G - 1) / G;
-		cpg = (cpg + world - 1) / world * world;          // a group holds whole rounds of the chunk -> owner rotation
-		if (cpg < world) cpg = world;
-		d->chunks_per_group = cpg;
-		d->groups = d->nchunks > 0 ? (d->nchunks + cpg - 1) / cpg : 1;
-	}
 	cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&d->base), d->bytes);
 	if (e == cudaSuccess) e = cudaMemset(d->base, 0, d->bytes);
 	if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&d->g_rest), ((size_t)d->nlocal_max * 128 * 45 + 64) * sizeof(float));
 	if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&d->status), sizeof(uint32_t));
 	if (e == cudaSuccess) e = cudaMemset(d->status, 0, sizeof(uint32_t));
 	if (e == cudaSuccess && world > 1) e = cudaIpcGetMemHandle(&d->handle, d->base);
-	if (e == cudaSuccess && d->groups > 1) e = cudaStreamCreateWithFlags(&d->adam_stream, cudaStreamNonBlocking);
 	if (e != cudaSuccess) {
 		set_error("psb_dp_create", e, __FILE__, __LINE__);
 		cudaFree(d->base); cudaFree(d->g_rest); cudaFree(d->status);
@@ -385,7 +409,6 @@ int psb_dp_destroy(psb_dp* d)
 	for (int j = 0; j < d->world; j++)
 		if (j != d->rank && d->peer[j]) cudaIpcCloseMemHandle(d->peer[j]);
 	cudaFree(d->base); cudaFree(d->g_rest); cudaFree(d->status);
-	if (d->adam_stream) cudaStreamDestroy(d->adam_stream);
 	delete d;
 	return 0;
 }
@@ -395,8 +418,8 @@ int psb_dp_destroy(psb_dp* d)
 int psb_dp_sync(psb_dp* d, void* stream_)
 {
 	if (!d) { set_error_msg("psb_dp_sync: null"); return PSB_ERR_ARG; }
-	if (d->epoch == 0 || d->P == 0 || (d->world == 1 && d->groups == 1)) return 0;   // (one rank, one group: everything is on the caller's stream)
-	return launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_pflag), d->groups * d->world, d->epoch, d->status, (cudaStream_t)stream_);
+	if (d->epoch == 0 || d->P == 0 || d->world == 1) return 0;   // (one rank: everything is on the caller's stream)
+	return launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_pflag), d->world, d->epoch, d->status, (cudaStream_t)stream_);
 }
 
 // 0 = healthy, 1 = a cross-rank wait timed out (a peer never arrived); synchronises the stream
@@ -426,21 +449,14 @@ int psb_dp_step_depth(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* 
 	const uint32_t epoch = ++d->epoch;
 	t->mark(psb_trainer::NSTAGE, stream);
 	// every rank's updated rows of the previous step must have landed here before this step reads the parameters
-	if (epoch > 1 && P > 0 && (d->world > 1 || d->groups > 1))   // (also orders this step behind the previous step's work on the adam stream)
-		if ((rc = launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_pflag), d->groups * d->world, epoch - 1, d->status, stream))) return rc;
+	if (epoch > 1 && P > 0 && d->world > 1)
+		if ((rc = launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_pflag), d->world, epoch - 1, d->status, stream))) return rc;
 	// render, loss, tile backward (the 9 screen-space sums per Gaussian; with a depth term also dL/dz in slot 11, which the push
 	// backward below must consume: a plain push backward would leave it in the sink for the next depth step)
-	if ((rc = step_impl(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, nullptr, stream, /*tiles_only=*/true, depth))) return rc;
-	if (P == 0) return 0;
-	const bool depth_loss = depth && depth->gt_depth;
-	char* gc = t->geom_chunk;
-	GeomState geom = GeomState::from_chunk(gc, (size_t)P);
-	const Camera cam = to_camera(camera);
-	TrainTensors tt;
-	for (int i = 0; i < 6; i++) { tt.p[i] = model->param[i]; tt.m[i] = model->exp_avg[i]; tt.v[i] = model->exp_avg_sq[i]; }
-	DensifyStats st;
-	st.enabled = (step->update_densify_stats && model->max_radii2D && model->xyz_gradient_accum && model->denom) ? 1 : 0;
-	st.max_radii2D = model->max_radii2D; st.xyz_gradient_accum = model->xyz_gradient_accum; st.denom = model->denom;
+	TileBackward tb;
+	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, stream, tb)) || P == 0)
+		return rc;
+	const TrainTensors tt = train_tensors(model, true);
 	const StepHyper h = to_hyper(step);
 	DpPush push;
 	memset(&push, 0, sizeof(push));
@@ -457,33 +473,18 @@ int psb_dp_step_depth(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* 
 	sh.inbox = reinterpret_cast<const float*>(d->base + d->off_inbox);
 	sh.meta = reinterpret_cast<const float*>(d->base + d->off_meta);
 	sh.g_rest = d->g_rest;
-	sh.world = d->world; sh.rank = d->rank; sh.nlocal_max = d->nlocal_max; sh.P = P; sh.epoch = epoch;
-	// Pipeline over groups of chunks: [main stream] push backward of group g (records go straight into the owners' inboxes) + signal;
-	// [adam stream] wait until every rank's records of group g have landed -> Adam of the owned rows of group g, updated rows stored to
-	// every replica + signal. With one group everything stays on the main stream. Flag word of (group g, rank r) = g * world + r.
-	cudaStream_t as = d->groups > 1 ? d->adam_stream : stream;
-	const int rows_per_group = d->chunks_per_group * 128;
-	for (int g = 0; g < d->groups; g++) {
-		DpPush pg = push;
-		for (int j = 0; j < d->world; j++) pg.grad_flag[j] = push.grad_flag[j] + g * d->world;
-		const int first = g * rows_per_group, last = (g + 1) * rows_per_group < P ? (g + 1) * rows_per_group : P;
-		if ((rc = launch_push_backward(first, last, tt, cam, geom, t->sink, h, st, geom.counters, (uint32_t)t->capacity, pg, stream, depth_loss))) return rc;
-	}
+	sh.world = d->world; sh.rank = d->rank; sh.nlocal_max = d->nlocal_max; sh.nlocal = d->nlocal; sh.P = P; sh.epoch = epoch;
+	// push backward (records go straight into the owners' inboxes) + signal; wait until every rank's records have landed -> Adam of
+	// the owned rows, updated rows stored to every replica + signal
+	if ((rc = launch_push_backward(P, tt, tb.cam, tb.geom, t->sink, h, densify_stats(model, step), tb.geom.counters, (uint32_t)t->capacity, push, stream,
+	                               tb.depth)))
+		return rc;
 	t->mark(7, stream);
 	t->mark(8, stream);
-	for (int g = 0; g < d->groups; g++) {
-		if ((rc = launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_gflag) + g * d->world, d->world, epoch, d->status, as))) return rc;
-		DpShard sg = sh;
-		for (int j = 0; j < d->world; j++) sg.param_flag[j] = sh.param_flag[j] + g * d->world;
-		sg.lc_first = g * (d->chunks_per_group / d->world);
-		const int lc_end = (g + 1) * (d->chunks_per_group / d->world) < d->nlocal ? (g + 1) * (d->chunks_per_group / d->world) : d->nlocal;
-		sg.nlocal = lc_end > sg.lc_first ? lc_end - sg.lc_first : 0;
-		if ((rc = launch_shard_adam(sg, tt, h, 1.0f / (float)d->world, as, (t->profiling && t->ev_ready && g == d->groups - 1) ? t->ev[10] : nullptr))) return rc;
-	}
-	t->mark(9, as);
-	t->last_stage = 9;
-	t->ev_recorded = t->profiling && t->ev_ready;
-	return rc;
+	if ((rc = launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_gflag), d->world, epoch, d->status, stream))) return rc;
+	if ((rc = launch_shard_adam(sh, tt, h, 1.0f / (float)d->world, stream, t->event(10)))) return rc;
+	t->end_stages(9, stream);
+	return 0;
 }
 
 int psb_dp_step(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
@@ -518,9 +519,10 @@ int psb_trainer_render(psb_trainer* t, int P, int M, const psb_model* model, con
 	int rc;
 	if (!t || !camera || !background || !out_color) { set_error_msg("psb_trainer_render: null argument"); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, false))) return rc;
-	GeomState geom; BinState bin; ImgState img; Camera cam;
+	Scratch sc;
+	Camera cam;
 	t->have_loss = false;
-	return forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, geom, bin, img, cam, (cudaStream_t)stream_);
+	return forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, sc, cam, (cudaStream_t)stream_);
 }
 
 int psb_trainer_render_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
@@ -529,24 +531,32 @@ int psb_trainer_render_depth(psb_trainer* t, int P, int M, const psb_model* mode
 	int rc;
 	if (!t || !camera || !background || !out_color) { set_error_msg("psb_trainer_render_depth: null argument"); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, false))) return rc;
-	GeomState geom; BinState bin; ImgState img; Camera cam;
+	Scratch sc;
+	Camera cam;
 	t->have_loss = false;
-	return forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, geom, bin, img, cam, (cudaStream_t)stream_, out_depth);
+	return forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, sc, cam, (cudaStream_t)stream_, out_depth);
 }
 
 int psb_trainer_step(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                      const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, void* stream_)
 {
-	return step_impl(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, nullptr, (cudaStream_t)stream_);
+	return psb_trainer_step_depth(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, nullptr, stream_);
 }
 
 int psb_trainer_step_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                            const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
                            void* stream_)
 {
+	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
 	if ((rc = check_depth(depth, "psb_trainer_step_depth"))) return rc;
-	return step_impl(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, nullptr, (cudaStream_t)stream_, false, depth);
+	TileBackward tb;
+	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, true, stream, tb)) || P == 0)
+		return rc;
+	rc = launch_fused_backward(true, 0, P, train_tensors(model, true), tb.cam, tb.geom, t->sink, t->seeds, to_hyper(step), GradSegments{},
+	                           densify_stats(model, step), tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), model->adam_live, tb.depth);
+	t->end_stages(8, stream);
+	return rc;
 }
 
 int psb_adam_live_rebuild(int P, const psb_model* model, void* stream_)
@@ -554,24 +564,26 @@ int psb_adam_live_rebuild(int P, const psb_model* model, void* stream_)
 	int rc;
 	if ((rc = check_model(P, 16, model, true))) return rc;
 	if (P > 0 && !model->adam_live) { set_error_msg("psb_adam_live_rebuild: model->adam_live is NULL"); return PSB_ERR_ARG; }
-	TrainTensors tt;
-	for (int i = 0; i < 6; i++) { tt.p[i] = model->param[i]; tt.m[i] = model->exp_avg[i]; tt.v[i] = model->exp_avg_sq[i]; }
-	return launch_adam_live_rebuild(P, tt, model->adam_live, (cudaStream_t)stream_);
+	return launch_adam_live_rebuild(P, train_tensors(model, true), model->adam_live, (cudaStream_t)stream_);
 }
 
 int psb_trainer_backward_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                                const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, float* const* grads,
                                const psb_depth* depth, void* stream_)
 {
+	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
 	if ((rc = check_depth(depth, "psb_trainer_backward_depth"))) return rc;
-	if (!grads) { set_error_msg("psb_trainer_backward: grads required"); return PSB_ERR_ARG; }
-	for (int i = 0; i < 6; i++) if (P > 0 && !grads[i]) { set_error_msg("psb_trainer_backward: null gradient segment"); return PSB_ERR_ARG; }
-	if (P > 0 && ((reinterpret_cast<uintptr_t>(grads[2]) | reinterpret_cast<uintptr_t>(grads[5])) & 15)) {
-		set_error_msg("psb_trainer_backward: the features_rest and rotation gradient segments must be 16-byte aligned");
-		return PSB_ERR_ARG;
-	}
-	return step_impl(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, grads, (cudaStream_t)stream_, false, depth);
+	if ((rc = check_grads(grads, P, "psb_trainer_backward"))) return rc;
+	TileBackward tb;
+	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, stream, tb)) || P == 0)
+		return rc;
+	GradSegments gs;
+	for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
+	rc = launch_fused_backward(false, 0, P, train_tensors(model, false), tb.cam, tb.geom, t->sink, t->seeds, to_hyper(step), gs, densify_stats(model, step),
+	                           tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), nullptr, tb.depth);
+	t->end_stages(8, stream);
+	return rc;
 }
 
 int psb_trainer_backward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
@@ -589,8 +601,8 @@ int psb_trainer_backward_begin_depth(psb_trainer* t, int P, int M, const psb_mod
 	if ((rc = check_depth(depth, "psb_trainer_backward_begin_depth"))) return rc;
 	// set whether or not the call below succeeds: the depth variant of _slab gives the plain result on rows without dL/dz
 	if (t) t->slab_depth = depth && depth->gt_depth;
-	return step_impl(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, nullptr, (cudaStream_t)stream_, /*tiles_only=*/true,
-	                 depth);
+	TileBackward tb;
+	return render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, (cudaStream_t)stream_, tb);
 }
 
 int psb_trainer_backward_begin(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
@@ -607,23 +619,12 @@ int psb_trainer_backward_slab(psb_trainer* t, int P, int M, const psb_model* mod
 	if ((rc = check_model(P, M, model, false))) return rc;
 	if (first < 0 || count < 0 || first + count > P || (first % 128) != 0) { set_error_msg("psb_trainer_backward_slab: slab must start at a multiple of 128"); return PSB_ERR_ARG; }
 	if (count == 0) return 0;
-	if ((reinterpret_cast<uintptr_t>(grads[2]) | reinterpret_cast<uintptr_t>(grads[5])) & 15) {
-		set_error_msg("psb_trainer_backward_slab: the features_rest and rotation gradient blocks must be 16-byte aligned");
-		return PSB_ERR_ARG;
-	}
-	char* gc = t->geom_chunk;
-	GeomState geom = GeomState::from_chunk(gc, (size_t)P);
-	const Camera cam = to_camera(camera);
-	TrainTensors tt;
-	for (int i = 0; i < 6; i++) { tt.p[i] = model->param[i]; tt.m[i] = nullptr; tt.v[i] = nullptr; }
+	if ((rc = check_grads(grads, count, "psb_trainer_backward_slab"))) return rc;
+	const GeomState geom = carve_scratch(t, P, t->last_W, t->last_H).geom;
 	GradSegments gs;
 	for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
-	DensifyStats st;
-	st.enabled = (step->update_densify_stats && model->max_radii2D && model->xyz_gradient_accum && model->denom) ? 1 : 0;
-	st.max_radii2D = model->max_radii2D; st.xyz_gradient_accum = model->xyz_gradient_accum; st.denom = model->denom;
-	const StepHyper h = to_hyper(step);
-	return launch_fused_backward(false, first, first + count, tt, cam, geom, t->sink, t->seeds, h, gs, st, geom.counters, (uint32_t)t->capacity, (cudaStream_t)stream_,
-	                             nullptr, nullptr, t->slab_depth);
+	return launch_fused_backward(false, first, first + count, train_tensors(model, false), to_camera(camera), geom, t->sink, t->seeds, to_hyper(step), gs,
+	                             densify_stats(model, step), geom.counters, (uint32_t)t->capacity, (cudaStream_t)stream_, nullptr, nullptr, t->slab_depth);
 }
 
 int psb_adam_update(int P, int M, const psb_model* model, float* const* grads, const psb_step* step, float grad_scale, void* stream_)
@@ -720,16 +721,13 @@ int psb_trainer_debug_state(psb_trainer* t, int width, int height, int* last_gau
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
 	if (!t || t->geom_P < 0 || t->last_W != width || t->last_H != height) { set_error_msg("psb_trainer_debug_state: no step of that size has run"); return PSB_ERR_ARG; }
-	char* gc = t->geom_chunk; GeomState geom = GeomState::from_chunk(gc, (size_t)t->geom_P);
-	char* ic = t->img_chunk; ImgState img = ImgState::from_chunk(ic, (size_t)width * height);
-	char* bc = t->bin_chunk; BinState bin = BinState::from_chunk(bc, t->capacity);
-	const int grid_x = (width + PSB_TILE_X - 1) / PSB_TILE_X, grid_y = (height + PSB_TILE_Y - 1) / PSB_TILE_Y;
-	const int res = make_sort_plan(tile_id_bits(grid_x * grid_y)).npass & 1;
-	export_last_splat_kernel<<<(width * height + 255) / 256, 256, 0, stream>>>(width, height, grid_x, img.ranges, bin.inst[res], img.n_contrib, img.final_T,
+	const Scratch sc = carve_scratch(t, t->geom_P, width, height);
+	export_last_splat_kernel<<<(width * height + 255) / 256, 256, 0, stream>>>(width, height, tile_grid(width, height).x, sc.img.ranges,
+	                                                                        sc.bin.inst[sorted_slot(width, height)], sc.img.n_contrib, sc.img.final_T,
 	                                                                        last_gauss, final_T);
 	PSB_LAUNCH_OK();
 	if (num_rendered) {
-		PSB_CUDA_OK(cudaMemcpyAsync(num_rendered, geom.counters, sizeof(int), cudaMemcpyDeviceToHost, stream));
+		PSB_CUDA_OK(cudaMemcpyAsync(num_rendered, sc.geom.counters, sizeof(int), cudaMemcpyDeviceToHost, stream));
 		PSB_CUDA_OK(cudaStreamSynchronize(stream));
 	}
 	return 0;

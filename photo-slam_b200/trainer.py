@@ -757,8 +757,8 @@ class DataParallelTrainer(GaussianTrainer):
         return self.L.psb_dp_status(self.dp, torch.cuda.current_stream().cuda_stream) if self.mode == "p2p" else 0
 
     def render(self, cam, out=None, radii=None, check=True, out_depth=None):
-        """Forward only, on the complete replica: the owner-side Adam of the last step runs on the context's own stream and the peers
-        store their rows asynchronously, so the render is ordered behind both (device-side wait)."""
+        """Forward only, on the complete replica: the peers store their rows of the last step asynchronously, so the render is
+        ordered behind every rank's rows (device-side wait)."""
         self.sync()
         return super().render(cam, out, radii, check, out_depth)
 

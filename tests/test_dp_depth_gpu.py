@@ -139,26 +139,6 @@ def test_plain_steps_between_depth_steps_leave_no_stale_depth_gradient(cuda, kw)
     tb.close()
 
 
-def test_p2p_depth_step_with_three_pipeline_groups_equals_one_group(cuda, monkeypatch):
-    from photo_slam_b200 import trainer
-    sc, c, gt, gd = _inputs(cuda, 20_000)
-    a, b = _model(sc, cuda), _model(sc, cuda)
-    monkeypatch.setenv("PSB_DP_GROUPS", "1")
-    ta = trainer.DataParallelTrainer(a, mode="p2p")
-    monkeypatch.setenv("PSB_DP_GROUPS", "3")
-    tb = trainer.DataParallelTrainer(b, mode="p2p")
-    for it in range(4):
-        ta.trainForOneIteration(c, gt, gt_depth=gd, lambda_depth=LAMBDA_DEPTH)
-        tb.trainForOneIteration(c, gt, gt_depth=gd, lambda_depth=LAMBDA_DEPTH)
-        _assert_same_result(ta.result_depth(), tb.result_depth(), it)
-    _finish(ta)
-    _finish(tb)
-    assert ta.status() == 0 and tb.status() == 0
-    _assert_same_state(a, b)
-    ta.close()
-    tb.close()
-
-
 def test_p2p_depth_only_rows_are_updated_like_the_fused_step(cuda):
     """Every colour target equals the render and lambda_dssim = 0: only dL/dz reaches the rows, and the records carry it."""
     from photo_slam_b200 import trainer
