@@ -331,6 +331,17 @@ int psb_trainer_debug_state(psb_trainer* t, int width, int height, int* last_gau
 int psb_trainer_set_profiling(psb_trainer* t, int enable);
 int psb_trainer_stage_times(psb_trainer* t, float* ms, int n);
 
+/* Deterministic mode of a context (off by default; PSB_ERR_ARG for a NULL context). While it is on, every output of these calls
+ * is bit-identical from run to run for the same inputs, the same build and the same GPU model: psb_trainer_step(_depth),
+ * psb_trainer_backward(_depth), psb_trainer_backward_begin(_depth) + psb_trainer_backward_slab, psb_dp_step(_depth) at any
+ * world size, and the scalars of psb_trainer_result(_depth). The tile backward then stores each (Gaussian, tile) sum in a slot
+ * of its own and a gather adds every Gaussian's slots in a fixed order, instead of adding them into the Gaussian's row with
+ * float atomics in whatever order the tiles finish; the loss sums are reduced in a fixed order too. It costs a slot buffer of
+ * 48 B per instance of the binning capacity (grown with it) and the time of the gather, counted in the "render backward" stage.
+ * Not covered: the B1/B2 operator path (psb_rasterize_backward*), and the NCCL all-reduce that a caller runs between
+ * psb_trainer_backward* and psb_adam_update: each rank's gradients are deterministic, the all-reduce's order is NCCL's. */
+int psb_trainer_set_deterministic(psb_trainer* t, int enable);
+
 /* Stand-alone fused loss (tests / evaluation): L = (1-lambda) L1 + lambda (1 - SSIM), reference
  * include/loss_utils.h:28-124. image/gt/mask/dL_dimage device [3,H,W] (mask, dL_dimage may be NULL);
  * out3_host = {loss, l1, ssim}. Synchronises the stream. */

@@ -249,6 +249,28 @@ constexpr uint32_t TT_VISIBLE = 0x80000000u;  // tight lists: tiles_touched = ex
 constexpr uint32_t TT_COUNT = 0x7FFFFFFFu;
 constexpr int TIGHT_MAX_AREA = 32;             // larger rectangles keep every tile (one 32-bit mask per Gaussian, bounded loop)
 
+// The instances of one Gaussian (tile_info = GeomState::tile_info[g], tt = its instance count): the tiles of its rectangle,
+// row-major, and on a tight list over at most TIGHT_MAX_AREA tiles only those of the mask. emit_warp emits them in this order and
+// the deterministic tile backward stores the flush of (Gaussian, tile) at the same rank, so both take the order from here.
+struct InstRect {
+	uint32_t x0, y0, w, mask;
+	bool masked;
+	__device__ __forceinline__ InstRect(const uint4 info, bool tight, uint32_t tt)
+	{
+		x0 = info.x & 0xFFFFu;
+		y0 = info.x >> 16;
+		w = max((info.y & 0xFFFFu) - x0, 1u);
+		masked = tight && tt > 0 && w * ((info.y >> 16) - y0) <= (uint32_t)TIGHT_MAX_AREA;
+		mask = masked ? info.w : 0xffffffffu;
+	}
+	// rank among the Gaussian's instances of tile a (row-major in the rectangle), which must be one of its instances
+	static __device__ __forceinline__ uint32_t rank(bool masked, uint32_t mask, uint32_t a)
+	{
+		return masked ? (uint32_t)__popc(mask & ((1u << a) - 1u)) : a;
+	}
+	__device__ __forceinline__ uint32_t rank_of(uint32_t tx, uint32_t ty) const { return rank(masked, mask, (ty - y0) * w + (tx - x0)); }
+};
+
 // ---- async-copy / mbarrier PTX wrappers (TMA 1-D bulk copies) ----
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 

@@ -289,15 +289,14 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_offsets_kernel(int P, const
 template <bool TIGHT, typename Put>
 __device__ __forceinline__ void emit_warp(uint32_t g, uint32_t tt, uint32_t off, const uint4 info, int grid_x, int lane, Put put)
 {
-	const uint32_t x0 = info.x & 0xFFFFu, y0 = info.x >> 16;
-	const uint32_t w = max((info.y & 0xFFFFu) - x0, 1u);
-	const bool masked = TIGHT && tt > 0 && w * ((info.y >> 16) - y0) <= (uint32_t)TIGHT_MAX_AREA;
-	const uint32_t mask = masked ? info.w : 0xffffffffu;
+	const InstRect r(info, TIGHT, tt);
+	const uint32_t x0 = r.x0, y0 = r.y0, w = r.w, mask = r.mask;
+	const bool masked = r.masked;
 	constexpr uint32_t SMALL = 6;
 	if (tt > 0 && tt <= SMALL) {
 		if (masked) {
 			uint32_t m = mask;
-			for (uint32_t k = 0; k < tt; k++) {
+			for (uint32_t k = 0; k < tt; k++) {  // the k-th set bit of the mask has rank k
 				const uint32_t a = (uint32_t)__ffs(m) - 1u;
 				m &= m - 1u;
 				put(off + k, (y0 + a / w) * grid_x + x0 + a % w, g);
@@ -323,7 +322,7 @@ __device__ __forceinline__ void emit_warp(uint32_t g, uint32_t tt, uint32_t off,
 		const uint32_t bmask = __shfl_sync(0xffffffffu, mask, src);
 		const bool bmasked = __shfl_sync(0xffffffffu, (int)masked, src) != 0;
 		if (bmasked) {  // masked rectangle (<= 32 tiles): lane k owns tile k
-			if ((bmask >> lane) & 1u) put(boff + __popc(bmask & ((1u << lane) - 1u)), (by0 + lane / bw) * grid_x + bx0 + lane % bw, bg);
+			if ((bmask >> lane) & 1u) put(boff + InstRect::rank(true, bmask, lane), (by0 + lane / bw) * grid_x + bx0 + lane % bw, bg);
 			continue;
 		}
 		for (uint32_t k = lane; k < btt; k += 32) put(boff + k, (by0 + k / bw) * grid_x + bx0 + k % bw, bg);
@@ -354,12 +353,14 @@ __global__ void __launch_bounds__(256) emit_instances_kernel(int P, const uint32
 // their block-local offsets (which need no look-back: warp 0 resolves the block's global prefix meanwhile) and leave as
 // one contiguous, coalesced run. counters[0] <- total instance count; instances beyond `capacity` are not written (the
 // step then degrades to a no-op, see psb_trainer.cu).
+// DET (deterministic mode): also base[g] <- emission offset of every Gaussian with instances (its first instance's index).
 constexpr int EM_THREADS = 256, EM_ITEMS = 4, EM_TILE = EM_THREADS * EM_ITEMS;
 constexpr int EM_STAGE = 5120;  // instances staged per block (40 KB); a block with more writes to global memory directly
-template <bool TIGHT>
+template <bool TIGHT, bool DET = false>
 __global__ void __launch_bounds__(EM_THREADS) emit_scan_kernel(int P, const uint32_t* __restrict__ order, const uint4* __restrict__ tile_info,
                                                                uint32_t* __restrict__ tile_key, uint32_t* __restrict__ inst, int grid_x,
-                                                               uint32_t capacity, uint32_t* __restrict__ counters, uint32_t* __restrict__ status)
+                                                               uint32_t capacity, uint32_t* __restrict__ counters, uint32_t* __restrict__ status,
+                                                               uint32_t* __restrict__ base_out = nullptr)
 {
 	__shared__ uint32_t s_key[EM_STAGE], s_ins[EM_STAGE];
 	__shared__ uint32_t s_warp[EM_THREADS / 32];
@@ -419,9 +420,21 @@ __global__ void __launch_bounds__(EM_THREADS) emit_scan_kernel(int P, const uint
 			});
 		run += cnt[i];
 	}
-	if (!staged) return;
+	auto write_base = [&](uint32_t prefix) {
+		uint32_t o = prefix + wb + inc - sum;
+#pragma unroll
+		for (int i = 0; i < EM_ITEMS; i++) {
+			if (cnt[i] > 0) base_out[g[i]] = o;
+			o += cnt[i];
+		}
+	};
+	if (!staged) {
+		if (DET) write_base(s_prefix);
+		return;
+	}
 	__syncthreads();
 	const uint32_t prefix = s_prefix;
+	if (DET) write_base(prefix);
 	for (uint32_t k = tid; k < block_total; k += EM_THREADS) {
 		const uint32_t pos = prefix + k;
 		if (pos < capacity) { tile_key[pos] = s_key[k]; inst[pos] = s_ins[k]; }
@@ -520,13 +533,20 @@ int launch_binning(int P, const Camera& cam, const GeomState& geom, BinState& bi
 // Trainer path: scan + emit in one kernel, tile sort, ranges. The instance count stays on the device
 // (geom.counters[0]); `capacity` = size the binning chunk was carved for.
 int launch_scan_binning(int P, const Camera& cam, const GeomState& geom, BinState& bin, const ImgState& img, size_t capacity, bool tight,
-                        uint32_t* ovf, uint32_t seq, cudaStream_t stream)
+                        uint32_t* ovf, uint32_t seq, cudaStream_t stream, uint32_t* base)
 {
 	const int num_tiles = cam.grid_x * cam.grid_y;
 	PSB_CUDA_OK(cudaMemsetAsync(img.ranges, 0, (size_t)num_tiles * sizeof(uint2), stream));
 	if (P == 0 || capacity == 0) return 0;
 	const SortPlan plan = make_sort_plan(tile_id_bits(num_tiles));
-	if (tight)
+	if (base) {
+		if (tight)
+			emit_scan_kernel<true, true><<<cdiv(P, EM_TILE), EM_THREADS, 0, stream>>>(P, geom.order[0], geom.tile_info, bin.tile_key[0], bin.inst[0], cam.grid_x,
+			                                                                        (uint32_t)capacity, geom.counters, geom.scan_status, base);
+		else
+			emit_scan_kernel<false, true><<<cdiv(P, EM_TILE), EM_THREADS, 0, stream>>>(P, geom.order[0], geom.tile_info, bin.tile_key[0], bin.inst[0], cam.grid_x,
+			                                                                         (uint32_t)capacity, geom.counters, geom.scan_status, base);
+	} else if (tight)
 		emit_scan_kernel<true><<<cdiv(P, EM_TILE), EM_THREADS, 0, stream>>>(P, geom.order[0], geom.tile_info, bin.tile_key[0], bin.inst[0], cam.grid_x,
 		                                                                  (uint32_t)capacity, geom.counters, geom.scan_status);
 	else

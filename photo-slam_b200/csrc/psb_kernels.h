@@ -33,6 +33,20 @@ struct GradSink {
 	float* z = nullptr; int z_stride = 0;  // unpacked sink with a depth gradient: the tenth sum, dL/dz (the packed row keeps it in slot 11)
 };
 
+// Deterministic mode of the trainer's tile backward (packed sink only). Float atomics from tiles that finish in any order would
+// sum a Gaussian's (Gaussian, tile) flushes in a different order every run; instead each flush is STORED in the slot of its
+// instance's emission index, base[g] + (rank of the tile among g's instances, InstRect), and gather_slots_kernel then sums every
+// Gaussian's slots in emission order and writes its sink row. A slot counts only when tagged with this pass's `seq`: entries the
+// tile backward does not flush (behind a tile's deepest contributor, culled by the reach tests) keep an older tag and read as zero.
+struct DetSlots {
+	float4* slots;              // [capacity][3]: one packed sink row per instance; lane 2 (padding) = seq of the pass that wrote it
+	const uint32_t* base;       // [P] emission offset of each Gaussian with instances (emit_scan_kernel, DET)
+	const uint4* tile_info;     // GeomState::tile_info
+	const uint32_t* counters;   // GeomState::counters: an overflowing pass (counters[0] > capacity) gathers nothing
+	uint32_t capacity, seq;
+	int P, tight;
+};
+
 // Outputs of the per-Gaussian backward (any pointer may be null = not wanted).
 struct GaussGradOut {
 	float* dL_dmeans3D;  // [P,3]
@@ -71,16 +85,18 @@ int launch_preprocess(const GaussIn& in, const Camera& cam, int* radii_out, cons
 int launch_mark_visible(int P, const float* means3D, const float* view, uint8_t* present, cudaStream_t stream);
 int launch_depth_sort_and_scan(int P, GeomState& geom, bool scan, cudaStream_t stream);
 int launch_binning(int P, const Camera& cam, const GeomState& geom, BinState& bin, const ImgState& img, size_t n_host, cudaStream_t stream);
+// base != null (deterministic mode): base[g] <- emission offset of every Gaussian with instances (DetSlots::base)
 int launch_scan_binning(int P, const Camera& cam, const GeomState& geom, BinState& bin, const ImgState& img, size_t capacity, bool tight,
-                        uint32_t* ovf, uint32_t seq, cudaStream_t stream);
+                        uint32_t* ovf, uint32_t seq, cudaStream_t stream, uint32_t* base = nullptr);
 int launch_render_forward(const Camera& cam, const uint2* ranges, const uint32_t* point_list, const GaussRec* rec, const float* bg,
                           float* out_color, float* final_T, uint32_t* n_contrib, cudaStream_t stream,
                           float* out_depth = nullptr /* [H,W]: also render the expected depth (depth variant of the kernel) */);
 // dL_ddepth [H,W]: depth variant, dL/dz of every Gaussian lands in slot 11 of its packed sink row, or at sink.z (unpacked sink;
-// refused without either destination)
+// refused without either destination). det != null (packed sink only): the deterministic variant — slot stores, then the ordered gather
+// into the sink rows
 int launch_render_backward(const Camera& cam, const uint2* ranges, const uint32_t* point_list, const GaussRec* rec, const float* bg,
                            const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, const GradSink& sink,
-                           cudaStream_t stream, const float* dL_ddepth = nullptr);
+                           cudaStream_t stream, const float* dL_ddepth = nullptr, const DetSlots* det = nullptr);
 // dL_dz [P] (non-null: depth variant): dL/dmean3D += dL/dz (V[2], V[6], V[10]) for every visible Gaussian
 int launch_preprocess_backward(const GaussIn& in, const Camera& cam, const GeomState& geom, const float* dL_dmean2D, int mean2D_stride,
                                const float* dL_dconic, int conic_stride, const float* dL_dcolor, int color_stride,

@@ -33,10 +33,27 @@ __device__ __forceinline__ float block_sum_256(float v, float* s_red)
 	return t;
 }
 
+// The two block sums of a block: added to sums[0..1] (double atomics, in whatever order the blocks finish) or, DET, stored as the
+// block's partials at sums[2 * block ..] for reduce_partials_kernel.
+template <bool DET>
+__device__ __forceinline__ void block_sums_out(float a, float b, double* __restrict__ sums)
+{
+	if (threadIdx.x != 0) return;
+	if (DET) {
+		const size_t blk = ((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+		sums[2 * blk] = (double)a;
+		sums[2 * blk + 1] = (double)b;
+	} else {
+		atomicAdd(&sums[0], (double)a);
+		atomicAdd(&sums[1], (double)b);
+	}
+}
+
 // grid (tiles_x, tiles_y, 3), block 256 (16x16).
-__global__ void __launch_bounds__(256) loss_fwd_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
-                                                       const float* __restrict__ mask, Win win, float g_ssim,
-                                                       float* __restrict__ dmap /* [3 maps][3][H][W] */, double* __restrict__ sums /* [2] */)
+template <bool DET>
+__device__ __forceinline__ void loss_fwd_body(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
+                                              const float* __restrict__ mask, const Win& win, float g_ssim,
+                                              float* __restrict__ dmap /* [3 maps][3][H][W] */, double* __restrict__ sums /* [2] | DET: [blocks][2] */)
 {
 	__shared__ float s_x[LS][LS + 1], s_y[LS][LS + 1];
 	__shared__ float s_h[5][LS][LT + 1];
@@ -100,7 +117,39 @@ __global__ void __launch_bounds__(256) loss_fwd_kernel(int H, int W, const float
 	}
 	const float tl1 = block_sum_256(l1, s_red);
 	const float tss = block_sum_256(ss, s_red);
-	if (tid == 0) { atomicAdd(&sums[0], (double)tl1); atomicAdd(&sums[1], (double)tss); }
+	block_sums_out<DET>(tl1, tss, sums);
+}
+
+__global__ void __launch_bounds__(256) loss_fwd_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
+                                                       const float* __restrict__ mask, Win win, float g_ssim, float* __restrict__ dmap,
+                                                       double* __restrict__ sums)
+{
+	loss_fwd_body<false>(H, W, img, gt, mask, win, g_ssim, dmap, sums);
+}
+
+__global__ void __launch_bounds__(256) loss_fwd_det_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
+                                                           const float* __restrict__ mask, Win win, float g_ssim, float* __restrict__ dmap,
+                                                           double* __restrict__ partials)
+{
+	loss_fwd_body<true>(H, W, img, gt, mask, win, g_ssim, dmap, partials);
+}
+
+// Deterministic mode: sums[c] = the n block partials partials[2 b + c] (c = 0, 1) added in a fixed order (one block: strided
+// per-thread sums, then a fixed tree), whatever order the blocks that wrote them ran in.
+__global__ void __launch_bounds__(256) reduce_partials_kernel(int n, const double* __restrict__ partials, double* __restrict__ sums)
+{
+	__shared__ double s[2][256];
+	const int tid = threadIdx.x;
+	double a = 0.0, b = 0.0;
+	for (int i = tid; i < n; i += 256) { a += partials[2 * i]; b += partials[2 * i + 1]; }
+	s[0][tid] = a;
+	s[1][tid] = b;
+	__syncthreads();
+	for (int o = 128; o > 0; o >>= 1) {
+		if (tid < o) { s[0][tid] += s[0][tid + o]; s[1][tid] += s[1][tid + o]; }
+		__syncthreads();
+	}
+	if (tid == 0) { sums[0] = s[0][0]; sums[1] = s[1][0]; }
 }
 
 __global__ void __launch_bounds__(256) loss_bwd_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
@@ -154,9 +203,10 @@ __global__ void __launch_bounds__(256) loss_bwd_kernel(int H, int W, const float
 }
 
 // Depth L1, pass 1 (grid-stride, 256 threads): per valid pixel |D - G| and sign(D - G) (-> dL_dD, scaled by pass 2); block sums of
-// |D - G| and of the valid count go to sums[0], sums[1] in double (the count is exact).
-__global__ void __launch_bounds__(256) depth_loss_kernel(int n, const float* __restrict__ D, const float* __restrict__ G, const float* __restrict__ mask,
-                                                         float* __restrict__ dL_dD, double* __restrict__ sums)
+// |D - G| and of the valid count go to sums[0], sums[1] in double (the count is exact); DET: to the block's partials.
+template <bool DET>
+__device__ __forceinline__ void depth_loss_body(int n, const float* __restrict__ D, const float* __restrict__ G, const float* __restrict__ mask,
+                                                float* __restrict__ dL_dD, double* __restrict__ sums)
 {
 	__shared__ float s_red[8];
 	float acc = 0.f, cnt = 0.f;
@@ -174,7 +224,19 @@ __global__ void __launch_bounds__(256) depth_loss_kernel(int n, const float* __r
 	}
 	const float tacc = block_sum_256(acc, s_red);
 	const float tcnt = block_sum_256(cnt, s_red);
-	if (threadIdx.x == 0) { atomicAdd(&sums[0], (double)tacc); atomicAdd(&sums[1], (double)tcnt); }
+	block_sums_out<DET>(tacc, tcnt, sums);
+}
+
+__global__ void __launch_bounds__(256) depth_loss_kernel(int n, const float* __restrict__ D, const float* __restrict__ G, const float* __restrict__ mask,
+                                                         float* __restrict__ dL_dD, double* __restrict__ sums)
+{
+	depth_loss_body<false>(n, D, G, mask, dL_dD, sums);
+}
+
+__global__ void __launch_bounds__(256) depth_loss_det_kernel(int n, const float* __restrict__ D, const float* __restrict__ G, const float* __restrict__ mask,
+                                                             float* __restrict__ dL_dD, double* __restrict__ partials)
+{
+	depth_loss_body<true>(n, D, G, mask, dL_dD, partials);
 }
 
 // Depth L1, pass 2: dL_dD *= lambda / max(N_valid, 1), N_valid read on the device (no host round trip).
@@ -187,12 +249,18 @@ __global__ void __launch_bounds__(256) depth_grad_scale_kernel(int n, float lamb
 }  // namespace
 
 int launch_depth_loss(int H, int W, const float* depth, const float* gt_depth, const float* mask, float lambda_depth, double* sums, float* dL_dD,
-                      cudaStream_t stream)
+                      cudaStream_t stream, double* partials)
 {
 	const int n = H * W;
-	const int grid = min(cdiv(n, 256), kNumSMs * 8);
-	PSB_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), stream));
-	depth_loss_kernel<<<grid, 256, 0, stream>>>(n, depth, gt_depth, mask, dL_dD, sums);
+	const int grid = depth_loss_blocks(H, W);
+	if (partials) {
+		depth_loss_det_kernel<<<grid, 256, 0, stream>>>(n, depth, gt_depth, mask, dL_dD, partials);
+		PSB_LAUNCH_OK();
+		reduce_partials_kernel<<<1, 256, 0, stream>>>(grid, partials, sums);
+	} else {
+		PSB_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), stream));
+		depth_loss_kernel<<<grid, 256, 0, stream>>>(n, depth, gt_depth, mask, dL_dD, sums);
+	}
 	PSB_LAUNCH_OK();
 	depth_grad_scale_kernel<<<grid, 256, 0, stream>>>(n, lambda_depth, sums, dL_dD);
 	PSB_LAUNCH_OK();
@@ -202,16 +270,22 @@ int launch_depth_loss(int H, int W, const float* depth, const float* gt_depth, c
 // sums: device double[2] (zeroed here); after the launch sums[0] = sum|I-G|, sums[1] = sum ssim_map.
 // dmap: device float[9*H*W] scratch. dL_dimg may be null (loss value only).
 int launch_loss(int H, int W, const float* img, const float* gt, const float* mask, float lambda_dssim, float* dmap, double* sums,
-                float* dL_dimg, cudaStream_t stream)
+                float* dL_dimg, cudaStream_t stream, double* partials)
 {
 	Win win;
 	float s = 0.f;
 	for (int x = 0; x < 11; x++) { const int t = x - 5; win.w[x] = expf(-(float)(t * t) / (2.0f * 1.5f * 1.5f)); s += win.w[x]; }
 	for (int x = 0; x < 11; x++) win.w[x] /= s;
 	const float inv_n = 1.0f / (3.0f * (float)H * (float)W);
-	PSB_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), stream));
 	dim3 grid((W + LT - 1) / LT, (H + LT - 1) / LT, 3);
-	loss_fwd_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, -lambda_dssim * inv_n, dmap, sums);
+	if (partials) {
+		loss_fwd_det_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, -lambda_dssim * inv_n, dmap, partials);
+		PSB_LAUNCH_OK();
+		reduce_partials_kernel<<<1, 256, 0, stream>>>((int)(grid.x * grid.y * grid.z), partials, sums);
+	} else {
+		PSB_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), stream));
+		loss_fwd_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, -lambda_dssim * inv_n, dmap, sums);
+	}
 	PSB_LAUNCH_OK();
 	if (dL_dimg) {
 		loss_bwd_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, (1.0f - lambda_dssim) * inv_n, dmap, dL_dimg);

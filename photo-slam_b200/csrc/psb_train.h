@@ -68,11 +68,21 @@ int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, co
 // adam_live[i] = any moment of row i non-zero (t.m / t.v: the 12 moment tensors)
 int launch_adam_live_rebuild(int P, const TrainTensors& t, unsigned char* adam_live, cudaStream_t stream);
 int launch_adam(size_t n, float* p, float* m, float* v, const float* g, float lr, const StepHyper& h, float grad_scale, cudaStream_t stream);
+// partials != null (deterministic mode): scratch of loss_partials_doubles(H, W); the blocks store their sums there and one more
+// launch adds them in a fixed order, so sums[] is the same every run (the default double atomics add in completion order)
 int launch_loss(int H, int W, const float* img, const float* gt, const float* mask, float lambda_dssim, float* dmap, double* sums,
-                float* dL_dimg, cudaStream_t stream);
+                float* dL_dimg, cudaStream_t stream, double* partials = nullptr);
 // Depth L1 over the valid pixels (gt > 0 and, with a mask, mask[0, p] != 0): sums[0] = sum |D - G|, sums[1] = N_valid (zeroed here);
 // dL_dD [H,W] = lambda * sign(D - G) / max(N_valid, 1) on valid pixels, 0 elsewhere. Two launches, no host synchronisation.
+// partials: as launch_loss.
 int launch_depth_loss(int H, int W, const float* depth, const float* gt_depth, const float* mask, float lambda_depth, double* sums, float* dL_dD,
-                      cudaStream_t stream);
+                      cudaStream_t stream, double* partials = nullptr);
+inline int depth_loss_blocks(int H, int W) { return min(cdiv(H * W, 256), kNumSMs * 8); }
+// launch_loss runs one block per 16 x 16 tile and channel
+inline size_t loss_partials_doubles(int H, int W)
+{
+	const int loss_blocks = 3 * cdiv(W, 16) * cdiv(H, 16);
+	return 2 * (size_t)(loss_blocks > depth_loss_blocks(H, W) ? loss_blocks : depth_loss_blocks(H, W));
+}
 
 }  // namespace psb

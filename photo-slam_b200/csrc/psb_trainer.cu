@@ -37,6 +37,13 @@ struct psb_trainer {
 	// tight instance lists: only the tiles a splat can reach get an instance (see preprocess_fwd_kernel); PSB_TIGHT=0 keeps the
 	// reference's full rectangles (A/B measurements only — images and gradients are the same either way)
 	bool tight = !(getenv("PSB_TIGHT") && atoi(getenv("PSB_TIGHT")) == 0);
+	// deterministic mode (psb_trainer_set_deterministic): its own scratch, made only while the mode is on and grown with the binning
+	// capacity — the instance slots [det_cap][12] floats (zeroed when allocated: every tag reads "not this pass"), the emission offsets
+	// [det_P] and the loss partials [det_parts] doubles
+	bool deterministic = false;
+	float* det_slots = nullptr; size_t det_cap = 0;
+	uint32_t* det_base = nullptr; size_t det_P = 0;
+	double* det_partials = nullptr; size_t det_parts = 0;
 	// optional per-stage timing (CUDA events on the step's stream)
 	bool profiling = false;
 	// stage boundaries: 0 start | 1 preprocess | 2 depth sort | 3 binning | 4 render fwd | 5 loss | 6 render bwd |
@@ -114,6 +121,24 @@ int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_
 		t->capacity = t->capacity > want ? t->capacity : want;
 		t->bin_bytes = required_bytes<BinState>(t->capacity);
 		if ((rc = dev_alloc(&t->bin_chunk, t->bin_bytes))) return rc;
+	}
+	if (t->deterministic) {
+		if (t->det_cap < t->capacity) {
+			PSB_CUDA_OK(cudaStreamSynchronize(stream));
+			if ((rc = dev_alloc(&t->det_slots, t->capacity * 12))) return rc;
+			PSB_CUDA_OK(cudaMemsetAsync(t->det_slots, 0, t->capacity * 12 * sizeof(float), stream));
+			t->det_cap = t->capacity;
+		}
+		if (t->det_P < (size_t)P) {
+			PSB_CUDA_OK(cudaStreamSynchronize(stream));
+			if ((rc = dev_alloc(&t->det_base, (size_t)P))) return rc;
+			t->det_P = (size_t)P;
+		}
+		if (t->det_parts < loss_partials_doubles(H, W)) {
+			PSB_CUDA_OK(cudaStreamSynchronize(stream));
+			if ((rc = dev_alloc(&t->det_partials, loss_partials_doubles(H, W)))) return rc;
+			t->det_parts = loss_partials_doubles(H, W);
+		}
 	}
 	t->last_P = P; t->last_W = W; t->last_H = H;
 	return 0;
@@ -238,7 +263,8 @@ int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, con
 	t->mark(1, stream);
 	if ((rc = launch_depth_sort_and_scan(P, geom, /*scan=*/false, stream))) return rc;
 	t->mark(2, stream);
-	if ((rc = launch_scan_binning(P, cam, geom, bin, img, t->capacity, t->tight, t->ovf, ++t->seq, stream))) return rc;
+	if ((rc = launch_scan_binning(P, cam, geom, bin, img, t->capacity, t->tight, t->ovf, ++t->seq, stream, t->deterministic ? t->det_base : nullptr)))
+		return rc;
 	t->mark(3, stream);
 	// the instance count travels to pinned memory as soon as it exists: psb_trainer_result waits on `readback`, not on the stream
 	PSB_CUDA_OK(cudaMemcpyAsync(t->h_count, geom.counters, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
@@ -281,8 +307,10 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	Camera cam;
 	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, sc, cam, stream, depth_plane))) return rc;
 	const float* image = out_color ? out_color : t->image;
-	if ((rc = launch_loss(cam.H, cam.W, image, gt_image, mask, step->lambda_dssim, t->dmap, t->sums, t->dL_dpix, stream))) return rc;
-	if (depth_loss && (rc = launch_depth_loss(cam.H, cam.W, depth_plane, depth->gt_depth, mask, depth->lambda_depth, t->sums + 2, dL_ddepth, stream)))
+	double* partials = t->deterministic ? t->det_partials : nullptr;
+	if ((rc = launch_loss(cam.H, cam.W, image, gt_image, mask, step->lambda_dssim, t->dmap, t->sums, t->dL_dpix, stream, partials))) return rc;
+	if (depth_loss &&
+	    (rc = launch_depth_loss(cam.H, cam.W, depth_plane, depth->gt_depth, mask, depth->lambda_depth, t->sums + 2, dL_ddepth, stream, partials)))
 		return rc;
 	// loss sums -> pinned memory right behind the loss kernel, so the host can read the loss of this iteration (and start
 	// enqueueing the next one) while the backward half is still running
@@ -300,8 +328,18 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	sink.opacity = t->sink + 7; sink.opacity_stride = 12;
 	sink.color = t->sink + 8; sink.color_stride = 12;
 	sink.packed = 1;
+	DetSlots det;
+	det.slots = reinterpret_cast<float4*>(t->det_slots);
+	det.base = t->det_base;
+	det.tile_info = sc.geom.tile_info;
+	det.counters = sc.geom.counters;
+	det.capacity = (uint32_t)t->capacity;
+	det.seq = t->seq;
+	det.P = P;
+	det.tight = t->tight ? 1 : 0;
+	// (the deterministic gather runs inside this call: stage "render bwd" covers it)
 	if ((rc = launch_render_backward(cam, sc.img.ranges, sc.bin.inst[sorted_slot(cam.W, cam.H)], sc.geom.rec, background, sc.img.final_T, sc.img.n_contrib,
-	                                 t->dL_dpix, sink, stream, dL_ddepth)))
+	                                 t->dL_dpix, sink, stream, dL_ddepth, t->deterministic ? &det : nullptr)))
 		return rc;
 	t->mark(6, stream);
 	out.geom = sc.geom;
@@ -505,6 +543,7 @@ int psb_trainer_destroy(psb_trainer* t)
 	if (!t) return 0;
 	cudaFree(t->geom_chunk); cudaFree(t->img_chunk); cudaFree(t->bin_chunk); cudaFree(t->image); cudaFree(t->dL_dpix); cudaFree(t->dmap);
 	cudaFree(t->sink); cudaFree(t->seeds); cudaFree(t->sums); cudaFree(t->ovf); cudaFree(t->depth_buf);
+	cudaFree(t->det_slots); cudaFree(t->det_base); cudaFree(t->det_partials);
 	if (t->ev_ready) for (int i = 0; i <= psb_trainer::NSTAGE; i++) cudaEventDestroy(t->ev[i]);
 	if (t->h_sums) cudaFreeHost(t->h_sums);
 	if (t->h_count) cudaFreeHost(t->h_count);
@@ -751,6 +790,13 @@ int psb_trainer_set_profiling(psb_trainer* t, int enable)
 	}
 	t->profiling = enable != 0;
 	t->ev_recorded = false;
+	return 0;
+}
+
+int psb_trainer_set_deterministic(psb_trainer* t, int enable)
+{
+	if (!t) { set_error_msg("psb_trainer_set_deterministic: null context"); return PSB_ERR_ARG; }
+	t->deterministic = enable != 0;   // (its scratch is made by the next call that runs a pass)
 	return 0;
 }
 

@@ -27,6 +27,15 @@ def _ptr(t):
     return t.data_ptr()
 
 
+def _alert_not_deterministic():
+    """The operator backward adds each (Gaussian, tile) sum with float atomics, so its gradients vary run to run: under
+    torch.use_deterministic_algorithms(True) it raises (warns with warn_only=True), like PyTorch's own nondeterministic ops.
+    The trainer contexts (GaussianTrainer / DataParallelTrainer with deterministic=True) have a deterministic backward.
+    (PyTorch's Python-level alert; it does nothing while the flag is off.)"""
+    from torch._prims_common import alert_not_deterministic
+    alert_not_deterministic("psb200 rasterize backward")
+
+
 def _f32c(t):
     if t is None:
         return None
@@ -199,6 +208,7 @@ class _RasterizeGaussians(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out_color, _grad_radii):
+        _alert_not_deterministic()
         rs = ctx.raster_settings
         colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer = ctx.saved_tensors
         (grad_means2D, grad_colors_precomp, grad_opacities, grad_means3D, grad_cov3Ds_precomp, grad_sh, grad_scales,
@@ -233,6 +243,7 @@ class _RasterizeGaussiansDepth(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out_color, _grad_radii, grad_out_depth):
+        _alert_not_deterministic()
         rs = ctx.raster_settings
         colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer = ctx.saved_tensors
         if grad_out_color is None:

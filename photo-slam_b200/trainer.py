@@ -80,9 +80,11 @@ def _bind():
     L.psb_trainer_backward_begin_depth.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp,
                                                    vp, C.POINTER(_Depth), vp]
     L.psb_loss.argtypes = [C.c_int, C.c_int, vp, vp, vp, C.c_float, vp, C.POINTER(C.c_float), vp]
+    L.psb_trainer_set_deterministic.argtypes = [vp, C.c_int]
     for n in ("psb_trainer_create", "psb_trainer_destroy", "psb_trainer_render", "psb_trainer_step", "psb_trainer_backward",
               "psb_adam_update", "psb_trainer_result", "psb_loss", "psb_trainer_render_depth", "psb_trainer_step_depth",
-              "psb_trainer_backward_depth", "psb_trainer_result_depth", "psb_dp_step_depth", "psb_trainer_backward_begin_depth"):
+              "psb_trainer_backward_depth", "psb_trainer_result_depth", "psb_dp_step_depth", "psb_trainer_backward_begin_depth",
+              "psb_trainer_set_deterministic"):
         getattr(L, n).restype = C.c_int
     L.psb_densify_workspace_bytes.argtypes = [C.c_int]
     L.psb_densify_workspace_bytes.restype = C.c_size_t
@@ -440,9 +442,13 @@ def _ccamera(cam):
 
 
 class GaussianTrainer:
-    """One fused training iteration per call. `cam` = dict(viewmatrix, projmatrix, campos: device tensors; tanfovx, tanfovy, W, H)."""
+    """One fused training iteration per call. `cam` = dict(viewmatrix, projmatrix, campos: device tensors; tanfovx, tanfovy, W, H).
 
-    def __init__(self, model: GaussianModel, opt: GaussianOptimizationParams = None, background=None):
+    deterministic: True makes every training call of this trainer bit-identical from run to run (same inputs, build and GPU model;
+    psb_trainer_set_deterministic), False keeps the default (faster) kernels, None follows torch.are_deterministic_algorithms_enabled()
+    at each call."""
+
+    def __init__(self, model: GaussianModel, opt: GaussianOptimizationParams = None, background=None, deterministic=None):
         self.L = _bind()
         self.model = model
         self.opt = opt or GaussianOptimizationParams()
@@ -451,6 +457,22 @@ class GaussianTrainer:
         self.h = h
         self.background = background if background is not None else torch.zeros(3, device=model.device)
         self.iteration = 0
+        self._deterministic = deterministic
+        self._det_applied = False      # the mode the context is in (a new context starts with it off)
+        self._apply_deterministic()
+
+    @property
+    def deterministic(self):
+        """Whether the next training call runs in deterministic mode."""
+        if self._deterministic is None:
+            return torch.are_deterministic_algorithms_enabled()
+        return bool(self._deterministic)
+
+    def _apply_deterministic(self):
+        want = self.deterministic
+        if want != self._det_applied:
+            _lib.check(self.L.psb_trainer_set_deterministic(self.h, int(want)), "psb_trainer_set_deterministic")
+            self._det_applied = want
 
     def __del__(self):
         try:
@@ -500,6 +522,7 @@ class GaussianTrainer:
         over the valid pixels (psb_trainer_step_depth); out_depth: [H,W] float32 tensor that receives the rendered depth."""
         m = self.model
         depth = _cdepth(gt_depth, lambda_depth, out_depth)
+        self._apply_deterministic()
         self.iteration += 1
         if densify_stats is None:
             densify_stats = self.iteration < self.opt.densify_until_iter
@@ -644,10 +667,12 @@ class DataParallelTrainer(GaussianTrainer):
         context's IPC-mapped arena; Adam moments are valid on the owner rank only (gather_moments() before densification
         or a checkpoint).
     mode="nccl": round-1 path kept for A/B — slab-wise backward, one NCCL all-reduce per slab on a side stream, replicated Adam.
-    world == 1 and mode=None: backward -> Adam split path on one GPU (tests)."""
+    world == 1 and mode=None: backward -> Adam split path on one GPU (tests).
+    deterministic: as in GaussianTrainer, kept across rebuild(). "p2p" is then bit-identical run to run at any world size; "nccl"
+    gives deterministic per-rank gradients, but the all-reduce's summation order is NCCL's."""
 
-    def __init__(self, model, opt=None, background=None, group=None, pipeline=None, nslabs=4, mode=None):
-        super().__init__(model, opt, background)
+    def __init__(self, model, opt=None, background=None, group=None, pipeline=None, nslabs=4, mode=None, deterministic=None):
+        super().__init__(model, opt, background, deterministic=deterministic)
         import os
         import torch.distributed as dist
         self.dist = dist
@@ -812,6 +837,7 @@ class DataParallelTrainer(GaussianTrainer):
         target or none: ranks with and without a depth term may train in the same step."""
         m = self.model
         depth = _cdepth(gt_depth, lambda_depth, out_depth)
+        self._apply_deterministic()
         self.iteration += 1
         if densify_stats is None:
             densify_stats = self.iteration < self.opt.densify_until_iter
