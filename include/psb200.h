@@ -215,6 +215,44 @@ typedef struct psb_depth {
 /* psb_trainer_render plus D -> out_depth [H,W] (device; NULL = psb_trainer_render). */
 int psb_trainer_render_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
                              const float* background, int sh_degree, float* out_color, int* radii, float* out_depth, void* stream);
+/* ------------------------------------------------------------------------------------------------
+ * Training against the caller's loss: the fused step split at the loss. psb_trainer_forward renders (colour, optional depth and
+ * accumulated opacity) and returns the pass number; the caller evaluates any loss on those planes and its gradients w.r.t. them;
+ * psb_trainer_backward_pixels runs the tile backward of that pass on the caller's planes, then the per-Gaussian stage of
+ * psb_trainer_step (fused Adam) or of psb_trainer_backward (raw-parameter gradients). The built-in step runs the same kernels with
+ * its own loss in between.
+ * Accumulated opacity: A(p) = 1 - T_final(p) = sum_i alpha_i T_i, the weight of the splats in the pixel (D / A is the normalised
+ * depth; 1 - A is the background's share of the colour). dA/dalpha_i = T_final / (1 - alpha_i).
+ * ------------------------------------------------------------------------------------------------ */
+/* psb_trainer_render_depth plus out_alpha [H,W] (device or NULL) = A. Colour, depth, radii and the pass's scratch are bit-identical to
+ * psb_trainer_render_depth's. *pass (host, may be NULL) receives the pass number (the sequence number psb_trainer_overflow_info counts),
+ * which psb_trainer_backward_pixels takes. Asynchronous on `stream`. */
+int psb_trainer_forward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                        const float* background, int sh_degree, float* out_color, int* radii, float* out_depth, float* out_alpha,
+                        unsigned* pass, void* stream);
+/* Per-pixel gradients of the caller's loss w.r.t. the outputs of one forward pass (device, contiguous float32). */
+typedef struct psb_pixel_grads {
+	const float* dL_dcolor;   /* [3,H,W], required */
+	const float* dL_ddepth;   /* [H,W] or NULL: gradient w.r.t. the depth D */
+	const float* dL_dalpha;   /* [H,W] or NULL: gradient w.r.t. the accumulated opacity A */
+} psb_pixel_grads;
+/* Backward of forward pass `pass` on the caller's gradients, then:
+ *   grads == NULL: the fused Adam of psb_trainer_step (parameters, moments, model->adam_live and, with step->update_densify_stats,
+ *                  the densification statistics are updated; step->step is the Adam step count of this update);
+ *   grads != NULL: the raw-parameter gradients of psb_trainer_backward into grads[0..5] (and the statistics); parameters untouched.
+ * A depth gradient takes dL/dz into the xyz gradient, as psb_trainer_step_depth does. In deterministic mode the result is bit-identical
+ * from run to run for the same planes. step->lambda_dssim is not read.
+ * Contract: `pass` is the context's latest forward pass, made by psb_trainer_forward (or psb_trainer_render / _render_depth), and
+ * model, camera and background are those of that pass (the model's parameters must not change in between). PSB_ERR_ARG when `pass`
+ * is not the latest pass, when the latest pass was a training call (step, backward, _begin: it has had its backward), when
+ * psb_trainer_result regrew the arena since, when P, the image size or step->sh_degree differ from that pass, when the deterministic mode was switched in between, for a
+ * NULL dL_dcolor and for misaligned gradient segments. A pass that overflowed the binning arena makes this call a no-op on the model
+ * and on grads' rows; psb_trainer_result reports PSB_ERR_RETRY for it. psb_trainer_result after this call reports the status and
+ * the instance count only: out3 is left untouched. Stage timing: stage "loss" is the stream time between the two calls.
+ * Asynchronous on `stream`. */
+int psb_trainer_backward_pixels(psb_trainer* t, unsigned pass, int P, int M, const psb_model* model, const psb_camera* camera,
+                                const float* background, const psb_pixel_grads* pixel_grads, const psb_step* step,
+                                float* const* grads, void* stream);
 /* psb_trainer_step / psb_trainer_backward with a depth term; depth == NULL is the plain call. PSB_ERR_ARG for a negative or
  * non-finite lambda_depth, or gt_depth without lambda_depth > 0 (or the reverse). */
 int psb_trainer_step_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,

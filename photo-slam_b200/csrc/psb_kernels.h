@@ -90,13 +90,14 @@ int launch_scan_binning(int P, const Camera& cam, const GeomState& geom, BinStat
                         uint32_t* ovf, uint32_t seq, cudaStream_t stream, uint32_t* base = nullptr);
 int launch_render_forward(const Camera& cam, const uint2* ranges, const uint32_t* point_list, const GaussRec* rec, const float* bg,
                           float* out_color, float* final_T, uint32_t* n_contrib, cudaStream_t stream,
-                          float* out_depth = nullptr /* [H,W]: also render the expected depth (depth variant of the kernel) */);
+                          float* out_depth = nullptr /* [H,W]: also render the expected depth (depth variant of the kernel) */,
+                          float* out_alpha = nullptr /* [H,W]: also write the accumulated opacity 1 - final_T (opacity variant) */);
 // dL_ddepth [H,W]: depth variant, dL/dz of every Gaussian lands in slot 11 of its packed sink row, or at sink.z (unpacked sink;
 // refused without either destination). det != null (packed sink only): the deterministic variant — slot stores, then the ordered gather
-// into the sink rows
+// into the sink rows. dL_dalpha [H,W]: opacity variant, the gradient of the accumulated opacity 1 - final_T joins dL/dalpha of every splat
 int launch_render_backward(const Camera& cam, const uint2* ranges, const uint32_t* point_list, const GaussRec* rec, const float* bg,
                            const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, const GradSink& sink,
-                           cudaStream_t stream, const float* dL_ddepth = nullptr, const DetSlots* det = nullptr);
+                           cudaStream_t stream, const float* dL_ddepth = nullptr, const DetSlots* det = nullptr, const float* dL_dalpha = nullptr);
 // dL_dz [P] (non-null: depth variant): dL/dmean3D += dL/dz (V[2], V[6], V[10]) for every visible Gaussian
 int launch_preprocess_backward(const GaussIn& in, const Camera& cam, const GeomState& geom, const float* dL_dmean2D, int mean2D_stride,
                                const float* dL_dconic, int conic_stride, const float* dL_dcolor, int color_stride,

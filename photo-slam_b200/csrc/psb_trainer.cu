@@ -2,6 +2,8 @@
 // training iteration, and the iteration itself:
 //   preprocess(raw params) -> depth sort -> scan -> emit -> tile sort -> ranges -> render
 //   -> fused L1+SSIM loss fwd/bwd -> tile backward -> fused per-Gaussian backward + Adam (+ densify stats)
+// The same forward, tile backward and per-Gaussian stages also run around a caller's loss (psb_trainer_forward ->
+// the caller's dL/dpixel planes -> psb_trainer_backward_pixels).
 // No host synchronisation inside a step: the instance count stays on the device (the binning arena is sized
 // from the previous iterations and grown on demand; an overflowing step degrades to a no-op and is reported
 // by psb_trainer_result so the caller repeats it).
@@ -26,6 +28,10 @@ struct psb_trainer {
 	uint32_t* h_count = nullptr; // pinned [4]: instance count of the last call | sticky overflow record {count, first seq, largest count}
 	uint32_t* ovf = nullptr;     // device [4]: the sticky overflow record (tile_ranges_kernel), collected by psb_trainer_result
 	uint32_t seq = 0;            // sequence number of the last forward pass (render / step / backward) of this context
+	// what psb_trainer_backward_pixels must match: the SH degree and the mode of pass `seq` (-1: no pass a backward may follow: a
+	// training call's pass, which had its own backward, or a pass whose arena psb_trainer_result regrew)
+	int pass_D = -1;
+	bool pass_det = false;
 	uint32_t ovf_first = 0, ovf_count = 0;  // what the last PSB_ERR_RETRY was about (psb_trainer_overflow_info)
 	cudaEvent_t readback = nullptr;  // recorded once the instance count (and the loss sums) of the last call are in pinned memory
 	int last_P = 0, last_W = 0, last_H = 0;
@@ -246,11 +252,13 @@ int check_grads(float* const* grads, int P, const char* fn)
 	return 0;
 }
 
-// forward from raw parameters into t->image (or out_color); out_depth != NULL: the depth variant also writes the expected depth there
+// Stage 1 of every pass: forward from raw parameters into t->image (or out_color); out_depth != NULL: the depth variant also writes the
+// expected depth there; out_alpha != NULL: the opacity variant also writes 1 - final_T there
 int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, const psb_camera* camera, const float* background,
-                float* out_color, int* radii, Scratch& sc, Camera& cam, cudaStream_t stream, float* out_depth = nullptr)
+                float* out_color, int* radii, Scratch& sc, Camera& cam, cudaStream_t stream, float* out_depth = nullptr, float* out_alpha = nullptr)
 {
 	int rc;
+	t->pass_D = -1;
 	if ((rc = ensure(t, P, camera->width, camera->height, stream))) return rc;
 	cam = to_camera(camera);
 	sc = carve_scratch(t, P, camera->width, camera->height);
@@ -265,15 +273,46 @@ int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, con
 	t->mark(2, stream);
 	if ((rc = launch_scan_binning(P, cam, geom, bin, img, t->capacity, t->tight, t->ovf, ++t->seq, stream, t->deterministic ? t->det_base : nullptr)))
 		return rc;
+	t->pass_D = D;
+	t->pass_det = t->deterministic;
 	t->mark(3, stream);
 	// the instance count travels to pinned memory as soon as it exists: psb_trainer_result waits on `readback`, not on the stream
 	PSB_CUDA_OK(cudaMemcpyAsync(t->h_count, geom.counters, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
 	PSB_CUDA_OK(cudaMemcpyAsync(t->h_count + 1, t->ovf, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
 	PSB_CUDA_OK(cudaEventRecord(t->readback, stream));
 	rc = launch_render_forward(cam, img.ranges, bin.inst[sorted_slot(cam.W, cam.H)], geom.rec, background, out_color ? out_color : t->image, img.final_T,
-	                           img.n_contrib, stream, out_depth);
+	                           img.n_contrib, stream, out_depth, out_alpha);
 	t->mark(4, stream);
 	return rc;
+}
+
+// Stage 3 of every pass: the tile backward of the context's last forward pass (scratch sc, camera cam) on per-pixel gradients -> the
+// packed sink rows (dL_ddepth: also dL/dz in slot 11; dL_dalpha: the opacity variant). P > 0.
+int tile_backward(psb_trainer* t, int P, const Scratch& sc, const Camera& cam, const float* background, const float* dL_dpix, const float* dL_ddepth,
+                  const float* dL_dalpha, cudaStream_t stream)
+{
+	GradSink sink;
+	sink.mean2D = t->sink; sink.mean2D_stride = 12;
+	sink.conic = t->sink + 3; sink.conic_stride = 12;
+	sink.opacity = t->sink + 7; sink.opacity_stride = 12;
+	sink.color = t->sink + 8; sink.color_stride = 12;
+	sink.packed = 1;
+	DetSlots det;
+	det.slots = reinterpret_cast<float4*>(t->det_slots);
+	det.base = t->det_base;
+	det.tile_info = sc.geom.tile_info;
+	det.counters = sc.geom.counters;
+	det.capacity = (uint32_t)t->capacity;
+	det.seq = t->seq;
+	det.P = P;
+	det.tight = t->tight ? 1 : 0;
+	// (the deterministic gather runs inside this call: stage "render bwd" covers it)
+	int rc;
+	if ((rc = launch_render_backward(cam, sc.img.ranges, sc.bin.inst[sorted_slot(cam.W, cam.H)], sc.geom.rec, background, sc.img.final_T, sc.img.n_contrib,
+	                                 dL_dpix, sink, stream, dL_ddepth, t->pass_det ? &det : nullptr, dL_dalpha)))
+		return rc;
+	t->mark(6, stream);
+	return 0;
 }
 
 // What the first half of a training step leaves for its per-Gaussian stage: the sink rows hold the view's screen-space sums
@@ -284,8 +323,8 @@ struct TileBackward {
 	bool depth;
 };
 
-// render -> loss (+ depth loss) -> pinned read-back of the loss sums -> tile backward. `moments`: the caller's per-Gaussian stage
-// updates the Adam moments of the model.
+// The built-in loss around the shared stages: forward -> loss (+ depth loss) -> pinned read-back of the loss sums -> tile backward.
+// `moments`: the caller's per-Gaussian stage updates the Adam moments of the model.
 int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                          const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
                          bool moments, cudaStream_t stream, TileBackward& out)
@@ -306,6 +345,9 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	Scratch sc;
 	Camera cam;
 	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, sc, cam, stream, depth_plane))) return rc;
+	// this pass gets its own tile backward below and its sink rows belong to this call's per-Gaussian stage (or to the _slab calls
+	// that follow a _begin): psb_trainer_backward_pixels must not add a second backward of it
+	t->pass_D = -1;
 	const float* image = out_color ? out_color : t->image;
 	double* partials = t->deterministic ? t->det_partials : nullptr;
 	if ((rc = launch_loss(cam.H, cam.W, image, gt_image, mask, step->lambda_dssim, t->dmap, t->sums, t->dL_dpix, stream, partials))) return rc;
@@ -322,26 +364,7 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	t->have_depth_loss = depth_loss;
 	t->mark(5, stream);
 	if (P == 0) return 0;
-	GradSink sink;
-	sink.mean2D = t->sink; sink.mean2D_stride = 12;
-	sink.conic = t->sink + 3; sink.conic_stride = 12;
-	sink.opacity = t->sink + 7; sink.opacity_stride = 12;
-	sink.color = t->sink + 8; sink.color_stride = 12;
-	sink.packed = 1;
-	DetSlots det;
-	det.slots = reinterpret_cast<float4*>(t->det_slots);
-	det.base = t->det_base;
-	det.tile_info = sc.geom.tile_info;
-	det.counters = sc.geom.counters;
-	det.capacity = (uint32_t)t->capacity;
-	det.seq = t->seq;
-	det.P = P;
-	det.tight = t->tight ? 1 : 0;
-	// (the deterministic gather runs inside this call: stage "render bwd" covers it)
-	if ((rc = launch_render_backward(cam, sc.img.ranges, sc.bin.inst[sorted_slot(cam.W, cam.H)], sc.geom.rec, background, sc.img.final_T, sc.img.n_contrib,
-	                                 t->dL_dpix, sink, stream, dL_ddepth, t->deterministic ? &det : nullptr)))
-		return rc;
-	t->mark(6, stream);
+	if ((rc = tile_backward(t, P, sc, cam, background, t->dL_dpix, dL_ddepth, nullptr, stream))) return rc;
 	out.geom = sc.geom;
 	out.cam = cam;
 	out.depth = depth_loss;
@@ -552,28 +575,77 @@ int psb_trainer_destroy(psb_trainer* t)
 	return 0;
 }
 
-int psb_trainer_render(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
-                       float* out_color, int* radii, void* stream_)
+static int forward_impl(const char* fn, psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                        int sh_degree, float* out_color, int* radii, float* out_depth, float* out_alpha, unsigned* pass, cudaStream_t stream)
 {
 	int rc;
-	if (!t || !camera || !background || !out_color) { set_error_msg("psb_trainer_render: null argument"); return PSB_ERR_ARG; }
+	if (!t || !camera || !background || !out_color) { set_error_msg(std::string(fn).append(": null argument").c_str()); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, false))) return rc;
 	Scratch sc;
 	Camera cam;
 	t->have_loss = false;
-	return forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, sc, cam, (cudaStream_t)stream_);
+	if ((rc = forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, sc, cam, stream, out_depth, out_alpha))) return rc;
+	if (pass) *pass = t->seq;
+	return 0;
+}
+
+int psb_trainer_forward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
+                        float* out_color, int* radii, float* out_depth, float* out_alpha, unsigned* pass, void* stream_)
+{
+	return forward_impl("psb_trainer_forward", t, P, M, model, camera, background, sh_degree, out_color, radii, out_depth, out_alpha, pass,
+	                    (cudaStream_t)stream_);
+}
+
+int psb_trainer_render(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
+                       float* out_color, int* radii, void* stream_)
+{
+	return forward_impl("psb_trainer_render", t, P, M, model, camera, background, sh_degree, out_color, radii, nullptr, nullptr, nullptr,
+	                    (cudaStream_t)stream_);
 }
 
 int psb_trainer_render_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
                              float* out_color, int* radii, float* out_depth, void* stream_)
 {
+	return forward_impl("psb_trainer_render_depth", t, P, M, model, camera, background, sh_degree, out_color, radii, out_depth, nullptr, nullptr,
+	                    (cudaStream_t)stream_);
+}
+
+int psb_trainer_backward_pixels(psb_trainer* t, unsigned pass, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                                const psb_pixel_grads* pixel_grads, const psb_step* step, float* const* grads, void* stream_)
+{
+	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
-	if (!t || !camera || !background || !out_color) { set_error_msg("psb_trainer_render_depth: null argument"); return PSB_ERR_ARG; }
-	if ((rc = check_model(P, M, model, false))) return rc;
-	Scratch sc;
-	Camera cam;
+	const bool adam = grads == nullptr;
+	if (!t || !camera || !background || !pixel_grads || !step) { set_error_msg("psb_trainer_backward_pixels: null argument"); return PSB_ERR_ARG; }
+	if (!pixel_grads->dL_dcolor) { set_error_msg("psb_trainer_backward_pixels: dL_dcolor is required"); return PSB_ERR_ARG; }
+	if (pass == 0 || pass != t->seq || t->pass_D < 0) {
+		set_error_msg("psb_trainer_backward_pixels: `pass` is not the context's latest forward pass (or the arena was regrown since)");
+		return PSB_ERR_ARG;
+	}
+	if (P != t->last_P || P != t->geom_P || camera->width != t->last_W || camera->height != t->last_H || step->sh_degree != t->pass_D) {
+		set_error_msg("psb_trainer_backward_pixels: P, the image size and step->sh_degree must be those of the forward pass");
+		return PSB_ERR_ARG;
+	}
+	if (t->pass_det != t->deterministic) {
+		set_error_msg("psb_trainer_backward_pixels: the deterministic mode changed since the forward pass");
+		return PSB_ERR_ARG;
+	}
+	if (step->step < 1) { set_error_msg("psb_trainer_backward_pixels: step >= 1 required"); return PSB_ERR_ARG; }
+	if ((rc = check_model(P, M, model, adam))) return rc;
+	if (!adam && (rc = check_grads(grads, P, "psb_trainer_backward_pixels"))) return rc;
 	t->have_loss = false;
-	return forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, sc, cam, (cudaStream_t)stream_, out_depth);
+	t->mark(5, stream);   // stage "loss": the caller's, between the two calls
+	if (P == 0) return 0;
+	const Scratch sc = carve_scratch(t, P, camera->width, camera->height);
+	const Camera cam = to_camera(camera);
+	if ((rc = tile_backward(t, P, sc, cam, background, pixel_grads->dL_dcolor, pixel_grads->dL_ddepth, pixel_grads->dL_dalpha, stream))) return rc;
+	GradSegments gs{};
+	if (!adam)
+		for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
+	rc = launch_fused_backward(adam, 0, P, train_tensors(model, adam), cam, sc.geom, t->sink, t->seeds, to_hyper(step), gs, densify_stats(model, step),
+	                           sc.geom.counters, (uint32_t)t->capacity, stream, t->event(7), adam ? model->adam_live : nullptr, pixel_grads->dL_ddepth != nullptr);
+	t->end_stages(8, stream);
+	return rc;
 }
 
 int psb_trainer_step(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
@@ -709,6 +781,7 @@ static int result_impl(psb_trainer* t, float* out, bool with_depth, int* num_ren
 		const uint32_t init[4] = {0u, 0xFFFFFFFFu, 0u, 0u};
 		PSB_CUDA_OK(cudaMemcpy(t->ovf, init, sizeof(init), cudaMemcpyHostToDevice));
 		t->h_count[1] = 0;
+		t->pass_D = -1;   // the scratch of the last pass is gone: no psb_trainer_backward_pixels for it
 		t->capacity = (size_t)(rec[2] * 1.25) + (1u << 16);
 		t->bin_bytes = required_bytes<BinState>(t->capacity);
 		int rc;

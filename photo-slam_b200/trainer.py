@@ -12,6 +12,7 @@ PyTorch provides device memory, streams and (for the data-parallel variant) torc
 """
 import ctypes as C
 import math
+from collections import namedtuple
 from dataclasses import dataclass
 
 import torch
@@ -51,6 +52,26 @@ def _cdepth(gt_depth, lambda_depth, out_depth):
                   out_depth.data_ptr() if out_depth is not None else None)
 
 
+class _PixelGrads(C.Structure):
+    _fields_ = [("dL_dcolor", C.c_void_p), ("dL_ddepth", C.c_void_p), ("dL_dalpha", C.c_void_p)]
+
+
+def _plane(t, shape, what):
+    """a gradient plane for psb_trainer_backward_pixels: None, or a contiguous float32 tensor of `shape` on the model's device type"""
+    if t is None:
+        return None
+    if not torch.is_tensor(t) or tuple(t.shape) != tuple(shape) or t.dtype != torch.float32 or not t.is_contiguous():
+        raise ValueError(f"{what}: want a contiguous float32 tensor of shape {tuple(shape)}, got "
+                         f"{tuple(t.shape) if torch.is_tensor(t) else type(t).__name__}")
+    return t
+
+
+# what result() needs to repeat a trainWithLoss call whose forward overflowed the binning arena
+_LossCall = namedtuple("_LossCall", "cam loss_fn depth alpha out_color radii densify_stats")
+# a backwardPixels call on a render of the caller's: result() cannot repeat the caller's loss, it undoes the counters and raises
+_PixelsCall = namedtuple("_PixelsCall", "adam")
+
+
 class _DensifyCfg(C.Structure):
     _fields_ = [("max_grad", C.c_float), ("min_opacity", C.c_float), ("extent", C.c_float), ("percent_dense", C.c_float), ("max_screen_size", C.c_int),
                 ("seed", C.c_ulonglong), ("offset", C.c_ulonglong)]
@@ -81,10 +102,13 @@ def _bind():
                                                    vp, C.POINTER(_Depth), vp]
     L.psb_loss.argtypes = [C.c_int, C.c_int, vp, vp, vp, C.c_float, vp, C.POINTER(C.c_float), vp]
     L.psb_trainer_set_deterministic.argtypes = [vp, C.c_int]
+    L.psb_trainer_forward.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, C.c_int, vp, vp, vp, vp, C.POINTER(C.c_uint), vp]
+    L.psb_trainer_backward_pixels.argtypes = [vp, C.c_uint, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, C.POINTER(_PixelGrads),
+                                              C.POINTER(_Step), C.POINTER(vp), vp]
     for n in ("psb_trainer_create", "psb_trainer_destroy", "psb_trainer_render", "psb_trainer_step", "psb_trainer_backward",
               "psb_adam_update", "psb_trainer_result", "psb_loss", "psb_trainer_render_depth", "psb_trainer_step_depth",
               "psb_trainer_backward_depth", "psb_trainer_result_depth", "psb_dp_step_depth", "psb_trainer_backward_begin_depth",
-              "psb_trainer_set_deterministic"):
+              "psb_trainer_set_deterministic", "psb_trainer_forward", "psb_trainer_backward_pixels"):
         getattr(L, n).restype = C.c_int
     L.psb_densify_workspace_bytes.argtypes = [C.c_int]
     L.psb_densify_workspace_bytes.restype = C.c_size_t
@@ -494,26 +518,104 @@ class GaussianTrainer:
         s.update_densify_stats = int(densify_stats)
         return s
 
-    def render(self, cam, out=None, radii=None, check=True, out_depth=None):
+    def render(self, cam, out=None, radii=None, check=True, out_depth=None, out_alpha=None):
         """Forward only. check=True waits for the instance count and renders again if the binning arena had to grow (an
         overflowing render leaves `out` blank); pass check=False to only enqueue (call result() yourself before using `out`).
-        out_depth: [H,W] float32 tensor that receives the expected depth sum_i z_i alpha_i T_i (psb_trainer_render_depth)."""
+        out_depth: [H,W] float32 tensor that receives the expected depth sum_i z_i alpha_i T_i; out_alpha: [H,W] float32 tensor that
+        receives the accumulated opacity 1 - T_final (psb_trainer_forward). backwardPixels() back-propagates through this render."""
         m = self.model
         out = out if out is not None else torch.empty((3, cam["H"], cam["W"]), device=m.device)
+        for t in (out_depth, out_alpha):
+            assert t is None or (t.is_contiguous() and t.dtype == torch.float32 and t.numel() == cam["H"] * cam["W"])
         cm, cc = m._cmodel(False), _ccamera(cam)
-        args = (self.h, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(), m.active_sh_degree_, out.data_ptr(),
-                radii.data_ptr() if radii is not None else None)
-        stream = torch.cuda.current_stream().cuda_stream
-        if out_depth is None:
-            _lib.check(self.L.psb_trainer_render(*args, stream), "psb_trainer_render")
-        else:
-            assert out_depth.is_contiguous() and out_depth.dtype == torch.float32 and out_depth.numel() == cam["H"] * cam["W"]
-            _lib.check(self.L.psb_trainer_render_depth(*args, out_depth.data_ptr(), stream), "psb_trainer_render_depth")
-        self._last_render = (cam, out, radii, out_depth)
+        pass_no = C.c_uint()
+        _lib.check(self.L.psb_trainer_forward(self.h, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(), m.active_sh_degree_,
+                                              out.data_ptr(), radii.data_ptr() if radii is not None else None,
+                                              out_depth.data_ptr() if out_depth is not None else None,
+                                              out_alpha.data_ptr() if out_alpha is not None else None, C.byref(pass_no),
+                                              torch.cuda.current_stream().cuda_stream), "psb_trainer_forward")
+        self._pass = pass_no.value
+        self._last_render = (cam, out, radii, out_depth, out_alpha)
         self._last = None
         if check:
             self.result()
         return out
+
+    def backwardPixels(self, dL_dcolor, dL_ddepth=None, dL_dalpha=None, grads=None, densify_stats=None):
+        """Back-propagates per-pixel gradients of the caller's loss through the last render() (psb_trainer_backward_pixels).
+        dL_dcolor [3,H,W] (required), dL_ddepth / dL_dalpha [H,W] or None: contiguous float32 gradients w.r.t. the image, the depth and
+        the accumulated opacity of that render. grads=None: the fused Adam step of trainForOneIteration (advances step_ and iteration);
+        grads = six contiguous float32 tensors shaped like the model's parameters: they receive the raw-parameter gradients and the
+        parameters stay as they are (for a caller's own optimizer or all-reduce). The model must not change between the render and
+        this call. densify_stats as in trainForOneIteration (both modes fold the densification statistics in).
+        If the render overflowed the binning arena (render(check=False) not followed by result()), this call is a no-op on the model and
+        on `grads`; the next result() then rolls step_ / iteration back and raises: render again, recompute the loss, call again."""
+        m = self.model
+        if getattr(self, "_last_render", None) is None or getattr(self, "_pass", None) is None:
+            raise _lib.PsbError("backwardPixels: no forward pass to back-propagate through; call render() first")
+        cam = self._last_render[0]
+        H, W = int(cam["H"]), int(cam["W"])
+        _plane(dL_dcolor, (3, H, W), "dL_dcolor")
+        if dL_dcolor is None:
+            raise ValueError("dL_dcolor is required")
+        _plane(dL_ddepth, (H, W), "dL_ddepth")
+        _plane(dL_dalpha, (H, W), "dL_dalpha")
+        if grads is not None:
+            grads = list(grads)
+            if len(grads) != 6:
+                raise ValueError(f"grads: want six tensors (order {GROUPS}), got {len(grads)}")
+            for name, g, p in zip(GROUPS, grads, m.tensors()):
+                _plane(g, p.shape, "grads[" + name + "]")
+        adam = grads is None
+        if adam:
+            self.iteration += 1
+        if densify_stats is None:
+            densify_stats = self.iteration < self.opt.densify_until_iter
+        cm = m._cmodel(live=m.adamLive()) if adam else m._cmodel()
+        cc, cs = _ccamera(cam), self._cstep(densify_stats)
+        px = _PixelGrads(dL_dcolor.data_ptr(), dL_ddepth.data_ptr() if dL_ddepth is not None else None,
+                         dL_dalpha.data_ptr() if dL_dalpha is not None else None)
+        ptrs = None if adam else (C.c_void_p * 6)(*[g.data_ptr() for g in grads])
+        rc = self.L.psb_trainer_backward_pixels(self.h, self._pass, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(),
+                                                C.byref(px), C.byref(cs), ptrs, torch.cuda.current_stream().cuda_stream)
+        if rc < 0 and adam:
+            self.iteration -= 1
+        _lib.check(rc, "psb_trainer_backward_pixels")
+        if adam:
+            m.step_ += 1
+        self._last = _PixelsCall(adam)     # (trainWithLoss replaces it with its own record)
+
+    def trainWithLoss(self, cam, loss_fn, depth=False, alpha=False, out_color=None, radii=None, densify_stats=None):
+        """One training iteration against the caller's loss: enqueues the forward (no host synchronisation of its own), calls
+        loss = loss_fn(image[, depth][, alpha]) on leaf tensors that require grad (image [3,H,W]; depth [H,W] = sum z alpha T with
+        depth=True; alpha [H,W] = 1 - T_final with alpha=True), takes torch.autograd.grad of the loss w.r.t. those outputs only, and
+        back-propagates it through the fused kernels into a fused Adam step (backwardPixels). The model tensors never enter autograd.
+        Advances step_ / iteration like trainForOneIteration and returns the (detached) loss tensor; result() repeats the whole call
+        if the forward overflowed the binning arena. out_color / radii: optional tensors that receive the image / radii."""
+        if not callable(loss_fn):
+            raise TypeError("loss_fn must be callable")
+        m = self.model
+        H, W = int(cam["H"]), int(cam["W"])
+        image = out_color if out_color is not None else torch.empty((3, H, W), device=m.device)
+        _plane(image, (3, H, W), "out_color")
+        D = torch.empty((H, W), device=m.device) if depth else None
+        A = torch.empty((H, W), device=m.device) if alpha else None
+        self._apply_deterministic()
+        self.render(cam, image, radii, check=False, out_depth=D, out_alpha=A)
+        outs = [t for t in (image, D, A) if t is not None]
+        leaves = [t.detach().requires_grad_(True) for t in outs]
+        with torch.enable_grad():
+            loss = loss_fn(*leaves)
+            g = torch.autograd.grad(loss, leaves, allow_unused=True)
+        g = iter([None if x is None else x.to(torch.float32).contiguous() for x in g])
+        gc = next(g)
+        gc = gc if gc is not None else torch.zeros_like(image)
+        gd = next(g) if depth else None
+        ga = next(g) if alpha else None
+        self.backwardPixels(gc, gd, ga, densify_stats=densify_stats)
+        self._last = _LossCall(cam, loss_fn, depth, alpha, out_color, radii, densify_stats)
+        self._last_loss = loss.detach()
+        return self._last_loss
 
     def trainForOneIteration(self, cam, gt_image, mask=None, out_color=None, radii=None, densify_stats=None, gt_depth=None, lambda_depth=0.0,
                              out_depth=None):
@@ -546,6 +648,7 @@ class GaussianTrainer:
 
     def result(self):
         """Blocks; -> (loss, l1, ssim, num_rendered). Transparently repeats the call if the binning arena had to grow for it.
+        After trainWithLoss: (the caller's loss, nan, nan, num_rendered).
         The overflow record is sticky on the device: if an EARLIER queued step overflowed (it was a no-op on the model while
         step_ advanced), this raises instead of silently continuing. The loss includes the depth term of a depth step."""
         return self._result(False)
@@ -563,22 +666,39 @@ class GaussianTrainer:
             rc = self.L.psb_trainer_result(self.h, out, C.byref(n), stream)
         if rc == -4:
             first, count, cur = self._overflow_info()
+            last = getattr(self, "_last", None)
             if not (count == 1 and first == cur):
-                if getattr(self, "_last", None) is not None:
+                if last is not None and last != _PixelsCall(False):
                     self.model.step_ -= count      # those updates never happened
                     self.iteration -= count
                 raise _lib.PsbError(f"{count} queued call(s) (first: pass {first} of {cur}) overflowed the binning arena and were dropped; the arena has "
                                     "been grown. Collect result() after every step, or render() the view once before queueing steps on it.")
             if getattr(self, "_last", None) is None:  # a render overflowed the arena: render again
-                cam, o, rad, od = self._last_render
-                self.render(cam, o, rad, check=False, out_depth=od)
+                cam, o, rad, od, oa = self._last_render
+                self.render(cam, o, rad, check=False, out_depth=od, out_alpha=oa)
                 return self._result(with_depth)
+            if isinstance(self._last, _PixelsCall):
+                if self._last.adam:
+                    self.model.step_ -= 1             # the Adam step of backwardPixels was a no-op
+                    self.iteration -= 1
+                self._last = None
+                raise _lib.PsbError("the render that backwardPixels back-propagated through overflowed the binning arena, so that call was a "
+                                    "no-op; the arena has been grown. Render again (with check=True, or collect result() before computing the "
+                                    "loss) and repeat the loss and backwardPixels.")
             self.model.step_ -= 1                     # PSB_ERR_RETRY: the step was a no-op
             self.iteration -= 1
-            cam, gt, mask, oc, rad, ds, gd, ld, od = self._last
-            self.trainForOneIteration(cam, gt, mask, oc, rad, ds, gt_depth=gd, lambda_depth=ld, out_depth=od)
+            if isinstance(self._last, _LossCall):
+                self.trainWithLoss(*self._last)
+            else:
+                cam, gt, mask, oc, rad, ds, gd, ld, od = self._last
+                self.trainForOneIteration(cam, gt, mask, oc, rad, ds, gt_depth=gd, lambda_depth=ld, out_depth=od)
             return self._result(with_depth)
         _lib.check(rc, "psb_trainer_result_depth" if with_depth else "psb_trainer_result")
+        if isinstance(getattr(self, "_last", None), _LossCall):
+            # the caller's loss: only its value is known (l1, ssim and depth_l1 are the built-in loss's terms)
+            nan = float("nan")
+            loss = float(self._last_loss)
+            return (loss, nan, nan, nan, n.value) if with_depth else (loss, nan, nan, n.value)
         if with_depth:
             return out[0], out[1], out[2], out[3], n.value
         return out[0], out[1], out[2], n.value
@@ -781,11 +901,11 @@ class DataParallelTrainer(GaussianTrainer):
     def status(self):
         return self.L.psb_dp_status(self.dp, torch.cuda.current_stream().cuda_stream) if self.mode == "p2p" else 0
 
-    def render(self, cam, out=None, radii=None, check=True, out_depth=None):
+    def render(self, cam, out=None, radii=None, check=True, out_depth=None, out_alpha=None):
         """Forward only, on the complete replica: the peers store their rows of the last step asynchronously, so the render is
         ordered behind every rank's rows (device-side wait)."""
         self.sync()
-        return super().render(cam, out, radii, check, out_depth)
+        return super().render(cam, out, radii, check, out_depth, out_alpha)
 
     def gather_moments(self):
         """Every rank receives the Adam moments of all rows (they are only maintained on the owner): call before
@@ -909,6 +1029,18 @@ class DataParallelTrainer(GaussianTrainer):
             return (nan, nan, nan, nan, n.value) if with_depth else (nan, nan, nan, n.value)
         _lib.check(rc, "psb_trainer_result_depth" if with_depth else "psb_trainer_result")
         return (out[0], out[1], out[2], out[3], n.value) if with_depth else (out[0], out[1], out[2], n.value)
+
+    def trainWithLoss(self, *args, **kwargs):
+        raise NotImplementedError("DataParallelTrainer.trainWithLoss: a caller's loss is not wired into the data-parallel steps (the "
+                                  "fused Adam of one rank would desynchronise the replicas); use GaussianTrainer.trainWithLoss on one GPU, or "
+                                  "render() + backwardPixels(..., grads=...) + your own all-reduce + psb_adam_update")
+
+    def backwardPixels(self, dL_dcolor, dL_ddepth=None, dL_dalpha=None, grads=None, densify_stats=None):
+        """Gradient mode only (grads= required): a one-rank Adam step would desynchronise the replicas."""
+        if grads is None:
+            raise NotImplementedError("DataParallelTrainer.backwardPixels: pass grads= (the gradient mode); a one-rank Adam step would "
+                                      "desynchronise the replicas")
+        return super().backwardPixels(dL_dcolor, dL_ddepth, dL_dalpha, grads=grads, densify_stats=densify_stats)
 
     def sync_densify_stats(self):
         """Reduce the rank-local densification statistics (call right before densify/prune)."""
