@@ -136,6 +136,11 @@ int psb_debug_export(int P, int R, int width, int height,
                      uint32_t* tiles_touched, uint64_t* keys_sorted, uint32_t* values_sorted,
                      uint32_t* ranges, uint32_t* n_contrib, float* final_T, void* stream);
 
+/* Diagnostics: occupancy of the tile backward kernel on the current device. variant bit 0: depth, bit 1: deterministic, bit 2: opacity
+ * gradient (dL/dA). Writes the resident blocks per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor at the dynamic shared memory the
+ * launch uses), that dynamic shared memory in bytes, and the kernel's registers per thread. Any output may be NULL. */
+int psb_debug_render_bwd_occupancy(int variant, int* blocks_per_sm, int* dyn_smem_bytes, int* regs_per_thread);
+
 /* ------------------------------------------------------------------------------------------------
  * Trainer-level surface: one fused training iteration on the RAW model tensors.
  *
