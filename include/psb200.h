@@ -116,6 +116,36 @@ int psb_rasterize_backward_depth(int P, int D, int M, int R,
                                  float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
                                  const float* dL_ddepth, float* dL_dz, void* stream);
 
+/*
+ * Deterministic backward on the operator path: for the same inputs and the same forward scratch, every output is bit-identical from
+ * call to call. psb_rasterize_backward[_depth] add each (Gaussian, tile) sum into the gradient arrays with float atomics, so their
+ * last bits depend on the order in which tiles finish; here each sum is stored in a slot of its own and one thread per Gaussian adds
+ * its slots in a fixed order (the instances' emission order) and writes the result.
+ *
+ * psb_rasterize_backward_det_bytes: size of the scratch this needs, a pure function of (P, R): 48 B per instance and 4 B per Gaussian,
+ * plus alignment (0 for a negative argument). It is separate from the three forward chunks, whose sizes and contents do not change.
+ *
+ * psb_rasterize_backward_deterministic: the argument list of psb_rasterize_backward_depth plus det_scratch (device, at least
+ * psb_rasterize_backward_det_bytes(P, R) bytes, caller-allocated; its contents are irrelevant: the call zeroes what it reads) and
+ * det_scratch_bytes, before the stream. dL_ddepth == NULL is colour only; with dL_ddepth, dL_dz is required. Outputs and their
+ * meaning are those of psb_rasterize_backward[_depth] (caller-zeroed arrays; rows of invisible Gaussians left untouched).
+ * PSB_ERR_ARG for a NULL or too small det_scratch, for dL_ddepth without dL_dz, and for everything psb_rasterize_backward rejects,
+ * all checked before any CUDA call. P == 0 does nothing.
+ */
+size_t psb_rasterize_backward_det_bytes(int P, int R);
+int psb_rasterize_backward_deterministic(int P, int D, int M, int R,
+                                         const float* background, int width, int height,
+                                         const float* means3D, const float* shs, const float* colors_precomp,
+                                         const float* scales, float scale_modifier, const float* rotations,
+                                         const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix,
+                                         const float* campos, float tan_fovx, float tan_fovy, const int* radii,
+                                         char* geom_buffer, char* binning_buffer, char* image_buffer,
+                                         const float* dL_dpix,
+                                         float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                                         float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
+                                         const float* dL_ddepth, float* dL_dz, void* det_scratch, size_t det_scratch_bytes,
+                                         void* stream);
+
 /* Near-plane visibility (view z > 0.2). Replaces CudaRasterizer::Rasterizer::markVisible
  * (cuda_rasterizer/rasterizer.h:24-29, rasterizer_impl.cu:141-153). present: [P] bytes (bool), device. */
 int psb_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,
@@ -381,7 +411,7 @@ int psb_trainer_stage_times(psb_trainer* t, float* ms, int n);
  * of its own and a gather adds every Gaussian's slots in a fixed order, instead of adding them into the Gaussian's row with
  * float atomics in whatever order the tiles finish; the loss sums are reduced in a fixed order too. It costs a slot buffer of
  * 48 B per instance of the binning capacity (grown with it) and the time of the gather, counted in the "render backward" stage.
- * Not covered: the B1/B2 operator path (psb_rasterize_backward*), and the NCCL all-reduce that a caller runs between
+ * The operator path has its own entry point, psb_rasterize_backward_deterministic. Not covered: the NCCL all-reduce that a caller runs between
  * psb_trainer_backward* and psb_adam_update: each rank's gradients are deterministic, the all-reduce's order is NCCL's. */
 int psb_trainer_set_deterministic(psb_trainer* t, int enable);
 

@@ -42,6 +42,11 @@ def lib():
     L.psb_rasterize_forward_depth.argtypes = L.psb_rasterize_forward.argtypes[:-1] + [fp, vp]
     L.psb_rasterize_backward_depth.restype = C.c_int
     L.psb_rasterize_backward_depth.argtypes = L.psb_rasterize_backward.argtypes[:-1] + [fp, fp, vp]
+    # the deterministic backward: the _depth argument list plus det_scratch, det_scratch_bytes, before the stream
+    L.psb_rasterize_backward_det_bytes.restype = C.c_size_t
+    L.psb_rasterize_backward_det_bytes.argtypes = [C.c_int, C.c_int]
+    L.psb_rasterize_backward_deterministic.restype = C.c_int
+    L.psb_rasterize_backward_deterministic.argtypes = L.psb_rasterize_backward_depth.argtypes[:-1] + [vp, C.c_size_t, vp]
     L.psb_mark_visible.restype = C.c_int
     L.psb_mark_visible.argtypes = [C.c_int, fp, fp, fp, u8p, vp]
     L.psb_debug_export.restype = C.c_int

@@ -115,19 +115,28 @@ static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void*
 	return (int)num_rendered;
 }
 
-// Body of psb_rasterize_backward[_depth]. dL_ddepth [H,W] or NULL; with it, dL_dz [P] receives dL/dz and the depth variants run.
+// Scratch bytes of the deterministic operator backward; 0 for a negative size.
+static size_t op_det_bytes(int P, int R) { return (P < 0 || R < 0) ? 0 : OpDetState::required_bytes((size_t)P, (size_t)R); }
+
+// Body of psb_rasterize_backward[_depth|_deterministic]. dL_ddepth [H,W] or NULL; with it, dL_dz [P] receives dL/dz and the depth
+// variants run. det: the deterministic variant over det_scratch (det_bytes: its size; both checked here, before any CUDA call).
 static int rasterize_backward(const char* fn, int P, int D, int M, int R, const float* background, int width, int height, const float* means3D,
                               const float* shs, const float* colors_precomp, const float* scales, float scale_modifier, const float* rotations,
                               const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix, const float* campos, float tan_fovx,
                               float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer, const float* dL_dpix,
                               float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dmean3D, float* dL_dcov3D,
-                              float* dL_dsh, float* dL_dscale, float* dL_drot, const float* dL_ddepth, float* dL_dz, void* stream_)
+                              float* dL_dsh, float* dL_dscale, float* dL_drot, const float* dL_ddepth, float* dL_dz, void* stream_,
+                              bool det = false, void* det_scratch = nullptr, size_t det_bytes = 0)
 {
 	(void)radii;  // visibility is re-derived from the private geometry state (tiles_touched), identical to radii > 0
 	cudaStream_t stream = (cudaStream_t)stream_;
 	if (P == 0) return 0;
 	if (P < 0 || R < 0 || !geom_buffer || !binning_buffer || !image_buffer || !dL_dpix || !dL_dmean2D || !dL_dconic || !dL_dopacity || !dL_dcolor)
 		return arg_error(fn, "bad argument");
+	if (det && !det_scratch) return arg_error(fn, "det_scratch is NULL");
+	if (det && det_bytes < op_det_bytes(P, R))
+		return arg_error(fn, ("det_scratch holds " + std::to_string(det_bytes) + " bytes, psb_rasterize_backward_det_bytes(P, R) = " +
+		                      std::to_string(op_det_bytes(P, R))).c_str());
 	const Camera cam = make_camera(width, height, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy);
 	GeomState geom = GeomState::from_chunk(geom_buffer, (size_t)P);
 	BinState bin = BinState::from_chunk(binning_buffer, (size_t)R);
@@ -141,7 +150,21 @@ static int rasterize_backward(const char* fn, int P, int D, int M, int R, const 
 	sink.packed = 0;
 	if (dL_ddepth) { sink.z = dL_dz; sink.z_stride = 1; }
 	int rc;
-	if (R > 0)
+	if (R > 0 && det) {
+		// Every (Gaussian, tile) sum goes to the slot of its instance, base[g] + the tile's row-major rank in g's full rectangle (the
+		// emission order of emit_instances_kernel), and the gather adds each Gaussian's slots in that order. The slots are zeroed on
+		// every call: a block handed back by the caller's allocator may hold tags of an earlier call, which the fixed seq would accept.
+		char* chunk = static_cast<char*>(det_scratch);
+		const OpDetState ds = OpDetState::from_chunk(chunk, (size_t)P, (size_t)R);
+		PSB_CUDA_OK(cudaMemsetAsync(ds.slots, 0, (size_t)R * 3 * sizeof(float4), stream));
+		if ((rc = launch_det_base(P, geom, ds.base, stream))) return rc;
+		DetSlots slots;
+		slots.slots = ds.slots; slots.base = ds.base; slots.tile_info = geom.tile_info; slots.counters = geom.counters;
+		slots.capacity = (uint32_t)R; slots.seq = 1u; slots.P = P; slots.tight = 0;
+		if ((rc = launch_render_backward(cam, img.ranges, bin.inst[sorted_slot(width, height)], geom.rec, background, img.final_T, img.n_contrib, dL_dpix,
+		                                 sink, stream, dL_ddepth, &slots)))
+			return rc;
+	} else if (R > 0)
 		if ((rc = launch_render_backward(cam, img.ranges, bin.inst[sorted_slot(width, height)], geom.rec, background, img.final_T, img.n_contrib, dL_dpix, sink, stream, dL_ddepth)))
 			return rc;
 
@@ -215,6 +238,24 @@ int psb_rasterize_backward_depth(int P, int D, int M, int R, const float* backgr
 	                          scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, radii, geom_buffer,
 	                          binning_buffer, image_buffer, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh,
 	                          dL_dscale, dL_drot, dL_ddepth, dL_dz, stream);
+}
+
+size_t psb_rasterize_backward_det_bytes(int P, int R) { return op_det_bytes(P, R); }
+
+int psb_rasterize_backward_deterministic(int P, int D, int M, int R, const float* background, int width, int height, const float* means3D,
+                                         const float* shs, const float* colors_precomp, const float* scales, float scale_modifier,
+                                         const float* rotations, const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix,
+                                         const float* campos, float tan_fovx, float tan_fovy, const int* radii, char* geom_buffer,
+                                         char* binning_buffer, char* image_buffer, const float* dL_dpix, float* dL_dmean2D, float* dL_dconic,
+                                         float* dL_dopacity, float* dL_dcolor, float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh,
+                                         float* dL_dscale, float* dL_drot, const float* dL_ddepth, float* dL_dz, void* det_scratch,
+                                         size_t det_scratch_bytes, void* stream)
+{
+	if (dL_ddepth && !dL_dz) return arg_error("psb_rasterize_backward_deterministic", "dL_ddepth needs a dL_dz array");
+	return rasterize_backward("psb_rasterize_backward_deterministic", P, D, M, R, background, width, height, means3D, shs, colors_precomp, scales,
+	                          scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, radii, geom_buffer,
+	                          binning_buffer, image_buffer, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh,
+	                          dL_dscale, dL_drot, dL_ddepth, dL_dz, stream, /*det=*/true, det_scratch, det_scratch_bytes);
 }
 
 int psb_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix, unsigned char* present, void* stream_)

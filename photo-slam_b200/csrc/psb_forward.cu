@@ -441,6 +441,17 @@ __global__ void __launch_bounds__(EM_THREADS) emit_scan_kernel(int P, const uint
 	}
 }
 
+// B1/B2 path, deterministic backward: scan_offsets_kernel left the emission offset of depth rank j in offsets[j]; the tile backward
+// and the gather index by Gaussian, so invert the permutation for the Gaussians that have instances.
+__global__ void __launch_bounds__(256) det_base_kernel(int P, const uint32_t* __restrict__ order, const uint4* __restrict__ tile_info,
+                                                       const uint32_t* __restrict__ offsets, uint32_t* __restrict__ base)
+{
+	const int j = blockIdx.x * blockDim.x + threadIdx.x;
+	if (j >= P) return;
+	const uint32_t g = order[j];
+	if (tile_info[g].z & TT_COUNT) base[g] = offsets[j];
+}
+
 // Start/end of every tile in the tile-sorted instance list (semantics of reference
 // rasterizer_impl.cu:116-138; ranges must be zeroed beforehand so untouched tiles read {0,0}).
 // ovf (trainer path, may be null): sticky record of overflowing views {count, first sequence number, largest instance count}
@@ -504,6 +515,14 @@ int launch_depth_sort_and_scan(int P, GeomState& geom, bool scan, cudaStream_t s
 		                                                                    geom.scan_status);
 		PSB_LAUNCH_OK();
 	}
+	return 0;
+}
+
+int launch_det_base(int P, const GeomState& geom, uint32_t* base, cudaStream_t stream)
+{
+	if (P == 0) return 0;
+	det_base_kernel<<<cdiv(P, 256), 256, 0, stream>>>(P, geom.order[0], geom.tile_info, geom.offsets, base);
+	PSB_LAUNCH_OK();
 	return 0;
 }
 

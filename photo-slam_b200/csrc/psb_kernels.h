@@ -33,14 +33,14 @@ struct GradSink {
 	float* z = nullptr; int z_stride = 0;  // unpacked sink with a depth gradient: the tenth sum, dL/dz (the packed row keeps it in slot 11)
 };
 
-// Deterministic mode of the trainer's tile backward (packed sink only). Float atomics from tiles that finish in any order would
+// Deterministic mode of the tile backward (the trainer's packed sink, or the operator's unpacked one). Float atomics from tiles that finish in any order would
 // sum a Gaussian's (Gaussian, tile) flushes in a different order every run; instead each flush is STORED in the slot of its
 // instance's emission index, base[g] + (rank of the tile among g's instances, InstRect), and gather_slots_kernel then sums every
-// Gaussian's slots in emission order and writes its sink row. A slot counts only when tagged with this pass's `seq`: entries the
+// Gaussian's slots in emission order and writes its sink row(s). A slot counts only when tagged with this pass's `seq`: entries the
 // tile backward does not flush (behind a tile's deepest contributor, culled by the reach tests) keep an older tag and read as zero.
 struct DetSlots {
 	float4* slots;              // [capacity][3]: one packed sink row per instance; lane 2 (padding) = seq of the pass that wrote it
-	const uint32_t* base;       // [P] emission offset of each Gaussian with instances (emit_scan_kernel, DET)
+	const uint32_t* base;       // [P] emission offset of each Gaussian with instances (emit_scan_kernel, DET; operator path: launch_det_base)
 	const uint4* tile_info;     // GeomState::tile_info
 	const uint32_t* counters;   // GeomState::counters: an overflowing pass (counters[0] > capacity) gathers nothing
 	uint32_t capacity, seq;
@@ -85,6 +85,9 @@ int launch_preprocess(const GaussIn& in, const Camera& cam, int* radii_out, cons
 int launch_mark_visible(int P, const float* means3D, const float* view, uint8_t* present, cudaStream_t stream);
 int launch_depth_sort_and_scan(int P, GeomState& geom, bool scan, cudaStream_t stream);
 int launch_binning(int P, const Camera& cam, const GeomState& geom, BinState& bin, const ImgState& img, size_t n_host, cudaStream_t stream);
+// B1/B2 path after launch_depth_sort_and_scan(scan = true): base[order[0][j]] <- offsets[j] for every Gaussian with instances, the
+// emission offsets by Gaussian index that the deterministic tile backward needs (DetSlots::base); other entries are not written
+int launch_det_base(int P, const GeomState& geom, uint32_t* base, cudaStream_t stream);
 // base != null (deterministic mode): base[g] <- emission offset of every Gaussian with instances (DetSlots::base)
 int launch_scan_binning(int P, const Camera& cam, const GeomState& geom, BinState& bin, const ImgState& img, size_t capacity, bool tight,
                         uint32_t* ovf, uint32_t seq, cudaStream_t stream, uint32_t* base = nullptr);
@@ -93,8 +96,8 @@ int launch_render_forward(const Camera& cam, const uint2* ranges, const uint32_t
                           float* out_depth = nullptr /* [H,W]: also render the expected depth (depth variant of the kernel) */,
                           float* out_alpha = nullptr /* [H,W]: also write the accumulated opacity 1 - final_T (opacity variant) */);
 // dL_ddepth [H,W]: depth variant, dL/dz of every Gaussian lands in slot 11 of its packed sink row, or at sink.z (unpacked sink;
-// refused without either destination). det != null (packed sink only): the deterministic variant — slot stores, then the ordered gather
-// into the sink rows. dL_dalpha [H,W]: opacity variant, the gradient of the accumulated opacity 1 - final_T joins dL/dalpha of every splat
+// refused without either destination). det != null: the deterministic variant — slot stores, then the ordered gather, which WRITES the
+// sink rows (packed: gather_slots_kernel; unpacked: gather_slots_unpacked_kernel, dL/dz at sink.z with dL_ddepth). dL_dalpha [H,W]: opacity variant, the gradient of the accumulated opacity 1 - final_T joins dL/dalpha of every splat
 int launch_render_backward(const Camera& cam, const uint2* ranges, const uint32_t* point_list, const GaussRec* rec, const float* bg,
                            const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, const GradSink& sink,
                            cudaStream_t stream, const float* dL_ddepth = nullptr, const DetSlots* det = nullptr, const float* dL_dalpha = nullptr);

@@ -93,6 +93,27 @@ struct ImgState {
 	}
 };
 
+// Scratch of the deterministic operator backward (psb_rasterize_backward_deterministic): function of (P, R). It is a separate,
+// caller-allocated chunk, so the three chunks above and psb_*_bytes stay what the forward carved.
+struct OpDetState {
+	float4* slots;    // [R][3]: one packed sink row per instance (DetSlots::slots)
+	uint32_t* base;   // [P] emission offset of each Gaussian with instances (DetSlots::base)
+
+	static OpDetState from_chunk(char*& chunk, size_t P, size_t R)
+	{
+		OpDetState s;
+		s.slots = carve<float4>(chunk, 3 * R);
+		s.base = carve<uint32_t>(chunk, P);
+		return s;
+	}
+	static size_t required_bytes(size_t P, size_t R)
+	{
+		char* p = nullptr;
+		from_chunk(p, P, R);
+		return reinterpret_cast<size_t>(p) + 128;
+	}
+};
+
 template <typename S>
 static inline size_t required_bytes(size_t n)
 {

@@ -191,6 +191,55 @@ RasterizeGaussiansBackwardDepthCUDA(const torch::Tensor& background, const torch
 	return std::make_tuple(dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations);
 }
 
+// RasterizeGaussiansBackwardDepthCUDA whose outputs are bit-identical from call to call (psb_rasterize_backward_deterministic): the
+// (Gaussian, tile) sums are added in a fixed order instead of with float atomics. An undefined or empty dL_dout_depth is colour only.
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
+RasterizeGaussiansBackwardDeterministicCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii,
+                                            const torch::Tensor& colors, const torch::Tensor& scales, const torch::Tensor& rotations,
+                                            const float scale_modifier, const torch::Tensor& cov3D_precomp, const torch::Tensor& viewmatrix,
+                                            const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
+                                            const torch::Tensor& dL_dout_color, const torch::Tensor& dL_dout_depth, const torch::Tensor& sh,
+                                            const int degree, const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R,
+                                            const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer)
+{
+	const int P = means3D.size(0);
+	const int H = dL_dout_color.size(1), W = dL_dout_color.size(2);
+	const bool depth = dL_dout_depth.defined() && dL_dout_depth.numel() != 0;
+	if (depth && (dL_dout_depth.ndimension() != 2 || dL_dout_depth.size(0) != H || dL_dout_depth.size(1) != W)) {
+		AT_ERROR("dL_dout_depth must have dimensions (", H, ", ", W, ")");
+	}
+	int M = 0;
+	if (sh.size(0) != 0) M = sh.size(1);
+	torch::Tensor dL_dmeans3D = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_dmeans2D = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_dcolors = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_dconic = torch::zeros({P, 2, 2}, means3D.options());
+	torch::Tensor dL_dopacity = torch::zeros({P, 1}, means3D.options());
+	torch::Tensor dL_dcov3D = torch::zeros({P, 6}, means3D.options());
+	torch::Tensor dL_dsh = torch::zeros({P, M, 3}, means3D.options());
+	torch::Tensor dL_dscales = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_drotations = torch::zeros({P, 4}, means3D.options());
+	torch::Tensor dL_dz = torch::zeros({depth ? P : 0}, means3D.options());
+	if (P != 0) {
+		const auto bg = background.contiguous(), m3 = means3D.contiguous(), shc = sh.contiguous(), col = colors.contiguous(), sc = scales.contiguous(),
+		           rot = rotations.contiguous(), cov = cov3D_precomp.contiguous(), vm = viewmatrix.contiguous(), pm = projmatrix.contiguous(),
+		           cp = campos.contiguous(), dpix = dL_dout_color.contiguous(), rad = radii.contiguous();
+		const torch::Tensor ddep = depth ? dL_dout_depth.contiguous() : torch::Tensor();
+		const size_t det_bytes = psb_rasterize_backward_det_bytes(P, R);
+		torch::Tensor det_scratch = torch::empty({(long long)det_bytes}, means3D.options().dtype(torch::kByte));
+		const int rc = psb_rasterize_backward_deterministic(
+			P, degree, M, R, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
+			tan_fovx, tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(geomBuffer.contiguous().data_ptr()),
+			reinterpret_cast<char*>(binningBuffer.contiguous().data_ptr()), reinterpret_cast<char*>(imageBuffer.contiguous().data_ptr()), fptr(dpix),
+			dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(), dL_dopacity.data_ptr<float>(), dL_dcolors.data_ptr<float>(),
+			dL_dmeans3D.data_ptr<float>(), dL_dcov3D.data_ptr<float>(), M ? dL_dsh.data_ptr<float>() : nullptr, dL_dscales.data_ptr<float>(),
+			dL_drotations.data_ptr<float>(), depth ? ddep.data_ptr<float>() : nullptr, depth ? dL_dz.data_ptr<float>() : nullptr, det_scratch.data_ptr(),
+			det_bytes, current_stream());
+		if (rc < 0) { AT_ERROR("psb_rasterize_backward_deterministic: ", psb_last_error()); }
+	}
+	return std::make_tuple(dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations);
+}
+
 torch::Tensor markVisible(torch::Tensor& means3D, torch::Tensor& viewmatrix, torch::Tensor& projmatrix)
 {
 	const int P = means3D.size(0);
@@ -378,6 +427,14 @@ std::tuple<T, T, T, T, T, T, T, T> op_bwd_depth(const T& bg, const T& m3, const 
 	return RasterizeGaussiansBackwardDepthCUDA(bg, m3, radii, col, sc, rot, (float)smod, cov, vm, pm, (float)tfx, (float)tfy, dpix, ddep.value_or(T()), sh,
 	                                           (int)deg, cp, gb, (int)R, bb, ib);
 }
+std::tuple<T, T, T, T, T, T, T, T> op_bwd_det(const T& bg, const T& m3, const T& radii, const T& col, const T& sc, const T& rot, double smod,
+                                              const T& cov, const T& vm, const T& pm, double tfx, double tfy, const T& dpix,
+                                              const std::optional<T>& ddep, const T& sh, int64_t deg, const T& cp, const T& gb, int64_t R, const T& bb,
+                                              const T& ib)
+{
+	return RasterizeGaussiansBackwardDeterministicCUDA(bg, m3, radii, col, sc, rot, (float)smod, cov, vm, pm, (float)tfx, (float)tfy, dpix, ddep.value_or(T()),
+	                                                   sh, (int)deg, cp, gb, (int)R, bb, ib);
+}
 T op_vis(T m3, T vm, T pm) { return markVisible(m3, vm, pm); }
 T op_dist(const T& p) { return distCUDA2(p); }
 T op_xform(T p, T m) { transformPoints(p, m); return p; }
@@ -413,6 +470,7 @@ TORCH_LIBRARY(psb200, m)
 	m.def("rasterize_gaussians_backward", &op_bwd);
 	m.def("rasterize_gaussians_depth", &op_fwd_depth);
 	m.def("rasterize_gaussians_backward_depth", &op_bwd_depth);
+	m.def("rasterize_gaussians_backward_deterministic", &op_bwd_det);
 	m.def("mark_visible", &op_vis);
 	m.def("b2_forward", &op_b2_fwd);
 	m.def("dist_cuda2", &op_dist);

@@ -11,6 +11,9 @@ Rendered depth D(p) = sum_i z_i alpha_i T_i (include/psb200.h), which the refere
   RasterizeGaussiansDepthCUDA / RasterizeGaussiansBackwardDepthCUDA   the two functions above plus the depth image and its gradient
   _RasterizeGaussiansDepth, GaussianRasterizer.forward(..., return_depth=True)   autograd through colour and depth
 
+deterministic=True (keyword) on the backward functions, rasterize_gaussians and GaussianRasterizer.forward selects
+psb_rasterize_backward_deterministic: the same gradients, bit-identical from run to run. The default keeps the float-atomic backward.
+
 PyTorch is used only for device memory, streams and autograd bookkeeping.
 """
 from dataclasses import dataclass
@@ -30,7 +33,8 @@ def _ptr(t):
 def _alert_not_deterministic():
     """The operator backward adds each (Gaussian, tile) sum with float atomics, so its gradients vary run to run: under
     torch.use_deterministic_algorithms(True) it raises (warns with warn_only=True), like PyTorch's own nondeterministic ops.
-    The trainer contexts (GaussianTrainer / DataParallelTrainer with deterministic=True) have a deterministic backward.
+    The operator's deterministic=True backward and the trainer contexts (GaussianTrainer / DataParallelTrainer with
+    deterministic=True) do not alert.
     (PyTorch's Python-level alert; it does nothing while the flag is off.)"""
     from torch._prims_common import alert_not_deterministic
     alert_not_deterministic("psb200 rasterize backward")
@@ -110,8 +114,10 @@ def RasterizeGaussiansDepthCUDA(background, means3D, colors, opacity, scales, ro
 
 
 def _backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
-              tan_fovx, tan_fovy, dL_dout_color, dL_dout_depth, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer):
-    """RasterizeGaussiansBackwardCUDA, and with a depth gradient psb_rasterize_backward_depth."""
+              tan_fovx, tan_fovy, dL_dout_color, dL_dout_depth, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer,
+              deterministic=False):
+    """RasterizeGaussiansBackwardCUDA, and with a depth gradient psb_rasterize_backward_depth; deterministic=True calls
+    psb_rasterize_backward_deterministic (either gradient set) over a scratch of psb_rasterize_backward_det_bytes(P, R)."""
     L = _lib.lib()
     P = means3D.size(0)
     H, W = dL_dout_color.size(1), dL_dout_color.size(2)
@@ -135,11 +141,18 @@ def _backward(background, means3D, radii, colors, scales, rotations, scale_modif
                 _ptr(radii), _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imageBuffer), _ptr(dpix),
                 dL_dmeans2D.data_ptr(), dL_dconic.data_ptr(), dL_dopacity.data_ptr(), dL_dcolors.data_ptr(),
                 dL_dmeans3D.data_ptr(), dL_dcov3D.data_ptr(), _ptr(dL_dsh), dL_dscales.data_ptr(), dL_drotations.data_ptr()]
+        ddep = dL_dz = None
         if dL_dout_depth is not None:
             ddep = _f32c(dL_dout_depth)
             if tuple(ddep.shape) != (H, W):
                 raise RuntimeError(f"dL_dout_depth must have dimensions ({H}, {W})")
             dL_dz = torch.zeros((P,), **o)      # [P], zero-initialised as the C-ABI requires; folded into dL_dmeans3D there
+        if deterministic:
+            nbytes = L.psb_rasterize_backward_det_bytes(P, int(R))
+            scratch = torch.empty((nbytes,), dtype=torch.uint8, device=means3D.device)    # the call zeroes what it reads
+            _lib.check(L.psb_rasterize_backward_deterministic(*args, _ptr(ddep), _ptr(dL_dz), scratch.data_ptr(), nbytes, _stream()),
+                       "psb_rasterize_backward_deterministic")
+        elif ddep is not None:
             _lib.check(L.psb_rasterize_backward_depth(*args, ddep.data_ptr(), dL_dz.data_ptr(), _stream()), "psb_rasterize_backward_depth")
         else:
             _lib.check(L.psb_rasterize_backward(*args, _stream()), "psb_rasterize_backward")
@@ -148,19 +161,21 @@ def _backward(background, means3D, radii, colors, scales, rotations, scale_modif
 
 def RasterizeGaussiansBackwardCUDA(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp,
                                    viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, sh, degree, campos,
-                                   geomBuffer, R, binningBuffer, imageBuffer):
-    """-> (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations)."""
+                                   geomBuffer, R, binningBuffer, imageBuffer, *, deterministic=False):
+    """-> (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations).
+    deterministic=True: the same gradients, bit-identical from call to call (summed in a fixed order instead of with float atomics)."""
     return _backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
-                     tan_fovx, tan_fovy, dL_dout_color, None, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer)
+                     tan_fovx, tan_fovy, dL_dout_color, None, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer, deterministic)
 
 
 def RasterizeGaussiansBackwardDepthCUDA(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp,
                                         viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, dL_dout_depth, sh, degree, campos,
-                                        geomBuffer, R, binningBuffer, imageBuffer):
+                                        geomBuffer, R, binningBuffer, imageBuffer, *, deterministic=False):
     """RasterizeGaussiansBackwardCUDA with the gradient of the depth image as well (dL_dout_depth [H,W]; None = the plain backward).
-    dL/dz is folded into dL_dmeans3D, and dL_dmeans2D includes the depth term. Returns the same 8-tuple."""
+    dL/dz is folded into dL_dmeans3D, and dL_dmeans2D includes the depth term. Returns the same 8-tuple. deterministic: as there."""
     return _backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
-                     tan_fovx, tan_fovy, dL_dout_color, dL_dout_depth, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer)
+                     tan_fovx, tan_fovy, dL_dout_color, dL_dout_depth, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer,
+                     deterministic)
 
 
 def markVisible(means3D, viewmatrix, projmatrix):
@@ -193,7 +208,7 @@ class _RasterizeGaussians(torch.autograd.Function):
     """reference GaussianRasterizerFunction (src/gaussian_rasterizer.cpp:28-180)."""
 
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):
+    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings, deterministic=False):
         rs = raster_settings
         num_rendered, color, radii, geomBuffer, binningBuffer, imgBuffer = RasterizeGaussiansCUDA(
             rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
@@ -201,6 +216,7 @@ class _RasterizeGaussians(torch.autograd.Function):
             rs.campos, rs.prefiltered)
         ctx.raster_settings = rs
         ctx.num_rendered = num_rendered
+        ctx.deterministic = bool(deterministic)
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
                               binningBuffer, imgBuffer)
         ctx.mark_non_differentiable(radii)
@@ -208,26 +224,27 @@ class _RasterizeGaussians(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out_color, _grad_radii):
-        _alert_not_deterministic()
+        if not ctx.deterministic:
+            _alert_not_deterministic()
         rs = ctx.raster_settings
         colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer = ctx.saved_tensors
         (grad_means2D, grad_colors_precomp, grad_opacities, grad_means3D, grad_cov3Ds_precomp, grad_sh, grad_scales,
          grad_rotations) = RasterizeGaussiansBackwardCUDA(
             rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix,
             rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_out_color, sh, rs.sh_degree, rs.campos, geomBuffer,
-            ctx.num_rendered, binningBuffer, imgBuffer)
+            ctx.num_rendered, binningBuffer, imgBuffer, deterministic=ctx.deterministic)
         # order of reference gaussian_rasterizer.cpp:159-179
         def g(t, ref):
             return t if (ref is not None and ref.numel() != 0) else None
         return (grad_means3D, grad_means2D, g(grad_sh, sh), g(grad_colors_precomp, colors_precomp), grad_opacities,
-                g(grad_scales, scales), g(grad_rotations, rotations), g(grad_cov3Ds_precomp, cov3Ds_precomp), None)
+                g(grad_scales, scales), g(grad_rotations, rotations), g(grad_cov3Ds_precomp, cov3Ds_precomp), None, None)
 
 
 class _RasterizeGaussiansDepth(torch.autograd.Function):
     """_RasterizeGaussians with the depth image as a third, differentiable output."""
 
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):
+    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings, deterministic=False):
         rs = raster_settings
         num_rendered, color, depth, radii, geomBuffer, binningBuffer, imgBuffer = RasterizeGaussiansDepthCUDA(
             rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
@@ -235,6 +252,7 @@ class _RasterizeGaussiansDepth(torch.autograd.Function):
             rs.campos, rs.prefiltered)
         ctx.raster_settings = rs
         ctx.num_rendered = num_rendered
+        ctx.deterministic = bool(deterministic)
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
                               binningBuffer, imgBuffer)
         ctx.mark_non_differentiable(radii)
@@ -243,7 +261,8 @@ class _RasterizeGaussiansDepth(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out_color, _grad_radii, grad_out_depth):
-        _alert_not_deterministic()
+        if not ctx.deterministic:
+            _alert_not_deterministic()
         rs = ctx.raster_settings
         colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer = ctx.saved_tensors
         if grad_out_color is None:
@@ -252,18 +271,21 @@ class _RasterizeGaussiansDepth(torch.autograd.Function):
          grad_rotations) = RasterizeGaussiansBackwardDepthCUDA(
             rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix,
             rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_out_color, grad_out_depth, sh, rs.sh_degree, rs.campos, geomBuffer,
-            ctx.num_rendered, binningBuffer, imgBuffer)
+            ctx.num_rendered, binningBuffer, imgBuffer, deterministic=ctx.deterministic)
 
         def g(t, ref):
             return t if (ref is not None and ref.numel() != 0) else None
         return (grad_means3D, grad_means2D, g(grad_sh, sh), g(grad_colors_precomp, colors_precomp), grad_opacities,
-                g(grad_scales, scales), g(grad_rotations, rotations), g(grad_cov3Ds_precomp, cov3Ds_precomp), None)
+                g(grad_scales, scales), g(grad_rotations, rotations), g(grad_cov3Ds_precomp, cov3Ds_precomp), None, None)
 
 
-def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):
-    """reference rasterizeGaussians (include/gaussian_rasterizer.h:77-99)."""
+def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings, *,
+                        deterministic=False):
+    """reference rasterizeGaussians (include/gaussian_rasterizer.h:77-99). deterministic=True: the backward's gradients are
+    bit-identical from run to run (psb_rasterize_backward_deterministic), and it does not alert under
+    torch.use_deterministic_algorithms(True)."""
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                                     raster_settings)
+                                     raster_settings, deterministic)
 
 
 class GaussianRasterizer:
@@ -277,8 +299,9 @@ class GaussianRasterizer:
             return markVisible(positions, self.raster_settings.viewmatrix, self.raster_settings.projmatrix)
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
-                cov3D_precomp=None, return_depth=False):
-        """-> (color, radii), or (color, radii, depth [H,W]) with return_depth=True (differentiable, as the colour)."""
+                cov3D_precomp=None, return_depth=False, deterministic=False):
+        """-> (color, radii), or (color, radii, depth [H,W]) with return_depth=True (differentiable, as the colour).
+        deterministic=True: bit-identical gradients from run to run (see rasterize_gaussians)."""
         has = lambda t: t is not None and t.numel() != 0
         if has(shs) == has(colors_precomp):
             raise RuntimeError("Please provide excatly one of either SHs or precomputed colors!")
@@ -288,8 +311,8 @@ class GaussianRasterizer:
         e = lambda t: t if has(t) else empty
         if return_depth:
             return _RasterizeGaussiansDepth.apply(means3D, means2D, e(shs), e(colors_precomp), opacities, e(scales), e(rotations),
-                                                  e(cov3D_precomp), self.raster_settings)
+                                                  e(cov3D_precomp), self.raster_settings, deterministic)
         return rasterize_gaussians(means3D, means2D, e(shs), e(colors_precomp), opacities, e(scales), e(rotations),
-                                   e(cov3D_precomp), self.raster_settings)
+                                   e(cov3D_precomp), self.raster_settings, deterministic=deterministic)
 
     __call__ = forward

@@ -54,11 +54,12 @@ def get_covariance_activation(model, scaling_modifier=1.0):
 
 
 def render(viewpoint_camera, image_height, image_width, pc, pipe=None, bg_color=None, override_color=None, scaling_modifier=1.0,
-           use_override_color=False, return_depth=False):
+           use_override_color=False, return_depth=False, deterministic=False):
     """viewpoint_camera: dict(viewmatrix, projmatrix, campos: device tensors; tanfovx, tanfovy) — the fields of GaussianKeyframe the
     reference reads (world_view_transform_, full_proj_transform_, camera_center_, FoVx_/FoVy_ as tangents). pc: trainer.GaussianModel.
     return_depth=True appends the rendered depth [H,W] (include/psb200.h: sum z alpha T, no background term) to the tuple, in every
-    branch; gradients flow through it like through the image."""
+    branch; gradients flow through it like through the image. deterministic=True: the rasterizer's backward is bit-identical from run to
+    run (GaussianRasterizer.forward), so are the gradients it sends into the model tensors and viewspace_points."""
     pipe = pipe or GaussianPipelineParams()
     dev = pc.xyz_.device
     bg_color = bg_color if bg_color is not None else torch.zeros(3, device=dev)
@@ -88,8 +89,9 @@ def render(viewpoint_camera, image_height, image_width, pc, pipe=None, bg_color=
         shs = get_features(pc)
     if return_depth:
         rendered_image, radii, depth = rasterizer(means3D, means2D, opacity, shs=shs, colors_precomp=colors_precomp, scales=scales,
-                                                  rotations=rotations, cov3D_precomp=cov3D_precomp, return_depth=True)
+                                                  rotations=rotations, cov3D_precomp=cov3D_precomp, return_depth=True,
+                                                  deterministic=deterministic)
         return rendered_image, screenspace_points, radii > 0, radii, depth
     rendered_image, radii = rasterizer(means3D, means2D, opacity, shs=shs, colors_precomp=colors_precomp, scales=scales, rotations=rotations,
-                                       cov3D_precomp=cov3D_precomp)
+                                       cov3D_precomp=cov3D_precomp, deterministic=deterministic)
     return rendered_image, screenspace_points, radii > 0, radii
