@@ -146,6 +146,50 @@ int psb_rasterize_backward_deterministic(int P, int D, int M, int R,
                                          const float* dL_ddepth, float* dL_dz, void* det_scratch, size_t det_scratch_bytes,
                                          void* stream);
 
+/*
+ * Anti-aliasing on the operator path (the 2D Mip filter of Mip-Splatting, upstream diff-gaussian-rasterization's `antialiasing`).
+ * With (a0, b, c0) the 2D covariance of a visible Gaussian before the 0.3 px^2 dilation, det0 = a0 c0 - b^2 and det1 the
+ * determinant after it, h = sqrt(max(det0 / det1, 2.5e-5)) in [0.005, 1] and the splat blends with opacity o' = o h. A splat that
+ * the dilation widens keeps the energy it had before, so small splats do not brighten at low resolution. Conic, radius, tile
+ * rectangle, depth key, colour and clamp bits are unchanged, so radii, num_rendered, the sorted keys and values and the ranges are
+ * bit-identical with antialiasing on and off; the exported conic_opacity[:, 3] (psb_debug_export) is o'.
+ *
+ * psb_rasterize_forward_aa: the argument list of psb_rasterize_forward_depth plus `antialiasing` (0 or 1) before the stream.
+ * out_depth may be NULL. antialiasing = 0 is psb_rasterize_forward_depth bit for bit.
+ *
+ * psb_rasterize_backward_aa: the argument list of psb_rasterize_backward_deterministic plus `antialiasing` before the stream, for the
+ * scratch of a psb_rasterize_forward_aa with the same flag. det_scratch == NULL selects the atomic backward (det_scratch_bytes is then
+ * ignored), dL_ddepth == NULL means colour only. With antialiasing = 1, dL_dopacity receives dL/do (h dL/do'), and dL/dh joins the
+ * covariance gradient (dL_dcov3D, dL_dscale, dL_drot, dL_dmean3D). antialiasing = 0 is psb_rasterize_backward_deterministic (or,
+ * without det_scratch, psb_rasterize_backward_depth) bit for bit. No opacity argument is needed: o' is in the geometry scratch.
+ *
+ * Both return PSB_ERR_ARG, before any CUDA call, for an antialiasing value other than 0 or 1 and for everything the calls they extend
+ * reject. The scratch sizes (psb_*_bytes, psb_rasterize_backward_det_bytes) do not change.
+ */
+int psb_rasterize_forward_aa(psb_alloc_fn geometry_buffer, void* geometry_user,
+                             psb_alloc_fn binning_buffer, void* binning_user,
+                             psb_alloc_fn image_buffer, void* image_user,
+                             int P, int D, int M,
+                             const float* background, int width, int height,
+                             const float* means3D, const float* shs, const float* colors_precomp,
+                             const float* opacities, const float* scales, float scale_modifier,
+                             const float* rotations, const float* cov3D_precomp,
+                             const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                             float tan_fovx, float tan_fovy, int prefiltered,
+                             float* out_color, int* radii, float* out_depth, int antialiasing, void* stream);
+int psb_rasterize_backward_aa(int P, int D, int M, int R,
+                              const float* background, int width, int height,
+                              const float* means3D, const float* shs, const float* colors_precomp,
+                              const float* scales, float scale_modifier, const float* rotations,
+                              const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix,
+                              const float* campos, float tan_fovx, float tan_fovy, const int* radii,
+                              char* geom_buffer, char* binning_buffer, char* image_buffer,
+                              const float* dL_dpix,
+                              float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                              float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
+                              const float* dL_ddepth, float* dL_dz, void* det_scratch, size_t det_scratch_bytes,
+                              int antialiasing, void* stream);
+
 /* Near-plane visibility (view z > 0.2). Replaces CudaRasterizer::Rasterizer::markVisible
  * (cuda_rasterizer/rasterizer.h:24-29, rasterizer_impl.cu:141-153). present: [P] bytes (bool), device. */
 int psb_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,
@@ -280,7 +324,7 @@ typedef struct psb_pixel_grads {
  * Contract: `pass` is the context's latest forward pass, made by psb_trainer_forward (or psb_trainer_render / _render_depth), and
  * model, camera and background are those of that pass (the model's parameters must not change in between). PSB_ERR_ARG when `pass`
  * is not the latest pass, when the latest pass was a training call (step, backward, _begin: it has had its backward), when
- * psb_trainer_result regrew the arena since, when P, the image size or step->sh_degree differ from that pass, when the deterministic mode was switched in between, for a
+ * psb_trainer_result regrew the arena since, when P, the image size or step->sh_degree differ from that pass, when the deterministic or the anti-aliasing mode was switched in between, for a
  * NULL dL_dcolor and for misaligned gradient segments. A pass that overflowed the binning arena makes this call a no-op on the model
  * and on grads' rows; psb_trainer_result reports PSB_ERR_RETRY for it. psb_trainer_result after this call reports the status and
  * the instance count only: out3 is left untouched. Stage timing: stage "loss" is the stream time between the two calls.
@@ -358,7 +402,8 @@ int psb_dp_params(psb_dp* dp, float** out6);                   /* device address
  * owners -> (device-side wait for every rank's records) -> Adam of the owned rows, updated rows stored to every rank.
  * Asynchronous: no host synchronisation, every cross-rank dependency is a device-side wait on an epoch flag. A view
  * whose binning arena overflows contributes a zero gradient to the step (psb_trainer_result still reports
- * PSB_ERR_RETRY and grows the arena): the replicas stay identical and no rank waits forever. */
+ * PSB_ERR_RETRY and grows the arena): the replicas stay identical and no rank waits forever. Every rank must run with the same
+ * psb_trainer_set_antialiasing mode: the records of an anti-aliased view differentiate o' = o h, and the owner adds them as they are. */
 int psb_dp_step(psb_trainer* t, psb_dp* dp, int P, int M, const psb_model* model, const psb_camera* camera,
                 const float* background, const float* gt_image, const float* mask, const psb_step* step,
                 float* out_color, int* radii, void* stream);
@@ -414,6 +459,16 @@ int psb_trainer_stage_times(psb_trainer* t, float* ms, int n);
  * The operator path has its own entry point, psb_rasterize_backward_deterministic. Not covered: the NCCL all-reduce that a caller runs between
  * psb_trainer_backward* and psb_adam_update: each rank's gradients are deterministic, the all-reduce's order is NCCL's. */
 int psb_trainer_set_deterministic(psb_trainer* t, int enable);
+
+/* Anti-aliasing mode of a context (off by default; PSB_ERR_ARG for a NULL context): while it is on, every pass of the context blends
+ * each splat with o' = o h, the 2D Mip filter defined for psb_rasterize_forward_aa, and every backward behind such a pass
+ * differentiates it (dL/do = h dL/do', dL/dh into the covariance gradient). It covers psb_trainer_render(_depth),
+ * psb_trainer_forward, psb_trainer_step(_depth), psb_trainer_backward(_depth), psb_trainer_backward_begin(_depth) +
+ * psb_trainer_backward_slab (the slabs follow the mode of their _begin), psb_trainer_backward_pixels and psb_dp_step(_depth), with no
+ * new signatures, and combines with the deterministic mode. The mode is read when a pass starts; psb_trainer_backward_pixels refuses
+ * a pass whose mode was switched after it. Every rank of a psb_dp_step must set the same mode (the owner-side Adam sums the ranks'
+ * records as they are). With o' < o the tight instance lists can only get shorter. */
+int psb_trainer_set_antialiasing(psb_trainer* t, int enable);
 
 /* Stand-alone fused loss (tests / evaluation): L = (1-lambda) L1 + lambda (1 - SSIM), reference
  * include/loss_utils.h:28-124. image/gt/mask/dL_dimage device [3,H,W] (mask, dL_dimage may be NULL);

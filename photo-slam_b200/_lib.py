@@ -47,6 +47,11 @@ def lib():
     L.psb_rasterize_backward_det_bytes.argtypes = [C.c_int, C.c_int]
     L.psb_rasterize_backward_deterministic.restype = C.c_int
     L.psb_rasterize_backward_deterministic.argtypes = L.psb_rasterize_backward_depth.argtypes[:-1] + [vp, C.c_size_t, vp]
+    # anti-aliasing: the _depth forward's and the deterministic backward's argument lists plus `antialiasing`, before the stream
+    L.psb_rasterize_forward_aa.restype = C.c_int
+    L.psb_rasterize_forward_aa.argtypes = L.psb_rasterize_forward_depth.argtypes[:-1] + [C.c_int, vp]
+    L.psb_rasterize_backward_aa.restype = C.c_int
+    L.psb_rasterize_backward_aa.argtypes = L.psb_rasterize_backward_deterministic.argtypes[:-1] + [C.c_int, vp]
     L.psb_mark_visible.restype = C.c_int
     L.psb_mark_visible.argtypes = [C.c_int, fp, fp, fp, u8p, vp]
     L.psb_debug_export.restype = C.c_int

@@ -72,7 +72,7 @@ static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void*
                              const float* means3D, const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
                              float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
                              const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered, float* out_color,
-                             int* radii, float* out_depth, void* stream_)
+                             int* radii, float* out_depth, void* stream_, bool aa = false)
 {
 	(void)prefiltered;  // the reference only uses it for a device-side assert (auxiliary.h:156-160)
 	cudaStream_t stream = (cudaStream_t)stream_;
@@ -95,7 +95,7 @@ static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void*
 
 	const GaussIn in = make_input(P, D, M, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp);
 	int rc;
-	if ((rc = launch_preprocess(in, cam, radii, geom, /*raw=*/false, /*tight=*/false, stream))) return rc;
+	if ((rc = launch_preprocess(in, cam, radii, geom, /*raw=*/false, /*tight=*/false, stream, aa))) return rc;
 	if ((rc = launch_depth_sort_and_scan(P, geom, /*scan=*/true, stream))) return rc;
 
 	uint32_t num_rendered = 0;
@@ -126,7 +126,7 @@ static int rasterize_backward(const char* fn, int P, int D, int M, int R, const 
                               float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer, const float* dL_dpix,
                               float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dmean3D, float* dL_dcov3D,
                               float* dL_dsh, float* dL_dscale, float* dL_drot, const float* dL_ddepth, float* dL_dz, void* stream_,
-                              bool det = false, void* det_scratch = nullptr, size_t det_bytes = 0)
+                              bool det = false, void* det_scratch = nullptr, size_t det_bytes = 0, bool aa = false)
 {
 	(void)radii;  // visibility is re-derived from the private geometry state (tiles_touched), identical to radii > 0
 	cudaStream_t stream = (cudaStream_t)stream_;
@@ -171,7 +171,10 @@ static int rasterize_backward(const char* fn, int P, int D, int M, int R, const 
 	const GaussIn in = make_input(P, D, M, means3D, shs, colors_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp);
 	GaussGradOut out;
 	out.dL_dmeans3D = dL_dmean3D; out.dL_dcov3D = dL_dcov3D; out.dL_dsh = dL_dsh; out.dL_dscales = dL_dscale; out.dL_drots = dL_drot;
-	if ((rc = launch_preprocess_backward(in, cam, geom, dL_dmean2D, 3, dL_dconic, 4, dL_dcolor, 3, out, stream, dL_ddepth ? dL_dz : nullptr))) return rc;
+	// (AA: dL_dopacity holds dL/do' here, the per-Gaussian kernel turns it into dL/do)
+	if ((rc = launch_preprocess_backward(in, cam, geom, dL_dmean2D, 3, dL_dconic, 4, dL_dcolor, 3, out, stream, dL_ddepth ? dL_dz : nullptr,
+	                                     aa ? dL_dopacity : nullptr)))
+		return rc;
 	return 0;
 }
 
@@ -256,6 +259,36 @@ int psb_rasterize_backward_deterministic(int P, int D, int M, int R, const float
 	                          scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, radii, geom_buffer,
 	                          binning_buffer, image_buffer, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh,
 	                          dL_dscale, dL_drot, dL_ddepth, dL_dz, stream, /*det=*/true, det_scratch, det_scratch_bytes);
+}
+
+int psb_rasterize_forward_aa(psb_alloc_fn geometry_buffer, void* geometry_user, psb_alloc_fn binning_buffer, void* binning_user,
+                             psb_alloc_fn image_buffer, void* image_user, int P, int D, int M, const float* background, int width, int height,
+                             const float* means3D, const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
+                             float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
+                             const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered, float* out_color,
+                             int* radii, float* out_depth, int antialiasing, void* stream)
+{
+	if (antialiasing != 0 && antialiasing != 1) return arg_error("psb_rasterize_forward_aa", "antialiasing must be 0 or 1");
+	return rasterize_forward("psb_rasterize_forward_aa", geometry_buffer, geometry_user, binning_buffer, binning_user, image_buffer, image_user, P, D,
+	                         M, background, width, height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp,
+	                         viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, out_depth, stream, antialiasing != 0);
+}
+
+int psb_rasterize_backward_aa(int P, int D, int M, int R, const float* background, int width, int height, const float* means3D, const float* shs,
+                              const float* colors_precomp, const float* scales, float scale_modifier, const float* rotations,
+                              const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix, const float* campos, float tan_fovx,
+                              float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer, const float* dL_dpix,
+                              float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dmean3D, float* dL_dcov3D,
+                              float* dL_dsh, float* dL_dscale, float* dL_drot, const float* dL_ddepth, float* dL_dz, void* det_scratch,
+                              size_t det_scratch_bytes, int antialiasing, void* stream)
+{
+	const char* fn = "psb_rasterize_backward_aa";
+	if (antialiasing != 0 && antialiasing != 1) return arg_error(fn, "antialiasing must be 0 or 1");
+	if (dL_ddepth && !dL_dz) return arg_error(fn, "dL_ddepth needs a dL_dz array");
+	return rasterize_backward(fn, P, D, M, R, background, width, height, means3D, shs, colors_precomp, scales, scale_modifier, rotations, cov3D_precomp,
+	                          viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dmean2D,
+	                          dL_dconic, dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_ddepth, dL_dz, stream,
+	                          /*det=*/det_scratch != nullptr, det_scratch, det_scratch_bytes, antialiasing != 0);
 }
 
 int psb_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix, unsigned char* present, void* stream_)

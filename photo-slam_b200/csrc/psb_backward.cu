@@ -10,11 +10,13 @@ namespace psb {
 
 // DEPTH: dL/dz (view-space depth, render_bwd_depth_kernel's tenth sum) joins dL/dmean3D through the view matrix's z row,
 // z = V[2] x + V[6] y + V[10] z + V[14] (column-major), as in gaussian_backward_kernel<MODE_DEPTH>.
-template <bool DEPTH>
+// AA: the forward blended o' = o h (preprocess_fwd_kernel<false, true>, o' in the record). dL_dopacity [P] holds dL/do' from the tile
+// backward (atomic or gathered); the h-term joins the covariance gradient and dL_dopacity[g] is rescaled in place to dL/do = h dL/do'.
+template <bool DEPTH, bool AA = false>
 __device__ __forceinline__ void preprocess_bwd_body(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
                                                     int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
                                                     const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out,
-                                                    const float* __restrict__ dL_dz)
+                                                    const float* __restrict__ dL_dz, float* __restrict__ dL_dopacity = nullptr)
 {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	if (idx >= in.P || geom.tile_info[idx].z == 0) return;
@@ -43,7 +45,11 @@ __device__ __forceinline__ void preprocess_bwd_body(GaussIn in, Camera cam, Geom
 	float3 dL_dmean, dL_dscale = make_float3(0, 0, 0);
 	float4 dL_drot = make_float4(0, 0, 0, 0);
 	float dL_dcov[6];
-	gaussian_backward(in, cam, idx, mean, cov3D, scale, rot, sh_row, clamp_bits, g2, gc, gcol, dsh_row, dL_dmean, dL_dcov, dL_dscale, dL_drot);
+	float aa_h = 1.f;
+	const float dL_dop = AA ? dL_dopacity[idx] : 0.f;
+	gaussian_backward<AA>(in, cam, idx, mean, cov3D, scale, rot, sh_row, clamp_bits, g2, gc, gcol, dsh_row, dL_dmean, dL_dcov, dL_dscale, dL_drot,
+	                      AA ? geom.rec[idx].q1.y : 0.f, dL_dop, &aa_h);
+	if (AA) dL_dopacity[idx] = aa_h * dL_dop;
 	if (DEPTH) {
 		const float dz = dL_dz[idx];
 		dL_dmean.x += dz * cam.view[2]; dL_dmean.y += dz * cam.view[6]; dL_dmean.z += dz * cam.view[10];
@@ -75,12 +81,36 @@ __global__ void __launch_bounds__(128) preprocess_bwd_depth_kernel(GaussIn in, C
 	preprocess_bwd_body<true>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out, dL_dz);
 }
 
+__global__ void __launch_bounds__(128) preprocess_bwd_aa_kernel(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
+                                                                int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
+                                                                const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out,
+                                                                float* __restrict__ dL_dopacity)
+{
+	preprocess_bwd_body<false, true>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out, nullptr,
+	                                 dL_dopacity);
+}
+
+__global__ void __launch_bounds__(128) preprocess_bwd_depth_aa_kernel(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
+                                                                      int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
+                                                                      const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out,
+                                                                      const float* __restrict__ dL_dz, float* __restrict__ dL_dopacity)
+{
+	preprocess_bwd_body<true, true>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out, dL_dz,
+	                                dL_dopacity);
+}
+
 int launch_preprocess_backward(const GaussIn& in, const Camera& cam, const GeomState& geom, const float* dL_dmean2D, int mean2D_stride,
                                const float* dL_dconic, int conic_stride, const float* dL_dcolor, int color_stride,
-                               const GaussGradOut& out, cudaStream_t stream, const float* dL_dz)
+                               const GaussGradOut& out, cudaStream_t stream, const float* dL_dz, float* aa_dL_dopacity)
 {
 	if (in.P == 0) return 0;
-	if (dL_dz)
+	if (aa_dL_dopacity && dL_dz)
+		preprocess_bwd_depth_aa_kernel<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor,
+		                                                                    color_stride, out, dL_dz, aa_dL_dopacity);
+	else if (aa_dL_dopacity)
+		preprocess_bwd_aa_kernel<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor,
+		                                                              color_stride, out, aa_dL_dopacity);
+	else if (dL_dz)
 		preprocess_bwd_depth_kernel<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor,
 		                                                                 color_stride, out, dL_dz);
 	else

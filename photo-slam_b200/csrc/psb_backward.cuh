@@ -143,8 +143,13 @@ __device__ __forceinline__ void cov3d_backward(const float3 scale, float mod, co
 
 // Projection part of the per-Gaussian backward: (dL/dmean2D, dL/dconic) -> dL/dcov3D[6] and the covariance- and
 // projection-induced parts of dL/dmean3D (reference backward.cu:155-273 and :366-387).
+// AA (anti-aliasing, see preprocess_fwd_kernel): the blend used o' = o h. With aa_dL_dop = dL/do' and aa_o = o (or o' when aa_o_is_prime),
+// dL/dh = o dL/do' joins dL/d(a, b, c) through dh/d(a0, b, c0) (0 where the clamp of h is active); *aa_h receives h, so the caller can
+// form dL/do = h dL/do'.
+template <bool AA = false>
 __device__ __forceinline__ void gaussian_backward_geom(const Camera& cam, const float3 mean, const float* cov3D, const float2 dL_dmean2D,
-                                                       const float3 dL_dconic, float3& dL_dmean, float* dL_dcov)
+                                                       const float3 dL_dconic, float3& dL_dmean, float* dL_dcov, float aa_o = 0.f,
+                                                       float aa_dL_dop = 0.f, bool aa_o_is_prime = false, float* aa_h = nullptr)
 {
 	Cov2DTerms ct;
 	cov2d_terms(mean, cam.focal_x, cam.focal_y, cam.tan_fovx, cam.tan_fovy, cov3D, cam.view, ct);
@@ -162,6 +167,20 @@ __device__ __forceinline__ void gaussian_backward_geom(const Camera& cam, const 
 		dL_da = denom2inv * (-c * c * dL_dconic.x + 2 * b * c * dL_dconic.y + (denom - a * c) * dL_dconic.z);
 		dL_dc = denom2inv * (-a * a * dL_dconic.z + 2 * a * b * dL_dconic.y + (denom - a * c) * dL_dconic.x);
 		dL_db = denom2inv * 2 * (b * c * dL_dconic.x - (denom + 2 * b * b) * dL_dconic.y + a * b * dL_dconic.z);
+		if (AA) {
+			// h = sqrt(det0 / det1): dh/da0 = h/2 (c0/det0 - c1/det1), dh/dc0 = h/2 (a0/det0 - a1/det1), dh/db = h b (1/det1 - 1/det0)
+			const float a0 = ct.cov(0, 0), c0 = ct.cov(1, 1);
+			const float det0 = aa_det0(ct);
+			const float h = aa_factor(det0, denom);
+			*aa_h = h;
+			if (det0 / denom > kAaMinRatio) {
+				const float dL_dh = (aa_o_is_prime ? aa_o / h : aa_o) * aa_dL_dop;
+				const float i0 = 1.f / det0, i1 = 1.f / denom;
+				dL_da += dL_dh * (0.5f * h * (c0 * i0 - c * i1));
+				dL_dc += dL_dh * (0.5f * h * (a0 * i0 - a * i1));
+				dL_db += dL_dh * (h * b * (i1 - i0));
+			}
+		}
 		dL_dcov[0] = (T(0, 0) * T(0, 0) * dL_da + T(0, 0) * T(1, 0) * dL_db + T(1, 0) * T(1, 0) * dL_dc);
 		dL_dcov[3] = (T(0, 1) * T(0, 1) * dL_da + T(0, 1) * T(1, 1) * dL_db + T(1, 1) * T(1, 1) * dL_dc);
 		dL_dcov[5] = (T(0, 2) * T(0, 2) * dL_da + T(0, 2) * T(1, 2) * dL_db + T(1, 2) * T(1, 2) * dL_dc);
@@ -215,15 +234,17 @@ __device__ __forceinline__ void gaussian_backward_geom(const Camera& cam, const 
 }
 
 // Everything between the 9 screen-space sums and the activated 3D parameters, for one visible Gaussian
-// (row-pointer SH layout [M][3]; dL/dsh written through the pointer if non-null).
+// (row-pointer SH layout [M][3]; dL/dsh written through the pointer if non-null). AA: as gaussian_backward_geom, with aa_o = o'.
+template <bool AA = false>
 __device__ __forceinline__ void gaussian_backward(const GaussIn& in, const Camera& cam, int idx, const float3 mean, const float* cov3D,
                                                   const float3 scale, const float4 rot, const float* __restrict__ sh_row,
                                                   uint32_t clamp_bits, const float2 dL_dmean2D, const float3 dL_dconic,
                                                   const float3 dL_dcolor, float* __restrict__ dL_dsh_row, float3& dL_dmean, float* dL_dcov,
-                                                  float3& dL_dscale, float4& dL_drot)
+                                                  float3& dL_dscale, float4& dL_drot, float aa_o_prime = 0.f, float aa_dL_dop = 0.f,
+                                                  float* aa_h = nullptr)
 {
 	(void)idx;
-	gaussian_backward_geom(cam, mean, cov3D, dL_dmean2D, dL_dconic, dL_dmean, dL_dcov);
+	gaussian_backward_geom<AA>(cam, mean, cov3D, dL_dmean2D, dL_dconic, dL_dmean, dL_dcov, aa_o_prime, aa_dL_dop, true, aa_h);
 	if (sh_row) {
 		const float3 campos = make_float3(cam.campos[0], cam.campos[1], cam.campos[2]);
 		const float3 dsh = sh_backward(in.D, mean, campos, sh_row, clamp_bits, dL_dcolor, dL_dsh_row);

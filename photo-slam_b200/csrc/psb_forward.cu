@@ -24,10 +24,14 @@ namespace psb {
 // RAW = true: inputs are the raw trainer parameters (log-scales, unnormalised quaternions, opacity
 // logits, SH split into dc/rest); the activations of reference gaussian_model.cpp:48-71 are applied
 // here instead of by five separate elementwise kernels and a 192 B/Gaussian concatenation.
+// AA = true: anti-aliasing (Mip-Splatting's 2D filter, upstream diff-gaussian-rasterization's `antialiasing`): the splat blends with
+// opacity o' = o h, h = sqrt(max(det0 / det1, 2.5e-5)), det0 / det1 the determinants of the 2D covariance before / after the 0.3 px^2
+// dilation. Conic, radius, tile rectangle, depth key, colour and clamp bits are those of AA = false; the record, pmin and the tight
+// tile cull all see o'.
 // ------------------------------------------------------------------------------------------------
 constexpr int PRE_TB = 128;  // Gaussians per block
 
-template <bool RAW>
+template <bool RAW, bool AA = false>
 __global__ void __launch_bounds__(PRE_TB) preprocess_fwd_kernel(GaussIn in, Camera cam, int* __restrict__ radii_out, GeomState geom, int tight)
 {
 	// SH rows of this block's Gaussians ([128][45] raw f_rest rows or [128][48] activated rows), one TMA bulk copy per block:
@@ -85,6 +89,7 @@ __global__ void __launch_bounds__(PRE_TB) preprocess_fwd_kernel(GaussIn in, Came
 	float3 p_view = make_float3(0, 0, 0), conic = make_float3(0, 0, 0);
 	float2 point_image = make_float2(0, 0);
 	float my_radius = 0.f;
+	float aa_h = 1.f;  // AA: the opacity factor h
 	int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
 	if (alive) {
 		p_view = xform4x3(p_orig, cam.view);
@@ -106,6 +111,7 @@ __global__ void __launch_bounds__(PRE_TB) preprocess_fwd_kernel(GaussIn in, Came
 
 		Cov2DTerms ct;
 		cov2d_terms(p_orig, cam.focal_x, cam.focal_y, cam.tan_fovx, cam.tan_fovy, cov3D, cam.view, ct);
+		const float det0 = AA ? aa_det0(ct) : 0.f;
 		ct.cov(0, 0) += 0.3f;
 		ct.cov(1, 1) += 0.3f;
 		const float3 cov = make_float3(float(ct.cov(0, 0)), float(ct.cov(0, 1)), float(ct.cov(1, 1)));
@@ -113,6 +119,7 @@ __global__ void __launch_bounds__(PRE_TB) preprocess_fwd_kernel(GaussIn in, Came
 		const float det = (cov.x * cov.z - cov.y * cov.y);
 		alive = det != 0.0f;
 		if (alive) {
+			if (AA) aa_h = aa_factor(det0, det);
 			const float det_inv = 1.f / det;
 			conic = make_float3(cov.z * det_inv, -cov.y * det_inv, cov.x * det_inv);
 
@@ -158,6 +165,7 @@ __global__ void __launch_bounds__(PRE_TB) preprocess_fwd_kernel(GaussIn in, Came
 	}
 
 	if (RAW) opacity = 1.0f / (1.0f + expf(-opacity));
+	if (AA) opacity *= aa_h;
 
 	const int radius_i = (int)my_radius;
 	GaussRec r;
@@ -479,11 +487,13 @@ __global__ void __launch_bounds__(256) tile_ranges_kernel(const uint32_t* __rest
 // ------------------------------------------------------------------------------------------------
 // Host orchestration
 // ------------------------------------------------------------------------------------------------
-int launch_preprocess(const GaussIn& in, const Camera& cam, int* radii_out, const GeomState& geom, bool raw, bool tight, cudaStream_t stream)
+int launch_preprocess(const GaussIn& in, const Camera& cam, int* radii_out, const GeomState& geom, bool raw, bool tight, cudaStream_t stream, bool aa)
 {
 	if (in.P == 0) return 0;
 	const int grid = cdiv(in.P, PRE_TB);
-	if (raw) preprocess_fwd_kernel<true><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tight ? 1 : 0);
+	if (aa && raw) preprocess_fwd_kernel<true, true><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tight ? 1 : 0);
+	else if (aa) preprocess_fwd_kernel<false, true><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tight ? 1 : 0);
+	else if (raw) preprocess_fwd_kernel<true><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tight ? 1 : 0);
 	else preprocess_fwd_kernel<false><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tight ? 1 : 0);
 	PSB_LAUNCH_OK();
 	return 0;

@@ -77,6 +77,12 @@ __device__ __forceinline__ void cov2d_terms(const float3 mean, float focal_x, fl
 	o.t = t;
 }
 
+// Anti-aliasing (2D Mip filter): the splat's opacity is scaled by h = sqrt(max(det0 / det1, 2.5e-5)), in [0.005, 1], where det0 is the
+// determinant of the 2D covariance before the 0.3 px^2 dilation (this function, on cov2d_terms' output) and det1 the one after it.
+__device__ __forceinline__ float aa_det0(const Cov2DTerms& ct) { return ct.cov(0, 0) * ct.cov(1, 1) - ct.cov(0, 1) * ct.cov(0, 1); }
+constexpr float kAaMinRatio = 2.5e-5f;
+__device__ __forceinline__ float aa_factor(float det0, float det1) { return sqrtf(fmaxf(det0 / det1, kAaMinRatio)); }
+
 // SH (degree <= 3) -> RGB for one Gaussian, all three channels; sh points at this Gaussian's
 // [M][3] coefficient row (forward.cu:20-71). Returns colour after +0.5 and clamp at 0; `clamp_bits`
 // bit c set when channel c was clamped.

@@ -81,7 +81,10 @@ inline int sorted_slot(int width, int height)
 }
 
 // tight: instance lists hold only the tiles a splat can reach (trainer path; see preprocess_fwd_kernel) — pass the same flag to launch_scan_binning
-int launch_preprocess(const GaussIn& in, const Camera& cam, int* radii_out, const GeomState& geom, bool raw, bool tight, cudaStream_t stream);
+// aa: anti-aliasing (the 2D Mip filter: the record holds o' = o h, see preprocess_fwd_kernel); pair it with the AA variant of the
+// per-Gaussian backward that follows
+int launch_preprocess(const GaussIn& in, const Camera& cam, int* radii_out, const GeomState& geom, bool raw, bool tight, cudaStream_t stream,
+                      bool aa = false);
 int launch_mark_visible(int P, const float* means3D, const float* view, uint8_t* present, cudaStream_t stream);
 int launch_depth_sort_and_scan(int P, GeomState& geom, bool scan, cudaStream_t stream);
 int launch_binning(int P, const Camera& cam, const GeomState& geom, BinState& bin, const ImgState& img, size_t n_host, cudaStream_t stream);
@@ -102,8 +105,9 @@ int launch_render_backward(const Camera& cam, const uint2* ranges, const uint32_
                            const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, const GradSink& sink,
                            cudaStream_t stream, const float* dL_ddepth = nullptr, const DetSlots* det = nullptr, const float* dL_dalpha = nullptr);
 // dL_dz [P] (non-null: depth variant): dL/dmean3D += dL/dz (V[2], V[6], V[10]) for every visible Gaussian
+// aa_dL_dopacity [P] (non-null: AA variant, after an anti-aliased forward): holds dL/do' on entry, dL/do on return
 int launch_preprocess_backward(const GaussIn& in, const Camera& cam, const GeomState& geom, const float* dL_dmean2D, int mean2D_stride,
                                const float* dL_dconic, int conic_stride, const float* dL_dcolor, int color_stride,
-                               const GaussGradOut& out, cudaStream_t stream, const float* dL_dz = nullptr);
+                               const GaussGradOut& out, cudaStream_t stream, const float* dL_dz = nullptr, float* aa_dL_dopacity = nullptr);
 
 }  // namespace psb

@@ -44,6 +44,8 @@ constexpr int MODE_ADAM_LIVE = 3;  // MODE_ADAM with the caller's per-row live b
                                    // reached by a gradient are not read beyond that byte and the visibility word
 constexpr int MODE_DEPTH = 8;      // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE / MODE_PUSH: slot 11 of the sink row holds dL/dz (view-space depth,
                                    // render_bwd_depth_kernel) and joins dL/dxyz through the view matrix's z row
+constexpr int MODE_AA = 16;        // OR'd into any of the above: the forward was anti-aliased (o' = o h, preprocess_fwd_kernel<true, true>), slot 7
+                                   // holds dL/do'; dL/dh joins the covariance gradient and the opacity gradient is h dL/do' sigma'
 
 // torch::optim::Adam single-tensor update (LibTorch adam.cpp): exp_avg.mul_(b1).add_(g, 1-b1);
 // exp_avg_sq.mul_(b2).addcmul_(g, g, 1-b2); denom = exp_avg_sq.sqrt()/sqrt(bc2) + eps; p.addcdiv_(exp_avg, denom, -lr/bc1).
@@ -170,7 +172,8 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
                                                             DpPush dp, unsigned char* __restrict__ adam_live)
 {
 	constexpr bool DEPTH = (MODE & MODE_DEPTH) != 0;
-	constexpr int BASE = MODE & ~MODE_DEPTH;
+	constexpr bool AA = (MODE & MODE_AA) != 0;
+	constexpr int BASE = MODE & ~(MODE_DEPTH | MODE_AA);
 	constexpr bool LIVE = BASE == MODE_ADAM_LIVE;
 	constexpr bool ADAM = BASE == MODE_ADAM || LIVE;
 	__shared__ __align__(128) float s_p[TB * REST];  // f_rest parameter rows of this block (TMA destination; LIVE: compacted per warp)
@@ -296,7 +299,8 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 			const float sig = 1.0f / (1.0f + expf(-oraw));
 			float cov3D[6], dL_dcov[6];
 			cov3d_from_scale_rot(s, 1.0f, q, cov3D);
-			gaussian_backward_geom(cam, mean, cov3D, dL_dmean2D, dL_dconic, g_xyz, dL_dcov);
+			float aa_h = 1.f;  // AA: dL/dh = sigma dL/do'
+			gaussian_backward_geom<AA>(cam, mean, cov3D, dL_dmean2D, dL_dconic, g_xyz, dL_dcov, sig, dL_dopacity, false, &aa_h);
 			float3 dL_dscale;
 			float4 dL_drot;
 			cov3d_backward(s, 1.0f, q, dL_dcov, dL_dscale, dL_drot);
@@ -304,7 +308,7 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 			g_scale = make_float3(dL_dscale.x * s.x, dL_dscale.y * s.y, dL_dscale.z * s.z);
 			const float qd = q.x * dL_drot.x + q.y * dL_drot.y + q.z * dL_drot.z + q.w * dL_drot.w;
 			g_rot = make_float4((dL_drot.x - q.x * qd) / qn, (dL_drot.y - q.y * qd) / qn, (dL_drot.z - q.z * qd) / qn, (dL_drot.w - q.w * qd) / qn);
-			g_opac = dL_dopacity * sig * (1.0f - sig);
+			g_opac = (AA ? aa_h * dL_dopacity : dL_dopacity) * sig * (1.0f - sig);
 			if (DEPTH) {  // z = V[2] x + V[6] y + V[10] z + V[14] (column-major view matrix)
 				const float dz = s2.w;
 				g_xyz.x += dz * cam.view[2]; g_xyz.y += dz * cam.view[6]; g_xyz.z += dz * cam.view[10];
@@ -676,7 +680,7 @@ void run_gaussian_backward(int first, int P, cudaStream_t stream, Args... args)
 	gaussian_backward_kernel<MODE><<<cdiv(P - first, TB), TB, 0, stream>>>(first, P, args...);
 }
 
-// Gaussians [first, P) in mode `mode` (MODE_GRADS, MODE_ADAM, MODE_ADAM_LIVE or MODE_PUSH, each optionally | MODE_DEPTH)
+// Gaussians [first, P) in mode `mode` (MODE_GRADS, MODE_ADAM, MODE_ADAM_LIVE or MODE_PUSH, each optionally | MODE_DEPTH and | MODE_AA)
 int launch_gaussian_backward(int mode, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink,
                              const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
                              float* seeds, const DpPush& dp, unsigned char* adam_live, cudaStream_t stream)
@@ -695,6 +699,14 @@ int launch_gaussian_backward(int mode, int first, int P, const TrainTensors& t, 
 		PSB_BACKWARD_CASE(MODE_ADAM | MODE_DEPTH);
 		PSB_BACKWARD_CASE(MODE_ADAM_LIVE | MODE_DEPTH);
 		PSB_BACKWARD_CASE(MODE_PUSH | MODE_DEPTH);
+		PSB_BACKWARD_CASE(MODE_GRADS | MODE_AA);
+		PSB_BACKWARD_CASE(MODE_ADAM | MODE_AA);
+		PSB_BACKWARD_CASE(MODE_ADAM_LIVE | MODE_AA);
+		PSB_BACKWARD_CASE(MODE_PUSH | MODE_AA);
+		PSB_BACKWARD_CASE(MODE_GRADS | MODE_DEPTH | MODE_AA);
+		PSB_BACKWARD_CASE(MODE_ADAM | MODE_DEPTH | MODE_AA);
+		PSB_BACKWARD_CASE(MODE_ADAM_LIVE | MODE_DEPTH | MODE_AA);
+		PSB_BACKWARD_CASE(MODE_PUSH | MODE_DEPTH | MODE_AA);
 		default: set_error_msg("launch_gaussian_backward: unknown mode"); return -1;
 	}
 #undef PSB_BACKWARD_CASE
@@ -719,7 +731,7 @@ int launch_signal(uint32_t* const* flag, float* const* meta, const float* campos
 
 int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, float* seeds,
                           const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
-                          cudaStream_t stream, cudaEvent_t between, unsigned char* adam_live, bool depth)
+                          cudaStream_t stream, cudaEvent_t between, unsigned char* adam_live, bool depth, bool aa)
 {
 	if (P - first <= 0) return 0;
 	if (!seeds) { set_error_msg("launch_fused_backward: seed scratch missing"); return -1; }
@@ -727,7 +739,7 @@ int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, co
 	DpPush nodp;
 	memset(&nodp, 0, sizeof(nodp));
 	unsigned char* live = adam ? adam_live : nullptr;
-	const int mode = (live ? MODE_ADAM_LIVE : adam ? MODE_ADAM : MODE_GRADS) | (depth ? MODE_DEPTH : 0);
+	const int mode = (live ? MODE_ADAM_LIVE : adam ? MODE_ADAM : MODE_GRADS) | (depth ? MODE_DEPTH : 0) | (aa ? MODE_AA : 0);
 	int rc;
 	if ((rc = launch_gaussian_backward(mode, first, P, t, cam, geom, sink, h, grads, st, counters, capacity, seeds, nodp, live, stream))) return rc;
 	if (between) cudaEventRecord(between, stream);
@@ -749,11 +761,12 @@ int launch_adam_live_rebuild(int P, const TrainTensors& t, unsigned char* live, 
 }
 
 int launch_push_backward(int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, const StepHyper& h,
-                         const DensifyStats& st, const uint32_t* counters, uint32_t capacity, const DpPush& dp, cudaStream_t stream, bool depth)
+                         const DensifyStats& st, const uint32_t* counters, uint32_t capacity, const DpPush& dp, cudaStream_t stream, bool depth,
+                         bool aa)
 {
 	const GradSegments nog = {};
 	int rc;
-	if ((rc = launch_gaussian_backward(MODE_PUSH | (depth ? MODE_DEPTH : 0), 0, P, t, cam, geom, sink, h, nog, st, counters, capacity, nullptr, dp,
+	if ((rc = launch_gaussian_backward(MODE_PUSH | (depth ? MODE_DEPTH : 0) | (aa ? MODE_AA : 0), 0, P, t, cam, geom, sink, h, nog, st, counters, capacity, nullptr, dp,
 	                                   nullptr, stream)))
 		return rc;
 	return launch_signal(dp.grad_flag, dp.meta, cam.campos, h.D, dp.world, dp.rank, dp.epoch, stream);

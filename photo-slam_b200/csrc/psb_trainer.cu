@@ -32,6 +32,11 @@ struct psb_trainer {
 	// training call's pass, which had its own backward, or a pass whose arena psb_trainer_result regrew)
 	int pass_D = -1;
 	bool pass_det = false;
+	bool pass_aa = false;
+	// anti-aliasing (psb_trainer_set_antialiasing): every forward pass blends with o' = o h (the 2D Mip filter), and every per-Gaussian
+	// backward behind it runs the AA variant
+	bool antialiasing = false;
+	bool slab_aa = false;          // the mode of the last psb_trainer_backward_begin*: every _slab after it runs that variant
 	uint32_t ovf_first = 0, ovf_count = 0;  // what the last PSB_ERR_RETRY was about (psb_trainer_overflow_info)
 	cudaEvent_t readback = nullptr;  // recorded once the instance count (and the loss sums) of the last call are in pinned memory
 	int last_P = 0, last_W = 0, last_H = 0;
@@ -267,7 +272,8 @@ int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, con
 	ImgState& img = sc.img;
 	const GaussIn in = raw_input(P, D, M, model);
 	t->mark(0, stream);
-	if ((rc = launch_preprocess(in, cam, radii, geom, /*raw=*/true, t->tight, stream))) return rc;
+	if ((rc = launch_preprocess(in, cam, radii, geom, /*raw=*/true, t->tight, stream, t->antialiasing))) return rc;
+	t->pass_aa = t->antialiasing;
 	t->mark(1, stream);
 	if ((rc = launch_depth_sort_and_scan(P, geom, /*scan=*/false, stream))) return rc;
 	t->mark(2, stream);
@@ -321,6 +327,7 @@ struct TileBackward {
 	GeomState geom;
 	Camera cam;
 	bool depth;
+	bool aa;     // the forward was anti-aliased: the per-Gaussian stage runs the AA variant
 };
 
 // The built-in loss around the shared stages: forward -> loss (+ depth loss) -> pinned read-back of the loss sums -> tile backward.
@@ -368,6 +375,7 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	out.geom = sc.geom;
 	out.cam = cam;
 	out.depth = depth_loss;
+	out.aa = t->pass_aa;
 	return 0;
 }
 
@@ -538,7 +546,7 @@ int psb_dp_step_depth(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* 
 	// push backward (records go straight into the owners' inboxes) + signal; wait until every rank's records have landed -> Adam of
 	// the owned rows, updated rows stored to every replica + signal
 	if ((rc = launch_push_backward(P, tt, tb.cam, tb.geom, t->sink, h, densify_stats(model, step), tb.geom.counters, (uint32_t)t->capacity, push, stream,
-	                               tb.depth)))
+	                               tb.depth, tb.aa)))
 		return rc;
 	t->mark(7, stream);
 	t->mark(8, stream);
@@ -630,6 +638,10 @@ int psb_trainer_backward_pixels(psb_trainer* t, unsigned pass, int P, int M, con
 		set_error_msg("psb_trainer_backward_pixels: the deterministic mode changed since the forward pass");
 		return PSB_ERR_ARG;
 	}
+	if (t->pass_aa != t->antialiasing) {
+		set_error_msg("psb_trainer_backward_pixels: the anti-aliasing mode changed since the forward pass");
+		return PSB_ERR_ARG;
+	}
 	if (step->step < 1) { set_error_msg("psb_trainer_backward_pixels: step >= 1 required"); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, adam))) return rc;
 	if (!adam && (rc = check_grads(grads, P, "psb_trainer_backward_pixels"))) return rc;
@@ -643,7 +655,8 @@ int psb_trainer_backward_pixels(psb_trainer* t, unsigned pass, int P, int M, con
 	if (!adam)
 		for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
 	rc = launch_fused_backward(adam, 0, P, train_tensors(model, adam), cam, sc.geom, t->sink, t->seeds, to_hyper(step), gs, densify_stats(model, step),
-	                           sc.geom.counters, (uint32_t)t->capacity, stream, t->event(7), adam ? model->adam_live : nullptr, pixel_grads->dL_ddepth != nullptr);
+	                           sc.geom.counters, (uint32_t)t->capacity, stream, t->event(7), adam ? model->adam_live : nullptr, pixel_grads->dL_ddepth != nullptr,
+	                           t->pass_aa);
 	t->end_stages(8, stream);
 	return rc;
 }
@@ -665,7 +678,7 @@ int psb_trainer_step_depth(psb_trainer* t, int P, int M, const psb_model* model,
 	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, true, stream, tb)) || P == 0)
 		return rc;
 	rc = launch_fused_backward(true, 0, P, train_tensors(model, true), tb.cam, tb.geom, t->sink, t->seeds, to_hyper(step), GradSegments{},
-	                           densify_stats(model, step), tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), model->adam_live, tb.depth);
+	                           densify_stats(model, step), tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), model->adam_live, tb.depth, tb.aa);
 	t->end_stages(8, stream);
 	return rc;
 }
@@ -692,7 +705,7 @@ int psb_trainer_backward_depth(psb_trainer* t, int P, int M, const psb_model* mo
 	GradSegments gs;
 	for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
 	rc = launch_fused_backward(false, 0, P, train_tensors(model, false), tb.cam, tb.geom, t->sink, t->seeds, to_hyper(step), gs, densify_stats(model, step),
-	                           tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), nullptr, tb.depth);
+	                           tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), nullptr, tb.depth, tb.aa);
 	t->end_stages(8, stream);
 	return rc;
 }
@@ -712,6 +725,7 @@ int psb_trainer_backward_begin_depth(psb_trainer* t, int P, int M, const psb_mod
 	if ((rc = check_depth(depth, "psb_trainer_backward_begin_depth"))) return rc;
 	// set whether or not the call below succeeds: the depth variant of _slab gives the plain result on rows without dL/dz
 	if (t) t->slab_depth = depth && depth->gt_depth;
+	if (t) t->slab_aa = t->antialiasing;
 	TileBackward tb;
 	return render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, (cudaStream_t)stream_, tb);
 }
@@ -735,7 +749,8 @@ int psb_trainer_backward_slab(psb_trainer* t, int P, int M, const psb_model* mod
 	GradSegments gs;
 	for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
 	return launch_fused_backward(false, first, first + count, train_tensors(model, false), to_camera(camera), geom, t->sink, t->seeds, to_hyper(step), gs,
-	                             densify_stats(model, step), geom.counters, (uint32_t)t->capacity, (cudaStream_t)stream_, nullptr, nullptr, t->slab_depth);
+	                             densify_stats(model, step), geom.counters, (uint32_t)t->capacity, (cudaStream_t)stream_, nullptr, nullptr, t->slab_depth,
+	                             t->slab_aa);
 }
 
 int psb_adam_update(int P, int M, const psb_model* model, float* const* grads, const psb_step* step, float grad_scale, void* stream_)
@@ -870,6 +885,13 @@ int psb_trainer_set_deterministic(psb_trainer* t, int enable)
 {
 	if (!t) { set_error_msg("psb_trainer_set_deterministic: null context"); return PSB_ERR_ARG; }
 	t->deterministic = enable != 0;   // (its scratch is made by the next call that runs a pass)
+	return 0;
+}
+
+int psb_trainer_set_antialiasing(psb_trainer* t, int enable)
+{
+	if (!t) { set_error_msg("psb_trainer_set_antialiasing: null context"); return PSB_ERR_ARG; }
+	t->antialiasing = enable != 0;   // (takes effect at the next pass; the scratch does not change)
 	return 0;
 }
 

@@ -240,6 +240,93 @@ RasterizeGaussiansBackwardDeterministicCUDA(const torch::Tensor& background, con
 	return std::make_tuple(dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations);
 }
 
+// ---- anti-aliasing (the 2D Mip filter, upstream diff-gaussian-rasterization's `antialiasing`; include/psb200.h psb_rasterize_forward_aa):
+// every splat blends with opacity o' = o h, h = sqrt(max(det0 / det1, 2.5e-5)) of its 2D covariance before / after the 0.3 px^2 dilation.
+// RasterizeGaussiansAntialiasedCUDA: the signature and 7-tuple of RasterizeGaussiansDepthCUDA (colour, depth, radii, buffers), anti-aliased.
+std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
+RasterizeGaussiansAntialiasedCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors,
+                                  const torch::Tensor& opacity, const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier,
+                                  const torch::Tensor& cov3D_precomp, const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix,
+                                  const float tan_fovx, const float tan_fovy, const int image_height, const int image_width, const torch::Tensor& sh,
+                                  const int degree, const torch::Tensor& campos, const bool prefiltered)
+{
+	if (means3D.ndimension() != 2 || means3D.size(1) != 3) { AT_ERROR("means3D must have dimensions (num_points, 3)"); }
+	const int P = means3D.size(0);
+	const int H = image_height, W = image_width;
+	auto float_opts = means3D.options().dtype(torch::kFloat32);
+	torch::Tensor out_color = torch::full({3, H, W}, 0.0, float_opts);
+	torch::Tensor out_depth = torch::full({H, W}, 0.0, float_opts);
+	torch::Tensor radii = torch::full({P}, 0, means3D.options().dtype(torch::kInt32));
+	torch::TensorOptions options(torch::kByte);
+	torch::Tensor geomBuffer = torch::empty({0}, options.device(means3D.device()));
+	torch::Tensor binningBuffer = torch::empty({0}, options.device(means3D.device()));
+	torch::Tensor imgBuffer = torch::empty({0}, options.device(means3D.device()));
+	int rendered = 0;
+	if (P != 0) {
+		int M = 0;
+		if (sh.size(0) != 0) M = sh.size(1);
+		const auto bg = background.contiguous(), m3 = means3D.contiguous(), shc = sh.contiguous(), col = colors.contiguous(), op = opacity.contiguous(),
+		           sc = scales.contiguous(), rot = rotations.contiguous(), cov = cov3D_precomp.contiguous(), vm = viewmatrix.contiguous(),
+		           pm = projmatrix.contiguous(), cp = campos.contiguous();
+		rendered = psb_rasterize_forward_aa(resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer, P, degree, M, fptr(bg), W, H,
+		                                    fptr(m3), fptr(shc), fptr(col), fptr(op), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm),
+		                                    fptr(pm), fptr(cp), tan_fovx, tan_fovy, prefiltered ? 1 : 0, out_color.data_ptr<float>(),
+		                                    radii.data_ptr<int>(), out_depth.data_ptr<float>(), 1, current_stream());
+		if (rendered < 0) { AT_ERROR("psb_rasterize_forward_aa: ", psb_last_error()); }
+	}
+	return std::make_tuple(rendered, out_color, out_depth, radii, geomBuffer, binningBuffer, imgBuffer);
+}
+
+// The backward of RasterizeGaussiansAntialiasedCUDA: the signature of RasterizeGaussiansBackwardDeterministicCUDA plus `deterministic`
+// (true: bit-identical from call to call; false: the float-atomic backward). dL_dopacity is dL/do; an undefined or empty dL_dout_depth is
+// colour only.
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
+RasterizeGaussiansBackwardAntialiasedCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii,
+                                          const torch::Tensor& colors, const torch::Tensor& scales, const torch::Tensor& rotations,
+                                          const float scale_modifier, const torch::Tensor& cov3D_precomp, const torch::Tensor& viewmatrix,
+                                          const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
+                                          const torch::Tensor& dL_dout_color, const torch::Tensor& dL_dout_depth, const torch::Tensor& sh,
+                                          const int degree, const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R,
+                                          const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const bool deterministic)
+{
+	const int P = means3D.size(0);
+	const int H = dL_dout_color.size(1), W = dL_dout_color.size(2);
+	const bool depth = dL_dout_depth.defined() && dL_dout_depth.numel() != 0;
+	if (depth && (dL_dout_depth.ndimension() != 2 || dL_dout_depth.size(0) != H || dL_dout_depth.size(1) != W)) {
+		AT_ERROR("dL_dout_depth must have dimensions (", H, ", ", W, ")");
+	}
+	int M = 0;
+	if (sh.size(0) != 0) M = sh.size(1);
+	torch::Tensor dL_dmeans3D = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_dmeans2D = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_dcolors = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_dconic = torch::zeros({P, 2, 2}, means3D.options());
+	torch::Tensor dL_dopacity = torch::zeros({P, 1}, means3D.options());
+	torch::Tensor dL_dcov3D = torch::zeros({P, 6}, means3D.options());
+	torch::Tensor dL_dsh = torch::zeros({P, M, 3}, means3D.options());
+	torch::Tensor dL_dscales = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_drotations = torch::zeros({P, 4}, means3D.options());
+	torch::Tensor dL_dz = torch::zeros({depth ? P : 0}, means3D.options());
+	if (P != 0) {
+		const auto bg = background.contiguous(), m3 = means3D.contiguous(), shc = sh.contiguous(), col = colors.contiguous(), sc = scales.contiguous(),
+		           rot = rotations.contiguous(), cov = cov3D_precomp.contiguous(), vm = viewmatrix.contiguous(), pm = projmatrix.contiguous(),
+		           cp = campos.contiguous(), dpix = dL_dout_color.contiguous(), rad = radii.contiguous();
+		const torch::Tensor ddep = depth ? dL_dout_depth.contiguous() : torch::Tensor();
+		const size_t det_bytes = deterministic ? psb_rasterize_backward_det_bytes(P, R) : 0;
+		torch::Tensor det_scratch = torch::empty({(long long)det_bytes}, means3D.options().dtype(torch::kByte));
+		const int rc = psb_rasterize_backward_aa(
+			P, degree, M, R, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
+			tan_fovx, tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(geomBuffer.contiguous().data_ptr()),
+			reinterpret_cast<char*>(binningBuffer.contiguous().data_ptr()), reinterpret_cast<char*>(imageBuffer.contiguous().data_ptr()), fptr(dpix),
+			dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(), dL_dopacity.data_ptr<float>(), dL_dcolors.data_ptr<float>(),
+			dL_dmeans3D.data_ptr<float>(), dL_dcov3D.data_ptr<float>(), M ? dL_dsh.data_ptr<float>() : nullptr, dL_dscales.data_ptr<float>(),
+			dL_drotations.data_ptr<float>(), depth ? ddep.data_ptr<float>() : nullptr, depth ? dL_dz.data_ptr<float>() : nullptr,
+			deterministic ? det_scratch.data_ptr() : nullptr, det_bytes, 1, current_stream());
+		if (rc < 0) { AT_ERROR("psb_rasterize_backward_aa: ", psb_last_error()); }
+	}
+	return std::make_tuple(dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations);
+}
+
 torch::Tensor markVisible(torch::Tensor& means3D, torch::Tensor& viewmatrix, torch::Tensor& projmatrix)
 {
 	const int P = means3D.size(0);
@@ -435,6 +522,22 @@ std::tuple<T, T, T, T, T, T, T, T> op_bwd_det(const T& bg, const T& m3, const T&
 	return RasterizeGaussiansBackwardDeterministicCUDA(bg, m3, radii, col, sc, rot, (float)smod, cov, vm, pm, (float)tfx, (float)tfy, dpix, ddep.value_or(T()),
 	                                                   sh, (int)deg, cp, gb, (int)R, bb, ib);
 }
+std::tuple<int64_t, T, T, T, T, T, T> op_fwd_aa(const T& bg, const T& m3, const T& col, const T& op, const T& sc, const T& rot, double smod,
+                                                const T& cov, const T& vm, const T& pm, double tfx, double tfy, int64_t H, int64_t W, const T& sh,
+                                                int64_t deg, const T& cp, bool pre)
+{
+	auto r = RasterizeGaussiansAntialiasedCUDA(bg, m3, col, op, sc, rot, (float)smod, cov, vm, pm, (float)tfx, (float)tfy, (int)H, (int)W, sh, (int)deg, cp,
+	                                           pre);
+	return std::make_tuple((int64_t)std::get<0>(r), std::get<1>(r), std::get<2>(r), std::get<3>(r), std::get<4>(r), std::get<5>(r), std::get<6>(r));
+}
+std::tuple<T, T, T, T, T, T, T, T> op_bwd_aa(const T& bg, const T& m3, const T& radii, const T& col, const T& sc, const T& rot, double smod,
+                                             const T& cov, const T& vm, const T& pm, double tfx, double tfy, const T& dpix,
+                                             const std::optional<T>& ddep, const T& sh, int64_t deg, const T& cp, const T& gb, int64_t R, const T& bb,
+                                             const T& ib, bool deterministic)
+{
+	return RasterizeGaussiansBackwardAntialiasedCUDA(bg, m3, radii, col, sc, rot, (float)smod, cov, vm, pm, (float)tfx, (float)tfy, dpix, ddep.value_or(T()),
+	                                                 sh, (int)deg, cp, gb, (int)R, bb, ib, deterministic);
+}
 T op_vis(T m3, T vm, T pm) { return markVisible(m3, vm, pm); }
 T op_dist(const T& p) { return distCUDA2(p); }
 T op_xform(T p, T m) { transformPoints(p, m); return p; }
@@ -471,6 +574,8 @@ TORCH_LIBRARY(psb200, m)
 	m.def("rasterize_gaussians_depth", &op_fwd_depth);
 	m.def("rasterize_gaussians_backward_depth", &op_bwd_depth);
 	m.def("rasterize_gaussians_backward_deterministic", &op_bwd_det);
+	m.def("rasterize_gaussians_antialiased", &op_fwd_aa);
+	m.def("rasterize_gaussians_backward_antialiased", &op_bwd_aa);
 	m.def("mark_visible", &op_vis);
 	m.def("b2_forward", &op_b2_fwd);
 	m.def("dist_cuda2", &op_dist);

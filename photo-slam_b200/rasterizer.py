@@ -14,6 +14,11 @@ Rendered depth D(p) = sum_i z_i alpha_i T_i (include/psb200.h), which the refere
 deterministic=True (keyword) on the backward functions, rasterize_gaussians and GaussianRasterizer.forward selects
 psb_rasterize_backward_deterministic: the same gradients, bit-identical from run to run. The default keeps the float-atomic backward.
 
+GaussianRasterizationSettings.antialiasing=True (upstream diff-gaussian-rasterization's field) selects the 2D Mip filter: every splat blends
+with opacity o' = o * sqrt(max(det0 / det1, 2.5e-5)), det0 / det1 the determinants of its 2D covariance before / after the 0.3 px^2
+dilation (psb_rasterize_forward_aa / psb_rasterize_backward_aa). The B1 functions take it as the keyword antialiasing=False, the
+autograd functions read it from the settings.
+
 PyTorch is used only for device memory, streams and autograd bookkeeping.
 """
 from dataclasses import dataclass
@@ -66,8 +71,9 @@ class _Scratch:
 
 
 def _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
-             tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, depth):
-    """RasterizeGaussiansCUDA, and with depth=True also the [H,W] depth image (psb_rasterize_forward_depth)."""
+             tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, depth, antialiasing=False):
+    """RasterizeGaussiansCUDA, and with depth=True also the [H,W] depth image (psb_rasterize_forward_depth); antialiasing=True:
+    psb_rasterize_forward_aa (depth or not)."""
     if means3D.dim() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")  # AT_ERROR in the reference
     L = _lib.lib()
@@ -87,7 +93,10 @@ def _forward(background, means3D, colors, opacity, scales, rotations, scale_modi
                 _ptr(m3), _ptr(shc), _ptr(col), _ptr(opa), _ptr(sca), float(scale_modifier), _ptr(rot), _ptr(cov),
                 _ptr(vm), _ptr(pm), _ptr(cp), float(tan_fovx), float(tan_fovy), int(bool(prefiltered)),
                 out_color.data_ptr(), radii.data_ptr()]
-        if depth:
+        if antialiasing:
+            rendered = _lib.check(L.psb_rasterize_forward_aa(*args, out_depth.data_ptr() if depth else None, 1, _stream()),
+                                  "psb_rasterize_forward_aa")
+        elif depth:
             rendered = _lib.check(L.psb_rasterize_forward_depth(*args, out_depth.data_ptr(), _stream()), "psb_rasterize_forward_depth")
         else:
             rendered = _lib.check(L.psb_rasterize_forward(*args, _stream()), "psb_rasterize_forward")
@@ -96,28 +105,30 @@ def _forward(background, means3D, colors, opacity, scales, rotations, scale_modi
 
 def RasterizeGaussiansCUDA(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                            viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos,
-                           prefiltered):
-    """-> (num_rendered, out_color [3,H,W], radii [P] int32, geomBuffer, binningBuffer, imgBuffer)."""
+                           prefiltered, *, antialiasing=False):
+    """-> (num_rendered, out_color [3,H,W], radii [P] int32, geomBuffer, binningBuffer, imgBuffer).
+    antialiasing=True: the 2D Mip filter (o' = o h); back-propagate with antialiasing=True as well."""
     rendered, out_color, _, radii, geom, binning, img = _forward(
         background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx,
-        tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, depth=False)
+        tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, depth=False, antialiasing=antialiasing)
     return rendered, out_color, radii, geom, binning, img
 
 
 def RasterizeGaussiansDepthCUDA(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                                 viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos,
-                                prefiltered):
+                                prefiltered, *, antialiasing=False):
     """RasterizeGaussiansCUDA plus the depth image -> (num_rendered, out_color [3,H,W], out_depth [H,W], radii [P] int32, geomBuffer,
-    binningBuffer, imgBuffer). Colour, radii and buffers are bit-identical to RasterizeGaussiansCUDA's."""
+    binningBuffer, imgBuffer). Colour, radii and buffers are bit-identical to RasterizeGaussiansCUDA's. antialiasing: as there."""
     return _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
-                    tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, depth=True)
+                    tan_fovx, tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, depth=True, antialiasing=antialiasing)
 
 
 def _backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
               tan_fovx, tan_fovy, dL_dout_color, dL_dout_depth, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer,
-              deterministic=False):
+              deterministic=False, antialiasing=False):
     """RasterizeGaussiansBackwardCUDA, and with a depth gradient psb_rasterize_backward_depth; deterministic=True calls
-    psb_rasterize_backward_deterministic (either gradient set) over a scratch of psb_rasterize_backward_det_bytes(P, R)."""
+    psb_rasterize_backward_deterministic (either gradient set) over a scratch of psb_rasterize_backward_det_bytes(P, R).
+    antialiasing=True: psb_rasterize_backward_aa (atomic, or deterministic over that scratch) for an anti-aliased forward."""
     L = _lib.lib()
     P = means3D.size(0)
     H, W = dL_dout_color.size(1), dL_dout_color.size(2)
@@ -147,7 +158,12 @@ def _backward(background, means3D, radii, colors, scales, rotations, scale_modif
             if tuple(ddep.shape) != (H, W):
                 raise RuntimeError(f"dL_dout_depth must have dimensions ({H}, {W})")
             dL_dz = torch.zeros((P,), **o)      # [P], zero-initialised as the C-ABI requires; folded into dL_dmeans3D there
-        if deterministic:
+        if antialiasing:
+            nbytes = L.psb_rasterize_backward_det_bytes(P, int(R)) if deterministic else 0
+            scratch = torch.empty((nbytes,), dtype=torch.uint8, device=means3D.device) if deterministic else None
+            _lib.check(L.psb_rasterize_backward_aa(*args, _ptr(ddep), _ptr(dL_dz), _ptr(scratch), nbytes, 1, _stream()),
+                       "psb_rasterize_backward_aa")
+        elif deterministic:
             nbytes = L.psb_rasterize_backward_det_bytes(P, int(R))
             scratch = torch.empty((nbytes,), dtype=torch.uint8, device=means3D.device)    # the call zeroes what it reads
             _lib.check(L.psb_rasterize_backward_deterministic(*args, _ptr(ddep), _ptr(dL_dz), scratch.data_ptr(), nbytes, _stream()),
@@ -161,21 +177,24 @@ def _backward(background, means3D, radii, colors, scales, rotations, scale_modif
 
 def RasterizeGaussiansBackwardCUDA(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp,
                                    viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, sh, degree, campos,
-                                   geomBuffer, R, binningBuffer, imageBuffer, *, deterministic=False):
+                                   geomBuffer, R, binningBuffer, imageBuffer, *, deterministic=False, antialiasing=False):
     """-> (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations).
-    deterministic=True: the same gradients, bit-identical from call to call (summed in a fixed order instead of with float atomics)."""
+    deterministic=True: the same gradients, bit-identical from call to call (summed in a fixed order instead of with float atomics).
+    antialiasing=True: the backward of an anti-aliased forward (the same flag there); dL_dopacity is then dL/do."""
     return _backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
-                     tan_fovx, tan_fovy, dL_dout_color, None, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer, deterministic)
+                     tan_fovx, tan_fovy, dL_dout_color, None, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer, deterministic,
+                     antialiasing)
 
 
 def RasterizeGaussiansBackwardDepthCUDA(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp,
                                         viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, dL_dout_depth, sh, degree, campos,
-                                        geomBuffer, R, binningBuffer, imageBuffer, *, deterministic=False):
+                                        geomBuffer, R, binningBuffer, imageBuffer, *, deterministic=False, antialiasing=False):
     """RasterizeGaussiansBackwardCUDA with the gradient of the depth image as well (dL_dout_depth [H,W]; None = the plain backward).
-    dL/dz is folded into dL_dmeans3D, and dL_dmeans2D includes the depth term. Returns the same 8-tuple. deterministic: as there."""
+    dL/dz is folded into dL_dmeans3D, and dL_dmeans2D includes the depth term. Returns the same 8-tuple. deterministic, antialiasing:
+    as there."""
     return _backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
                      tan_fovx, tan_fovy, dL_dout_color, dL_dout_depth, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer,
-                     deterministic)
+                     deterministic, antialiasing)
 
 
 def markVisible(means3D, viewmatrix, projmatrix):
@@ -190,7 +209,8 @@ def markVisible(means3D, viewmatrix, projmatrix):
 
 @dataclass
 class GaussianRasterizationSettings:
-    """Field for field the reference struct (include/gaussian_rasterizer.h:25-55), without trailing underscores."""
+    """Field for field the reference struct (include/gaussian_rasterizer.h:25-55), without trailing underscores, plus upstream
+    diff-gaussian-rasterization's `antialiasing` (the 2D Mip filter; off by default)."""
     image_height: int
     image_width: int
     tanfovx: float
@@ -202,6 +222,7 @@ class GaussianRasterizationSettings:
     sh_degree: int
     campos: torch.Tensor
     prefiltered: bool = False
+    antialiasing: bool = False
 
 
 class _RasterizeGaussians(torch.autograd.Function):
@@ -213,10 +234,11 @@ class _RasterizeGaussians(torch.autograd.Function):
         num_rendered, color, radii, geomBuffer, binningBuffer, imgBuffer = RasterizeGaussiansCUDA(
             rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
             rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, sh, rs.sh_degree,
-            rs.campos, rs.prefiltered)
+            rs.campos, rs.prefiltered, antialiasing=bool(rs.antialiasing))
         ctx.raster_settings = rs
         ctx.num_rendered = num_rendered
         ctx.deterministic = bool(deterministic)
+        ctx.antialiasing = bool(rs.antialiasing)     # the backward differentiates the forward that ran
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
                               binningBuffer, imgBuffer)
         ctx.mark_non_differentiable(radii)
@@ -232,7 +254,7 @@ class _RasterizeGaussians(torch.autograd.Function):
          grad_rotations) = RasterizeGaussiansBackwardCUDA(
             rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix,
             rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_out_color, sh, rs.sh_degree, rs.campos, geomBuffer,
-            ctx.num_rendered, binningBuffer, imgBuffer, deterministic=ctx.deterministic)
+            ctx.num_rendered, binningBuffer, imgBuffer, deterministic=ctx.deterministic, antialiasing=ctx.antialiasing)
         # order of reference gaussian_rasterizer.cpp:159-179
         def g(t, ref):
             return t if (ref is not None and ref.numel() != 0) else None
@@ -249,10 +271,11 @@ class _RasterizeGaussiansDepth(torch.autograd.Function):
         num_rendered, color, depth, radii, geomBuffer, binningBuffer, imgBuffer = RasterizeGaussiansDepthCUDA(
             rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
             rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, sh, rs.sh_degree,
-            rs.campos, rs.prefiltered)
+            rs.campos, rs.prefiltered, antialiasing=bool(rs.antialiasing))
         ctx.raster_settings = rs
         ctx.num_rendered = num_rendered
         ctx.deterministic = bool(deterministic)
+        ctx.antialiasing = bool(rs.antialiasing)     # the backward differentiates the forward that ran
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
                               binningBuffer, imgBuffer)
         ctx.mark_non_differentiable(radii)
@@ -271,7 +294,7 @@ class _RasterizeGaussiansDepth(torch.autograd.Function):
          grad_rotations) = RasterizeGaussiansBackwardDepthCUDA(
             rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix,
             rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_out_color, grad_out_depth, sh, rs.sh_degree, rs.campos, geomBuffer,
-            ctx.num_rendered, binningBuffer, imgBuffer, deterministic=ctx.deterministic)
+            ctx.num_rendered, binningBuffer, imgBuffer, deterministic=ctx.deterministic, antialiasing=ctx.antialiasing)
 
         def g(t, ref):
             return t if (ref is not None and ref.numel() != 0) else None

@@ -23,9 +23,11 @@ from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer
 
 @dataclass
 class GaussianPipelineParams:
-    """reference include/gaussian_parameters.h:38-47 (all shipped configs: both False)"""
+    """reference include/gaussian_parameters.h:38-47 (all shipped configs: both False), plus `antialiasing`: the rasterizer's 2D Mip
+    filter (GaussianRasterizationSettings.antialiasing) in every branch below; off by default"""
     convert_SHs: bool = False
     compute_cov3D: bool = False
+    antialiasing: bool = False
 
 
 def build_rotation(r):
@@ -66,7 +68,7 @@ def render(viewpoint_camera, image_height, image_width, pc, pipe=None, bg_color=
     screenspace_points = torch.zeros_like(pc.xyz_, requires_grad=True)
     settings = GaussianRasterizationSettings(int(image_height), int(image_width), float(viewpoint_camera["tanfovx"]), float(viewpoint_camera["tanfovy"]),
                                              bg_color, float(scaling_modifier), viewpoint_camera["viewmatrix"], viewpoint_camera["projmatrix"],
-                                             int(pc.active_sh_degree_), viewpoint_camera["campos"], False)
+                                             int(pc.active_sh_degree_), viewpoint_camera["campos"], False, bool(pipe.antialiasing))
     rasterizer = GaussianRasterizer(settings)
     means3D, means2D = pc.xyz_, screenspace_points
     opacity = torch.sigmoid(pc.opacity_)

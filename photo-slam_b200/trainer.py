@@ -102,13 +102,14 @@ def _bind():
                                                    vp, C.POINTER(_Depth), vp]
     L.psb_loss.argtypes = [C.c_int, C.c_int, vp, vp, vp, C.c_float, vp, C.POINTER(C.c_float), vp]
     L.psb_trainer_set_deterministic.argtypes = [vp, C.c_int]
+    L.psb_trainer_set_antialiasing.argtypes = [vp, C.c_int]
     L.psb_trainer_forward.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, C.c_int, vp, vp, vp, vp, C.POINTER(C.c_uint), vp]
     L.psb_trainer_backward_pixels.argtypes = [vp, C.c_uint, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, C.POINTER(_PixelGrads),
                                               C.POINTER(_Step), C.POINTER(vp), vp]
     for n in ("psb_trainer_create", "psb_trainer_destroy", "psb_trainer_render", "psb_trainer_step", "psb_trainer_backward",
               "psb_adam_update", "psb_trainer_result", "psb_loss", "psb_trainer_render_depth", "psb_trainer_step_depth",
               "psb_trainer_backward_depth", "psb_trainer_result_depth", "psb_dp_step_depth", "psb_trainer_backward_begin_depth",
-              "psb_trainer_set_deterministic", "psb_trainer_forward", "psb_trainer_backward_pixels"):
+              "psb_trainer_set_deterministic", "psb_trainer_forward", "psb_trainer_backward_pixels", "psb_trainer_set_antialiasing"):
         getattr(L, n).restype = C.c_int
     L.psb_densify_workspace_bytes.argtypes = [C.c_int]
     L.psb_densify_workspace_bytes.restype = C.c_size_t
@@ -470,9 +471,14 @@ class GaussianTrainer:
 
     deterministic: True makes every training call of this trainer bit-identical from run to run (same inputs, build and GPU model;
     psb_trainer_set_deterministic), False keeps the default (faster) kernels, None follows torch.are_deterministic_algorithms_enabled()
-    at each call."""
+    at each call.
 
-    def __init__(self, model: GaussianModel, opt: GaussianOptimizationParams = None, background=None, deterministic=None):
+    antialiasing: True renders and trains every pass of this trainer with the 2D Mip filter (psb_trainer_set_antialiasing: each splat
+    blends with opacity o * sqrt(max(det0 / det1, 2.5e-5)), det0 / det1 the determinants of its 2D covariance before / after the
+    0.3 px^2 dilation), as renderer.render(pipe=GaussianPipelineParams(antialiasing=True)) does on the operator path. Fixed for the
+    trainer's lifetime."""
+
+    def __init__(self, model: GaussianModel, opt: GaussianOptimizationParams = None, background=None, deterministic=None, antialiasing=False):
         self.L = _bind()
         self.model = model
         self.opt = opt or GaussianOptimizationParams()
@@ -484,6 +490,14 @@ class GaussianTrainer:
         self._deterministic = deterministic
         self._det_applied = False      # the mode the context is in (a new context starts with it off)
         self._apply_deterministic()
+        self._antialiasing = bool(antialiasing)
+        if self._antialiasing:
+            _lib.check(self.L.psb_trainer_set_antialiasing(self.h, 1), "psb_trainer_set_antialiasing")
+
+    @property
+    def antialiasing(self):
+        """Whether this trainer's passes use the 2D Mip filter (set at construction)."""
+        return self._antialiasing
 
     @property
     def deterministic(self):
@@ -789,10 +803,12 @@ class DataParallelTrainer(GaussianTrainer):
     mode="nccl": round-1 path kept for A/B — slab-wise backward, one NCCL all-reduce per slab on a side stream, replicated Adam.
     world == 1 and mode=None: backward -> Adam split path on one GPU (tests).
     deterministic: as in GaussianTrainer, kept across rebuild(). "p2p" is then bit-identical run to run at any world size; "nccl"
-    gives deterministic per-rank gradients, but the all-reduce's summation order is NCCL's."""
+    gives deterministic per-rank gradients, but the all-reduce's summation order is NCCL's.
+    antialiasing: as in GaussianTrainer, in every mode. Every rank must pass the same value."""
 
-    def __init__(self, model, opt=None, background=None, group=None, pipeline=None, nslabs=4, mode=None, deterministic=None):
-        super().__init__(model, opt, background, deterministic=deterministic)
+    def __init__(self, model, opt=None, background=None, group=None, pipeline=None, nslabs=4, mode=None, deterministic=None,
+                 antialiasing=False):
+        super().__init__(model, opt, background, deterministic=deterministic, antialiasing=antialiasing)
         import os
         import torch.distributed as dist
         self.dist = dist
