@@ -340,6 +340,38 @@ int psb_trainer_step_depth(psb_trainer* t, int P, int M, const psb_model* model,
 int psb_trainer_backward_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
                                const float* background, const float* gt_image, const float* mask, const psb_step* step,
                                float* out_color, int* radii, float* const* grads, const psb_depth* depth, void* stream);
+/* ------------------------------------------------------------------------------------------------
+ * Exposure compensation per keyframe: the built-in loss compares the target with the rendered image I [3,H,W] (background term
+ * included) through the keyframe's 3x4 affine row E (row-major, element (r, j) = param[4 r + j]; identity = eye(3, 4), the layout of
+ * graphdeco's exposure.json, where E[:3,:3] right-multiplies HWC pixels):
+ *   I'(c,p) = sum_k E[k][c] I(k,p) + E[c][3];   X = mask * I';   L = (1 - lambda) mean|X - G| + lambda (1 - mean SSIM(X, G)) [+ depth]
+ * The tile backward receives dL/dI(k,p) = sum_c E[k][c] g(c,p), g = dL/dI'. dL/dE[k][c] = sum_p g(c,p) I(k,p) (k < 3) and
+ * dL/dE[c][3] = sum_p g(c,p) are added in a fixed order (no atomics): bit-identical from run to run in every mode. out_color stays the
+ * raw render; psb_trainer_result reports the loss of X. Only the given row and its moments are read or written. The row's Adam step
+ * uses step->beta1 / beta2 / eps, its own lr and its own step count, which the device advances (no host round trip). A pass that
+ * overflows the binning arena leaves the row, its moments and its step count untouched (the repeated call then updates it once).
+ * The data-parallel calls take no exposure; on the operator path a caller applies E in torch.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct psb_exposure {
+	float* param;       /* [3,4] device, the row E_k (gradient mode: read only) */
+	float* exp_avg;     /* [3,4] device (step only) */
+	float* exp_avg_sq;  /* [3,4] device (step only) */
+	int*   step;        /* [1] device int32: this row's Adam step count, advanced on the device (step only) */
+	float  lr;          /* finite, >= 0 */
+} psb_exposure;
+/* psb_trainer_step_depth with an exposure row (NULL: exactly psb_trainer_step_depth). PSB_ERR_ARG, before any CUDA call, for everything
+ * psb_trainer_step_depth rejects, a NULL param, exp_avg, exp_avg_sq or step, and a negative or non-finite lr. */
+int psb_trainer_step_exposure(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                              const float* background, const float* gt_image, const float* mask, const psb_step* step,
+                              float* out_color, int* radii, const psb_depth* depth, const psb_exposure* exposure, void* stream);
+/* psb_trainer_backward_depth with an exposure row (NULL: exactly psb_trainer_backward_depth, exposure_grad ignored): the raw-parameter
+ * gradients of the compensated loss, and dL/dE -> exposure_grad [12] device (zeros for a pass that overflowed the binning arena).
+ * exposure->param is only read; lr must still be valid, the moments and step are ignored. PSB_ERR_ARG, before any CUDA call, for
+ * everything psb_trainer_backward_depth rejects, a NULL param, a negative or non-finite lr and a NULL exposure_grad. */
+int psb_trainer_backward_exposure(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                                  const float* background, const float* gt_image, const float* mask, const psb_step* step,
+                                  float* out_color, int* radii, float* const* grads, const psb_depth* depth,
+                                  const psb_exposure* exposure, float* exposure_grad, void* stream);
 /* psb_trainer_result with out4 = {loss, l1, ssim, depth_l1} (depth_l1 = 0 when the last step had no depth term). */
 int psb_trainer_result_depth(psb_trainer* t, float* out4, int* num_rendered, void* stream);
 

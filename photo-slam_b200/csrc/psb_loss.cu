@@ -1,5 +1,5 @@
 // Fused photometric loss of the training step:  L = (1 - lambda) * mean|I - G| + lambda * (1 - mean SSIM(I, G))
-// with I = rendered * mask, SSIM over an 11x11 Gaussian window (sigma 1.5), zero padding, per channel —
+// with I = rendered * mask (or, with exposure compensation, mask * the rendered image through the keyframe's 3x4 affine row), SSIM over an 11x11 Gaussian window (sigma 1.5), zero padding, per channel —
 // the loss of reference gaussian_mapper.cpp:692-698 / include/loss_utils.h:28-124, which the reference runs
 // as five grouped cuDNN convolutions plus ~20 elementwise kernels forward and the autograd mirror backward.
 // Here: two kernels. Forward computes the five windowed moments with a separable filter in shared memory,
@@ -49,11 +49,22 @@ __device__ __forceinline__ void block_sums_out(float a, float b, double* __restr
 	}
 }
 
-// grid (tiles_x, tiles_y, 3), block 256 (16x16).
-template <bool DET>
+// Exposure compensation: the column of the 3x4 row E (row-major, E[r][j] = E[4 r + j]) that makes channel c of the compensated image,
+// I'(c) = sum_k E[k][c] I(k) + E[c][3]. Loaded once per thread: E is the device copy the previous queued step may have updated.
+struct ExpCol { float e0, e1, e2, eb; };
+__device__ __forceinline__ ExpCol exp_col(const float* __restrict__ E, int c) { return {E[c], E[4 + c], E[8 + c], E[4 * c + 3]}; }
+// I'(c, q) at pixel q of the planar [3][HW] image; with the identity row it is I(c, q) exactly (products with 1 and sums with 0)
+__device__ __forceinline__ float exposed(const ExpCol& e, const float* __restrict__ img, size_t HW, size_t q)
+{
+	return e.e0 * img[q] + e.e1 * img[HW + q] + e.e2 * img[2 * HW + q] + e.eb;
+}
+
+// grid (tiles_x, tiles_y, 3), block 256 (16x16). EXP: the loss of X = mask * I' (E: the device row, see ExpCol) instead of mask * I.
+template <bool DET, bool EXP = false>
 __device__ __forceinline__ void loss_fwd_body(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
                                               const float* __restrict__ mask, const Win& win, float g_ssim,
-                                              float* __restrict__ dmap /* [3 maps][3][H][W] */, double* __restrict__ sums /* [2] | DET: [blocks][2] */)
+                                              float* __restrict__ dmap /* [3 maps][3][H][W] */, double* __restrict__ sums /* [2] | DET: [blocks][2] */,
+                                              const float* __restrict__ E = nullptr)
 {
 	__shared__ float s_x[LS][LS + 1], s_y[LS][LS + 1];
 	__shared__ float s_h[5][LS][LT + 1];
@@ -62,13 +73,15 @@ __device__ __forceinline__ void loss_fwd_body(int H, int W, const float* __restr
 	const size_t HW = (size_t)H * W;
 	const int x0 = blockIdx.x * LT, y0 = blockIdx.y * LT;
 	const int tid = threadIdx.x;
+	ExpCol e{};
+	if (EXP) e = exp_col(E, ch);
 	for (int i = tid; i < LS * LS; i += 256) {
 		const int ly = i / LS, lx = i % LS;
 		const int gy = y0 + ly - LH, gx = x0 + lx - LH;
 		float a = 0.f, b = 0.f;
 		if (gx >= 0 && gx < W && gy >= 0 && gy < H) {
 			const size_t p = ch * HW + (size_t)gy * W + gx;
-			a = img[p];
+			a = EXP ? exposed(e, img, HW, (size_t)gy * W + gx) : img[p];
 			if (mask) a *= mask[p];
 			b = gt[p];
 		}
@@ -134,6 +147,20 @@ __global__ void __launch_bounds__(256) loss_fwd_det_kernel(int H, int W, const f
 	loss_fwd_body<true>(H, W, img, gt, mask, win, g_ssim, dmap, partials);
 }
 
+__global__ void __launch_bounds__(256) loss_fwd_exp_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
+                                                           const float* __restrict__ mask, Win win, float g_ssim, float* __restrict__ dmap,
+                                                           double* __restrict__ sums, const float* __restrict__ E)
+{
+	loss_fwd_body<false, true>(H, W, img, gt, mask, win, g_ssim, dmap, sums, E);
+}
+
+__global__ void __launch_bounds__(256) loss_fwd_exp_det_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
+                                                               const float* __restrict__ mask, Win win, float g_ssim, float* __restrict__ dmap,
+                                                               double* __restrict__ partials, const float* __restrict__ E)
+{
+	loss_fwd_body<true, true>(H, W, img, gt, mask, win, g_ssim, dmap, partials, E);
+}
+
 // Deterministic mode: sums[c] = the n block partials partials[2 b + c] (c = 0, 1) added in a fixed order (one block: strided
 // per-thread sums, then a fixed tree), whatever order the blocks that wrote them ran in.
 __global__ void __launch_bounds__(256) reduce_partials_kernel(int n, const double* __restrict__ partials, double* __restrict__ sums)
@@ -152,9 +179,12 @@ __global__ void __launch_bounds__(256) reduce_partials_kernel(int n, const doubl
 	if (tid == 0) { sums[0] = s[0][0]; sums[1] = s[1][0]; }
 }
 
-__global__ void __launch_bounds__(256) loss_bwd_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
-                                                       const float* __restrict__ mask, Win win, float g_l1,
-                                                       const float* __restrict__ dmap, float* __restrict__ dL_dimg)
+// EXP: evaluated at x = X = mask * I' (see loss_fwd_body); dL_dimg then receives g = dL/dI' (mask factor applied), which
+// exposure_mix_kernel turns into dL/dI.
+template <bool EXP>
+__device__ __forceinline__ void loss_bwd_body(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
+                                              const float* __restrict__ mask, const Win& win, float g_l1,
+                                              const float* __restrict__ dmap, float* __restrict__ dL_dimg, const float* __restrict__ E)
 {
 	__shared__ float s_d[3][LS][LS + 1];
 	__shared__ float s_h[3][LS][LT + 1];
@@ -195,11 +225,113 @@ __global__ void __launch_bounds__(256) loss_bwd_kernel(int H, int W, const float
 		}
 		const size_t p = ch * HW + (size_t)gy * W + gx;
 		const float mk = mask ? mask[p] : 1.f;
-		const float x = img[p] * mk, y = gt[p];
+		const float x = (EXP ? exposed(exp_col(E, ch), img, HW, (size_t)gy * W + gx) : img[p]) * mk, y = gt[p];
 		const float d = x - y;
 		const float sgn = (d > 0.f) ? 1.f : ((d < 0.f) ? -1.f : 0.f);
 		dL_dimg[p] = (g_l1 * sgn + c1 + 2.f * x * c2 + y * c3) * mk;
 	}
+}
+
+__global__ void __launch_bounds__(256) loss_bwd_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
+                                                       const float* __restrict__ mask, Win win, float g_l1,
+                                                       const float* __restrict__ dmap, float* __restrict__ dL_dimg)
+{
+	loss_bwd_body<false>(H, W, img, gt, mask, win, g_l1, dmap, dL_dimg, nullptr);
+}
+
+__global__ void __launch_bounds__(256) loss_bwd_exp_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
+                                                           const float* __restrict__ mask, Win win, float g_l1,
+                                                           const float* __restrict__ dmap, float* __restrict__ dL_dimg, const float* __restrict__ E)
+{
+	loss_bwd_body<true>(H, W, img, gt, mask, win, g_l1, dmap, dL_dimg, E);
+}
+
+// Exposure, pass 1 (grid-stride over the n = H W pixels, 256 threads): g = dL/dI' in dL_dpix (loss_bwd_exp_kernel) becomes
+// dL/dI(k) = sum_c E[k][c] g(c) in place, the plane the tile backward reads; the block's 12 sums
+// dL/dE[k][c] = sum_p g(c) I(k) (k < 3) and dL/dE[c][3] = sum_p g(c) go to partials[12 block + 4 r + j] (the layout of E) in double.
+__global__ void __launch_bounds__(256) exposure_mix_kernel(int n, const float* __restrict__ E, const float* __restrict__ img,
+                                                           float* __restrict__ dL_dpix, double* __restrict__ partials)
+{
+	__shared__ double s_red[8][12];
+	float e[12];
+#pragma unroll
+	for (int j = 0; j < 12; j++) e[j] = E[j];
+	double acc[12];
+#pragma unroll
+	for (int j = 0; j < 12; j++) acc[j] = 0.0;
+	for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) {
+		const float g[3] = {dL_dpix[i], dL_dpix[n + i], dL_dpix[2 * n + i]};
+		const float x[3] = {img[i], img[n + i], img[2 * n + i]};
+#pragma unroll
+		for (int k = 0; k < 3; k++) dL_dpix[(size_t)k * n + i] = e[4 * k] * g[0] + e[4 * k + 1] * g[1] + e[4 * k + 2] * g[2];
+#pragma unroll
+		for (int c = 0; c < 3; c++) {
+#pragma unroll
+			for (int k = 0; k < 3; k++) acc[4 * k + c] += (double)g[c] * (double)x[k];
+			acc[4 * c + 3] += (double)g[c];
+		}
+	}
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+	for (int j = 0; j < 12; j++) {
+		double v = acc[j];
+#pragma unroll
+		for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+		if (lane == 0) s_red[warp][j] = v;
+	}
+	__syncthreads();
+	if (threadIdx.x < 12) {
+		double t = 0.0;
+#pragma unroll
+		for (int w = 0; w < 8; w++) t += s_red[w][threadIdx.x];
+		partials[12 * (size_t)blockIdx.x + threadIdx.x] = t;
+	}
+}
+
+// Exposure, pass 2 (one block): the 12 sums = the n block partials added in a fixed order (strided per-thread sums, then a fixed tree,
+// as reduce_partials_kernel), so the gradient is the same every run. Then, unless the pass overflowed the binning arena
+// (counters[0] > capacity: the step is a no-op and is repeated, so the row must not move), either the Adam step of the row with its
+// own device step count (grad == null), or the gradient -> grad[12] (zeros for an overflowing pass, like the raw-parameter gradients).
+__global__ void __launch_bounds__(256) exposure_update_kernel(int n, const double* __restrict__ partials, const uint32_t* __restrict__ counters,
+                                                              uint32_t capacity, ExposureUpdate u, float* __restrict__ grad)
+{
+	__shared__ double s[12][256];
+	const int tid = threadIdx.x;
+	const bool overflow = counters && counters[0] > capacity;   // (null: a pass without Gaussians, which cannot overflow)
+	if (overflow && !grad) return;
+	double a[12];
+#pragma unroll
+	for (int j = 0; j < 12; j++) a[j] = 0.0;
+	for (int i = tid; i < n; i += 256)
+#pragma unroll
+		for (int j = 0; j < 12; j++) a[j] += partials[12 * (size_t)i + j];
+#pragma unroll
+	for (int j = 0; j < 12; j++) s[j][tid] = a[j];
+	__syncthreads();
+	for (int o = 128; o > 0; o >>= 1) {
+		if (tid < o)
+#pragma unroll
+			for (int j = 0; j < 12; j++) s[j][tid] += s[j][tid + o];
+		__syncthreads();
+	}
+	if (grad) {
+		if (tid < 12) grad[tid] = overflow ? 0.f : (float)s[tid][0];
+		return;
+	}
+	const int t = u.step[0] + 1;   // read by every thread before thread 0 stores it
+	__syncthreads();
+	if (tid < 12) {
+		const float g = (float)s[tid][0];
+		const double bc1 = 1.0 - pow((double)u.beta1, t), bc2 = 1.0 - pow((double)u.beta2, t);
+		float m = u.exp_avg[tid], v = u.exp_avg_sq[tid];
+		m = m * u.beta1 + (1.f - u.beta1) * g;
+		v = v * u.beta2 + (1.f - u.beta2) * g * g;
+		u.exp_avg[tid] = m;
+		u.exp_avg_sq[tid] = v;
+		const float denom = sqrtf(v) / (float)sqrt(bc2) + u.eps;
+		u.param[tid] -= (float)(u.lr / bc1) * (m / denom);
+	}
+	if (tid == 0) u.step[0] = t;
 }
 
 // Depth L1, pass 1 (grid-stride, 256 threads): per valid pixel |D - G| and sign(D - G) (-> dL_dD, scaled by pass 2); block sums of
@@ -270,7 +402,7 @@ int launch_depth_loss(int H, int W, const float* depth, const float* gt_depth, c
 // sums: device double[2] (zeroed here); after the launch sums[0] = sum|I-G|, sums[1] = sum ssim_map.
 // dmap: device float[9*H*W] scratch. dL_dimg may be null (loss value only).
 int launch_loss(int H, int W, const float* img, const float* gt, const float* mask, float lambda_dssim, float* dmap, double* sums,
-                float* dL_dimg, cudaStream_t stream, double* partials)
+                float* dL_dimg, cudaStream_t stream, double* partials, const float* E)
 {
 	Win win;
 	float s = 0.f;
@@ -279,18 +411,35 @@ int launch_loss(int H, int W, const float* img, const float* gt, const float* ma
 	const float inv_n = 1.0f / (3.0f * (float)H * (float)W);
 	dim3 grid((W + LT - 1) / LT, (H + LT - 1) / LT, 3);
 	if (partials) {
-		loss_fwd_det_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, -lambda_dssim * inv_n, dmap, partials);
+		if (E) loss_fwd_exp_det_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, -lambda_dssim * inv_n, dmap, partials, E);
+		else loss_fwd_det_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, -lambda_dssim * inv_n, dmap, partials);
 		PSB_LAUNCH_OK();
 		reduce_partials_kernel<<<1, 256, 0, stream>>>((int)(grid.x * grid.y * grid.z), partials, sums);
 	} else {
 		PSB_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), stream));
-		loss_fwd_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, -lambda_dssim * inv_n, dmap, sums);
+		if (E) loss_fwd_exp_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, -lambda_dssim * inv_n, dmap, sums, E);
+		else loss_fwd_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, -lambda_dssim * inv_n, dmap, sums);
 	}
 	PSB_LAUNCH_OK();
 	if (dL_dimg) {
-		loss_bwd_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, (1.0f - lambda_dssim) * inv_n, dmap, dL_dimg);
+		if (E) loss_bwd_exp_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, (1.0f - lambda_dssim) * inv_n, dmap, dL_dimg, E);
+		else loss_bwd_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, (1.0f - lambda_dssim) * inv_n, dmap, dL_dimg);
 		PSB_LAUNCH_OK();
 	}
+	return 0;
+}
+
+int launch_exposure(int H, int W, const float* img, const float* E, float* dL_dpix, double* partials, const uint32_t* counters, uint32_t capacity,
+                    const ExposureUpdate* update, float* grad, cudaStream_t stream)
+{
+	const int n = H * W;
+	const int grid = exposure_blocks(H, W);
+	exposure_mix_kernel<<<grid, 256, 0, stream>>>(n, E, img, dL_dpix, partials);
+	PSB_LAUNCH_OK();
+	ExposureUpdate u{};
+	if (update) u = *update;
+	exposure_update_kernel<<<1, 256, 0, stream>>>(grid, partials, counters, capacity, u, update ? nullptr : grad);
+	PSB_LAUNCH_OK();
 	return 0;
 }
 

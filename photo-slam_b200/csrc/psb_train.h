@@ -72,8 +72,25 @@ int launch_adam_live_rebuild(int P, const TrainTensors& t, unsigned char* adam_l
 int launch_adam(size_t n, float* p, float* m, float* v, const float* g, float lr, const StepHyper& h, float grad_scale, cudaStream_t stream);
 // partials != null (deterministic mode): scratch of loss_partials_doubles(H, W); the blocks store their sums there and one more
 // launch adds them in a fixed order, so sums[] is the same every run (the default double atomics add in completion order)
+// E != null: exposure compensation, the loss of mask * I' with I'(c) = sum_k E[k][c] I(k) + E[c][3] (E: device [3][4], row-major);
+// dL_dimg then receives g = dL/dI' (mask factor applied) and launch_exposure must follow.
 int launch_loss(int H, int W, const float* img, const float* gt, const float* mask, float lambda_dssim, float* dmap, double* sums,
-                float* dL_dimg, cudaStream_t stream, double* partials = nullptr);
+                float* dL_dimg, cudaStream_t stream, double* partials = nullptr, const float* E = nullptr);
+// The Adam state of one exposure row (psb_exposure): all device pointers, the step count advanced on the device.
+struct ExposureUpdate {
+	float* param;
+	float* exp_avg;
+	float* exp_avg_sq;
+	int* step;
+	float lr, beta1, beta2, eps;
+};
+// After launch_loss with E: dL_dpix (g) -> dL/dI in place, and the 12 sums dL/dE added in a fixed order (no atomics: the same every run).
+// update != null: the Adam step of the row; else grad [12] device receives dL/dE. An overflowing pass (counters[0] > capacity) leaves
+// the row, its moments and its step count untouched (grad: zeros). partials: exposure_blocks(H, W) * 12 doubles. Two launches.
+int launch_exposure(int H, int W, const float* img, const float* E, float* dL_dpix, double* partials, const uint32_t* counters, uint32_t capacity,
+                    const ExposureUpdate* update, float* grad, cudaStream_t stream);
+inline int exposure_blocks(int H, int W) { return min(cdiv(H * W, 256), kNumSMs * 8); }
+constexpr size_t kExposurePartials = 12 * (size_t)kNumSMs * 8;   // doubles: enough for any image
 // Depth L1 over the valid pixels (gt > 0 and, with a mask, mask[0, p] != 0): sums[0] = sum |D - G|, sums[1] = N_valid (zeroed here);
 // dL_dD [H,W] = lambda * sign(D - G) / max(N_valid, 1) on valid pixels, 0 elsewhere. Two launches, no host synchronisation.
 // partials: as launch_loss.

@@ -55,6 +55,9 @@ struct psb_trainer {
 	float* det_slots = nullptr; size_t det_cap = 0;
 	uint32_t* det_base = nullptr; size_t det_P = 0;
 	double* det_partials = nullptr; size_t det_parts = 0;
+	// exposure compensation (psb_trainer_step_exposure / psb_trainer_backward_exposure): the block partials of the 12 exposure sums
+	// [kExposurePartials] doubles, made by the first such call
+	double* exp_partials = nullptr;
 	// optional per-stage timing (CUDA events on the step's stream)
 	bool profiling = false;
 	// stage boundaries: 0 start | 1 preprocess | 2 depth sort | 3 binning | 4 render fwd | 5 loss | 6 render bwd |
@@ -243,6 +246,22 @@ int check_depth(const psb_depth* d, const char* fn)
 	return 0;
 }
 
+// NULL: no exposure. Otherwise a row (param), a finite lr >= 0 and, for a step (`adam`), the moments and the device step count; for the
+// gradient mode a gradient output.
+int check_exposure(const psb_exposure* e, bool adam, const float* grad, const char* fn)
+{
+	if (!e) return 0;
+	if (!e->param || (adam && (!e->exp_avg || !e->exp_avg_sq || !e->step)) || (!adam && !grad)) {
+		set_error_msg(std::string(fn).append(adam ? ": exposure needs param, exp_avg, exp_avg_sq and step" : ": exposure needs param and exposure_grad").c_str());
+		return PSB_ERR_ARG;
+	}
+	if (!std::isfinite(e->lr) || e->lr < 0.f) {
+		set_error_msg(std::string(fn).append(": exposure lr must be finite and >= 0").c_str());
+		return PSB_ERR_ARG;
+	}
+	return 0;
+}
+
 // Gradient segments of P rows: six non-null pointers, features_rest and rotation 16-byte aligned (written with float4 stores).
 int check_grads(float* const* grads, int P, const char* fn)
 {
@@ -330,11 +349,12 @@ struct TileBackward {
 	bool aa;     // the forward was anti-aliased: the per-Gaussian stage runs the AA variant
 };
 
-// The built-in loss around the shared stages: forward -> loss (+ depth loss) -> pinned read-back of the loss sums -> tile backward.
-// `moments`: the caller's per-Gaussian stage updates the Adam moments of the model.
+// The built-in loss around the shared stages: forward -> loss (+ depth loss) -> pinned read-back of the loss sums -> (exposure) -> tile
+// backward. `moments`: the caller's per-Gaussian stage updates the Adam moments of the model. exposure != NULL: the loss is that of the
+// image through the row; exposure_grad == NULL: the row takes its Adam step (with step's betas and eps), else dL/dE -> exposure_grad.
 int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                          const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
-                         bool moments, cudaStream_t stream, TileBackward& out)
+                         bool moments, cudaStream_t stream, TileBackward& out, const psb_exposure* exposure = nullptr, float* exposure_grad = nullptr)
 {
 	int rc;
 	if (!t || !camera || !step || !background || !gt_image) { set_error_msg("psb_trainer_step: null argument"); return PSB_ERR_ARG; }
@@ -349,6 +369,10 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 		if (!depth_plane) depth_plane = t->depth_buf;
 		dL_ddepth = t->depth_buf + (size_t)camera->width * camera->height;
 	}
+	if (exposure && !t->exp_partials) {
+		PSB_CUDA_OK(cudaStreamSynchronize(stream));
+		if ((rc = dev_alloc(&t->exp_partials, kExposurePartials))) return rc;
+	}
 	Scratch sc;
 	Camera cam;
 	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, sc, cam, stream, depth_plane))) return rc;
@@ -357,7 +381,9 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	t->pass_D = -1;
 	const float* image = out_color ? out_color : t->image;
 	double* partials = t->deterministic ? t->det_partials : nullptr;
-	if ((rc = launch_loss(cam.H, cam.W, image, gt_image, mask, step->lambda_dssim, t->dmap, t->sums, t->dL_dpix, stream, partials))) return rc;
+	if ((rc = launch_loss(cam.H, cam.W, image, gt_image, mask, step->lambda_dssim, t->dmap, t->sums, t->dL_dpix, stream, partials,
+	                      exposure ? exposure->param : nullptr)))
+		return rc;
 	if (depth_loss &&
 	    (rc = launch_depth_loss(cam.H, cam.W, depth_plane, depth->gt_depth, mask, depth->lambda_depth, t->sums + 2, dL_ddepth, stream, partials)))
 		return rc;
@@ -369,6 +395,13 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	t->last_lambda_depth = depth_loss ? depth->lambda_depth : 0.f;
 	t->have_loss = true;
 	t->have_depth_loss = depth_loss;
+	if (exposure) {
+		// dL/dI for the tile backward and the row's update (or gradient), inside stage "loss"; the row moves only after every read of it
+		ExposureUpdate u{exposure->param, exposure->exp_avg, exposure->exp_avg_sq, exposure->step, exposure->lr, step->beta1, step->beta2, step->eps};
+		if ((rc = launch_exposure(cam.H, cam.W, image, exposure->param, t->dL_dpix, t->exp_partials, P > 0 ? sc.geom.counters : nullptr,
+		                          (uint32_t)t->capacity, exposure_grad ? nullptr : &u, exposure_grad, stream)))
+			return rc;
+	}
 	t->mark(5, stream);
 	if (P == 0) return 0;
 	if ((rc = tile_backward(t, P, sc, cam, background, t->dL_dpix, dL_ddepth, nullptr, stream))) return rc;
@@ -574,7 +607,7 @@ int psb_trainer_destroy(psb_trainer* t)
 	if (!t) return 0;
 	cudaFree(t->geom_chunk); cudaFree(t->img_chunk); cudaFree(t->bin_chunk); cudaFree(t->image); cudaFree(t->dL_dpix); cudaFree(t->dmap);
 	cudaFree(t->sink); cudaFree(t->seeds); cudaFree(t->sums); cudaFree(t->ovf); cudaFree(t->depth_buf);
-	cudaFree(t->det_slots); cudaFree(t->det_base); cudaFree(t->det_partials);
+	cudaFree(t->det_slots); cudaFree(t->det_base); cudaFree(t->det_partials); cudaFree(t->exp_partials);
 	if (t->ev_ready) for (int i = 0; i <= psb_trainer::NSTAGE; i++) cudaEventDestroy(t->ev[i]);
 	if (t->h_sums) cudaFreeHost(t->h_sums);
 	if (t->h_count) cudaFreeHost(t->h_count);
@@ -671,11 +704,21 @@ int psb_trainer_step_depth(psb_trainer* t, int P, int M, const psb_model* model,
                            const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
                            void* stream_)
 {
+	return psb_trainer_step_exposure(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, nullptr, stream_);
+}
+
+int psb_trainer_step_exposure(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                              const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
+                              const psb_exposure* exposure, void* stream_)
+{
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
-	if ((rc = check_depth(depth, "psb_trainer_step_depth"))) return rc;
+	const char* fn = exposure ? "psb_trainer_step_exposure" : "psb_trainer_step_depth";
+	if ((rc = check_depth(depth, fn))) return rc;
+	if ((rc = check_exposure(exposure, true, nullptr, fn))) return rc;
 	TileBackward tb;
-	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, true, stream, tb)) || P == 0)
+	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, true, stream, tb, exposure)) ||
+	    P == 0)
 		return rc;
 	rc = launch_fused_backward(true, 0, P, train_tensors(model, true), tb.cam, tb.geom, t->sink, t->seeds, to_hyper(step), GradSegments{},
 	                           densify_stats(model, step), tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), model->adam_live, tb.depth, tb.aa);
@@ -695,12 +738,23 @@ int psb_trainer_backward_depth(psb_trainer* t, int P, int M, const psb_model* mo
                                const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, float* const* grads,
                                const psb_depth* depth, void* stream_)
 {
+	return psb_trainer_backward_exposure(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, grads, depth, nullptr, nullptr,
+	                                     stream_);
+}
+
+int psb_trainer_backward_exposure(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                                  const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, float* const* grads,
+                                  const psb_depth* depth, const psb_exposure* exposure, float* exposure_grad, void* stream_)
+{
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
-	if ((rc = check_depth(depth, "psb_trainer_backward_depth"))) return rc;
+	if ((rc = check_depth(depth, exposure ? "psb_trainer_backward_exposure" : "psb_trainer_backward_depth"))) return rc;
+	if ((rc = check_exposure(exposure, false, exposure_grad, "psb_trainer_backward_exposure"))) return rc;
 	if ((rc = check_grads(grads, P, "psb_trainer_backward"))) return rc;
 	TileBackward tb;
-	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, stream, tb)) || P == 0)
+	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, stream, tb, exposure,
+	                               exposure ? exposure_grad : nullptr)) ||
+	    P == 0)
 		return rc;
 	GradSegments gs;
 	for (int i = 0; i < 6; i++) gs.g[i] = grads[i];

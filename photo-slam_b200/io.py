@@ -167,6 +167,38 @@ def save_model_params(path, eval_=False, images="images", model_path="", resolut
     return txt
 
 
+def save_exposure(path, rows):
+    """exposure.json in graphdeco's form, {"<id>": 3x4 list}: rows maps a keyframe id to its 3x4 exposure row (row-major, E[:3,:3]
+    right-multiplies HWC pixels, E[:3,3] is the bias)."""
+    out = {}
+    for k, row in rows.items():
+        a = np.asarray(row, np.float64)
+        if a.shape != (3, 4):
+            raise ValueError(f"exposure row {k}: want shape (3, 4), got {a.shape}")
+        out[str(int(k))] = [[float(x) for x in r] for r in a]
+    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
+    with open(path, "w") as f:
+        json.dump(out, f, indent=1)
+    return out
+
+
+def load_exposure(path):
+    """exposure.json -> {keyframe id (int): float32 [3,4] array}. Keys must be integer ids."""
+    with open(path) as f:
+        raw = json.load(f)
+    rows = {}
+    for k, v in raw.items():
+        try:
+            kid = int(k)
+        except ValueError:
+            raise ValueError(f"{path}: key {k!r} is not a keyframe id") from None
+        a = np.asarray(v, np.float32)
+        if a.shape != (3, 4) or kid < 0:
+            raise ValueError(f"{path}: entry {k!r}: want a 3x4 list under a non-negative id")
+        rows[kid] = a
+    return rows
+
+
 def save_result_dir(result_dir, iteration, model_arrays, keyframes=(), sparse_xyz=None, sparse_color=None, **model_params):
     """Directory layout of GaussianMapper::savePly (gaussian_mapper.cpp:1658-1673): cameras.json, cfg_args,
     point_cloud/iteration_<n>/point_cloud.ply, input.ply."""

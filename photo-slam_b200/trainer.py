@@ -52,6 +52,10 @@ def _cdepth(gt_depth, lambda_depth, out_depth):
                   out_depth.data_ptr() if out_depth is not None else None)
 
 
+class _Exposure(C.Structure):
+    _fields_ = [("param", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p), ("step", C.c_void_p), ("lr", C.c_float)]
+
+
 class _PixelGrads(C.Structure):
     _fields_ = [("dL_dcolor", C.c_void_p), ("dL_ddepth", C.c_void_p), ("dL_dalpha", C.c_void_p)]
 
@@ -96,6 +100,8 @@ def _bind():
     L.psb_trainer_backward_depth.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp, vp,
                                              C.POINTER(vp), C.POINTER(_Depth), vp]
     L.psb_trainer_result_depth.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int), vp]
+    L.psb_trainer_step_exposure.argtypes = L.psb_trainer_step_depth.argtypes[:-1] + [C.POINTER(_Exposure), vp]
+    L.psb_trainer_backward_exposure.argtypes = L.psb_trainer_backward_depth.argtypes[:-1] + [C.POINTER(_Exposure), vp, vp]
     L.psb_dp_step_depth.argtypes = [vp, vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp, vp,
                                     C.POINTER(_Depth), vp]
     L.psb_trainer_backward_begin_depth.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp,
@@ -109,7 +115,8 @@ def _bind():
     for n in ("psb_trainer_create", "psb_trainer_destroy", "psb_trainer_render", "psb_trainer_step", "psb_trainer_backward",
               "psb_adam_update", "psb_trainer_result", "psb_loss", "psb_trainer_render_depth", "psb_trainer_step_depth",
               "psb_trainer_backward_depth", "psb_trainer_result_depth", "psb_dp_step_depth", "psb_trainer_backward_begin_depth",
-              "psb_trainer_set_deterministic", "psb_trainer_forward", "psb_trainer_backward_pixels", "psb_trainer_set_antialiasing"):
+              "psb_trainer_set_deterministic", "psb_trainer_forward", "psb_trainer_backward_pixels", "psb_trainer_set_antialiasing",
+              "psb_trainer_step_exposure", "psb_trainer_backward_exposure"):
         getattr(L, n).restype = C.c_int
     L.psb_densify_workspace_bytes.argtypes = [C.c_int]
     L.psb_densify_workspace_bytes.restype = C.c_size_t
@@ -145,6 +152,7 @@ class GaussianOptimizationParams:
     densify_from_iter: int = 600
     densify_until_iter: int = 15000
     densify_grad_threshold: float = 0.001
+    exposure_lr: float = 0.01     # learning rate of the per-keyframe exposure rows (graphdeco's exposure_lr_init)
 
 
 class GaussianModel:
@@ -159,6 +167,12 @@ class GaussianModel:
         self.step_ = 0
         self.lr_delay_steps_ = 0
         self.percent_dense_ = 0.01
+        self.exposure_lr_ = GaussianOptimizationParams.exposure_lr
+        z = lambda *s, dtype=torch.float32: torch.zeros(s, dtype=dtype, device=self.device)
+        # per-keyframe exposure table (ensureExposures): row k = the 3x4 affine of the caller's keyframe id k, its Adam moments and its
+        # own Adam step count (advanced on the device by the fused step)
+        self.exposure_, self.exposure_exp_avg_, self.exposure_exp_avg_sq_ = z(0, 3, 4), z(0, 3, 4), z(0, 3, 4)
+        self.exposure_step_ = z(0, dtype=torch.int32)
 
     @classmethod
     def from_numpy(cls, scene, device="cuda", sh_degree=3):
@@ -194,6 +208,7 @@ class GaussianModel:
         self.lr_final_ = args.position_lr_final * self.spatial_lr_scale_
         self.lr_delay_mult_ = args.position_lr_delay_mult
         self.max_steps_ = args.position_lr_max_steps
+        self.exposure_lr_ = args.exposure_lr
 
     # --- training-state snapshot (parameters, Adam moments, densification statistics, step counter); restore copies in
     #     place so device pointers held elsewhere stay valid. Used by bench.py to time every leg on the same iterations.
@@ -202,7 +217,8 @@ class GaussianModel:
         live = self._live_tensor()
         return dict(p=c(self.tensors()), m=c(self.exp_avg_), v=c(self.exp_avg_sq_),
                     stats=c([self.xyz_gradient_accum_, self.denom_, self.max_radii2D_]), step=self.step_, lr=list(self.lr_),
-                    sh=self.active_sh_degree_, live=live.clone(), live_valid=self.adam_live_valid_)
+                    sh=self.active_sh_degree_, live=live.clone(), live_valid=self.adam_live_valid_,
+                    exposure=c(self._exposure_tensors()), exposure_lr=self.exposure_lr_)
 
     def restore(self, snap):
         assert snap["p"][0].shape == self.xyz_.shape, "restore: the model was resized since the snapshot"
@@ -212,6 +228,12 @@ class GaussianModel:
         self.step_, self.lr_, self.active_sh_degree_ = snap["step"], list(snap["lr"]), snap["sh"]
         self._live_tensor().copy_(snap["live"])
         self.adam_live_valid_ = snap["live_valid"]
+        if snap["exposure"][0].shape == self.exposure_.shape:
+            for dst, src in zip(self._exposure_tensors(), snap["exposure"]):
+                dst.copy_(src)
+        else:   # the table grew since the snapshot
+            self.exposure_, self.exposure_exp_avg_, self.exposure_exp_avg_sq_, self.exposure_step_ = [t.clone() for t in snap["exposure"]]
+        self.exposure_lr_ = snap["exposure_lr"]
 
     def _live_tensor(self):
         """adam_live_, (re)allocated when the row count changed (its content is then stale)."""
@@ -219,6 +241,53 @@ class GaussianModel:
             self.adam_live_ = torch.zeros(self.num_points(), dtype=torch.uint8, device=self.device)
             self.adam_live_valid_ = False
         return self.adam_live_
+
+    # --- per-keyframe exposure compensation: GaussianTrainer.trainForOneIteration(..., exposure_id=k) trains the map against keyframe k's
+    #     image through row k, I'(c) = sum_j E[j][c] I(j) + E[c][3] (psb_exposure), and takes one Adam step of that row
+    def _exposure_tensors(self):
+        return [self.exposure_, self.exposure_exp_avg_, self.exposure_exp_avg_sq_, self.exposure_step_]
+
+    def numExposures(self):
+        return self.exposure_.size(0)
+
+    def ensureExposures(self, K):
+        """Grows the exposure table to at least K rows. New rows are eye(3, 4) with zero moments and step count; existing rows,
+        moments and step counts are kept. Growing reallocates the tensors."""
+        n = self.numExposures()
+        if K <= n:
+            return
+        z = torch.zeros((K - n, 3, 4), dtype=torch.float32, device=self.device)
+        eye = torch.eye(3, 4, dtype=torch.float32, device=self.device).expand(K - n, 3, 4)
+        self.exposure_ = torch.cat([self.exposure_, eye], 0).contiguous()
+        self.exposure_exp_avg_ = torch.cat([self.exposure_exp_avg_, z], 0).contiguous()
+        self.exposure_exp_avg_sq_ = torch.cat([self.exposure_exp_avg_sq_, z.clone()], 0).contiguous()
+        self.exposure_step_ = torch.cat([self.exposure_step_, torch.zeros(K - n, dtype=torch.int32, device=self.device)]).contiguous()
+
+    def applyExposure(self, image, k):
+        """image [3,H,W] through exposure row k (graphdeco's form: HWC pixels times E[:3,:3], plus E[:3,3]): the image the fused
+        step compares with keyframe k's target. For evaluating against that keyframe and for display."""
+        E = self.exposure_[int(k)].to(image.dtype)
+        return torch.matmul(image.permute(1, 2, 0), E[:, :3]).permute(2, 0, 1) + E[:, 3, None, None]
+
+    def setExposureLearningRate(self, lr): self.exposure_lr_ = float(lr)
+
+    def saveExposure(self, path):
+        """exposure.json: {"<keyframe id>": 3x4 list} for every row of the table."""
+        from . import io
+        io.save_exposure(path, {k: row for k, row in enumerate(self.exposure_.detach().cpu().numpy())})
+
+    def loadExposure(self, path):
+        """Reads exposure.json into the table (grown as needed). The loaded rows restart their Adam state (zero moments and step)."""
+        from . import io
+        rows = io.load_exposure(path)
+        if not rows:
+            return
+        self.ensureExposures(max(rows) + 1)
+        for k, row in rows.items():
+            self.exposure_[k] = torch.from_numpy(row).to(self.device)
+            self.exposure_exp_avg_[k] = 0.0
+            self.exposure_exp_avg_sq_[k] = 0.0
+            self.exposure_step_[k] = 0
 
     def invalidateAdamLive(self):
         """Call after writing moments by any means other than the fused step (the next fused step rebuilds the live bytes)."""
@@ -632,12 +701,23 @@ class GaussianTrainer:
         return self._last_loss
 
     def trainForOneIteration(self, cam, gt_image, mask=None, out_color=None, radii=None, densify_stats=None, gt_depth=None, lambda_depth=0.0,
-                             out_depth=None):
+                             out_depth=None, exposure_id=None):
         """Enqueues render -> loss -> backward -> Adam on the current stream (no host sync).
         gt_depth: [H,W] float32 target depth in metres (<= 0: no measurement) trained with weight lambda_depth (> 0) as an L1 term
-        over the valid pixels (psb_trainer_step_depth); out_depth: [H,W] float32 tensor that receives the rendered depth."""
+        over the valid pixels (psb_trainer_step_depth); out_depth: [H,W] float32 tensor that receives the rendered depth.
+        exposure_id: the keyframe id k of gt_image, or None. With an id, the loss compares gt_image with the render through exposure row
+        k of the model (applyExposure; the table grows to k + 1 rows if needed) and that row takes one Adam step at
+        model.exposure_lr_ (psb_trainer_step_exposure). out_color stays the raw render; result() reports the compensated loss."""
         m = self.model
         depth = _cdepth(gt_depth, lambda_depth, out_depth)
+        exposure = None
+        if exposure_id is not None:
+            k = int(exposure_id)
+            if k < 0:
+                raise ValueError(f"exposure_id must be >= 0, got {exposure_id}")
+            m.ensureExposures(k + 1)
+            exposure = _Exposure(m.exposure_[k].data_ptr(), m.exposure_exp_avg_[k].data_ptr(), m.exposure_exp_avg_sq_[k].data_ptr(),
+                                 m.exposure_step_[k:].data_ptr(), float(m.exposure_lr_))
         self._apply_deterministic()
         self.iteration += 1
         if densify_stats is None:
@@ -647,12 +727,15 @@ class GaussianTrainer:
                 mask.data_ptr() if mask is not None else None, C.byref(cs), out_color.data_ptr() if out_color is not None else None,
                 radii.data_ptr() if radii is not None else None)
         stream = torch.cuda.current_stream().cuda_stream
-        if depth is None:
+        if exposure is not None:
+            _lib.check(self.L.psb_trainer_step_exposure(*args, C.byref(depth) if depth is not None else None, C.byref(exposure), stream),
+                       "psb_trainer_step_exposure")
+        elif depth is None:
             _lib.check(self.L.psb_trainer_step(*args, stream), "psb_trainer_step")
         else:
             _lib.check(self.L.psb_trainer_step_depth(*args, C.byref(depth), stream), "psb_trainer_step_depth")
         m.step_ += 1
-        self._last = (cam, gt_image, mask, out_color, radii, densify_stats, gt_depth, lambda_depth, out_depth)
+        self._last = (cam, gt_image, mask, out_color, radii, densify_stats, gt_depth, lambda_depth, out_depth, exposure_id)
 
     def _overflow_info(self):
         f, n, cur = C.c_uint(), C.c_uint(), C.c_uint()
@@ -704,8 +787,8 @@ class GaussianTrainer:
             if isinstance(self._last, _LossCall):
                 self.trainWithLoss(*self._last)
             else:
-                cam, gt, mask, oc, rad, ds, gd, ld, od = self._last
-                self.trainForOneIteration(cam, gt, mask, oc, rad, ds, gt_depth=gd, lambda_depth=ld, out_depth=od)
+                cam, gt, mask, oc, rad, ds, gd, ld, od, ek = self._last
+                self.trainForOneIteration(cam, gt, mask, oc, rad, ds, gt_depth=gd, lambda_depth=ld, out_depth=od, exposure_id=ek)
             return self._result(with_depth)
         _lib.check(rc, "psb_trainer_result_depth" if with_depth else "psb_trainer_result")
         if isinstance(getattr(self, "_last", None), _LossCall):
@@ -967,10 +1050,14 @@ class DataParallelTrainer(GaussianTrainer):
         self.flat = self.grads.flat
 
     def trainForOneIteration(self, cam, gt_image, mask=None, out_color=None, radii=None, densify_stats=None, gt_depth=None, lambda_depth=0.0,
-                             out_depth=None):
+                             out_depth=None, exposure_id=None):
         """Depth arguments as in GaussianTrainer, on every path: "p2p" (psb_dp_step_depth), the slab pipeline
         (psb_trainer_backward_begin_depth) and the flat "nccl" path (psb_trainer_backward_depth). Each rank passes its own view's
-        target or none: ranks with and without a depth term may train in the same step."""
+        target or none: ranks with and without a depth term may train in the same step. exposure_id must be None."""
+        if exposure_id is not None:
+            raise NotImplementedError("DataParallelTrainer: exposure compensation is not wired into the data-parallel steps: the per-keyframe "
+                                      "exposure table would have to be replicated across the ranks (each rank's row updates gathered to "
+                                      "every rank every step); train with exposure on one GPU through GaussianTrainer")
         m = self.model
         depth = _cdepth(gt_depth, lambda_depth, out_depth)
         self._apply_deterministic()
