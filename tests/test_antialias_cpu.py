@@ -15,6 +15,7 @@ import pytest
 import torch
 
 from photo_slam_b200 import _lib
+from splat64 import h_torch, quat_cov as _quat_cov
 
 DILATION = 0.3
 MIN_RATIO = 2.5e-5
@@ -86,50 +87,7 @@ def test_h_is_one_minus_dilation_effect_for_large_splats_and_the_clamp_for_thin_
     assert np.allclose(aa_h(np.array([4.0]), np.array([2.0]), np.array([1.0])), np.sqrt(MIN_RATIO))
 
 
-# ---- the torch restatement (the GPU tests' oracle) --------------------------------------------------------------------------------
-def _quat_cov(scales, rot):
-    """cov3D [P,6] of scale and (w, x, y, z) quaternion exactly as cov3d_from_scale_rot: the quaternion is not normalised"""
-    r, x, y, z = rot.unbind(1)
-    R = torch.stack([torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - r * z), 2 * (x * z + r * y)], 1),
-                     torch.stack([2 * (x * y + r * z), 1 - 2 * (x * x + z * z), 2 * (y * z - r * x)], 1),
-                     torch.stack([2 * (x * z - r * y), 2 * (y * z + r * x), 1 - 2 * (x * x + y * y)], 1)], 1)
-    S = R * scales.unsqueeze(1)              # R diag(s): Sigma = R diag(s^2) R^T
-    Sig = S @ S.transpose(1, 2)
-    return torch.stack([Sig[:, 0, 0], Sig[:, 0, 1], Sig[:, 0, 2], Sig[:, 1, 1], Sig[:, 1, 2], Sig[:, 2, 2]], 1)
-
-
-def h_torch(means3D, cov6, viewmatrix, W, H, tanfovx, tanfovy):
-    """h of every Gaussian (1 where view z <= 0.2), differentiable in means3D and cov6; the dtype of the inputs. The mean's 1.3 tanfov
-    clamp follows the kernels' backward (SURVEY.md Appendix A): a clamped coordinate passes no gradient to the mean, and J's
-    dependence on it through t.z is dropped."""
-    V = viewmatrix.reshape(4, 4).to(means3D.dtype)
-    t = means3D @ V[:3, :3] + V[3, :3]
-    front = (t[:, 2] > 0.2).detach()
-    t = torch.where(front.unsqueeze(1), t, torch.tensor([0.0, 0.0, 1.0], dtype=t.dtype, device=t.device))
-    tz = t[:, 2]
-    fx, fy = W / (2.0 * tanfovx), H / (2.0 * tanfovy)
-    cols = []
-    for k, lim in ((0, 1.3 * tanfovx), (1, 1.3 * tanfovy)):
-        r = t[:, k] / tz
-        out = (r < -lim) | (r > lim)
-        cols.append(torch.where(out, (r.clamp(-lim, lim) * tz).detach(), t[:, k]))
-    tx, ty = cols
-    zero = torch.zeros_like(tz)
-    J = torch.stack([torch.stack([fx / tz, zero, -(fx * tx) / (tz * tz)], 1),
-                     torch.stack([zero, fy / tz, -(fy * ty) / (tz * tz)], 1)], 1)           # [P,2,3]
-    Wr = V[:3, :3].T                                                                          # view rotation
-    c = cov6
-    Sig = torch.stack([torch.stack([c[:, 0], c[:, 1], c[:, 2]], 1), torch.stack([c[:, 1], c[:, 3], c[:, 4]], 1),
-                       torch.stack([c[:, 2], c[:, 4], c[:, 5]], 1)], 1)
-    T = J @ Wr
-    cov2 = T @ Sig @ T.transpose(1, 2)
-    a0, b, c0 = cov2[:, 0, 0], cov2[:, 0, 1], cov2[:, 1, 1]
-    det0 = a0 * c0 - b * b
-    det1 = (a0 + DILATION) * (c0 + DILATION) - b * b
-    h = torch.sqrt(torch.clamp_min(det0 / det1, MIN_RATIO))
-    return torch.where(front, h, torch.ones_like(h))
-
-
+# ---- the torch restatement (splat64.h_torch, the GPU tests' oracle) --------------------------------------------------------------------------------
 def _gradcheck_inputs(n=12, seed=0):
     import photo_slam_b200.synthetic as syn
     rng = np.random.default_rng(seed)

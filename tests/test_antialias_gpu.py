@@ -23,7 +23,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 from helpers import scene_tensors  # noqa: E402
-from test_antialias_cpu import _quat_cov, h_torch  # noqa: E402
+from splat64 import h_torch, quat_cov as _quat_cov  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(HERE)

@@ -9,50 +9,22 @@
 """
 import ctypes as C
 import json
-import math
 import os
 
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 from photo_slam_b200 import _lib, io, trainer
+from splat64 import exposed, loss64
 
 HEADER = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include", "psb200.h")
 ONE = 4096  # fake non-null device pointer; never dereferenced because validation fails first
 
 
 # ---- the spec ----------------------------------------------------------------------------------------------------------------------
-def _window64():
-    g = torch.tensor([math.exp(-(x - 5) ** 2 / (2.0 * 1.5 * 1.5)) for x in range(11)], dtype=torch.float64)
-    g = (g / g.sum()).unsqueeze(1)
-    return g.mm(g.t()).unsqueeze(0).unsqueeze(0).expand(3, 1, 11, 11).contiguous()
-
-
-def ssim64(img1, img2):
-    """oracle/ref_trainer.py's ssim with the window built in float64"""
-    window = _window64()
-    a, b = img1.unsqueeze(0), img2.unsqueeze(0)
-    mu1 = F.conv2d(a, window, padding=5, groups=3)
-    mu2 = F.conv2d(b, window, padding=5, groups=3)
-    mu1_sq, mu2_sq, mu1_mu2 = mu1.pow(2), mu2.pow(2), mu1 * mu2
-    sigma1_sq = F.conv2d(a * a, window, padding=5, groups=3) - mu1_sq
-    sigma2_sq = F.conv2d(b * b, window, padding=5, groups=3) - mu2_sq
-    sigma12 = F.conv2d(a * b, window, padding=5, groups=3) - mu1_mu2
-    C1, C2 = 0.01 * 0.01, 0.03 * 0.03
-    ssim_map = ((2 * mu1_mu2 + C1) * (2 * sigma12 + C2)) / ((mu1_sq + mu2_sq + C1) * (sigma1_sq + sigma2_sq + C2))
-    return ssim_map.mean()
-
-
-def exposed(I, E):
-    """I'(c, p) = sum_k E[k][c] I(k, p) + E[c][3]"""
-    return torch.einsum("khw,kc->chw", I, E[:, :3]) + E[:, 3, None, None]
-
-
 def loss_of_prime(Ip, G, mask, lam):
-    X = mask * Ip
-    return (1.0 - lam) * (X - G).abs().mean() + lam * (1.0 - ssim64(X, G))
+    return loss64(Ip, G, mask, lam)[0]
 
 
 def loss(I, E, G, mask, lam):

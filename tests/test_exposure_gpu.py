@@ -18,6 +18,7 @@ import pytest
 import torch
 
 from helpers import scene_tensors
+from splat64 import ssim64
 
 pytestmark = pytest.mark.gpu
 LAMBDA_DSSIM = 0.2
@@ -83,20 +84,6 @@ def _exposure_grads(tr, c, gt, mask, gd, E, segs):
     return egrad
 
 
-def _ssim64(img1, img2):
-    import torch.nn.functional as F
-    g = torch.tensor([math.exp(-(x - 5) ** 2 / (2.0 * 1.5 * 1.5)) for x in range(11)], dtype=torch.float64, device=img1.device)
-    g = (g / g.sum()).unsqueeze(1)
-    window = g.mm(g.t()).unsqueeze(0).unsqueeze(0).expand(3, 1, 11, 11).contiguous()
-    a, b = img1.unsqueeze(0), img2.unsqueeze(0)
-    mu1, mu2 = F.conv2d(a, window, padding=5, groups=3), F.conv2d(b, window, padding=5, groups=3)
-    s1 = F.conv2d(a * a, window, padding=5, groups=3) - mu1 * mu1
-    s2 = F.conv2d(b * b, window, padding=5, groups=3) - mu2 * mu2
-    s12 = F.conv2d(a * b, window, padding=5, groups=3) - mu1 * mu2
-    C1, C2 = 0.01 ** 2, 0.03 ** 2
-    return (((2 * mu1 * mu2 + C1) * (2 * s12 + C2)) / ((mu1 * mu1 + mu2 * mu2 + C1) * (s1 + s2 + C2))).mean()
-
-
 def _reference_grads(tr, c, gt, mask, gd, E, grads):
     """float64 autograd of the definition on render(), then dL/dI through backwardPixels(grads=...): -> dL/dE [3,4] float64"""
     m = tr.model
@@ -108,7 +95,7 @@ def _reference_grads(tr, c, gt, mask, gd, E, grads):
     E64 = E.double().requires_grad_(True)
     X = mask.double() * (torch.einsum("khw,kc->chw", I, E64[:, :3]) + E64[:, 3, None, None])
     G = gt.double()
-    L = (1 - LAMBDA_DSSIM) * (X - G).abs().mean() + LAMBDA_DSSIM * (1 - _ssim64(X, G))
+    L = (1 - LAMBDA_DSSIM) * (X - G).abs().mean() + LAMBDA_DSSIM * (1 - ssim64(X, G))
     dI, dE = torch.autograd.grad(L, (I, E64))
     dD = None
     if gd is not None:   # the built-in depth L1: lambda * sign(D - G) / max(N_valid, 1) on the valid pixels
