@@ -66,13 +66,13 @@ static int arg_error(const char* fn, const char* what)
 	return PSB_ERR_ARG;
 }
 
-// Body of psb_rasterize_forward[_depth]; fn names the entry point in error messages. out_depth [H,W] or NULL.
+// Body of psb_rasterize_forward[_depth|_aa]; fn names the entry point in error messages. out_depth [H,W] or NULL; aa: the 2D Mip filter.
 static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void* geometry_user, psb_alloc_fn binning_buffer, void* binning_user,
                              psb_alloc_fn image_buffer, void* image_user, int P, int D, int M, const float* background, int width, int height,
                              const float* means3D, const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
                              float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
                              const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered, float* out_color,
-                             int* radii, float* out_depth, void* stream_, bool aa = false)
+                             int* radii, float* out_depth, bool aa, void* stream_)
 {
 	(void)prefiltered;  // the reference only uses it for a device-side assert (auxiliary.h:156-160)
 	cudaStream_t stream = (cudaStream_t)stream_;
@@ -118,24 +118,36 @@ static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void*
 // Scratch bytes of the deterministic operator backward; 0 for a negative size.
 static size_t op_det_bytes(int P, int R) { return (P < 0 || R < 0) ? 0 : OpDetState::required_bytes((size_t)P, (size_t)R); }
 
-// Body of psb_rasterize_backward[_depth|_deterministic]. dL_ddepth [H,W] or NULL; with it, dL_dz [P] receives dL/dz and the depth
-// variants run. det: the deterministic variant over det_scratch (det_bytes: its size; both checked here, before any CUDA call).
+// What an entry point adds to the plain backward. dL_ddepth [H,W] or NULL; with it, dL_dz [P] receives dL/dz and the depth variants
+// run. det: the deterministic variant over det_scratch (det_bytes: its size). aa: the forward was anti-aliased.
+struct BwdVariant {
+	const float* dL_ddepth;
+	float* dL_dz;
+	void* det_scratch;
+	size_t det_bytes;
+	bool det, aa;
+};
+
+// Body of psb_rasterize_backward[_depth|_deterministic|_aa]; fn names the entry point in error messages. Every argument check comes
+// before any CUDA call.
 static int rasterize_backward(const char* fn, int P, int D, int M, int R, const float* background, int width, int height, const float* means3D,
                               const float* shs, const float* colors_precomp, const float* scales, float scale_modifier, const float* rotations,
                               const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix, const float* campos, float tan_fovx,
                               float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer, const float* dL_dpix,
                               float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dmean3D, float* dL_dcov3D,
-                              float* dL_dsh, float* dL_dscale, float* dL_drot, const float* dL_ddepth, float* dL_dz, void* stream_,
-                              bool det = false, void* det_scratch = nullptr, size_t det_bytes = 0, bool aa = false)
+                              float* dL_dsh, float* dL_dscale, float* dL_drot, const BwdVariant& v, void* stream_)
 {
 	(void)radii;  // visibility is re-derived from the private geometry state (tiles_touched), identical to radii > 0
 	cudaStream_t stream = (cudaStream_t)stream_;
+	const float* dL_ddepth = v.dL_ddepth;
+	float* dL_dz = v.dL_dz;
+	if (dL_ddepth && !dL_dz) return arg_error(fn, "dL_ddepth needs a dL_dz array");
 	if (P == 0) return 0;
 	if (P < 0 || R < 0 || !geom_buffer || !binning_buffer || !image_buffer || !dL_dpix || !dL_dmean2D || !dL_dconic || !dL_dopacity || !dL_dcolor)
 		return arg_error(fn, "bad argument");
-	if (det && !det_scratch) return arg_error(fn, "det_scratch is NULL");
-	if (det && det_bytes < op_det_bytes(P, R))
-		return arg_error(fn, ("det_scratch holds " + std::to_string(det_bytes) + " bytes, psb_rasterize_backward_det_bytes(P, R) = " +
+	if (v.det && !v.det_scratch) return arg_error(fn, "det_scratch is NULL");
+	if (v.det && v.det_bytes < op_det_bytes(P, R))
+		return arg_error(fn, ("det_scratch holds " + std::to_string(v.det_bytes) + " bytes, psb_rasterize_backward_det_bytes(P, R) = " +
 		                      std::to_string(op_det_bytes(P, R))).c_str());
 	const Camera cam = make_camera(width, height, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy);
 	GeomState geom = GeomState::from_chunk(geom_buffer, (size_t)P);
@@ -150,30 +162,30 @@ static int rasterize_backward(const char* fn, int P, int D, int M, int R, const 
 	sink.packed = 0;
 	if (dL_ddepth) { sink.z = dL_dz; sink.z_stride = 1; }
 	int rc;
-	if (R > 0 && det) {
-		// Every (Gaussian, tile) sum goes to the slot of its instance, base[g] + the tile's row-major rank in g's full rectangle (the
-		// emission order of emit_instances_kernel), and the gather adds each Gaussian's slots in that order. The slots are zeroed on
-		// every call: a block handed back by the caller's allocator may hold tags of an earlier call, which the fixed seq would accept.
-		char* chunk = static_cast<char*>(det_scratch);
-		const OpDetState ds = OpDetState::from_chunk(chunk, (size_t)P, (size_t)R);
-		PSB_CUDA_OK(cudaMemsetAsync(ds.slots, 0, (size_t)R * 3 * sizeof(float4), stream));
-		if ((rc = launch_det_base(P, geom, ds.base, stream))) return rc;
-		DetSlots slots;
-		slots.slots = ds.slots; slots.base = ds.base; slots.tile_info = geom.tile_info; slots.counters = geom.counters;
-		slots.capacity = (uint32_t)R; slots.seq = 1u; slots.P = P; slots.tight = 0;
+	if (R > 0) {
+		DetSlots slots{};
+		if (v.det) {
+			// Every (Gaussian, tile) sum goes to the slot of its instance, base[g] + the tile's row-major rank in g's full rectangle (the
+			// emission order of emit_instances_kernel), and the gather adds each Gaussian's slots in that order. The slots are zeroed on
+			// every call: a block handed back by the caller's allocator may hold tags of an earlier call, which the fixed seq would accept.
+			char* chunk = static_cast<char*>(v.det_scratch);
+			const OpDetState ds = OpDetState::from_chunk(chunk, (size_t)P, (size_t)R);
+			PSB_CUDA_OK(cudaMemsetAsync(ds.slots, 0, (size_t)R * 3 * sizeof(float4), stream));
+			if ((rc = launch_det_base(P, geom, ds.base, stream))) return rc;
+			slots.slots = ds.slots; slots.base = ds.base; slots.tile_info = geom.tile_info; slots.counters = geom.counters;
+			slots.capacity = (uint32_t)R; slots.seq = 1u; slots.P = P; slots.tight = 0;
+		}
 		if ((rc = launch_render_backward(cam, img.ranges, bin.inst[sorted_slot(width, height)], geom.rec, background, img.final_T, img.n_contrib, dL_dpix,
-		                                 sink, stream, dL_ddepth, &slots)))
+		                                 sink, stream, dL_ddepth, v.det ? &slots : nullptr)))
 			return rc;
-	} else if (R > 0)
-		if ((rc = launch_render_backward(cam, img.ranges, bin.inst[sorted_slot(width, height)], geom.rec, background, img.final_T, img.n_contrib, dL_dpix, sink, stream, dL_ddepth)))
-			return rc;
+	}
 
 	const GaussIn in = make_input(P, D, M, means3D, shs, colors_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp);
 	GaussGradOut out;
 	out.dL_dmeans3D = dL_dmean3D; out.dL_dcov3D = dL_dcov3D; out.dL_dsh = dL_dsh; out.dL_dscales = dL_dscale; out.dL_drots = dL_drot;
 	// (AA: dL_dopacity holds dL/do' here, the per-Gaussian kernel turns it into dL/do)
 	if ((rc = launch_preprocess_backward(in, cam, geom, dL_dmean2D, 3, dL_dconic, 4, dL_dcolor, 3, out, stream, dL_ddepth ? dL_dz : nullptr,
-	                                     aa ? dL_dopacity : nullptr)))
+	                                     v.aa ? dL_dopacity : nullptr)))
 		return rc;
 	return 0;
 }
@@ -200,7 +212,7 @@ int psb_rasterize_forward(psb_alloc_fn geometry_buffer, void* geometry_user, psb
 {
 	return rasterize_forward("psb_rasterize_forward", geometry_buffer, geometry_user, binning_buffer, binning_user, image_buffer, image_user, P, D, M,
 	                         background, width, height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp,
-	                         viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, nullptr, stream);
+	                         viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, /*out_depth=*/nullptr, /*aa=*/false, stream);
 }
 
 int psb_rasterize_forward_depth(psb_alloc_fn geometry_buffer, void* geometry_user, psb_alloc_fn binning_buffer, void* binning_user,
@@ -212,7 +224,7 @@ int psb_rasterize_forward_depth(psb_alloc_fn geometry_buffer, void* geometry_use
 {
 	return rasterize_forward("psb_rasterize_forward_depth", geometry_buffer, geometry_user, binning_buffer, binning_user, image_buffer, image_user, P,
 	                         D, M, background, width, height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations,
-	                         cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, out_depth, stream);
+	                         cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, out_depth, /*aa=*/false, stream);
 }
 
 int psb_rasterize_backward(int P, int D, int M, int R, const float* background, int width, int height, const float* means3D, const float* shs,
@@ -225,7 +237,7 @@ int psb_rasterize_backward(int P, int D, int M, int R, const float* background, 
 	return rasterize_backward("psb_rasterize_backward", P, D, M, R, background, width, height, means3D, shs, colors_precomp, scales, scale_modifier,
 	                          rotations, cov3D_precomp, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, radii, geom_buffer, binning_buffer,
 	                          image_buffer, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale,
-	                          dL_drot, nullptr, nullptr, stream);
+	                          dL_drot, BwdVariant{}, stream);
 }
 
 int psb_rasterize_backward_depth(int P, int D, int M, int R, const float* background, int width, int height, const float* means3D,
@@ -236,11 +248,12 @@ int psb_rasterize_backward_depth(int P, int D, int M, int R, const float* backgr
                                  float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot, const float* dL_ddepth,
                                  float* dL_dz, void* stream)
 {
-	if (dL_ddepth && !dL_dz) return arg_error("psb_rasterize_backward_depth", "dL_ddepth needs a dL_dz array");
+	BwdVariant v{};
+	v.dL_ddepth = dL_ddepth; v.dL_dz = dL_dz;
 	return rasterize_backward("psb_rasterize_backward_depth", P, D, M, R, background, width, height, means3D, shs, colors_precomp, scales,
 	                          scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, radii, geom_buffer,
 	                          binning_buffer, image_buffer, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh,
-	                          dL_dscale, dL_drot, dL_ddepth, dL_dz, stream);
+	                          dL_dscale, dL_drot, v, stream);
 }
 
 size_t psb_rasterize_backward_det_bytes(int P, int R) { return op_det_bytes(P, R); }
@@ -254,11 +267,13 @@ int psb_rasterize_backward_deterministic(int P, int D, int M, int R, const float
                                          float* dL_dscale, float* dL_drot, const float* dL_ddepth, float* dL_dz, void* det_scratch,
                                          size_t det_scratch_bytes, void* stream)
 {
-	if (dL_ddepth && !dL_dz) return arg_error("psb_rasterize_backward_deterministic", "dL_ddepth needs a dL_dz array");
+	BwdVariant v{};
+	v.dL_ddepth = dL_ddepth; v.dL_dz = dL_dz;
+	v.det = true; v.det_scratch = det_scratch; v.det_bytes = det_scratch_bytes;
 	return rasterize_backward("psb_rasterize_backward_deterministic", P, D, M, R, background, width, height, means3D, shs, colors_precomp, scales,
 	                          scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, radii, geom_buffer,
 	                          binning_buffer, image_buffer, dL_dpix, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh,
-	                          dL_dscale, dL_drot, dL_ddepth, dL_dz, stream, /*det=*/true, det_scratch, det_scratch_bytes);
+	                          dL_dscale, dL_drot, v, stream);
 }
 
 int psb_rasterize_forward_aa(psb_alloc_fn geometry_buffer, void* geometry_user, psb_alloc_fn binning_buffer, void* binning_user,
@@ -271,7 +286,7 @@ int psb_rasterize_forward_aa(psb_alloc_fn geometry_buffer, void* geometry_user, 
 	if (antialiasing != 0 && antialiasing != 1) return arg_error("psb_rasterize_forward_aa", "antialiasing must be 0 or 1");
 	return rasterize_forward("psb_rasterize_forward_aa", geometry_buffer, geometry_user, binning_buffer, binning_user, image_buffer, image_user, P, D,
 	                         M, background, width, height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp,
-	                         viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, out_depth, stream, antialiasing != 0);
+	                         viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, out_depth, antialiasing != 0, stream);
 }
 
 int psb_rasterize_backward_aa(int P, int D, int M, int R, const float* background, int width, int height, const float* means3D, const float* shs,
@@ -284,11 +299,13 @@ int psb_rasterize_backward_aa(int P, int D, int M, int R, const float* backgroun
 {
 	const char* fn = "psb_rasterize_backward_aa";
 	if (antialiasing != 0 && antialiasing != 1) return arg_error(fn, "antialiasing must be 0 or 1");
-	if (dL_ddepth && !dL_dz) return arg_error(fn, "dL_ddepth needs a dL_dz array");
+	BwdVariant v{};
+	v.dL_ddepth = dL_ddepth; v.dL_dz = dL_dz;
+	v.det = det_scratch != nullptr; v.det_scratch = det_scratch; v.det_bytes = det_scratch_bytes;
+	v.aa = antialiasing != 0;
 	return rasterize_backward(fn, P, D, M, R, background, width, height, means3D, shs, colors_precomp, scales, scale_modifier, rotations, cov3D_precomp,
 	                          viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dmean2D,
-	                          dL_dconic, dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_ddepth, dL_dz, stream,
-	                          /*det=*/det_scratch != nullptr, det_scratch, det_scratch_bytes, antialiasing != 0);
+	                          dL_dconic, dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, v, stream);
 }
 
 int psb_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix, unsigned char* present, void* stream_)

@@ -8,7 +8,7 @@
 
 namespace psb {
 
-// DEPTH: dL/dz (view-space depth, render_bwd_depth_kernel's tenth sum) joins dL/dmean3D through the view matrix's z row,
+// DEPTH: dL/dz (view-space depth, the depth tile backward's tenth sum) joins dL/dmean3D through the view matrix's z row,
 // z = V[2] x + V[6] y + V[10] z + V[14] (column-major), as in gaussian_backward_kernel<MODE_DEPTH>.
 // AA: the forward blended o' = o h (preprocess_fwd_kernel<false, true>, o' in the record). dL_dopacity [P] holds dL/do' from the tile
 // backward (atomic or gathered); the h-term joins the covariance gradient and dL_dopacity[g] is rescaled in place to dL/do = h dL/do'.
@@ -66,37 +66,15 @@ __device__ __forceinline__ void preprocess_bwd_body(GaussIn in, Camera cam, Geom
 	}
 }
 
+// One entry for the four (DEPTH, AA) variants: dL_dz is read only when DEPTH, dL_dopacity only when AA.
+template <bool DEPTH, bool AA>
 __global__ void __launch_bounds__(128) preprocess_bwd_kernel(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
                                                              int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
-                                                             const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out)
+                                                             const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out,
+                                                             const float* __restrict__ dL_dz, float* __restrict__ dL_dopacity)
 {
-	preprocess_bwd_body<false>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out, nullptr);
-}
-
-__global__ void __launch_bounds__(128) preprocess_bwd_depth_kernel(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
-                                                                   int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
-                                                                   const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out,
-                                                                   const float* __restrict__ dL_dz)
-{
-	preprocess_bwd_body<true>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out, dL_dz);
-}
-
-__global__ void __launch_bounds__(128) preprocess_bwd_aa_kernel(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
-                                                                int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
-                                                                const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out,
-                                                                float* __restrict__ dL_dopacity)
-{
-	preprocess_bwd_body<false, true>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out, nullptr,
-	                                 dL_dopacity);
-}
-
-__global__ void __launch_bounds__(128) preprocess_bwd_depth_aa_kernel(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
-                                                                      int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
-                                                                      const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out,
-                                                                      const float* __restrict__ dL_dz, float* __restrict__ dL_dopacity)
-{
-	preprocess_bwd_body<true, true>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out, dL_dz,
-	                                dL_dopacity);
+	preprocess_bwd_body<DEPTH, AA>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out, dL_dz,
+	                               dL_dopacity);
 }
 
 int launch_preprocess_backward(const GaussIn& in, const Camera& cam, const GeomState& geom, const float* dL_dmean2D, int mean2D_stride,
@@ -104,18 +82,10 @@ int launch_preprocess_backward(const GaussIn& in, const Camera& cam, const GeomS
                                const GaussGradOut& out, cudaStream_t stream, const float* dL_dz, float* aa_dL_dopacity)
 {
 	if (in.P == 0) return 0;
-	if (aa_dL_dopacity && dL_dz)
-		preprocess_bwd_depth_aa_kernel<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor,
-		                                                                    color_stride, out, dL_dz, aa_dL_dopacity);
-	else if (aa_dL_dopacity)
-		preprocess_bwd_aa_kernel<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor,
-		                                                              color_stride, out, aa_dL_dopacity);
-	else if (dL_dz)
-		preprocess_bwd_depth_kernel<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor,
-		                                                                 color_stride, out, dL_dz);
-	else
-		preprocess_bwd_kernel<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor,
-		                                                           color_stride, out);
+	auto kernel = aa_dL_dopacity ? (dL_dz ? preprocess_bwd_kernel<true, true> : preprocess_bwd_kernel<false, true>)
+	                             : (dL_dz ? preprocess_bwd_kernel<true, false> : preprocess_bwd_kernel<false, false>);
+	kernel<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out,
+	                                            dL_dz, aa_dL_dopacity);
 	PSB_LAUNCH_OK();
 	return 0;
 }

@@ -43,7 +43,7 @@ constexpr int MODE_PUSH = 2;   // NVLink data-parallel step: 80-byte gradient re
 constexpr int MODE_ADAM_LIVE = 3;  // MODE_ADAM with the caller's per-row live byte (psb_model.adam_live): rows that are neither live nor
                                    // reached by a gradient are not read beyond that byte and the visibility word
 constexpr int MODE_DEPTH = 8;      // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE / MODE_PUSH: slot 11 of the sink row holds dL/dz (view-space depth,
-                                   // render_bwd_depth_kernel) and joins dL/dxyz through the view matrix's z row
+                                   // render_bwd_kernel<true, ...>) and joins dL/dxyz through the view matrix's z row
 constexpr int MODE_AA = 16;        // OR'd into any of the above: the forward was anti-aliased (o' = o h, preprocess_fwd_kernel<true, true>), slot 7
                                    // holds dL/do'; dL/dh joins the covariance gradient and the opacity gradient is h dL/do' sigma'
 

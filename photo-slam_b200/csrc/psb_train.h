@@ -53,7 +53,7 @@ struct DpShard {             // what the owner-side Adam kernels need
 };
 int launch_push_backward(int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, const StepHyper& h,
                          const DensifyStats& st, const uint32_t* counters, uint32_t capacity, const DpPush& dp, cudaStream_t stream,
-                         bool depth = false /* the sink rows carry dL/dz in slot 11 (render_bwd_depth_kernel) */,
+                         bool depth = false /* the sink rows carry dL/dz in slot 11 (render_bwd_kernel<true, ...>) */,
                          bool aa = false /* the forward was anti-aliased (launch_preprocess aa): slot 7 holds dL/do' */);
 int launch_shard_adam(const DpShard& d, const TrainTensors& t, const StepHyper& h, float grad_scale, cudaStream_t stream, cudaEvent_t between = nullptr);
 // spins (device side) until flags[0..world) >= epoch (world <= 32 words); after `timeout_ms` writes 1 to *status and gives up
@@ -65,7 +65,7 @@ int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, co
                           const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
                           cudaStream_t stream, cudaEvent_t between = nullptr /* recorded between the two kernels (stage timing) */,
                           unsigned char* adam_live = nullptr /* adam only: psb_model.adam_live, or null (the moments tell idle rows) */,
-                          bool depth = false /* the sink rows carry dL/dz in slot 11 (render_bwd_depth_kernel) */,
+                          bool depth = false /* the sink rows carry dL/dz in slot 11 (render_bwd_kernel<true, ...>) */,
                           bool aa = false /* the forward was anti-aliased (launch_preprocess aa): slot 7 holds dL/do' */);
 // adam_live[i] = any moment of row i non-zero (t.m / t.v: the 12 moment tensors)
 int launch_adam_live_rebuild(int P, const TrainTensors& t, unsigned char* adam_live, cudaStream_t stream);

@@ -8,7 +8,8 @@
 //
 // libgaussian_mapper.so links against exactly these symbols (SURVEY.md §8b); building this file into
 // libcuda_rasterizer.so (+ libpsb200.so) swaps the rasterizer without touching any caller. Pure C++/LibTorch host
-// code: no kernels here. The TORCH_LIBRARY block at the end only exists so the Python test-suite can call the
+// code: no kernels here. Every RasterizeGaussians*CUDA forward is forward_impl and every backward is backward_impl (below), which
+// differ per export only in the C entry point they call. The TORCH_LIBRARY block at the end only exists so the Python test-suite can call the
 // C++ entry points (torch.ops.psb200.*).
 #include <functional>
 #include <optional>
@@ -21,8 +22,6 @@
 #include "../../include/psb200.h"
 
 namespace {
-
-struct TensorSlot { torch::Tensor* t; };
 
 char* resize_cb(size_t n, void* user)
 {
@@ -38,20 +37,25 @@ void* current_stream() { return (void*)c10::cuda::getCurrentCUDAStream().stream(
 
 char* fn_cb(size_t n, void* user) { return (*static_cast<std::function<char*(size_t)>*>(user))(n); }
 
-}  // namespace
+using Fwd7 = std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>;
+using Bwd8 = std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>;
 
-std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
-RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors, const torch::Tensor& opacity,
-                       const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier, const torch::Tensor& cov3D_precomp,
-                       const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
-                       const int image_height, const int image_width, const torch::Tensor& sh, const int degree, const torch::Tensor& campos,
-                       const bool prefiltered)
+// The one forward behind RasterizeGaussians[Depth|Antialiased]CUDA -> (rendered, out_color, out_depth, radii, geomBuffer, binningBuffer,
+// imgBuffer). depth: also the [H,W] depth image (out_depth stays undefined without it); aa: the 2D Mip filter. Each combination calls
+// the narrowest C entry point that has it.
+Fwd7 forward_impl(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors, const torch::Tensor& opacity,
+                  const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier, const torch::Tensor& cov3D_precomp,
+                  const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
+                  const int image_height, const int image_width, const torch::Tensor& sh, const int degree, const torch::Tensor& campos,
+                  const bool prefiltered, const bool depth, const bool aa)
 {
 	if (means3D.ndimension() != 2 || means3D.size(1) != 3) { AT_ERROR("means3D must have dimensions (num_points, 3)"); }
 	const int P = means3D.size(0);
 	const int H = image_height, W = image_width;
 	auto float_opts = means3D.options().dtype(torch::kFloat32);
 	torch::Tensor out_color = torch::full({3, H, W}, 0.0, float_opts);
+	torch::Tensor out_depth;
+	if (depth) out_depth = torch::full({H, W}, 0.0, float_opts);
 	torch::Tensor radii = torch::full({P}, 0, means3D.options().dtype(torch::kInt32));
 	torch::TensorOptions options(torch::kByte);
 	torch::Tensor geomBuffer = torch::empty({0}, options.device(means3D.device()));
@@ -65,96 +69,39 @@ RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::Tensor& mea
 		const auto bg = background.contiguous(), m3 = means3D.contiguous(), shc = sh.contiguous(), col = colors.contiguous(), op = opacity.contiguous(),
 		           sc = scales.contiguous(), rot = rotations.contiguous(), cov = cov3D_precomp.contiguous(), vm = viewmatrix.contiguous(),
 		           pm = projmatrix.contiguous(), cp = campos.contiguous();
-		rendered = psb_rasterize_forward(resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer, P, degree, M, fptr(bg), W, H,
-		                                 fptr(m3), fptr(shc), fptr(col), fptr(op), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm),
-		                                 fptr(cp), tan_fovx, tan_fovy, prefiltered ? 1 : 0, out_color.data_ptr<float>(), radii.data_ptr<int>(),
-		                                 current_stream());
-		if (rendered < 0) { AT_ERROR("psb_rasterize_forward: ", psb_last_error()); }
-	}
-	return std::make_tuple(rendered, out_color, radii, geomBuffer, binningBuffer, imgBuffer);
-}
-
-std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
-RasterizeGaussiansBackwardCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii, const torch::Tensor& colors,
-                               const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier,
-                               const torch::Tensor& cov3D_precomp, const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix,
-                               const float tan_fovx, const float tan_fovy, const torch::Tensor& dL_dout_color, const torch::Tensor& sh,
-                               const int degree, const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R,
-                               const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer)
-{
-	const int P = means3D.size(0);
-	const int H = dL_dout_color.size(1), W = dL_dout_color.size(2);
-	int M = 0;
-	if (sh.size(0) != 0) M = sh.size(1);
-	torch::Tensor dL_dmeans3D = torch::zeros({P, 3}, means3D.options());
-	torch::Tensor dL_dmeans2D = torch::zeros({P, 3}, means3D.options());
-	torch::Tensor dL_dcolors = torch::zeros({P, 3}, means3D.options());
-	torch::Tensor dL_dconic = torch::zeros({P, 2, 2}, means3D.options());
-	torch::Tensor dL_dopacity = torch::zeros({P, 1}, means3D.options());
-	torch::Tensor dL_dcov3D = torch::zeros({P, 6}, means3D.options());
-	torch::Tensor dL_dsh = torch::zeros({P, M, 3}, means3D.options());
-	torch::Tensor dL_dscales = torch::zeros({P, 3}, means3D.options());
-	torch::Tensor dL_drotations = torch::zeros({P, 4}, means3D.options());
-	if (P != 0) {
-		const auto bg = background.contiguous(), m3 = means3D.contiguous(), shc = sh.contiguous(), col = colors.contiguous(), sc = scales.contiguous(),
-		           rot = rotations.contiguous(), cov = cov3D_precomp.contiguous(), vm = viewmatrix.contiguous(), pm = projmatrix.contiguous(),
-		           cp = campos.contiguous(), dpix = dL_dout_color.contiguous(), rad = radii.contiguous();
-		const int rc = psb_rasterize_backward(
-			P, degree, M, R, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
-			tan_fovx, tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(geomBuffer.contiguous().data_ptr()),
-			reinterpret_cast<char*>(binningBuffer.contiguous().data_ptr()), reinterpret_cast<char*>(imageBuffer.contiguous().data_ptr()), fptr(dpix),
-			dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(), dL_dopacity.data_ptr<float>(), dL_dcolors.data_ptr<float>(),
-			dL_dmeans3D.data_ptr<float>(), dL_dcov3D.data_ptr<float>(), M ? dL_dsh.data_ptr<float>() : nullptr, dL_dscales.data_ptr<float>(),
-			dL_drotations.data_ptr<float>(), current_stream());
-		if (rc < 0) { AT_ERROR("psb_rasterize_backward: ", psb_last_error()); }
-	}
-	return std::make_tuple(dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations);
-}
-
-// ---- rendered depth D(p) = sum_i z_i alpha_i T_i (include/psb200.h), which the reference has no symbol for: the two functions
-// above with the depth image added, for a GaussianRasterizerFunction that returns and back-propagates depth (INTEGRATION.md §1)
-std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
-RasterizeGaussiansDepthCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors, const torch::Tensor& opacity,
-                            const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier, const torch::Tensor& cov3D_precomp,
-                            const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
-                            const int image_height, const int image_width, const torch::Tensor& sh, const int degree, const torch::Tensor& campos,
-                            const bool prefiltered)
-{
-	if (means3D.ndimension() != 2 || means3D.size(1) != 3) { AT_ERROR("means3D must have dimensions (num_points, 3)"); }
-	const int P = means3D.size(0);
-	const int H = image_height, W = image_width;
-	auto float_opts = means3D.options().dtype(torch::kFloat32);
-	torch::Tensor out_color = torch::full({3, H, W}, 0.0, float_opts);
-	torch::Tensor out_depth = torch::full({H, W}, 0.0, float_opts);
-	torch::Tensor radii = torch::full({P}, 0, means3D.options().dtype(torch::kInt32));
-	torch::TensorOptions options(torch::kByte);
-	torch::Tensor geomBuffer = torch::empty({0}, options.device(means3D.device()));
-	torch::Tensor binningBuffer = torch::empty({0}, options.device(means3D.device()));
-	torch::Tensor imgBuffer = torch::empty({0}, options.device(means3D.device()));
-	int rendered = 0;
-	if (P != 0) {
-		int M = 0;
-		if (sh.size(0) != 0) M = sh.size(1);
-		const auto bg = background.contiguous(), m3 = means3D.contiguous(), shc = sh.contiguous(), col = colors.contiguous(), op = opacity.contiguous(),
-		           sc = scales.contiguous(), rot = rotations.contiguous(), cov = cov3D_precomp.contiguous(), vm = viewmatrix.contiguous(),
-		           pm = projmatrix.contiguous(), cp = campos.contiguous();
-		rendered = psb_rasterize_forward_depth(resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer, P, degree, M, fptr(bg), W, H,
-		                                       fptr(m3), fptr(shc), fptr(col), fptr(op), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm),
-		                                       fptr(pm), fptr(cp), tan_fovx, tan_fovy, prefiltered ? 1 : 0, out_color.data_ptr<float>(),
-		                                       radii.data_ptr<int>(), out_depth.data_ptr<float>(), current_stream());
-		if (rendered < 0) { AT_ERROR("psb_rasterize_forward_depth: ", psb_last_error()); }
+		// the arguments every forward entry point starts with
+		const auto args = std::make_tuple(&resize_cb, (void*)&geomBuffer, &resize_cb, (void*)&binningBuffer, &resize_cb, (void*)&imgBuffer, P, degree, M,
+		                                  fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(op), fptr(sc), scale_modifier, fptr(rot), fptr(cov),
+		                                  fptr(vm), fptr(pm), fptr(cp), tan_fovx, tan_fovy, prefiltered ? 1 : 0, out_color.data_ptr<float>(),
+		                                  radii.data_ptr<int>());
+		float* dep = depth ? out_depth.data_ptr<float>() : nullptr;
+		void* stream = current_stream();
+		if (aa) {
+			rendered = std::apply([&](auto... a) { return psb_rasterize_forward_aa(a..., dep, 1, stream); }, args);
+			if (rendered < 0) { AT_ERROR("psb_rasterize_forward_aa: ", psb_last_error()); }
+		} else if (depth) {
+			rendered = std::apply([&](auto... a) { return psb_rasterize_forward_depth(a..., dep, stream); }, args);
+			if (rendered < 0) { AT_ERROR("psb_rasterize_forward_depth: ", psb_last_error()); }
+		} else {
+			rendered = std::apply([&](auto... a) { return psb_rasterize_forward(a..., stream); }, args);
+			if (rendered < 0) { AT_ERROR("psb_rasterize_forward: ", psb_last_error()); }
+		}
 	}
 	return std::make_tuple(rendered, out_color, out_depth, radii, geomBuffer, binningBuffer, imgBuffer);
 }
 
-// dL_dout_depth [H,W]; an undefined tensor is the plain backward. dL/dz is folded into dL_dmeans3D, and dL_dmeans2D includes the depth term.
-std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
-RasterizeGaussiansBackwardDepthCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii, const torch::Tensor& colors,
-                                    const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier,
-                                    const torch::Tensor& cov3D_precomp, const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix,
-                                    const float tan_fovx, const float tan_fovy, const torch::Tensor& dL_dout_color,
-                                    const torch::Tensor& dL_dout_depth, const torch::Tensor& sh, const int degree, const torch::Tensor& campos,
-                                    const torch::Tensor& geomBuffer, const int R, const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer)
+// Which C entry point a backward export calls: each the previous one plus one thing (a depth gradient; the fixed-order sums over a
+// scratch; the h-term of an anti-aliased forward, deterministic or not).
+enum class Bwd { Plain, Depth, Deterministic, Antialiased };
+
+// The one backward behind RasterizeGaussiansBackward[Depth|Deterministic|Antialiased]CUDA. dL_dout_depth [H,W]; undefined or empty is
+// colour only (and all Bwd::Plain takes). `deterministic` is read by Bwd::Antialiased alone.
+Bwd8 backward_impl(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii, const torch::Tensor& colors,
+                   const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier, const torch::Tensor& cov3D_precomp,
+                   const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
+                   const torch::Tensor& dL_dout_color, const torch::Tensor& dL_dout_depth, const torch::Tensor& sh, const int degree,
+                   const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R, const torch::Tensor& binningBuffer,
+                   const torch::Tensor& imageBuffer, const Bwd mode, const bool deterministic)
 {
 	const int P = means3D.size(0);
 	const int H = dL_dout_color.size(1), W = dL_dout_color.size(2);
@@ -173,22 +120,101 @@ RasterizeGaussiansBackwardDepthCUDA(const torch::Tensor& background, const torch
 	torch::Tensor dL_dsh = torch::zeros({P, M, 3}, means3D.options());
 	torch::Tensor dL_dscales = torch::zeros({P, 3}, means3D.options());
 	torch::Tensor dL_drotations = torch::zeros({P, 4}, means3D.options());
-	torch::Tensor dL_dz = torch::zeros({depth ? P : 0}, means3D.options());
 	if (P != 0) {
 		const auto bg = background.contiguous(), m3 = means3D.contiguous(), shc = sh.contiguous(), col = colors.contiguous(), sc = scales.contiguous(),
 		           rot = rotations.contiguous(), cov = cov3D_precomp.contiguous(), vm = viewmatrix.contiguous(), pm = projmatrix.contiguous(),
 		           cp = campos.contiguous(), dpix = dL_dout_color.contiguous(), rad = radii.contiguous();
-		const torch::Tensor ddep = depth ? dL_dout_depth.contiguous() : torch::Tensor();
-		const int rc = psb_rasterize_backward_depth(
+		// the arguments every backward entry point starts with
+		const auto args = std::make_tuple(
 			P, degree, M, R, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
-			tan_fovx, tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(geomBuffer.contiguous().data_ptr()),
+			tan_fovx, tan_fovy, (const int*)rad.data_ptr<int>(), reinterpret_cast<char*>(geomBuffer.contiguous().data_ptr()),
 			reinterpret_cast<char*>(binningBuffer.contiguous().data_ptr()), reinterpret_cast<char*>(imageBuffer.contiguous().data_ptr()), fptr(dpix),
 			dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(), dL_dopacity.data_ptr<float>(), dL_dcolors.data_ptr<float>(),
 			dL_dmeans3D.data_ptr<float>(), dL_dcov3D.data_ptr<float>(), M ? dL_dsh.data_ptr<float>() : nullptr, dL_dscales.data_ptr<float>(),
-			dL_drotations.data_ptr<float>(), depth ? ddep.data_ptr<float>() : nullptr, depth ? dL_dz.data_ptr<float>() : nullptr, current_stream());
-		if (rc < 0) { AT_ERROR("psb_rasterize_backward_depth: ", psb_last_error()); }
+			dL_drotations.data_ptr<float>());
+		const torch::Tensor ddep_t = depth ? dL_dout_depth.contiguous() : torch::Tensor();
+		torch::Tensor dL_dz, det_t;
+		if (depth) dL_dz = torch::zeros({P}, means3D.options());
+		const float* ddep = depth ? ddep_t.data_ptr<float>() : nullptr;
+		float* dz = depth ? dL_dz.data_ptr<float>() : nullptr;
+		const bool det = mode == Bwd::Deterministic || (mode == Bwd::Antialiased && deterministic);
+		const size_t det_bytes = det ? psb_rasterize_backward_det_bytes(P, R) : 0;
+		if (det) det_t = torch::empty({(long long)det_bytes}, means3D.options().dtype(torch::kByte));
+		void* det_scratch = det ? det_t.data_ptr() : nullptr;
+		void* stream = current_stream();
+		int rc = 0;
+		switch (mode) {
+		case Bwd::Plain:
+			rc = std::apply([&](auto... a) { return psb_rasterize_backward(a..., stream); }, args);
+			if (rc < 0) { AT_ERROR("psb_rasterize_backward: ", psb_last_error()); }
+			break;
+		case Bwd::Depth:
+			rc = std::apply([&](auto... a) { return psb_rasterize_backward_depth(a..., ddep, dz, stream); }, args);
+			if (rc < 0) { AT_ERROR("psb_rasterize_backward_depth: ", psb_last_error()); }
+			break;
+		case Bwd::Deterministic:
+			rc = std::apply([&](auto... a) { return psb_rasterize_backward_deterministic(a..., ddep, dz, det_scratch, det_bytes, stream); }, args);
+			if (rc < 0) { AT_ERROR("psb_rasterize_backward_deterministic: ", psb_last_error()); }
+			break;
+		case Bwd::Antialiased:
+			rc = std::apply([&](auto... a) { return psb_rasterize_backward_aa(a..., ddep, dz, det_scratch, det_bytes, 1, stream); }, args);
+			if (rc < 0) { AT_ERROR("psb_rasterize_backward_aa: ", psb_last_error()); }
+			break;
+		}
 	}
 	return std::make_tuple(dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations);
+}
+
+}  // namespace
+
+std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
+RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors, const torch::Tensor& opacity,
+                       const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier, const torch::Tensor& cov3D_precomp,
+                       const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
+                       const int image_height, const int image_width, const torch::Tensor& sh, const int degree, const torch::Tensor& campos,
+                       const bool prefiltered)
+{
+	const Fwd7 r = forward_impl(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx,
+	                            tan_fovy, image_height, image_width, sh, degree, campos, prefiltered, /*depth=*/false, /*aa=*/false);
+	return std::make_tuple(std::get<0>(r), std::get<1>(r), std::get<3>(r), std::get<4>(r), std::get<5>(r), std::get<6>(r));
+}
+
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
+RasterizeGaussiansBackwardCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii, const torch::Tensor& colors,
+                               const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier,
+                               const torch::Tensor& cov3D_precomp, const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix,
+                               const float tan_fovx, const float tan_fovy, const torch::Tensor& dL_dout_color, const torch::Tensor& sh,
+                               const int degree, const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R,
+                               const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer)
+{
+	return backward_impl(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+	                     dL_dout_color, torch::Tensor(), sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer, Bwd::Plain, false);
+}
+
+// ---- rendered depth D(p) = sum_i z_i alpha_i T_i (include/psb200.h), which the reference has no symbol for: the two functions
+// above with the depth image added, for a GaussianRasterizerFunction that returns and back-propagates depth (INTEGRATION.md §1)
+std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
+RasterizeGaussiansDepthCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors, const torch::Tensor& opacity,
+                            const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier, const torch::Tensor& cov3D_precomp,
+                            const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
+                            const int image_height, const int image_width, const torch::Tensor& sh, const int degree, const torch::Tensor& campos,
+                            const bool prefiltered)
+{
+	return forward_impl(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+	                    image_height, image_width, sh, degree, campos, prefiltered, /*depth=*/true, /*aa=*/false);
+}
+
+// dL_dout_depth [H,W]; an undefined tensor is the plain backward. dL/dz is folded into dL_dmeans3D, and dL_dmeans2D includes the depth term.
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
+RasterizeGaussiansBackwardDepthCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii, const torch::Tensor& colors,
+                                    const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier,
+                                    const torch::Tensor& cov3D_precomp, const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix,
+                                    const float tan_fovx, const float tan_fovy, const torch::Tensor& dL_dout_color,
+                                    const torch::Tensor& dL_dout_depth, const torch::Tensor& sh, const int degree, const torch::Tensor& campos,
+                                    const torch::Tensor& geomBuffer, const int R, const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer)
+{
+	return backward_impl(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+	                     dL_dout_color, dL_dout_depth, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer, Bwd::Depth, false);
 }
 
 // RasterizeGaussiansBackwardDepthCUDA whose outputs are bit-identical from call to call (psb_rasterize_backward_deterministic): the
@@ -202,42 +228,8 @@ RasterizeGaussiansBackwardDeterministicCUDA(const torch::Tensor& background, con
                                             const int degree, const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R,
                                             const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer)
 {
-	const int P = means3D.size(0);
-	const int H = dL_dout_color.size(1), W = dL_dout_color.size(2);
-	const bool depth = dL_dout_depth.defined() && dL_dout_depth.numel() != 0;
-	if (depth && (dL_dout_depth.ndimension() != 2 || dL_dout_depth.size(0) != H || dL_dout_depth.size(1) != W)) {
-		AT_ERROR("dL_dout_depth must have dimensions (", H, ", ", W, ")");
-	}
-	int M = 0;
-	if (sh.size(0) != 0) M = sh.size(1);
-	torch::Tensor dL_dmeans3D = torch::zeros({P, 3}, means3D.options());
-	torch::Tensor dL_dmeans2D = torch::zeros({P, 3}, means3D.options());
-	torch::Tensor dL_dcolors = torch::zeros({P, 3}, means3D.options());
-	torch::Tensor dL_dconic = torch::zeros({P, 2, 2}, means3D.options());
-	torch::Tensor dL_dopacity = torch::zeros({P, 1}, means3D.options());
-	torch::Tensor dL_dcov3D = torch::zeros({P, 6}, means3D.options());
-	torch::Tensor dL_dsh = torch::zeros({P, M, 3}, means3D.options());
-	torch::Tensor dL_dscales = torch::zeros({P, 3}, means3D.options());
-	torch::Tensor dL_drotations = torch::zeros({P, 4}, means3D.options());
-	torch::Tensor dL_dz = torch::zeros({depth ? P : 0}, means3D.options());
-	if (P != 0) {
-		const auto bg = background.contiguous(), m3 = means3D.contiguous(), shc = sh.contiguous(), col = colors.contiguous(), sc = scales.contiguous(),
-		           rot = rotations.contiguous(), cov = cov3D_precomp.contiguous(), vm = viewmatrix.contiguous(), pm = projmatrix.contiguous(),
-		           cp = campos.contiguous(), dpix = dL_dout_color.contiguous(), rad = radii.contiguous();
-		const torch::Tensor ddep = depth ? dL_dout_depth.contiguous() : torch::Tensor();
-		const size_t det_bytes = psb_rasterize_backward_det_bytes(P, R);
-		torch::Tensor det_scratch = torch::empty({(long long)det_bytes}, means3D.options().dtype(torch::kByte));
-		const int rc = psb_rasterize_backward_deterministic(
-			P, degree, M, R, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
-			tan_fovx, tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(geomBuffer.contiguous().data_ptr()),
-			reinterpret_cast<char*>(binningBuffer.contiguous().data_ptr()), reinterpret_cast<char*>(imageBuffer.contiguous().data_ptr()), fptr(dpix),
-			dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(), dL_dopacity.data_ptr<float>(), dL_dcolors.data_ptr<float>(),
-			dL_dmeans3D.data_ptr<float>(), dL_dcov3D.data_ptr<float>(), M ? dL_dsh.data_ptr<float>() : nullptr, dL_dscales.data_ptr<float>(),
-			dL_drotations.data_ptr<float>(), depth ? ddep.data_ptr<float>() : nullptr, depth ? dL_dz.data_ptr<float>() : nullptr, det_scratch.data_ptr(),
-			det_bytes, current_stream());
-		if (rc < 0) { AT_ERROR("psb_rasterize_backward_deterministic: ", psb_last_error()); }
-	}
-	return std::make_tuple(dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations);
+	return backward_impl(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+	                     dL_dout_color, dL_dout_depth, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer, Bwd::Deterministic, true);
 }
 
 // ---- anti-aliasing (the 2D Mip filter, upstream diff-gaussian-rasterization's `antialiasing`; include/psb200.h psb_rasterize_forward_aa):
@@ -250,31 +242,8 @@ RasterizeGaussiansAntialiasedCUDA(const torch::Tensor& background, const torch::
                                   const float tan_fovx, const float tan_fovy, const int image_height, const int image_width, const torch::Tensor& sh,
                                   const int degree, const torch::Tensor& campos, const bool prefiltered)
 {
-	if (means3D.ndimension() != 2 || means3D.size(1) != 3) { AT_ERROR("means3D must have dimensions (num_points, 3)"); }
-	const int P = means3D.size(0);
-	const int H = image_height, W = image_width;
-	auto float_opts = means3D.options().dtype(torch::kFloat32);
-	torch::Tensor out_color = torch::full({3, H, W}, 0.0, float_opts);
-	torch::Tensor out_depth = torch::full({H, W}, 0.0, float_opts);
-	torch::Tensor radii = torch::full({P}, 0, means3D.options().dtype(torch::kInt32));
-	torch::TensorOptions options(torch::kByte);
-	torch::Tensor geomBuffer = torch::empty({0}, options.device(means3D.device()));
-	torch::Tensor binningBuffer = torch::empty({0}, options.device(means3D.device()));
-	torch::Tensor imgBuffer = torch::empty({0}, options.device(means3D.device()));
-	int rendered = 0;
-	if (P != 0) {
-		int M = 0;
-		if (sh.size(0) != 0) M = sh.size(1);
-		const auto bg = background.contiguous(), m3 = means3D.contiguous(), shc = sh.contiguous(), col = colors.contiguous(), op = opacity.contiguous(),
-		           sc = scales.contiguous(), rot = rotations.contiguous(), cov = cov3D_precomp.contiguous(), vm = viewmatrix.contiguous(),
-		           pm = projmatrix.contiguous(), cp = campos.contiguous();
-		rendered = psb_rasterize_forward_aa(resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer, P, degree, M, fptr(bg), W, H,
-		                                    fptr(m3), fptr(shc), fptr(col), fptr(op), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm),
-		                                    fptr(pm), fptr(cp), tan_fovx, tan_fovy, prefiltered ? 1 : 0, out_color.data_ptr<float>(),
-		                                    radii.data_ptr<int>(), out_depth.data_ptr<float>(), 1, current_stream());
-		if (rendered < 0) { AT_ERROR("psb_rasterize_forward_aa: ", psb_last_error()); }
-	}
-	return std::make_tuple(rendered, out_color, out_depth, radii, geomBuffer, binningBuffer, imgBuffer);
+	return forward_impl(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+	                    image_height, image_width, sh, degree, campos, prefiltered, /*depth=*/true, /*aa=*/true);
 }
 
 // The backward of RasterizeGaussiansAntialiasedCUDA: the signature of RasterizeGaussiansBackwardDeterministicCUDA plus `deterministic`
@@ -289,42 +258,8 @@ RasterizeGaussiansBackwardAntialiasedCUDA(const torch::Tensor& background, const
                                           const int degree, const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R,
                                           const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const bool deterministic)
 {
-	const int P = means3D.size(0);
-	const int H = dL_dout_color.size(1), W = dL_dout_color.size(2);
-	const bool depth = dL_dout_depth.defined() && dL_dout_depth.numel() != 0;
-	if (depth && (dL_dout_depth.ndimension() != 2 || dL_dout_depth.size(0) != H || dL_dout_depth.size(1) != W)) {
-		AT_ERROR("dL_dout_depth must have dimensions (", H, ", ", W, ")");
-	}
-	int M = 0;
-	if (sh.size(0) != 0) M = sh.size(1);
-	torch::Tensor dL_dmeans3D = torch::zeros({P, 3}, means3D.options());
-	torch::Tensor dL_dmeans2D = torch::zeros({P, 3}, means3D.options());
-	torch::Tensor dL_dcolors = torch::zeros({P, 3}, means3D.options());
-	torch::Tensor dL_dconic = torch::zeros({P, 2, 2}, means3D.options());
-	torch::Tensor dL_dopacity = torch::zeros({P, 1}, means3D.options());
-	torch::Tensor dL_dcov3D = torch::zeros({P, 6}, means3D.options());
-	torch::Tensor dL_dsh = torch::zeros({P, M, 3}, means3D.options());
-	torch::Tensor dL_dscales = torch::zeros({P, 3}, means3D.options());
-	torch::Tensor dL_drotations = torch::zeros({P, 4}, means3D.options());
-	torch::Tensor dL_dz = torch::zeros({depth ? P : 0}, means3D.options());
-	if (P != 0) {
-		const auto bg = background.contiguous(), m3 = means3D.contiguous(), shc = sh.contiguous(), col = colors.contiguous(), sc = scales.contiguous(),
-		           rot = rotations.contiguous(), cov = cov3D_precomp.contiguous(), vm = viewmatrix.contiguous(), pm = projmatrix.contiguous(),
-		           cp = campos.contiguous(), dpix = dL_dout_color.contiguous(), rad = radii.contiguous();
-		const torch::Tensor ddep = depth ? dL_dout_depth.contiguous() : torch::Tensor();
-		const size_t det_bytes = deterministic ? psb_rasterize_backward_det_bytes(P, R) : 0;
-		torch::Tensor det_scratch = torch::empty({(long long)det_bytes}, means3D.options().dtype(torch::kByte));
-		const int rc = psb_rasterize_backward_aa(
-			P, degree, M, R, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
-			tan_fovx, tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(geomBuffer.contiguous().data_ptr()),
-			reinterpret_cast<char*>(binningBuffer.contiguous().data_ptr()), reinterpret_cast<char*>(imageBuffer.contiguous().data_ptr()), fptr(dpix),
-			dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(), dL_dopacity.data_ptr<float>(), dL_dcolors.data_ptr<float>(),
-			dL_dmeans3D.data_ptr<float>(), dL_dcov3D.data_ptr<float>(), M ? dL_dsh.data_ptr<float>() : nullptr, dL_dscales.data_ptr<float>(),
-			dL_drotations.data_ptr<float>(), depth ? ddep.data_ptr<float>() : nullptr, depth ? dL_dz.data_ptr<float>() : nullptr,
-			deterministic ? det_scratch.data_ptr() : nullptr, det_bytes, 1, current_stream());
-		if (rc < 0) { AT_ERROR("psb_rasterize_backward_aa: ", psb_last_error()); }
-	}
-	return std::make_tuple(dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations);
+	return backward_impl(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+	                     dL_dout_color, dL_dout_depth, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer, Bwd::Antialiased, deterministic);
 }
 
 torch::Tensor markVisible(torch::Tensor& means3D, torch::Tensor& viewmatrix, torch::Tensor& projmatrix)

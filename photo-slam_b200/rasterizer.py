@@ -9,7 +9,7 @@ Mirrors, name for name and argument for argument:
 
 Rendered depth D(p) = sum_i z_i alpha_i T_i (include/psb200.h), which the reference does not have:
   RasterizeGaussiansDepthCUDA / RasterizeGaussiansBackwardDepthCUDA   the two functions above plus the depth image and its gradient
-  _RasterizeGaussiansDepth, GaussianRasterizer.forward(..., return_depth=True)   autograd through colour and depth
+  _RasterizeGaussians(..., depth=True), GaussianRasterizer.forward(..., return_depth=True)   autograd through colour and depth
 
 deterministic=True (keyword) on the backward functions, rasterize_gaussians and GaussianRasterizer.forward selects
 psb_rasterize_backward_deterministic: the same gradients, bit-identical from run to run. The default keeps the float-atomic backward.
@@ -158,14 +158,14 @@ def _backward(background, means3D, radii, colors, scales, rotations, scale_modif
             if tuple(ddep.shape) != (H, W):
                 raise RuntimeError(f"dL_dout_depth must have dimensions ({H}, {W})")
             dL_dz = torch.zeros((P,), **o)      # [P], zero-initialised as the C-ABI requires; folded into dL_dmeans3D there
+        nbytes, scratch = 0, None
+        if deterministic:
+            nbytes = L.psb_rasterize_backward_det_bytes(P, int(R))
+            scratch = torch.empty((nbytes,), dtype=torch.uint8, device=means3D.device)    # the call zeroes what it reads
         if antialiasing:
-            nbytes = L.psb_rasterize_backward_det_bytes(P, int(R)) if deterministic else 0
-            scratch = torch.empty((nbytes,), dtype=torch.uint8, device=means3D.device) if deterministic else None
             _lib.check(L.psb_rasterize_backward_aa(*args, _ptr(ddep), _ptr(dL_dz), _ptr(scratch), nbytes, 1, _stream()),
                        "psb_rasterize_backward_aa")
         elif deterministic:
-            nbytes = L.psb_rasterize_backward_det_bytes(P, int(R))
-            scratch = torch.empty((nbytes,), dtype=torch.uint8, device=means3D.device)    # the call zeroes what it reads
             _lib.check(L.psb_rasterize_backward_deterministic(*args, _ptr(ddep), _ptr(dL_dz), scratch.data_ptr(), nbytes, _stream()),
                        "psb_rasterize_backward_deterministic")
         elif ddep is not None:
@@ -226,15 +226,17 @@ class GaussianRasterizationSettings:
 
 
 class _RasterizeGaussians(torch.autograd.Function):
-    """reference GaussianRasterizerFunction (src/gaussian_rasterizer.cpp:28-180)."""
+    """reference GaussianRasterizerFunction (src/gaussian_rasterizer.cpp:28-180). depth=True: the depth image as a third,
+    differentiable output."""
 
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings, deterministic=False):
+    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings, deterministic=False,
+                depth=False):
         rs = raster_settings
-        num_rendered, color, radii, geomBuffer, binningBuffer, imgBuffer = RasterizeGaussiansCUDA(
+        num_rendered, color, out_depth, radii, geomBuffer, binningBuffer, imgBuffer = _forward(
             rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
             rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, sh, rs.sh_degree,
-            rs.campos, rs.prefiltered, antialiasing=bool(rs.antialiasing))
+            rs.campos, rs.prefiltered, depth=bool(depth), antialiasing=bool(rs.antialiasing))
         ctx.raster_settings = rs
         ctx.num_rendered = num_rendered
         ctx.deterministic = bool(deterministic)
@@ -242,64 +244,29 @@ class _RasterizeGaussians(torch.autograd.Function):
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
                               binningBuffer, imgBuffer)
         ctx.mark_non_differentiable(radii)
-        return color, radii
+        if not depth:
+            return color, radii
+        ctx.set_materialize_grads(False)    # an output the loss does not use arrives as None, not as a zero image
+        return color, radii, out_depth
 
     @staticmethod
-    def backward(ctx, grad_out_color, _grad_radii):
+    def backward(ctx, grad_out_color, _grad_radii, grad_out_depth=None):
         if not ctx.deterministic:
             _alert_not_deterministic()
         rs = ctx.raster_settings
         colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer = ctx.saved_tensors
+        if grad_out_color is None:      # only with depth=True, which does not materialise the gradients
+            grad_out_color = torch.zeros((3, rs.image_height, rs.image_width), dtype=torch.float32, device=means3D.device)
         (grad_means2D, grad_colors_precomp, grad_opacities, grad_means3D, grad_cov3Ds_precomp, grad_sh, grad_scales,
-         grad_rotations) = RasterizeGaussiansBackwardCUDA(
+         grad_rotations) = _backward(
             rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix,
-            rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_out_color, sh, rs.sh_degree, rs.campos, geomBuffer,
+            rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_out_color, grad_out_depth, sh, rs.sh_degree, rs.campos, geomBuffer,
             ctx.num_rendered, binningBuffer, imgBuffer, deterministic=ctx.deterministic, antialiasing=ctx.antialiasing)
         # order of reference gaussian_rasterizer.cpp:159-179
         def g(t, ref):
             return t if (ref is not None and ref.numel() != 0) else None
         return (grad_means3D, grad_means2D, g(grad_sh, sh), g(grad_colors_precomp, colors_precomp), grad_opacities,
-                g(grad_scales, scales), g(grad_rotations, rotations), g(grad_cov3Ds_precomp, cov3Ds_precomp), None, None)
-
-
-class _RasterizeGaussiansDepth(torch.autograd.Function):
-    """_RasterizeGaussians with the depth image as a third, differentiable output."""
-
-    @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings, deterministic=False):
-        rs = raster_settings
-        num_rendered, color, depth, radii, geomBuffer, binningBuffer, imgBuffer = RasterizeGaussiansDepthCUDA(
-            rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
-            rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, sh, rs.sh_degree,
-            rs.campos, rs.prefiltered, antialiasing=bool(rs.antialiasing))
-        ctx.raster_settings = rs
-        ctx.num_rendered = num_rendered
-        ctx.deterministic = bool(deterministic)
-        ctx.antialiasing = bool(rs.antialiasing)     # the backward differentiates the forward that ran
-        ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
-                              binningBuffer, imgBuffer)
-        ctx.mark_non_differentiable(radii)
-        ctx.set_materialize_grads(False)    # an output the loss does not use arrives as None, not as a zero image
-        return color, radii, depth
-
-    @staticmethod
-    def backward(ctx, grad_out_color, _grad_radii, grad_out_depth):
-        if not ctx.deterministic:
-            _alert_not_deterministic()
-        rs = ctx.raster_settings
-        colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer = ctx.saved_tensors
-        if grad_out_color is None:
-            grad_out_color = torch.zeros((3, rs.image_height, rs.image_width), dtype=torch.float32, device=means3D.device)
-        (grad_means2D, grad_colors_precomp, grad_opacities, grad_means3D, grad_cov3Ds_precomp, grad_sh, grad_scales,
-         grad_rotations) = RasterizeGaussiansBackwardDepthCUDA(
-            rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix,
-            rs.projmatrix, rs.tanfovx, rs.tanfovy, grad_out_color, grad_out_depth, sh, rs.sh_degree, rs.campos, geomBuffer,
-            ctx.num_rendered, binningBuffer, imgBuffer, deterministic=ctx.deterministic, antialiasing=ctx.antialiasing)
-
-        def g(t, ref):
-            return t if (ref is not None and ref.numel() != 0) else None
-        return (grad_means3D, grad_means2D, g(grad_sh, sh), g(grad_colors_precomp, colors_precomp), grad_opacities,
-                g(grad_scales, scales), g(grad_rotations, rotations), g(grad_cov3Ds_precomp, cov3Ds_precomp), None, None)
+                g(grad_scales, scales), g(grad_rotations, rotations), g(grad_cov3Ds_precomp, cov3Ds_precomp), None, None, None)
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings, *,
@@ -333,8 +300,8 @@ class GaussianRasterizer:
         empty = torch.empty(0, dtype=torch.float32, device=means3D.device)
         e = lambda t: t if has(t) else empty
         if return_depth:
-            return _RasterizeGaussiansDepth.apply(means3D, means2D, e(shs), e(colors_precomp), opacities, e(scales), e(rotations),
-                                                  e(cov3D_precomp), self.raster_settings, deterministic)
+            return _RasterizeGaussians.apply(means3D, means2D, e(shs), e(colors_precomp), opacities, e(scales), e(rotations),
+                                             e(cov3D_precomp), self.raster_settings, deterministic, True)
         return rasterize_gaussians(means3D, means2D, e(shs), e(colors_precomp), opacities, e(scales), e(rotations),
                                    e(cov3D_precomp), self.raster_settings, deterministic=deterministic)
 

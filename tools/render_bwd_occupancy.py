@@ -11,9 +11,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from photo_slam_b200 import _lib  # noqa: E402
 
-NAMES = ["render_bwd_kernel", "render_bwd_depth_kernel", "render_bwd_det_kernel", "render_bwd_depth_det_kernel",
-         "render_bwd_alpha_kernel<false, false>", "render_bwd_alpha_kernel<true, false>",
-         "render_bwd_alpha_kernel<false, true>", "render_bwd_alpha_kernel<true, true>"]
+# variant v = depth | det << 1 | alpha << 2 is render_bwd_kernel<DEPTH, DET, ALPHA>
+NAMES = ["render_bwd_kernel<%s, %s, %s>" % tuple("true" if v >> b & 1 else "false" for b in range(3)) for v in range(8)]
 
 
 def main():
