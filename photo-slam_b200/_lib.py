@@ -56,6 +56,8 @@ def lib():
     L.psb_mark_visible.argtypes = [C.c_int, fp, fp, fp, u8p, vp]
     L.psb_debug_export.restype = C.c_int
     L.psb_debug_export.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp] + [vp] * 11 + [vp]
+    L.psb_debug_render_bwd_occupancy.restype = C.c_int
+    L.psb_debug_render_bwd_occupancy.argtypes = [C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.psb_debug_sort_pairs.restype = C.c_int
     L.psb_debug_sort_pairs.argtypes = [vp, vp, C.c_size_t, C.c_int, vp]
     _lib = L

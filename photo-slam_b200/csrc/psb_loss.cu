@@ -60,11 +60,11 @@ __device__ __forceinline__ float exposed(const ExpCol& e, const float* __restric
 }
 
 // grid (tiles_x, tiles_y, 3), block 256 (16x16). EXP: the loss of X = mask * I' (E: the device row, see ExpCol) instead of mask * I.
-template <bool DET, bool EXP = false>
-__device__ __forceinline__ void loss_fwd_body(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
-                                              const float* __restrict__ mask, const Win& win, float g_ssim,
-                                              float* __restrict__ dmap /* [3 maps][3][H][W] */, double* __restrict__ sums /* [2] | DET: [blocks][2] */,
-                                              const float* __restrict__ E = nullptr)
+template <bool DET, bool EXP>
+__global__ void __launch_bounds__(256) loss_fwd_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
+                                                       const float* __restrict__ mask, Win win, float g_ssim,
+                                                       float* __restrict__ dmap /* [3 maps][3][H][W] */,
+                                                       double* __restrict__ sums /* [2] | DET: [blocks][2] */, const float* __restrict__ E)
 {
 	__shared__ float s_x[LS][LS + 1], s_y[LS][LS + 1];
 	__shared__ float s_h[5][LS][LT + 1];
@@ -133,34 +133,6 @@ __device__ __forceinline__ void loss_fwd_body(int H, int W, const float* __restr
 	block_sums_out<DET>(tl1, tss, sums);
 }
 
-__global__ void __launch_bounds__(256) loss_fwd_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
-                                                       const float* __restrict__ mask, Win win, float g_ssim, float* __restrict__ dmap,
-                                                       double* __restrict__ sums)
-{
-	loss_fwd_body<false>(H, W, img, gt, mask, win, g_ssim, dmap, sums);
-}
-
-__global__ void __launch_bounds__(256) loss_fwd_det_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
-                                                           const float* __restrict__ mask, Win win, float g_ssim, float* __restrict__ dmap,
-                                                           double* __restrict__ partials)
-{
-	loss_fwd_body<true>(H, W, img, gt, mask, win, g_ssim, dmap, partials);
-}
-
-__global__ void __launch_bounds__(256) loss_fwd_exp_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
-                                                           const float* __restrict__ mask, Win win, float g_ssim, float* __restrict__ dmap,
-                                                           double* __restrict__ sums, const float* __restrict__ E)
-{
-	loss_fwd_body<false, true>(H, W, img, gt, mask, win, g_ssim, dmap, sums, E);
-}
-
-__global__ void __launch_bounds__(256) loss_fwd_exp_det_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
-                                                               const float* __restrict__ mask, Win win, float g_ssim, float* __restrict__ dmap,
-                                                               double* __restrict__ partials, const float* __restrict__ E)
-{
-	loss_fwd_body<true, true>(H, W, img, gt, mask, win, g_ssim, dmap, partials, E);
-}
-
 // Deterministic mode: sums[c] = the n block partials partials[2 b + c] (c = 0, 1) added in a fixed order (one block: strided
 // per-thread sums, then a fixed tree), whatever order the blocks that wrote them ran in.
 __global__ void __launch_bounds__(256) reduce_partials_kernel(int n, const double* __restrict__ partials, double* __restrict__ sums)
@@ -179,12 +151,12 @@ __global__ void __launch_bounds__(256) reduce_partials_kernel(int n, const doubl
 	if (tid == 0) { sums[0] = s[0][0]; sums[1] = s[1][0]; }
 }
 
-// EXP: evaluated at x = X = mask * I' (see loss_fwd_body); dL_dimg then receives g = dL/dI' (mask factor applied), which
+// EXP: evaluated at x = X = mask * I' (see loss_fwd_kernel); dL_dimg then receives g = dL/dI' (mask factor applied), which
 // exposure_mix_kernel turns into dL/dI.
 template <bool EXP>
-__device__ __forceinline__ void loss_bwd_body(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
-                                              const float* __restrict__ mask, const Win& win, float g_l1,
-                                              const float* __restrict__ dmap, float* __restrict__ dL_dimg, const float* __restrict__ E)
+__global__ void __launch_bounds__(256) loss_bwd_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
+                                                       const float* __restrict__ mask, Win win, float g_l1,
+                                                       const float* __restrict__ dmap, float* __restrict__ dL_dimg, const float* __restrict__ E)
 {
 	__shared__ float s_d[3][LS][LS + 1];
 	__shared__ float s_h[3][LS][LT + 1];
@@ -232,21 +204,7 @@ __device__ __forceinline__ void loss_bwd_body(int H, int W, const float* __restr
 	}
 }
 
-__global__ void __launch_bounds__(256) loss_bwd_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
-                                                       const float* __restrict__ mask, Win win, float g_l1,
-                                                       const float* __restrict__ dmap, float* __restrict__ dL_dimg)
-{
-	loss_bwd_body<false>(H, W, img, gt, mask, win, g_l1, dmap, dL_dimg, nullptr);
-}
-
-__global__ void __launch_bounds__(256) loss_bwd_exp_kernel(int H, int W, const float* __restrict__ img, const float* __restrict__ gt,
-                                                           const float* __restrict__ mask, Win win, float g_l1,
-                                                           const float* __restrict__ dmap, float* __restrict__ dL_dimg, const float* __restrict__ E)
-{
-	loss_bwd_body<true>(H, W, img, gt, mask, win, g_l1, dmap, dL_dimg, E);
-}
-
-// Exposure, pass 1 (grid-stride over the n = H W pixels, 256 threads): g = dL/dI' in dL_dpix (loss_bwd_exp_kernel) becomes
+// Exposure, pass 1 (grid-stride over the n = H W pixels, 256 threads): g = dL/dI' in dL_dpix (loss_bwd_kernel<true>) becomes
 // dL/dI(k) = sum_c E[k][c] g(c) in place, the plane the tile backward reads; the block's 12 sums
 // dL/dE[k][c] = sum_p g(c) I(k) (k < 3) and dL/dE[c][3] = sum_p g(c) go to partials[12 block + 4 r + j] (the layout of E) in double.
 __global__ void __launch_bounds__(256) exposure_mix_kernel(int n, const float* __restrict__ E, const float* __restrict__ img,
@@ -337,8 +295,8 @@ __global__ void __launch_bounds__(256) exposure_update_kernel(int n, const doubl
 // Depth L1, pass 1 (grid-stride, 256 threads): per valid pixel |D - G| and sign(D - G) (-> dL_dD, scaled by pass 2); block sums of
 // |D - G| and of the valid count go to sums[0], sums[1] in double (the count is exact); DET: to the block's partials.
 template <bool DET>
-__device__ __forceinline__ void depth_loss_body(int n, const float* __restrict__ D, const float* __restrict__ G, const float* __restrict__ mask,
-                                                float* __restrict__ dL_dD, double* __restrict__ sums)
+__global__ void __launch_bounds__(256) depth_loss_kernel(int n, const float* __restrict__ D, const float* __restrict__ G, const float* __restrict__ mask,
+                                                         float* __restrict__ dL_dD, double* __restrict__ sums)
 {
 	__shared__ float s_red[8];
 	float acc = 0.f, cnt = 0.f;
@@ -359,18 +317,6 @@ __device__ __forceinline__ void depth_loss_body(int n, const float* __restrict__
 	block_sums_out<DET>(tacc, tcnt, sums);
 }
 
-__global__ void __launch_bounds__(256) depth_loss_kernel(int n, const float* __restrict__ D, const float* __restrict__ G, const float* __restrict__ mask,
-                                                         float* __restrict__ dL_dD, double* __restrict__ sums)
-{
-	depth_loss_body<false>(n, D, G, mask, dL_dD, sums);
-}
-
-__global__ void __launch_bounds__(256) depth_loss_det_kernel(int n, const float* __restrict__ D, const float* __restrict__ G, const float* __restrict__ mask,
-                                                             float* __restrict__ dL_dD, double* __restrict__ partials)
-{
-	depth_loss_body<true>(n, D, G, mask, dL_dD, partials);
-}
-
 // Depth L1, pass 2: dL_dD *= lambda / max(N_valid, 1), N_valid read on the device (no host round trip).
 __global__ void __launch_bounds__(256) depth_grad_scale_kernel(int n, float lambda, const double* __restrict__ sums, float* __restrict__ dL_dD)
 {
@@ -385,15 +331,14 @@ int launch_depth_loss(int H, int W, const float* depth, const float* gt_depth, c
 {
 	const int n = H * W;
 	const int grid = depth_loss_blocks(H, W);
-	if (partials) {
-		depth_loss_det_kernel<<<grid, 256, 0, stream>>>(n, depth, gt_depth, mask, dL_dD, partials);
-		PSB_LAUNCH_OK();
-		reduce_partials_kernel<<<1, 256, 0, stream>>>(grid, partials, sums);
-	} else {
-		PSB_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), stream));
-		depth_loss_kernel<<<grid, 256, 0, stream>>>(n, depth, gt_depth, mask, dL_dD, sums);
-	}
+	const bool det = partials != nullptr;
+	if (!det) PSB_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), stream));
+	(det ? depth_loss_kernel<true> : depth_loss_kernel<false>)<<<grid, 256, 0, stream>>>(n, depth, gt_depth, mask, dL_dD, det ? partials : sums);
 	PSB_LAUNCH_OK();
+	if (det) {
+		reduce_partials_kernel<<<1, 256, 0, stream>>>(grid, partials, sums);
+		PSB_LAUNCH_OK();
+	}
 	depth_grad_scale_kernel<<<grid, 256, 0, stream>>>(n, lambda_depth, sums, dL_dD);
 	PSB_LAUNCH_OK();
 	return 0;
@@ -410,20 +355,19 @@ int launch_loss(int H, int W, const float* img, const float* gt, const float* ma
 	for (int x = 0; x < 11; x++) win.w[x] /= s;
 	const float inv_n = 1.0f / (3.0f * (float)H * (float)W);
 	dim3 grid((W + LT - 1) / LT, (H + LT - 1) / LT, 3);
-	if (partials) {
-		if (E) loss_fwd_exp_det_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, -lambda_dssim * inv_n, dmap, partials, E);
-		else loss_fwd_det_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, -lambda_dssim * inv_n, dmap, partials);
-		PSB_LAUNCH_OK();
-		reduce_partials_kernel<<<1, 256, 0, stream>>>((int)(grid.x * grid.y * grid.z), partials, sums);
-	} else {
-		PSB_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), stream));
-		if (E) loss_fwd_exp_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, -lambda_dssim * inv_n, dmap, sums, E);
-		else loss_fwd_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, -lambda_dssim * inv_n, dmap, sums);
-	}
+	const bool det = partials != nullptr;
+	const auto fwd = det ? (E ? loss_fwd_kernel<true, true> : loss_fwd_kernel<true, false>)
+	                     : (E ? loss_fwd_kernel<false, true> : loss_fwd_kernel<false, false>);
+	if (!det) PSB_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), stream));
+	fwd<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, -lambda_dssim * inv_n, dmap, det ? partials : sums, E);
 	PSB_LAUNCH_OK();
+	if (det) {
+		reduce_partials_kernel<<<1, 256, 0, stream>>>((int)(grid.x * grid.y * grid.z), partials, sums);
+		PSB_LAUNCH_OK();
+	}
 	if (dL_dimg) {
-		if (E) loss_bwd_exp_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, (1.0f - lambda_dssim) * inv_n, dmap, dL_dimg, E);
-		else loss_bwd_kernel<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, (1.0f - lambda_dssim) * inv_n, dmap, dL_dimg);
+		(E ? loss_bwd_kernel<true> : loss_bwd_kernel<false>)<<<grid, 256, 0, stream>>>(H, W, img, gt, mask, win, (1.0f - lambda_dssim) * inv_n, dmap,
+		                                                                              dL_dimg, E);
 		PSB_LAUNCH_OK();
 	}
 	return 0;

@@ -731,7 +731,7 @@ int launch_signal(uint32_t* const* flag, float* const* meta, const float* campos
 
 int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, float* seeds,
                           const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
-                          cudaStream_t stream, cudaEvent_t between, unsigned char* adam_live, bool depth, bool aa)
+                          cudaStream_t stream, cudaEvent_t between, unsigned char* adam_live, const PassMode& mode)
 {
 	if (P - first <= 0) return 0;
 	if (!seeds) { set_error_msg("launch_fused_backward: seed scratch missing"); return -1; }
@@ -739,9 +739,9 @@ int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, co
 	DpPush nodp;
 	memset(&nodp, 0, sizeof(nodp));
 	unsigned char* live = adam ? adam_live : nullptr;
-	const int mode = (live ? MODE_ADAM_LIVE : adam ? MODE_ADAM : MODE_GRADS) | (depth ? MODE_DEPTH : 0) | (aa ? MODE_AA : 0);
+	const int variant = (live ? MODE_ADAM_LIVE : adam ? MODE_ADAM : MODE_GRADS) | (mode.depth ? MODE_DEPTH : 0) | (mode.aa ? MODE_AA : 0);
 	int rc;
-	if ((rc = launch_gaussian_backward(mode, first, P, t, cam, geom, sink, h, grads, st, counters, capacity, seeds, nodp, live, stream))) return rc;
+	if ((rc = launch_gaussian_backward(variant, first, P, t, cam, geom, sink, h, grads, st, counters, capacity, seeds, nodp, live, stream))) return rc;
 	if (between) cudaEventRecord(between, stream);
 	const AdamCoef ac(h);
 	const uint32_t e0 = (uint32_t)first * REST, e1 = (uint32_t)P * REST;
@@ -761,12 +761,12 @@ int launch_adam_live_rebuild(int P, const TrainTensors& t, unsigned char* live, 
 }
 
 int launch_push_backward(int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, const StepHyper& h,
-                         const DensifyStats& st, const uint32_t* counters, uint32_t capacity, const DpPush& dp, cudaStream_t stream, bool depth,
-                         bool aa)
+                         const DensifyStats& st, const uint32_t* counters, uint32_t capacity, const DpPush& dp, cudaStream_t stream,
+                         const PassMode& mode)
 {
 	const GradSegments nog = {};
 	int rc;
-	if ((rc = launch_gaussian_backward(MODE_PUSH | (depth ? MODE_DEPTH : 0) | (aa ? MODE_AA : 0), 0, P, t, cam, geom, sink, h, nog, st, counters, capacity, nullptr, dp,
+	if ((rc = launch_gaussian_backward(MODE_PUSH | (mode.depth ? MODE_DEPTH : 0) | (mode.aa ? MODE_AA : 0), 0, P, t, cam, geom, sink, h, nog, st, counters, capacity, nullptr, dp,
 	                                   nullptr, stream)))
 		return rc;
 	return launch_signal(dp.grad_flag, dp.meta, cam.campos, h.D, dp.world, dp.rank, dp.epoch, stream);

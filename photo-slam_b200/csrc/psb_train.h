@@ -28,6 +28,13 @@ struct DensifyStats {
 	float* xyz_gradient_accum;  // [P,1]
 	float* denom;               // [P,1]
 };
+// The mode of one training-context pass, recorded when the pass runs; its tile backward and per-Gaussian stage run this variant.
+struct PassMode {
+	int D;       // SH degree of the pass; -1: no psb_trainer_backward_pixels may follow it
+	bool det;    // deterministic mode
+	bool aa;     // the forward was anti-aliased (launch_preprocess aa): slot 7 of the sink rows holds dL/do'
+	bool depth;  // the sink rows carry dL/dz in slot 11 (render_bwd_kernel<true, ...>)
+};
 
 // ---- NVLink data-parallel step (psb_dp_*, include/psb200.h) -----------------------------------------------------------
 // Ownership: Gaussians are cut into chunks of 128 (one block of the per-Gaussian backward); chunk c belongs to rank
@@ -53,8 +60,7 @@ struct DpShard {             // what the owner-side Adam kernels need
 };
 int launch_push_backward(int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, const StepHyper& h,
                          const DensifyStats& st, const uint32_t* counters, uint32_t capacity, const DpPush& dp, cudaStream_t stream,
-                         bool depth = false /* the sink rows carry dL/dz in slot 11 (render_bwd_kernel<true, ...>) */,
-                         bool aa = false /* the forward was anti-aliased (launch_preprocess aa): slot 7 holds dL/do' */);
+                         const PassMode& mode);
 int launch_shard_adam(const DpShard& d, const TrainTensors& t, const StepHyper& h, float grad_scale, cudaStream_t stream, cudaEvent_t between = nullptr);
 // spins (device side) until flags[0..world) >= epoch (world <= 32 words); after `timeout_ms` writes 1 to *status and gives up
 int launch_wait_flags(const uint32_t* flags, int world, uint32_t epoch, uint32_t* status, cudaStream_t stream);
@@ -63,10 +69,8 @@ int launch_wait_flags(const uint32_t* flags, int world, uint32_t epoch, uint32_t
 // seeds: scratch [P][20] floats (per-Gaussian SH gradient seeds handed from the per-Gaussian kernel to the f_rest stream kernel)
 int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, float* seeds,
                           const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
-                          cudaStream_t stream, cudaEvent_t between = nullptr /* recorded between the two kernels (stage timing) */,
-                          unsigned char* adam_live = nullptr /* adam only: psb_model.adam_live, or null (the moments tell idle rows) */,
-                          bool depth = false /* the sink rows carry dL/dz in slot 11 (render_bwd_kernel<true, ...>) */,
-                          bool aa = false /* the forward was anti-aliased (launch_preprocess aa): slot 7 holds dL/do' */);
+                          cudaStream_t stream, cudaEvent_t between /* recorded between the two kernels (stage timing), or null */,
+                          unsigned char* adam_live /* adam only: psb_model.adam_live, or null (the moments tell idle rows) */, const PassMode& mode);
 // adam_live[i] = any moment of row i non-zero (t.m / t.v: the 12 moment tensors)
 int launch_adam_live_rebuild(int P, const TrainTensors& t, unsigned char* adam_live, cudaStream_t stream);
 int launch_adam(size_t n, float* p, float* m, float* v, const float* g, float lr, const StepHyper& h, float grad_scale, cudaStream_t stream);
@@ -75,7 +79,7 @@ int launch_adam(size_t n, float* p, float* m, float* v, const float* g, float lr
 // E != null: exposure compensation, the loss of mask * I' with I'(c) = sum_k E[k][c] I(k) + E[c][3] (E: device [3][4], row-major);
 // dL_dimg then receives g = dL/dI' (mask factor applied) and launch_exposure must follow.
 int launch_loss(int H, int W, const float* img, const float* gt, const float* mask, float lambda_dssim, float* dmap, double* sums,
-                float* dL_dimg, cudaStream_t stream, double* partials = nullptr, const float* E = nullptr);
+                float* dL_dimg, cudaStream_t stream, double* partials, const float* E);
 // The Adam state of one exposure row (psb_exposure): all device pointers, the step count advanced on the device.
 struct ExposureUpdate {
 	float* param;
@@ -95,7 +99,7 @@ constexpr size_t kExposurePartials = 12 * (size_t)kNumSMs * 8;   // doubles: eno
 // dL_dD [H,W] = lambda * sign(D - G) / max(N_valid, 1) on valid pixels, 0 elsewhere. Two launches, no host synchronisation.
 // partials: as launch_loss.
 int launch_depth_loss(int H, int W, const float* depth, const float* gt_depth, const float* mask, float lambda_depth, double* sums, float* dL_dD,
-                      cudaStream_t stream, double* partials = nullptr);
+                      cudaStream_t stream, double* partials);
 inline int depth_loss_blocks(int H, int W) { return min(cdiv(H * W, 256), kNumSMs * 8); }
 // launch_loss runs one block per 16 x 16 tile and channel
 inline size_t loss_partials_doubles(int H, int W)

@@ -28,15 +28,12 @@ struct psb_trainer {
 	uint32_t* h_count = nullptr; // pinned [4]: instance count of the last call | sticky overflow record {count, first seq, largest count}
 	uint32_t* ovf = nullptr;     // device [4]: the sticky overflow record (tile_ranges_kernel), collected by psb_trainer_result
 	uint32_t seq = 0;            // sequence number of the last forward pass (render / step / backward) of this context
-	// what psb_trainer_backward_pixels must match: the SH degree and the mode of pass `seq` (-1: no pass a backward may follow: a
-	// training call's pass, which had its own backward, or a pass whose arena psb_trainer_result regrew)
-	int pass_D = -1;
-	bool pass_det = false;
-	bool pass_aa = false;
+	// the mode of pass `seq`: what psb_trainer_backward_pixels must match, and the variant every per-Gaussian stage behind it runs
+	// (a psb_trainer_backward_begin* records it before its pass, so the _slab calls after it run that variant even if it failed)
+	PassMode pass = {-1, false, false, false};
 	// anti-aliasing (psb_trainer_set_antialiasing): every forward pass blends with o' = o h (the 2D Mip filter), and every per-Gaussian
 	// backward behind it runs the AA variant
 	bool antialiasing = false;
-	bool slab_aa = false;          // the mode of the last psb_trainer_backward_begin*: every _slab after it runs that variant
 	uint32_t ovf_first = 0, ovf_count = 0;  // what the last PSB_ERR_RETRY was about (psb_trainer_overflow_info)
 	cudaEvent_t readback = nullptr;  // recorded once the instance count (and the loss sums) of the last call are in pinned memory
 	int last_P = 0, last_W = 0, last_H = 0;
@@ -44,7 +41,6 @@ struct psb_trainer {
 	float last_lambda_depth = 0.f;
 	bool have_loss = false;
 	bool have_depth_loss = false;  // the last step had a depth term (h_sums[2..3] belong to it)
-	bool slab_depth = false;       // the last psb_trainer_backward_begin* had a depth term: its sink rows carry dL/dz, every _slab must consume slot 11
 	// tight instance lists: only the tiles a splat can reach get an instance (see preprocess_fwd_kernel); PSB_TIGHT=0 keeps the
 	// reference's full rectangles (A/B measurements only — images and gradients are the same either way)
 	bool tight = !(getenv("PSB_TIGHT") && atoi(getenv("PSB_TIGHT")) == 0);
@@ -76,81 +72,73 @@ struct psb_trainer {
 
 namespace {
 
+// An arena buffer that is missing or too small: drain the stream (the last call's kernels may still use the old buffer), free it and
+// allocate `count` elements, zeroed on the stream when `zero`.
 template <typename T>
-int dev_alloc(T** p, size_t count)
+int regrow(T** p, size_t count, bool zero, cudaStream_t stream)
 {
+	PSB_CUDA_OK(cudaStreamSynchronize(stream));
 	if (*p) { cudaFree(*p); *p = nullptr; }
 	PSB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(p), count * sizeof(T) + 256));
+	if (zero) PSB_CUDA_OK(cudaMemsetAsync(*p, 0, count * sizeof(T), stream));
 	return 0;
 }
 
-int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_loss = false)
+int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_loss)
 {
 	const size_t N = (size_t)W * H;
 	int rc;
 	if (t->geom_P != P) {
-		PSB_CUDA_OK(cudaStreamSynchronize(stream));
 		t->geom_bytes = required_bytes<GeomState>((size_t)P);
-		if ((rc = dev_alloc(&t->geom_chunk, t->geom_bytes))) return rc;
+		if ((rc = regrow(&t->geom_chunk, t->geom_bytes, false, stream))) return rc;
 		t->geom_P = P;
 	}
 	if (t->img_N != (int)N) {
-		PSB_CUDA_OK(cudaStreamSynchronize(stream));
 		t->img_bytes = required_bytes<ImgState>(N);
-		if ((rc = dev_alloc(&t->img_chunk, t->img_bytes))) return rc;
+		if ((rc = regrow(&t->img_chunk, t->img_bytes, false, stream))) return rc;
 		t->img_N = (int)N;
 	}
 	if (t->pix_alloc < N) {
-		PSB_CUDA_OK(cudaStreamSynchronize(stream));
-		if ((rc = dev_alloc(&t->image, 3 * N))) return rc;
-		if ((rc = dev_alloc(&t->dL_dpix, 3 * N))) return rc;
-		if ((rc = dev_alloc(&t->dmap, 9 * N))) return rc;
+		if ((rc = regrow(&t->image, 3 * N, false, stream)) || (rc = regrow(&t->dL_dpix, 3 * N, false, stream)) ||
+		    (rc = regrow(&t->dmap, 9 * N, false, stream)))
+			return rc;
 		t->pix_alloc = N;
 	}
 	if (depth_loss && t->depth_alloc < N) {
-		PSB_CUDA_OK(cudaStreamSynchronize(stream));
-		if ((rc = dev_alloc(&t->depth_buf, 2 * N))) return rc;
+		if ((rc = regrow(&t->depth_buf, 2 * N, false, stream))) return rc;
 		t->depth_alloc = N;
 	}
 	if (t->sink_P < (size_t)P) {
-		PSB_CUDA_OK(cudaStreamSynchronize(stream));
-		if ((rc = dev_alloc(&t->sink, (size_t)P * 12))) return rc;
-		if ((rc = dev_alloc(&t->seeds, (size_t)P * 20))) return rc;
-		PSB_CUDA_OK(cudaMemsetAsync(t->sink, 0, (size_t)P * 12 * sizeof(float), stream));
+		if ((rc = regrow(&t->sink, (size_t)P * 12, true, stream)) || (rc = regrow(&t->seeds, (size_t)P * 20, false, stream))) return rc;
 		t->sink_P = (size_t)P;
 	}
 	if (!t->sums) {
-		if ((rc = dev_alloc(&t->sums, 4))) return rc;
+		if ((rc = regrow(&t->sums, 4, false, stream))) return rc;
 		PSB_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&t->h_sums), 4 * sizeof(double)));
 		PSB_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&t->h_count), 4 * sizeof(uint32_t)));
 		memset(t->h_count, 0, 4 * sizeof(uint32_t));
-		if ((rc = dev_alloc(&t->ovf, 4))) return rc;
+		if ((rc = regrow(&t->ovf, 4, false, stream))) return rc;
 		const uint32_t init[4] = {0u, 0xFFFFFFFFu, 0u, 0u};
 		PSB_CUDA_OK(cudaMemcpy(t->ovf, init, sizeof(init), cudaMemcpyHostToDevice));
 		PSB_CUDA_OK(cudaEventCreateWithFlags(&t->readback, cudaEventDisableTiming));
 	}
 	const size_t want = (size_t)P * 6 + (1u << 16);
 	if (t->capacity == 0 || (t->capacity < want && t->last_P != P)) {
-		PSB_CUDA_OK(cudaStreamSynchronize(stream));
 		t->capacity = t->capacity > want ? t->capacity : want;
 		t->bin_bytes = required_bytes<BinState>(t->capacity);
-		if ((rc = dev_alloc(&t->bin_chunk, t->bin_bytes))) return rc;
+		if ((rc = regrow(&t->bin_chunk, t->bin_bytes, false, stream))) return rc;
 	}
 	if (t->deterministic) {
 		if (t->det_cap < t->capacity) {
-			PSB_CUDA_OK(cudaStreamSynchronize(stream));
-			if ((rc = dev_alloc(&t->det_slots, t->capacity * 12))) return rc;
-			PSB_CUDA_OK(cudaMemsetAsync(t->det_slots, 0, t->capacity * 12 * sizeof(float), stream));
+			if ((rc = regrow(&t->det_slots, t->capacity * 12, true, stream))) return rc;
 			t->det_cap = t->capacity;
 		}
 		if (t->det_P < (size_t)P) {
-			PSB_CUDA_OK(cudaStreamSynchronize(stream));
-			if ((rc = dev_alloc(&t->det_base, (size_t)P))) return rc;
+			if ((rc = regrow(&t->det_base, (size_t)P, false, stream))) return rc;
 			t->det_P = (size_t)P;
 		}
 		if (t->det_parts < loss_partials_doubles(H, W)) {
-			PSB_CUDA_OK(cudaStreamSynchronize(stream));
-			if ((rc = dev_alloc(&t->det_partials, loss_partials_doubles(H, W)))) return rc;
+			if ((rc = regrow(&t->det_partials, loss_partials_doubles(H, W), false, stream))) return rc;
 			t->det_parts = loss_partials_doubles(H, W);
 		}
 	}
@@ -276,14 +264,19 @@ int check_grads(float* const* grads, int P, const char* fn)
 	return 0;
 }
 
-// Stage 1 of every pass: forward from raw parameters into t->image (or out_color); out_depth != NULL: the depth variant also writes the
-// expected depth there; out_alpha != NULL: the opacity variant also writes 1 - final_T there
+// The mode of a pass that starts now, in the context's deterministic and anti-aliasing modes.
+PassMode pass_mode(const psb_trainer* t, int D, bool depth) { return {D, t->deterministic, t->antialiasing, depth}; }
+
+// Stage 1 of every pass: forward of SH degree D from raw parameters into t->image (or out_color); out_depth != NULL: the depth variant
+// also writes the expected depth there; out_alpha != NULL: the opacity variant also writes 1 - final_T there. The pass is recorded as
+// `mode`, with D = -1 until it has been binned.
 int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, const psb_camera* camera, const float* background,
-                float* out_color, int* radii, Scratch& sc, Camera& cam, cudaStream_t stream, float* out_depth = nullptr, float* out_alpha = nullptr)
+                float* out_color, int* radii, Scratch& sc, Camera& cam, cudaStream_t stream, float* out_depth, float* out_alpha, const PassMode& mode)
 {
 	int rc;
-	t->pass_D = -1;
-	if ((rc = ensure(t, P, camera->width, camera->height, stream))) return rc;
+	t->pass = mode;
+	t->pass.D = -1;
+	if ((rc = ensure(t, P, camera->width, camera->height, stream, mode.depth))) return rc;
 	cam = to_camera(camera);
 	sc = carve_scratch(t, P, camera->width, camera->height);
 	GeomState& geom = sc.geom;
@@ -291,15 +284,13 @@ int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, con
 	ImgState& img = sc.img;
 	const GaussIn in = raw_input(P, D, M, model);
 	t->mark(0, stream);
-	if ((rc = launch_preprocess(in, cam, radii, geom, /*raw=*/true, t->tight, stream, t->antialiasing))) return rc;
-	t->pass_aa = t->antialiasing;
+	if ((rc = launch_preprocess(in, cam, radii, geom, /*raw=*/true, t->tight, stream, mode.aa))) return rc;
 	t->mark(1, stream);
 	if ((rc = launch_depth_sort_and_scan(P, geom, /*scan=*/false, stream))) return rc;
 	t->mark(2, stream);
-	if ((rc = launch_scan_binning(P, cam, geom, bin, img, t->capacity, t->tight, t->ovf, ++t->seq, stream, t->deterministic ? t->det_base : nullptr)))
+	if ((rc = launch_scan_binning(P, cam, geom, bin, img, t->capacity, t->tight, t->ovf, ++t->seq, stream, mode.det ? t->det_base : nullptr)))
 		return rc;
-	t->pass_D = D;
-	t->pass_det = t->deterministic;
+	t->pass.D = mode.D;
 	t->mark(3, stream);
 	// the instance count travels to pinned memory as soon as it exists: psb_trainer_result waits on `readback`, not on the stream
 	PSB_CUDA_OK(cudaMemcpyAsync(t->h_count, geom.counters, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
@@ -311,8 +302,8 @@ int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, con
 	return rc;
 }
 
-// Stage 3 of every pass: the tile backward of the context's last forward pass (scratch sc, camera cam) on per-pixel gradients -> the
-// packed sink rows (dL_ddepth: also dL/dz in slot 11; dL_dalpha: the opacity variant). P > 0.
+// Stage 3 of every pass: the tile backward of the context's last forward pass (scratch sc, camera cam, mode t->pass) on per-pixel
+// gradients -> the packed sink rows (dL_ddepth: also dL/dz in slot 11; dL_dalpha: the opacity variant). P > 0.
 int tile_backward(psb_trainer* t, int P, const Scratch& sc, const Camera& cam, const float* background, const float* dL_dpix, const float* dL_ddepth,
                   const float* dL_dalpha, cudaStream_t stream)
 {
@@ -334,19 +325,17 @@ int tile_backward(psb_trainer* t, int P, const Scratch& sc, const Camera& cam, c
 	// (the deterministic gather runs inside this call: stage "render bwd" covers it)
 	int rc;
 	if ((rc = launch_render_backward(cam, sc.img.ranges, sc.bin.inst[sorted_slot(cam.W, cam.H)], sc.geom.rec, background, sc.img.final_T, sc.img.n_contrib,
-	                                 dL_dpix, sink, stream, dL_ddepth, t->pass_det ? &det : nullptr, dL_dalpha)))
+	                                 dL_dpix, sink, stream, dL_ddepth, t->pass.det ? &det : nullptr, dL_dalpha)))
 		return rc;
 	t->mark(6, stream);
 	return 0;
 }
 
-// What the first half of a training step leaves for its per-Gaussian stage: the sink rows hold the view's screen-space sums
-// (with a depth term also dL/dz in slot 11, which the per-Gaussian kernel that follows must consume).
+// What the first half of a training step leaves for its per-Gaussian stage, besides the sink rows (the view's screen-space sums; with a
+// depth term also dL/dz in slot 11, which the per-Gaussian kernel that follows must consume: it runs the variant t->pass names).
 struct TileBackward {
 	GeomState geom;
 	Camera cam;
-	bool depth;
-	bool aa;     // the forward was anti-aliased: the per-Gaussian stage runs the AA variant
 };
 
 // The built-in loss around the shared stages: forward -> loss (+ depth loss) -> pinned read-back of the loss sums -> (exposure) -> tile
@@ -354,7 +343,7 @@ struct TileBackward {
 // image through the row; exposure_grad == NULL: the row takes its Adam step (with step's betas and eps), else dL/dE -> exposure_grad.
 int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                          const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
-                         bool moments, cudaStream_t stream, TileBackward& out, const psb_exposure* exposure = nullptr, float* exposure_grad = nullptr)
+                         bool moments, cudaStream_t stream, TileBackward& out, const psb_exposure* exposure, float* exposure_grad)
 {
 	int rc;
 	if (!t || !camera || !step || !background || !gt_image) { set_error_msg("psb_trainer_step: null argument"); return PSB_ERR_ARG; }
@@ -369,16 +358,14 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 		if (!depth_plane) depth_plane = t->depth_buf;
 		dL_ddepth = t->depth_buf + (size_t)camera->width * camera->height;
 	}
-	if (exposure && !t->exp_partials) {
-		PSB_CUDA_OK(cudaStreamSynchronize(stream));
-		if ((rc = dev_alloc(&t->exp_partials, kExposurePartials))) return rc;
-	}
+	if (exposure && !t->exp_partials && (rc = regrow(&t->exp_partials, kExposurePartials, false, stream))) return rc;
 	Scratch sc;
 	Camera cam;
-	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, sc, cam, stream, depth_plane))) return rc;
 	// this pass gets its own tile backward below and its sink rows belong to this call's per-Gaussian stage (or to the _slab calls
-	// that follow a _begin): psb_trainer_backward_pixels must not add a second backward of it
-	t->pass_D = -1;
+	// that follow a _begin): psb_trainer_backward_pixels must not add a second backward of it (D = -1)
+	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, sc, cam, stream, depth_plane, nullptr,
+	                      pass_mode(t, -1, depth_loss))))
+		return rc;
 	const float* image = out_color ? out_color : t->image;
 	double* partials = t->deterministic ? t->det_partials : nullptr;
 	if ((rc = launch_loss(cam.H, cam.W, image, gt_image, mask, step->lambda_dssim, t->dmap, t->sums, t->dL_dpix, stream, partials,
@@ -407,8 +394,6 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	if ((rc = tile_backward(t, P, sc, cam, background, t->dL_dpix, dL_ddepth, nullptr, stream))) return rc;
 	out.geom = sc.geom;
 	out.cam = cam;
-	out.depth = depth_loss;
-	out.aa = t->pass_aa;
 	return 0;
 }
 
@@ -556,7 +541,9 @@ int psb_dp_step_depth(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* 
 	// render, loss, tile backward (the 9 screen-space sums per Gaussian; with a depth term also dL/dz in slot 11, which the push
 	// backward below must consume: a plain push backward would leave it in the sink for the next depth step)
 	TileBackward tb;
-	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, stream, tb)) || P == 0)
+	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, stream, tb, nullptr,
+	                               nullptr)) ||
+	    P == 0)
 		return rc;
 	const TrainTensors tt = train_tensors(model, true);
 	const StepHyper h = to_hyper(step);
@@ -579,7 +566,7 @@ int psb_dp_step_depth(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* 
 	// push backward (records go straight into the owners' inboxes) + signal; wait until every rank's records have landed -> Adam of
 	// the owned rows, updated rows stored to every replica + signal
 	if ((rc = launch_push_backward(P, tt, tb.cam, tb.geom, t->sink, h, densify_stats(model, step), tb.geom.counters, (uint32_t)t->capacity, push, stream,
-	                               tb.depth, tb.aa)))
+	                               t->pass)))
 		return rc;
 	t->mark(7, stream);
 	t->mark(8, stream);
@@ -625,7 +612,9 @@ static int forward_impl(const char* fn, psb_trainer* t, int P, int M, const psb_
 	Scratch sc;
 	Camera cam;
 	t->have_loss = false;
-	if ((rc = forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, sc, cam, stream, out_depth, out_alpha))) return rc;
+	if ((rc = forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, sc, cam, stream, out_depth, out_alpha,
+	                      pass_mode(t, sh_degree, false))))
+		return rc;
 	if (pass) *pass = t->seq;
 	return 0;
 }
@@ -659,19 +648,19 @@ int psb_trainer_backward_pixels(psb_trainer* t, unsigned pass, int P, int M, con
 	const bool adam = grads == nullptr;
 	if (!t || !camera || !background || !pixel_grads || !step) { set_error_msg("psb_trainer_backward_pixels: null argument"); return PSB_ERR_ARG; }
 	if (!pixel_grads->dL_dcolor) { set_error_msg("psb_trainer_backward_pixels: dL_dcolor is required"); return PSB_ERR_ARG; }
-	if (pass == 0 || pass != t->seq || t->pass_D < 0) {
+	if (pass == 0 || pass != t->seq || t->pass.D < 0) {
 		set_error_msg("psb_trainer_backward_pixels: `pass` is not the context's latest forward pass (or the arena was regrown since)");
 		return PSB_ERR_ARG;
 	}
-	if (P != t->last_P || P != t->geom_P || camera->width != t->last_W || camera->height != t->last_H || step->sh_degree != t->pass_D) {
+	if (P != t->last_P || P != t->geom_P || camera->width != t->last_W || camera->height != t->last_H || step->sh_degree != t->pass.D) {
 		set_error_msg("psb_trainer_backward_pixels: P, the image size and step->sh_degree must be those of the forward pass");
 		return PSB_ERR_ARG;
 	}
-	if (t->pass_det != t->deterministic) {
+	if (t->pass.det != t->deterministic) {
 		set_error_msg("psb_trainer_backward_pixels: the deterministic mode changed since the forward pass");
 		return PSB_ERR_ARG;
 	}
-	if (t->pass_aa != t->antialiasing) {
+	if (t->pass.aa != t->antialiasing) {
 		set_error_msg("psb_trainer_backward_pixels: the anti-aliasing mode changed since the forward pass");
 		return PSB_ERR_ARG;
 	}
@@ -683,13 +672,13 @@ int psb_trainer_backward_pixels(psb_trainer* t, unsigned pass, int P, int M, con
 	if (P == 0) return 0;
 	const Scratch sc = carve_scratch(t, P, camera->width, camera->height);
 	const Camera cam = to_camera(camera);
+	t->pass.depth = pixel_grads->dL_ddepth != nullptr;
 	if ((rc = tile_backward(t, P, sc, cam, background, pixel_grads->dL_dcolor, pixel_grads->dL_ddepth, pixel_grads->dL_dalpha, stream))) return rc;
 	GradSegments gs{};
 	if (!adam)
 		for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
 	rc = launch_fused_backward(adam, 0, P, train_tensors(model, adam), cam, sc.geom, t->sink, t->seeds, to_hyper(step), gs, densify_stats(model, step),
-	                           sc.geom.counters, (uint32_t)t->capacity, stream, t->event(7), adam ? model->adam_live : nullptr, pixel_grads->dL_ddepth != nullptr,
-	                           t->pass_aa);
+	                           sc.geom.counters, (uint32_t)t->capacity, stream, t->event(7), adam ? model->adam_live : nullptr, t->pass);
 	t->end_stages(8, stream);
 	return rc;
 }
@@ -717,11 +706,12 @@ int psb_trainer_step_exposure(psb_trainer* t, int P, int M, const psb_model* mod
 	if ((rc = check_depth(depth, fn))) return rc;
 	if ((rc = check_exposure(exposure, true, nullptr, fn))) return rc;
 	TileBackward tb;
-	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, true, stream, tb, exposure)) ||
+	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, true, stream, tb, exposure,
+	                               nullptr)) ||
 	    P == 0)
 		return rc;
 	rc = launch_fused_backward(true, 0, P, train_tensors(model, true), tb.cam, tb.geom, t->sink, t->seeds, to_hyper(step), GradSegments{},
-	                           densify_stats(model, step), tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), model->adam_live, tb.depth, tb.aa);
+	                           densify_stats(model, step), tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), model->adam_live, t->pass);
 	t->end_stages(8, stream);
 	return rc;
 }
@@ -759,7 +749,7 @@ int psb_trainer_backward_exposure(psb_trainer* t, int P, int M, const psb_model*
 	GradSegments gs;
 	for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
 	rc = launch_fused_backward(false, 0, P, train_tensors(model, false), tb.cam, tb.geom, t->sink, t->seeds, to_hyper(step), gs, densify_stats(model, step),
-	                           tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), nullptr, tb.depth, tb.aa);
+	                           tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), nullptr, t->pass);
 	t->end_stages(8, stream);
 	return rc;
 }
@@ -777,11 +767,11 @@ int psb_trainer_backward_begin_depth(psb_trainer* t, int P, int M, const psb_mod
 {
 	int rc;
 	if ((rc = check_depth(depth, "psb_trainer_backward_begin_depth"))) return rc;
-	// set whether or not the call below succeeds: the depth variant of _slab gives the plain result on rows without dL/dz
-	if (t) t->slab_depth = depth && depth->gt_depth;
-	if (t) t->slab_aa = t->antialiasing;
+	// recorded whether or not the call below succeeds: the depth variant of _slab gives the plain result on rows without dL/dz
+	if (t) t->pass = pass_mode(t, -1, depth && depth->gt_depth);
 	TileBackward tb;
-	return render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, (cudaStream_t)stream_, tb);
+	return render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, (cudaStream_t)stream_, tb,
+	                            nullptr, nullptr);
 }
 
 int psb_trainer_backward_begin(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
@@ -803,8 +793,7 @@ int psb_trainer_backward_slab(psb_trainer* t, int P, int M, const psb_model* mod
 	GradSegments gs;
 	for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
 	return launch_fused_backward(false, first, first + count, train_tensors(model, false), to_camera(camera), geom, t->sink, t->seeds, to_hyper(step), gs,
-	                             densify_stats(model, step), geom.counters, (uint32_t)t->capacity, (cudaStream_t)stream_, nullptr, nullptr, t->slab_depth,
-	                             t->slab_aa);
+	                             densify_stats(model, step), geom.counters, (uint32_t)t->capacity, (cudaStream_t)stream_, nullptr, nullptr, t->pass);
 }
 
 int psb_adam_update(int P, int M, const psb_model* model, float* const* grads, const psb_step* step, float grad_scale, void* stream_)
@@ -850,11 +839,11 @@ static int result_impl(psb_trainer* t, float* out, bool with_depth, int* num_ren
 		const uint32_t init[4] = {0u, 0xFFFFFFFFu, 0u, 0u};
 		PSB_CUDA_OK(cudaMemcpy(t->ovf, init, sizeof(init), cudaMemcpyHostToDevice));
 		t->h_count[1] = 0;
-		t->pass_D = -1;   // the scratch of the last pass is gone: no psb_trainer_backward_pixels for it
+		t->pass.D = -1;   // the scratch of the last pass is gone: no psb_trainer_backward_pixels for it
 		t->capacity = (size_t)(rec[2] * 1.25) + (1u << 16);
 		t->bin_bytes = required_bytes<BinState>(t->capacity);
 		int rc;
-		if ((rc = dev_alloc(&t->bin_chunk, t->bin_bytes))) return rc;
+		if ((rc = regrow(&t->bin_chunk, t->bin_bytes, false, stream))) return rc;
 		set_error_msg("psb_trainer: binning arena was too small for a view; it has been grown, repeat the call (psb_trainer_overflow_info says which)");
 		return PSB_ERR_RETRY;
 	}
@@ -981,7 +970,7 @@ int psb_loss(int height, int width, const float* image, const float* gt_image, c
 		set_error_msg("psb_loss: out of device memory");
 		return PSB_ERR_CUDA;
 	}
-	int rc = launch_loss(height, width, image, gt_image, mask, lambda_dssim, dmap, sums, dL_dimage, stream);
+	int rc = launch_loss(height, width, image, gt_image, mask, lambda_dssim, dmap, sums, dL_dimage, stream, nullptr, nullptr);
 	double h[2] = {0, 0};
 	if (rc == 0) {
 		cudaMemcpyAsync(h, sums, sizeof(h), cudaMemcpyDeviceToHost, stream);

@@ -7,7 +7,7 @@
   GaussianTrainer              reference GaussianMapper::trainForOneIteration (src/gaussian_mapper.cpp:614-774) /
                                GaussianTrainer::trainingOnce (src/gaussian_trainer.cpp:31-135): one iteration =
                                render, L1 + DSSIM, backward, densification statistics, Adam step — here ONE call
-                               into psb_trainer_step.
+                               into psb_trainer_step_exposure.
 PyTorch provides device memory, streams and (for the data-parallel variant) torch.distributed.
 """
 import ctypes as C
@@ -43,7 +43,7 @@ class _Depth(C.Structure):
 
 
 def _cdepth(gt_depth, lambda_depth, out_depth):
-    """psb_depth for a call, or None when it has no depth argument (the plain C function is called then)."""
+    """psb_depth for a call, or None when it has no depth argument (NULL is passed then)."""
     if gt_depth is None and out_depth is None and not lambda_depth:
         return None
     for t in (gt_depth, out_depth):
@@ -70,10 +70,11 @@ def _plane(t, shape, what):
     return t
 
 
-# what result() needs to repeat a trainWithLoss call whose forward overflowed the binning arena
-_LossCall = namedtuple("_LossCall", "cam loss_fn depth alpha out_color radii densify_stats")
-# a backwardPixels call on a render of the caller's: result() cannot repeat the caller's loss, it undoes the counters and raises
-_PixelsCall = namedtuple("_PixelsCall", "adam")
+# What result() knows of the last enqueuing call when its pass overflowed the binning arena: whether it advanced model.step_ and
+# iteration by one, how to enqueue it again (None: it cannot be repeated — backwardPixels on a render the caller computed a loss from),
+# and whether its loss is the caller's (result() then reports only that loss's value).
+_Call = namedtuple("_Call", "advanced repeat callers_loss")
+_NO_CALL = _Call(False, None, False)
 
 
 class _DensifyCfg(C.Structure):
@@ -82,54 +83,65 @@ class _DensifyCfg(C.Structure):
 
 
 def _bind():
+    """The library with every trainer, data-parallel, densification and debug entry point declared (include/psb200.h)."""
     L = _lib.lib()
     if getattr(L, "_trainer_bound", False):
         return L
-    vp = C.c_void_p
-    L.psb_trainer_create.argtypes = [C.POINTER(vp)]
-    L.psb_trainer_destroy.argtypes = [vp]
-    L.psb_trainer_render.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, C.c_int, vp, vp, vp]
-    L.psb_trainer_step.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp, vp, vp]
-    L.psb_trainer_backward.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp, vp,
-                                       C.POINTER(vp), vp]
-    L.psb_adam_update.argtypes = [C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(vp), C.POINTER(_Step), C.c_float, vp]
-    L.psb_trainer_result.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int), vp]
-    L.psb_trainer_render_depth.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, C.c_int, vp, vp, vp, vp]
-    L.psb_trainer_step_depth.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp, vp,
-                                         C.POINTER(_Depth), vp]
-    L.psb_trainer_backward_depth.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp, vp,
-                                             C.POINTER(vp), C.POINTER(_Depth), vp]
-    L.psb_trainer_result_depth.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_int), vp]
-    L.psb_trainer_step_exposure.argtypes = L.psb_trainer_step_depth.argtypes[:-1] + [C.POINTER(_Exposure), vp]
-    L.psb_trainer_backward_exposure.argtypes = L.psb_trainer_backward_depth.argtypes[:-1] + [C.POINTER(_Exposure), vp, vp]
-    L.psb_dp_step_depth.argtypes = [vp, vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp, vp,
-                                    C.POINTER(_Depth), vp]
-    L.psb_trainer_backward_begin_depth.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp,
-                                                   vp, C.POINTER(_Depth), vp]
-    L.psb_loss.argtypes = [C.c_int, C.c_int, vp, vp, vp, C.c_float, vp, C.POINTER(C.c_float), vp]
-    L.psb_trainer_set_deterministic.argtypes = [vp, C.c_int]
-    L.psb_trainer_set_antialiasing.argtypes = [vp, C.c_int]
-    L.psb_trainer_forward.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, C.c_int, vp, vp, vp, vp, C.POINTER(C.c_uint), vp]
-    L.psb_trainer_backward_pixels.argtypes = [vp, C.c_uint, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, C.POINTER(_PixelGrads),
-                                              C.POINTER(_Step), C.POINTER(vp), vp]
-    for n in ("psb_trainer_create", "psb_trainer_destroy", "psb_trainer_render", "psb_trainer_step", "psb_trainer_backward",
-              "psb_adam_update", "psb_trainer_result", "psb_loss", "psb_trainer_render_depth", "psb_trainer_step_depth",
-              "psb_trainer_backward_depth", "psb_trainer_result_depth", "psb_dp_step_depth", "psb_trainer_backward_begin_depth",
-              "psb_trainer_set_deterministic", "psb_trainer_forward", "psb_trainer_backward_pixels", "psb_trainer_set_antialiasing",
-              "psb_trainer_step_exposure", "psb_trainer_backward_exposure"):
-        getattr(L, n).restype = C.c_int
-    L.psb_densify_workspace_bytes.argtypes = [C.c_int]
-    L.psb_densify_workspace_bytes.restype = C.c_size_t
-    L.psb_densify_plan.argtypes = [C.c_int, C.POINTER(_Model), C.POINTER(_DensifyCfg), vp, C.POINTER(C.c_int), vp]
-    L.psb_densify_apply.argtypes = [C.c_int, C.POINTER(_Model), C.POINTER(_Model), C.c_int, C.POINTER(_DensifyCfg), vp, vp, vp]
-    L.psb_prune_plan.argtypes = [C.c_int, vp, vp, C.POINTER(C.c_int), vp]
-    L.psb_prune_apply.argtypes = [C.c_int, C.POINTER(_Model), C.POINTER(_Model), C.c_int, vp, C.c_int, vp]
-    L.psb_insert_points.argtypes = [C.c_int, C.POINTER(_Model), C.POINTER(_Model), C.c_int, vp, vp, vp, C.c_int, vp]
-    L.psb_reset_opacity.argtypes = [C.c_int, vp, vp, vp, vp]
-    L.psb_adam_live_rebuild.argtypes = [C.c_int, C.POINTER(_Model), vp]
-    for n in ("psb_densify_plan", "psb_densify_apply", "psb_prune_plan", "psb_prune_apply", "psb_insert_points", "psb_reset_opacity",
-              "psb_adam_live_rebuild"):
-        getattr(L, n).restype = C.c_int
+    vp, i, f, u, size_t = C.c_void_p, C.c_int, C.c_float, C.c_uint, C.c_size_t
+    P = C.POINTER
+    Model, Cam, Step, Depth, Exp, Cfg = P(_Model), P(_Camera), P(_Step), P(_Depth), P(_Exposure), P(_DensifyCfg)
+    # the arguments every built-in-loss training call starts with: t, P, M, model, camera, background, gt_image, mask, step, out_color, radii
+    call = [vp, i, i, Model, Cam, vp, vp, vp, Step, vp, vp]
+    render = [vp, i, i, Model, Cam, vp, i, vp, vp]   # t, P, M, model, camera, background, sh_degree, out_color, radii
+    sigs = {
+        "psb_trainer_create": [P(vp)],
+        "psb_trainer_destroy": [vp],
+        "psb_trainer_render": render + [vp],
+        "psb_trainer_render_depth": render + [vp, vp],
+        "psb_trainer_forward": render + [vp, vp, P(u), vp],
+        "psb_trainer_backward_pixels": [vp, u, i, i, Model, Cam, vp, P(_PixelGrads), Step, P(vp), vp],
+        "psb_trainer_step": call + [vp],
+        "psb_trainer_step_depth": call + [Depth, vp],
+        "psb_trainer_step_exposure": call + [Depth, Exp, vp],
+        "psb_trainer_backward": call + [P(vp), vp],
+        "psb_trainer_backward_depth": call + [P(vp), Depth, vp],
+        "psb_trainer_backward_exposure": call + [P(vp), Depth, Exp, vp, vp],
+        "psb_trainer_backward_begin": call + [vp],
+        "psb_trainer_backward_begin_depth": call + [Depth, vp],
+        "psb_trainer_backward_slab": [vp, i, i, Model, Cam, Step, i, i, P(vp), vp],
+        "psb_trainer_result": [vp, P(f), P(i), vp],
+        "psb_trainer_result_depth": [vp, P(f), P(i), vp],
+        "psb_trainer_overflow_info": [vp, P(u), P(u), P(u)],
+        "psb_trainer_debug_state": [vp, i, i, vp, vp, P(i), vp],
+        "psb_trainer_set_profiling": [vp, i],
+        "psb_trainer_stage_times": [vp, P(f), i],
+        "psb_trainer_set_deterministic": [vp, i],
+        "psb_trainer_set_antialiasing": [vp, i],
+        "psb_adam_update": [i, i, Model, P(vp), Step, f, vp],
+        "psb_adam_flat": [size_t, vp, vp, vp, vp, f, Step, f, vp],
+        "psb_adam_live_rebuild": [i, Model, vp],
+        "psb_loss": [i, i, vp, vp, vp, f, vp, P(f), vp],
+        "psb_dp_create": [P(vp), i, i, i],
+        "psb_dp_handle_bytes": [],
+        "psb_dp_ipc_handle": [vp, vp],
+        "psb_dp_connect": [vp, vp],
+        "psb_dp_params": [vp, P(vp)],
+        "psb_dp_step": [vp] + call + [vp],
+        "psb_dp_step_depth": [vp] + call + [Depth, vp],
+        "psb_dp_sync": [vp, vp],
+        "psb_dp_status": [vp, vp],
+        "psb_dp_destroy": [vp],
+        "psb_densify_plan": [i, Model, Cfg, vp, P(i), vp],
+        "psb_densify_apply": [i, Model, Model, i, Cfg, vp, vp, vp],
+        "psb_prune_plan": [i, vp, vp, P(i), vp],
+        "psb_prune_apply": [i, Model, Model, i, vp, i, vp],
+        "psb_insert_points": [i, Model, Model, i, vp, vp, vp, i, vp],
+        "psb_reset_opacity": [i, vp, vp, vp, vp],
+    }
+    for name, args in sigs.items():
+        fn = getattr(L, name)
+        fn.argtypes, fn.restype = args, i
+    L.psb_densify_workspace_bytes.argtypes, L.psb_densify_workspace_bytes.restype = [i], size_t
     L._trainer_bound = True
     return L
 
@@ -556,6 +568,7 @@ class GaussianTrainer:
         self.h = h
         self.background = background if background is not None else torch.zeros(3, device=model.device)
         self.iteration = 0
+        self._last = _NO_CALL
         self._deterministic = deterministic
         self._det_applied = False      # the mode the context is in (a new context starts with it off)
         self._apply_deterministic()
@@ -619,7 +632,7 @@ class GaussianTrainer:
                                               torch.cuda.current_stream().cuda_stream), "psb_trainer_forward")
         self._pass = pass_no.value
         self._last_render = (cam, out, radii, out_depth, out_alpha)
-        self._last = None
+        self._last = _Call(False, lambda: self.render(cam, out, radii, check=False, out_depth=out_depth, out_alpha=out_alpha), False)
         if check:
             self.result()
         return out
@@ -666,7 +679,7 @@ class GaussianTrainer:
         _lib.check(rc, "psb_trainer_backward_pixels")
         if adam:
             m.step_ += 1
-        self._last = _PixelsCall(adam)     # (trainWithLoss replaces it with its own record)
+        self._last = _Call(adam, None, False)     # (trainWithLoss replaces it with its own record)
 
     def trainWithLoss(self, cam, loss_fn, depth=False, alpha=False, out_color=None, radii=None, densify_stats=None):
         """One training iteration against the caller's loss: enqueues the forward (no host synchronisation of its own), calls
@@ -696,7 +709,7 @@ class GaussianTrainer:
         gd = next(g) if depth else None
         ga = next(g) if alpha else None
         self.backwardPixels(gc, gd, ga, densify_stats=densify_stats)
-        self._last = _LossCall(cam, loss_fn, depth, alpha, out_color, radii, densify_stats)
+        self._last = _Call(True, lambda: self.trainWithLoss(cam, loss_fn, depth, alpha, out_color, radii, densify_stats), True)
         self._last_loss = loss.detach()
         return self._last_loss
 
@@ -704,10 +717,10 @@ class GaussianTrainer:
                              out_depth=None, exposure_id=None):
         """Enqueues render -> loss -> backward -> Adam on the current stream (no host sync).
         gt_depth: [H,W] float32 target depth in metres (<= 0: no measurement) trained with weight lambda_depth (> 0) as an L1 term
-        over the valid pixels (psb_trainer_step_depth); out_depth: [H,W] float32 tensor that receives the rendered depth.
+        over the valid pixels; out_depth: [H,W] float32 tensor that receives the rendered depth.
         exposure_id: the keyframe id k of gt_image, or None. With an id, the loss compares gt_image with the render through exposure row
         k of the model (applyExposure; the table grows to k + 1 rows if needed) and that row takes one Adam step at
-        model.exposure_lr_ (psb_trainer_step_exposure). out_color stays the raw render; result() reports the compensated loss."""
+        model.exposure_lr_. out_color stays the raw render; result() reports the compensated loss. One psb_trainer_step_exposure call."""
         m = self.model
         depth = _cdepth(gt_depth, lambda_depth, out_depth)
         exposure = None
@@ -723,23 +736,22 @@ class GaussianTrainer:
         if densify_stats is None:
             densify_stats = self.iteration < self.opt.densify_until_iter
         cm, cc, cs = m._cmodel(live=m.adamLive()), _ccamera(cam), self._cstep(densify_stats)
-        args = (self.h, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(), gt_image.data_ptr(),
+        _lib.check(self.L.psb_trainer_step_exposure(*self._call_args(m, cm, cc, cs, gt_image, mask, out_color, radii),
+                                                    C.byref(depth) if depth is not None else None,
+                                                    C.byref(exposure) if exposure is not None else None, torch.cuda.current_stream().cuda_stream),
+                   "psb_trainer_step_exposure")
+        m.step_ += 1
+        self._last = _Call(True, lambda: self.trainForOneIteration(cam, gt_image, mask, out_color, radii, densify_stats, gt_depth, lambda_depth,
+                                                                   out_depth, exposure_id), False)
+
+    def _call_args(self, m, cm, cc, cs, gt_image, mask, out_color, radii):
+        """The leading arguments of a built-in-loss training call (t ... radii)."""
+        return (self.h, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(), gt_image.data_ptr(),
                 mask.data_ptr() if mask is not None else None, C.byref(cs), out_color.data_ptr() if out_color is not None else None,
                 radii.data_ptr() if radii is not None else None)
-        stream = torch.cuda.current_stream().cuda_stream
-        if exposure is not None:
-            _lib.check(self.L.psb_trainer_step_exposure(*args, C.byref(depth) if depth is not None else None, C.byref(exposure), stream),
-                       "psb_trainer_step_exposure")
-        elif depth is None:
-            _lib.check(self.L.psb_trainer_step(*args, stream), "psb_trainer_step")
-        else:
-            _lib.check(self.L.psb_trainer_step_depth(*args, C.byref(depth), stream), "psb_trainer_step_depth")
-        m.step_ += 1
-        self._last = (cam, gt_image, mask, out_color, radii, densify_stats, gt_depth, lambda_depth, out_depth, exposure_id)
 
     def _overflow_info(self):
         f, n, cur = C.c_uint(), C.c_uint(), C.c_uint()
-        self.L.psb_trainer_overflow_info.argtypes = [C.c_void_p, C.POINTER(C.c_uint), C.POINTER(C.c_uint), C.POINTER(C.c_uint)]
         self.L.psb_trainer_overflow_info(self.h, C.byref(f), C.byref(n), C.byref(cur))
         return f.value, n.value, cur.value
 
@@ -756,49 +768,32 @@ class GaussianTrainer:
 
     def _result(self, with_depth):
         out, n = (C.c_float * 4)(), C.c_int()
-        stream = torch.cuda.current_stream().cuda_stream
-        if with_depth:
-            rc = self.L.psb_trainer_result_depth(self.h, out, C.byref(n), stream)
-        else:
-            rc = self.L.psb_trainer_result(self.h, out, C.byref(n), stream)
+        rc = self.L.psb_trainer_result_depth(self.h, out, C.byref(n), torch.cuda.current_stream().cuda_stream)
         if rc == -4:
             first, count, cur = self._overflow_info()
-            last = getattr(self, "_last", None)
+            last = self._last
             if not (count == 1 and first == cur):
-                if last is not None and last != _PixelsCall(False):
+                if last.advanced:
                     self.model.step_ -= count      # those updates never happened
                     self.iteration -= count
                 raise _lib.PsbError(f"{count} queued call(s) (first: pass {first} of {cur}) overflowed the binning arena and were dropped; the arena has "
                                     "been grown. Collect result() after every step, or render() the view once before queueing steps on it.")
-            if getattr(self, "_last", None) is None:  # a render overflowed the arena: render again
-                cam, o, rad, od, oa = self._last_render
-                self.render(cam, o, rad, check=False, out_depth=od, out_alpha=oa)
-                return self._result(with_depth)
-            if isinstance(self._last, _PixelsCall):
-                if self._last.adam:
-                    self.model.step_ -= 1             # the Adam step of backwardPixels was a no-op
-                    self.iteration -= 1
-                self._last = None
+            if last.advanced:                      # PSB_ERR_RETRY: the call was a no-op
+                self.model.step_ -= 1
+                self.iteration -= 1
+            if last.repeat is None:
+                self._last = _NO_CALL
                 raise _lib.PsbError("the render that backwardPixels back-propagated through overflowed the binning arena, so that call was a "
                                     "no-op; the arena has been grown. Render again (with check=True, or collect result() before computing the "
                                     "loss) and repeat the loss and backwardPixels.")
-            self.model.step_ -= 1                     # PSB_ERR_RETRY: the step was a no-op
-            self.iteration -= 1
-            if isinstance(self._last, _LossCall):
-                self.trainWithLoss(*self._last)
-            else:
-                cam, gt, mask, oc, rad, ds, gd, ld, od, ek = self._last
-                self.trainForOneIteration(cam, gt, mask, oc, rad, ds, gt_depth=gd, lambda_depth=ld, out_depth=od, exposure_id=ek)
+            last.repeat()
             return self._result(with_depth)
-        _lib.check(rc, "psb_trainer_result_depth" if with_depth else "psb_trainer_result")
-        if isinstance(getattr(self, "_last", None), _LossCall):
+        _lib.check(rc, "psb_trainer_result_depth")
+        if self._last.callers_loss:
             # the caller's loss: only its value is known (l1, ssim and depth_l1 are the built-in loss's terms)
             nan = float("nan")
-            loss = float(self._last_loss)
-            return (loss, nan, nan, nan, n.value) if with_depth else (loss, nan, nan, n.value)
-        if with_depth:
-            return out[0], out[1], out[2], out[3], n.value
-        return out[0], out[1], out[2], n.value
+            out = (float(self._last_loss), nan, nan, nan)
+        return (*out[:4 if with_depth else 3], n.value)
 
     # ------------------------------------------------------------------------------------------------------------
     # Host-input front end: what the mapper thread does every iteration — `gt_image = original_image_.cuda()`
@@ -831,10 +826,8 @@ class GaussianTrainer:
             slot["ev"].record(self._copy)
         cam = dict(host_cam, viewmatrix=slot["viewmatrix"], projmatrix=slot["projmatrix"], campos=slot["campos"])
         main.wait_event(slot["ev"])
-        if host_depth is not None:
-            self.trainForOneIteration(cam, slot["gt"], mask, gt_depth=slot["depth"], lambda_depth=lambda_depth)
-        else:
-            self.trainForOneIteration(cam, slot["gt"], mask)
+        depth = slot["depth"] if host_depth is not None else None
+        self.trainForOneIteration(cam, slot["gt"], mask, gt_depth=depth, lambda_depth=lambda_depth if depth is not None else 0.0)
         loss = self.result()[0]                           # waits for the loss scalars only (repeats the step on RETRY)
         slot["done"].record(main)
         self._hslot ^= 1
@@ -849,13 +842,11 @@ class GaussianTrainer:
                  "shard_adam_frest_part")
 
     def set_profiling(self, enable=True):
-        self.L.psb_trainer_set_profiling.argtypes = [C.c_void_p, C.c_int]
         _lib.check(self.L.psb_trainer_set_profiling(self.h, int(enable)), "psb_trainer_set_profiling")
 
     def stage_times(self):
         """ms per stage of the last profiled step (CUDA events on the step's stream)."""
         ms = (C.c_float * 11)()
-        self.L.psb_trainer_stage_times.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_int]
         n = _lib.check(self.L.psb_trainer_stage_times(self.h, ms, 11), "psb_trainer_stage_times")
         names = self.DP_STAGES if n >= 10 else self.STAGES
         return dict(zip(names[:n], [float(x) for x in ms][:n]))
@@ -923,26 +914,7 @@ class DataParallelTrainer(GaussianTrainer):
             self._setup_nccl(pipeline, nslabs)
 
     # ---- p2p -----------------------------------------------------------------------------------------------------------
-    def _bind_dp(self):
-        L, vp = self.L, C.c_void_p
-        if getattr(L, "_dp_bound", False):
-            return
-        L.psb_dp_create.argtypes = [C.POINTER(vp), C.c_int, C.c_int, C.c_int]
-        L.psb_dp_ipc_handle.argtypes = [vp, vp]
-        L.psb_dp_connect.argtypes = [vp, vp]
-        L.psb_dp_params.argtypes = [vp, C.POINTER(vp)]
-        L.psb_dp_step.argtypes = [vp, vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp, vp, vp]
-        L.psb_dp_sync.argtypes = [vp, vp]
-        L.psb_dp_status.argtypes = [vp, vp]
-        L.psb_dp_destroy.argtypes = [vp]
-        for n in ("psb_dp_create", "psb_dp_handle_bytes", "psb_dp_ipc_handle", "psb_dp_connect", "psb_dp_params", "psb_dp_step", "psb_dp_sync",
-                  "psb_dp_status", "psb_dp_destroy"):
-            getattr(L, n).restype = C.c_int
-        L._dp_bound = True
-
     def _setup_p2p(self):
-        from .parallel import SIZES
-        self._bind_dp()
         m, L = self.model, self.L
         P = m.num_points()
         h = C.c_void_p()
@@ -1037,13 +1009,6 @@ class DataParallelTrainer(GaussianTrainer):
             n = len(self.grads.slabs)
             self._ev_k = [torch.cuda.Event() for _ in range(n)]
             self._ev_c = [torch.cuda.Event() for _ in range(n)]
-            vp = C.c_void_p
-            self.L.psb_trainer_backward_begin.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), vp, vp, vp, C.POINTER(_Step), vp, vp, vp]
-            self.L.psb_trainer_backward_slab.argtypes = [vp, C.c_int, C.c_int, C.POINTER(_Model), C.POINTER(_Camera), C.POINTER(_Step), C.c_int, C.c_int,
-                                                         C.POINTER(vp), vp]
-            self.L.psb_adam_flat.argtypes = [C.c_size_t, vp, vp, vp, vp, C.c_float, C.POINTER(_Step), C.c_float, vp]
-            for nme in ("psb_trainer_backward_begin", "psb_trainer_backward_slab", "psb_adam_flat"):
-                getattr(self.L, nme).restype = C.c_int
         else:
             self.grads = GradBuffer(P, model.device)
             self.segs = self.grads.segments
@@ -1068,30 +1033,20 @@ class DataParallelTrainer(GaussianTrainer):
         main = torch.cuda.current_stream()
         stream = main.cuda_stream
         P = m.num_points()
-        args = (self.h, P, 16, C.byref(cm), C.byref(cc), self.background.data_ptr(), gt_image.data_ptr(),
-                mask.data_ptr() if mask is not None else None, C.byref(cs), out_color.data_ptr() if out_color is not None else None,
-                radii.data_ptr() if radii is not None else None)
+        args = self._call_args(m, cm, cc, cs, gt_image, mask, out_color, radii)
+        cdepth = C.byref(depth) if depth is not None else None
         if self.mode == "p2p":
-            if depth is None:
-                _lib.check(self.L.psb_dp_step(self.h, self.dp, *args[1:], stream), "psb_dp_step")
-            else:
-                _lib.check(self.L.psb_dp_step_depth(self.h, self.dp, *args[1:], C.byref(depth), stream), "psb_dp_step_depth")
+            _lib.check(self.L.psb_dp_step_depth(self.h, self.dp, *args[1:], cdepth, stream), "psb_dp_step_depth")
         elif not self.pipeline:
             assert self.grads.P == P, "gradient buffer was built for a different model size: call rebuild() after densify/prune"
             ptrs = (C.c_void_p * 6)(*[s.data_ptr() for s in self.segs])
-            if depth is None:
-                _lib.check(self.L.psb_trainer_backward(*args, ptrs, stream), "psb_trainer_backward")
-            else:
-                _lib.check(self.L.psb_trainer_backward_depth(*args, ptrs, C.byref(depth), stream), "psb_trainer_backward_depth")
+            _lib.check(self.L.psb_trainer_backward_depth(*args, ptrs, cdepth, stream), "psb_trainer_backward_depth")
             scale = self.grads.all_reduce(self.group)   # ONE collective per step: 59 floats per Gaussian
             _lib.check(self.L.psb_adam_update(P, 16, C.byref(cm), ptrs, C.byref(cs), scale, stream), "psb_adam_update")
         else:
             from .parallel import SIZES
             assert self.grads.P == P, "gradient buffer was built for a different model size: call rebuild() after densify/prune"
-            if depth is None:
-                _lib.check(self.L.psb_trainer_backward_begin(*args, stream), "psb_trainer_backward_begin")
-            else:
-                _lib.check(self.L.psb_trainer_backward_begin_depth(*args, C.byref(depth), stream), "psb_trainer_backward_begin_depth")
+            _lib.check(self.L.psb_trainer_backward_begin_depth(*args, cdepth, stream), "psb_trainer_backward_begin_depth")
             scale = 1.0 / self.world
             for s, (first, count) in enumerate(self.grads.slabs):
                 ptrs = (C.c_void_p * 6)(*self.grads.kernel_pointers(s))
@@ -1113,7 +1068,6 @@ class DataParallelTrainer(GaussianTrainer):
                                                     C.byref(cs), scale, stream), "psb_adam_flat")
         m.step_ += 1
         m.invalidateAdamLive()   # these steps write moments without maintaining the live bytes (and p2p: only on the owner rank)
-        self._last = (cam, gt_image, mask, out_color, radii, densify_stats, gt_depth, lambda_depth, out_depth)
 
     def result(self):
         """-> (loss, l1, ssim, num_rendered) of this rank's view. A view whose binning arena overflowed contributed a zero
@@ -1124,14 +1078,13 @@ class DataParallelTrainer(GaussianTrainer):
 
     def _result(self, with_depth):
         out, n = (C.c_float * 4)(), C.c_int()
-        stream = torch.cuda.current_stream().cuda_stream
-        rc = self.L.psb_trainer_result_depth(self.h, out, C.byref(n), stream) if with_depth else self.L.psb_trainer_result(self.h, out, C.byref(n), stream)
+        rc = self.L.psb_trainer_result_depth(self.h, out, C.byref(n), torch.cuda.current_stream().cuda_stream)
         if rc == -4:
             self.dropped_views += 1
-            nan = float("nan")
-            return (nan, nan, nan, nan, n.value) if with_depth else (nan, nan, nan, n.value)
-        _lib.check(rc, "psb_trainer_result_depth" if with_depth else "psb_trainer_result")
-        return (out[0], out[1], out[2], out[3], n.value) if with_depth else (out[0], out[1], out[2], n.value)
+            out = (float("nan"),) * 4
+        else:
+            _lib.check(rc, "psb_trainer_result_depth")
+        return (*out[:4 if with_depth else 3], n.value)
 
     def trainWithLoss(self, *args, **kwargs):
         raise NotImplementedError("DataParallelTrainer.trainWithLoss: a caller's loss is not wired into the data-parallel steps (the "

@@ -1,6 +1,5 @@
 """CPU: the deterministic-mode switch of the trainer context — declared, exported, validated before any CUDA call, and followed by
 the Python trainers' deterministic=None."""
-import ctypes as C
 import os
 
 import pytest
@@ -18,9 +17,8 @@ def test_symbol_declared_and_exported():
 
 
 def test_null_context_is_an_argument_error():
-    L = _lib.lib()
-    L.psb_trainer_set_deterministic.argtypes = [C.c_void_p, C.c_int]
-    L.psb_trainer_set_deterministic.restype = C.c_int
+    from photo_slam_b200 import trainer
+    L = trainer._bind()
     assert L.psb_trainer_set_deterministic(None, 1) == -1
     assert L.psb_trainer_set_deterministic(None, 0) == -1
 

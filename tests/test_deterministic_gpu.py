@@ -161,10 +161,7 @@ def _slab_grads(tr, m, c, gt, gd=None, nslabs=3):
     """psb_trainer_backward_begin_depth + one psb_trainer_backward_slab per slab, written into the flat layout of GradBuffer."""
     from photo_slam_b200 import _lib, trainer
     from photo_slam_b200.parallel import GradBuffer, SlabGradBuffer
-    L, vp = tr.L, C.c_void_p
-    L.psb_trainer_backward_slab.argtypes = [vp, C.c_int, C.c_int, C.POINTER(trainer._Model), C.POINTER(trainer._Camera), C.POINTER(trainer._Step),
-                                            C.c_int, C.c_int, C.POINTER(vp), vp]
-    L.psb_trainer_backward_slab.restype = C.c_int
+    L = tr.L
     P = m.num_points()
     buf = GradBuffer(P, m.device)
     stream = torch.cuda.current_stream().cuda_stream

@@ -8,10 +8,7 @@ from photo_slam_b200 import _lib
 
 
 def _query():
-    fn = _lib.lib().psb_debug_render_bwd_occupancy
-    fn.restype = C.c_int
-    fn.argtypes = [C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    return fn
+    return _lib.lib().psb_debug_render_bwd_occupancy
 
 
 def test_unknown_variant_is_rejected():

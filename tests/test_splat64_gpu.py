@@ -339,8 +339,6 @@ def _debug_state(tr, W, H, dev):
     """psb_trainer_debug_state: per pixel the Gaussian index of the last blended splat (-1 = none) and the final transmittance"""
     import ctypes as C
     from photo_slam_b200 import _lib
-    tr.L.psb_trainer_debug_state.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_void_p]
-    tr.L.psb_trainer_debug_state.restype = C.c_int
     last = torch.empty(W * H, dtype=torch.int32, device=dev)
     fT = torch.empty(W * H, dtype=torch.float32, device=dev)
     _lib.check(tr.L.psb_trainer_debug_state(tr.h, W, H, last.data_ptr(), fT.data_ptr(), None, torch.cuda.current_stream().cuda_stream),

@@ -57,8 +57,6 @@ def _camera(camname, wh, dev):
 
 
 def _debug_state(tr, W, H, dev):
-    tr.L.psb_trainer_debug_state.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_void_p]
-    tr.L.psb_trainer_debug_state.restype = C.c_int
     last = torch.empty(W * H, dtype=torch.int32, device=dev)
     fT = torch.empty(W * H, dtype=torch.float32, device=dev)
     n = C.c_int()

@@ -17,10 +17,7 @@ NAMES = ["render_bwd_kernel<%s, %s, %s>" % tuple("true" if v >> b & 1 else "fals
 
 def main():
     import torch
-    L = _lib.lib()
-    fn = L.psb_debug_render_bwd_occupancy
-    fn.restype = C.c_int
-    fn.argtypes = [C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    fn = _lib.lib().psb_debug_render_bwd_occupancy
     out = {"device": torch.cuda.get_device_name(0), "threads_per_block": 128, "kernels": {}}
     for v, name in enumerate(NAMES):
         blocks, smem, regs = C.c_int(), C.c_int(), C.c_int()
