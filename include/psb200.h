@@ -245,7 +245,8 @@ typedef struct psb_model {
 	                             reads and updates nothing of a row whose byte is 0 and that no gradient reaches (Adam is an exact no-op on
 	                             it), and sets the byte of every row it updates with a non-zero gradient. Anything else that writes moments
 	                             must leave the contract intact or be followed by psb_adam_live_rebuild. NULL: the moments themselves are
-	                             read to find such rows. Every other entry point ignores the field. */
+	                             read to find such rows. psb_relocate clears the bytes of the rows whose moments it zeroes. Every other entry point ignores
+	                             the field. */
 } psb_model;
 
 typedef struct psb_camera {
@@ -551,6 +552,72 @@ int psb_insert_points(int P, const psb_model* src, const psb_model* dst, int n, 
                       const float* dist2, int iteration, void* stream);
 /* GaussianModel::resetOpacity (src/gaussian_model.cpp:556-565, incl. its no-op clamp) + zeroed opacity moments, in place. */
 int psb_reset_opacity(int P, float* opacity, float* exp_avg, float* exp_avg_sq, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Bounded-budget densification: relocation of dead Gaussians and growth to a cap (3DGS-MCMC, Kheradmand et al., NeurIPS 2024; the
+ * semantics of gsplat's MCMCStrategy relocate / sample_add). The reference has no counterpart. With o = sigmoid(opacity) and
+ * s = exp(scaling), a row is DEAD when o <= min_opacity and ALIVE otherwise.
+ *   Sampling     n draws with replacement from a candidate set with probability proportional to o: inclusive prefix sum of o over the
+ *                candidates in row order, in double and in a fixed order; draw j takes u_j in [0, 1) and picks the first candidate
+ *                whose cumulative sum exceeds (double)u_j * total (binary search). u_j = uniforms[j] when given, else the first word
+ *                w of Philox4x32-10(counter = (j, sub, offset low, offset high), key = (seed low, seed high)) as
+ *                min(((float)w + 0.5f) * 2^-32, 1 - 2^-24), sub = 1 in psb_relocate and 2 in psb_grow (the normals of the densify split
+ *                and of the position noise use 0). Counter-based: every data-parallel replica draws the same rows.
+ *   Multiplicity N_i = min(1 + number of draws that picked row i, 51).
+ *   Correction   of a picked row (the paper's Eq. 9): o' = 1 - (1 - o)^(1/N), D = sum_{a=1..N} sum_{k=0..a-1} C(a-1,k) (-1)^k
+ *                o'^(k+1) / sqrt(k+1), s' = s o / D on all three axes, o' clamped to [min_opacity, 1 - 1e-7]; stored as logit(o'),
+ *                log(s') (a logit at the lower clamp is raised by a few ulps until sigmoid(logit) > min_opacity: a corrected row is
+ *                alive). N copies of (o', s') have the alpha of the original at its centre. All 118 moments of a picked row are zeroed.
+ * psb_relocate (in place, P unchanged): candidates = the alive rows, n = the number of dead rows. Dead row number j (in row order)
+ *   becomes a copy of the corrected source of draw j (all 59 parameters) with zero moments, zero max_radii2D / xyz_gradient_accum /
+ *   denom (those given) and exist_since_iter = cfg.iteration (if given). (gsplat leaves the overwritten rows' stale moments in place;
+ *   here they are zeroed, which the adam_live contract wants anyway.) model->adam_live, when given, is cleared for the picked and the
+ *   overwritten rows, so the contract holds afterwards. No dead row or no alive row: nothing is written. counts_host (host, may be
+ *   NULL) receives {rows overwritten, dead rows}; only then does the call synchronise the stream — with NULL it is asynchronous.
+ * psb_grow (out of place): dst = the P rows of src followed by n = P_new - P rows (0 <= n <= P; the caller picks
+ *   P_new = min(cap, floor(factor P))). n draws over ALL rows; picked rows are corrected in dst; new row P + j is a copy of the
+ *   corrected source of draw j with zero moments, zero statistics and exist_since_iter = cfg.iteration. The old rows keep their
+ *   statistics, exist_since_iter and (unless picked) moments. n == 0 copies src. dst->adam_live is ignored. Asynchronous.
+ * workspace: psb_relocate_workspace_bytes(P) device bytes, 8-byte aligned. uniforms: device [n] floats in [0, 1), or NULL.
+ * PSB_ERR_ARG, before any CUDA call, for P < 0, P_new outside [P, 2 P], min_opacity outside [0, 1), and a missing model tensor or
+ * workspace.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct psb_relocate_cfg {
+	float min_opacity;       /* dead at or below (3DGS-MCMC: 0.005) */
+	int iteration;           /* exist_since_iter of the rows written */
+	unsigned long long seed, offset;
+} psb_relocate_cfg;
+size_t psb_relocate_workspace_bytes(int P);
+int psb_relocate(int P, const psb_model* model, const psb_relocate_cfg* cfg, void* workspace, const float* uniforms, int* counts_host,
+                 void* stream);
+int psb_grow(int P, const psb_model* src, const psb_model* dst, int P_new, const psb_relocate_cfg* cfg, void* workspace,
+             const float* uniforms, void* stream);
+
+/* Position noise of 3DGS-MCMC behind an optimizer step (gsplat inject_noise_to_position), on the rows of the context's latest pass:
+ *   xyz += Sigma xi * (lr_xyz * noise_lr) * g(o),  Sigma = R(q) diag(s^2) R(q)^T (q the normalised quaternion),
+ *   g(o) = 1 / (1 + exp(-100 ((1 - o) - 0.995))):  ~1 for dead rows, < 1e-4 above o = 0.1, so only nearly dead Gaussians move.
+ * xi ~ N(0, I_3): Box-Muller on the four words w0..w3 of Philox4x32-10(counter = (row, 0, step low, step high), key = seed) with
+ * u_k = ((float)w_k + 0.5f) 2^-32: xi = (r0 cos(2 pi u1), r0 sin(2 pi u1), r1 cos(2 pi u3)), r0 = sqrt(-2 log min(u0, 1 - 2^-24)),
+ * r1 likewise from u2 (the draw of the densify split). Counter-based and free of atomics: bit-identical from run to run.
+ * It does nothing when the latest pass overflowed the binning arena (like every kernel of that step), so the repeated step adds the
+ * noise exactly once. visible_only != 0 restricts it to the rows that pass saw (radius > 0): a region no recent keyframe sees gets no
+ * gradient that could pull a row back, and noise there would be a random walk of the unobserved map; 0 is gsplat's behaviour.
+ * PSB_ERR_ARG when the context has run no pass of P rows, for a missing tensor, and for a negative or non-finite lr_xyz / noise_lr.
+ * Asynchronous on `stream`. */
+int psb_trainer_inject_noise(psb_trainer* t, int P, const psb_model* model, float lr_xyz, float noise_lr, unsigned long long seed,
+                             unsigned long long step, int visible_only, void* stream);
+
+/* Opacity and scale regularisers of 3DGS-MCMC on the per-Gaussian stage: L += lambda_opacity mean sigmoid(opacity) + lambda_scale mean
+ * exp(scaling) (means over the P rows; the scale term sums the three axes of a row, so gsplat's mean over all 3 P values is
+ * lambda_scale / 3 here; the paper uses 0.01 for both). In raw-parameter terms
+ * g_opacity += (lambda_opacity / P) o (1 - o) and g_scaling[c] += (lambda_scale / P) s_c, added where the kernel forms the raw
+ * gradients, before Adam or the gradient store. They apply to THE ROWS THE PASS UPDATES (rows whose screen-space sums are non-zero),
+ * not to all P rows as in gsplat: the fused step touches no other row, and decaying whatever this keyframe does not see would be wrong
+ * for a SLAM map anyway (Adam turns a constant-sign gradient into a full step). Read when a pass starts, like anti-aliasing; both 0
+ * (the default) runs exactly the kernels of a context that never called this. Covers psb_trainer_step*, psb_trainer_backward*
+ * (the _begin / _slab pair included) and psb_trainer_backward_pixels; not psb_dp_step*, which ignore it. The loss scalars of
+ * psb_trainer_result stay the image terms. PSB_ERR_ARG for a NULL context and a negative or non-finite lambda. */
+int psb_trainer_set_regularizers(psb_trainer* t, float lambda_opacity, float lambda_scale);
 
 /* ------------------------------------------------------------------------------------------------
  * Point-cloud helpers exported by the same shared objects in the reference.

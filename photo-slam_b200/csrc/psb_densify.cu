@@ -308,6 +308,329 @@ __global__ void insert_fill_kernel(int P, int n, const float* __restrict__ point
 	if (t.dexist) t.dexist[d] = iteration;
 }
 
+// ------------------------------------------------------------------------------------------------------------------------
+// Bounded-budget densification (3DGS-MCMC, Kheradmand et al., NeurIPS 2024; gsplat's MCMCStrategy — no counterpart in the reference):
+// psb_relocate moves dead rows onto live ones, psb_grow appends copies of sampled rows. Both are
+//   reloc_weight_kernel   per block of 128 rows: weight o = sigmoid(opacity) of the candidates (0 for the others), inclusive prefix sum
+//                         inside the block in double and in a fixed order, the block's sum and its number of dead rows;
+//   reloc_scan_kernel     one block: exclusive scan of the block sums (double) and of the dead counts -> the total weight, the dead count;
+//   reloc_draw_kernel     one thread per draw: u in [0, 1) -> the first row whose cumulative weight exceeds u * total (binary search),
+//                         integer histogram of the picks (atomicAdd on ints: order-independent);
+//   reloc_correct_kernel  per block of 128 rows: every picked row gets (o', s') for its multiplicity and zero moments, in place;
+//   reloc_copy_kernel     per block of 128 targets: target row <- its (corrected) source row, zero moments and statistics.
+// No float atomics anywhere: the result is bit-identical from run to run and on every data-parallel replica.
+// ------------------------------------------------------------------------------------------------------------------------
+constexpr int RL_MAXN = 51;   // multiplicities are clamped here (gsplat's n_max)
+
+// C(n, k) for n, k < 51, exact in double (C(50, 25) < 2^53)
+struct BinomTable {
+	double c[RL_MAXN][RL_MAXN];
+	constexpr BinomTable() : c()
+	{
+		for (int n = 0; n < RL_MAXN; n++)
+			for (int k = 0; k < RL_MAXN; k++) c[n][k] = k == 0 ? 1.0 : (n == 0 || k > n ? 0.0 : c[n - 1][k - 1] + c[n - 1][k]);
+	}
+};
+__constant__ BinomTable c_binom = BinomTable();
+
+// A row of opacity o and scale s that stands for N co-located copies (the paper's Eq. 9, gsplat compute_relocation):
+//   o' = 1 - (1 - o)^(1/N);  D = sum_{a=1..N} sum_{k=0..a-1} C(a-1, k) (-1)^k o'^(k+1) / sqrt(k+1);  s' = s o / D.
+// Returns o' clamped to [min_opacity, 1 - 1e-7] and the scale factor o / D of the unclamped o'. The alternating sum cancels up to 1e4
+// of its terms at N = 51, so it is formed in double (a few hundred picked rows per thousand: not on any hot path).
+__device__ __forceinline__ void relocation(float o, int N, float min_opacity, float& o_new, float& scale_factor)
+{
+	const double od = (double)o;
+	const double on = 1.0 - pow(1.0 - od, 1.0 / (double)N);
+	double D = 0.0;
+	for (int a = 1; a <= N; a++) {
+		double pw = on, sgn = 1.0;
+		for (int k = 0; k < a; k++) {
+			D += c_binom.c[a - 1][k] * sgn * pw * rsqrt((double)(k + 1));
+			pw *= on; sgn = -sgn;
+		}
+	}
+	scale_factor = (float)(od / D);
+	o_new = fminf(fmaxf((float)on, min_opacity), 1.0f - 1e-7f);
+}
+
+struct RelocTotals {
+	double total;       // sum of the candidates' weights
+	uint32_t n_dead;    // rows with sigmoid(opacity) <= min_opacity
+	uint32_t pad;
+};
+
+// flags[i]: bit 0 = dead. all_rows: every row is a candidate (grow), else the alive rows (relocate)
+__global__ void __launch_bounds__(DN_TB) reloc_weight_kernel(int P, const float* __restrict__ opacity, float min_opacity, int all_rows,
+                                                           uint8_t* __restrict__ flags, double* __restrict__ cum, int* __restrict__ mult,
+                                                           double* __restrict__ block_sum, uint32_t* __restrict__ block_dead)
+{
+	__shared__ double s_w[DN_TB / 32];
+	__shared__ uint32_t s_d[DN_TB / 32];
+	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	const int i = blockIdx.x * DN_TB + tid;
+	bool dead = false;
+	double w = 0.0;
+	if (i < P) {
+		const float o = sigmoidf(opacity[i]);
+		dead = o <= min_opacity;
+		if (all_rows || !dead) w = (double)o;
+		flags[i] = dead ? 1 : 0;
+		mult[i] = 0;
+	}
+	double inc = w;
+#pragma unroll
+	for (int d = 1; d < 32; d <<= 1) {
+		const double u = __shfl_up_sync(0xffffffffu, inc, d);
+		if (lane >= d) inc += u;
+	}
+	const uint32_t b = __ballot_sync(0xffffffffu, dead);
+	if (lane == 31) s_w[warp] = inc;
+	if (lane == 0) s_d[warp] = __popc(b);
+	__syncthreads();
+	for (int k = 0; k < warp; k++) inc += s_w[k];
+	if (i < P) cum[i] = inc;
+	if (tid == DN_TB - 1) {
+		block_sum[blockIdx.x] = inc;
+		uint32_t nd = 0;
+		for (int k = 0; k < DN_TB / 32; k++) nd += s_d[k];
+		block_dead[blockIdx.x] = nd;
+	}
+}
+
+__global__ void __launch_bounds__(1024) reloc_scan_kernel(int nblocks, const double* __restrict__ block_sum, const uint32_t* __restrict__ block_dead,
+                                                        double* __restrict__ sum_off, uint32_t* __restrict__ dead_off, RelocTotals* __restrict__ totals)
+{
+	__shared__ double s_w[32];
+	__shared__ uint32_t s_d[32];
+	__shared__ double s_run;
+	__shared__ uint32_t s_rund;
+	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	if (tid == 0) { s_run = 0.0; s_rund = 0u; }
+	__syncthreads();
+	for (int b0 = 0; b0 < nblocks; b0 += 1024) {
+		const int b = b0 + tid;
+		const double w = b < nblocks ? block_sum[b] : 0.0;
+		const uint32_t d = b < nblocks ? block_dead[b] : 0u;
+		double inc = w;
+		uint32_t incd = d;
+#pragma unroll
+		for (int o = 1; o < 32; o <<= 1) {
+			const double u = __shfl_up_sync(0xffffffffu, inc, o);
+			const uint32_t ud = __shfl_up_sync(0xffffffffu, incd, o);
+			if (lane >= o) { inc += u; incd += ud; }
+		}
+		if (lane == 31) { s_w[warp] = inc; s_d[warp] = incd; }
+		__syncthreads();
+		double base = s_run;
+		uint32_t based = s_rund;
+		for (int k = 0; k < warp; k++) { base += s_w[k]; based += s_d[k]; }
+		if (b < nblocks) { sum_off[b] = base + inc - w; dead_off[b] = based + incd - d; }
+		__syncthreads();
+		if (tid == 1023) { s_run = base + inc; s_rund = based + incd; }
+		__syncthreads();
+	}
+	if (tid == 0) { totals->total = s_run; totals->n_dead = s_rund; totals->pad = 0u; }
+}
+
+// u of draw j: injected, or the first word of Philox(counter = (j, sub, offset), key = seed) as (word + 0.5) 2^-32 in float, at most
+// 1 - 2^-24. sub = 1 (relocate) or 2 (grow) keeps the two draws of one refinement, and the normals of normal3 (sub 0), on streams of their own.
+__device__ __forceinline__ float uniform1(const float* __restrict__ uniforms, unsigned long long seed, unsigned long long offset, uint32_t sub, uint32_t j)
+{
+	if (uniforms) return uniforms[j];
+	const uint4 r = philox4x32_10(make_uint4(j, sub, (uint32_t)offset, (uint32_t)(offset >> 32)), make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
+	return fminf(((float)r.x + 0.5f) * 2.3283064365386963e-10f, 0.99999994f);
+}
+
+// n_host < 0: one draw per dead row (totals->n_dead)
+__global__ void __launch_bounds__(256) reloc_draw_kernel(int P, int n_host, const RelocTotals* __restrict__ totals, const double* __restrict__ cum,
+                                                       const double* __restrict__ sum_off, const float* __restrict__ uniforms, unsigned long long seed,
+                                                       unsigned long long offset, uint32_t sub, int* __restrict__ pick, int* __restrict__ mult)
+{
+	const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+	const uint32_t n = n_host < 0 ? totals->n_dead : (uint32_t)n_host;
+	const double total = totals->total;
+	if (j >= n || (n_host < 0 && !(total > 0.0))) return;   // relocate without an alive row: nothing to draw from
+	const float u = uniform1(uniforms, seed, offset, sub, j);
+	const double target = (double)u * total;
+	int lo = 0, hi = P - 1;   // first row whose cumulative weight exceeds the target (the last row's equals the total > target)
+	if (!(total > 0.0)) lo = hi = min((int)(u * (float)P), P - 1);   // grow over rows whose opacities all underflowed: uniform picks
+	while (lo < hi) {
+		const int mid = (lo + hi) >> 1;
+		if (sum_off[mid / DN_TB] + cum[mid] > target) hi = mid; else lo = mid + 1;
+	}
+	pick[j] = lo;
+	atomicAdd(&mult[lo], 1);
+}
+
+struct RelocTensors {
+	float* p[6]; float* m[6]; float* v[6];
+	float* stat[3];            // max_radii2D, xyz_gradient_accum, denom (any may be null)
+	int* exist;                // or null
+	unsigned char* live;       // psb_model.adam_live or null
+};
+
+__global__ void __launch_bounds__(DN_TB) reloc_correct_kernel(int P, RelocTensors t, const int* __restrict__ mult, float min_opacity)
+{
+	__shared__ int s_picked[DN_TB];
+	const int tid = threadIdx.x;
+	const int base = blockIdx.x * DN_TB;
+	const int rows = min(DN_TB, P - base);
+	const int i = base + tid;
+	const int cnt = i < P ? mult[i] : 0;
+	s_picked[tid] = cnt;
+	if (cnt > 0) {
+		float o_new, f;
+		relocation(sigmoidf(t.p[3][i]), min(cnt + 1, RL_MAXN), min_opacity, o_new, f);
+		// a corrected row is alive: where o' was clamped to min_opacity, the stored logit is nudged until its sigmoid clears the threshold
+		float lo = logf(o_new / (1.0f - o_new));
+		for (int k = 0; k < 16 && !(sigmoidf(lo) > min_opacity * 1.000001f); k++) lo = nextafterf(lo, 100.f);
+		t.p[3][i] = lo;
+#pragma unroll
+		for (int c = 0; c < 3; c++) t.p[4][3 * i + c] = logf(expf(t.p[4][3 * i + c]) * f);
+		if (t.live) t.live[i] = 0;
+	}
+	__syncthreads();
+#pragma unroll
+	for (int ti = 0; ti < 6; ti++) {
+		const int k = dn_row(ti);
+		float* __restrict__ dm = t.m[ti] + (size_t)base * k;
+		float* __restrict__ dv = t.v[ti] + (size_t)base * k;
+		for (int e = tid; e < rows * k; e += DN_TB)
+			if (s_picked[e / k] > 0) { dm[e] = 0.f; dv[e] = 0.f; }
+	}
+}
+
+// Targets of block b are rows tbase + [b * 128, ...). flags != null (relocate): row i is a target when it is dead, its source is the
+// pick of its rank among the dead rows; flags == null (grow): target n_old + j is draw j's.
+__global__ void __launch_bounds__(DN_TB) reloc_copy_kernel(int n_targets, int tbase, RelocTensors t, const uint8_t* __restrict__ flags,
+                                                         const uint32_t* __restrict__ dead_off, const RelocTotals* __restrict__ totals,
+                                                         const int* __restrict__ pick, int iteration)
+{
+	__shared__ int s_src[DN_TB];
+	__shared__ uint32_t s_wcnt[DN_TB / 32];
+	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	const int base = blockIdx.x * DN_TB;
+	const int rows = min(DN_TB, n_targets - base);
+	const int j = base + tid;
+	const bool go = !flags || totals->total > 0.0;
+	int src = -1;
+	if (flags) {
+		const bool dead = j < n_targets && flags[j] != 0;
+		const uint32_t b = __ballot_sync(0xffffffffu, dead);
+		if (lane == 0) s_wcnt[warp] = __popc(b);
+		__syncthreads();
+		uint32_t rank = dead_off[blockIdx.x] + __popc(b & ((1u << lane) - 1u));
+		for (int w = 0; w < warp; w++) rank += s_wcnt[w];
+		if (dead && go) src = pick[rank];
+	} else if (j < n_targets && go) {
+		src = pick[j];
+	}
+	s_src[tid] = src;
+	if (src >= 0) {
+		const size_t d = (size_t)tbase + j;
+#pragma unroll
+		for (int q = 0; q < 3; q++) if (t.stat[q]) t.stat[q][d] = 0.f;
+		if (t.exist) t.exist[d] = iteration;
+		if (t.live) t.live[d] = 0;
+	}
+	__syncthreads();
+#pragma unroll
+	for (int ti = 0; ti < 6; ti++) {
+		const int k = dn_row(ti);
+		const size_t o = ((size_t)tbase + base) * k;
+		for (int e = tid; e < rows * k; e += DN_TB) {
+			const int r = e / k, s = s_src[r];
+			if (s < 0) continue;
+			t.p[ti][o + e] = t.p[ti][(size_t)s * k + (e - r * k)];
+			t.m[ti][o + e] = 0.f; t.v[ti][o + e] = 0.f;
+		}
+	}
+}
+
+// Position noise of 3DGS-MCMC (gsplat inject_noise_to_position): xyz += Sigma xi lr g(o), Sigma = R(q) diag(exp(scaling)^2) R(q)^T with q
+// the normalised quaternion, g(o) = 1 / (1 + exp(-100 ((1 - o) - 0.995))), xi = normal3(seed, step, row). One thread per row, no atomics.
+// Nothing moves when the pass overflowed the binning arena; visible_only: only rows the pass saw (tile_info.z != 0).
+__global__ void __launch_bounds__(256) position_noise_kernel(int P, float* __restrict__ xyz, const float* __restrict__ opacity, const float* __restrict__ scaling,
+                                                           const float* __restrict__ rotation, float lr, unsigned long long seed, unsigned long long step,
+                                                           const uint4* __restrict__ tile_info, const uint32_t* __restrict__ counters, uint32_t capacity)
+{
+	if (counters[0] > capacity) return;
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= P || (tile_info && tile_info[i].z == 0)) return;
+	const float o = sigmoidf(opacity[i]);
+	const float g = 1.0f / (1.0f + expf(-100.0f * ((1.0f - o) - 0.995f)));
+	const float4 qr = reinterpret_cast<const float4*>(rotation)[i];
+	const float n = fmaxf(sqrtf(qr.x * qr.x + qr.y * qr.y + qr.z * qr.z + qr.w * qr.w), 1e-12f);
+	const float r = qr.x / n, x = qr.y / n, y = qr.z / n, z = qr.w / n;
+	const float R00 = 1.f - 2.f * (y * y + z * z), R01 = 2.f * (x * y - r * z), R02 = 2.f * (x * z + r * y);
+	const float R10 = 2.f * (x * y + r * z), R11 = 1.f - 2.f * (x * x + z * z), R12 = 2.f * (y * z - r * x);
+	const float R20 = 2.f * (x * z - r * y), R21 = 2.f * (y * z + r * x), R22 = 1.f - 2.f * (x * x + y * y);
+	const float s0 = expf(scaling[3 * i]), s1 = expf(scaling[3 * i + 1]), s2 = expf(scaling[3 * i + 2]);
+	const float3 xi = normal3(seed, step, (uint32_t)i);
+	// Sigma xi = R (s^2 * (R^T xi))
+	const float a = (R00 * xi.x + R10 * xi.y + R20 * xi.z) * s0 * s0;
+	const float b = (R01 * xi.x + R11 * xi.y + R21 * xi.z) * s1 * s1;
+	const float c = (R02 * xi.x + R12 * xi.y + R22 * xi.z) * s2 * s2;
+	const float k = lr * g;
+	xyz[3 * i] += (R00 * a + R01 * b + R02 * c) * k;
+	xyz[3 * i + 1] += (R10 * a + R11 * b + R12 * c) * k;
+	xyz[3 * i + 2] += (R20 * a + R21 * b + R22 * c) * k;
+}
+
+struct RelocWorkspace {
+	uint8_t* flags; double* cum; int* mult; int* pick; double* block_sum; double* sum_off; uint32_t* block_dead; uint32_t* dead_off; RelocTotals* totals;
+};
+size_t reloc_ws_bytes(int P)
+{
+	const size_t nb = ((size_t)P + DN_TB - 1) / DN_TB, p = (size_t)P;
+	return align_up(p, 256) + align_up(p * 8, 256) + 2 * align_up(p * 4, 256) + 2 * align_up(nb * 8, 256) + 2 * align_up(nb * 4, 256) + 256;
+}
+RelocWorkspace reloc_ws_carve(void* w, int P)
+{
+	const size_t nb = ((size_t)P + DN_TB - 1) / DN_TB, p = (size_t)P;
+	char* c = static_cast<char*>(w);
+	RelocWorkspace s;
+	s.cum = reinterpret_cast<double*>(c); c += align_up(p * 8, 256);
+	s.block_sum = reinterpret_cast<double*>(c); c += align_up(nb * 8, 256);
+	s.sum_off = reinterpret_cast<double*>(c); c += align_up(nb * 8, 256);
+	s.totals = reinterpret_cast<RelocTotals*>(c); c += 256;
+	s.mult = reinterpret_cast<int*>(c); c += align_up(p * 4, 256);
+	s.pick = reinterpret_cast<int*>(c); c += align_up(p * 4, 256);
+	s.block_dead = reinterpret_cast<uint32_t*>(c); c += align_up(nb * 4, 256);
+	s.dead_off = reinterpret_cast<uint32_t*>(c); c += align_up(nb * 4, 256);
+	s.flags = reinterpret_cast<uint8_t*>(c);
+	return s;
+}
+// the tensors of a model that relocate / grow write; false when one of the 18 parameter / moment tensors is missing
+bool reloc_tensors(const psb_model* m, RelocTensors& t)
+{
+	for (int i = 0; i < 6; i++) {
+		if (!m->param[i] || !m->exp_avg[i] || !m->exp_avg_sq[i]) return false;
+		t.p[i] = m->param[i]; t.m[i] = m->exp_avg[i]; t.v[i] = m->exp_avg_sq[i];
+	}
+	t.stat[0] = m->max_radii2D; t.stat[1] = m->xyz_gradient_accum; t.stat[2] = m->denom;
+	t.exist = m->exist_since_iter;
+	t.live = m->adam_live;
+	return true;
+}
+bool reloc_cfg_ok(const psb_relocate_cfg* c)
+{
+	return c && c->min_opacity >= 0.f && c->min_opacity < 1.f;   // (also false for a NaN)
+}
+// weights, scan and n draws (n < 0: one per dead row) over the P rows of `opacity` into the workspace
+int reloc_sample(int P, const float* opacity, const psb_relocate_cfg* cfg, int all_rows, int n, const RelocWorkspace& w, const float* uniforms,
+                 cudaStream_t stream)
+{
+	const int nb = (P + DN_TB - 1) / DN_TB;
+	reloc_weight_kernel<<<nb, DN_TB, 0, stream>>>(P, opacity, cfg->min_opacity, all_rows, w.flags, w.cum, w.mult, w.block_sum, w.block_dead);
+	PSB_LAUNCH_OK();
+	reloc_scan_kernel<<<1, 1024, 0, stream>>>(nb, w.block_sum, w.block_dead, w.sum_off, w.dead_off, w.totals);
+	PSB_LAUNCH_OK();
+	reloc_draw_kernel<<<((n < 0 ? P : n) + 255) / 256, 256, 0, stream>>>(P, n, w.totals, w.cum, w.sum_off, uniforms, cfg->seed, cfg->offset, all_rows ? 2u : 1u, w.pick, w.mult);
+	PSB_LAUNCH_OK();
+	return 0;
+}
+
 struct Workspace {
 	uint8_t* flags; uint32_t* counts; uint32_t* offsets; uint32_t* totals;
 };
@@ -338,11 +661,86 @@ DensifyCfg to_cfg(const psb_densify_cfg* c)
 }
 
 }  // namespace
+
+int launch_position_noise(int P, float* xyz, const float* opacity, const float* scaling, const float* rotation, float lr, unsigned long long seed,
+                          unsigned long long step, const uint4* tile_info, const uint32_t* counters, uint32_t capacity, cudaStream_t stream)
+{
+	if (P <= 0) return 0;
+	position_noise_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, xyz, opacity, scaling, rotation, lr, seed, step, tile_info, counters, capacity);
+	PSB_LAUNCH_OK();
+	return 0;
+}
+
 }  // namespace psb
 
 using namespace psb;
 
 extern "C" {
+
+size_t psb_relocate_workspace_bytes(int P) { return P > 0 ? reloc_ws_bytes(P) : 256; }
+
+int psb_relocate(int P, const psb_model* model, const psb_relocate_cfg* cfg, void* workspace, const float* uniforms, int* counts_host, void* stream_)
+{
+	cudaStream_t stream = (cudaStream_t)stream_;
+	RelocTensors t;
+	if (P < 0 || !reloc_cfg_ok(cfg) || (P > 0 && (!model || !workspace || !reloc_tensors(model, t)))) {
+		set_error_msg("psb_relocate: bad argument (P >= 0, min_opacity in [0, 1), a model with parameters and moments, and a workspace required)");
+		return PSB_ERR_ARG;
+	}
+	if (P > 0 && (reinterpret_cast<uintptr_t>(workspace) & 7)) { set_error_msg("psb_relocate: workspace must be 8-byte aligned"); return PSB_ERR_ARG; }
+	if (counts_host) counts_host[0] = counts_host[1] = 0;
+	if (P == 0) return 0;
+	const RelocWorkspace w = reloc_ws_carve(workspace, P);
+	int rc;
+	if ((rc = reloc_sample(P, t.p[3], cfg, 0, -1, w, uniforms, stream))) return rc;
+	const int nb = (P + DN_TB - 1) / DN_TB;
+	reloc_correct_kernel<<<nb, DN_TB, 0, stream>>>(P, t, w.mult, cfg->min_opacity);
+	PSB_LAUNCH_OK();
+	reloc_copy_kernel<<<nb, DN_TB, 0, stream>>>(P, 0, t, w.flags, w.dead_off, w.totals, w.pick, cfg->iteration);
+	PSB_LAUNCH_OK();
+	if (counts_host) {   // the one host round trip, only for a caller that wants the count
+		RelocTotals tot;
+		PSB_CUDA_OK(cudaMemcpyAsync(&tot, w.totals, sizeof(tot), cudaMemcpyDeviceToHost, stream));
+		PSB_CUDA_OK(cudaStreamSynchronize(stream));
+		counts_host[1] = (int)tot.n_dead;
+		counts_host[0] = tot.total > 0.0 ? (int)tot.n_dead : 0;
+	}
+	return 0;
+}
+
+int psb_grow(int P, const psb_model* src, const psb_model* dst, int P_new, const psb_relocate_cfg* cfg, void* workspace, const float* uniforms,
+             void* stream_)
+{
+	cudaStream_t stream = (cudaStream_t)stream_;
+	RelocTensors ts, t;
+	const long long n = (long long)P_new - P;
+	if (P < 0 || n < 0 || n > P || !reloc_cfg_ok(cfg) || (P_new > 0 && (!src || !dst || !workspace || !reloc_tensors(src, ts) || !reloc_tensors(dst, t)))) {
+		set_error_msg("psb_grow: bad argument (P <= P_new <= 2 P, min_opacity in [0, 1), two models with parameters and moments, and a workspace required)");
+		return PSB_ERR_ARG;
+	}
+	if (P_new > 0 && (reinterpret_cast<uintptr_t>(workspace) & 7)) { set_error_msg("psb_grow: workspace must be 8-byte aligned"); return PSB_ERR_ARG; }
+	if (P == 0) return 0;
+	// the P old rows as they are (statistics and exist_since_iter included), then the picked ones are corrected in place in dst
+	for (int i = 0; i < 6; i++) {
+		const size_t bytes = (size_t)P * dn_row(i) * sizeof(float);
+		PSB_CUDA_OK(cudaMemcpyAsync(t.p[i], ts.p[i], bytes, cudaMemcpyDeviceToDevice, stream));
+		PSB_CUDA_OK(cudaMemcpyAsync(t.m[i], ts.m[i], bytes, cudaMemcpyDeviceToDevice, stream));
+		PSB_CUDA_OK(cudaMemcpyAsync(t.v[i], ts.v[i], bytes, cudaMemcpyDeviceToDevice, stream));
+	}
+	for (int q = 0; q < 3; q++)
+		if (t.stat[q] && ts.stat[q]) PSB_CUDA_OK(cudaMemcpyAsync(t.stat[q], ts.stat[q], (size_t)P * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+	if (t.exist && ts.exist) PSB_CUDA_OK(cudaMemcpyAsync(t.exist, ts.exist, (size_t)P * sizeof(int), cudaMemcpyDeviceToDevice, stream));
+	t.live = nullptr;   // dst is a new model: its live bytes are the caller's to rebuild
+	if (n == 0) return 0;
+	const RelocWorkspace w = reloc_ws_carve(workspace, P);
+	int rc;
+	if ((rc = reloc_sample(P, t.p[3], cfg, 1, (int)n, w, uniforms, stream))) return rc;
+	reloc_correct_kernel<<<(P + DN_TB - 1) / DN_TB, DN_TB, 0, stream>>>(P, t, w.mult, cfg->min_opacity);
+	PSB_LAUNCH_OK();
+	reloc_copy_kernel<<<((int)n + DN_TB - 1) / DN_TB, DN_TB, 0, stream>>>((int)n, P, t, nullptr, nullptr, w.totals, w.pick, cfg->iteration);
+	PSB_LAUNCH_OK();
+	return 0;
+}
 
 size_t psb_densify_workspace_bytes(int P) { return P > 0 ? ws_bytes(P) : 256; }
 

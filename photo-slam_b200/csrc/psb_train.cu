@@ -46,6 +46,9 @@ constexpr int MODE_DEPTH = 8;      // OR'd into MODE_GRADS / MODE_ADAM / MODE_AD
                                    // render_bwd_kernel<true, ...>) and joins dL/dxyz through the view matrix's z row
 constexpr int MODE_AA = 16;        // OR'd into any of the above: the forward was anti-aliased (o' = o h, preprocess_fwd_kernel<true, true>), slot 7
                                    // holds dL/do'; dL/dh joins the covariance gradient and the opacity gradient is h dL/do' sigma'
+constexpr int MODE_REG = 32;       // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE (each optionally | MODE_DEPTH | MODE_AA), not MODE_PUSH: the opacity
+                                   // and scale regularisers of 3DGS-MCMC (psb_trainer_set_regularizers) join the raw gradients of the rows the
+                                   // pass reached: g_opacity += reg.opacity o (1 - o), g_scaling[c] += reg.scale s_c (reg = lambda / P)
 
 // torch::optim::Adam single-tensor update (LibTorch adam.cpp): exp_avg.mul_(b1).add_(g, 1-b1);
 // exp_avg_sq.mul_(b2).addcmul_(g, g, 1-b2); denom = exp_avg_sq.sqrt()/sqrt(bc2) + eps; p.addcdiv_(exp_avg, denom, -lr/bc1).
@@ -165,15 +168,19 @@ __device__ __forceinline__ void adam_small(SmallRow& p, SmallRow& m, SmallRow& v
 //
 // MODE_DEPTH: dL/dxyz += dL/dz (V[2], V[6], V[10]). A row whose only non-zero sum is slot 11 has a gradient (its parameters are loaded and
 // updated, its live byte set) but no SH gradient: the view-direction term depends on dL/dRGB only, so its f_rest row is not staged.
+//
+// MODE_REG: `reg` is read by these instantiations only. The regularisers touch exactly the rows that have a gradient anyway (`reached`), so
+// the dirty / live decisions and the memory traffic are those of the variant without it.
 template <int MODE>
 __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int first, int P, TrainTensors t, Camera cam, GeomState geom, float4* __restrict__ sink,
                                                             StepHyper h, GradSegments grads, DensifyStats st,
                                                             const uint32_t* __restrict__ counters, uint32_t capacity, float4* __restrict__ seeds,
-                                                            DpPush dp, unsigned char* __restrict__ adam_live)
+                                                            DpPush dp, unsigned char* __restrict__ adam_live, RegCoef reg)
 {
 	constexpr bool DEPTH = (MODE & MODE_DEPTH) != 0;
 	constexpr bool AA = (MODE & MODE_AA) != 0;
-	constexpr int BASE = MODE & ~(MODE_DEPTH | MODE_AA);
+	constexpr bool REG = (MODE & MODE_REG) != 0;
+	constexpr int BASE = MODE & ~(MODE_DEPTH | MODE_AA | MODE_REG);
 	constexpr bool LIVE = BASE == MODE_ADAM_LIVE;
 	constexpr bool ADAM = BASE == MODE_ADAM || LIVE;
 	__shared__ __align__(128) float s_p[TB * REST];  // f_rest parameter rows of this block (TMA destination; LIVE: compacted per warp)
@@ -312,6 +319,10 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 			if (DEPTH) {  // z = V[2] x + V[6] y + V[10] z + V[14] (column-major view matrix)
 				const float dz = s2.w;
 				g_xyz.x += dz * cam.view[2]; g_xyz.y += dz * cam.view[6]; g_xyz.z += dz * cam.view[10];
+			}
+			if (REG && reached) {
+				g_opac += reg.opacity * sig * (1.0f - sig);
+				g_scale.x += reg.scale * s.x; g_scale.y += reg.scale * s.y; g_scale.z += reg.scale * s.z;
 			}
 		}
 		// every visible row counts, hidden ones included (the reference's denom counts them too)
@@ -680,35 +691,38 @@ void run_gaussian_backward(int first, int P, cudaStream_t stream, Args... args)
 	gaussian_backward_kernel<MODE><<<cdiv(P - first, TB), TB, 0, stream>>>(first, P, args...);
 }
 
-// Gaussians [first, P) in mode `mode` (MODE_GRADS, MODE_ADAM, MODE_ADAM_LIVE or MODE_PUSH, each optionally | MODE_DEPTH and | MODE_AA)
+// Gaussians [first, P) in mode `mode` (MODE_GRADS, MODE_ADAM, MODE_ADAM_LIVE or MODE_PUSH, each optionally | MODE_DEPTH and | MODE_AA; all but
+// MODE_PUSH optionally | MODE_REG)
 int launch_gaussian_backward(int mode, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink,
                              const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
-                             float* seeds, const DpPush& dp, unsigned char* adam_live, cudaStream_t stream)
+                             float* seeds, const DpPush& dp, unsigned char* adam_live, cudaStream_t stream, const RegCoef& reg)
 {
 	if (P - first <= 0) return 0;
 	float4* sink4 = reinterpret_cast<float4*>(sink);
 	float4* seeds4 = reinterpret_cast<float4*>(seeds);
 #define PSB_BACKWARD_CASE(M) \
-	case M: run_gaussian_backward<M>(first, P, stream, t, cam, geom, sink4, h, grads, st, counters, capacity, seeds4, dp, adam_live); break
+	case M: run_gaussian_backward<M>(first, P, stream, t, cam, geom, sink4, h, grads, st, counters, capacity, seeds4, dp, adam_live, reg); break
+#define PSB_BACKWARD_CASE_REG(M) PSB_BACKWARD_CASE(M); PSB_BACKWARD_CASE(M | MODE_REG)
 	switch (mode) {
-		PSB_BACKWARD_CASE(MODE_GRADS);
-		PSB_BACKWARD_CASE(MODE_ADAM);
-		PSB_BACKWARD_CASE(MODE_ADAM_LIVE);
+		PSB_BACKWARD_CASE_REG(MODE_GRADS);
+		PSB_BACKWARD_CASE_REG(MODE_ADAM);
+		PSB_BACKWARD_CASE_REG(MODE_ADAM_LIVE);
 		PSB_BACKWARD_CASE(MODE_PUSH);
-		PSB_BACKWARD_CASE(MODE_GRADS | MODE_DEPTH);
-		PSB_BACKWARD_CASE(MODE_ADAM | MODE_DEPTH);
-		PSB_BACKWARD_CASE(MODE_ADAM_LIVE | MODE_DEPTH);
+		PSB_BACKWARD_CASE_REG(MODE_GRADS | MODE_DEPTH);
+		PSB_BACKWARD_CASE_REG(MODE_ADAM | MODE_DEPTH);
+		PSB_BACKWARD_CASE_REG(MODE_ADAM_LIVE | MODE_DEPTH);
 		PSB_BACKWARD_CASE(MODE_PUSH | MODE_DEPTH);
-		PSB_BACKWARD_CASE(MODE_GRADS | MODE_AA);
-		PSB_BACKWARD_CASE(MODE_ADAM | MODE_AA);
-		PSB_BACKWARD_CASE(MODE_ADAM_LIVE | MODE_AA);
+		PSB_BACKWARD_CASE_REG(MODE_GRADS | MODE_AA);
+		PSB_BACKWARD_CASE_REG(MODE_ADAM | MODE_AA);
+		PSB_BACKWARD_CASE_REG(MODE_ADAM_LIVE | MODE_AA);
 		PSB_BACKWARD_CASE(MODE_PUSH | MODE_AA);
-		PSB_BACKWARD_CASE(MODE_GRADS | MODE_DEPTH | MODE_AA);
-		PSB_BACKWARD_CASE(MODE_ADAM | MODE_DEPTH | MODE_AA);
-		PSB_BACKWARD_CASE(MODE_ADAM_LIVE | MODE_DEPTH | MODE_AA);
+		PSB_BACKWARD_CASE_REG(MODE_GRADS | MODE_DEPTH | MODE_AA);
+		PSB_BACKWARD_CASE_REG(MODE_ADAM | MODE_DEPTH | MODE_AA);
+		PSB_BACKWARD_CASE_REG(MODE_ADAM_LIVE | MODE_DEPTH | MODE_AA);
 		PSB_BACKWARD_CASE(MODE_PUSH | MODE_DEPTH | MODE_AA);
 		default: set_error_msg("launch_gaussian_backward: unknown mode"); return -1;
 	}
+#undef PSB_BACKWARD_CASE_REG
 #undef PSB_BACKWARD_CASE
 	PSB_LAUNCH_OK();
 	return 0;
@@ -731,7 +745,7 @@ int launch_signal(uint32_t* const* flag, float* const* meta, const float* campos
 
 int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, float* seeds,
                           const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
-                          cudaStream_t stream, cudaEvent_t between, unsigned char* adam_live, const PassMode& mode)
+                          cudaStream_t stream, cudaEvent_t between, unsigned char* adam_live, const PassMode& mode, const RegCoef& reg)
 {
 	if (P - first <= 0) return 0;
 	if (!seeds) { set_error_msg("launch_fused_backward: seed scratch missing"); return -1; }
@@ -739,9 +753,10 @@ int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, co
 	DpPush nodp;
 	memset(&nodp, 0, sizeof(nodp));
 	unsigned char* live = adam ? adam_live : nullptr;
-	const int variant = (live ? MODE_ADAM_LIVE : adam ? MODE_ADAM : MODE_GRADS) | (mode.depth ? MODE_DEPTH : 0) | (mode.aa ? MODE_AA : 0);
+	const int variant = (live ? MODE_ADAM_LIVE : adam ? MODE_ADAM : MODE_GRADS) | (mode.depth ? MODE_DEPTH : 0) | (mode.aa ? MODE_AA : 0) |
+	                    (reg.opacity != 0.f || reg.scale != 0.f ? MODE_REG : 0);
 	int rc;
-	if ((rc = launch_gaussian_backward(variant, first, P, t, cam, geom, sink, h, grads, st, counters, capacity, seeds, nodp, live, stream))) return rc;
+	if ((rc = launch_gaussian_backward(variant, first, P, t, cam, geom, sink, h, grads, st, counters, capacity, seeds, nodp, live, stream, reg))) return rc;
 	if (between) cudaEventRecord(between, stream);
 	const AdamCoef ac(h);
 	const uint32_t e0 = (uint32_t)first * REST, e1 = (uint32_t)P * REST;
@@ -767,7 +782,7 @@ int launch_push_backward(int P, const TrainTensors& t, const Camera& cam, const 
 	const GradSegments nog = {};
 	int rc;
 	if ((rc = launch_gaussian_backward(MODE_PUSH | (mode.depth ? MODE_DEPTH : 0) | (mode.aa ? MODE_AA : 0), 0, P, t, cam, geom, sink, h, nog, st, counters, capacity, nullptr, dp,
-	                                   nullptr, stream)))
+	                                   nullptr, stream, RegCoef{0.f, 0.f})))
 		return rc;
 	return launch_signal(dp.grad_flag, dp.meta, cam.campos, h.D, dp.world, dp.rank, dp.epoch, stream);
 }

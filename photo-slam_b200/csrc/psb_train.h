@@ -34,7 +34,13 @@ struct PassMode {
 	bool det;    // deterministic mode
 	bool aa;     // the forward was anti-aliased (launch_preprocess aa): slot 7 of the sink rows holds dL/do'
 	bool depth;  // the sink rows carry dL/dz in slot 11 (render_bwd_kernel<true, ...>)
+	float reg_opacity, reg_scale;  // psb_trainer_set_regularizers: lambda_opacity, lambda_scale (both 0: the variants without MODE_REG)
 };
+// lambda / P of the opacity and scale regularisers for the rows a per-Gaussian backward updates; both 0 = no regulariser
+struct RegCoef {
+	float opacity, scale;
+};
+inline RegCoef reg_coef(const PassMode& m, int P) { return {P > 0 ? m.reg_opacity / (float)P : 0.f, P > 0 ? m.reg_scale / (float)P : 0.f}; }
 
 // ---- NVLink data-parallel step (psb_dp_*, include/psb200.h) -----------------------------------------------------------
 // Ownership: Gaussians are cut into chunks of 128 (one block of the per-Gaussian backward); chunk c belongs to rank
@@ -70,7 +76,12 @@ int launch_wait_flags(const uint32_t* flags, int world, uint32_t epoch, uint32_t
 int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, float* seeds,
                           const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
                           cudaStream_t stream, cudaEvent_t between /* recorded between the two kernels (stage timing), or null */,
-                          unsigned char* adam_live /* adam only: psb_model.adam_live, or null (the moments tell idle rows) */, const PassMode& mode);
+                          unsigned char* adam_live /* adam only: psb_model.adam_live, or null (the moments tell idle rows) */, const PassMode& mode,
+                          const RegCoef& reg /* reg_coef(mode, the model's row count) */);
+// 3DGS-MCMC position noise on xyz [P,3] (psb_trainer_inject_noise; kernel in psb_densify.cu, beside the Philox draw it shares with the
+// split): lr = lr_xyz * noise_lr; tile_info != null: only rows the pass saw; no-op when counters[0] > capacity
+int launch_position_noise(int P, float* xyz, const float* opacity, const float* scaling, const float* rotation, float lr, unsigned long long seed,
+                          unsigned long long step, const uint4* tile_info, const uint32_t* counters, uint32_t capacity, cudaStream_t stream);
 // adam_live[i] = any moment of row i non-zero (t.m / t.v: the 12 moment tensors)
 int launch_adam_live_rebuild(int P, const TrainTensors& t, unsigned char* adam_live, cudaStream_t stream);
 int launch_adam(size_t n, float* p, float* m, float* v, const float* g, float lr, const StepHyper& h, float grad_scale, cudaStream_t stream);

@@ -30,10 +30,12 @@ struct psb_trainer {
 	uint32_t seq = 0;            // sequence number of the last forward pass (render / step / backward) of this context
 	// the mode of pass `seq`: what psb_trainer_backward_pixels must match, and the variant every per-Gaussian stage behind it runs
 	// (a psb_trainer_backward_begin* records it before its pass, so the _slab calls after it run that variant even if it failed)
-	PassMode pass = {-1, false, false, false};
+	PassMode pass = {-1, false, false, false, 0.f, 0.f};
 	// anti-aliasing (psb_trainer_set_antialiasing): every forward pass blends with o' = o h (the 2D Mip filter), and every per-Gaussian
 	// backward behind it runs the AA variant
 	bool antialiasing = false;
+	// opacity / scale regularisers (psb_trainer_set_regularizers): recorded in the mode of every pass that starts while they are set
+	float reg_opacity = 0.f, reg_scale = 0.f;
 	uint32_t ovf_first = 0, ovf_count = 0;  // what the last PSB_ERR_RETRY was about (psb_trainer_overflow_info)
 	cudaEvent_t readback = nullptr;  // recorded once the instance count (and the loss sums) of the last call are in pinned memory
 	int last_P = 0, last_W = 0, last_H = 0;
@@ -265,7 +267,7 @@ int check_grads(float* const* grads, int P, const char* fn)
 }
 
 // The mode of a pass that starts now, in the context's deterministic and anti-aliasing modes.
-PassMode pass_mode(const psb_trainer* t, int D, bool depth) { return {D, t->deterministic, t->antialiasing, depth}; }
+PassMode pass_mode(const psb_trainer* t, int D, bool depth) { return {D, t->deterministic, t->antialiasing, depth, t->reg_opacity, t->reg_scale}; }
 
 // Stage 1 of every pass: forward of SH degree D from raw parameters into t->image (or out_color); out_depth != NULL: the depth variant
 // also writes the expected depth there; out_alpha != NULL: the opacity variant also writes 1 - final_T there. The pass is recorded as
@@ -678,7 +680,7 @@ int psb_trainer_backward_pixels(psb_trainer* t, unsigned pass, int P, int M, con
 	if (!adam)
 		for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
 	rc = launch_fused_backward(adam, 0, P, train_tensors(model, adam), cam, sc.geom, t->sink, t->seeds, to_hyper(step), gs, densify_stats(model, step),
-	                           sc.geom.counters, (uint32_t)t->capacity, stream, t->event(7), adam ? model->adam_live : nullptr, t->pass);
+	                           sc.geom.counters, (uint32_t)t->capacity, stream, t->event(7), adam ? model->adam_live : nullptr, t->pass, reg_coef(t->pass, P));
 	t->end_stages(8, stream);
 	return rc;
 }
@@ -711,7 +713,7 @@ int psb_trainer_step_exposure(psb_trainer* t, int P, int M, const psb_model* mod
 	    P == 0)
 		return rc;
 	rc = launch_fused_backward(true, 0, P, train_tensors(model, true), tb.cam, tb.geom, t->sink, t->seeds, to_hyper(step), GradSegments{},
-	                           densify_stats(model, step), tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), model->adam_live, t->pass);
+	                           densify_stats(model, step), tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), model->adam_live, t->pass, reg_coef(t->pass, P));
 	t->end_stages(8, stream);
 	return rc;
 }
@@ -749,7 +751,7 @@ int psb_trainer_backward_exposure(psb_trainer* t, int P, int M, const psb_model*
 	GradSegments gs;
 	for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
 	rc = launch_fused_backward(false, 0, P, train_tensors(model, false), tb.cam, tb.geom, t->sink, t->seeds, to_hyper(step), gs, densify_stats(model, step),
-	                           tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), nullptr, t->pass);
+	                           tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), nullptr, t->pass, reg_coef(t->pass, P));
 	t->end_stages(8, stream);
 	return rc;
 }
@@ -793,7 +795,7 @@ int psb_trainer_backward_slab(psb_trainer* t, int P, int M, const psb_model* mod
 	GradSegments gs;
 	for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
 	return launch_fused_backward(false, first, first + count, train_tensors(model, false), to_camera(camera), geom, t->sink, t->seeds, to_hyper(step), gs,
-	                             densify_stats(model, step), geom.counters, (uint32_t)t->capacity, (cudaStream_t)stream_, nullptr, nullptr, t->pass);
+	                             densify_stats(model, step), geom.counters, (uint32_t)t->capacity, (cudaStream_t)stream_, nullptr, nullptr, t->pass, reg_coef(t->pass, P));
 }
 
 int psb_adam_update(int P, int M, const psb_model* model, float* const* grads, const psb_step* step, float grad_scale, void* stream_)
@@ -936,6 +938,34 @@ int psb_trainer_set_antialiasing(psb_trainer* t, int enable)
 	if (!t) { set_error_msg("psb_trainer_set_antialiasing: null context"); return PSB_ERR_ARG; }
 	t->antialiasing = enable != 0;   // (takes effect at the next pass; the scratch does not change)
 	return 0;
+}
+
+int psb_trainer_set_regularizers(psb_trainer* t, float lambda_opacity, float lambda_scale)
+{
+	if (!t || !std::isfinite(lambda_opacity) || !std::isfinite(lambda_scale) || lambda_opacity < 0.f || lambda_scale < 0.f) {
+		set_error_msg("psb_trainer_set_regularizers: a context and finite lambdas >= 0 required");
+		return PSB_ERR_ARG;
+	}
+	t->reg_opacity = lambda_opacity; t->reg_scale = lambda_scale;   // (take effect at the next pass)
+	return 0;
+}
+
+int psb_trainer_inject_noise(psb_trainer* t, int P, const psb_model* model, float lr_xyz, float noise_lr, unsigned long long seed,
+                             unsigned long long step, int visible_only, void* stream_)
+{
+	if (!t || !model || P < 0 || !std::isfinite(lr_xyz) || !std::isfinite(noise_lr) || lr_xyz < 0.f || noise_lr < 0.f) {
+		set_error_msg("psb_trainer_inject_noise: a context, a model, P >= 0 and finite lr_xyz, noise_lr >= 0 required");
+		return PSB_ERR_ARG;
+	}
+	if (t->geom_P != P || t->last_P != P) { set_error_msg("psb_trainer_inject_noise: the context's latest pass was not over P rows"); return PSB_ERR_ARG; }
+	if (P == 0) return 0;
+	if (!model->param[0] || !model->param[3] || !model->param[4] || !model->param[5] || (reinterpret_cast<uintptr_t>(model->param[5]) & 15)) {
+		set_error_msg("psb_trainer_inject_noise: xyz, opacity, scaling and a 16-byte aligned rotation tensor required");
+		return PSB_ERR_ARG;
+	}
+	const GeomState geom = carve_scratch(t, P, t->last_W, t->last_H).geom;
+	return launch_position_noise(P, model->param[0], model->param[3], model->param[4], model->param[5], lr_xyz * noise_lr, seed, step,
+	                             visible_only ? geom.tile_info : nullptr, geom.counters, (uint32_t)t->capacity, (cudaStream_t)stream_);
 }
 
 // ms[i] = time between stage boundaries i and i+1 of the last profiled step (see psb_trainer::ev), i < n; entries beyond the last

@@ -82,6 +82,10 @@ class _DensifyCfg(C.Structure):
                 ("seed", C.c_ulonglong), ("offset", C.c_ulonglong)]
 
 
+class _RelocateCfg(C.Structure):
+    _fields_ = [("min_opacity", C.c_float), ("iteration", C.c_int), ("seed", C.c_ulonglong), ("offset", C.c_ulonglong)]
+
+
 def _bind():
     """The library with every trainer, data-parallel, densification and debug entry point declared (include/psb200.h)."""
     L = _lib.lib()
@@ -90,6 +94,7 @@ def _bind():
     vp, i, f, u, size_t = C.c_void_p, C.c_int, C.c_float, C.c_uint, C.c_size_t
     P = C.POINTER
     Model, Cam, Step, Depth, Exp, Cfg = P(_Model), P(_Camera), P(_Step), P(_Depth), P(_Exposure), P(_DensifyCfg)
+    ull = C.c_ulonglong
     # the arguments every built-in-loss training call starts with: t, P, M, model, camera, background, gt_image, mask, step, out_color, radii
     call = [vp, i, i, Model, Cam, vp, vp, vp, Step, vp, vp]
     render = [vp, i, i, Model, Cam, vp, i, vp, vp]   # t, P, M, model, camera, background, sh_degree, out_color, radii
@@ -117,6 +122,8 @@ def _bind():
         "psb_trainer_stage_times": [vp, P(f), i],
         "psb_trainer_set_deterministic": [vp, i],
         "psb_trainer_set_antialiasing": [vp, i],
+        "psb_trainer_set_regularizers": [vp, f, f],
+        "psb_trainer_inject_noise": [vp, i, Model, f, f, ull, ull, i, vp],
         "psb_adam_update": [i, i, Model, P(vp), Step, f, vp],
         "psb_adam_flat": [size_t, vp, vp, vp, vp, f, Step, f, vp],
         "psb_adam_live_rebuild": [i, Model, vp],
@@ -137,11 +144,14 @@ def _bind():
         "psb_prune_apply": [i, Model, Model, i, vp, i, vp],
         "psb_insert_points": [i, Model, Model, i, vp, vp, vp, i, vp],
         "psb_reset_opacity": [i, vp, vp, vp, vp],
+        "psb_relocate": [i, Model, P(_RelocateCfg), vp, vp, P(i), vp],
+        "psb_grow": [i, Model, Model, i, P(_RelocateCfg), vp, vp, vp],
     }
     for name, args in sigs.items():
         fn = getattr(L, name)
         fn.argtypes, fn.restype = args, i
     L.psb_densify_workspace_bytes.argtypes, L.psb_densify_workspace_bytes.restype = [i], size_t
+    L.psb_relocate_workspace_bytes.argtypes, L.psb_relocate_workspace_bytes.restype = [i], size_t
     L._trainer_bound = True
     return L
 
@@ -165,6 +175,16 @@ class GaussianOptimizationParams:
     densify_until_iter: int = 15000
     densify_grad_threshold: float = 0.001
     exposure_lr: float = 0.01     # learning rate of the per-keyframe exposure rows (graphdeco's exposure_lr_init)
+    # bounded-budget densification (3DGS-MCMC, Kheradmand et al. 2024; the defaults are the paper's / gsplat MCMCStrategy's). Off by default.
+    mcmc: bool = False            # GaussianTrainer: regularisers on the step, position noise behind it, mcmcRefine() instead of densifyAndPrune
+    cap_max: int = 1_000_000      # the map never holds more Gaussians than this
+    mcmc_noise_lr: float = 5e5    # the noise is Sigma xi * position lr * this * g(opacity)
+    mcmc_noise_visible_only: bool = True   # noise only on rows the step's view saw (False: every row, as in offline training)
+    opacity_reg: float = 0.01     # lambda of mean sigmoid(opacity)
+    scale_reg: float = 0.01       # lambda of mean exp(scaling)
+    mcmc_min_opacity: float = 0.005   # a Gaussian at or below is dead and gets relocated
+    mcmc_grow_factor: float = 1.05    # growth per mcmcRefine, up to cap_max
+    mcmc_seed: int = 0            # key of the relocation draws and of the noise
 
 
 class GaussianModel:
@@ -451,6 +471,55 @@ class GaussianModel:
         self._adopt(d)
         return tuple(counts)
 
+    # --- bounded-budget densification (3DGS-MCMC; gsplat MCMCStrategy's relocate / sample_add): psb_relocate / psb_grow
+    def _uniforms(self, uniforms):
+        return None if uniforms is None else uniforms.to(self.device, torch.float32).contiguous()
+
+    def relocateGaussians(self, min_opacity=0.005, seed=0, offset=None, iteration=0, uniforms=None):
+        """Every dead row (sigmoid(opacity) <= min_opacity) becomes a copy of an alive row drawn with probability proportional to its
+        opacity; the drawn rows and their copies share the corrected opacity and scale that keep the rendered picture (psb_relocate).
+        In place, the row count does not change; moments of the rows involved are zeroed. The draw is Philox(seed, offset) — identical
+        on every replica — unless `uniforms` (one number in [0, 1) per dead row, at least that many) is injected (tests).
+        Returns the number of rows relocated (one host round trip)."""
+        L = _bind()
+        P = self.num_points()
+        cfg = _RelocateCfg(float(min_opacity), int(iteration), int(seed), int(self.step_ if offset is None else offset))
+        ws = torch.empty(L.psb_relocate_workspace_bytes(P), dtype=torch.uint8, device=self.device)
+        src = self._src()
+        live = self._live_tensor()
+        if self.adam_live_valid_:
+            src.adam_live = live.data_ptr()     # kept exact: the bytes of the rows whose moments are zeroed are cleared
+        u = self._uniforms(uniforms)
+        counts = (C.c_int * 2)()
+        _lib.check(L.psb_relocate(P, C.byref(src), C.byref(cfg), ws.data_ptr(), u.data_ptr() if u is not None and u.numel() else None, counts,
+                                  torch.cuda.current_stream().cuda_stream), "psb_relocate")
+        if u is not None:
+            assert u.numel() >= counts[1], (u.numel(), counts[1])
+        return counts[0]
+
+    def addNewGaussians(self, cap_max, grow_factor=1.05, min_opacity=0.005, seed=0, offset=None, iteration=0, uniforms=None):
+        """Grows the model to min(cap_max, floor(grow_factor * P)) rows: the new rows are copies of rows drawn (over all rows) with
+        probability proportional to opacity, corrected together with their sources like relocateGaussians does (psb_grow); they
+        start with zero moments and statistics and exist_since_iter = iteration. Returns the number of rows added (0 at the cap)."""
+        L = _bind()
+        P = self.num_points()
+        if not 1.0 < grow_factor <= 2.0:
+            raise ValueError(f"grow_factor must be in (1, 2], got {grow_factor}")
+        P_new = min(int(cap_max), int(math.floor(grow_factor * P)))
+        if P_new <= P:
+            return 0
+        cfg = _RelocateCfg(float(min_opacity), int(iteration), int(seed), int(self.step_ if offset is None else offset))
+        ws = torch.empty(L.psb_relocate_workspace_bytes(P), dtype=torch.uint8, device=self.device)
+        u = self._uniforms(uniforms)
+        if u is not None:
+            assert u.numel() >= P_new - P, (u.numel(), P_new - P)
+        d = self._blank(P_new)
+        src, dst = self._src(), self._cm(d["p"], d["m"], d["v"], d["accum"], d["denom"], d["max_radii"], d["exist"])
+        _lib.check(L.psb_grow(P, C.byref(src), C.byref(dst), P_new, C.byref(cfg), ws.data_ptr(), u.data_ptr() if u is not None else None,
+                              torch.cuda.current_stream().cuda_stream), "psb_grow")
+        self._adopt(d)
+        return P_new - P
+
     def densifySplitCount(self, max_grad, extent):
         """number of rows densifyAndSplit would select right now (plan only; for tests that inject the normal draw)"""
         L = _bind()
@@ -557,7 +626,13 @@ class GaussianTrainer:
     antialiasing: True renders and trains every pass of this trainer with the 2D Mip filter (psb_trainer_set_antialiasing: each splat
     blends with opacity o * sqrt(max(det0 / det1, 2.5e-5)), det0 / det1 the determinants of its 2D covariance before / after the
     0.3 px^2 dilation), as renderer.render(pipe=GaussianPipelineParams(antialiasing=True)) does on the operator path. Fixed for the
-    trainer's lifetime."""
+    trainer's lifetime.
+
+    opt.mcmc: bounded-budget densification (3DGS-MCMC). The step's per-Gaussian stage adds the opacity and scale regularisers
+    (opt.opacity_reg, opt.scale_reg; psb_trainer_set_regularizers: on the rows the step updates), trainForOneIteration and
+    trainWithLoss enqueue the position noise behind the step (psb_trainer_inject_noise, keyed by opt.mcmc_seed and model.step_), and
+    mcmcRefine() replaces densifyAndPrune: it relocates the dead Gaussians and grows the map by opt.mcmc_grow_factor up to
+    opt.cap_max. With mcmc off nothing of this is launched."""
 
     def __init__(self, model: GaussianModel, opt: GaussianOptimizationParams = None, background=None, deterministic=None, antialiasing=False):
         self.L = _bind()
@@ -575,6 +650,28 @@ class GaussianTrainer:
         self._antialiasing = bool(antialiasing)
         if self._antialiasing:
             _lib.check(self.L.psb_trainer_set_antialiasing(self.h, 1), "psb_trainer_set_antialiasing")
+        if self.opt.mcmc:
+            _lib.check(self.L.psb_trainer_set_regularizers(self.h, float(self.opt.opacity_reg), float(self.opt.scale_reg)),
+                       "psb_trainer_set_regularizers")
+
+    def _inject_noise(self):
+        """opt.mcmc: the position noise behind the step just enqueued (a no-op on the device if that step's pass overflowed)."""
+        if not self.opt.mcmc:
+            return
+        m, o = self.model, self.opt
+        cm = m._cmodel(False)
+        _lib.check(self.L.psb_trainer_inject_noise(self.h, m.num_points(), C.byref(cm), float(m.lr_[0]), float(o.mcmc_noise_lr), int(o.mcmc_seed),
+                                                   int(m.step_), int(bool(o.mcmc_noise_visible_only)), torch.cuda.current_stream().cuda_stream),
+                   "psb_trainer_inject_noise")
+
+    def mcmcRefine(self, iteration=None):
+        """The refinement round of 3DGS-MCMC, in place of densifyAndPrune: relocateGaussians, then addNewGaussians up to opt.cap_max, both
+        keyed by (opt.mcmc_seed, model.step_) like densifyAndPrune's split draw. Returns (rows relocated, rows added)."""
+        m, o = self.model, self.opt
+        it = self.iteration if iteration is None else int(iteration)
+        n_rel = m.relocateGaussians(o.mcmc_min_opacity, seed=o.mcmc_seed, iteration=it)
+        n_add = m.addNewGaussians(o.cap_max, o.mcmc_grow_factor, o.mcmc_min_opacity, seed=o.mcmc_seed, iteration=it)
+        return n_rel, n_add
 
     @property
     def antialiasing(self):
@@ -709,6 +806,7 @@ class GaussianTrainer:
         gd = next(g) if depth else None
         ga = next(g) if alpha else None
         self.backwardPixels(gc, gd, ga, densify_stats=densify_stats)
+        self._inject_noise()
         self._last = _Call(True, lambda: self.trainWithLoss(cam, loss_fn, depth, alpha, out_color, radii, densify_stats), True)
         self._last_loss = loss.detach()
         return self._last_loss
@@ -741,6 +839,7 @@ class GaussianTrainer:
                                                     C.byref(exposure) if exposure is not None else None, torch.cuda.current_stream().cuda_stream),
                    "psb_trainer_step_exposure")
         m.step_ += 1
+        self._inject_noise()
         self._last = _Call(True, lambda: self.trainForOneIteration(cam, gt_image, mask, out_color, radii, densify_stats, gt_depth, lambda_depth,
                                                                    out_depth, exposure_id), False)
 
@@ -882,6 +981,10 @@ class DataParallelTrainer(GaussianTrainer):
 
     def __init__(self, model, opt=None, background=None, group=None, pipeline=None, nslabs=4, mode=None, deterministic=None,
                  antialiasing=False):
+        if opt is not None and opt.mcmc:
+            raise NotImplementedError("DataParallelTrainer: opt.mcmc is not wired into the data-parallel steps (the owner-side Adam would need the "
+                                      "regularisers, every rank the noise, and a refinement gather_moments() first); train with it on one GPU "
+                                      "through GaussianTrainer")
         super().__init__(model, opt, background, deterministic=deterministic, antialiasing=antialiasing)
         import os
         import torch.distributed as dist
