@@ -620,6 +620,43 @@ int psb_trainer_inject_noise(psb_trainer* t, int P, const psb_model* model, floa
 int psb_trainer_set_regularizers(psb_trainer* t, float lambda_opacity, float lambda_scale);
 
 /* ------------------------------------------------------------------------------------------------
+ * 3D smoothing filter (Mip-Splatting, Yu et al., CVPR 2024: compute_3D_filter, get_scaling_with_3D_filter,
+ * get_opacity_with_3D_filter). It bounds every Gaussian from below by the finest sampling interval at which any keyframe saw it, so a
+ * Gaussian cannot shrink into a high-frequency artefact that shows when the map is viewed closer or at a higher resolution than it was
+ * trained at. (The 2D filter of psb_trainer_set_antialiasing handles the opposite case, zooming out.)
+ * Filter. Inputs: the rows' xyz [P,3] and K cameras, each with its view matrix (the layout of psb_camera.viewmatrix),
+ *   focal_x = W / (2 tan_fovx), focal_y = H / (2 tan_fovy), W and H: the full-resolution keyframes. For row i and camera k,
+ *   (x, y, z) = the view matrix applied to xyz_i exactly as the forward does, so the z test is the forward's near cull bit for bit.
+ *   Camera k SEES row i when z > 0.2, u = x / z focal_x + W / 2 in [-0.15 W, 1.15 W] and v = y / z focal_y + H / 2 in [-0.15 H, 1.15 H].
+ *   d_i = min z over the cameras that see row i; F = max focal_x over all K cameras; a row no camera sees takes d_i = max d over the rows
+ *   that are seen; filter_i = d_i / F * sqrt(0.2). No row seen (K = 0 included): every filter_i = 0. Only minima and maxima are involved:
+ *   the result is bit-identical from run to run.
+ * Application. s = exp(scaling), o = sigmoid(opacity), f = filter_i:
+ *   s'_c = sqrt(s_c^2 + f^2),  c = sqrt(prod_c s_c^2 / prod_c s'_c^2) (formed as the product of the three ratios),  o' = o c.
+ *   R diag(s')^2 R^T = Sigma + f^2 I: the splat is the plain one with its 3D covariance widened isotropically, and c keeps its integral.
+ *   With anti-aliasing the blend opacity is o c h, h from the 2D covariance of the widened splat. IEEE sqrt and division: f = 0 is the
+ *   plain splat bit for bit (s' = s, c = 1).
+ * Backward (the per-Gaussian stage), with dL/ds' from the covariance chain and g = dL/d(o c) (the opacity sum, times h with anti-aliasing):
+ *   dL/ds_c = dL/ds'_c s_c / s'_c + o c g f^2 / (s_c s'_c^2),  dL/do = c g, then the exp and sigmoid chain to the raw parameters.
+ * Not filtered: dL/dmean2D and the densification statistics, the densification size tests, the 3DGS-MCMC regularisers and position noise
+ *   read the raw activations. max_radii2D takes the forward's radii, which are those of the filtered splat.
+ * The caller decides when to recompute the filter (Mip-Splatting: after each densification and every 100 iterations); nothing here does.
+ * ------------------------------------------------------------------------------------------------ */
+/* filter [P] device float32 <- the filter of the P rows of xyz [P,3] (device) for the K cameras cams [K][20] (device: the view matrix's
+ * 16 floats, then focal_x, focal_y, W, H; focal lengths and sizes positive). seen_host (host, may be NULL) receives the number of rows
+ * seen by at least one camera; only then does the call synchronise the stream, otherwise it is asynchronous. PSB_ERR_ARG, before any CUDA
+ * call, for P < 0, K < 0, a NULL xyz or filter with P > 0 and a NULL cams with K > 0. */
+int psb_filter3d(int P, const float* xyz, int K, const float* cams, float* filter, int* seen_host, void* stream);
+/* The 3D filter of a context: filter [P] device (as psb_filter3d leaves it) or NULL = off (the default; P is then ignored). While it is
+ * set, every pass of the context applies it: psb_trainer_render(_depth), psb_trainer_forward, psb_trainer_step*, psb_trainer_backward*
+ * and psb_trainer_backward_pixels, whose per-Gaussian stage differentiates it. The array is read by the passes (not copied): it must
+ * stay valid and unchanged while they run. A pass whose P differs from the filter's returns PSB_ERR_ARG before any CUDA call. The
+ * setting is recorded in the mode of every pass; psb_trainer_backward_pixels refuses a pass whose filter was switched (or replaced by
+ * another array) after it. psb_dp_step*, psb_trainer_backward_begin* and psb_trainer_backward_slab return PSB_ERR_ARG while it is set.
+ * Combines with the deterministic, anti-aliasing and regulariser modes. PSB_ERR_ARG for a NULL context and a filter with P < 0. */
+int psb_trainer_set_filter3d(psb_trainer* t, const float* filter, int P);
+
+/* ------------------------------------------------------------------------------------------------
  * Point-cloud helpers exported by the same shared objects in the reference.
  * ------------------------------------------------------------------------------------------------ */
 

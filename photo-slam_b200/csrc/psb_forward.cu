@@ -28,12 +28,17 @@ namespace psb {
 // opacity o' = o h, h = sqrt(max(det0 / det1, 2.5e-5)), det0 / det1 the determinants of the 2D covariance before / after the 0.3 px^2
 // dilation. Conic, radius, tile rectangle, depth key, colour and clamp bits are those of AA = false; the record, pmin and the tight
 // tile cull all see o'.
+// F3D = true (trainer variant only, RAW): the 3D smoothing filter of Mip-Splatting (psb_filter3d): the covariance is built from
+// s' = sqrt(s^2 + f^2) and the opacity is o c, c = sqrt(prod s^2 / prod s'^2), f = f3d[idx]; with AA the blend opacity is o c h, h taken
+// from the 2D covariance of the widened splat. Radius, rectangle, the record, pmin and the tight tile cull all see the filtered splat.
 // ------------------------------------------------------------------------------------------------
 constexpr int PRE_TB = 128;  // Gaussians per block
 
-template <bool RAW, bool AA = false>
-__global__ void __launch_bounds__(PRE_TB) preprocess_fwd_kernel(GaussIn in, Camera cam, int* __restrict__ radii_out, GeomState geom, int tight)
+template <bool RAW, bool AA = false, bool F3D = false>
+__global__ void __launch_bounds__(PRE_TB) preprocess_fwd_kernel(GaussIn in, Camera cam, int* __restrict__ radii_out, GeomState geom, int tight,
+                                                                const float* __restrict__ f3d)
 {
+	static_assert(RAW || !F3D, "the 3D filter is applied to the raw trainer parameters only");
 	// SH rows of this block's Gaussians ([128][45] raw f_rest rows or [128][48] activated rows), one TMA bulk copy per block:
 	// they are consumed last (after both culls), so the copy hides behind the projection / covariance arithmetic and each
 	// thread then walks its own row in shared memory (odd / 48-word row stride: at most 2-way bank conflicts on the 48 case).
@@ -68,8 +73,10 @@ __global__ void __launch_bounds__(PRE_TB) preprocess_fwd_kernel(GaussIn in, Came
 	float3 p_orig = make_float3(0, 0, 1), s = make_float3(0, 0, 0), dc = make_float3(0, 0, 0);
 	float4 q = make_float4(1, 0, 0, 0);
 	float opacity = 0.f;
+	float f3d_f = 0.f;  // F3D: this row's filter
 	float cov3D[6] = {0, 0, 0, 0, 0, 0};
 	if (alive) {
+		if (F3D) f3d_f = f3d[idx];
 		p_orig = make_float3(in.means3D[3 * idx], in.means3D[3 * idx + 1], in.means3D[3 * idx + 2]);
 		if (in.cov3D_precomp != nullptr) {
 #pragma unroll
@@ -90,6 +97,7 @@ __global__ void __launch_bounds__(PRE_TB) preprocess_fwd_kernel(GaussIn in, Came
 	float2 point_image = make_float2(0, 0);
 	float my_radius = 0.f;
 	float aa_h = 1.f;  // AA: the opacity factor h
+	float f3d_c = 1.f; // F3D: the opacity factor c
 	int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
 	if (alive) {
 		p_view = xform4x3(p_orig, cam.view);
@@ -106,6 +114,7 @@ __global__ void __launch_bounds__(PRE_TB) preprocess_fwd_kernel(GaussIn in, Came
 				const float n = fmaxf(sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w), 1e-12f);
 				q = make_float4(q.x / n, q.y / n, q.z / n, q.w / n);
 			}
+			if (F3D) f3d_c = filter3d_widen(s, f3d_f);
 			cov3d_from_scale_rot(s, in.scale_modifier, q, cov3D);
 		}
 
@@ -165,6 +174,7 @@ __global__ void __launch_bounds__(PRE_TB) preprocess_fwd_kernel(GaussIn in, Came
 	}
 
 	if (RAW) opacity = 1.0f / (1.0f + expf(-opacity));
+	if (F3D) opacity *= f3d_c;
 	if (AA) opacity *= aa_h;
 
 	const int radius_i = (int)my_radius;
@@ -487,14 +497,19 @@ __global__ void __launch_bounds__(256) tile_ranges_kernel(const uint32_t* __rest
 // ------------------------------------------------------------------------------------------------
 // Host orchestration
 // ------------------------------------------------------------------------------------------------
-int launch_preprocess(const GaussIn& in, const Camera& cam, int* radii_out, const GeomState& geom, bool raw, bool tight, cudaStream_t stream, bool aa)
+int launch_preprocess(const GaussIn& in, const Camera& cam, int* radii_out, const GeomState& geom, bool raw, bool tight, cudaStream_t stream, bool aa,
+                      const float* f3d)
 {
 	if (in.P == 0) return 0;
+	if (f3d && !raw) { set_error_msg("launch_preprocess: the 3D filter needs the raw trainer parameters"); return -1; }
 	const int grid = cdiv(in.P, PRE_TB);
-	if (aa && raw) preprocess_fwd_kernel<true, true><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tight ? 1 : 0);
-	else if (aa) preprocess_fwd_kernel<false, true><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tight ? 1 : 0);
-	else if (raw) preprocess_fwd_kernel<true><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tight ? 1 : 0);
-	else preprocess_fwd_kernel<false><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tight ? 1 : 0);
+	const int tt = tight ? 1 : 0;
+	if (f3d && aa) preprocess_fwd_kernel<true, true, true><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tt, f3d);
+	else if (f3d) preprocess_fwd_kernel<true, false, true><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tt, f3d);
+	else if (aa && raw) preprocess_fwd_kernel<true, true><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tt, nullptr);
+	else if (aa) preprocess_fwd_kernel<false, true><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tt, nullptr);
+	else if (raw) preprocess_fwd_kernel<true><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tt, nullptr);
+	else preprocess_fwd_kernel<false><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tt, nullptr);
 	PSB_LAUNCH_OK();
 	return 0;
 }

@@ -83,6 +83,19 @@ __device__ __forceinline__ float aa_det0(const Cov2DTerms& ct) { return ct.cov(0
 constexpr float kAaMinRatio = 2.5e-5f;
 __device__ __forceinline__ float aa_factor(float det0, float det1) { return sqrtf(fmaxf(det0 / det1, kAaMinRatio)); }
 
+// 3D smoothing filter (Mip-Splatting; include/psb200.h, psb_filter3d): s <- s' = sqrt(s^2 + f^2) per axis, and returns the opacity factor
+// c = sqrt(prod_c s_c^2 / s'_c^2), formed as the product of the per-axis ratios (the products of three squares can underflow). IEEE sqrt and
+// division: f = 0 leaves s bit for bit (sqrt(fl(s^2)) = s) and returns exactly 1.
+__device__ __forceinline__ float filter3d_widen(float3& s, float f)
+{
+	const float f2 = f * f;
+	const float sx2 = s.x * s.x, sy2 = s.y * s.y, sz2 = s.z * s.z;
+	const float px2 = sx2 + f2, py2 = sy2 + f2, pz2 = sz2 + f2;
+	const float r = (px2 > 0.f ? sx2 / px2 : 1.f) * (py2 > 0.f ? sy2 / py2 : 1.f) * (pz2 > 0.f ? sz2 / pz2 : 1.f);
+	s = make_float3(sqrtf(px2), sqrtf(py2), sqrtf(pz2));
+	return sqrtf(r);
+}
+
 // SH (degree <= 3) -> RGB for one Gaussian, all three channels; sh points at this Gaussian's
 // [M][3] coefficient row (forward.cu:20-71). Returns colour after +0.5 and clamp at 0; `clamp_bits`
 // bit c set when channel c was clamped.

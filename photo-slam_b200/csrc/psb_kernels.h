@@ -83,8 +83,10 @@ inline int sorted_slot(int width, int height)
 // tight: instance lists hold only the tiles a splat can reach (trainer path; see preprocess_fwd_kernel) — pass the same flag to launch_scan_binning
 // aa: anti-aliasing (the 2D Mip filter: the record holds o' = o h, see preprocess_fwd_kernel); pair it with the AA variant of the
 // per-Gaussian backward that follows
+// f3d [P] (raw only; null = off): the 3D smoothing filter (psb_filter3d) per row, see preprocess_fwd_kernel; pair it with the F3D variant of the
+// per-Gaussian backward that follows
 int launch_preprocess(const GaussIn& in, const Camera& cam, int* radii_out, const GeomState& geom, bool raw, bool tight, cudaStream_t stream,
-                      bool aa = false);
+                      bool aa = false, const float* f3d = nullptr);
 int launch_mark_visible(int P, const float* means3D, const float* view, uint8_t* present, cudaStream_t stream);
 int launch_depth_sort_and_scan(int P, GeomState& geom, bool scan, cudaStream_t stream);
 int launch_binning(int P, const Camera& cam, const GeomState& geom, BinState& bin, const ImgState& img, size_t n_host, cudaStream_t stream);

@@ -49,6 +49,9 @@ constexpr int MODE_AA = 16;        // OR'd into any of the above: the forward wa
 constexpr int MODE_REG = 32;       // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE (each optionally | MODE_DEPTH | MODE_AA), not MODE_PUSH: the opacity
                                    // and scale regularisers of 3DGS-MCMC (psb_trainer_set_regularizers) join the raw gradients of the rows the
                                    // pass reached: g_opacity += reg.opacity o (1 - o), g_scaling[c] += reg.scale s_c (reg = lambda / P)
+constexpr int MODE_F3D = 64;       // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE (each optionally | MODE_DEPTH | MODE_AA | MODE_REG), not MODE_PUSH:
+                                   // the forward applied the 3D smoothing filter f3d[idx] (preprocess_fwd_kernel<true, AA, true>): the covariance is
+                                   // rebuilt from s' = sqrt(s^2 + f^2), and the filter's opacity factor c joins the scale and opacity gradients
 
 // torch::optim::Adam single-tensor update (LibTorch adam.cpp): exp_avg.mul_(b1).add_(g, 1-b1);
 // exp_avg_sq.mul_(b2).addcmul_(g, g, 1-b2); denom = exp_avg_sq.sqrt()/sqrt(bc2) + eps; p.addcdiv_(exp_avg, denom, -lr/bc1).
@@ -171,16 +174,23 @@ __device__ __forceinline__ void adam_small(SmallRow& p, SmallRow& m, SmallRow& v
 //
 // MODE_REG: `reg` is read by these instantiations only. The regularisers touch exactly the rows that have a gradient anyway (`reached`), so
 // the dirty / live decisions and the memory traffic are those of the variant without it.
+//
+// MODE_F3D: `f3d` is read by these instantiations only, for the rows whose backward runs. With dL/ds' from the covariance chain and
+// g = dL/d(o c) (slot 7, times h under AA): dL/ds_c = dL/ds'_c s_c / s'_c + o c g f^2 / (s_c s'_c^2) and dL/do = c g. The regularisers, the
+// densification statistics and dL/dmean2D keep the unfiltered activations.
 template <int MODE>
 __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int first, int P, TrainTensors t, Camera cam, GeomState geom, float4* __restrict__ sink,
                                                             StepHyper h, GradSegments grads, DensifyStats st,
                                                             const uint32_t* __restrict__ counters, uint32_t capacity, float4* __restrict__ seeds,
-                                                            DpPush dp, unsigned char* __restrict__ adam_live, RegCoef reg)
+                                                            DpPush dp, unsigned char* __restrict__ adam_live, RegCoef reg,
+                                                            const float* __restrict__ f3d)
 {
 	constexpr bool DEPTH = (MODE & MODE_DEPTH) != 0;
 	constexpr bool AA = (MODE & MODE_AA) != 0;
 	constexpr bool REG = (MODE & MODE_REG) != 0;
-	constexpr int BASE = MODE & ~(MODE_DEPTH | MODE_AA | MODE_REG);
+	constexpr bool F3D = (MODE & MODE_F3D) != 0;
+	constexpr int BASE = MODE & ~(MODE_DEPTH | MODE_AA | MODE_REG | MODE_F3D);
+	static_assert(!F3D || BASE != MODE_PUSH, "no 3D filter on the NVLink step");
 	constexpr bool LIVE = BASE == MODE_ADAM_LIVE;
 	constexpr bool ADAM = BASE == MODE_ADAM || LIVE;
 	__shared__ __align__(128) float s_p[TB * REST];  // f_rest parameter rows of this block (TMA destination; LIVE: compacted per warp)
@@ -304,18 +314,32 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 			const float qn = fmaxf(sqrtf(qraw.x * qraw.x + qraw.y * qraw.y + qraw.z * qraw.z + qraw.w * qraw.w), 1e-12f);
 			const float4 q = make_float4(qraw.x / qn, qraw.y / qn, qraw.z / qn, qraw.w / qn);
 			const float sig = 1.0f / (1.0f + expf(-oraw));
+			float3 sf = s;  // F3D: s', the scale the forward drew
+			float f2 = 0.f, f3d_c = 1.f;
+			if (F3D) {
+				const float f = f3d[idx];
+				f2 = f * f;
+				f3d_c = filter3d_widen(sf, f);
+			}
 			float cov3D[6], dL_dcov[6];
-			cov3d_from_scale_rot(s, 1.0f, q, cov3D);
-			float aa_h = 1.f;  // AA: dL/dh = sigma dL/do'
-			gaussian_backward_geom<AA>(cam, mean, cov3D, dL_dmean2D, dL_dconic, g_xyz, dL_dcov, sig, dL_dopacity, false, &aa_h);
+			cov3d_from_scale_rot(sf, 1.0f, q, cov3D);
+			float aa_h = 1.f;  // AA: dL/dh = o c dL/do'
+			gaussian_backward_geom<AA>(cam, mean, cov3D, dL_dmean2D, dL_dconic, g_xyz, dL_dcov, F3D ? sig * f3d_c : sig, dL_dopacity, false, &aa_h);
 			float3 dL_dscale;
 			float4 dL_drot;
-			cov3d_backward(s, 1.0f, q, dL_dcov, dL_dscale, dL_drot);
+			cov3d_backward(sf, 1.0f, q, dL_dcov, dL_dscale, dL_drot);
+			if (F3D && f2 > 0.f) {  // (f = 0: s' = s and c = 1, nothing to add)
+				const float k = sig * f3d_c * (AA ? aa_h * dL_dopacity : dL_dopacity) * f2;   // o c dL/d(o c) f^2
+				dL_dscale.x = dL_dscale.x * (s.x / sf.x) + (k != 0.f ? k / (s.x * sf.x * sf.x) : 0.f);
+				dL_dscale.y = dL_dscale.y * (s.y / sf.y) + (k != 0.f ? k / (s.y * sf.y * sf.y) : 0.f);
+				dL_dscale.z = dL_dscale.z * (s.z / sf.z) + (k != 0.f ? k / (s.z * sf.z * sf.z) : 0.f);
+			}
 			// autograd of the activations (src/gaussian_model.cpp:48-71): exp, normalize, sigmoid
 			g_scale = make_float3(dL_dscale.x * s.x, dL_dscale.y * s.y, dL_dscale.z * s.z);
 			const float qd = q.x * dL_drot.x + q.y * dL_drot.y + q.z * dL_drot.z + q.w * dL_drot.w;
 			g_rot = make_float4((dL_drot.x - q.x * qd) / qn, (dL_drot.y - q.y * qd) / qn, (dL_drot.z - q.z * qd) / qn, (dL_drot.w - q.w * qd) / qn);
-			g_opac = (AA ? aa_h * dL_dopacity : dL_dopacity) * sig * (1.0f - sig);
+			// dL/do = c dL/d(o c); c sits at the leaf so that f = 0 (c = 1) rounds and contracts exactly like the variant without F3D
+			g_opac = (AA ? aa_h * dL_dopacity : dL_dopacity) * (F3D ? f3d_c : 1.0f) * sig * (1.0f - sig);
 			if (DEPTH) {  // z = V[2] x + V[6] y + V[10] z + V[14] (column-major view matrix)
 				const float dz = s2.w;
 				g_xyz.x += dz * cam.view[2]; g_xyz.y += dz * cam.view[6]; g_xyz.z += dz * cam.view[10];
@@ -692,17 +716,18 @@ void run_gaussian_backward(int first, int P, cudaStream_t stream, Args... args)
 }
 
 // Gaussians [first, P) in mode `mode` (MODE_GRADS, MODE_ADAM, MODE_ADAM_LIVE or MODE_PUSH, each optionally | MODE_DEPTH and | MODE_AA; all but
-// MODE_PUSH optionally | MODE_REG)
+// MODE_PUSH optionally | MODE_REG and | MODE_F3D)
 int launch_gaussian_backward(int mode, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink,
                              const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
-                             float* seeds, const DpPush& dp, unsigned char* adam_live, cudaStream_t stream, const RegCoef& reg)
+                             float* seeds, const DpPush& dp, unsigned char* adam_live, cudaStream_t stream, const RegCoef& reg, const float* f3d)
 {
 	if (P - first <= 0) return 0;
 	float4* sink4 = reinterpret_cast<float4*>(sink);
 	float4* seeds4 = reinterpret_cast<float4*>(seeds);
 #define PSB_BACKWARD_CASE(M) \
-	case M: run_gaussian_backward<M>(first, P, stream, t, cam, geom, sink4, h, grads, st, counters, capacity, seeds4, dp, adam_live, reg); break
-#define PSB_BACKWARD_CASE_REG(M) PSB_BACKWARD_CASE(M); PSB_BACKWARD_CASE(M | MODE_REG)
+	case M: run_gaussian_backward<M>(first, P, stream, t, cam, geom, sink4, h, grads, st, counters, capacity, seeds4, dp, adam_live, reg, f3d); break
+#define PSB_BACKWARD_CASE_F3D(M) PSB_BACKWARD_CASE(M); PSB_BACKWARD_CASE(M | MODE_F3D)
+#define PSB_BACKWARD_CASE_REG(M) PSB_BACKWARD_CASE_F3D(M); PSB_BACKWARD_CASE_F3D(M | MODE_REG)
 	switch (mode) {
 		PSB_BACKWARD_CASE_REG(MODE_GRADS);
 		PSB_BACKWARD_CASE_REG(MODE_ADAM);
@@ -723,6 +748,7 @@ int launch_gaussian_backward(int mode, int first, int P, const TrainTensors& t, 
 		default: set_error_msg("launch_gaussian_backward: unknown mode"); return -1;
 	}
 #undef PSB_BACKWARD_CASE_REG
+#undef PSB_BACKWARD_CASE_F3D
 #undef PSB_BACKWARD_CASE
 	PSB_LAUNCH_OK();
 	return 0;
@@ -754,9 +780,10 @@ int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, co
 	memset(&nodp, 0, sizeof(nodp));
 	unsigned char* live = adam ? adam_live : nullptr;
 	const int variant = (live ? MODE_ADAM_LIVE : adam ? MODE_ADAM : MODE_GRADS) | (mode.depth ? MODE_DEPTH : 0) | (mode.aa ? MODE_AA : 0) |
-	                    (reg.opacity != 0.f || reg.scale != 0.f ? MODE_REG : 0);
+	                    (reg.opacity != 0.f || reg.scale != 0.f ? MODE_REG : 0) | (mode.f3d ? MODE_F3D : 0);
 	int rc;
-	if ((rc = launch_gaussian_backward(variant, first, P, t, cam, geom, sink, h, grads, st, counters, capacity, seeds, nodp, live, stream, reg))) return rc;
+	if ((rc = launch_gaussian_backward(variant, first, P, t, cam, geom, sink, h, grads, st, counters, capacity, seeds, nodp, live, stream, reg, mode.f3d)))
+		return rc;
 	if (between) cudaEventRecord(between, stream);
 	const AdamCoef ac(h);
 	const uint32_t e0 = (uint32_t)first * REST, e1 = (uint32_t)P * REST;
@@ -781,8 +808,9 @@ int launch_push_backward(int P, const TrainTensors& t, const Camera& cam, const 
 {
 	const GradSegments nog = {};
 	int rc;
+	if (mode.f3d) { set_error_msg("launch_push_backward: the 3D filter is not wired into the NVLink step"); return -1; }
 	if ((rc = launch_gaussian_backward(MODE_PUSH | (mode.depth ? MODE_DEPTH : 0) | (mode.aa ? MODE_AA : 0), 0, P, t, cam, geom, sink, h, nog, st, counters, capacity, nullptr, dp,
-	                                   nullptr, stream, RegCoef{0.f, 0.f})))
+	                                   nullptr, stream, RegCoef{0.f, 0.f}, nullptr)))
 		return rc;
 	return launch_signal(dp.grad_flag, dp.meta, cam.campos, h.D, dp.world, dp.rank, dp.epoch, stream);
 }

@@ -35,6 +35,7 @@ struct PassMode {
 	bool aa;     // the forward was anti-aliased (launch_preprocess aa): slot 7 of the sink rows holds dL/do'
 	bool depth;  // the sink rows carry dL/dz in slot 11 (render_bwd_kernel<true, ...>)
 	float reg_opacity, reg_scale;  // psb_trainer_set_regularizers: lambda_opacity, lambda_scale (both 0: the variants without MODE_REG)
+	const float* f3d;              // psb_trainer_set_filter3d: the 3D smoothing filter [P] the pass applies, or null (the variants without it)
 };
 // lambda / P of the opacity and scale regularisers for the rows a per-Gaussian backward updates; both 0 = no regulariser
 struct RegCoef {

@@ -30,12 +30,16 @@ struct psb_trainer {
 	uint32_t seq = 0;            // sequence number of the last forward pass (render / step / backward) of this context
 	// the mode of pass `seq`: what psb_trainer_backward_pixels must match, and the variant every per-Gaussian stage behind it runs
 	// (a psb_trainer_backward_begin* records it before its pass, so the _slab calls after it run that variant even if it failed)
-	PassMode pass = {-1, false, false, false, 0.f, 0.f};
+	PassMode pass = {-1, false, false, false, 0.f, 0.f, nullptr};
 	// anti-aliasing (psb_trainer_set_antialiasing): every forward pass blends with o' = o h (the 2D Mip filter), and every per-Gaussian
 	// backward behind it runs the AA variant
 	bool antialiasing = false;
 	// opacity / scale regularisers (psb_trainer_set_regularizers): recorded in the mode of every pass that starts while they are set
 	float reg_opacity = 0.f, reg_scale = 0.f;
+	// 3D smoothing filter (psb_trainer_set_filter3d): the caller's [filter3d_P] device array, recorded in the mode of every pass that starts
+	// while it is set; null = off
+	const float* filter3d = nullptr;
+	int filter3d_P = 0;
 	uint32_t ovf_first = 0, ovf_count = 0;  // what the last PSB_ERR_RETRY was about (psb_trainer_overflow_info)
 	cudaEvent_t readback = nullptr;  // recorded once the instance count (and the loss sums) of the last call are in pinned memory
 	int last_P = 0, last_W = 0, last_H = 0;
@@ -266,8 +270,31 @@ int check_grads(float* const* grads, int P, const char* fn)
 	return 0;
 }
 
-// The mode of a pass that starts now, in the context's deterministic and anti-aliasing modes.
-PassMode pass_mode(const psb_trainer* t, int D, bool depth) { return {D, t->deterministic, t->antialiasing, depth, t->reg_opacity, t->reg_scale}; }
+// The mode of a pass that starts now, in the context's deterministic, anti-aliasing, regulariser and 3D-filter modes.
+PassMode pass_mode(const psb_trainer* t, int D, bool depth)
+{
+	return {D, t->deterministic, t->antialiasing, depth, t->reg_opacity, t->reg_scale, t->filter3d};
+}
+
+// A pass over P rows while a 3D filter is set must be over the filter's rows.
+int check_filter3d(const psb_trainer* t, int P, const char* fn)
+{
+	if (t->filter3d && P != t->filter3d_P) {
+		set_error_msg(std::string(fn).append(": the 3D filter set with psb_trainer_set_filter3d has a different row count than P").c_str());
+		return PSB_ERR_ARG;
+	}
+	return 0;
+}
+
+// The NVLink and slab-pipelined data-parallel calls take no 3D filter.
+int refuse_filter3d(const psb_trainer* t, const char* fn)
+{
+	if (t && t->filter3d) {
+		set_error_msg(std::string(fn).append(": the 3D filter is not wired into the data-parallel steps; psb_trainer_set_filter3d(t, NULL, 0) first").c_str());
+		return PSB_ERR_ARG;
+	}
+	return 0;
+}
 
 // Stage 1 of every pass: forward of SH degree D from raw parameters into t->image (or out_color); out_depth != NULL: the depth variant
 // also writes the expected depth there; out_alpha != NULL: the opacity variant also writes 1 - final_T there. The pass is recorded as
@@ -286,7 +313,7 @@ int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, con
 	ImgState& img = sc.img;
 	const GaussIn in = raw_input(P, D, M, model);
 	t->mark(0, stream);
-	if ((rc = launch_preprocess(in, cam, radii, geom, /*raw=*/true, t->tight, stream, mode.aa))) return rc;
+	if ((rc = launch_preprocess(in, cam, radii, geom, /*raw=*/true, t->tight, stream, mode.aa, mode.f3d))) return rc;
 	t->mark(1, stream);
 	if ((rc = launch_depth_sort_and_scan(P, geom, /*scan=*/false, stream))) return rc;
 	t->mark(2, stream);
@@ -350,6 +377,7 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	int rc;
 	if (!t || !camera || !step || !background || !gt_image) { set_error_msg("psb_trainer_step: null argument"); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, moments))) return rc;
+	if ((rc = check_filter3d(t, P, "psb_trainer_step"))) return rc;
 	if (step->sh_degree < 0 || step->sh_degree > 3 || step->step < 1) { set_error_msg("psb_trainer_step: sh_degree in 0..3 and step >= 1 required"); return PSB_ERR_ARG; }
 	// depth loss: the depth plane is the caller's out_depth or the context's own; dL/dD lives in the context
 	const bool depth_loss = depth && depth->gt_depth;
@@ -528,6 +556,7 @@ int psb_dp_step_depth(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* 
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
 	if ((rc = check_depth(depth, "psb_dp_step_depth"))) return rc;
+	if ((rc = refuse_filter3d(t, "psb_dp_step_depth"))) return rc;
 	if (!d || !d->connected || P != d->P || !model) { set_error_msg("psb_dp_step: context not connected or built for a different P"); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, true))) return rc;
 	for (int i = 0; i < 6; i++)
@@ -611,6 +640,7 @@ static int forward_impl(const char* fn, psb_trainer* t, int P, int M, const psb_
 	int rc;
 	if (!t || !camera || !background || !out_color) { set_error_msg(std::string(fn).append(": null argument").c_str()); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, false))) return rc;
+	if ((rc = check_filter3d(t, P, fn))) return rc;
 	Scratch sc;
 	Camera cam;
 	t->have_loss = false;
@@ -664,6 +694,10 @@ int psb_trainer_backward_pixels(psb_trainer* t, unsigned pass, int P, int M, con
 	}
 	if (t->pass.aa != t->antialiasing) {
 		set_error_msg("psb_trainer_backward_pixels: the anti-aliasing mode changed since the forward pass");
+		return PSB_ERR_ARG;
+	}
+	if (t->pass.f3d != t->filter3d) {
+		set_error_msg("psb_trainer_backward_pixels: the 3D filter changed since the forward pass");
 		return PSB_ERR_ARG;
 	}
 	if (step->step < 1) { set_error_msg("psb_trainer_backward_pixels: step >= 1 required"); return PSB_ERR_ARG; }
@@ -769,6 +803,7 @@ int psb_trainer_backward_begin_depth(psb_trainer* t, int P, int M, const psb_mod
 {
 	int rc;
 	if ((rc = check_depth(depth, "psb_trainer_backward_begin_depth"))) return rc;
+	if ((rc = refuse_filter3d(t, "psb_trainer_backward_begin_depth"))) return rc;
 	// recorded whether or not the call below succeeds: the depth variant of _slab gives the plain result on rows without dL/dz
 	if (t) t->pass = pass_mode(t, -1, depth && depth->gt_depth);
 	TileBackward tb;
@@ -788,6 +823,7 @@ int psb_trainer_backward_slab(psb_trainer* t, int P, int M, const psb_model* mod
 	int rc;
 	if (!t || !camera || !step || !grads || t->geom_P != P) { set_error_msg("psb_trainer_backward_slab: bad argument / no matching backward_begin"); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, false))) return rc;
+	if ((rc = refuse_filter3d(t, "psb_trainer_backward_slab"))) return rc;
 	if (first < 0 || count < 0 || first + count > P || (first % 128) != 0) { set_error_msg("psb_trainer_backward_slab: slab must start at a multiple of 128"); return PSB_ERR_ARG; }
 	if (count == 0) return 0;
 	if ((rc = check_grads(grads, count, "psb_trainer_backward_slab"))) return rc;
@@ -947,6 +983,14 @@ int psb_trainer_set_regularizers(psb_trainer* t, float lambda_opacity, float lam
 		return PSB_ERR_ARG;
 	}
 	t->reg_opacity = lambda_opacity; t->reg_scale = lambda_scale;   // (take effect at the next pass)
+	return 0;
+}
+
+int psb_trainer_set_filter3d(psb_trainer* t, const float* filter, int P)
+{
+	if (!t || (filter && P < 0)) { set_error_msg("psb_trainer_set_filter3d: a context, and P >= 0 with a filter"); return PSB_ERR_ARG; }
+	t->filter3d = filter;   // (takes effect at the next pass)
+	t->filter3d_P = filter ? P : 0;
 	return 0;
 }
 

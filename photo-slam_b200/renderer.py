@@ -24,10 +24,13 @@ from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer
 @dataclass
 class GaussianPipelineParams:
     """reference include/gaussian_parameters.h:38-47 (all shipped configs: both False), plus `antialiasing`: the rasterizer's 2D Mip
-    filter (GaussianRasterizationSettings.antialiasing) in every branch below; off by default"""
+    filter (GaussianRasterizationSettings.antialiasing) in every branch below, and `filter_3d`: the model's 3D smoothing filter
+    (GaussianModel.computeFilter3D; scale s' and opacity o' of getScalingWithFilter3D / getOpacityWithFilter3D) in every branch below;
+    both off by default"""
     convert_SHs: bool = False
     compute_cov3D: bool = False
     antialiasing: bool = False
+    filter_3d: bool = False
 
 
 def build_rotation(r):
@@ -46,10 +49,11 @@ def get_features(model):
     return torch.cat((model.features_dc_, model.features_rest_), dim=1)
 
 
-def get_covariance_activation(model, scaling_modifier=1.0):
-    """GaussianModel::getCovarianceActivation (gaussian_model.cpp:73-101): L = R diag(s), Sigma = L L^T, upper triangle [P, 6]"""
+def get_covariance_activation(model, scaling_modifier=1.0, scales=None):
+    """GaussianModel::getCovarianceActivation (gaussian_model.cpp:73-101): L = R diag(s), Sigma = L L^T, upper triangle [P, 6];
+    scales: the activated scales to use instead of exp(scaling_) (the 3D filter's s')"""
     R = build_rotation(model.rotation_)
-    s = scaling_modifier * torch.exp(model.scaling_)
+    s = scaling_modifier * (torch.exp(model.scaling_) if scales is None else scales)
     Lm = R * s.unsqueeze(1)                    # R @ diag(s)
     cov = Lm @ Lm.transpose(1, 2)
     return torch.stack((cov[:, 0, 0], cov[:, 0, 1], cov[:, 0, 2], cov[:, 1, 1], cov[:, 1, 2], cov[:, 2, 2]), dim=1)
@@ -71,12 +75,13 @@ def render(viewpoint_camera, image_height, image_width, pc, pipe=None, bg_color=
                                              int(pc.active_sh_degree_), viewpoint_camera["campos"], False, bool(pipe.antialiasing))
     rasterizer = GaussianRasterizer(settings)
     means3D, means2D = pc.xyz_, screenspace_points
-    opacity = torch.sigmoid(pc.opacity_)
+    opacity = pc.getOpacityWithFilter3D() if pipe.filter_3d else torch.sigmoid(pc.opacity_)
+    activated_scales = pc.getScalingWithFilter3D() if pipe.filter_3d else torch.exp(pc.scaling_)
     scales = rotations = cov3D_precomp = None
     if pipe.compute_cov3D:
-        cov3D_precomp = get_covariance_activation(pc, scaling_modifier)
+        cov3D_precomp = get_covariance_activation(pc, scaling_modifier, activated_scales)
     else:
-        scales = torch.exp(pc.scaling_)
+        scales = activated_scales
         rotations = torch.nn.functional.normalize(pc.rotation_)
     shs = colors_precomp = None
     if use_override_color:

@@ -123,6 +123,8 @@ def _bind():
         "psb_trainer_set_deterministic": [vp, i],
         "psb_trainer_set_antialiasing": [vp, i],
         "psb_trainer_set_regularizers": [vp, f, f],
+        "psb_trainer_set_filter3d": [vp, vp, i],
+        "psb_filter3d": [i, vp, i, vp, vp, P(i), vp],
         "psb_trainer_inject_noise": [vp, i, Model, f, f, ull, ull, i, vp],
         "psb_adam_update": [i, i, Model, P(vp), Step, f, vp],
         "psb_adam_flat": [size_t, vp, vp, vp, vp, f, Step, f, vp],
@@ -205,6 +207,8 @@ class GaussianModel:
         # own Adam step count (advanced on the device by the fused step)
         self.exposure_, self.exposure_exp_avg_, self.exposure_exp_avg_sq_ = z(0, 3, 4), z(0, 3, 4), z(0, 3, 4)
         self.exposure_step_ = z(0, dtype=torch.int32)
+        # 3D smoothing filter (computeFilter3D): [P] float32, or None when it has not been computed for the current rows
+        self.filter_3D_ = None
 
     @classmethod
     def from_numpy(cls, scene, device="cuda", sh_degree=3):
@@ -250,7 +254,8 @@ class GaussianModel:
         return dict(p=c(self.tensors()), m=c(self.exp_avg_), v=c(self.exp_avg_sq_),
                     stats=c([self.xyz_gradient_accum_, self.denom_, self.max_radii2D_]), step=self.step_, lr=list(self.lr_),
                     sh=self.active_sh_degree_, live=live.clone(), live_valid=self.adam_live_valid_,
-                    exposure=c(self._exposure_tensors()), exposure_lr=self.exposure_lr_)
+                    exposure=c(self._exposure_tensors()), exposure_lr=self.exposure_lr_,
+                    filter_3D=self.filter_3D_.clone() if self.filter_3D_ is not None else None)
 
     def restore(self, snap):
         assert snap["p"][0].shape == self.xyz_.shape, "restore: the model was resized since the snapshot"
@@ -266,6 +271,11 @@ class GaussianModel:
         else:   # the table grew since the snapshot
             self.exposure_, self.exposure_exp_avg_, self.exposure_exp_avg_sq_, self.exposure_step_ = [t.clone() for t in snap["exposure"]]
         self.exposure_lr_ = snap["exposure_lr"]
+        f = snap["filter_3D"]
+        if f is not None and self.filter_3D_ is not None and self.filter_3D_.shape == f.shape:
+            self.filter_3D_.copy_(f)
+        else:
+            self.filter_3D_ = f.clone() if f is not None else None
 
     def _live_tensor(self):
         """adam_live_, (re)allocated when the row count changed (its content is then stale)."""
@@ -335,10 +345,67 @@ class GaussianModel:
             self.adam_live_valid_ = True
         return live
 
+    # --- 3D smoothing filter (Mip-Splatting; include/psb200.h, psb_filter3d): every Gaussian is widened to at least the finest sampling
+    #     interval at which a keyframe saw it. computeFilter3D computes it; GaussianTrainer(filter3d=True) and
+    #     renderer.render(pipe=GaussianPipelineParams(filter_3d=True)) apply it. Every method that changes which row is which, or the map's
+    #     spatial scale, drops it (filter_3D_ = None): recompute it after densification, as Mip-Splatting does (and every ~100 iterations).
+    def computeFilter3D(self, cams):
+        """cams: camera dicts in the form GaussianTrainer takes (viewmatrix: 16 floats; tanfovx, tanfovy, W, H), the full-resolution keyframes.
+        Sets filter_3D_ [P] (psb_filter3d) and returns the number of rows at least one camera sees (one host round trip)."""
+        rows = []
+        for k, cam in enumerate(cams):
+            try:
+                view = torch.as_tensor(cam["viewmatrix"]).detach().to("cpu", torch.float64).reshape(-1)
+                tx, ty, W, H = float(cam["tanfovx"]), float(cam["tanfovy"]), cam["W"], cam["H"]
+            except (KeyError, TypeError, ValueError, RuntimeError) as e:
+                raise ValueError(f"computeFilter3D: camera {k} is not a camera dict (viewmatrix, tanfovx, tanfovy, W, H): {e}") from None
+            if view.numel() != 16 or not bool(torch.isfinite(view).all()):
+                raise ValueError(f"computeFilter3D: camera {k}: viewmatrix must hold 16 finite values")
+            if int(W) != W or int(H) != H or W <= 0 or H <= 0:
+                raise ValueError(f"computeFilter3D: camera {k}: W and H must be positive integers, got {W}, {H}")
+            fx, fy = W / (2.0 * tx) if tx else math.inf, H / (2.0 * ty) if ty else math.inf
+            if not (math.isfinite(tx) and math.isfinite(ty) and tx > 0 and ty > 0 and math.isfinite(fx) and math.isfinite(fy)):
+                raise ValueError(f"computeFilter3D: camera {k}: tanfovx and tanfovy must be finite and positive, got {tx}, {ty}")
+            rows.append(torch.cat([view, torch.tensor([fx, fy, float(W), float(H)], dtype=torch.float64)]))
+        packed = (torch.stack(rows) if rows else torch.zeros((0, 20), dtype=torch.float64)).to(self.device, torch.float32).contiguous()
+        P = self.num_points()
+        f = torch.empty(P, dtype=torch.float32, device=self.device)
+        seen = C.c_int()
+        _lib.check(_bind().psb_filter3d(P, self.xyz_.data_ptr() if P else None, len(rows), packed.data_ptr() if rows else None,
+                                        f.data_ptr() if P else None, C.byref(seen), torch.cuda.current_stream().cuda_stream), "psb_filter3d")
+        self.filter_3D_ = f
+        return seen.value
+
+    def filter3D(self):
+        """filter_3D_, checked to belong to the current rows (ValueError otherwise)."""
+        f = self.filter_3D_
+        if f is None or tuple(f.shape) != (self.num_points(),):
+            raise ValueError("the 3D filter is missing or stale (the rows changed since it was computed): call computeFilter3D(cams)")
+        return f
+
+    def getScalingWithFilter3D(self):
+        """s' = sqrt(s^2 + f^2) per axis (differentiable w.r.t. scaling_)"""
+        s = torch.exp(self.scaling_)
+        return torch.sqrt(s * s + self.filter3D().square().unsqueeze(1))
+
+    def getOpacityWithFilter3D(self):
+        """o' = o sqrt(prod s^2 / prod s'^2) (differentiable w.r.t. opacity_ and scaling_)"""
+        s2 = torch.exp(self.scaling_).square()
+        c = torch.sqrt((s2 / (s2 + self.filter3D().square().unsqueeze(1))).prod(dim=1, keepdim=True))
+        return torch.sigmoid(self.opacity_) * c
+
     # --- on-disk point cloud (reference GaussianModel::savePly / loadPly / saveSparsePointsPly, gaussian_model.cpp:838-1088)
-    def savePly(self, path):
+    def savePly(self, path, fuse_filter3d=False):
+        """fuse_filter3d=True writes log s' and logit(o') of the 3D filter instead of the raw scaling and opacity (Mip-Splatting's fused
+        export): any standard 3DGS viewer then draws what the trainer draws with the filter on."""
         from . import io
-        io.save_ply(path, *[t.detach().cpu().numpy() for t in self.tensors()])
+        ts = self.tensors()
+        if fuse_filter3d:
+            with torch.no_grad():
+                ts = list(ts)
+                ts[3] = torch.logit(self.getOpacityWithFilter3D())
+                ts[4] = torch.log(self.getScalingWithFilter3D())
+        io.save_ply(path, *[t.detach().cpu().numpy() for t in ts])
 
     def loadPly(self, path):
         """Replaces the parameter tensors by the file's content and activates every SH degree (gaussian_model.cpp:951)."""
@@ -348,6 +415,7 @@ class GaussianModel:
         self._set([t(a[k]) for k in ("xyz", "features_dc", "features_rest", "opacity", "scaling", "rotation")])
         self.active_sh_degree_ = self.max_sh_degree_
         self.invalidateAdamLive()
+        self.filter_3D_ = None
 
     def setSparsePoints(self, xyz, color):
         """sparse SLAM map points + colours in [0,1] kept for input.ply (reference gaussian_model.cpp: sparse_points_xyz_ / _color_)"""
@@ -425,6 +493,7 @@ class GaussianModel:
         self.exp_avg_, self.exp_avg_sq_ = d["m"], d["v"]
         self.xyz_gradient_accum_, self.denom_, self.max_radii2D_, self.exist_since_iter_ = d["accum"], d["denom"], d["max_radii"], d["exist"]
         self.invalidateAdamLive()   # rows moved: rebuilt from the new moments before the next fused step
+        self.filter_3D_ = None
 
     def resetOpacity(self):
         """reference gaussian_model.cpp:556-565. NOTE: the reference's misplaced parenthesis makes this
@@ -495,6 +564,7 @@ class GaussianModel:
                                   torch.cuda.current_stream().cuda_stream), "psb_relocate")
         if u is not None:
             assert u.numel() >= counts[1], (u.numel(), counts[1])
+        self.filter_3D_ = None
         return counts[0]
 
     def addNewGaussians(self, cap_max, grow_factor=1.05, min_opacity=0.005, seed=0, offset=None, iteration=0, uniforms=None):
@@ -562,6 +632,7 @@ class GaussianModel:
     def scaledTransformationPostfix(self, new_xyz, new_scaling):
         """:403-418: the two tensors replace xyz / scaling in the optimizer with FRESH (zero) moments (replaceTensorToOptimizer :567-586)"""
         self.xyz_, self.scaling_ = new_xyz.contiguous(), new_scaling.contiguous()
+        self.filter_3D_ = None
         for i in (0, 4):
             self.exp_avg_[i] = torch.zeros_like(self.tensors()[i])
             self.exp_avg_sq_[i] = torch.zeros_like(self.tensors()[i])
@@ -586,6 +657,7 @@ class GaussianModel:
         num_transformed = scaleAndTransformThenMarkVisiblePoints(points, rots, point_not_transformed_flags, unstable, diff_pose,
                                                                  kf_world_view_transform, kf_full_proj_transform, num_transformed, scale)
         self.xyz_, self.rotation_ = points.contiguous(), rots.contiguous()
+        self.filter_3D_ = None
         for i in (0, 5):
             self.exp_avg_[i] = torch.zeros_like(self.tensors()[i])
             self.exp_avg_sq_[i] = torch.zeros_like(self.tensors()[i])
@@ -632,9 +704,15 @@ class GaussianTrainer:
     (opt.opacity_reg, opt.scale_reg; psb_trainer_set_regularizers: on the rows the step updates), trainForOneIteration and
     trainWithLoss enqueue the position noise behind the step (psb_trainer_inject_noise, keyed by opt.mcmc_seed and model.step_), and
     mcmcRefine() replaces densifyAndPrune: it relocates the dead Gaussians and grows the map by opt.mcmc_grow_factor up to
-    opt.cap_max. With mcmc off nothing of this is launched."""
+    opt.cap_max. With mcmc off nothing of this is launched.
 
-    def __init__(self, model: GaussianModel, opt: GaussianOptimizationParams = None, background=None, deterministic=None, antialiasing=False):
+    filter3d: True applies the model's 3D smoothing filter (model.computeFilter3D; psb_trainer_set_filter3d) in every render and training call,
+    as renderer.render(pipe=GaussianPipelineParams(filter_3d=True)) does on the operator path. Each call hands over model.filter_3D_ as it is
+    then; a missing or stale filter raises ValueError. Recomputing it is the caller's choice (Mip-Splatting: after each densification and
+    every 100 iterations). Fixed for the trainer's lifetime."""
+
+    def __init__(self, model: GaussianModel, opt: GaussianOptimizationParams = None, background=None, deterministic=None, antialiasing=False,
+                 filter3d=False):
         self.L = _bind()
         self.model = model
         self.opt = opt or GaussianOptimizationParams()
@@ -653,6 +731,18 @@ class GaussianTrainer:
         if self.opt.mcmc:
             _lib.check(self.L.psb_trainer_set_regularizers(self.h, float(self.opt.opacity_reg), float(self.opt.scale_reg)),
                        "psb_trainer_set_regularizers")
+        self._filter3d = bool(filter3d)
+
+    def _hand_filter3d(self):
+        """filter3d: the context takes model.filter_3D_ as it is now (ValueError when it is missing or stale)."""
+        if self._filter3d:
+            f = self.model.filter3D()
+            _lib.check(self.L.psb_trainer_set_filter3d(self.h, f.data_ptr(), self.model.num_points()), "psb_trainer_set_filter3d")
+
+    @property
+    def filter3d(self):
+        """Whether this trainer's calls apply the model's 3D filter (set at construction)."""
+        return self._filter3d
 
     def _inject_noise(self):
         """opt.mcmc: the position noise behind the step just enqueued (a no-op on the device if that step's pass overflowed)."""
@@ -720,6 +810,7 @@ class GaussianTrainer:
         out = out if out is not None else torch.empty((3, cam["H"], cam["W"]), device=m.device)
         for t in (out_depth, out_alpha):
             assert t is None or (t.is_contiguous() and t.dtype == torch.float32 and t.numel() == cam["H"] * cam["W"])
+        self._hand_filter3d()
         cm, cc = m._cmodel(False), _ccamera(cam)
         pass_no = C.c_uint()
         _lib.check(self.L.psb_trainer_forward(self.h, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(), m.active_sh_degree_,
@@ -760,6 +851,7 @@ class GaussianTrainer:
             for name, g, p in zip(GROUPS, grads, m.tensors()):
                 _plane(g, p.shape, "grads[" + name + "]")
         adam = grads is None
+        self._hand_filter3d()
         if adam:
             self.iteration += 1
         if densify_stats is None:
@@ -829,6 +921,7 @@ class GaussianTrainer:
             m.ensureExposures(k + 1)
             exposure = _Exposure(m.exposure_[k].data_ptr(), m.exposure_exp_avg_[k].data_ptr(), m.exposure_exp_avg_sq_[k].data_ptr(),
                                  m.exposure_step_[k:].data_ptr(), float(m.exposure_lr_))
+        self._hand_filter3d()
         self._apply_deterministic()
         self.iteration += 1
         if densify_stats is None:
@@ -980,7 +1073,10 @@ class DataParallelTrainer(GaussianTrainer):
     antialiasing: as in GaussianTrainer, in every mode. Every rank must pass the same value."""
 
     def __init__(self, model, opt=None, background=None, group=None, pipeline=None, nslabs=4, mode=None, deterministic=None,
-                 antialiasing=False):
+                 antialiasing=False, filter3d=False):
+        if filter3d:
+            raise NotImplementedError("DataParallelTrainer: the 3D filter is not wired into the data-parallel steps (the NVLink push backward and "
+                                      "the slab pipeline have no filtered variant); train with it on one GPU through GaussianTrainer(filter3d=True)")
         if opt is not None and opt.mcmc:
             raise NotImplementedError("DataParallelTrainer: opt.mcmc is not wired into the data-parallel steps (the owner-side Adam would need the "
                                       "regularisers, every rank the noise, and a refinement gather_moments() first); train with it on one GPU "
