@@ -552,6 +552,8 @@ int psb_insert_points(int P, const psb_model* src, const psb_model* dst, int n, 
                       const float* dist2, int iteration, void* stream);
 /* GaussianModel::resetOpacity (src/gaussian_model.cpp:556-565, incl. its no-op clamp) + zeroed opacity moments, in place. */
 int psb_reset_opacity(int P, float* opacity, float* exp_avg, float* exp_avg_sq, void* stream);
+/* Every entry point above, from psb_densify_plan on, checks all of its arguments before its first CUDA call: a call that returns
+ * PSB_ERR_ARG has enqueued nothing and written no device memory. */
 
 /* ------------------------------------------------------------------------------------------------
  * Bounded-budget densification: relocation of dead Gaussians and growth to a cap (3DGS-MCMC, Kheradmand et al., NeurIPS 2024; the

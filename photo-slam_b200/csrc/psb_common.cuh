@@ -40,6 +40,16 @@ static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 // SMs of an H100 SXM: caps the grids of the grid-stride kernels at a few resident blocks per SM.
 constexpr int kNumSMs = 132;
 
+// Floats per Gaussian row of the six parameter tensors, in psb_model.param order: xyz, features_dc, features_rest (15 SH coefficients
+// x 3 channels: every entry point that moves rows or steps Adam requires all 16 coefficients), opacity, scaling, rotation. The Adam
+// moments have the same rows.
+__host__ __device__ constexpr int row_floats(int tensor)
+{
+	constexpr int k[6] = {3, 3, 45, 1, 3, 4};
+	return k[tensor];
+}
+constexpr int kRestFloats = row_floats(2);
+
 // ---------------------------------------------------------------------------------------------
 // Per-Gaussian screen-space record produced by the forward preprocess and consumed (as one
 // 48-byte bulk copy) by the tile kernels. 16-byte aligned, three float4 lanes:

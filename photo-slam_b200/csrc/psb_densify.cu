@@ -23,7 +23,7 @@
 //                           either injected (tests: same numbers as the oracle) or drawn from Philox4x32-10 + Box-Muller keyed by
 //                           (seed, offset, child row) — counter-based, so every data-parallel replica draws identical samples.
 #include <cmath>
-#include <cstring>
+#include <string>
 #include "psb_common.cuh"
 #include "../../include/psb200.h"
 
@@ -33,7 +33,6 @@ namespace {
 
 constexpr int DN_TB = 128;
 constexpr uint32_t F_ORIG = 1u, F_CLONE = 2u, F_CHILD = 4u, F_SPLIT = 8u;
-__host__ __device__ constexpr int dn_row(int ti) { return ti == 2 ? 45 : (ti == 3 ? 1 : (ti == 5 ? 4 : 3)); }  // floats per row of xyz, f_dc, f_rest, opacity, scaling, rotation
 
 struct DensifyCfg {
 	float tau, min_opacity, size_thr, ws_thr;
@@ -228,7 +227,7 @@ __global__ void __launch_bounds__(DN_TB) densify_scatter_kernel(int P, DensifyTe
 	const float inv = 1.0f / 1.6f;
 #pragma unroll
 	for (int ti = 0; ti < 6; ti++) {
-		const int k = dn_row(ti);
+		const int k = row_floats(ti);
 		const float* __restrict__ sp = t.p[ti] + (size_t)base * k;
 		const float* __restrict__ sm = t.m[ti] + (size_t)base * k;
 		const float* __restrict__ sv = t.v[ti] + (size_t)base * k;
@@ -302,7 +301,7 @@ __global__ void insert_fill_kernel(int P, int n, const float* __restrict__ point
 		t.dp[1][3 * d + c] = (colors[3 * (size_t)j + c] - 0.5f) / kSH_C0;   // RGB2SH
 		t.dp[4][3 * d + c] = sc;
 	}
-	for (int c = 0; c < 45; c++) t.dp[2][45 * d + c] = 0.f;
+	for (int c = 0; c < kRestFloats; c++) t.dp[2][kRestFloats * d + c] = 0.f;
 	t.dp[3][d] = op;
 	reinterpret_cast<float4*>(t.dp[5])[d] = make_float4(1.f, 0.f, 0.f, 0.f);
 	if (t.dexist) t.dexist[d] = iteration;
@@ -462,6 +461,7 @@ __global__ void __launch_bounds__(256) reloc_draw_kernel(int P, int n_host, cons
 	atomicAdd(&mult[lo], 1);
 }
 
+// a model's tensors as the row kernels take them (rows_of); relocate and grow write them in place
 struct RelocTensors {
 	float* p[6]; float* m[6]; float* v[6];
 	float* stat[3];            // max_radii2D, xyz_gradient_accum, denom (any may be null)
@@ -492,7 +492,7 @@ __global__ void __launch_bounds__(DN_TB) reloc_correct_kernel(int P, RelocTensor
 	__syncthreads();
 #pragma unroll
 	for (int ti = 0; ti < 6; ti++) {
-		const int k = dn_row(ti);
+		const int k = row_floats(ti);
 		float* __restrict__ dm = t.m[ti] + (size_t)base * k;
 		float* __restrict__ dv = t.v[ti] + (size_t)base * k;
 		for (int e = tid; e < rows * k; e += DN_TB)
@@ -536,7 +536,7 @@ __global__ void __launch_bounds__(DN_TB) reloc_copy_kernel(int n_targets, int tb
 	__syncthreads();
 #pragma unroll
 	for (int ti = 0; ti < 6; ti++) {
-		const int k = dn_row(ti);
+		const int k = row_floats(ti);
 		const size_t o = ((size_t)tbase + base) * k;
 		for (int e = tid; e < rows * k; e += DN_TB) {
 			const int r = e / k, s = s_src[r];
@@ -601,17 +601,42 @@ RelocWorkspace reloc_ws_carve(void* w, int P)
 	s.flags = reinterpret_cast<uint8_t*>(c);
 	return s;
 }
-// the tensors of a model that relocate / grow write; false when one of the 18 parameter / moment tensors is missing
-bool reloc_tensors(const psb_model* m, RelocTensors& t)
+// the tensors of a model (all null for a null model)
+RelocTensors rows_of(const psb_model* m)
 {
-	for (int i = 0; i < 6; i++) {
-		if (!m->param[i] || !m->exp_avg[i] || !m->exp_avg_sq[i]) return false;
-		t.p[i] = m->param[i]; t.m[i] = m->exp_avg[i]; t.v[i] = m->exp_avg_sq[i];
-	}
+	RelocTensors t = {};
+	if (!m) return t;
+	for (int i = 0; i < 6; i++) { t.p[i] = m->param[i]; t.m[i] = m->exp_avg[i]; t.v[i] = m->exp_avg_sq[i]; }
 	t.stat[0] = m->max_radii2D; t.stat[1] = m->xyz_gradient_accum; t.stat[2] = m->denom;
 	t.exist = m->exist_since_iter;
 	t.live = m->adam_live;
+	return t;
+}
+// all 18 parameter / moment tensors are given
+bool has_rows(const RelocTensors& t)
+{
+	for (int i = 0; i < 6; i++)
+		if (!t.p[i] || !t.m[i] || !t.v[i]) return false;
 	return true;
+}
+// rows [0, P) of dst := those of src: the 18 parameter / moment tensors, and exist_since_iter when both models have it
+int copy_rows(int P, const RelocTensors& s, const RelocTensors& d, cudaStream_t stream)
+{
+	for (int i = 0; i < 6; i++) {
+		const size_t bytes = (size_t)P * row_floats(i) * sizeof(float);
+		PSB_CUDA_OK(cudaMemcpyAsync(d.p[i], s.p[i], bytes, cudaMemcpyDeviceToDevice, stream));
+		PSB_CUDA_OK(cudaMemcpyAsync(d.m[i], s.m[i], bytes, cudaMemcpyDeviceToDevice, stream));
+		PSB_CUDA_OK(cudaMemcpyAsync(d.v[i], s.v[i], bytes, cudaMemcpyDeviceToDevice, stream));
+	}
+	if (d.exist && s.exist) PSB_CUDA_OK(cudaMemcpyAsync(d.exist, s.exist, (size_t)P * sizeof(int), cudaMemcpyDeviceToDevice, stream));
+	return 0;
+}
+// rows [0, n) of the statistics the model has := 0 (reference densificationPostfix :709-711)
+int zero_stats(const RelocTensors& t, size_t n, cudaStream_t stream)
+{
+	for (int q = 0; q < 3; q++)
+		if (t.stat[q]) PSB_CUDA_OK(cudaMemsetAsync(t.stat[q], 0, n * sizeof(float), stream));
+	return 0;
 }
 bool reloc_cfg_ok(const psb_relocate_cfg* c)
 {
@@ -660,6 +685,46 @@ DensifyCfg to_cfg(const psb_densify_cfg* c)
 	return d;
 }
 
+// the plans' tail: scan of the block counts, then the one host round trip (the caller sizes the output tensors from the totals)
+int plan_totals(int P, const Workspace& w, uint32_t tot[4], cudaStream_t stream)
+{
+	densify_scan_kernel<<<1, 1024, 0, stream>>>((P + DN_TB - 1) / DN_TB, w.counts, w.offsets, w.totals);
+	PSB_LAUNCH_OK();
+	PSB_CUDA_OK(cudaMemcpyAsync(tot, w.totals, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+	PSB_CUDA_OK(cudaStreamSynchronize(stream));
+	return 0;
+}
+
+// psb_densify_apply and psb_prune_apply: dst's P_new rows from src's P rows by the plan in the workspace. keep_stats: the statistics
+// of the surviving originals are compacted (when both models have all three); otherwise those of dst are zeroed.
+int scatter_apply(const char* fn, int P, const psb_model* src, const psb_model* dst, int P_new, const psb_densify_cfg* cfg,
+                  const void* workspace, bool keep_stats, const float* normal_samples, cudaStream_t stream)
+{
+	const RelocTensors s = rows_of(src), d = rows_of(dst);
+	const bool rows = P > 0 && P_new > 0;
+	const char* err = nullptr;
+	if (P < 0 || P_new < 0 || !cfg || (P > 0 && (!src || !workspace)) || (P_new > 0 && !dst)) err = ": bad argument";
+	else if (rows && (!has_rows(s) || !has_rows(d))) err = ": null tensor";
+	else if (rows && (reinterpret_cast<uintptr_t>(s.p[5]) & 15)) err = ": rotation tensor must be 16-byte aligned";
+	if (err) { set_error_msg((std::string(fn) + err).c_str()); return PSB_ERR_ARG; }
+	int rc;
+	if (!keep_stats && P_new > 0 && (rc = zero_stats(d, (size_t)P_new, stream))) return rc;
+	if (!rows) return 0;
+	const bool stats = keep_stats && s.stat[0] && s.stat[1] && s.stat[2] && d.stat[0] && d.stat[1] && d.stat[2];
+	DensifyTensors t;
+	for (int i = 0; i < 6; i++) {
+		t.p[i] = s.p[i]; t.m[i] = s.m[i]; t.v[i] = s.v[i];
+		t.dp[i] = d.p[i]; t.dm[i] = d.m[i]; t.dv[i] = d.v[i];
+	}
+	t.exist = s.exist && d.exist ? s.exist : nullptr;
+	t.dexist = d.exist;
+	for (int q = 0; q < 3; q++) { t.stat[q] = stats ? s.stat[q] : nullptr; t.dstat[q] = stats ? d.stat[q] : nullptr; }
+	const Workspace w = ws_carve(const_cast<void*>(workspace), P);
+	densify_scatter_kernel<<<(P + DN_TB - 1) / DN_TB, DN_TB, 0, stream>>>(P, t, w.flags, w.offsets, w.totals, normal_samples, cfg->seed, cfg->offset);
+	PSB_LAUNCH_OK();
+	return 0;
+}
+
 }  // namespace
 
 int launch_position_noise(int P, float* xyz, const float* opacity, const float* scaling, const float* rotation, float lr, unsigned long long seed,
@@ -682,8 +747,8 @@ size_t psb_relocate_workspace_bytes(int P) { return P > 0 ? reloc_ws_bytes(P) : 
 int psb_relocate(int P, const psb_model* model, const psb_relocate_cfg* cfg, void* workspace, const float* uniforms, int* counts_host, void* stream_)
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
-	RelocTensors t;
-	if (P < 0 || !reloc_cfg_ok(cfg) || (P > 0 && (!model || !workspace || !reloc_tensors(model, t)))) {
+	const RelocTensors t = rows_of(model);
+	if (P < 0 || !reloc_cfg_ok(cfg) || (P > 0 && (!workspace || !has_rows(t)))) {
 		set_error_msg("psb_relocate: bad argument (P >= 0, min_opacity in [0, 1), a model with parameters and moments, and a workspace required)");
 		return PSB_ERR_ARG;
 	}
@@ -712,28 +777,23 @@ int psb_grow(int P, const psb_model* src, const psb_model* dst, int P_new, const
              void* stream_)
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
-	RelocTensors ts, t;
+	const RelocTensors ts = rows_of(src);
+	RelocTensors t = rows_of(dst);
 	const long long n = (long long)P_new - P;
-	if (P < 0 || n < 0 || n > P || !reloc_cfg_ok(cfg) || (P_new > 0 && (!src || !dst || !workspace || !reloc_tensors(src, ts) || !reloc_tensors(dst, t)))) {
+	if (P < 0 || n < 0 || n > P || !reloc_cfg_ok(cfg) || (P_new > 0 && (!workspace || !has_rows(ts) || !has_rows(t)))) {
 		set_error_msg("psb_grow: bad argument (P <= P_new <= 2 P, min_opacity in [0, 1), two models with parameters and moments, and a workspace required)");
 		return PSB_ERR_ARG;
 	}
 	if (P_new > 0 && (reinterpret_cast<uintptr_t>(workspace) & 7)) { set_error_msg("psb_grow: workspace must be 8-byte aligned"); return PSB_ERR_ARG; }
 	if (P == 0) return 0;
 	// the P old rows as they are (statistics and exist_since_iter included), then the picked ones are corrected in place in dst
-	for (int i = 0; i < 6; i++) {
-		const size_t bytes = (size_t)P * dn_row(i) * sizeof(float);
-		PSB_CUDA_OK(cudaMemcpyAsync(t.p[i], ts.p[i], bytes, cudaMemcpyDeviceToDevice, stream));
-		PSB_CUDA_OK(cudaMemcpyAsync(t.m[i], ts.m[i], bytes, cudaMemcpyDeviceToDevice, stream));
-		PSB_CUDA_OK(cudaMemcpyAsync(t.v[i], ts.v[i], bytes, cudaMemcpyDeviceToDevice, stream));
-	}
+	int rc;
+	if ((rc = copy_rows(P, ts, t, stream))) return rc;
 	for (int q = 0; q < 3; q++)
 		if (t.stat[q] && ts.stat[q]) PSB_CUDA_OK(cudaMemcpyAsync(t.stat[q], ts.stat[q], (size_t)P * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-	if (t.exist && ts.exist) PSB_CUDA_OK(cudaMemcpyAsync(t.exist, ts.exist, (size_t)P * sizeof(int), cudaMemcpyDeviceToDevice, stream));
 	t.live = nullptr;   // dst is a new model: its live bytes are the caller's to rebuild
 	if (n == 0) return 0;
 	const RelocWorkspace w = reloc_ws_carve(workspace, P);
-	int rc;
 	if ((rc = reloc_sample(P, t.p[3], cfg, 1, (int)n, w, uniforms, stream))) return rc;
 	reloc_correct_kernel<<<(P + DN_TB - 1) / DN_TB, DN_TB, 0, stream>>>(P, t, w.mult, cfg->min_opacity);
 	PSB_LAUNCH_OK();
@@ -754,14 +814,11 @@ int psb_densify_plan(int P, const psb_model* src, const psb_densify_cfg* cfg, vo
 	for (int k = 0; k < 5; k++) counts_host[k] = 0;
 	if (P == 0) return 0;
 	const Workspace w = ws_carve(workspace, P);
-	const int nb = (P + DN_TB - 1) / DN_TB;
-	densify_mask_kernel<<<nb, DN_TB, 0, stream>>>(P, src->param[4], src->param[3], src->xyz_gradient_accum, src->denom, to_cfg(cfg), w.flags, w.counts);
-	PSB_LAUNCH_OK();
-	densify_scan_kernel<<<1, 1024, 0, stream>>>(nb, w.counts, w.offsets, w.totals);
+	densify_mask_kernel<<<(P + DN_TB - 1) / DN_TB, DN_TB, 0, stream>>>(P, src->param[4], src->param[3], src->xyz_gradient_accum, src->denom, to_cfg(cfg), w.flags, w.counts);
 	PSB_LAUNCH_OK();
 	uint32_t tot[4];
-	PSB_CUDA_OK(cudaMemcpyAsync(tot, w.totals, sizeof(tot), cudaMemcpyDeviceToHost, stream));
-	PSB_CUDA_OK(cudaStreamSynchronize(stream));  // the one host round trip: the caller must size the output tensors
+	int rc;
+	if ((rc = plan_totals(P, w, tot, stream))) return rc;
 	counts_host[0] = (int)(tot[0] + tot[1] + 2 * tot[2]);
 	counts_host[1] = (int)tot[0]; counts_host[2] = (int)tot[1]; counts_host[3] = (int)tot[2]; counts_host[4] = (int)tot[3];
 	return 0;
@@ -770,30 +827,7 @@ int psb_densify_plan(int P, const psb_model* src, const psb_densify_cfg* cfg, vo
 int psb_densify_apply(int P, const psb_model* src, const psb_model* dst, int P_new, const psb_densify_cfg* cfg, const void* workspace,
                       const float* normal_samples, void* stream_)
 {
-	cudaStream_t stream = (cudaStream_t)stream_;
-	if (P < 0 || P_new < 0 || !cfg || (P > 0 && (!src || !workspace)) || (P_new > 0 && !dst)) { set_error_msg("psb_densify_apply: bad argument"); return PSB_ERR_ARG; }
-	if (P_new > 0) {
-		if (dst->max_radii2D) PSB_CUDA_OK(cudaMemsetAsync(dst->max_radii2D, 0, (size_t)P_new * sizeof(float), stream));          // :709-711
-		if (dst->xyz_gradient_accum) PSB_CUDA_OK(cudaMemsetAsync(dst->xyz_gradient_accum, 0, (size_t)P_new * sizeof(float), stream));
-		if (dst->denom) PSB_CUDA_OK(cudaMemsetAsync(dst->denom, 0, (size_t)P_new * sizeof(float), stream));
-	}
-	if (P == 0 || P_new == 0) return 0;
-	DensifyTensors t;
-	for (int i = 0; i < 6; i++) {
-		if (!src->param[i] || !src->exp_avg[i] || !src->exp_avg_sq[i] || !dst->param[i] || !dst->exp_avg[i] || !dst->exp_avg_sq[i]) {
-			set_error_msg("psb_densify_apply: null tensor"); return PSB_ERR_ARG;
-		}
-		t.p[i] = src->param[i]; t.m[i] = src->exp_avg[i]; t.v[i] = src->exp_avg_sq[i];
-		t.dp[i] = dst->param[i]; t.dm[i] = dst->exp_avg[i]; t.dv[i] = dst->exp_avg_sq[i];
-	}
-	t.exist = (src->exist_since_iter && dst->exist_since_iter) ? src->exist_since_iter : nullptr;
-	t.dexist = dst->exist_since_iter;
-	for (int q = 0; q < 3; q++) { t.stat[q] = nullptr; t.dstat[q] = nullptr; }
-	if (reinterpret_cast<uintptr_t>(src->param[5]) & 15) { set_error_msg("psb_densify_apply: rotation tensor must be 16-byte aligned"); return PSB_ERR_ARG; }
-	const Workspace w = ws_carve(const_cast<void*>(workspace), P);
-	densify_scatter_kernel<<<(P + DN_TB - 1) / DN_TB, DN_TB, 0, stream>>>(P, t, w.flags, w.offsets, w.totals, normal_samples, cfg->seed, cfg->offset);
-	PSB_LAUNCH_OK();
-	return 0;
+	return scatter_apply("psb_densify_apply", P, src, dst, P_new, cfg, workspace, false, normal_samples, (cudaStream_t)stream_);
 }
 
 int psb_prune_plan(int P, const unsigned char* mask, void* workspace, int* counts_host, void* stream_)
@@ -803,75 +837,42 @@ int psb_prune_plan(int P, const unsigned char* mask, void* workspace, int* count
 	for (int k = 0; k < 5; k++) counts_host[k] = 0;
 	if (P == 0) return 0;
 	const Workspace w = ws_carve(workspace, P);
-	const int nb = (P + DN_TB - 1) / DN_TB;
-	prune_mask_kernel<<<nb, DN_TB, 0, stream>>>(P, mask, w.flags, w.counts);
-	PSB_LAUNCH_OK();
-	densify_scan_kernel<<<1, 1024, 0, stream>>>(nb, w.counts, w.offsets, w.totals);
+	prune_mask_kernel<<<(P + DN_TB - 1) / DN_TB, DN_TB, 0, stream>>>(P, mask, w.flags, w.counts);
 	PSB_LAUNCH_OK();
 	uint32_t tot[4];
-	PSB_CUDA_OK(cudaMemcpyAsync(tot, w.totals, sizeof(tot), cudaMemcpyDeviceToHost, stream));
-	PSB_CUDA_OK(cudaStreamSynchronize(stream));
+	int rc;
+	if ((rc = plan_totals(P, w, tot, stream))) return rc;
 	counts_host[0] = counts_host[1] = (int)tot[0];
 	return 0;
 }
 
 int psb_prune_apply(int P, const psb_model* src, const psb_model* dst, int P_new, const void* workspace, int keep_stats, void* stream_)
 {
-	cudaStream_t stream = (cudaStream_t)stream_;
-	if (P < 0 || P_new < 0 || (P > 0 && (!src || !workspace)) || (P_new > 0 && !dst)) { set_error_msg("psb_prune_apply: bad argument"); return PSB_ERR_ARG; }
-	if (P == 0 || P_new == 0) return 0;
-	DensifyTensors t;
-	for (int i = 0; i < 6; i++) {
-		if (!src->param[i] || !src->exp_avg[i] || !src->exp_avg_sq[i] || !dst->param[i] || !dst->exp_avg[i] || !dst->exp_avg_sq[i]) {
-			set_error_msg("psb_prune_apply: null tensor"); return PSB_ERR_ARG;
-		}
-		t.p[i] = src->param[i]; t.m[i] = src->exp_avg[i]; t.v[i] = src->exp_avg_sq[i];
-		t.dp[i] = dst->param[i]; t.dm[i] = dst->exp_avg[i]; t.dv[i] = dst->exp_avg_sq[i];
-	}
-	t.exist = (src->exist_since_iter && dst->exist_since_iter) ? src->exist_since_iter : nullptr;
-	t.dexist = dst->exist_since_iter;
-	const bool stats = keep_stats && src->max_radii2D && src->xyz_gradient_accum && src->denom && dst->max_radii2D && dst->xyz_gradient_accum && dst->denom;
-	t.stat[0] = stats ? src->max_radii2D : nullptr; t.stat[1] = src->xyz_gradient_accum; t.stat[2] = src->denom;
-	t.dstat[0] = dst->max_radii2D; t.dstat[1] = dst->xyz_gradient_accum; t.dstat[2] = dst->denom;
-	if (reinterpret_cast<uintptr_t>(src->param[5]) & 15) { set_error_msg("psb_prune_apply: rotation tensor must be 16-byte aligned"); return PSB_ERR_ARG; }
-	const Workspace w = ws_carve(const_cast<void*>(workspace), P);
-	densify_scatter_kernel<<<(P + DN_TB - 1) / DN_TB, DN_TB, 0, stream>>>(P, t, w.flags, w.offsets, w.totals, nullptr, 0ull, 0ull);
-	PSB_LAUNCH_OK();
-	return 0;
+	static const psb_densify_cfg no_draw = {};   // a prune draws nothing: no samples, seed 0, offset 0
+	return scatter_apply("psb_prune_apply", P, src, dst, P_new, &no_draw, workspace, keep_stats != 0, nullptr, (cudaStream_t)stream_);
 }
 
 int psb_insert_points(int P, const psb_model* src, const psb_model* dst, int n, const float* points, const float* colors, const float* dist2,
                       int iteration, void* stream_)
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
-	if (P < 0 || n < 0 || !dst || (P > 0 && !src) || (n > 0 && (!points || !colors || !dist2))) { set_error_msg("psb_insert_points: bad argument"); return PSB_ERR_ARG; }
+	const RelocTensors s = rows_of(src), d = rows_of(dst);
 	const size_t Q = (size_t)P + n;
-	DensifyTensors t;
-	memset(&t, 0, sizeof(t));
-	for (int i = 0; i < 6; i++) {
-		if (Q > 0 && (!dst->param[i] || !dst->exp_avg[i] || !dst->exp_avg_sq[i])) { set_error_msg("psb_insert_points: null tensor"); return PSB_ERR_ARG; }
-		const size_t k = (size_t)dn_row(i);
-		if (P > 0) {
-			PSB_CUDA_OK(cudaMemcpyAsync(dst->param[i], src->param[i], (size_t)P * k * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-			PSB_CUDA_OK(cudaMemcpyAsync(dst->exp_avg[i], src->exp_avg[i], (size_t)P * k * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-			PSB_CUDA_OK(cudaMemcpyAsync(dst->exp_avg_sq[i], src->exp_avg_sq[i], (size_t)P * k * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-		}
-		if (n > 0) {   // moments of the new rows: zeros (cat(..., zeros_like(extension)), :675-676)
-			PSB_CUDA_OK(cudaMemsetAsync(dst->exp_avg[i] + (size_t)P * k, 0, (size_t)n * k * sizeof(float), stream));
-			PSB_CUDA_OK(cudaMemsetAsync(dst->exp_avg_sq[i] + (size_t)P * k, 0, (size_t)n * k * sizeof(float), stream));
-		}
-		t.dp[i] = dst->param[i];
+	if (P < 0 || n < 0 || !dst || (P > 0 && !src) || (n > 0 && (!points || !colors || !dist2))) { set_error_msg("psb_insert_points: bad argument"); return PSB_ERR_ARG; }
+	if ((Q > 0 && !has_rows(d)) || (P > 0 && !has_rows(s))) { set_error_msg("psb_insert_points: null tensor"); return PSB_ERR_ARG; }
+	if (n > 0 && (reinterpret_cast<uintptr_t>(d.p[5]) & 15)) { set_error_msg("psb_insert_points: rotation tensor must be 16-byte aligned"); return PSB_ERR_ARG; }
+	int rc;
+	if (P > 0 && (rc = copy_rows(P, s, d, stream))) return rc;
+	for (int i = 0; i < 6 && n > 0; i++) {   // moments of the new rows: zeros (cat(..., zeros_like(extension)), :675-676)
+		const size_t k = (size_t)row_floats(i);
+		PSB_CUDA_OK(cudaMemsetAsync(d.m[i] + (size_t)P * k, 0, (size_t)n * k * sizeof(float), stream));
+		PSB_CUDA_OK(cudaMemsetAsync(d.v[i] + (size_t)P * k, 0, (size_t)n * k * sizeof(float), stream));
 	}
-	if (P > 0 && src->exist_since_iter && dst->exist_since_iter)
-		PSB_CUDA_OK(cudaMemcpyAsync(dst->exist_since_iter, src->exist_since_iter, (size_t)P * sizeof(int), cudaMemcpyDeviceToDevice, stream));
-	t.dexist = dst->exist_since_iter;
-	if (Q > 0) {
-		if (dst->max_radii2D) PSB_CUDA_OK(cudaMemsetAsync(dst->max_radii2D, 0, Q * sizeof(float), stream));
-		if (dst->xyz_gradient_accum) PSB_CUDA_OK(cudaMemsetAsync(dst->xyz_gradient_accum, 0, Q * sizeof(float), stream));
-		if (dst->denom) PSB_CUDA_OK(cudaMemsetAsync(dst->denom, 0, Q * sizeof(float), stream));
-	}
+	if (Q > 0 && (rc = zero_stats(d, Q, stream))) return rc;
 	if (n > 0) {
-		if (reinterpret_cast<uintptr_t>(dst->param[5]) & 15) { set_error_msg("psb_insert_points: rotation tensor must be 16-byte aligned"); return PSB_ERR_ARG; }
+		DensifyTensors t = {};
+		for (int i = 0; i < 6; i++) t.dp[i] = d.p[i];
+		t.dexist = d.exist;
 		insert_fill_kernel<<<(n + 127) / 128, 128, 0, stream>>>(P, n, points, colors, dist2, iteration, t);
 		PSB_LAUNCH_OK();
 	}

@@ -27,7 +27,7 @@ namespace {
 
 constexpr int TB = 128;        // Gaussians per block
 constexpr int A_MINBLOCKS = 5; // __launch_bounds__ minimum blocks per SM of gaussian_backward_kernel
-constexpr int REST = 45;       // floats per f_rest row (15 coefficients x 3 channels)
+constexpr int REST = kRestFloats;  // floats per f_rest row (15 coefficients x 3 channels)
 constexpr int SEED = 20;       // floats per seed row: w_1..w_15 at [0..14], masked dL/dRGB at [16..18]
 
 struct AdamCoef {
@@ -503,7 +503,7 @@ __global__ void __launch_bounds__(256) adam_live_rebuild_kernel(int P, TrainTens
 {
 	const int i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= P) return;
-	const int width[6] = {3, 3, REST, 1, 3, 4};
+	const int width[6] = {row_floats(0), row_floats(1), row_floats(2), row_floats(3), row_floats(4), row_floats(5)};
 	bool nz = false;
 #pragma unroll
 	for (int q = 0; q < 6; q++) {

@@ -446,11 +446,10 @@ struct psb_dp {
 };
 
 namespace {
-constexpr size_t DP_ROW[6] = {3, 3, 45, 1, 3, 4};
 void dp_layout(psb_dp* d)
 {
 	size_t o = 0;
-	for (int i = 0; i < 6; i++) { d->off_param[i] = o; o = align_up(o + (size_t)d->P * DP_ROW[i] * sizeof(float), 256); }
+	for (int i = 0; i < 6; i++) { d->off_param[i] = o; o = align_up(o + (size_t)d->P * row_floats(i) * sizeof(float), 256); }
 	d->off_inbox = o; o = align_up(o + (size_t)d->world * d->nlocal_max * 128 * DP_REC * sizeof(float), 256);
 	d->off_meta = o; o += 256;
 	d->off_gflag = o; o += 256;
@@ -472,7 +471,7 @@ int psb_dp_create(psb_dp** out, int rank, int world, int P)
 	dp_layout(d);
 	cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&d->base), d->bytes);
 	if (e == cudaSuccess) e = cudaMemset(d->base, 0, d->bytes);
-	if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&d->g_rest), ((size_t)d->nlocal_max * 128 * 45 + 64) * sizeof(float));
+	if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&d->g_rest), ((size_t)d->nlocal_max * 128 * kRestFloats + 64) * sizeof(float));
 	if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&d->status), sizeof(uint32_t));
 	if (e == cudaSuccess) e = cudaMemset(d->status, 0, sizeof(uint32_t));
 	if (e == cudaSuccess && world > 1) e = cudaIpcGetMemHandle(&d->handle, d->base);
@@ -840,9 +839,8 @@ int psb_adam_update(int P, int M, const psb_model* model, float* const* grads, c
 	if ((rc = check_model(P, M, model, true))) return rc;
 	if (!grads || !step || step->step < 1) { set_error_msg("psb_adam_update: bad argument"); return PSB_ERR_ARG; }
 	const StepHyper h = to_hyper(step);
-	const size_t per[6] = {3, 3, (size_t)(M - 1) * 3, 1, 3, 4};
 	for (int i = 0; i < 6; i++)
-		if ((rc = launch_adam((size_t)P * per[i], model->param[i], model->exp_avg[i], model->exp_avg_sq[i], grads[i], step->lr[i], h, grad_scale,
+		if ((rc = launch_adam((size_t)P * row_floats(i), model->param[i], model->exp_avg[i], model->exp_avg_sq[i], grads[i], step->lr[i], h, grad_scale,
 		                      (cudaStream_t)stream_)))
 			return rc;
 	return 0;

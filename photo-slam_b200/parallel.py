@@ -3,8 +3,13 @@ any device, any torch.distributed backend): exercised with gloo on CPU in tests/
 on the GPUs by trainer.DataParallelTrainer / bench.py --gpus N."""
 import torch
 
-SIZES = (3, 3, 45, 1, 3, 4)   # floats per Gaussian of xyz, features_dc, features_rest, opacity, scaling, rotation
+SIZES = (3, 3, 45, 1, 3, 4)   # floats per Gaussian of xyz, features_dc, features_rest, opacity, scaling, rotation (csrc row_floats)
 PER_GAUSSIAN = sum(SIZES)     # 59
+
+
+def row_shapes(P):
+    """Shapes of the six tensors of a P-row model: [P, 3], [P, 1, 3], [P, 15, 3], [P, 1], [P, 3], [P, 4] (the SH features per channel)."""
+    return [(P, k // 3, 3) if i in (1, 2) else (P, k) for i, k in enumerate(SIZES)]
 
 
 def shard_schedule(schedule, rank, world):
@@ -54,9 +59,7 @@ class GradBuffer:
             o += _pad4(P * s)
 
     def views(self):
-        P = self.P
-        shapes = [(P, 3), (P, 1, 3), (P, 15, 3), (P, 1), (P, 3), (P, 4)]
-        return [seg.view(*sh) for seg, sh in zip(self.segments, shapes)]
+        return [seg.view(*sh) for seg, sh in zip(self.segments, row_shapes(self.P))]
 
     def all_reduce(self, group=None):
         """Sum over ranks; returns the factor the optimizer applies (mean over the K views of the step)."""

@@ -18,6 +18,7 @@ from dataclasses import dataclass
 import torch
 
 from . import _lib
+from .parallel import SIZES, row_shapes
 
 GROUPS = ("xyz", "features_dc", "features_rest", "opacity", "scaling", "rotation")
 
@@ -26,6 +27,19 @@ class _Model(C.Structure):
     _fields_ = [("param", C.c_void_p * 6), ("exp_avg", C.c_void_p * 6), ("exp_avg_sq", C.c_void_p * 6),
                 ("max_radii2D", C.c_void_p), ("xyz_gradient_accum", C.c_void_p), ("denom", C.c_void_p), ("exist_since_iter", C.c_void_p),
                 ("adam_live", C.c_void_p)]
+
+
+def _cmodel_of(p, m=None, v=None, accum=None, denom=None, max_radii=None, exist=None, live=None):
+    """psb_model over the given tensors (p, m, v: the six parameter / moment tensors); what is None is passed as NULL."""
+    c = _Model()
+    ptr = lambda t: None if t is None else t.data_ptr()
+    for i in range(6):
+        c.param[i] = p[i].data_ptr()
+        if m is not None:
+            c.exp_avg[i], c.exp_avg_sq[i] = m[i].data_ptr(), v[i].data_ptr()
+    c.max_radii2D, c.xyz_gradient_accum, c.denom = ptr(max_radii), ptr(accum), ptr(denom)
+    c.exist_since_iter, c.adam_live = ptr(exist), ptr(live)
+    return c
 
 
 class _Camera(C.Structure):
@@ -339,8 +353,7 @@ class GaussianModel:
         """adam_live_, rebuilt from the moments (psb_adam_live_rebuild) if it is stale."""
         live = self._live_tensor()
         if not self.adam_live_valid_:
-            m = self._cmodel()
-            m.adam_live = live.data_ptr()
+            m = self._cmodel(live=live)
             _lib.check(_bind().psb_adam_live_rebuild(self.num_points(), C.byref(m), torch.cuda.current_stream().cuda_stream), "psb_adam_live_rebuild")
             self.adam_live_valid_ = True
         return live
@@ -414,8 +427,7 @@ class GaussianModel:
         t = lambda x: torch.from_numpy(x).to(self.device).contiguous()
         self._set([t(a[k]) for k in ("xyz", "features_dc", "features_rest", "opacity", "scaling", "rotation")])
         self.active_sh_degree_ = self.max_sh_degree_
-        self.invalidateAdamLive()
-        self.filter_3D_ = None
+        self._rows_replaced()
 
     def setSparsePoints(self, xyz, color):
         """sparse SLAM map points + colours in [0,1] kept for input.ply (reference gaussian_model.cpp: sparse_points_xyz_ / _color_)"""
@@ -469,31 +481,46 @@ class GaussianModel:
         return self.exist_since_iter_
 
     def _blank(self, P):
-        """Uninitialised tensors of a P-row model (parameters, both moments, statistics, exist_since_iter)."""
-        M = (self.max_sh_degree_ + 1) ** 2
-        shapes = [(P, 3), (P, 1, 3), (P, M - 1, 3), (P, 1), (P, 3), (P, 4)]
+        """Uninitialised tensors of a P-row model (parameters, both moments, statistics, exist_since_iter), keyed like _rows()."""
+        shapes = row_shapes(P)
         e = lambda sh: torch.empty(sh, dtype=torch.float32, device=self.device)
         return dict(p=[e(sh) for sh in shapes], m=[e(sh) for sh in shapes], v=[e(sh) for sh in shapes], accum=e((P, 1)), denom=e((P, 1)),
                     max_radii=e((P,)), exist=torch.empty(P, dtype=torch.int32, device=self.device))
 
-    @staticmethod
-    def _cm(p, m, v, accum, denom, max_radii, exist):
-        c = _Model()
-        for i in range(6):
-            c.param[i], c.exp_avg[i], c.exp_avg_sq[i] = p[i].data_ptr(), m[i].data_ptr(), v[i].data_ptr()
-        c.max_radii2D, c.xyz_gradient_accum, c.denom, c.exist_since_iter = max_radii.data_ptr(), accum.data_ptr(), denom.data_ptr(), exist.data_ptr()
-        return c
+    def _rows(self):
+        """The model's tensors as the row operations take them (_cmodel_of(**rows))."""
+        return dict(p=self.tensors(), m=self.exp_avg_, v=self.exp_avg_sq_, accum=self.xyz_gradient_accum_, denom=self.denom_,
+                    max_radii=self.max_radii2D_, exist=self._exist())
 
-    def _src(self):
-        self._exist()
-        return self._cm(self.tensors(), self.exp_avg_, self.exp_avg_sq_, self.xyz_gradient_accum_, self.denom_, self.max_radii2D_, self.exist_since_iter_)
+    def _check_rows(self):
+        """The C row operations move 45 features_rest floats per row: any other SH storage is refused before the first C call."""
+        want = row_shapes(self.num_points())[2]
+        if tuple(self.features_rest_.shape) != want:
+            raise ValueError(f"row operations need features_rest of shape {list(want)} (all 16 SH coefficients), got {list(self.features_rest_.shape)}")
+
+    def _out_of_place(self, P_new, call, what):
+        """call(src, dst) is a C row operation from the current rows into P_new new ones; the model then adopts the new rows."""
+        d = self._blank(P_new)
+        _lib.check(call(C.byref(_cmodel_of(**self._rows())), C.byref(_cmodel_of(**d))), what)
+        self._adopt(d)
 
     def _adopt(self, d):
         self._set(d["p"])
         self.exp_avg_, self.exp_avg_sq_ = d["m"], d["v"]
         self.xyz_gradient_accum_, self.denom_, self.max_radii2D_, self.exist_since_iter_ = d["accum"], d["denom"], d["max_radii"], d["exist"]
-        self.invalidateAdamLive()   # rows moved: rebuilt from the new moments before the next fused step
+        self._rows_replaced()
+
+    def _rows_replaced(self):
+        """Rows renumbered or replaced: the live bytes are stale (the next fused step rebuilds them) and the 3D filter is dropped."""
+        self.invalidateAdamLive()
         self.filter_3D_ = None
+
+    def _geometry_changed(self, fresh_moments=()):
+        """Rows moved in place: the 3D filter is dropped; the groups in fresh_moments restart Adam from zero (the live bytes stay valid)."""
+        self.filter_3D_ = None
+        for i in fresh_moments:
+            self.exp_avg_[i] = torch.zeros_like(self.tensors()[i])
+            self.exp_avg_sq_[i] = torch.zeros_like(self.tensors()[i])
 
     def resetOpacity(self):
         """reference gaussian_model.cpp:556-565. NOTE: the reference's misplaced parenthesis makes this
@@ -504,6 +531,7 @@ class GaussianModel:
 
     def prunePoints(self, mask):
         """reference gaussian_model.cpp:588-642 (statistics are compacted, not reset)"""
+        self._check_rows()
         L = _bind()
         P = self.num_points()
         stream = torch.cuda.current_stream().cuda_stream
@@ -511,16 +539,14 @@ class GaussianModel:
         counts = (C.c_int * 5)()
         m8 = mask.to(torch.uint8).contiguous()
         _lib.check(L.psb_prune_plan(P, m8.data_ptr(), ws.data_ptr(), counts, stream), "psb_prune_plan")
-        d = self._blank(counts[0])
-        src, dst = self._src(), self._cm(d["p"], d["m"], d["v"], d["accum"], d["denom"], d["max_radii"], d["exist"])
-        _lib.check(L.psb_prune_apply(P, C.byref(src), C.byref(dst), counts[0], ws.data_ptr(), 1, stream), "psb_prune_apply")
-        self._adopt(d)
+        self._out_of_place(counts[0], lambda src, dst: L.psb_prune_apply(P, src, dst, counts[0], ws.data_ptr(), 1, stream), "psb_prune_apply")
 
     def densifyAndPrune(self, max_grad, min_opacity, extent, max_screen_size, seed=0, offset=None, samples=None):
         """reference gaussian_model.cpp:795-815 with densifyAndClone / densifyAndSplit / prunePoints / densificationPostfix folded
         into one plan + one scatter pass. The split draw is Philox(seed, offset) — identical on every data-parallel replica —
         unless `samples` ([2 * n_split, 3] standard normals in the reference's repeat order) is injected (tests).
         Returns (P_new, kept originals, clones, kept split children per copy, split-selected)."""
+        self._check_rows()
         L = _bind()
         P = self.num_points()
         stream = torch.cuda.current_stream().cuda_stream
@@ -528,16 +554,13 @@ class GaussianModel:
                           int(self.step_ if offset is None else offset))
         ws = torch.empty(L.psb_densify_workspace_bytes(P), dtype=torch.uint8, device=self.device)
         counts = (C.c_int * 5)()
-        src = self._src()
-        _lib.check(L.psb_densify_plan(P, C.byref(src), C.byref(cfg), ws.data_ptr(), counts, stream), "psb_densify_plan")
+        _lib.check(L.psb_densify_plan(P, C.byref(_cmodel_of(**self._rows())), C.byref(cfg), ws.data_ptr(), counts, stream), "psb_densify_plan")
         if samples is not None:
             samples = samples.to(self.device, torch.float32).contiguous()
             assert samples.shape == (2 * counts[4], 3), (samples.shape, counts[4])
-        d = self._blank(counts[0])
-        dst = self._cm(d["p"], d["m"], d["v"], d["accum"], d["denom"], d["max_radii"], d["exist"])
-        _lib.check(L.psb_densify_apply(P, C.byref(src), C.byref(dst), counts[0], C.byref(cfg), ws.data_ptr(),
-                                       samples.data_ptr() if samples is not None and samples.numel() else None, stream), "psb_densify_apply")
-        self._adopt(d)
+        z = samples.data_ptr() if samples is not None and samples.numel() else None
+        self._out_of_place(counts[0], lambda src, dst: L.psb_densify_apply(P, src, dst, counts[0], C.byref(cfg), ws.data_ptr(), z, stream),
+                           "psb_densify_apply")
         return tuple(counts)
 
     # --- bounded-budget densification (3DGS-MCMC; gsplat MCMCStrategy's relocate / sample_add): psb_relocate / psb_grow
@@ -550,27 +573,27 @@ class GaussianModel:
         In place, the row count does not change; moments of the rows involved are zeroed. The draw is Philox(seed, offset) — identical
         on every replica — unless `uniforms` (one number in [0, 1) per dead row, at least that many) is injected (tests).
         Returns the number of rows relocated (one host round trip)."""
+        self._check_rows()
         L = _bind()
         P = self.num_points()
         cfg = _RelocateCfg(float(min_opacity), int(iteration), int(seed), int(self.step_ if offset is None else offset))
         ws = torch.empty(L.psb_relocate_workspace_bytes(P), dtype=torch.uint8, device=self.device)
-        src = self._src()
-        live = self._live_tensor()
-        if self.adam_live_valid_:
-            src.adam_live = live.data_ptr()     # kept exact: the bytes of the rows whose moments are zeroed are cleared
+        live = self._live_tensor()   # a valid one is kept exact: the bytes of the rows whose moments are zeroed are cleared
+        model = _cmodel_of(**self._rows(), live=live if self.adam_live_valid_ else None)
         u = self._uniforms(uniforms)
         counts = (C.c_int * 2)()
-        _lib.check(L.psb_relocate(P, C.byref(src), C.byref(cfg), ws.data_ptr(), u.data_ptr() if u is not None and u.numel() else None, counts,
+        _lib.check(L.psb_relocate(P, C.byref(model), C.byref(cfg), ws.data_ptr(), u.data_ptr() if u is not None and u.numel() else None, counts,
                                   torch.cuda.current_stream().cuda_stream), "psb_relocate")
         if u is not None:
             assert u.numel() >= counts[1], (u.numel(), counts[1])
-        self.filter_3D_ = None
+        self._geometry_changed()
         return counts[0]
 
     def addNewGaussians(self, cap_max, grow_factor=1.05, min_opacity=0.005, seed=0, offset=None, iteration=0, uniforms=None):
         """Grows the model to min(cap_max, floor(grow_factor * P)) rows: the new rows are copies of rows drawn (over all rows) with
         probability proportional to opacity, corrected together with their sources like relocateGaussians does (psb_grow); they
         start with zero moments and statistics and exist_since_iter = iteration. Returns the number of rows added (0 at the cap)."""
+        self._check_rows()
         L = _bind()
         P = self.num_points()
         if not 1.0 < grow_factor <= 2.0:
@@ -583,11 +606,8 @@ class GaussianModel:
         u = self._uniforms(uniforms)
         if u is not None:
             assert u.numel() >= P_new - P, (u.numel(), P_new - P)
-        d = self._blank(P_new)
-        src, dst = self._src(), self._cm(d["p"], d["m"], d["v"], d["accum"], d["denom"], d["max_radii"], d["exist"])
-        _lib.check(L.psb_grow(P, C.byref(src), C.byref(dst), P_new, C.byref(cfg), ws.data_ptr(), u.data_ptr() if u is not None else None,
-                              torch.cuda.current_stream().cuda_stream), "psb_grow")
-        self._adopt(d)
+        self._out_of_place(P_new, lambda src, dst: L.psb_grow(P, src, dst, P_new, C.byref(cfg), ws.data_ptr(), u.data_ptr() if u is not None else None,
+                                                              torch.cuda.current_stream().cuda_stream), "psb_grow")
         return P_new - P
 
     def densifySplitCount(self, max_grad, extent):
@@ -597,14 +617,15 @@ class GaussianModel:
         cfg = _DensifyCfg(float(max_grad), 0.0, float(extent), float(self.percent_dense_), 0, 0, 0)
         ws = torch.empty(L.psb_densify_workspace_bytes(P), dtype=torch.uint8, device=self.device)
         counts = (C.c_int * 5)()
-        src = self._src()
-        _lib.check(L.psb_densify_plan(P, C.byref(src), C.byref(cfg), ws.data_ptr(), counts, torch.cuda.current_stream().cuda_stream), "psb_densify_plan")
+        _lib.check(L.psb_densify_plan(P, C.byref(_cmodel_of(**self._rows())), C.byref(cfg), ws.data_ptr(), counts, torch.cuda.current_stream().cuda_stream),
+                   "psb_densify_plan")
         return counts[4]
 
     def increasePcd(self, points, colors, iteration=0):
         """reference gaussian_model.cpp:193-377 (both overloads: host vectors / tensors): new Gaussians from sparse points — RGB2SH
         colour, scale from the 3-NN mean distance (distCUDA2 = psb_dist_cuda2), identity rotation, opacity = logit(0.1)."""
         from .points import distCUDA2
+        self._check_rows()
         L = _bind()
         points = torch.as_tensor(points, dtype=torch.float32).reshape(-1, 3)
         colors = torch.as_tensor(colors, dtype=torch.float32).reshape(-1, 3)
@@ -622,20 +643,14 @@ class GaussianModel:
         P = self.num_points()
         if not hasattr(self, "exp_avg_"):
             raise RuntimeError("increasePcd: call trainingSetup() first (the optimizer state is extended together with the parameters)")
-        d = self._blank(P + n)
-        src, dst = self._src(), self._cm(d["p"], d["m"], d["v"], d["accum"], d["denom"], d["max_radii"], d["exist"])
-        _lib.check(L.psb_insert_points(P, C.byref(src), C.byref(dst), n, pts.data_ptr(), cols.data_ptr(), dist2.data_ptr(), int(iteration),
-                                       torch.cuda.current_stream().cuda_stream), "psb_insert_points")
-        self._adopt(d)
+        self._out_of_place(P + n, lambda src, dst: L.psb_insert_points(P, src, dst, n, pts.data_ptr(), cols.data_ptr(), dist2.data_ptr(), int(iteration),
+                                                                       torch.cuda.current_stream().cuda_stream), "psb_insert_points")
 
     # --- loop closure / scale refinement (reference gaussian_model.cpp:379-475)
     def scaledTransformationPostfix(self, new_xyz, new_scaling):
         """:403-418: the two tensors replace xyz / scaling in the optimizer with FRESH (zero) moments (replaceTensorToOptimizer :567-586)"""
         self.xyz_, self.scaling_ = new_xyz.contiguous(), new_scaling.contiguous()
-        self.filter_3D_ = None
-        for i in (0, 4):
-            self.exp_avg_[i] = torch.zeros_like(self.tensors()[i])
-            self.exp_avg_sq_[i] = torch.zeros_like(self.tensors()[i])
+        self._geometry_changed(fresh_moments=(0, 4))
 
     def applyScaledTransformation(self, s, T):
         """:379-401: xyz <- T (s * xyz) through transformPoints; scaling_ (the LOG scale) is multiplied by s like the reference does.
@@ -657,28 +672,16 @@ class GaussianModel:
         num_transformed = scaleAndTransformThenMarkVisiblePoints(points, rots, point_not_transformed_flags, unstable, diff_pose,
                                                                  kf_world_view_transform, kf_full_proj_transform, num_transformed, scale)
         self.xyz_, self.rotation_ = points.contiguous(), rots.contiguous()
-        self.filter_3D_ = None
-        for i in (0, 5):
-            self.exp_avg_[i] = torch.zeros_like(self.tensors()[i])
-            self.exp_avg_sq_[i] = torch.zeros_like(self.tensors()[i])
+        self._geometry_changed(fresh_moments=(0, 5))
         return num_transformed
 
     def _cmodel(self, with_state=True, live=None):
-        """live: adam_live_ (valid) for the fused step; every other caller passes NULL."""
-        m = _Model()
-        if live is not None:
-            m.adam_live = live.data_ptr()
-        for i, t in enumerate(self.tensors()):
+        """live: adam_live_ (valid) for the fused step; every other caller passes NULL. exist_since_iter is always NULL."""
+        for t in self.tensors():
             assert t.is_contiguous() and t.dtype == torch.float32
-            m.param[i] = t.data_ptr()
-            if with_state:
-                m.exp_avg[i] = self.exp_avg_[i].data_ptr()
-                m.exp_avg_sq[i] = self.exp_avg_sq_[i].data_ptr()
-        if with_state:
-            m.max_radii2D = self.max_radii2D_.data_ptr()
-            m.xyz_gradient_accum = self.xyz_gradient_accum_.data_ptr()
-            m.denom = self.denom_.data_ptr()
-        return m
+        if not with_state:
+            return _cmodel_of(self.tensors(), live=live)
+        return _cmodel_of(self.tensors(), self.exp_avg_, self.exp_avg_sq_, self.xyz_gradient_accum_, self.denom_, self.max_radii2D_, live=live)
 
 
 def _ccamera(cam):
@@ -1131,9 +1134,8 @@ class DataParallelTrainer(GaussianTrainer):
             _lib.check(L.psb_dp_connect(h, None), "psb_dp_connect")
         ptrs = (C.c_void_p * 6)()
         _lib.check(L.psb_dp_params(h, ptrs), "psb_dp_params")
-        shapes = [(P, 3), (P, 1, 3), (P, 15, 3), (P, 1), (P, 3), (P, 4)]
         homed = []
-        for ptr, shp, src in zip(ptrs, shapes, m.tensors()):
+        for ptr, shp, src in zip(ptrs, row_shapes(P), m.tensors()):
             t = torch.as_tensor(_DevArray(ptr, shp), device=m.device) if P > 0 else torch.empty(shp, device=m.device)
             t.copy_(src)
             homed.append(t)
@@ -1243,7 +1245,6 @@ class DataParallelTrainer(GaussianTrainer):
             scale = self.grads.all_reduce(self.group)   # ONE collective per step: 59 floats per Gaussian
             _lib.check(self.L.psb_adam_update(P, 16, C.byref(cm), ptrs, C.byref(cs), scale, stream), "psb_adam_update")
         else:
-            from .parallel import SIZES
             assert self.grads.P == P, "gradient buffer was built for a different model size: call rebuild() after densify/prune"
             _lib.check(self.L.psb_trainer_backward_begin_depth(*args, cdepth, stream), "psb_trainer_backward_begin_depth")
             scale = 1.0 / self.world

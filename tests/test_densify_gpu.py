@@ -168,3 +168,32 @@ def test_prune_insert_reset_and_training_after_surgery(cuda):
     tr = trainer.GaussianTrainer(m)
     tr.trainForOneIteration(c, torch.rand((3, H, W), device=cuda))
     assert math.isfinite(tr.result()[0])
+
+
+def test_prune_apply_without_keep_stats_zeroes_the_statistics(cuda):
+    import ctypes as C
+    from photo_slam_b200 import _lib, trainer
+
+    def cm(p, m, v, accum, denom, max_radii, exist):
+        c = trainer._Model()
+        for i in range(6):
+            c.param[i], c.exp_avg[i], c.exp_avg_sq[i] = p[i].data_ptr(), m[i].data_ptr(), v[i].data_ptr()
+        c.max_radii2D, c.xyz_gradient_accum, c.denom, c.exist_since_iter = max_radii.data_ptr(), accum.data_ptr(), denom.data_ptr(), exist.data_ptr()
+        return c
+    m = _state(5_003, 3, 5.0, cuda)
+    L, P, stream = trainer._bind(), m.num_points(), torch.cuda.current_stream().cuda_stream
+    mask = torch.rand(P, device=cuda) < 0.3
+    ws = torch.empty(L.psb_densify_workspace_bytes(P), dtype=torch.uint8, device=cuda)
+    counts = (C.c_int * 5)()
+    _lib.check(L.psb_prune_plan(P, mask.to(torch.uint8).data_ptr(), ws.data_ptr(), counts, stream), "psb_prune_plan")
+    keep = ~mask
+    assert counts[0] == int(keep.sum())
+    d = m._blank(counts[0])
+    for t in (d["accum"], d["denom"], d["max_radii"]):
+        t.fill_(7.0)
+    src = cm(m.tensors(), m.exp_avg_, m.exp_avg_sq_, m.xyz_gradient_accum_, m.denom_, m.max_radii2D_, m.exist_since_iter_)
+    _lib.check(L.psb_prune_apply(P, C.byref(src), C.byref(cm(**d)), counts[0], ws.data_ptr(), 0, stream), "psb_prune_apply")
+    torch.cuda.synchronize()
+    assert not d["accum"].any() and not d["denom"].any() and not d["max_radii"].any()
+    for mine, a in zip(d["p"] + d["m"] + d["v"] + [d["exist"]], m.tensors() + m.exp_avg_ + m.exp_avg_sq_ + [m.exist_since_iter_]):
+        assert torch.equal(mine, a[keep])

@@ -46,18 +46,20 @@ def main():
                 cfg = trainer._DensifyCfg(tau, min_op, extent, m.percent_dense_, 20, 1, rep)
                 ws = torch.empty(L.psb_densify_workspace_bytes(P), dtype=torch.uint8, device=dev)
                 cnt = (C.c_int * 5)()
-                src = m._src()
+                src = trainer._cmodel_of(**m._rows())
                 ta = time.perf_counter()
                 L.psb_densify_plan(P, C.byref(src), C.byref(cfg), ws.data_ptr(), cnt, stream)
-                tb = time.perf_counter()
-                d = m._blank(cnt[0])
-                torch.cuda.synchronize()
-                tc = time.perf_counter()
-                dst = m._cm(d["p"], d["m"], d["v"], d["accum"], d["denom"], d["max_radii"], d["exist"])
-                L.psb_densify_apply(P, C.byref(src), C.byref(dst), cnt[0], C.byref(cfg), ws.data_ptr(), None, stream)
-                torch.cuda.synchronize()
-                td = time.perf_counter()
-                m._adopt(d)
+                tb = tc = td = time.perf_counter()
+
+                def apply(src, dst):   # runs after _out_of_place has allocated the new rows
+                    nonlocal tc, td
+                    torch.cuda.synchronize()
+                    tc = time.perf_counter()
+                    rc = L.psb_densify_apply(P, src, dst, cnt[0], C.byref(cfg), ws.data_ptr(), None, stream)
+                    torch.cuda.synchronize()
+                    td = time.perf_counter()
+                    return rc
+                m._out_of_place(cnt[0], apply, "psb_densify_apply")
                 counts = tuple(cnt)
                 print(f"  breakdown P={P}: setup {1e3*(ta-t0):.2f} plan {1e3*(tb-ta):.2f} alloc {1e3*(tc-tb):.2f} apply {1e3*(td-tc):.2f} ms", file=sys.stderr, flush=True)
             else:
