@@ -345,21 +345,20 @@ int psb_debug_sort_pairs(uint32_t* keys, uint32_t* vals, size_t n, int nbits, vo
 	cudaStream_t stream = (cudaStream_t)stream_;
 	if (n == 0) return 0;
 	const SortPlan plan = make_sort_plan(nbits);
-	uint32_t *k1 = nullptr, *v1 = nullptr;
-	void* scratch = nullptr;
+	CudaBuffer<uint32_t> k1, v1;
+	CudaBuffer<char> scratch;
 	const size_t sb = sort_scratch_bytes(n, plan.npass);
-	PSB_CUDA_OK(cudaMalloc(&k1, n * 4));
-	PSB_CUDA_OK(cudaMalloc(&v1, n * 4));
-	PSB_CUDA_OK(cudaMalloc(&scratch, sb));
-	uint32_t* kk[2] = {keys, k1};
-	uint32_t* vv[2] = {vals, v1};
-	int rc = radix_sort_pairs(kk, vv, false, nullptr, n, plan, scratch, sb, stream);
+	PSB_CUDA_OK(k1.grow(n, Fit::exact, false, stream));
+	PSB_CUDA_OK(v1.grow(n, Fit::exact, false, stream));
+	PSB_CUDA_OK(scratch.grow(sb, Fit::exact, false, stream));
+	uint32_t* kk[2] = {keys, k1.get()};
+	uint32_t* vv[2] = {vals, v1.get()};
+	int rc = radix_sort_pairs(kk, vv, false, nullptr, n, plan, scratch.get(), sb, stream);
 	if (rc == 0 && plan.result() == 1) {
-		cudaMemcpyAsync(keys, k1, n * 4, cudaMemcpyDeviceToDevice, stream);
-		cudaMemcpyAsync(vals, v1, n * 4, cudaMemcpyDeviceToDevice, stream);
+		cudaMemcpyAsync(keys, k1.get(), n * 4, cudaMemcpyDeviceToDevice, stream);
+		cudaMemcpyAsync(vals, v1.get(), n * 4, cudaMemcpyDeviceToDevice, stream);
 	}
 	cudaStreamSynchronize(stream);
-	cudaFree(k1); cudaFree(v1); cudaFree(scratch);
 	return rc;
 }
 

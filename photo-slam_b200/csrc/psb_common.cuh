@@ -3,6 +3,7 @@
 #pragma once
 #include <cstdint>
 #include <cstddef>
+#include <cstring>
 #include <cuda_runtime.h>
 
 #define PSB_TILE_X 16
@@ -33,6 +34,99 @@ void set_error_msg(const char* what);
 			return -2;                                                 \
 		}                                                              \
 	} while (0)
+
+// ---- Owned CUDA memory: nothing is freed by hand ----
+// How CudaBuffer::grow treats a buffer that already exists: keep it only at exactly the requested count, or at any count at least that
+// large.
+enum class Fit { exact, at_least };
+
+// The bytes of `count` elements of T. A chunk that one scratch state is carved from counts rows of that state instead (StateBytes,
+// psb_state.h).
+template <typename T>
+struct ElementBytes {
+	static size_t of(size_t count) { return count * sizeof(T); }
+};
+
+// One allocation and the count of elements it was made for: device memory, or page-locked host memory when `Pinned`, with `Slack`
+// bytes past the elements. Not copyable; the destructor frees it.
+template <typename T, size_t Slack = 0, bool Pinned = false, typename Bytes = ElementBytes<T>>
+class CudaBuffer {
+public:
+	CudaBuffer() = default;
+	CudaBuffer(const CudaBuffer&) = delete;
+	CudaBuffer& operator=(const CudaBuffer&) = delete;
+	~CudaBuffer() { release(); }
+
+	T* get() const { return p_; }
+	size_t count() const { return count_; }
+
+	// Keeps the buffer if it holds `count` elements (Fit::exact) or at least that many (Fit::at_least). Otherwise drains `stream` (work
+	// on it may still use the old buffer), frees the old buffer, allocates Bytes::of(count) + Slack bytes and, when `zero`, zeroes the
+	// elements on `stream` (pinned memory: on the host). After a failed allocation the buffer is empty (null, count 0), so the next call
+	// allocates again, and the error is reported only through the return value: it is taken off the runtime's last error, where a later
+	// launch check would find it.
+	cudaError_t grow(size_t count, Fit fit, bool zero, cudaStream_t stream)
+	{
+		if (fit == Fit::exact ? p_ && count_ == count : count_ >= count) return cudaSuccess;
+		cudaError_t e;
+		if (p_) {
+			if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
+			release();
+		}
+		const size_t bytes = Bytes::of(count);
+		void* p = nullptr;
+		e = Pinned ? cudaMallocHost(&p, bytes + Slack) : cudaMalloc(&p, bytes + Slack);
+		if (e != cudaSuccess) {
+			cudaGetLastError();
+			return e;
+		}
+		p_ = static_cast<T*>(p);
+		count_ = count;
+		if (zero) {
+			if (Pinned) memset(p, 0, bytes);
+			else if ((e = cudaMemsetAsync(p, 0, bytes, stream)) != cudaSuccess) release();
+		}
+		return e;
+	}
+
+private:
+	void release()
+	{
+		if (p_) Pinned ? cudaFreeHost(p_) : cudaFree(p_);
+		p_ = nullptr;
+		count_ = 0;
+	}
+	T* p_ = nullptr;
+	size_t count_ = 0;
+};
+
+// Stream-ordered scratch of one call: alloc() takes it with cudaMallocAsync on `stream`, and it goes back with cudaFreeAsync on the
+// same stream when the scope ends, on every path out of it.
+template <typename T>
+class StreamScratch {
+public:
+	explicit StreamScratch(cudaStream_t stream) : stream_(stream) {}
+	StreamScratch(const StreamScratch&) = delete;
+	StreamScratch& operator=(const StreamScratch&) = delete;
+	~StreamScratch()
+	{
+		if (p_) cudaFreeAsync(p_, stream_);
+	}
+
+	// once per scope
+	cudaError_t alloc(size_t count)
+	{
+		void* p = nullptr;
+		const cudaError_t e = cudaMallocAsync(&p, count * sizeof(T), stream_);
+		if (e == cudaSuccess) p_ = static_cast<T*>(p);
+		return e;
+	}
+	T* get() const { return p_; }
+
+private:
+	cudaStream_t stream_;
+	T* p_ = nullptr;
+};
 
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }

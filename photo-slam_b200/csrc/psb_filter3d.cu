@@ -84,24 +84,20 @@ extern "C" int psb_filter3d(int P, const float* xyz, int K, const float* cams, f
 		if (seen_host) *seen_host = 0;
 		return 0;
 	}
-	Filter3dScratch* sc = nullptr;
-	PSB_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&sc), sizeof(Filter3dScratch), stream));
-	int rc = 0;
-	uint32_t seen = 0;
-	if (cudaMemsetAsync(sc, 0, sizeof(Filter3dScratch), stream) != cudaSuccess) rc = PSB_ERR_CUDA;
-	if (rc == 0) {
-		const int grid = cdiv(P, F3D_TB);
-		filter3d_kernel<<<grid, F3D_TB, 0, stream>>>(P, xyz, K, cams, filter, sc);
-		filter3d_finish_kernel<<<grid, F3D_TB, 0, stream>>>(P, filter, sc);
-		const cudaError_t e = cudaGetLastError();
-		if (e != cudaSuccess) { set_error("psb_filter3d: kernel launch", e, __FILE__, __LINE__); rc = PSB_ERR_CUDA; }
-	}
-	if (rc == 0 && seen_host) {
-		cudaError_t e = cudaMemcpyAsync(&seen, &sc->seen, sizeof(seen), cudaMemcpyDeviceToHost, stream);
+	StreamScratch<Filter3dScratch> sc(stream);
+	PSB_CUDA_OK(sc.alloc(1));
+	if (cudaMemsetAsync(sc.get(), 0, sizeof(Filter3dScratch), stream) != cudaSuccess) return PSB_ERR_CUDA;
+	const int grid = cdiv(P, F3D_TB);
+	filter3d_kernel<<<grid, F3D_TB, 0, stream>>>(P, xyz, K, cams, filter, sc.get());
+	filter3d_finish_kernel<<<grid, F3D_TB, 0, stream>>>(P, filter, sc.get());
+	cudaError_t e = cudaGetLastError();
+	if (e != cudaSuccess) { set_error("psb_filter3d: kernel launch", e, __FILE__, __LINE__); return PSB_ERR_CUDA; }
+	if (seen_host) {
+		uint32_t seen = 0;
+		e = cudaMemcpyAsync(&seen, &sc.get()->seen, sizeof(seen), cudaMemcpyDeviceToHost, stream);
 		if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-		if (e != cudaSuccess) { set_error("psb_filter3d", e, __FILE__, __LINE__); rc = PSB_ERR_CUDA; }
-		else *seen_host = (int)seen;
+		if (e != cudaSuccess) { set_error("psb_filter3d", e, __FILE__, __LINE__); return PSB_ERR_CUDA; }
+		*seen_host = (int)seen;
 	}
-	cudaFreeAsync(sc, stream);
-	return rc;
+	return 0;
 }

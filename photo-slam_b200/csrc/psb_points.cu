@@ -316,9 +316,9 @@ int psb_dist_cuda2(int P, const float* points, float* mean_dists, void* stream_)
 	const size_t sb = sort_scratch_bytes((size_t)P, plan.npass);
 	const int nbox = (P + KNN_TILE - 1) / KNN_TILE;
 	const size_t bytes = align_up((size_t)P * 4, 256) * 4 + align_up(sb, 256) + align_up((size_t)nbox * sizeof(Box), 256) + align_up((size_t)P * sizeof(float4), 256) + 512;
-	char* mem = nullptr;
-	PSB_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&mem), bytes, stream));
-	char* c = mem;
+	StreamScratch<char> mem(stream);
+	PSB_CUDA_OK(mem.alloc(bytes));
+	char* c = mem.get();
 	uint32_t* keys[2]; uint32_t* vals[2];
 	keys[0] = carve<uint32_t>(c, P, 256); keys[1] = carve<uint32_t>(c, P, 256);
 	vals[0] = carve<uint32_t>(c, P, 256); vals[1] = carve<uint32_t>(c, P, 256);
@@ -332,17 +332,15 @@ int psb_dist_cuda2(int P, const float* points, float* mean_dists, void* stream_)
 	knn_bounds_kernel<<<grid, 256, 0, stream>>>(P, points, bounds);
 	knn_morton_kernel<<<cdiv(P, 256), 256, 0, stream>>>(P, points, bounds, keys[0]);
 	PSB_LAUNCH_OK();
-	int rc = radix_sort_pairs(keys, vals, /*iota_vals=*/true, nullptr, (size_t)P, plan, scratch, sb, stream);
-	if (rc == 0) {
-		const uint32_t* order = vals[plan.result()];
-		knn_gather_kernel<<<cdiv(P, 256), 256, 0, stream>>>(P, points, order, sorted);
-		knn_tile_box_kernel<<<nbox, KNN_TILE, 0, stream>>>(P, sorted, boxes);
-		knn_search_kernel<<<nbox, KNN_TILE, 0, stream>>>(P, nbox, sorted, boxes, mean_dists);
-		cudaError_t e = cudaGetLastError();
-		if (e != cudaSuccess) { set_error("knn kernels", e, __FILE__, __LINE__); rc = PSB_ERR_CUDA; }
-	}
-	cudaFreeAsync(mem, stream);
-	return rc;
+	int rc;
+	if ((rc = radix_sort_pairs(keys, vals, /*iota_vals=*/true, nullptr, (size_t)P, plan, scratch, sb, stream))) return rc;
+	const uint32_t* order = vals[plan.result()];
+	knn_gather_kernel<<<cdiv(P, 256), 256, 0, stream>>>(P, points, order, sorted);
+	knn_tile_box_kernel<<<nbox, KNN_TILE, 0, stream>>>(P, sorted, boxes);
+	knn_search_kernel<<<nbox, KNN_TILE, 0, stream>>>(P, nbox, sorted, boxes, mean_dists);
+	const cudaError_t e = cudaGetLastError();
+	if (e != cudaSuccess) { set_error("knn kernels", e, __FILE__, __LINE__); return PSB_ERR_CUDA; }
+	return 0;
 }
 
 int psb_reproject_depth_pinhole(int P, int width, float fx, float fy, float cx, float cy, const float* depths, const unsigned char* mask,

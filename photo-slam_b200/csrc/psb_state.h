@@ -122,6 +122,12 @@ static inline size_t required_bytes(size_t n)
 	return reinterpret_cast<size_t>(p) + 128;
 }
 
+// The bytes of a chunk that state S is carved from for `count` rows (P, R or W*H): a CudaBuffer<char, ..., StateBytes<S>> counts rows.
+template <typename S>
+struct StateBytes {
+	static size_t of(size_t count) { return required_bytes<S>(count); }
+};
+
 static inline int tile_id_bits(int num_tiles)
 {
 	int b = 1;

@@ -16,17 +16,27 @@
 
 using namespace psb;
 
+// The context's arena: every buffer has 256 bytes of slack past its elements. A chunk counts rows of the scratch state carved from it.
+template <typename T>
+using ArenaBuffer = CudaBuffer<T, 256>;
+template <typename S>
+using ArenaChunk = CudaBuffer<char, 256, false, StateBytes<S>>;
+
 struct psb_trainer {
-	char* geom_chunk = nullptr; size_t geom_bytes = 0; int geom_P = -1;
-	char* img_chunk = nullptr; size_t img_bytes = 0; int img_N = -1;
-	char* bin_chunk = nullptr; size_t bin_bytes = 0; size_t capacity = 0;
-	float* image = nullptr; float* dL_dpix = nullptr; float* dmap = nullptr; size_t pix_alloc = 0;
-	float* sink = nullptr; float* seeds = nullptr; size_t sink_P = 0;
-	float* depth_buf = nullptr; size_t depth_alloc = 0;  // depth loss: [2][H*W] = rendered depth (when the caller passes no out_depth) | dL/dD
-	double* sums = nullptr;      // device [4]: sum |I - G|, sum SSIM | depth loss: sum |D - G|, N_valid
-	double* h_sums = nullptr;    // pinned [4]
-	uint32_t* h_count = nullptr; // pinned [4]: instance count of the last call | sticky overflow record {count, first seq, largest count}
-	uint32_t* ovf = nullptr;     // device [4]: the sticky overflow record (tile_ranges_kernel), collected by psb_trainer_result
+	ArenaChunk<GeomState> geom;  // P rows: reallocated whenever P changes
+	ArenaChunk<ImgState> img;    // W*H pixels: reallocated whenever W*H changes
+	ArenaChunk<BinState> bin;    // its count is the binning capacity (instances)
+	ArenaBuffer<float> image, dL_dpix, dmap;  // [3][H*W], [3][H*W], [9][H*W]
+	ArenaBuffer<float> sink, seeds;           // [P][12] (zeroed when allocated), [P][20]
+	ArenaBuffer<float> depth_buf;  // depth loss: [2][H*W] = rendered depth (when the caller passes no out_depth) | dL/dD
+	ArenaBuffer<double> sums;      // device [4]: sum |I - G|, sum SSIM | depth loss: sum |D - G|, N_valid
+	CudaBuffer<double, 0, true> h_sums;     // pinned [4]
+	CudaBuffer<uint32_t, 0, true> h_count;  // pinned [4]: instance count of the last call | sticky overflow record {count, first seq, largest count}
+	ArenaBuffer<uint32_t> ovf;     // device [4]: the sticky overflow record (tile_ranges_kernel), collected by psb_trainer_result
+	// what the scratch was last carved for: set when ensure() succeeds, cleared (P = -1) when it fails or the binning chunk is lost
+	struct Carved {
+		int P = -1, W = 0, H = 0;
+	} carved;
 	uint32_t seq = 0;            // sequence number of the last forward pass (render / step / backward) of this context
 	// the mode of pass `seq`: what psb_trainer_backward_pixels must match, and the variant every per-Gaussian stage behind it runs
 	// (a psb_trainer_backward_begin* records it before its pass, so the _slab calls after it run that variant even if it failed)
@@ -41,8 +51,9 @@ struct psb_trainer {
 	const float* filter3d = nullptr;
 	int filter3d_P = 0;
 	uint32_t ovf_first = 0, ovf_count = 0;  // what the last PSB_ERR_RETRY was about (psb_trainer_overflow_info)
-	cudaEvent_t readback = nullptr;  // recorded once the instance count (and the loss sums) of the last call are in pinned memory
-	int last_P = 0, last_W = 0, last_H = 0;
+	// recorded once the instance count (and the loss sums) of the last call are in pinned memory; made last of the read-back set
+	// (sums, h_sums, h_count, ovf), so it exists only when the whole set does
+	cudaEvent_t readback = nullptr;
 	float last_lambda = 0.2f;
 	float last_lambda_depth = 0.f;
 	bool have_loss = false;
@@ -51,15 +62,15 @@ struct psb_trainer {
 	// reference's full rectangles (A/B measurements only — images and gradients are the same either way)
 	bool tight = !(getenv("PSB_TIGHT") && atoi(getenv("PSB_TIGHT")) == 0);
 	// deterministic mode (psb_trainer_set_deterministic): its own scratch, made only while the mode is on and grown with the binning
-	// capacity — the instance slots [det_cap][12] floats (zeroed when allocated: every tag reads "not this pass"), the emission offsets
-	// [det_P] and the loss partials [det_parts] doubles
+	// capacity — the instance slots [capacity][12] floats (zeroed when allocated: every tag reads "not this pass"), the emission offsets
+	// [P] and the loss partials
 	bool deterministic = false;
-	float* det_slots = nullptr; size_t det_cap = 0;
-	uint32_t* det_base = nullptr; size_t det_P = 0;
-	double* det_partials = nullptr; size_t det_parts = 0;
+	ArenaBuffer<float> det_slots;
+	ArenaBuffer<uint32_t> det_base;
+	ArenaBuffer<double> det_partials;
 	// exposure compensation (psb_trainer_step_exposure / psb_trainer_backward_exposure): the block partials of the 12 exposure sums
 	// [kExposurePartials] doubles, made by the first such call
-	double* exp_partials = nullptr;
+	ArenaBuffer<double> exp_partials;
 	// optional per-stage timing (CUDA events on the step's stream)
 	bool profiling = false;
 	// stage boundaries: 0 start | 1 preprocess | 2 depth sort | 3 binning | 4 render fwd | 5 loss | 6 render bwd |
@@ -74,81 +85,48 @@ struct psb_trainer {
 	cudaEvent_t event(int i) const { return profiling && ev_ready ? ev[i] : nullptr; }
 	// the last boundary of a profiled call: psb_trainer_stage_times reads the stages up to it
 	void end_stages(int last, cudaStream_t s) { mark(last, s); last_stage = last; ev_recorded = profiling && ev_ready; }
+	~psb_trainer()
+	{
+		if (ev_ready) for (cudaEvent_t e : ev) cudaEventDestroy(e);
+		if (readback) cudaEventDestroy(readback);
+	}
 };
 
 namespace {
 
-// An arena buffer that is missing or too small: drain the stream (the last call's kernels may still use the old buffer), free it and
-// allocate `count` elements, zeroed on the stream when `zero`.
-template <typename T>
-int regrow(T** p, size_t count, bool zero, cudaStream_t stream)
-{
-	PSB_CUDA_OK(cudaStreamSynchronize(stream));
-	if (*p) { cudaFree(*p); *p = nullptr; }
-	PSB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(p), count * sizeof(T) + 256));
-	if (zero) PSB_CUDA_OK(cudaMemsetAsync(*p, 0, count * sizeof(T), stream));
-	return 0;
-}
-
+// The scratch of a pass of P Gaussians over W x H pixels, each buffer's need stated once (CudaBuffer::grow drains the stream before it
+// frees a buffer the last call's kernels may still use). Any failure leaves t->carved cleared: no call reads this scratch until an
+// ensure() succeeds.
 int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_loss)
 {
 	const size_t N = (size_t)W * H;
-	int rc;
-	if (t->geom_P != P) {
-		t->geom_bytes = required_bytes<GeomState>((size_t)P);
-		if ((rc = regrow(&t->geom_chunk, t->geom_bytes, false, stream))) return rc;
-		t->geom_P = P;
-	}
-	if (t->img_N != (int)N) {
-		t->img_bytes = required_bytes<ImgState>(N);
-		if ((rc = regrow(&t->img_chunk, t->img_bytes, false, stream))) return rc;
-		t->img_N = (int)N;
-	}
-	if (t->pix_alloc < N) {
-		if ((rc = regrow(&t->image, 3 * N, false, stream)) || (rc = regrow(&t->dL_dpix, 3 * N, false, stream)) ||
-		    (rc = regrow(&t->dmap, 9 * N, false, stream)))
-			return rc;
-		t->pix_alloc = N;
-	}
-	if (depth_loss && t->depth_alloc < N) {
-		if ((rc = regrow(&t->depth_buf, 2 * N, false, stream))) return rc;
-		t->depth_alloc = N;
-	}
-	if (t->sink_P < (size_t)P) {
-		if ((rc = regrow(&t->sink, (size_t)P * 12, true, stream)) || (rc = regrow(&t->seeds, (size_t)P * 20, false, stream))) return rc;
-		t->sink_P = (size_t)P;
-	}
-	if (!t->sums) {
-		if ((rc = regrow(&t->sums, 4, false, stream))) return rc;
-		PSB_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&t->h_sums), 4 * sizeof(double)));
-		PSB_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&t->h_count), 4 * sizeof(uint32_t)));
-		memset(t->h_count, 0, 4 * sizeof(uint32_t));
-		if ((rc = regrow(&t->ovf, 4, false, stream))) return rc;
+	// the binning arena grows to P * 6 + 64 Ki instances when it is empty, or when it is smaller and the last pass was over another P
+	const size_t bin_need = t->bin.count() == 0 || t->carved.P != P ? (size_t)P * 6 + (1u << 16) : 0;
+	t->carved = {};
+	PSB_CUDA_OK(t->geom.grow((size_t)P, Fit::exact, false, stream));
+	PSB_CUDA_OK(t->img.grow(N, Fit::exact, false, stream));
+	PSB_CUDA_OK(t->image.grow(3 * N, Fit::at_least, false, stream));
+	PSB_CUDA_OK(t->dL_dpix.grow(3 * N, Fit::at_least, false, stream));
+	PSB_CUDA_OK(t->dmap.grow(9 * N, Fit::at_least, false, stream));
+	if (depth_loss) PSB_CUDA_OK(t->depth_buf.grow(2 * N, Fit::at_least, false, stream));
+	PSB_CUDA_OK(t->sink.grow((size_t)P * 12, Fit::at_least, true, stream));
+	PSB_CUDA_OK(t->seeds.grow((size_t)P * 20, Fit::at_least, false, stream));
+	if (!t->readback) {
+		PSB_CUDA_OK(t->sums.grow(4, Fit::at_least, false, stream));
+		PSB_CUDA_OK(t->h_sums.grow(4, Fit::at_least, false, stream));
+		PSB_CUDA_OK(t->h_count.grow(4, Fit::at_least, true, stream));
+		PSB_CUDA_OK(t->ovf.grow(4, Fit::at_least, false, stream));
 		const uint32_t init[4] = {0u, 0xFFFFFFFFu, 0u, 0u};
-		PSB_CUDA_OK(cudaMemcpy(t->ovf, init, sizeof(init), cudaMemcpyHostToDevice));
+		PSB_CUDA_OK(cudaMemcpy(t->ovf.get(), init, sizeof(init), cudaMemcpyHostToDevice));
 		PSB_CUDA_OK(cudaEventCreateWithFlags(&t->readback, cudaEventDisableTiming));
 	}
-	const size_t want = (size_t)P * 6 + (1u << 16);
-	if (t->capacity == 0 || (t->capacity < want && t->last_P != P)) {
-		t->capacity = t->capacity > want ? t->capacity : want;
-		t->bin_bytes = required_bytes<BinState>(t->capacity);
-		if ((rc = regrow(&t->bin_chunk, t->bin_bytes, false, stream))) return rc;
-	}
+	PSB_CUDA_OK(t->bin.grow(bin_need, Fit::at_least, false, stream));
 	if (t->deterministic) {
-		if (t->det_cap < t->capacity) {
-			if ((rc = regrow(&t->det_slots, t->capacity * 12, true, stream))) return rc;
-			t->det_cap = t->capacity;
-		}
-		if (t->det_P < (size_t)P) {
-			if ((rc = regrow(&t->det_base, (size_t)P, false, stream))) return rc;
-			t->det_P = (size_t)P;
-		}
-		if (t->det_parts < loss_partials_doubles(H, W)) {
-			if ((rc = regrow(&t->det_partials, loss_partials_doubles(H, W), false, stream))) return rc;
-			t->det_parts = loss_partials_doubles(H, W);
-		}
+		PSB_CUDA_OK(t->det_slots.grow(t->bin.count() * 12, Fit::at_least, true, stream));
+		PSB_CUDA_OK(t->det_base.grow((size_t)P, Fit::at_least, false, stream));
+		PSB_CUDA_OK(t->det_partials.grow(loss_partials_doubles(H, W), Fit::at_least, false, stream));
 	}
-	t->last_P = P; t->last_W = W; t->last_H = H;
+	t->carved = {P, W, H};
 	return 0;
 }
 
@@ -165,10 +143,10 @@ struct Scratch {
 };
 Scratch carve_scratch(const psb_trainer* t, int P, int width, int height)
 {
-	char* gc = t->geom_chunk;
-	char* ic = t->img_chunk;
-	char* bc = t->bin_chunk;
-	return {GeomState::from_chunk(gc, (size_t)P), ImgState::from_chunk(ic, (size_t)width * height), BinState::from_chunk(bc, t->capacity)};
+	char* gc = t->geom.get();
+	char* ic = t->img.get();
+	char* bc = t->bin.get();
+	return {GeomState::from_chunk(gc, (size_t)P), ImgState::from_chunk(ic, (size_t)width * height), BinState::from_chunk(bc, t->bin.count())};
 }
 
 GaussIn raw_input(int P, int D, int M, const psb_model* m)
@@ -317,15 +295,15 @@ int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, con
 	t->mark(1, stream);
 	if ((rc = launch_depth_sort_and_scan(P, geom, /*scan=*/false, stream))) return rc;
 	t->mark(2, stream);
-	if ((rc = launch_scan_binning(P, cam, geom, bin, img, t->capacity, t->tight, t->ovf, ++t->seq, stream, mode.det ? t->det_base : nullptr)))
+	if ((rc = launch_scan_binning(P, cam, geom, bin, img, t->bin.count(), t->tight, t->ovf.get(), ++t->seq, stream, mode.det ? t->det_base.get() : nullptr)))
 		return rc;
 	t->pass.D = mode.D;
 	t->mark(3, stream);
 	// the instance count travels to pinned memory as soon as it exists: psb_trainer_result waits on `readback`, not on the stream
-	PSB_CUDA_OK(cudaMemcpyAsync(t->h_count, geom.counters, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
-	PSB_CUDA_OK(cudaMemcpyAsync(t->h_count + 1, t->ovf, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+	PSB_CUDA_OK(cudaMemcpyAsync(t->h_count.get(), geom.counters, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+	PSB_CUDA_OK(cudaMemcpyAsync(t->h_count.get() + 1, t->ovf.get(), 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
 	PSB_CUDA_OK(cudaEventRecord(t->readback, stream));
-	rc = launch_render_forward(cam, img.ranges, bin.inst[sorted_slot(cam.W, cam.H)], geom.rec, background, out_color ? out_color : t->image, img.final_T,
+	rc = launch_render_forward(cam, img.ranges, bin.inst[sorted_slot(cam.W, cam.H)], geom.rec, background, out_color ? out_color : t->image.get(), img.final_T,
 	                           img.n_contrib, stream, out_depth, out_alpha);
 	t->mark(4, stream);
 	return rc;
@@ -336,18 +314,19 @@ int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, con
 int tile_backward(psb_trainer* t, int P, const Scratch& sc, const Camera& cam, const float* background, const float* dL_dpix, const float* dL_ddepth,
                   const float* dL_dalpha, cudaStream_t stream)
 {
+	float* const rows = t->sink.get();
 	GradSink sink;
-	sink.mean2D = t->sink; sink.mean2D_stride = 12;
-	sink.conic = t->sink + 3; sink.conic_stride = 12;
-	sink.opacity = t->sink + 7; sink.opacity_stride = 12;
-	sink.color = t->sink + 8; sink.color_stride = 12;
+	sink.mean2D = rows; sink.mean2D_stride = 12;
+	sink.conic = rows + 3; sink.conic_stride = 12;
+	sink.opacity = rows + 7; sink.opacity_stride = 12;
+	sink.color = rows + 8; sink.color_stride = 12;
 	sink.packed = 1;
 	DetSlots det;
-	det.slots = reinterpret_cast<float4*>(t->det_slots);
-	det.base = t->det_base;
+	det.slots = reinterpret_cast<float4*>(t->det_slots.get());
+	det.base = t->det_base.get();
 	det.tile_info = sc.geom.tile_info;
 	det.counters = sc.geom.counters;
-	det.capacity = (uint32_t)t->capacity;
+	det.capacity = (uint32_t)t->bin.count();
 	det.seq = t->seq;
 	det.P = P;
 	det.tight = t->tight ? 1 : 0;
@@ -385,10 +364,10 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	float* dL_ddepth = nullptr;
 	if (depth_loss) {
 		if ((rc = ensure(t, P, camera->width, camera->height, stream, true))) return rc;
-		if (!depth_plane) depth_plane = t->depth_buf;
-		dL_ddepth = t->depth_buf + (size_t)camera->width * camera->height;
+		if (!depth_plane) depth_plane = t->depth_buf.get();
+		dL_ddepth = t->depth_buf.get() + (size_t)camera->width * camera->height;
 	}
-	if (exposure && !t->exp_partials && (rc = regrow(&t->exp_partials, kExposurePartials, false, stream))) return rc;
+	if (exposure) PSB_CUDA_OK(t->exp_partials.grow(kExposurePartials, Fit::at_least, false, stream));
 	Scratch sc;
 	Camera cam;
 	// this pass gets its own tile backward below and its sink rows belong to this call's per-Gaussian stage (or to the _slab calls
@@ -396,17 +375,17 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, sc, cam, stream, depth_plane, nullptr,
 	                      pass_mode(t, -1, depth_loss))))
 		return rc;
-	const float* image = out_color ? out_color : t->image;
-	double* partials = t->deterministic ? t->det_partials : nullptr;
-	if ((rc = launch_loss(cam.H, cam.W, image, gt_image, mask, step->lambda_dssim, t->dmap, t->sums, t->dL_dpix, stream, partials,
+	const float* image = out_color ? out_color : t->image.get();
+	double* partials = t->deterministic ? t->det_partials.get() : nullptr;
+	if ((rc = launch_loss(cam.H, cam.W, image, gt_image, mask, step->lambda_dssim, t->dmap.get(), t->sums.get(), t->dL_dpix.get(), stream, partials,
 	                      exposure ? exposure->param : nullptr)))
 		return rc;
 	if (depth_loss &&
-	    (rc = launch_depth_loss(cam.H, cam.W, depth_plane, depth->gt_depth, mask, depth->lambda_depth, t->sums + 2, dL_ddepth, stream, partials)))
+	    (rc = launch_depth_loss(cam.H, cam.W, depth_plane, depth->gt_depth, mask, depth->lambda_depth, t->sums.get() + 2, dL_ddepth, stream, partials)))
 		return rc;
 	// loss sums -> pinned memory right behind the loss kernel, so the host can read the loss of this iteration (and start
 	// enqueueing the next one) while the backward half is still running
-	PSB_CUDA_OK(cudaMemcpyAsync(t->h_sums, t->sums, (depth_loss ? 4 : 2) * sizeof(double), cudaMemcpyDeviceToHost, stream));
+	PSB_CUDA_OK(cudaMemcpyAsync(t->h_sums.get(), t->sums.get(), (depth_loss ? 4 : 2) * sizeof(double), cudaMemcpyDeviceToHost, stream));
 	PSB_CUDA_OK(cudaEventRecord(t->readback, stream));
 	t->last_lambda = step->lambda_dssim;
 	t->last_lambda_depth = depth_loss ? depth->lambda_depth : 0.f;
@@ -415,13 +394,13 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	if (exposure) {
 		// dL/dI for the tile backward and the row's update (or gradient), inside stage "loss"; the row moves only after every read of it
 		ExposureUpdate u{exposure->param, exposure->exp_avg, exposure->exp_avg_sq, exposure->step, exposure->lr, step->beta1, step->beta2, step->eps};
-		if ((rc = launch_exposure(cam.H, cam.W, image, exposure->param, t->dL_dpix, t->exp_partials, P > 0 ? sc.geom.counters : nullptr,
-		                          (uint32_t)t->capacity, exposure_grad ? nullptr : &u, exposure_grad, stream)))
+		if ((rc = launch_exposure(cam.H, cam.W, image, exposure->param, t->dL_dpix.get(), t->exp_partials.get(), P > 0 ? sc.geom.counters : nullptr,
+		                          (uint32_t)t->bin.count(), exposure_grad ? nullptr : &u, exposure_grad, stream)))
 			return rc;
 	}
 	t->mark(5, stream);
 	if (P == 0) return 0;
-	if ((rc = tile_backward(t, P, sc, cam, background, t->dL_dpix, dL_ddepth, nullptr, stream))) return rc;
+	if ((rc = tile_backward(t, P, sc, cam, background, t->dL_dpix.get(), dL_ddepth, nullptr, stream))) return rc;
 	out.geom = sc.geom;
 	out.cam = cam;
 	return 0;
@@ -435,11 +414,11 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 struct psb_dp {
 	int rank = 0, world = 1, P = 0;
 	int nchunks = 0, nlocal_max = 0, nlocal = 0;
-	char* base = nullptr;                       // local arena (cudaMalloc: exportable through CUDA IPC)
+	CudaBuffer<char> base;                      // local arena (cudaMalloc: exportable through CUDA IPC)
 	char* peer[DP_MAX_WORLD] = {};              // arena of every rank in this process' address space (peer[rank] == base)
 	size_t off_param[6] = {}, off_inbox = 0, off_meta = 0, off_gflag = 0, off_pflag = 0, bytes = 0;
-	float* g_rest = nullptr;                    // local scratch
-	uint32_t* status = nullptr;                 // local word: 1 = a cross-rank wait timed out
+	CudaBuffer<float> g_rest;                   // local scratch
+	CudaBuffer<uint32_t> status;                // local word: 1 = a cross-rank wait timed out
 	uint32_t epoch = 0;
 	bool connected = false;
 	cudaIpcMemHandle_t handle;
@@ -469,19 +448,17 @@ int psb_dp_create(psb_dp** out, int rank, int world, int P)
 	d->nlocal_max = (d->nchunks + world - 1) / world;
 	d->nlocal = d->nchunks > rank ? (d->nchunks - rank + world - 1) / world : 0;
 	dp_layout(d);
-	cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&d->base), d->bytes);
-	if (e == cudaSuccess) e = cudaMemset(d->base, 0, d->bytes);
-	if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&d->g_rest), ((size_t)d->nlocal_max * 128 * kRestFloats + 64) * sizeof(float));
-	if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&d->status), sizeof(uint32_t));
-	if (e == cudaSuccess) e = cudaMemset(d->status, 0, sizeof(uint32_t));
-	if (e == cudaSuccess && world > 1) e = cudaIpcGetMemHandle(&d->handle, d->base);
+	// (zeroed on the legacy default stream, as cudaMemset does)
+	cudaError_t e = d->base.grow(d->bytes, Fit::exact, true, nullptr);
+	if (e == cudaSuccess) e = d->g_rest.grow((size_t)d->nlocal_max * 128 * kRestFloats + 64, Fit::exact, false, nullptr);
+	if (e == cudaSuccess) e = d->status.grow(1, Fit::exact, true, nullptr);
+	if (e == cudaSuccess && world > 1) e = cudaIpcGetMemHandle(&d->handle, d->base.get());
 	if (e != cudaSuccess) {
 		set_error("psb_dp_create", e, __FILE__, __LINE__);
-		cudaFree(d->base); cudaFree(d->g_rest); cudaFree(d->status);
 		delete d;
 		return PSB_ERR_CUDA;
 	}
-	d->peer[rank] = d->base;
+	d->peer[rank] = d->base.get();
 	d->connected = world == 1;
 	*out = d;
 	return 0;
@@ -514,7 +491,7 @@ int psb_dp_connect(psb_dp* d, const void* handles)
 int psb_dp_params(psb_dp* d, float** out6)
 {
 	if (!d || !out6) { set_error_msg("psb_dp_params: null"); return PSB_ERR_ARG; }
-	for (int i = 0; i < 6; i++) out6[i] = reinterpret_cast<float*>(d->base + d->off_param[i]);
+	for (int i = 0; i < 6; i++) out6[i] = reinterpret_cast<float*>(d->base.get() + d->off_param[i]);
 	return 0;
 }
 
@@ -524,7 +501,6 @@ int psb_dp_destroy(psb_dp* d)
 	cudaDeviceSynchronize();
 	for (int j = 0; j < d->world; j++)
 		if (j != d->rank && d->peer[j]) cudaIpcCloseMemHandle(d->peer[j]);
-	cudaFree(d->base); cudaFree(d->g_rest); cudaFree(d->status);
 	delete d;
 	return 0;
 }
@@ -535,7 +511,7 @@ int psb_dp_sync(psb_dp* d, void* stream_)
 {
 	if (!d) { set_error_msg("psb_dp_sync: null"); return PSB_ERR_ARG; }
 	if (d->epoch == 0 || d->P == 0 || d->world == 1) return 0;   // (one rank: everything is on the caller's stream)
-	return launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_pflag), d->world, d->epoch, d->status, (cudaStream_t)stream_);
+	return launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base.get() + d->off_pflag), d->world, d->epoch, d->status.get(), (cudaStream_t)stream_);
 }
 
 // 0 = healthy, 1 = a cross-rank wait timed out (a peer never arrived); synchronises the stream
@@ -543,7 +519,7 @@ int psb_dp_status(psb_dp* d, void* stream_)
 {
 	if (!d) { set_error_msg("psb_dp_status: null"); return PSB_ERR_ARG; }
 	uint32_t st = 0;
-	PSB_CUDA_OK(cudaMemcpyAsync(&st, d->status, sizeof(st), cudaMemcpyDeviceToHost, (cudaStream_t)stream_));
+	PSB_CUDA_OK(cudaMemcpyAsync(&st, d->status.get(), sizeof(st), cudaMemcpyDeviceToHost, (cudaStream_t)stream_));
 	PSB_CUDA_OK(cudaStreamSynchronize((cudaStream_t)stream_));
 	return (int)st;
 }
@@ -559,7 +535,7 @@ int psb_dp_step_depth(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* 
 	if (!d || !d->connected || P != d->P || !model) { set_error_msg("psb_dp_step: context not connected or built for a different P"); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, true))) return rc;
 	for (int i = 0; i < 6; i++)
-		if (P > 0 && model->param[i] != reinterpret_cast<float*>(d->base + d->off_param[i])) {
+		if (P > 0 && model->param[i] != reinterpret_cast<float*>(d->base.get() + d->off_param[i])) {
 			set_error_msg("psb_dp_step: the model's parameter tensors must be the arena tensors returned by psb_dp_params");
 			return PSB_ERR_ARG;
 		}
@@ -567,7 +543,7 @@ int psb_dp_step_depth(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* 
 	t->mark(psb_trainer::NSTAGE, stream);
 	// every rank's updated rows of the previous step must have landed here before this step reads the parameters
 	if (epoch > 1 && P > 0 && d->world > 1)
-		if ((rc = launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_pflag), d->world, epoch - 1, d->status, stream))) return rc;
+		if ((rc = launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base.get() + d->off_pflag), d->world, epoch - 1, d->status.get(), stream))) return rc;
 	// render, loss, tile backward (the 9 screen-space sums per Gaussian; with a depth term also dL/dz in slot 11, which the push
 	// backward below must consume: a plain push backward would leave it in the sink for the next depth step)
 	TileBackward tb;
@@ -589,18 +565,18 @@ int psb_dp_step_depth(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* 
 		for (int i = 0; i < 6; i++) sh.param[j][i] = reinterpret_cast<float*>(d->peer[j] + d->off_param[i]);
 	}
 	push.world = d->world; push.rank = d->rank; push.nlocal_max = d->nlocal_max; push.epoch = epoch;
-	sh.inbox = reinterpret_cast<const float*>(d->base + d->off_inbox);
-	sh.meta = reinterpret_cast<const float*>(d->base + d->off_meta);
-	sh.g_rest = d->g_rest;
+	sh.inbox = reinterpret_cast<const float*>(d->base.get() + d->off_inbox);
+	sh.meta = reinterpret_cast<const float*>(d->base.get() + d->off_meta);
+	sh.g_rest = d->g_rest.get();
 	sh.world = d->world; sh.rank = d->rank; sh.nlocal_max = d->nlocal_max; sh.nlocal = d->nlocal; sh.P = P; sh.epoch = epoch;
 	// push backward (records go straight into the owners' inboxes) + signal; wait until every rank's records have landed -> Adam of
 	// the owned rows, updated rows stored to every replica + signal
-	if ((rc = launch_push_backward(P, tt, tb.cam, tb.geom, t->sink, h, densify_stats(model, step), tb.geom.counters, (uint32_t)t->capacity, push, stream,
+	if ((rc = launch_push_backward(P, tt, tb.cam, tb.geom, t->sink.get(), h, densify_stats(model, step), tb.geom.counters, (uint32_t)t->bin.count(), push, stream,
 	                               t->pass)))
 		return rc;
 	t->mark(7, stream);
 	t->mark(8, stream);
-	if ((rc = launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base + d->off_gflag), d->world, epoch, d->status, stream))) return rc;
+	if ((rc = launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base.get() + d->off_gflag), d->world, epoch, d->status.get(), stream))) return rc;
 	if ((rc = launch_shard_adam(sh, tt, h, 1.0f / (float)d->world, stream, t->event(10)))) return rc;
 	t->end_stages(9, stream);
 	return 0;
@@ -621,14 +597,6 @@ int psb_trainer_create(psb_trainer** out)
 
 int psb_trainer_destroy(psb_trainer* t)
 {
-	if (!t) return 0;
-	cudaFree(t->geom_chunk); cudaFree(t->img_chunk); cudaFree(t->bin_chunk); cudaFree(t->image); cudaFree(t->dL_dpix); cudaFree(t->dmap);
-	cudaFree(t->sink); cudaFree(t->seeds); cudaFree(t->sums); cudaFree(t->ovf); cudaFree(t->depth_buf);
-	cudaFree(t->det_slots); cudaFree(t->det_base); cudaFree(t->det_partials); cudaFree(t->exp_partials);
-	if (t->ev_ready) for (int i = 0; i <= psb_trainer::NSTAGE; i++) cudaEventDestroy(t->ev[i]);
-	if (t->h_sums) cudaFreeHost(t->h_sums);
-	if (t->h_count) cudaFreeHost(t->h_count);
-	if (t->readback) cudaEventDestroy(t->readback);
 	delete t;
 	return 0;
 }
@@ -683,7 +651,7 @@ int psb_trainer_backward_pixels(psb_trainer* t, unsigned pass, int P, int M, con
 		set_error_msg("psb_trainer_backward_pixels: `pass` is not the context's latest forward pass (or the arena was regrown since)");
 		return PSB_ERR_ARG;
 	}
-	if (P != t->last_P || P != t->geom_P || camera->width != t->last_W || camera->height != t->last_H || step->sh_degree != t->pass.D) {
+	if (P != t->carved.P || camera->width != t->carved.W || camera->height != t->carved.H || step->sh_degree != t->pass.D) {
 		set_error_msg("psb_trainer_backward_pixels: P, the image size and step->sh_degree must be those of the forward pass");
 		return PSB_ERR_ARG;
 	}
@@ -712,8 +680,8 @@ int psb_trainer_backward_pixels(psb_trainer* t, unsigned pass, int P, int M, con
 	GradSegments gs{};
 	if (!adam)
 		for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
-	rc = launch_fused_backward(adam, 0, P, train_tensors(model, adam), cam, sc.geom, t->sink, t->seeds, to_hyper(step), gs, densify_stats(model, step),
-	                           sc.geom.counters, (uint32_t)t->capacity, stream, t->event(7), adam ? model->adam_live : nullptr, t->pass, reg_coef(t->pass, P));
+	rc = launch_fused_backward(adam, 0, P, train_tensors(model, adam), cam, sc.geom, t->sink.get(), t->seeds.get(), to_hyper(step), gs, densify_stats(model, step),
+	                           sc.geom.counters, (uint32_t)t->bin.count(), stream, t->event(7), adam ? model->adam_live : nullptr, t->pass, reg_coef(t->pass, P));
 	t->end_stages(8, stream);
 	return rc;
 }
@@ -745,8 +713,8 @@ int psb_trainer_step_exposure(psb_trainer* t, int P, int M, const psb_model* mod
 	                               nullptr)) ||
 	    P == 0)
 		return rc;
-	rc = launch_fused_backward(true, 0, P, train_tensors(model, true), tb.cam, tb.geom, t->sink, t->seeds, to_hyper(step), GradSegments{},
-	                           densify_stats(model, step), tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), model->adam_live, t->pass, reg_coef(t->pass, P));
+	rc = launch_fused_backward(true, 0, P, train_tensors(model, true), tb.cam, tb.geom, t->sink.get(), t->seeds.get(), to_hyper(step), GradSegments{},
+	                           densify_stats(model, step), tb.geom.counters, (uint32_t)t->bin.count(), stream, t->event(7), model->adam_live, t->pass, reg_coef(t->pass, P));
 	t->end_stages(8, stream);
 	return rc;
 }
@@ -783,8 +751,8 @@ int psb_trainer_backward_exposure(psb_trainer* t, int P, int M, const psb_model*
 		return rc;
 	GradSegments gs;
 	for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
-	rc = launch_fused_backward(false, 0, P, train_tensors(model, false), tb.cam, tb.geom, t->sink, t->seeds, to_hyper(step), gs, densify_stats(model, step),
-	                           tb.geom.counters, (uint32_t)t->capacity, stream, t->event(7), nullptr, t->pass, reg_coef(t->pass, P));
+	rc = launch_fused_backward(false, 0, P, train_tensors(model, false), tb.cam, tb.geom, t->sink.get(), t->seeds.get(), to_hyper(step), gs, densify_stats(model, step),
+	                           tb.geom.counters, (uint32_t)t->bin.count(), stream, t->event(7), nullptr, t->pass, reg_coef(t->pass, P));
 	t->end_stages(8, stream);
 	return rc;
 }
@@ -820,17 +788,17 @@ int psb_trainer_backward_slab(psb_trainer* t, int P, int M, const psb_model* mod
                               int count, float* const* grads, void* stream_)
 {
 	int rc;
-	if (!t || !camera || !step || !grads || t->geom_P != P) { set_error_msg("psb_trainer_backward_slab: bad argument / no matching backward_begin"); return PSB_ERR_ARG; }
+	if (!t || !camera || !step || !grads || t->carved.P != P) { set_error_msg("psb_trainer_backward_slab: bad argument / no matching backward_begin"); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, false))) return rc;
 	if ((rc = refuse_filter3d(t, "psb_trainer_backward_slab"))) return rc;
 	if (first < 0 || count < 0 || first + count > P || (first % 128) != 0) { set_error_msg("psb_trainer_backward_slab: slab must start at a multiple of 128"); return PSB_ERR_ARG; }
 	if (count == 0) return 0;
 	if ((rc = check_grads(grads, count, "psb_trainer_backward_slab"))) return rc;
-	const GeomState geom = carve_scratch(t, P, t->last_W, t->last_H).geom;
+	const GeomState geom = carve_scratch(t, P, t->carved.W, t->carved.H).geom;
 	GradSegments gs;
 	for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
-	return launch_fused_backward(false, first, first + count, train_tensors(model, false), to_camera(camera), geom, t->sink, t->seeds, to_hyper(step), gs,
-	                             densify_stats(model, step), geom.counters, (uint32_t)t->capacity, (cudaStream_t)stream_, nullptr, nullptr, t->pass, reg_coef(t->pass, P));
+	return launch_fused_backward(false, first, first + count, train_tensors(model, false), to_camera(camera), geom, t->sink.get(), t->seeds.get(), to_hyper(step), gs,
+	                             densify_stats(model, step), geom.counters, (uint32_t)t->bin.count(), (cudaStream_t)stream_, nullptr, nullptr, t->pass, reg_coef(t->pass, P));
 }
 
 int psb_adam_update(int P, int M, const psb_model* model, float* const* grads, const psb_step* step, float grad_scale, void* stream_)
@@ -857,11 +825,12 @@ int psb_adam_flat(size_t n, float* param, float* exp_avg, float* exp_avg_sq, con
 static int result_impl(psb_trainer* t, float* out, bool with_depth, int* num_rendered, void* stream_)
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
-	if (!t || t->geom_P < 0) { set_error_msg("psb_trainer_result: no step has run"); return PSB_ERR_ARG; }
+	if (!t || t->carved.P < 0) { set_error_msg("psb_trainer_result: no step has run"); return PSB_ERR_ARG; }
 	PSB_CUDA_OK(cudaEventSynchronize(t->readback));
-	const uint32_t n = t->geom_P > 0 ? t->h_count[0] : 0;
+	uint32_t* const h_count = t->h_count.get();
+	const uint32_t n = t->carved.P > 0 ? h_count[0] : 0;
 	if (num_rendered) *num_rendered = (int)n;
-	const uint32_t n_ovf = t->geom_P > 0 ? t->h_count[1] : 0;
+	const uint32_t n_ovf = t->carved.P > 0 ? h_count[1] : 0;
 	if (n_ovf > 0) {
 		// One or more views since the last collection needed more instances than the binning arena holds: those calls were
 		// no-ops on the model (fused step) / contributed zero gradients (data-parallel modes). The record is sticky on the device,
@@ -870,23 +839,26 @@ static int result_impl(psb_trainer* t, float* out, bool with_depth, int* num_ren
 		PSB_CUDA_OK(cudaStreamSynchronize(stream));
 		PSB_CUDA_OK(cudaDeviceSynchronize());
 		uint32_t rec[3];
-		PSB_CUDA_OK(cudaMemcpy(rec, t->ovf, sizeof(rec), cudaMemcpyDeviceToHost));
+		PSB_CUDA_OK(cudaMemcpy(rec, t->ovf.get(), sizeof(rec), cudaMemcpyDeviceToHost));
 		t->ovf_count = rec[0]; t->ovf_first = rec[1];
 		const uint32_t init[4] = {0u, 0xFFFFFFFFu, 0u, 0u};
-		PSB_CUDA_OK(cudaMemcpy(t->ovf, init, sizeof(init), cudaMemcpyHostToDevice));
-		t->h_count[1] = 0;
+		PSB_CUDA_OK(cudaMemcpy(t->ovf.get(), init, sizeof(init), cudaMemcpyHostToDevice));
+		h_count[1] = 0;
 		t->pass.D = -1;   // the scratch of the last pass is gone: no psb_trainer_backward_pixels for it
-		t->capacity = (size_t)(rec[2] * 1.25) + (1u << 16);
-		t->bin_bytes = required_bytes<BinState>(t->capacity);
-		int rc;
-		if ((rc = regrow(&t->bin_chunk, t->bin_bytes, false, stream))) return rc;
+		const cudaError_t e = t->bin.grow((size_t)(rec[2] * 1.25) + (1u << 16), Fit::exact, false, stream);
+		if (e != cudaSuccess) {
+			t->carved = {};   // no binning chunk: nothing may read the last pass's scratch
+			set_error("psb_trainer_result: growing the binning arena", e, __FILE__, __LINE__);
+			return PSB_ERR_CUDA;
+		}
 		set_error_msg("psb_trainer: binning arena was too small for a view; it has been grown, repeat the call (psb_trainer_overflow_info says which)");
 		return PSB_ERR_RETRY;
 	}
 	if (out && t->have_loss) {
-		const double inv_n = 1.0 / (3.0 * (double)t->last_W * (double)t->last_H);
-		const float l1 = (float)(t->h_sums[0] * inv_n), ss = (float)(t->h_sums[1] * inv_n);
-		const float dl1 = t->have_depth_loss ? (float)(t->h_sums[2] / (t->h_sums[3] > 1.0 ? t->h_sums[3] : 1.0)) : 0.f;
+		const double* h_sums = t->h_sums.get();
+		const double inv_n = 1.0 / (3.0 * (double)t->carved.W * (double)t->carved.H);
+		const float l1 = (float)(h_sums[0] * inv_n), ss = (float)(h_sums[1] * inv_n);
+		const float dl1 = t->have_depth_loss ? (float)(h_sums[2] / (h_sums[3] > 1.0 ? h_sums[3] : 1.0)) : 0.f;
 		out[0] = (1.0f - t->last_lambda) * l1 + t->last_lambda * (1.0f - ss);
 		if (t->have_depth_loss) out[0] += t->last_lambda_depth * dl1;
 		out[1] = l1;
@@ -926,8 +898,8 @@ __global__ void export_last_splat_kernel(int W, int H, int grid_x, const uint2* 
 int psb_trainer_debug_state(psb_trainer* t, int width, int height, int* last_gauss, float* final_T, int* num_rendered, void* stream_)
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
-	if (!t || t->geom_P < 0 || t->last_W != width || t->last_H != height) { set_error_msg("psb_trainer_debug_state: no step of that size has run"); return PSB_ERR_ARG; }
-	const Scratch sc = carve_scratch(t, t->geom_P, width, height);
+	if (!t || t->carved.P < 0 || t->carved.W != width || t->carved.H != height) { set_error_msg("psb_trainer_debug_state: no step of that size has run"); return PSB_ERR_ARG; }
+	const Scratch sc = carve_scratch(t, t->carved.P, width, height);
 	export_last_splat_kernel<<<(width * height + 255) / 256, 256, 0, stream>>>(width, height, tile_grid(width, height).x, sc.img.ranges,
 	                                                                        sc.bin.inst[sorted_slot(width, height)], sc.img.n_contrib, sc.img.final_T,
 	                                                                        last_gauss, final_T);
@@ -952,7 +924,14 @@ int psb_trainer_set_profiling(psb_trainer* t, int enable)
 {
 	if (!t) return PSB_ERR_ARG;
 	if (enable && !t->ev_ready) {
-		for (int i = 0; i <= psb_trainer::NSTAGE; i++) PSB_CUDA_OK(cudaEventCreate(&t->ev[i]));
+		for (int i = 0; i <= psb_trainer::NSTAGE; i++) {
+			const cudaError_t e = cudaEventCreate(&t->ev[i]);
+			if (e != cudaSuccess) {   // all of them or none
+				while (i-- > 0) cudaEventDestroy(t->ev[i]);
+				set_error("cudaEventCreate(&t->ev[i])", e, __FILE__, __LINE__);
+				return PSB_ERR_CUDA;
+			}
+		}
 		t->ev_ready = true;
 	}
 	t->profiling = enable != 0;
@@ -999,15 +978,15 @@ int psb_trainer_inject_noise(psb_trainer* t, int P, const psb_model* model, floa
 		set_error_msg("psb_trainer_inject_noise: a context, a model, P >= 0 and finite lr_xyz, noise_lr >= 0 required");
 		return PSB_ERR_ARG;
 	}
-	if (t->geom_P != P || t->last_P != P) { set_error_msg("psb_trainer_inject_noise: the context's latest pass was not over P rows"); return PSB_ERR_ARG; }
+	if (t->carved.P != P) { set_error_msg("psb_trainer_inject_noise: the context's latest pass was not over P rows"); return PSB_ERR_ARG; }
 	if (P == 0) return 0;
 	if (!model->param[0] || !model->param[3] || !model->param[4] || !model->param[5] || (reinterpret_cast<uintptr_t>(model->param[5]) & 15)) {
 		set_error_msg("psb_trainer_inject_noise: xyz, opacity, scaling and a 16-byte aligned rotation tensor required");
 		return PSB_ERR_ARG;
 	}
-	const GeomState geom = carve_scratch(t, P, t->last_W, t->last_H).geom;
+	const GeomState geom = carve_scratch(t, P, t->carved.W, t->carved.H).geom;
 	return launch_position_noise(P, model->param[0], model->param[3], model->param[4], model->param[5], lr_xyz * noise_lr, seed, step,
-	                             visible_only ? geom.tile_info : nullptr, geom.counters, (uint32_t)t->capacity, (cudaStream_t)stream_);
+	                             visible_only ? geom.tile_info : nullptr, geom.counters, (uint32_t)t->bin.count(), (cudaStream_t)stream_);
 }
 
 // ms[i] = time between stage boundaries i and i+1 of the last profiled step (see psb_trainer::ev), i < n; entries beyond the last
@@ -1032,31 +1011,25 @@ int psb_loss(int height, int width, const float* image, const float* gt_image, c
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
 	if (height <= 0 || width <= 0 || !image || !gt_image) { set_error_msg("psb_loss: bad argument"); return PSB_ERR_ARG; }
-	float* dmap = nullptr;
-	double* sums = nullptr;
 	const size_t N = (size_t)height * width;
-	// stream-ordered scratch: no device-wide synchronisation, freed on every path
-	PSB_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&dmap), 9 * N * sizeof(float), stream));
-	if (cudaMallocAsync(reinterpret_cast<void**>(&sums), 2 * sizeof(double), stream) != cudaSuccess) {
-		cudaFreeAsync(dmap, stream);
-		set_error_msg("psb_loss: out of device memory");
-		return PSB_ERR_CUDA;
-	}
-	int rc = launch_loss(height, width, image, gt_image, mask, lambda_dssim, dmap, sums, dL_dimage, stream, nullptr, nullptr);
+	// stream-ordered scratch: no device-wide synchronisation
+	StreamScratch<float> dmap(stream);
+	StreamScratch<double> sums(stream);
+	PSB_CUDA_OK(dmap.alloc(9 * N));
+	if (sums.alloc(2) != cudaSuccess) { set_error_msg("psb_loss: out of device memory"); return PSB_ERR_CUDA; }
+	int rc;
+	if ((rc = launch_loss(height, width, image, gt_image, mask, lambda_dssim, dmap.get(), sums.get(), dL_dimage, stream, nullptr, nullptr))) return rc;
 	double h[2] = {0, 0};
-	if (rc == 0) {
-		cudaMemcpyAsync(h, sums, sizeof(h), cudaMemcpyDeviceToHost, stream);
-		if (cudaStreamSynchronize(stream) != cudaSuccess) rc = PSB_ERR_CUDA;
-	}
-	cudaFreeAsync(dmap, stream); cudaFreeAsync(sums, stream);
-	if (rc == 0 && out3_host) {
+	cudaMemcpyAsync(h, sums.get(), sizeof(h), cudaMemcpyDeviceToHost, stream);
+	if (cudaStreamSynchronize(stream) != cudaSuccess) return PSB_ERR_CUDA;
+	if (out3_host) {
 		const double inv_n = 1.0 / (3.0 * (double)N);
 		const float l1 = (float)(h[0] * inv_n), ss = (float)(h[1] * inv_n);
 		out3_host[0] = (1.0f - lambda_dssim) * l1 + lambda_dssim * (1.0f - ss);
 		out3_host[1] = l1;
 		out3_host[2] = ss;
 	}
-	return rc;
+	return 0;
 }
 
 }  // extern "C"
