@@ -659,6 +659,29 @@ int psb_filter3d(int P, const float* xyz, int K, const float* cams, float* filte
 int psb_trainer_set_filter3d(psb_trainer* t, const float* filter, int P);
 
 /* ------------------------------------------------------------------------------------------------
+ * Contribution scores: how much each Gaussian shows in a set of views, for pruning the ones no view shows.
+ * For one pass (view) and one pixel p, Gaussian i blends with w_i(p) = alpha_i(p) T_i(p): exactly the factor the forward multiplies
+ * its colour by (C = fma(T, c alpha, C)), T the transmittance before the splat, alpha that of the pass (anti-aliased opacity o h and
+ * 3D-filtered opacity o c in those modes, the 0.99 clamp). Only (pixel, splat) pairs that blend count: not those with power > 0,
+ * below pmin, with alpha < 1/255, nor the pair whose T test (T (1 - alpha) < 1e-4) ends the pixel. Over the passes of a sweep:
+ *   max_weight[i] = max w_i(p) over all pixels and views, as the bits of a float32 (0 = never blended);
+ *   sum_weight[i] = sum w_i(p) over all pixels and views, in units of 2^-PSB_CONTRIB_SUM_FRAC_BITS, each pixel's w truncated
+ *                   (floor(w 2^26)) before it is added.
+ * Both are integers accumulated with integer atomics (atomicMax on the bits: non-negative floats order like their bits; a u64 add), so
+ * a sweep's result is bit-identical from run to run, in either deterministic mode and in any order of the views, and sums of
+ * separate sweeps add exactly. A weight is at least 1e-4 / 255 (about 26 units), so every blended pair adds to the sum.
+ * ------------------------------------------------------------------------------------------------ */
+#define PSB_CONTRIB_SUM_FRAC_BITS 26
+/* One pass of the sweep: psb_trainer_render of the view (in the context's anti-aliasing and 3D-filter modes; an ordinary forward pass of
+ * the context, with the same colour, final T and last contributors) that also ADDS this view's scores into max_weight [P] (u32) and
+ * sum_weight [P] (u64), device arrays the caller zeroes once per sweep. out_color [3,H,W] device, or NULL: the context's own image.
+ * Asynchronous (no host synchronisation). A pass that overflows the binning arena adds nothing and is reported by psb_trainer_result
+ * like a render: zero the arrays and repeat the sweep on the grown arena. PSB_ERR_ARG, before any CUDA call, for a NULL context,
+ * camera, background, max_weight or sum_weight, P < 0, and a P that differs from the context's 3D filter's. */
+int psb_trainer_contribution(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                             int sh_degree, uint32_t* max_weight, uint64_t* sum_weight, float* out_color, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Point-cloud helpers exported by the same shared objects in the reference.
  * ------------------------------------------------------------------------------------------------ */
 

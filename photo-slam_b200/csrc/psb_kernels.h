@@ -47,6 +47,14 @@ struct DetSlots {
 	int P, tight;
 };
 
+// Where the score pass of the forward tile kernel adds its contribution scores (include/psb200.h, psb_trainer_contribution): [P] each.
+struct ScoreSink {
+	uint32_t* max;             // largest blending weight, as the bits of a non-negative float (atomicMax)
+	unsigned long long* sum;   // summed blending weight in units of 2^-kScoreFracBits, each pixel's weight truncated (atomicAdd)
+};
+constexpr int kScoreFracBits = 26;   // PSB_CONTRIB_SUM_FRAC_BITS
+constexpr float kScoreUnitsPerWeight = (float)(1u << kScoreFracBits);
+
 // Outputs of the per-Gaussian backward (any pointer may be null = not wanted).
 struct GaussGradOut {
 	float* dL_dmeans3D;  // [P,3]
@@ -99,7 +107,8 @@ int launch_scan_binning(int P, const Camera& cam, const GeomState& geom, BinStat
 int launch_render_forward(const Camera& cam, const uint2* ranges, const uint32_t* point_list, const GaussRec* rec, const float* bg,
                           float* out_color, float* final_T, uint32_t* n_contrib, cudaStream_t stream,
                           float* out_depth = nullptr /* [H,W]: also render the expected depth (depth variant of the kernel) */,
-                          float* out_alpha = nullptr /* [H,W]: also write the accumulated opacity 1 - final_T (opacity variant) */);
+                          float* out_alpha = nullptr /* [H,W]: also write the accumulated opacity 1 - final_T (opacity variant) */,
+                          const ScoreSink* score = nullptr /* also add the contribution scores (score variant; no depth or opacity) */);
 // dL_ddepth [H,W]: depth variant, dL/dz of every Gaussian lands in slot 11 of its packed sink row, or at sink.z (unpacked sink;
 // refused without either destination). det != null: the deterministic variant — slot stores, then the ordered gather, which WRITES the
 // sink rows (packed: gather_slots_kernel; unpacked: gather_slots_unpacked_kernel, dL/dz at sink.z with dL_ddepth). dL_dalpha [H,W]: opacity variant, the gradient of the accumulated opacity 1 - final_T joins dL/dalpha of every splat

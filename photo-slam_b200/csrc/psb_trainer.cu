@@ -276,9 +276,11 @@ int refuse_filter3d(const psb_trainer* t, const char* fn)
 
 // Stage 1 of every pass: forward of SH degree D from raw parameters into t->image (or out_color); out_depth != NULL: the depth variant
 // also writes the expected depth there; out_alpha != NULL: the opacity variant also writes 1 - final_T there. The pass is recorded as
-// `mode`, with D = -1 until it has been binned.
+// `mode`, with D = -1 until it has been binned. score != NULL: the score variant also adds the contribution scores there (no depth or
+// opacity plane).
 int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, const psb_camera* camera, const float* background,
-                float* out_color, int* radii, Scratch& sc, Camera& cam, cudaStream_t stream, float* out_depth, float* out_alpha, const PassMode& mode)
+                float* out_color, int* radii, Scratch& sc, Camera& cam, cudaStream_t stream, float* out_depth, float* out_alpha, const PassMode& mode,
+                const ScoreSink* score = nullptr)
 {
 	int rc;
 	t->pass = mode;
@@ -304,7 +306,7 @@ int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, con
 	PSB_CUDA_OK(cudaMemcpyAsync(t->h_count.get() + 1, t->ovf.get(), 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
 	PSB_CUDA_OK(cudaEventRecord(t->readback, stream));
 	rc = launch_render_forward(cam, img.ranges, bin.inst[sorted_slot(cam.W, cam.H)], geom.rec, background, out_color ? out_color : t->image.get(), img.final_T,
-	                           img.n_contrib, stream, out_depth, out_alpha);
+	                           img.n_contrib, stream, out_depth, out_alpha, score);
 	t->mark(4, stream);
 	return rc;
 }
@@ -637,6 +639,25 @@ int psb_trainer_render_depth(psb_trainer* t, int P, int M, const psb_model* mode
 {
 	return forward_impl("psb_trainer_render_depth", t, P, M, model, camera, background, sh_degree, out_color, radii, out_depth, nullptr, nullptr,
 	                    (cudaStream_t)stream_);
+}
+
+static_assert(kScoreFracBits == PSB_CONTRIB_SUM_FRAC_BITS, "the score kernel's fixed-point unit is the header's");
+
+int psb_trainer_contribution(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
+                             uint32_t* max_weight, uint64_t* sum_weight, float* out_color, void* stream_)
+{
+	const char* fn = "psb_trainer_contribution";
+	int rc;
+	if (!t || !camera || !background || !max_weight || !sum_weight) { set_error_msg("psb_trainer_contribution: null argument"); return PSB_ERR_ARG; }
+	if (P < 0) { set_error_msg("psb_trainer_contribution: need P >= 0"); return PSB_ERR_ARG; }
+	if ((rc = check_model(P, M, model, false))) return rc;
+	if ((rc = check_filter3d(t, P, fn))) return rc;
+	Scratch sc;
+	Camera cam;
+	t->have_loss = false;
+	const ScoreSink score{max_weight, reinterpret_cast<unsigned long long*>(sum_weight)};
+	return forward_raw(t, P, M, sh_degree, model, camera, background, out_color, nullptr, sc, cam, (cudaStream_t)stream_, nullptr, nullptr,
+	                   pass_mode(t, sh_degree, false), &score);
 }
 
 int psb_trainer_backward_pixels(psb_trainer* t, unsigned pass, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,

@@ -100,6 +100,38 @@ class _RelocateCfg(C.Structure):
     _fields_ = [("min_opacity", C.c_float), ("iteration", C.c_int), ("seed", C.c_ulonglong), ("offset", C.c_ulonglong)]
 
 
+# The unit of the summed contribution score (include/psb200.h, PSB_CONTRIB_SUM_FRAC_BITS = 26).
+CONTRIB_SUM_UNIT = 2.0 ** -26
+
+
+def _check_cams(cams, what):
+    """cams: a non-empty list of camera dicts in the form GaussianTrainer takes (ValueError otherwise, before any C call)."""
+    if not isinstance(cams, (list, tuple)) or not cams:
+        raise ValueError(f"{what}: want a non-empty list of camera dicts")
+    for k, cam in enumerate(cams):
+        try:
+            W, H = cam["W"], cam["H"]
+            for key in ("viewmatrix", "projmatrix", "campos", "tanfovx", "tanfovy"):
+                cam[key]
+        except (KeyError, TypeError) as e:
+            raise ValueError(f"{what}: camera {k} is not a camera dict (viewmatrix, projmatrix, campos, tanfovx, tanfovy, W, H): {e}") from None
+        if isinstance(W, bool) or isinstance(H, bool) or int(W) != W or int(H) != H or W <= 0 or H <= 0:
+            raise ValueError(f"{what}: camera {k}: W and H must be positive integers, got {W}, {H}")
+    return list(cams)
+
+
+def contribution_prune_mask(max_weight, sum_weight, min_weight, keep=None, young=None):
+    """bool [P], True = remove: the rows whose max_weight < min_weight and, with keep, every row but the `keep` of highest sum_weight (ties
+    go to the lower row index). Rows marked in `young` (bool [P] or None) are never removed."""
+    mask = max_weight < min_weight
+    if keep is not None and keep < mask.numel():
+        order = torch.sort(sum_weight, descending=True, stable=True).indices
+        mask[order[keep:]] = True
+    if young is not None:
+        mask &= ~young
+    return mask
+
+
 def _bind():
     """The library with every trainer, data-parallel, densification and debug entry point declared (include/psb200.h)."""
     L = _lib.lib()
@@ -139,6 +171,7 @@ def _bind():
         "psb_trainer_set_regularizers": [vp, f, f],
         "psb_trainer_set_filter3d": [vp, vp, i],
         "psb_filter3d": [i, vp, i, vp, vp, P(i), vp],
+        "psb_trainer_contribution": [vp, i, i, Model, Cam, vp, i, vp, vp, vp, vp],
         "psb_trainer_inject_noise": [vp, i, Model, f, f, ull, ull, i, vp],
         "psb_adam_update": [i, i, Model, P(vp), Step, f, vp],
         "psb_adam_flat": [size_t, vp, vp, vp, vp, f, Step, f, vp],
@@ -766,6 +799,60 @@ class GaussianTrainer:
         n_add = m.addNewGaussians(o.cap_max, o.mcmc_grow_factor, o.mcmc_min_opacity, seed=o.mcmc_seed, iteration=it)
         return n_rel, n_add
 
+    # --- contribution pruning (include/psb200.h, psb_trainer_contribution): a Gaussian's score is the blending weight alpha T it receives in
+    #     the pixels of the keyframes, in this trainer's own forward (tight lists, anti-aliasing, 3D filter). When and on which keyframes to
+    #     prune is the caller's choice, as with computeFilter3D.
+    def contributionScores(self, cams):
+        """cams: a non-empty list of camera dicts (the form trainForOneIteration takes). -> (max_weight [P] float32, sum_weight [P] float64):
+        the largest and the summed blending weight of every row over all pixels of all views (0: no view blends it). Bit-identical from run
+        to run, in either deterministic mode and in any order of the views. One host round trip for the whole sweep; if a view overflowed the
+        binning arena, the sweep is repeated once on the grown arena."""
+        cams = _check_cams(cams, "contributionScores")
+        m = self.model
+        P = m.num_points()
+        mx = torch.zeros(P, dtype=torch.int32, device=m.device)
+        sm = torch.zeros(P, dtype=torch.int64, device=m.device)
+        if P > 0:
+            self._hand_filter3d()
+            cm = m._cmodel(False)
+            stream = torch.cuda.current_stream().cuda_stream
+            self._last = _NO_CALL
+            for attempt in range(2):
+                for cam in cams:
+                    cc = _ccamera(cam)
+                    _lib.check(self.L.psb_trainer_contribution(self.h, P, 16, C.byref(cm), C.byref(cc), self.background.data_ptr(), m.active_sh_degree_,
+                                                               mx.data_ptr(), sm.data_ptr(), None, stream), "psb_trainer_contribution")
+                rc = self.L.psb_trainer_result(self.h, None, None, stream)
+                if rc != -4:
+                    _lib.check(rc, "psb_trainer_result")
+                    break
+                if attempt:
+                    raise _lib.PsbError("contributionScores: a view overflowed the binning arena again after it was grown")
+                mx.zero_()
+                sm.zero_()
+        return mx.view(torch.float32), sm.to(torch.float64) * CONTRIB_SUM_UNIT
+
+    def pruneByContribution(self, cams, min_weight, keep=None, min_age=0):
+        """Removes the rows that no view in `cams` shows: max_weight < min_weight (contributionScores) and, with keep, all but the `keep`
+        rows of highest sum_weight (ties: the lower row index stays). Rows younger than min_age iterations (iteration - exist_since_iter_ <
+        min_age) are never removed. Goes through model.prunePoints (statistics compacted, live bytes and 3D filter dropped). Returns the
+        number of rows removed."""
+        if isinstance(min_weight, bool) or not isinstance(min_weight, (int, float)) or not math.isfinite(min_weight) or not 0 <= min_weight < 1:
+            raise ValueError(f"pruneByContribution: min_weight must be finite and in [0, 1), got {min_weight!r}")
+        if keep is not None and (isinstance(keep, bool) or not isinstance(keep, int) or keep <= 0):
+            raise ValueError(f"pruneByContribution: keep must be a positive int or None, got {keep!r}")
+        if isinstance(min_age, bool) or not isinstance(min_age, int) or min_age < 0:
+            raise ValueError(f"pruneByContribution: min_age must be an int >= 0, got {min_age!r}")
+        cams = _check_cams(cams, "pruneByContribution")
+        m = self.model
+        mx, sm = self.contributionScores(cams)
+        young = (self.iteration - m._exist()) < min_age if min_age > 0 else None
+        mask = contribution_prune_mask(mx, sm, float(min_weight), keep, young)
+        n = int(mask.sum())
+        if n:
+            m.prunePoints(mask)
+        return n
+
     @property
     def antialiasing(self):
         """Whether this trainer's passes use the 2D Mip filter (set at construction)."""
@@ -1178,6 +1265,16 @@ class DataParallelTrainer(GaussianTrainer):
         ordered behind every rank's rows (device-side wait)."""
         self.sync()
         return super().render(cam, out, radii, check, out_depth, out_alpha)
+
+    def contributionScores(self, cams):
+        """As in GaussianTrainer, on the complete replica (ordered behind every rank's rows, like render)."""
+        self.sync()
+        return super().contributionScores(cams)
+
+    def pruneByContribution(self, cams, min_weight, keep=None, min_age=0):
+        raise NotImplementedError("DataParallelTrainer.pruneByContribution: pruning is not wired into the data-parallel steps (in p2p mode the "
+                                  "parameters live in the IPC arena, and every rank would need the same mask: an exact all-reduce of the "
+                                  "integer scores, then rebuild()); score with contributionScores and prune on one GPU through GaussianTrainer")
 
     def gather_moments(self):
         """Every rank receives the Adam moments of all rows (they are only maintained on the owner): call before
