@@ -556,6 +556,53 @@ int psb_reset_opacity(int P, float* opacity, float* exp_avg, float* exp_avg_sq, 
  * PSB_ERR_ARG has enqueued nothing and written no device memory. */
 
 /* ------------------------------------------------------------------------------------------------
+ * Depth-guided seeding: new Gaussians on the pixels of an RGB-D keyframe that the map does not explain (the dense rule of SplaTAM,
+ * Gaussian-SLAM and MonoGS: where the map's silhouette is weak, or where the sensor sees a surface in front of the map's). The reference
+ * only adds rows at ORB keypoints, so a textureless wall, floor or ceiling never gets any.
+ * Inputs: a camera (any pyramid level, W x H), A and D [H,W] = the accumulated opacity and the depth sum_i z_i alpha_i T_i the map renders
+ * from it (psb_trainer_forward), G [H,W] = the keyframe's depth in metres (<= 0: no measurement), its image [3,H,W] and an optional mask
+ * [3,H,W] of which only mask[0] is read (the depth loss's convention: mask[0,p] == 0 makes p unusable).
+ *   grid      only pixels (u, v) with u % stride == 0 and v % stride == 0 are considered;
+ *   valid     G finite, min_depth < G < max_depth, and not masked out;
+ *   hole      A < alpha_min;
+ *   in front  A >= alpha_min and __fmul_rn(G, A) < __fmul_rn(k, D), k = 1 - depth_rel formed in float32 on the host, each product rounded
+ *             on its own (no FMA): the sensor sees a surface nearer than the map's normalised depth D / A by more than depth_rel
+ *             (depth_rel = 1 turns the test off);
+ *   selected  valid and (hole or in front).
+ * Order and cap: the selected pixels are ranked in raster order (v W + u); with c selected and n <= c kept, the pixel of rank k is kept
+ * iff floor((k + 1) n / c) > floor(k n / c) (64-bit integers): exactly n pixels, spread evenly over the image; n = c keeps all.
+ * The row of a kept pixel (u, v), z = G(u, v): fx = W / (2 tan_fovx), fy = H / (2 tan_fovy);
+ *   camera point (x, y, z) = ((u + 0.5 - W / 2) z / fx, (v + 0.5 - H / 2) z / fy, z): the exact inverse of the forward's projection
+ *   (ndc_to_pix's half pixel included), so the centre projects onto the centre of pixel (u, v) at depth z;
+ *   world point xyz = R^T (p - t), R[r][c] = viewmatrix[4 c + r], t[r] = viewmatrix[12 + r] (a rigid view matrix);
+ *   colour = image(u, v); dist2 = (stride z / ((fx + fy) / 2))^2, i.e. an isotropic scale of one grid cell's footprint at depth z;
+ *   everything else is psb_insert_points: features_dc = RGB2SH(colour), features_rest = 0, opacity = logit(0.1), rotation = (1,0,0,0),
+ *   zero moments, exist_since_iter = iteration, the statistics of all rows zeroed. dst = the P rows of src (bit for bit) followed by the
+ *   n new rows in the order of their rank.
+ * No float atomics: the result is bit-identical from run to run and independent of the launch configuration.
+ * psb_seed_plan selects and counts: counts_host[3] = {selected, holes, in front}; its read-back of the counts is the one host round trip.
+ * psb_seed_apply writes dst (P + n rows) from src and the plan in `workspace`; asynchronous. The library remembers on the host, for the
+ * last 16 workspaces planned, the camera size, the stride and the selected count of their plan; apply refuses a workspace without one.
+ * workspace: psb_seed_workspace_bytes(W, H, stride) device bytes (0 for a bad size or stride), the same buffer for plan and apply.
+ * Both return PSB_ERR_ARG, before any CUDA call, for a config outside the ranges below (NaN included), a missing camera, plane,
+ * workspace or count array, and (apply) a view matrix missing, a tan_fov not finite and positive, n < 0, n > max_new, n above the plan's
+ * selected count, and everything psb_insert_points rejects.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct psb_seed_cfg {
+	float alpha_min;    /* (0, 1]: hole below this accumulated opacity */
+	float depth_rel;    /* [0, 1]: in front when G < (1 - depth_rel) D / A */
+	float min_depth;    /* >= 0 */
+	float max_depth;    /* > min_depth */
+	int stride;         /* >= 1 */
+	int max_new;        /* >= 0: apply adds at most this many rows */
+} psb_seed_cfg;
+size_t psb_seed_workspace_bytes(int width, int height, int stride);
+int psb_seed_plan(const psb_camera* camera, const float* alpha, const float* depth, const float* gt_depth, const float* mask,
+                  const psb_seed_cfg* cfg, void* workspace, int* counts_host, void* stream);
+int psb_seed_apply(int P, const psb_model* src, const psb_model* dst, int n, const psb_camera* camera, const float* gt_image,
+                   const float* gt_depth, const psb_seed_cfg* cfg, const void* workspace, int iteration, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Bounded-budget densification: relocation of dead Gaussians and growth to a cap (3DGS-MCMC, Kheradmand et al., NeurIPS 2024; the
  * semantics of gsplat's MCMCStrategy relocate / sample_add). The reference has no counterpart. With o = sigmoid(opacity) and
  * s = exp(scaling), a row is DEAD when o <= min_opacity and ALIVE otherwise.

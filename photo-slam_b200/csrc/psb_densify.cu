@@ -22,7 +22,9 @@
 //                           split children get xyz = R(q) (z * exp(s)) + xyz and scaling = log(exp(s) / 1.6) (:733-738), with z
 //                           either injected (tests: same numbers as the oracle) or drawn from Philox4x32-10 + Box-Muller keyed by
 //                           (seed, offset, child row) — counter-based, so every data-parallel replica draws identical samples.
+#include <climits>
 #include <cmath>
+#include <mutex>
 #include <string>
 #include "psb_common.cuh"
 #include "../../include/psb200.h"
@@ -305,6 +307,97 @@ __global__ void insert_fill_kernel(int P, int n, const float* __restrict__ point
 	t.dp[3][d] = op;
 	reinterpret_cast<float4*>(t.dp[5])[d] = make_float4(1.f, 0.f, 0.f, 0.f);
 	if (t.dexist) t.dexist[d] = iteration;
+}
+
+// ------------------------------------------------------------------------------------------------------------------------
+// Depth-guided seeding (include/psb200.h, psb_seed_*): the pixels of an RGB-D keyframe that the map does not explain become new rows
+// through the insert body above. Both kernels walk the stride grid, g = gv * gw + gu for the pixel (gu * stride, gv * stride); g grows
+// with the raster index v * W + u, so the rank of a pixel among the selected ones is its rank in g. Counts per block of 128 grid pixels
+// are [selected, holes, in front, 0], the [nblocks][4] shape densify_scan_kernel scans. No atomics: the result does not depend on the
+// launch configuration.
+// ------------------------------------------------------------------------------------------------------------------------
+constexpr uint8_t SEED_HOLE = 1, SEED_FRONT = 2;
+
+struct SeedGrid {
+	int W, H, stride, gw, ng;   // image size, stride, grid width, grid pixels
+};
+
+struct SeedTest {
+	float alpha_min, k, min_depth, max_depth;   // k = 1 - depth_rel, formed in float32 on the host
+};
+
+__global__ void __launch_bounds__(DN_TB) seed_mask_kernel(SeedGrid g, SeedTest s, const float* __restrict__ alpha, const float* __restrict__ depth,
+                                                        const float* __restrict__ gt_depth, const float* __restrict__ mask,
+                                                        uint8_t* __restrict__ flags, uint32_t* __restrict__ block_counts)
+{
+	__shared__ uint32_t s_cnt[DN_TB / 32][3];
+	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	const int i = blockIdx.x * DN_TB + tid;
+	uint32_t f = 0;
+	if (i < g.ng) {
+		const int gv = i / g.gw, gu = i - gv * g.gw;
+		const size_t idx = (size_t)gv * g.stride * g.W + (size_t)gu * g.stride;
+		const float G = gt_depth[idx];
+		const bool valid = isfinite(G) && G > s.min_depth && G < s.max_depth && (!mask || mask[idx] != 0.f);
+		const float A = alpha[idx];
+		const bool hole = A < s.alpha_min;
+		const bool front = A >= s.alpha_min && __fmul_rn(G, A) < __fmul_rn(s.k, depth[idx]);
+		f = valid ? (hole ? SEED_HOLE : (front ? SEED_FRONT : 0u)) : 0u;
+		flags[i] = (uint8_t)f;
+	}
+	const uint32_t b_sel = __ballot_sync(0xffffffffu, f != 0u), b_hole = __ballot_sync(0xffffffffu, f == SEED_HOLE);
+	const uint32_t b_front = __ballot_sync(0xffffffffu, f == SEED_FRONT);
+	if (lane == 0) { s_cnt[warp][0] = __popc(b_sel); s_cnt[warp][1] = __popc(b_hole); s_cnt[warp][2] = __popc(b_front); }
+	__syncthreads();
+	if (tid < 4) {
+		uint32_t t = 0;
+		if (tid < 3)
+			for (int w = 0; w < DN_TB / 32; w++) t += s_cnt[w][tid];
+		block_counts[4 * blockIdx.x + tid] = t;
+	}
+}
+
+struct SeedCam {
+	const float* view;       // device, column-major: R[r][c] = view[4 c + r], t[r] = view[12 + r]
+	float fx, fy, half_w, half_h, scale;   // scale = stride / ((fx + fy) / 2)
+};
+
+// Rank of each selected pixel (block offset from the scan + the block's ballots), the cap test against the n of the caller, and the
+// kept pixel's point, colour and dist2 at its output slot floor(k n / c). n <= c = totals[0], n > 0.
+__global__ void __launch_bounds__(DN_TB) seed_emit_kernel(SeedGrid g, SeedCam cam, int n, const uint8_t* __restrict__ flags,
+                                                        const uint32_t* __restrict__ block_offsets, const uint32_t* __restrict__ totals,
+                                                        const float* __restrict__ gt_image, const float* __restrict__ gt_depth,
+                                                        float* __restrict__ points, float* __restrict__ colors, float* __restrict__ dist2)
+{
+	__shared__ uint32_t s_wcnt[DN_TB / 32];
+	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	const int i = blockIdx.x * DN_TB + tid;
+	const bool sel = i < g.ng && flags[i] != 0;
+	const uint32_t b = __ballot_sync(0xffffffffu, sel);
+	if (lane == 0) s_wcnt[warp] = __popc(b);
+	__syncthreads();
+	if (!sel) return;
+	uint64_t k = block_offsets[4 * blockIdx.x] + __popc(b & ((1u << lane) - 1u));
+	for (int w = 0; w < warp; w++) k += s_wcnt[w];
+	const uint64_t c = totals[0], nn = (uint64_t)n;
+	const uint64_t j = k * nn / c;
+	if ((k + 1) * nn / c == j) return;   // not kept
+	const int gv = i / g.gw, gu = i - gv * g.gw;
+	const int u = gu * g.stride, v = gv * g.stride;
+	const size_t idx = (size_t)v * g.W + u, plane = (size_t)g.W * g.H;
+	const float z = gt_depth[idx];
+	// the inverse of the forward's projection (ndc_to_pix: pix = x / z f + W / 2 - 1 / 2): the point lands on the centre of pixel (u, v)
+	const float px = ((float)u + 0.5f - cam.half_w) * z / cam.fx;
+	const float py = ((float)v + 0.5f - cam.half_h) * z / cam.fy;
+	const float* m = cam.view;
+	const float d0 = px - m[12], d1 = py - m[13], d2 = z - m[14];
+#pragma unroll
+	for (int r = 0; r < 3; r++) {
+		points[3 * j + r] = m[4 * r] * d0 + m[4 * r + 1] * d1 + m[4 * r + 2] * d2;   // R^T (p - t)
+		colors[3 * j + r] = gt_image[r * plane + idx];
+	}
+	const float s = z * cam.scale;
+	dist2[j] = s * s;
 }
 
 // ------------------------------------------------------------------------------------------------------------------------
@@ -725,6 +818,105 @@ int scatter_apply(const char* fn, int P, const psb_model* src, const psb_model* 
 	return 0;
 }
 
+// psb_insert_points' argument checks (messages prefixed with fn) and its body; seeding runs the same two with its emitted points
+int insert_check(const char* fn, int P, const psb_model* src, const psb_model* dst, int n, const float* points, const float* colors, const float* dist2)
+{
+	const RelocTensors s = rows_of(src), d = rows_of(dst);
+	const size_t Q = (size_t)P + n;
+	const char* err = nullptr;
+	if (P < 0 || n < 0 || !dst || (P > 0 && !src) || (n > 0 && (!points || !colors || !dist2))) err = ": bad argument";
+	else if ((Q > 0 && !has_rows(d)) || (P > 0 && !has_rows(s))) err = ": null tensor";
+	else if (n > 0 && (reinterpret_cast<uintptr_t>(d.p[5]) & 15)) err = ": rotation tensor must be 16-byte aligned";
+	if (err) { set_error_msg((std::string(fn) + err).c_str()); return PSB_ERR_ARG; }
+	return 0;
+}
+int insert_run(int P, const psb_model* src, const psb_model* dst, int n, const float* points, const float* colors, const float* dist2, int iteration,
+               cudaStream_t stream)
+{
+	const RelocTensors s = rows_of(src), d = rows_of(dst);
+	const size_t Q = (size_t)P + n;
+	int rc;
+	if (P > 0 && (rc = copy_rows(P, s, d, stream))) return rc;
+	for (int i = 0; i < 6 && n > 0; i++) {   // moments of the new rows: zeros (cat(..., zeros_like(extension)), :675-676)
+		const size_t k = (size_t)row_floats(i);
+		PSB_CUDA_OK(cudaMemsetAsync(d.m[i] + (size_t)P * k, 0, (size_t)n * k * sizeof(float), stream));
+		PSB_CUDA_OK(cudaMemsetAsync(d.v[i] + (size_t)P * k, 0, (size_t)n * k * sizeof(float), stream));
+	}
+	if (Q > 0 && (rc = zero_stats(d, Q, stream))) return rc;
+	if (n > 0) {
+		DensifyTensors t = {};
+		for (int i = 0; i < 6; i++) t.dp[i] = d.p[i];
+		t.dexist = d.exist;
+		insert_fill_kernel<<<(n + 127) / 128, 128, 0, stream>>>(P, n, points, colors, dist2, iteration, t);
+		PSB_LAUNCH_OK();
+	}
+	return 0;
+}
+
+// ---- seeding: the workspace is the densify workspace of the ng grid pixels (flags, counts, offsets, totals), then points [ng,3],
+//      colours [ng,3] and dist2 [ng]
+bool seed_grid(int W, int H, int stride, SeedGrid& g)
+{
+	if (W <= 0 || H <= 0 || stride < 1 || (long long)W * H > INT_MAX) return false;
+	g.W = W; g.H = H; g.stride = stride;
+	g.gw = (W + stride - 1) / stride;
+	g.ng = g.gw * ((H + stride - 1) / stride);
+	return true;
+}
+size_t seed_ws_bytes(const SeedGrid& g)
+{
+	const size_t n = (size_t)g.ng;
+	return ws_bytes(g.ng) + 2 * align_up(n * 3 * sizeof(float), 256) + align_up(n * sizeof(float), 256);
+}
+struct SeedOut { float* points; float* colors; float* dist2; };
+SeedOut seed_out(void* w, const SeedGrid& g)
+{
+	const size_t n = (size_t)g.ng;
+	char* c = static_cast<char*>(w) + ws_bytes(g.ng);
+	SeedOut o;
+	o.points = reinterpret_cast<float*>(c); c += align_up(n * 3 * sizeof(float), 256);
+	o.colors = reinterpret_cast<float*>(c); c += align_up(n * 3 * sizeof(float), 256);
+	o.dist2 = reinterpret_cast<float*>(c);
+	return o;
+}
+bool seed_cfg_ok(const psb_seed_cfg* c)
+{
+	// written so that a NaN fails every test
+	return c && c->alpha_min > 0.f && c->alpha_min <= 1.f && c->depth_rel >= 0.f && c->depth_rel <= 1.f && c->min_depth >= 0.f &&
+	       c->min_depth < c->max_depth && c->stride >= 1 && c->max_new >= 0;
+}
+
+// What a plan left in a workspace, kept on the host so that psb_seed_apply can refuse an n above the selected count before it enqueues
+// anything: the last kSeedPlans workspaces planned, each with the grid it was planned on.
+struct SeedPlan { const void* ws; int W, H, stride, selected; };
+constexpr int kSeedPlans = 16;
+std::mutex g_seed_mu;
+SeedPlan g_seed_plans[kSeedPlans];
+int g_seed_next = 0;
+
+void seed_record(const void* ws, const SeedGrid& g, int selected)
+{
+	std::lock_guard<std::mutex> lk(g_seed_mu);
+	for (SeedPlan& p : g_seed_plans)
+		if (p.ws == ws) p.ws = nullptr;
+	g_seed_plans[g_seed_next] = {ws, g.W, g.H, g.stride, selected};
+	g_seed_next = (g_seed_next + 1) % kSeedPlans;
+}
+// the selected count of the plan in ws on grid g, or -1
+int seed_lookup(const void* ws, const SeedGrid& g)
+{
+	std::lock_guard<std::mutex> lk(g_seed_mu);
+	for (const SeedPlan& p : g_seed_plans)
+		if (p.ws == ws && p.W == g.W && p.H == g.H && p.stride == g.stride) return p.selected;
+	return -1;
+}
+void seed_forget(const void* ws)
+{
+	std::lock_guard<std::mutex> lk(g_seed_mu);
+	for (SeedPlan& p : g_seed_plans)
+		if (p.ws == ws) p.ws = nullptr;
+}
+
 }  // namespace
 
 int launch_position_noise(int P, float* xyz, const float* opacity, const float* scaling, const float* rotation, float lr, unsigned long long seed,
@@ -855,28 +1047,73 @@ int psb_prune_apply(int P, const psb_model* src, const psb_model* dst, int P_new
 int psb_insert_points(int P, const psb_model* src, const psb_model* dst, int n, const float* points, const float* colors, const float* dist2,
                       int iteration, void* stream_)
 {
-	cudaStream_t stream = (cudaStream_t)stream_;
-	const RelocTensors s = rows_of(src), d = rows_of(dst);
-	const size_t Q = (size_t)P + n;
-	if (P < 0 || n < 0 || !dst || (P > 0 && !src) || (n > 0 && (!points || !colors || !dist2))) { set_error_msg("psb_insert_points: bad argument"); return PSB_ERR_ARG; }
-	if ((Q > 0 && !has_rows(d)) || (P > 0 && !has_rows(s))) { set_error_msg("psb_insert_points: null tensor"); return PSB_ERR_ARG; }
-	if (n > 0 && (reinterpret_cast<uintptr_t>(d.p[5]) & 15)) { set_error_msg("psb_insert_points: rotation tensor must be 16-byte aligned"); return PSB_ERR_ARG; }
 	int rc;
-	if (P > 0 && (rc = copy_rows(P, s, d, stream))) return rc;
-	for (int i = 0; i < 6 && n > 0; i++) {   // moments of the new rows: zeros (cat(..., zeros_like(extension)), :675-676)
-		const size_t k = (size_t)row_floats(i);
-		PSB_CUDA_OK(cudaMemsetAsync(d.m[i] + (size_t)P * k, 0, (size_t)n * k * sizeof(float), stream));
-		PSB_CUDA_OK(cudaMemsetAsync(d.v[i] + (size_t)P * k, 0, (size_t)n * k * sizeof(float), stream));
+	if ((rc = insert_check("psb_insert_points", P, src, dst, n, points, colors, dist2))) return rc;
+	return insert_run(P, src, dst, n, points, colors, dist2, iteration, (cudaStream_t)stream_);
+}
+
+size_t psb_seed_workspace_bytes(int width, int height, int stride)
+{
+	SeedGrid g;
+	return seed_grid(width, height, stride, g) ? seed_ws_bytes(g) : 0;
+}
+
+int psb_seed_plan(const psb_camera* camera, const float* alpha, const float* depth, const float* gt_depth, const float* mask, const psb_seed_cfg* cfg,
+                  void* workspace, int* counts_host, void* stream_)
+{
+	cudaStream_t stream = (cudaStream_t)stream_;
+	SeedGrid g;
+	if (!camera || !seed_cfg_ok(cfg) || !seed_grid(camera->width, camera->height, cfg->stride, g) || !alpha || !depth || !gt_depth || !workspace ||
+	    !counts_host) {
+		set_error_msg("psb_seed_plan: bad argument (a camera of positive size, the alpha, depth and gt_depth planes, alpha_min in (0, 1], depth_rel "
+		              "in [0, 1], 0 <= min_depth < max_depth, stride >= 1, max_new >= 0, a workspace and counts_host required)");
+		return PSB_ERR_ARG;
 	}
-	if (Q > 0 && (rc = zero_stats(d, Q, stream))) return rc;
+	for (int k = 0; k < 3; k++) counts_host[k] = 0;
+	seed_forget(workspace);   // a plan that fails below leaves no plan behind
+	const SeedTest s = {cfg->alpha_min, 1.0f - cfg->depth_rel, cfg->min_depth, cfg->max_depth};
+	const Workspace w = ws_carve(workspace, g.ng);
+	seed_mask_kernel<<<(g.ng + DN_TB - 1) / DN_TB, DN_TB, 0, stream>>>(g, s, alpha, depth, gt_depth, mask, w.flags, w.counts);
+	PSB_LAUNCH_OK();
+	uint32_t tot[4];
+	int rc;
+	if ((rc = plan_totals(g.ng, w, tot, stream))) return rc;
+	counts_host[0] = (int)tot[0]; counts_host[1] = (int)tot[1]; counts_host[2] = (int)tot[2];
+	seed_record(workspace, g, (int)tot[0]);
+	return 0;
+}
+
+int psb_seed_apply(int P, const psb_model* src, const psb_model* dst, int n, const psb_camera* camera, const float* gt_image, const float* gt_depth,
+                   const psb_seed_cfg* cfg, const void* workspace, int iteration, void* stream_)
+{
+	cudaStream_t stream = (cudaStream_t)stream_;
+	SeedGrid g;
+	if (!camera || !camera->viewmatrix || !seed_cfg_ok(cfg) || !seed_grid(camera->width, camera->height, cfg->stride, g) ||
+	    !(camera->tan_fovx > 0.f) || !(camera->tan_fovy > 0.f) || !std::isfinite(camera->tan_fovx) || !std::isfinite(camera->tan_fovy) ||
+	    !gt_image || !gt_depth || !workspace || n < 0 || n > cfg->max_new) {
+		set_error_msg("psb_seed_apply: bad argument (a camera with a view matrix, positive size and finite positive tan_fov, gt_image, gt_depth, "
+		              "a valid cfg, the plan's workspace and 0 <= n <= max_new required)");
+		return PSB_ERR_ARG;
+	}
+	const int selected = seed_lookup(workspace, g);
+	if (selected < 0) { set_error_msg("psb_seed_apply: the workspace holds no psb_seed_plan of this camera size and stride"); return PSB_ERR_ARG; }
+	if (n > selected) { set_error_msg("psb_seed_apply: n exceeds the number of pixels the plan selected"); return PSB_ERR_ARG; }
+	const SeedOut o = seed_out(const_cast<void*>(workspace), g);
+	int rc;
+	if ((rc = insert_check("psb_seed_apply", P, src, dst, n, o.points, o.colors, o.dist2))) return rc;
 	if (n > 0) {
-		DensifyTensors t = {};
-		for (int i = 0; i < 6; i++) t.dp[i] = d.p[i];
-		t.dexist = d.exist;
-		insert_fill_kernel<<<(n + 127) / 128, 128, 0, stream>>>(P, n, points, colors, dist2, iteration, t);
+		const Workspace w = ws_carve(const_cast<void*>(workspace), g.ng);
+		SeedCam c;
+		c.view = camera->viewmatrix;
+		c.fx = (float)g.W / (2.0f * camera->tan_fovx);
+		c.fy = (float)g.H / (2.0f * camera->tan_fovy);
+		c.half_w = 0.5f * (float)g.W; c.half_h = 0.5f * (float)g.H;
+		c.scale = (float)g.stride / (0.5f * (c.fx + c.fy));
+		seed_emit_kernel<<<(g.ng + DN_TB - 1) / DN_TB, DN_TB, 0, stream>>>(g, c, n, w.flags, w.offsets, w.totals, gt_image, gt_depth, o.points,
+		                                                                  o.colors, o.dist2);
 		PSB_LAUNCH_OK();
 	}
-	return 0;
+	return insert_run(P, src, dst, n, o.points, o.colors, o.dist2, iteration, stream);
 }
 
 int psb_reset_opacity(int P, float* opacity, float* exp_avg, float* exp_avg_sq, void* stream_)

@@ -100,6 +100,14 @@ class _RelocateCfg(C.Structure):
     _fields_ = [("min_opacity", C.c_float), ("iteration", C.c_int), ("seed", C.c_ulonglong), ("offset", C.c_ulonglong)]
 
 
+class _SeedCfg(C.Structure):
+    _fields_ = [("alpha_min", C.c_float), ("depth_rel", C.c_float), ("min_depth", C.c_float), ("max_depth", C.c_float), ("stride", C.c_int),
+                ("max_new", C.c_int)]
+
+
+_INT_MAX = 2 ** 31 - 1
+
+
 # The unit of the summed contribution score (include/psb200.h, PSB_CONTRIB_SUM_FRAC_BITS = 26).
 CONTRIB_SUM_UNIT = 2.0 ** -26
 
@@ -195,12 +203,15 @@ def _bind():
         "psb_reset_opacity": [i, vp, vp, vp, vp],
         "psb_relocate": [i, Model, P(_RelocateCfg), vp, vp, P(i), vp],
         "psb_grow": [i, Model, Model, i, P(_RelocateCfg), vp, vp, vp],
+        "psb_seed_plan": [Cam, vp, vp, vp, vp, P(_SeedCfg), vp, P(i), vp],
+        "psb_seed_apply": [i, Model, Model, i, Cam, vp, vp, P(_SeedCfg), vp, i, vp],
     }
     for name, args in sigs.items():
         fn = getattr(L, name)
         fn.argtypes, fn.restype = args, i
     L.psb_densify_workspace_bytes.argtypes, L.psb_densify_workspace_bytes.restype = [i], size_t
     L.psb_relocate_workspace_bytes.argtypes, L.psb_relocate_workspace_bytes.restype = [i], size_t
+    L.psb_seed_workspace_bytes.argtypes, L.psb_seed_workspace_bytes.restype = [i, i, i], size_t
     L._trainer_bound = True
     return L
 
@@ -853,6 +864,69 @@ class GaussianTrainer:
             m.prunePoints(mask)
         return n
 
+    # --- depth-guided seeding (include/psb200.h, psb_seed_*): new rows on the pixels of an RGB-D keyframe where this trainer's render of the
+    #     map is nearly transparent (a hole) or lies behind the sensor's surface (in front). ORB keypoints miss textureless surfaces; this
+    #     fills them. When to seed is the caller's choice (INTEGRATION §2: once per new RGB-D keyframe, after its pose is set).
+    def seedFromDepth(self, cam, gt_image, gt_depth, mask=None, alpha_min=0.5, depth_rel=0.1, min_depth=0.2, max_depth=40.0, stride=1, max_new=None,
+                      iteration=None):
+        """Adds a Gaussian on every `stride`-th pixel (in u and v) of the keyframe whose depth gt_depth [H,W] (metres, <= 0: none) lies in
+        (min_depth, max_depth), that mask[0] (mask [3,H,W] or None, the depth loss's convention) does not exclude, and where this trainer's
+        render of the view has accumulated opacity A < alpha_min (hole) or a normalised depth D / A beyond gt_depth / (1 - depth_rel) (in
+        front). At most max_new are added, spread evenly over the image. Each new row sits at the pixel's centre at depth gt_depth, takes
+        the colour of gt_image [3,H,W] and the scale of one grid cell at that depth, and is otherwise what increasePcd writes (opacity 0.1,
+        identity rotation, zero moments, exist_since_iter = iteration, default self.iteration; statistics of all rows reset). Seeded points
+        are not SLAM map points: sparse_points_xyz_ is untouched. Like every row operation it drops the live bytes and the 3D filter.
+        Defaults: alpha_min = 0.5 is SplaTAM's silhouette threshold; min_depth = 0.2 is the forward's near cull (a seed nearer than that
+        is never drawn from this keyframe); max_depth = 40 is RGBD.max_depth in the shipped configs; with opt.mcmc, max_new defaults to
+        max(opt.cap_max - P, 0), so seeding never exceeds the budget, and otherwise to no limit.
+        Returns (rows added, holes, in front): the counts of selected pixels before the cap."""
+        num = lambda x: not isinstance(x, bool) and isinstance(x, (int, float)) and not math.isnan(x)
+        if not num(alpha_min) or not 0 < alpha_min <= 1:
+            raise ValueError(f"seedFromDepth: alpha_min must be in (0, 1], got {alpha_min!r}")
+        if not num(depth_rel) or not 0 <= depth_rel <= 1:
+            raise ValueError(f"seedFromDepth: depth_rel must be in [0, 1], got {depth_rel!r}")
+        if not num(min_depth) or not num(max_depth) or not 0 <= min_depth < max_depth or math.isinf(min_depth):
+            raise ValueError(f"seedFromDepth: want 0 <= min_depth < max_depth, got {min_depth!r}, {max_depth!r}")
+        if isinstance(stride, bool) or not isinstance(stride, int) or stride < 1:
+            raise ValueError(f"seedFromDepth: stride must be an int >= 1, got {stride!r}")
+        if max_new is not None and (isinstance(max_new, bool) or not isinstance(max_new, int) or max_new < 0):
+            raise ValueError(f"seedFromDepth: max_new must be an int >= 0 or None, got {max_new!r}")
+        if iteration is not None and (isinstance(iteration, bool) or not isinstance(iteration, int)):
+            raise ValueError(f"seedFromDepth: iteration must be an int or None, got {iteration!r}")
+        cam = _check_cams([cam], "seedFromDepth")[0]
+        H, W = int(cam["H"]), int(cam["W"])
+        _plane(gt_image, (3, H, W), "seedFromDepth: gt_image")
+        _plane(gt_depth, (H, W), "seedFromDepth: gt_depth")
+        _plane(mask, (3, H, W), "seedFromDepth: mask")
+        if gt_image is None or gt_depth is None:
+            raise ValueError("seedFromDepth: gt_image and gt_depth are required")
+        m = self.model
+        m._check_rows()
+        if not hasattr(m, "exp_avg_"):
+            raise RuntimeError("seedFromDepth: call trainingSetup() first (the optimizer state is extended together with the parameters)")
+        P = m.num_points()
+        if max_new is None:
+            max_new = max(int(self.opt.cap_max) - P, 0) if self.opt.mcmc else _INT_MAX
+        max_new = min(max_new, _INT_MAX)
+        it = self.iteration if iteration is None else iteration
+        alpha = torch.zeros((H, W), dtype=torch.float32, device=m.device)
+        depth = torch.zeros((H, W), dtype=torch.float32, device=m.device)
+        if P > 0:     # an empty map is transparent everywhere: A = D = 0 makes every valid grid pixel a hole
+            self.render(cam, out_depth=depth, out_alpha=alpha)
+        L = self.L
+        stream = torch.cuda.current_stream().cuda_stream
+        cfg = _SeedCfg(float(alpha_min), float(depth_rel), float(min_depth), float(max_depth), stride, max_new)
+        cc = _ccamera(cam)
+        ws = torch.empty(L.psb_seed_workspace_bytes(W, H, stride), dtype=torch.uint8, device=m.device)
+        counts = (C.c_int * 3)()
+        _lib.check(L.psb_seed_plan(C.byref(cc), alpha.data_ptr(), depth.data_ptr(), gt_depth.data_ptr(), mask.data_ptr() if mask is not None else None,
+                                   C.byref(cfg), ws.data_ptr(), counts, stream), "psb_seed_plan")
+        n = min(counts[0], max_new)
+        if n:
+            m._out_of_place(P + n, lambda src, dst: L.psb_seed_apply(P, src, dst, n, C.byref(cc), gt_image.data_ptr(), gt_depth.data_ptr(), C.byref(cfg),
+                                                                     ws.data_ptr(), int(it), stream), "psb_seed_apply")
+        return n, counts[1], counts[2]
+
     @property
     def antialiasing(self):
         """Whether this trainer's passes use the 2D Mip filter (set at construction)."""
@@ -1275,6 +1349,10 @@ class DataParallelTrainer(GaussianTrainer):
         raise NotImplementedError("DataParallelTrainer.pruneByContribution: pruning is not wired into the data-parallel steps (in p2p mode the "
                                   "parameters live in the IPC arena, and every rank would need the same mask: an exact all-reduce of the "
                                   "integer scores, then rebuild()); score with contributionScores and prune on one GPU through GaussianTrainer")
+
+    def seedFromDepth(self, *args, **kwargs):
+        raise NotImplementedError("DataParallelTrainer.seedFromDepth: each rank trains its own keyframe, so rows seeded from it would exist on "
+                                  "one replica only and the replicas would diverge; seed on one GPU through GaussianTrainer, then rebuild()")
 
     def gather_moments(self):
         """Every rank receives the Adam moments of all rows (they are only maintained on the owner): call before
