@@ -5,7 +5,7 @@ Camera conventions restate reference src/gaussian_keyframe.cpp:119-204 and inclu
   projection P: P00 = 1/tan(fovx/2), P11 = 1/tan(fovy/2), P22 = zfar/(zfar-znear),
                 P23 = -zfar*znear/(zfar-znear), P32 = 1;   full_proj = (P @ Rt)^T,
   camera_center = inverse(world_view_transform)[3, :3], fov = 2*atan(pixels / (2*focal)).
-numpy only; the caller moves arrays to the device.
+numpy only at import; device_camera moves a camera to the device.
 """
 import math
 
@@ -101,3 +101,35 @@ def activate(scene):
 def target_image(H, W, seed=1):
     rng = np.random.default_rng(seed)
     return rng.uniform(0.0, 1.0, size=(3, H, W)).astype(np.float32)
+
+
+def device_camera(cam, device):
+    """The camera dict the trainer and the renderer take (viewmatrix / projmatrix / campos tensors on `device`, tanfovx / tanfovy
+    floats, W / H ints), built from a make_camera dict."""
+    import torch
+    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(device)
+    return dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
+                tanfovy=float(cam["tanfovy"]), W=int(cam["W"]), H=int(cam["H"]))
+
+
+def quality_scene():
+    """The scene of the quality test: 200 k Gaussians laid out in front of the identity view at 640x480 (TUM focal length), seen from six
+    small random poses. -> (scene, [six make_camera dicts])."""
+    P, W, H, fx = 200_000, 640, 480, 520.9
+    scene = make_scene(P, make_camera(W, H, fx, fx), seed=21, scale_px=3.0)
+    cams = [make_camera(W, H, fx, fx, *random_pose(np.random.default_rng(50 + k), max_angle=0.06, max_trans=0.12)) for k in range(6)]
+    return scene, cams
+
+
+def thinned_trainee(scene, seed=3):
+    """A trainee for `scene`: about 80 % of its rows, positions, colours, opacities and scales perturbed, f_rest zeroed (so training and
+    densification have something to do)."""
+    rng = np.random.default_rng(seed)
+    keep = rng.random(len(scene["xyz"])) < 0.8
+    start = {k: v[keep].copy() for k, v in scene.items()}
+    start["xyz"] += rng.normal(0, 0.01, start["xyz"].shape).astype(np.float32)
+    start["features_dc"] += rng.normal(0, 0.6, start["features_dc"].shape).astype(np.float32)
+    start["features_rest"] *= 0
+    start["opacity"] += rng.normal(0, 0.7, start["opacity"].shape).astype(np.float32)
+    start["scaling"] += np.float32(0.15)
+    return start

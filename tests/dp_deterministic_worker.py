@@ -32,9 +32,7 @@ def main():
     assert tr.mode == "p2p", getattr(tr, "_p2p_error", "")
     R, t = syn.random_pose(np.random.default_rng(100 + rank), max_angle=0.08, max_trans=0.15)
     cam = syn.make_camera(W, H, fx, fy, R, t)
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-    c = dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-             tanfovy=float(cam["tanfovy"]), W=W, H=H)
+    c = syn.device_camera(cam, dev)
     gt = torch.from_numpy(syn.target_image(H, W, seed=7 + rank)).to(dev)
     gd = (1.0 + 6.0 * torch.rand((H, W), generator=torch.Generator().manual_seed(rank))).to(dev)
     tr.render(c)        # grows the binning arena: no step is a dropped view

@@ -25,9 +25,7 @@ LRS = [0.00032, 0.0025, 0.0025 / 20, 0.05, 0.005, 0.001]
 def view(rank, W, H, fx, fy, dev):
     R, t = syn.random_pose(np.random.default_rng(100 + rank), max_angle=0.08, max_trans=0.15)
     cam = syn.make_camera(W, H, fx, fy, R, t)
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-    c = dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-             tanfovy=float(cam["tanfovy"]), W=W, H=H)
+    c = syn.device_camera(cam, dev)
     gt = torch.from_numpy(syn.target_image(H, W, seed=7 + rank)).to(dev)
     return c, gt
 

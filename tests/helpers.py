@@ -22,8 +22,7 @@ def scene_tensors(P, camname="tum", seed=0, pose_seed=None, dev="cuda", scale=1.
     act = syn.activate(sc)
     T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
     g = {k: T(v) for k, v in act.items()}
-    c = dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]),
-             tanfovx=float(cam["tanfovx"]), tanfovy=float(cam["tanfovy"]), W=W, H=H)
+    c = syn.device_camera(cam, dev)
     return cam, sc, act, g, c
 
 

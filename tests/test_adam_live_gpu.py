@@ -24,9 +24,7 @@ def _setup(cuda, P=40_000, W=320, H=240, seed=5):
     sc["xyz"][::2, 0] += 1000.0          # half of the rows far outside the view: never reached
     m = trainer.GaussianModel.from_numpy(sc, cuda)
     m.trainingSetup(trainer.GaussianOptimizationParams())
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(cuda)
-    c = dict(viewmatrix=T(cam0["viewmatrix"]), projmatrix=T(cam0["projmatrix"]), campos=T(cam0["campos"]), tanfovx=float(cam0["tanfovx"]),
-             tanfovy=float(cam0["tanfovy"]), W=W, H=H)
+    c = syn.device_camera(cam0, cuda)
     gt = torch.from_numpy(syn.target_image(H, W, seed=2)).to(cuda)
     return m, trainer.GaussianTrainer(m), c, gt
 

@@ -435,9 +435,7 @@ def _worker(steps):
     torch.cuda.set_device(dev)
     sc, c0, gt, gd = _train_inputs(dev, P=30_001, wh=(320, 240), seed=9)
     cam = syn.make_camera(320, 240, 600.0 * 320 / 1200, 600.0 * 240 / 680, *syn.random_pose(np.random.default_rng(100 + rank)))
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-    c = dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-             tanfovy=float(cam["tanfovy"]), W=320, H=240)
+    c = syn.device_camera(cam, dev)
     m = _model(sc, dev, sh=1)
     tr = trainer.DataParallelTrainer(m, mode="p2p", deterministic=True, antialiasing=True)
     assert tr.mode == "p2p"

@@ -32,15 +32,6 @@ GATE_SUM_REL = 1e-4        # sum_weight: relative, plus one 2^-26 unit per blend
 QUALITY_MARGIN_DB = 0.05
 
 
-def _T(a, dev):
-    return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-
-
-def _dev_cam(cam, dev):
-    return dict(viewmatrix=_T(cam["viewmatrix"], dev), projmatrix=_T(cam["projmatrix"], dev), campos=_T(cam["campos"], dev),
-                tanfovx=float(cam["tanfovx"]), tanfovy=float(cam["tanfovy"]), W=int(cam["W"]), H=int(cam["H"]))
-
-
 def _views(W, H, f, n, seed, angle=0.05, trans=0.05):
     """the identity camera and n - 1 small random poses around it (numpy camera dicts)"""
     rng = np.random.default_rng(seed)
@@ -121,7 +112,7 @@ def test_scores_against_the_restatement(cuda, mode):
     m = _model(sc, cuda)
     tr = trainer.GaussianTrainer(m, background=torch.tensor([0.2, 0.3, 0.4], device=cuda), antialiasing=mode == "aa",
                                  filter3d=mode == "filter3d")
-    dcams = [_dev_cam(c, cuda) for c in cams]
+    dcams = [syn.device_camera(c, cuda) for c in cams]
     f = None
     if mode == "filter3d":
         m.computeFilter3D(dcams)
@@ -169,7 +160,7 @@ def test_scores_are_bit_identical_across_runs_orders_and_modes(cuda):
     cam, sc, _, _, c = scene_tensors(200_000, "tum", seed=7, pose_seed=8, dev=cuda)
     W, H = c["W"], c["H"]
     fx = W / (2 * c["tanfovx"])
-    views = [_dev_cam(v, cuda) for v in _views(W, H, fx, 5, seed=9, angle=0.1, trans=0.1)]
+    views = [syn.device_camera(v, cuda) for v in _views(W, H, fx, 5, seed=9, angle=0.1, trans=0.1)]
     m = _model(sc, cuda)
     tr = trainer.GaussianTrainer(m, deterministic=False)
     a = tr.contributionScores(views)
@@ -192,7 +183,7 @@ def test_overflowing_sweep_ends_as_on_a_grown_arena(cuda):
     from photo_slam_b200 import trainer
     cam, sc, _, _, c = scene_tensors(20_000, "tum", seed=5, pose_seed=6, dev=cuda, scale_px=30.0)
     W, H = c["W"], c["H"]
-    views = [_dev_cam(v, cuda) for v in _views(W, H, W / (2 * c["tanfovx"]), 3, seed=1, angle=0.1, trans=0.1)]
+    views = [syn.device_camera(v, cuda) for v in _views(W, H, W / (2 * c["tanfovx"]), 3, seed=1, angle=0.1, trans=0.1)]
     m = _model(sc, cuda)
     fresh = trainer.GaussianTrainer(m)
     a = fresh.contributionScores(views)
@@ -244,7 +235,7 @@ def _walled_scene(W=128, H=96, f=110.0):
 def test_prune_removes_what_no_view_shows(cuda):
     from photo_slam_b200 import trainer
     sc, cams, injected = _walled_scene()
-    dcams = [_dev_cam(c, cuda) for c in cams]
+    dcams = [syn.device_camera(c, cuda) for c in cams]
     m = _model(sc, cuda)
     tr = trainer.GaussianTrainer(m)
     mx, sm = tr.contributionScores(dcams)
@@ -267,7 +258,7 @@ def test_prune_removes_what_no_view_shows(cuda):
 def test_min_age_protects_fresh_rows(cuda):
     from photo_slam_b200 import trainer
     sc, cams, injected = _walled_scene()
-    dcams = [_dev_cam(c, cuda) for c in cams]
+    dcams = [syn.device_camera(c, cuda) for c in cams]
     m = _model(sc, cuda)
     tr = trainer.GaussianTrainer(m)
     tr.iteration = 500
@@ -288,7 +279,7 @@ def test_pruning_unscored_rows_leaves_the_views_bit_identical(cuda):
     sc["xyz"][200:400, 0] += 50.0
     ref = contrib64.scores(s64.raw64(sc, "cpu"), [s64.camera64(c, "cpu") for c in cams], D=3)
     assert not any(bool(s.any()) for s in ref["stopped"]), "the scene must have no pixel that ends at the T test"
-    dcams = [_dev_cam(c, cuda) for c in cams]
+    dcams = [syn.device_camera(c, cuda) for c in cams]
     m = _model(sc, cuda)
     tr = trainer.GaussianTrainer(m, background=torch.tensor([0.3, 0.2, 0.1], device=cuda))
 
@@ -316,7 +307,7 @@ def test_pruning_unscored_rows_leaves_the_views_bit_identical(cuda):
 def test_filter3d_trainer_needs_the_filter_again(cuda):
     from photo_slam_b200 import trainer
     sc, cams, injected = _walled_scene()
-    dcams = [_dev_cam(c, cuda) for c in cams]
+    dcams = [syn.device_camera(c, cuda) for c in cams]
     m = _model(sc, cuda)
     tr = trainer.GaussianTrainer(m, filter3d=True)
     with pytest.raises(ValueError, match="computeFilter3D"):
@@ -335,7 +326,7 @@ def test_quality_after_the_prune(cuda):
     P, W, H, fx = 20_000, 320, 240, 260.0
     cam0 = syn.make_camera(W, H, fx, fx)
     gt_scene = syn.make_scene(P, cam0, seed=31, scale_px=3.0)
-    views = [_dev_cam(v, cuda) for v in _views(W, H, fx, 6, seed=60, angle=0.06, trans=0.12)]
+    views = [syn.device_camera(v, cuda) for v in _views(W, H, fx, 6, seed=60, angle=0.06, trans=0.12)]
     gt_tr = trainer.GaussianTrainer(trainer.GaussianModel.from_numpy(gt_scene, cuda))
     gts = [gt_tr.render(c).clamp(0, 1).clone() for c in views]
     rng = np.random.default_rng(4)

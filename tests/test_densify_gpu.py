@@ -163,8 +163,7 @@ def test_prune_insert_reset_and_training_after_surgery(cuda):
     # and the model still trains after all of it
     W, H = 160, 120
     camn = syn.make_camera(W, H, 130.0, 130.0)
-    c = dict(viewmatrix=torch.from_numpy(camn["viewmatrix"]).to(cuda), projmatrix=torch.from_numpy(camn["projmatrix"]).to(cuda),
-             campos=torch.from_numpy(camn["campos"]).to(cuda), tanfovx=float(camn["tanfovx"]), tanfovy=float(camn["tanfovy"]), W=W, H=H)
+    c = syn.device_camera(camn, cuda)
     tr = trainer.GaussianTrainer(m)
     tr.trainForOneIteration(c, torch.rand((3, H, W), device=cuda))
     assert math.isfinite(tr.result()[0])

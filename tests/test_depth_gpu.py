@@ -299,9 +299,7 @@ def test_depth_term_converges_towards_the_target_depth(cuda):
     P, W, H = 20_000, 200, 150
     cam = syn.make_camera(W, H, 170.0, 170.0, *syn.random_pose(np.random.default_rng(3)))
     sc = syn.make_scene(P, cam, seed=4, scale_px=4.0)
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(cuda)
-    c = dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-             tanfovy=float(cam["tanfovy"]), W=W, H=H)
+    c = syn.device_camera(cam, cuda)
     rng = np.random.default_rng(5)
     sc2 = {k: v.copy() for k, v in sc.items()}
     V = cam["viewmatrix"].reshape(-1)

@@ -48,8 +48,7 @@ def _inputs(cuda, case):
     sc = syn.make_scene(P, cam, seed=21, scale_px=5.0, culled_frac=0.4 if case == "culled" else 0.05)
     act = syn.activate(sc)
     T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(cuda)
-    c = dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-             tanfovy=float(cam["tanfovy"]), W=W, H=H)
+    c = syn.device_camera(cam, cuda)
     x = dict(means3D=T(act["means3D"]), opacities=T(act["opacities"]), shs=T(act["shs"]), scales=T(act["scales"]),
              rotations=T(act["rotations"]))
     if case == "colors":

@@ -263,12 +263,10 @@ def _recovery(cuda, compensate, steps, W=300, H=170, views=8):
     import photo_slam_b200.synthetic as syn
     from photo_slam_b200 import trainer
     rng = np.random.default_rng(1)
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(cuda)
     cams = []
     for _ in range(views):
         cam = syn.make_camera(W, H, 150.0, 150.0, *syn.random_pose(rng, max_angle=0.1, max_trans=0.1))
-        cams.append((cam, dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]),
-                               tanfovx=float(cam["tanfovx"]), tanfovy=float(cam["tanfovy"]), W=W, H=H)))
+        cams.append((cam, syn.device_camera(cam, cuda)))
     tm = trainer.GaussianModel.from_numpy(syn.make_scene(20_000, cams[0][0], seed=11, scale_px=2.0), cuda)
     raw = [trainer.GaussianTrainer(tm).render(c) for _, c in cams]
     Es = torch.zeros(views, 3, 4)

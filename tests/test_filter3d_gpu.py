@@ -49,9 +49,7 @@ def _cams(dev, K, seed, W=640, H=480, f=500.0):
         R, t = syn.random_pose(rng, max_angle=0.3, max_trans=0.5)
         fk = f * (0.7 + 0.6 * rng.random())
         cam = syn.make_camera(W, H, fk, fk * (0.9 + 0.2 * rng.random()), R, t)
-        T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-        out.append(dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-                        tanfovy=float(cam["tanfovy"]), W=W, H=H))
+        out.append(syn.device_camera(cam, dev))
     return out
 
 
@@ -396,12 +394,10 @@ def test_trained_run_with_the_filter(dev):
     W, H, f = 320, 240, 260.0
     rng = np.random.default_rng(3)
     poses = [syn.random_pose(rng, max_angle=0.1, max_trans=0.1) for _ in range(8)]
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
     cams = []
     for p in poses:
         cm = syn.make_camera(W, H, f, f, *p)
-        cams.append((cm, dict(viewmatrix=T(cm["viewmatrix"]), projmatrix=T(cm["projmatrix"]), campos=T(cm["campos"]), tanfovx=float(cm["tanfovx"]),
-                              tanfovy=float(cm["tanfovy"]), W=W, H=H)))
+        cams.append((cm, syn.device_camera(cm, dev)))
     target = trainer.GaussianModel.from_numpy(syn.make_scene(20_000, cams[0][0], seed=31, scale_px=2.0), dev)
     gts = [trainer.GaussianTrainer(target).render(c) for _, c in cams]
     res = {}

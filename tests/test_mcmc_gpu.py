@@ -24,13 +24,11 @@ MIN_OP = 0.005
 
 
 def _views(cuda, W, H, fx, n, seed=50):
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(cuda)
     out = []
     for k in range(n):
         R, t = (None, None) if k == 0 else syn.random_pose(np.random.default_rng(seed + k), max_angle=0.06, max_trans=0.12)
         cam = syn.make_camera(W, H, fx, fx, R, t)
-        out.append(dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-                        tanfovy=float(cam["tanfovy"]), W=W, H=H))
+        out.append(syn.device_camera(cam, cuda))
     return out
 
 
@@ -392,14 +390,7 @@ def test_capped_training_end_to_end(cuda):
     gt_scene = syn.make_scene(P, syn.make_camera(W, H, fx, fx), seed=21, scale_px=3.0)
     gt_tr = trainer.GaussianTrainer(trainer.GaussianModel.from_numpy(gt_scene, cuda))
     gts = [gt_tr.render(c).clamp(0, 1).clone() for c in views]
-    rng = np.random.default_rng(3)
-    keep = rng.random(P) < 0.8
-    start = {k: v[keep].copy() for k, v in gt_scene.items()}
-    start["xyz"] += rng.normal(0, 0.01, start["xyz"].shape).astype(np.float32)
-    start["features_dc"] += rng.normal(0, 0.6, start["features_dc"].shape).astype(np.float32)
-    start["features_rest"] *= 0
-    start["opacity"] += rng.normal(0, 0.7, start["opacity"].shape).astype(np.float32)
-    start["scaling"] += np.float32(0.15)
+    start = syn.thinned_trainee(gt_scene)
     start["opacity"][::50] = -6.0                              # 2 % dead on arrival (o = 0.0025), as after an insertion that did not take
 
     def run(mcmc):

@@ -22,29 +22,14 @@ def _run(cuda, gold=None):
     """psb200's 600 iterations; with gold=None the reference chain runs beside it and its record is returned, otherwise the
     reference's stored densification threshold and split counts drive the same schedule."""
     from photo_slam_b200 import trainer
-    P, W, H, fx = 200_000, 640, 480, 520.9
-    cam0 = syn.make_camera(W, H, fx, fx)
-    gt_scene = syn.make_scene(P, cam0, seed=21, scale_px=3.0)
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(cuda)
-    views = []
-    for k in range(6):
-        R, t = syn.random_pose(np.random.default_rng(50 + k), max_angle=0.06, max_trans=0.12)
-        cam = syn.make_camera(W, H, fx, fx, R, t)
-        views.append(dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-                          tanfovy=float(cam["tanfovy"]), W=W, H=H))
+    gt_scene, cams = syn.quality_scene()
+    views = [syn.device_camera(cam, cuda) for cam in cams]
     gt_model = trainer.GaussianModel.from_numpy(gt_scene, cuda)
     gt_tr = trainer.GaussianTrainer(gt_model)
     gts = [gt_tr.render(c).clamp(0, 1).clone() for c in views]
     # the trainee: a perturbed, thinned copy of the scene (so densification has something to do)
-    rng = np.random.default_rng(3)
-    keep = rng.random(P) < 0.8
-    start = {k: v[keep].copy() for k, v in gt_scene.items()}
-    n0 = int(keep.sum())
-    start["xyz"] += rng.normal(0, 0.01, start["xyz"].shape).astype(np.float32)
-    start["features_dc"] += rng.normal(0, 0.6, start["features_dc"].shape).astype(np.float32)
-    start["features_rest"] *= 0
-    start["opacity"] += rng.normal(0, 0.7, start["opacity"].shape).astype(np.float32)
-    start["scaling"] += np.float32(0.15)
+    start = syn.thinned_trainee(gt_scene)
+    n0 = len(start["xyz"])
 
     opt = trainer.GaussianOptimizationParams()
     model = trainer.GaussianModel.from_numpy(start, cuda)

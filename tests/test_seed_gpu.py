@@ -19,12 +19,6 @@ pytestmark = pytest.mark.gpu
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools"))
 
 
-def _dev_cam(cam, dev):
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-    return dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-                tanfovy=float(cam["tanfovy"]), W=int(cam["W"]), H=int(cam["H"]))
-
-
 def _model(scene, dev):
     m = trainer.GaussianModel.from_numpy(scene, dev)
     m.trainingSetup(trainer.GaussianOptimizationParams())
@@ -81,7 +75,7 @@ def _check_new_rows(m, P, s, iteration):
 def test_selection_and_cap_equal_the_restatement(cuda, stride):
     W, H = 31, 23
     npcam = syn.make_camera(W, H, 25.0, 27.0, *syn.random_pose(np.random.default_rng(4)))
-    cam = _dev_cam(npcam, cuda)
+    cam = syn.device_camera(npcam, cuda)
     A, D, G, mask = _planes(H, W)
     img = np.random.default_rng(1).uniform(0, 1, (3, H, W)).astype(np.float32)
     for msk in (mask, None):
@@ -103,13 +97,13 @@ def test_apply_refuses_more_rows_than_the_plan_selected(cuda):
     A, D, G, mask = _planes(H, W)
     c = seed64.seed(npcam, A, D, G, np.zeros((3, H, W)), mask)["counts"][0]
     with pytest.raises(_lib.PsbError, match="exceeds"):
-        _seed_c(_empty(cuda), _dev_cam(npcam, cuda), A, D, G, np.zeros((3, H, W)), mask, n=c + 1)
+        _seed_c(_empty(cuda), syn.device_camera(npcam, cuda), A, D, G, np.zeros((3, H, W)), mask, n=c + 1)
 
 
 def test_old_rows_are_copied_bit_for_bit_and_new_rows_follow_insert(cuda):
     W, H = 64, 48
     npcam = syn.make_camera(W, H, 50.0, 50.0, *syn.random_pose(np.random.default_rng(7), max_angle=0.8, max_trans=2.0))
-    cam = _dev_cam(npcam, cuda)
+    cam = syn.device_camera(npcam, cuda)
     m = _model(syn.make_scene(3000, npcam, seed=2), cuda)
     P = m.num_points()
     g = torch.Generator(device="cpu").manual_seed(0)
@@ -134,7 +128,7 @@ def test_old_rows_are_copied_bit_for_bit_and_new_rows_follow_insert(cuda):
 def _trainer_case(cuda, **kw):
     W, H = 96, 64
     npcam = syn.make_camera(W, H, 80.0, 80.0, *syn.random_pose(np.random.default_rng(1)))
-    cam = _dev_cam(npcam, cuda)
+    cam = syn.device_camera(npcam, cuda)
     scene = syn.make_scene(4000, npcam, seed=5, scale_px=2.0)
     img = torch.rand((3, H, W), generator=torch.Generator().manual_seed(1)).to(cuda)
     gt = torch.from_numpy(np.random.default_rng(3).uniform(0.5, 6.0, (H, W)).astype(np.float32)).to(cuda)
@@ -180,7 +174,7 @@ def test_selection_sees_what_the_trainer_draws(cuda):
 def test_an_empty_model_is_bootstrapped_from_one_keyframe(cuda):
     W, H = 128, 96
     npcam = syn.make_camera(W, H, 100.0, 100.0)
-    cam = _dev_cam(npcam, cuda)
+    cam = syn.device_camera(npcam, cuda)
     yy, xx = np.mgrid[0:H, 0:W]
     G = (2.0 + 0.01 * xx + 0.005 * yy).astype(np.float32)          # a slanted plane
     G[:10, :] = 0.0                                                  # no measurement
@@ -220,7 +214,7 @@ def _cat(a, b):
 def test_holes_and_objects_in_front(cuda):
     import seed_bench
     W, H, fx = 320, 240, 260.0
-    cam = _dev_cam(syn.make_camera(W, H, fx, fx), cuda)
+    cam = syn.device_camera(syn.make_camera(W, H, fx, fx), cuda)
     wall = _wall(30_000, W, H, fx)
     gt_tr = trainer.GaussianTrainer(_model(wall, cuda))
     img, G, A_full = seed_bench.sensor_depth(gt_tr, cam)

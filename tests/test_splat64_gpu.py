@@ -26,6 +26,7 @@ import numpy as np
 import pytest
 import torch
 
+import photo_slam_b200.synthetic as syn
 import splat64 as s64
 
 pytestmark = pytest.mark.gpu
@@ -45,7 +46,6 @@ GATE_LOSS_GRAD = 3e-6     # dL/dimage, max abs relative to its largest entry: me
 
 # ---- scenes -------------------------------------------------------------------------------------------------------------------------
 def _cam(W, H, f=None):
-    import photo_slam_b200.synthetic as syn
     f = f if f is not None else 0.9 * max(W, H)
     return syn.make_camera(W, H, f, f)
 
@@ -198,12 +198,6 @@ def _bg(name):
     return BG["black" if sum(map(ord, name)) % 2 else "colour"]
 
 
-def _dev_cam(cam, dev):
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(dev)
-    return dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-                tanfovy=float(cam["tanfovy"]), W=int(cam["W"]), H=int(cam["H"]))
-
-
 def _weights(H, W, dev, seed=0):
     gen = torch.Generator().manual_seed(seed)
     return ((torch.rand((3, H, W), generator=gen) - 0.5).to(dev), (0.2 * (torch.rand((H, W), generator=gen) - 0.5)).to(dev),
@@ -292,7 +286,7 @@ OP_CASES = [(n, aa) for n in SCENES for aa in (False, True)]
 def test_operator_against_truth(cuda, name, aa):
     s = _scene(name)
     cam, D, bg = s["cam"], s["D"], _bg(name)
-    c, g = _dev_cam(cam, cuda), _op_inputs(s["sc"], cuda)
+    c, g = syn.device_camera(cam, cuda), _op_inputs(s["sc"], cuda)
     bgt = torch.tensor(bg, device=cuda)
     P, W, H = g["means3D"].shape[0], cam["W"], cam["H"]
     R, color, depth, radii, geom, binning, img = _op_forward(g, c, bgt, D, aa)
@@ -375,7 +369,7 @@ def _trainer_pass(s, name, cuda, aa, det, conv=s64.CONV):
     """render + backwardPixels(random wc, wd, wa) on the trainer, and the same on the truth -> (kernel outputs, truth, raw leaves)"""
     from photo_slam_b200 import trainer
     cam, D, bg = s["cam"], s["D"], _bg(name)
-    c = _dev_cam(cam, cuda)
+    c = syn.device_camera(cam, cuda)
     W, H = cam["W"], cam["H"]
     m = _model(s["sc"], cuda, D)
     P = m.num_points()
@@ -454,7 +448,7 @@ def _builtin_backward(s, name, cuda, entry, det, aa, gt, mask, gd):
     m = _model(s["sc"], cuda, s["D"])
     tr = trainer.GaussianTrainer(m, background=torch.tensor(_bg(name), device=cuda), deterministic=det, antialiasing=aa)
     tr._apply_deterministic()
-    c = _dev_cam(s["cam"], cuda)       # held until the call has run: _ccamera keeps only its device pointers
+    c = syn.device_camera(s["cam"], cuda)       # held until the call has run: _ccamera keeps only its device pointers
     tr.render(c)
     buf = GradBuffer(m.num_points(), cuda)
     cm, cc, cs = m._cmodel(), trainer._ccamera(c), tr._cstep(True)
@@ -544,7 +538,7 @@ def test_builtin_step_against_float64_adam(cuda, name, det):
     p0 = [p.detach().double().clone() for p in params]
     mv0 = [(a.double().clone(), b.double().clone()) for a, b in moms]
     tr = trainer.GaussianTrainer(m, background=torch.tensor(_bg(name), device=cuda), deterministic=det)
-    c = _dev_cam(cam, cuda)
+    c = syn.device_camera(cam, cuda)
     tr.render(c)
     tr.trainForOneIteration(c, gt, mask, gt_depth=gd, lambda_depth=LAMBDA_DEPTH, exposure_id=0)
     loss = tr.result_depth()[0]
@@ -610,7 +604,7 @@ def test_perturbed_truth_fails_the_gate(cuda, what):
     kw, name, out = PERTURB[what]
     s = _scene(name)
     cam, D, bg = s["cam"], s["D"], _bg(name)
-    c, g = _dev_cam(cam, cuda), _op_inputs(s["sc"], cuda)
+    c, g = syn.device_camera(cam, cuda), _op_inputs(s["sc"], cuda)
     bgt = torch.tensor(bg, device=cuda)
     R, color, depth, radii, geom, binning, img = _op_forward(g, c, bgt, D, False)
     leaves, tr = _truth_op(g, cam, bg, D, False, conv=dataclasses.replace(s64.CONV, **kw))

@@ -50,9 +50,7 @@ def _camera(camname, wh, dev):
     W0, H0, fx, fy = syn.CAMERAS[camname]
     W, H = wh
     cam = syn.make_camera(W, H, fx * W / W0, fy * H / H0)
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-    c = dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-             tanfovy=float(cam["tanfovy"]), W=W, H=H)
+    c = syn.device_camera(cam, dev)
     return cam, c
 
 

@@ -7,52 +7,13 @@ at 1/2 and 1/4 resolution and compared (PSNR) with area-downsampled full-resolut
 Prints one JSON object. Writes nothing."""
 import argparse
 import json
-import os
-import sys
-import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import photo_slam_b200.synthetic as syn  # noqa: E402
-from photo_slam_b200 import rasterizer, trainer  # noqa: E402
-
-CONFIGS = {"B": (500_000, "replica"), "D": (3_000_000, "replica")}
-
-
-def _cam(dev, W, H, fx, fy, pose=None):
-    cam = syn.make_camera(W, H, fx, fy, *(pose or (None, None)))
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-    return cam, dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-                     tanfovy=float(cam["tanfovy"]), W=W, H=H)
-
-
-def _leg(sc, c, gt, dev, aa, steps, warmup):
-    m = trainer.GaussianModel.from_numpy(sc, dev)
-    m.trainingSetup(trainer.GaussianOptimizationParams())
-    tr = trainer.GaussianTrainer(m, antialiasing=aa)
-    tr.render(c)
-    for _ in range(warmup):
-        tr.trainForOneIteration(c, gt)
-        tr.result()
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(steps):
-        tr.trainForOneIteration(c, gt)
-    tr.result()
-    torch.cuda.synchronize()
-    its = steps / (time.perf_counter() - t0)
-    tr.set_profiling(True)
-    st = {}
-    for _ in range(5):
-        tr.trainForOneIteration(c, gt)
-        tr.result()
-        for k, v in tr.stage_times().items():
-            st[k] = st.get(k, 0.0) + v / 5
-    n = tr.result()[3]
-    return its, st, int(n)
+import harness
+import photo_slam_b200.synthetic as syn
+from photo_slam_b200 import rasterizer, trainer
 
 
 def _operator(sc, c, dev, aa, reps=10):
@@ -62,35 +23,38 @@ def _operator(sc, c, dev, aa, reps=10):
     args = (bg, act["means3D"], e, act["opacities"], act["scales"], act["rotations"], 1.0, e, c["viewmatrix"], c["projmatrix"], c["tanfovx"],
             c["tanfovy"], c["H"], c["W"], act["shs"], 3, c["campos"], False)
     dpix = torch.full((3, c["H"], c["W"]), 1e-6, device=dev)
-    times = []
-    for i in range(reps + 2):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
+
+    def call():
         f = rasterizer.RasterizeGaussiansCUDA(*args, antialiasing=aa)
         rasterizer.RasterizeGaussiansBackwardCUDA(bg, act["means3D"], f[2], e, act["scales"], act["rotations"], 1.0, e, c["viewmatrix"],
                                                   c["projmatrix"], c["tanfovx"], c["tanfovy"], dpix, act["shs"], 3, c["campos"], f[3], f[0], f[4], f[5],
                                                   antialiasing=aa)
-        torch.cuda.synchronize()
-        if i >= 2:
-            times.append(1e3 * (time.perf_counter() - t0))
-    return float(np.median(times))
+    return harness.cuda_ms(call, reps, warmup=2)
 
 
 def cost(dev, config, steps, warmup, rounds):
-    P, camname = CONFIGS[config]
-    W, H, fx, fy = syn.CAMERAS[camname]
-    cam, c = _cam(dev, W, H, fx, fy)
-    sc = syn.make_scene(P, cam, seed=0)
-    gt = torch.from_numpy(syn.target_image(H, W)).to(dev)
-    res = {"off": [], "on": []}
-    for _ in range(rounds):
-        for aa in (False, True):
-            res["on" if aa else "off"].append(_leg(sc, c, gt, dev, aa, steps, warmup))
+    sc, _, _, c, gt = harness.workload(config, dev)
+    m = trainer.GaussianModel.from_numpy(sc, dev)
+    m.trainingSetup(trainer.GaussianOptimizationParams())
+    trs = {"off": trainer.GaussianTrainer(m, antialiasing=False), "on": trainer.GaussianTrainer(m, antialiasing=True)}
+    rewind = harness.rewinder(m, *trs.values())   # every leg starts from the untrained model: the warm-up grows the arenas
+    for _ in range(warmup):
+        for tr in trs.values():
+            tr.trainForOneIteration(c, gt)
+            tr.result()
+    res = harness.alternate({k: (lambda tr=tr: harness.step_leg(tr, c, gt, steps, rewind)) for k, tr in trs.items()}, rounds, rewind)
+    instances = {}
+    for k, tr in trs.items():      # read after as many steps as a leg used to take: its warm-up, timed and 5 profiled steps
+        rewind()
+        for _ in range(warmup + steps + 5):
+            tr.trainForOneIteration(c, gt)
+        instances[k] = int(tr.result()[3])
+    rewind()
     out = {}
     for k, legs in res.items():
-        stages = {s: round(float(np.mean([x[1][s] for x in legs])), 3) for s in legs[0][1]}
+        stages = {s: round(v, 3) for s, v in harness.mean_stages([x[1] for x in legs]).items()}
         out[k] = {"it_s": [round(x[0], 1) for x in legs], "stage_ms": stages,
-                  "instances": legs[-1][2], "operator_fwd_bwd_ms": round(_operator(sc, c, dev, k == "on"), 3)}
+                  "instances": instances[k], "operator_fwd_bwd_ms": round(_operator(sc, c, dev, k == "on"), 3)}
     return out
 
 
@@ -99,7 +63,8 @@ def evidence(dev, steps=300):
     W, H = 600, 340
     rng = np.random.default_rng(1)
     poses = [syn.random_pose(rng, max_angle=0.1, max_trans=0.1) for _ in range(8)]
-    cams = [_cam(dev, W, H, 300.0, 300.0, p) for p in poses]
+    cams = [syn.make_camera(W, H, 300.0, 300.0, *p) for p in poses]
+    cams = [(cam, syn.device_camera(cam, dev)) for cam in cams]
     target = syn.make_scene(40_000, cams[0][0], seed=11, scale_px=1.2)     # small splats: the case the filter is for
     tm = trainer.GaussianModel.from_numpy(target, dev)
     gts = [trainer.GaussianTrainer(tm).render(c) for _, c in cams]
@@ -116,7 +81,7 @@ def evidence(dev, steps=300):
         for f in (1, 2, 4):
             ps = []
             for (cam, c), (pose, gt) in zip(cams, zip(poses, gts)):
-                _, cs = _cam(dev, W // f, H // f, 300.0 / f, 300.0 / f, pose)
+                cs = syn.device_camera(syn.make_camera(W // f, H // f, 300.0 / f, 300.0 / f, *pose), dev)
                 img = tr.render(cs)
                 ref = torch.nn.functional.avg_pool2d(gt[None], f)[0] if f > 1 else gt
                 mse = ((img - ref[:, :img.shape[1], :img.shape[2]]) ** 2).mean().item()
@@ -134,14 +99,8 @@ if __name__ == "__main__":
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--evidence-steps", type=int, default=300)
     a = ap.parse_args()
-    dev = torch.device("cuda:0")
-    props = torch.cuda.get_device_properties(dev)
-    try:
-        import subprocess
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True).stdout.strip()
-    except Exception:  # noqa: BLE001
-        pl = "unknown"
-    res = {"gpu": props.name, "power_limit": pl, "cost": {cfg: cost(dev, cfg, a.steps, a.warmup, a.rounds) for cfg in a.configs}}
+    dev = harness.device()
+    res = {"card": harness.card(), "cost": {cfg: cost(dev, cfg, a.steps, a.warmup, a.rounds) for cfg in a.configs}}
     if a.evidence_steps > 0:
         res["evidence"] = evidence(dev, a.evidence_steps)
     print(json.dumps(res))

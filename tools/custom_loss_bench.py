@@ -19,15 +19,11 @@ alternating pair by pair; reported as the mean render_fwd / render_bwd stage tim
 writes nothing."""
 import argparse
 import json
-import os
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path[:0] = [ROOT, os.path.join(ROOT, "oracle")]
-import bench  # noqa: E402  (its workload: make_inputs)
+import harness
 
 
 def make_loss(gt, mask, gt_depth, lam):
@@ -47,11 +43,10 @@ def main():
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--lambda-depth", type=float, default=0.1)
     a = ap.parse_args()
-    a.points, a.camera = {"B": (500_000, "replica"), "C": (1_000_000, "tum"), "D": (3_000_000, "replica")}[a.config]
+    dev = harness.device()
     from photo_slam_b200 import renderer
     from photo_slam_b200 import trainer as T
-    dev = torch.device("cuda", 0)
-    scene, cam, host, devcam, gt = bench.make_inputs(a, 0, dev)
+    scene, cam, host, devcam, gt = harness.workload(a.config, dev)
     model = T.GaussianModel.from_numpy(scene, dev)
     model.trainingSetup(T.GaussianOptimizationParams())
     tr = T.GaussianTrainer(model)
@@ -89,13 +84,11 @@ def main():
     for _ in range(max(a.warmup, 2)):
         builtin(); tr.result()
         pixels(); tr.result()
-    snap, it0 = model.snapshot(), tr.iteration
+    model_rewind = harness.rewinder(model, tr)
     start = [t.detach().clone() for t in leaves]
 
     def rewind():
-        torch.cuda.synchronize()
-        model.restore(snap)
-        tr.iteration = it0
+        model_rewind()
         with torch.no_grad():
             for t, s in zip(leaves, start):
                 t.copy_(s)
@@ -104,33 +97,18 @@ def main():
     opt = rewind()
     for _ in range(max(a.warmup, 2)):
         op_step(opt)
-    legs = ("builtin", "pixels", "operator")
-    res = {k: dict(ms=[], stages=[]) for k in legs}
-    for rnd in range(a.rounds):
-        for name in legs[rnd % 3:] + legs[:rnd % 3]:
-            opt = rewind()
-            step = {"builtin": builtin, "pixels": pixels, "operator": lambda: op_step(opt)}[name]
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(a.steps):
-                step()
-            e1.record()
-            if name != "operator":
-                tr.result()
-            torch.cuda.synchronize()
-            res[name]["ms"].append(e0.elapsed_time(e1) / a.steps)
-            if name == "operator":
-                continue
-            rewind()
-            tr.set_profiling(True)
-            acc = {}
-            for _ in range(a.steps):
-                step()
-                tr.result()
-                for k, v in tr.stage_times().items():
-                    acc.setdefault(k, []).append(v)
-            tr.set_profiling(False)
-            res[name]["stages"].append({k: float(np.mean(v)) for k, v in acc.items()})
+
+    def leg(name):
+        opt = rewind()
+        step = {"builtin": builtin, "pixels": pixels, "operator": lambda: op_step(opt)}[name]
+        ms = harness.window_ms(step, a.steps)
+        if name == "operator":
+            return ms, None
+        tr.result()
+        rewind()
+        return ms, harness.stage_ms(tr, step, a.steps)
+
+    res = harness.alternate({k: (lambda k=k: leg(k)) for k in ("builtin", "pixels", "operator")}, a.rounds)
     # the opacity variants against the same passes without them (gradient mode: no drift between the two)
     rewind()
     gen = torch.Generator().manual_seed(2)
@@ -151,12 +129,13 @@ def main():
                 variant[with_alpha].setdefault(k, []).append(v)
     tr.set_profiling(False)
     rewind()
-    out = {"config": a.config, "gaussians": a.points, "width": W, "height": H, "steps": a.steps, "rounds": a.rounds, "lambda_depth": a.lambda_depth,
-           "device": torch.cuda.get_device_name(dev), "unit": "ms per step (CUDA events over K steps), ms per stage (K profiled steps)"}
+    out = {"config": a.config, "gaussians": model.num_points(), "width": W, "height": H, "steps": a.steps, "rounds": a.rounds,
+           "lambda_depth": a.lambda_depth, "card": harness.card(), "unit": "ms per step (CUDA events over K steps), ms per stage (K profiled steps)"}
     for name, r in res.items():
-        out[name] = {"ms_per_step": r["ms"], "ms_per_step_mean": float(np.mean(r["ms"]))}
-        if r["stages"]:
-            out[name]["stages"] = {k: float(np.mean([s[k] for s in r["stages"]])) for k in r["stages"][0]}
+        ms = [x[0] for x in r]
+        out[name] = {"ms_per_step": ms, "ms_per_step_mean": float(np.mean(ms))}
+        if r[0][1] is not None:
+            out[name]["stages"] = harness.mean_stages([x[1] for x in r])
     out["pixels_minus_builtin_stage_ms"] = {k: out["pixels"]["stages"][k] - out["builtin"]["stages"][k] for k in out["builtin"]["stages"]}
     out["opacity_variants"] = {"with_ms": {k: float(np.mean(variant[True][k])) for k in ("render_fwd", "render_bwd")},
                                "without_ms": {k: float(np.mean(variant[False][k])) for k in ("render_fwd", "render_bwd")}}

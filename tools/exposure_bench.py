@@ -10,78 +10,37 @@ Prints one JSON object. Writes nothing."""
 import argparse
 import json
 import math
-import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import photo_slam_b200.synthetic as syn  # noqa: E402
-from photo_slam_b200 import trainer  # noqa: E402
-
-CONFIGS = {"B": (500_000, "replica"), "D": (3_000_000, "replica")}
-
-
-def _cam(dev, W, H, fx, fy, pose=None):
-    cam = syn.make_camera(W, H, fx, fy, *(pose or (None, None)))
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-    return cam, dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-                     tanfovy=float(cam["tanfovy"]), W=W, H=H)
-
-
-def _leg(m, tr, snap, c, gt, exposure, steps, warmup):
-    m.restore(snap)
-    k = 0 if exposure else None
-    for _ in range(warmup):
-        tr.trainForOneIteration(c, gt, exposure_id=k)
-        tr.result()
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(steps):
-        tr.trainForOneIteration(c, gt, exposure_id=k)
-    tr.result()
-    torch.cuda.synchronize()
-    its = steps / (time.perf_counter() - t0)
-    tr.set_profiling(True)
-    st = {}
-    for _ in range(5):
-        tr.trainForOneIteration(c, gt, exposure_id=k)
-        tr.result()
-        for name, v in tr.stage_times().items():
-            st[name] = st.get(name, 0.0) + v / 5
-    tr.set_profiling(False)
-    return its, st
+import harness
+import photo_slam_b200.synthetic as syn
+from photo_slam_b200 import trainer
 
 
 def cost(dev, config, steps, warmup, rounds):
-    P, camname = CONFIGS[config]
-    W, H, fx, fy = syn.CAMERAS[camname]
-    cam, c = _cam(dev, W, H, fx, fy)
-    m = trainer.GaussianModel.from_numpy(syn.make_scene(P, cam, seed=0), dev)
+    sc, _, _, c, gt = harness.workload(config, dev)
+    m = trainer.GaussianModel.from_numpy(sc, dev)
     m.trainingSetup(trainer.GaussianOptimizationParams())
     m.ensureExposures(1)
-    gt = torch.from_numpy(syn.target_image(H, W)).to(dev)
     tr = trainer.GaussianTrainer(m)
-    tr.render(c)
-    snap = m.snapshot()
-    res = {"off": [], "on": []}
-    for _ in range(rounds):
-        for on in (False, True):
-            res["on" if on else "off"].append(_leg(m, tr, snap, c, gt, on, steps, warmup))
-    out = {}
-    for key, legs in res.items():
-        out[key] = {"it_s": [round(x[0], 1) for x in legs],
-                    "stage_ms": {s: round(float(np.mean([x[1][s] for x in legs])), 4) for s in legs[0][1]}}
-    return out
+    legs = {"off": None, "on": 0}
+    rewind = harness.rewinder(m, tr)   # every leg starts from the untrained model: the warm-up grows the arenas
+    for _ in range(warmup):
+        for k in legs.values():
+            tr.trainForOneIteration(c, gt, exposure_id=k)
+            tr.result()
+    res = harness.alternate({key: (lambda k=k: harness.step_leg(tr, c, gt, steps, rewind, exposure_id=k)) for key, k in legs.items()}, rounds, rewind)
+    rewind()
+    return {key: {"it_s": [round(x[0], 1) for x in r], "stage_ms": {s: round(v, 4) for s, v in harness.mean_stages([x[1] for x in r]).items()}}
+            for key, r in res.items()}
 
 
 def evidence(dev, steps, W=600, H=340, views=8, P=40_000):
     rng = np.random.default_rng(1)
-    cams = [_cam(dev, W, H, 300.0, 300.0, syn.random_pose(rng, max_angle=0.1, max_trans=0.1)) for _ in range(views)]
+    cams = [syn.make_camera(W, H, 300.0, 300.0, *syn.random_pose(rng, max_angle=0.1, max_trans=0.1)) for _ in range(views)]
+    cams = [(cam, syn.device_camera(cam, dev)) for cam in cams]
     tm = trainer.GaussianModel.from_numpy(syn.make_scene(P, cams[0][0], seed=11, scale_px=2.0), dev)
     raw = [trainer.GaussianTrainer(tm).render(c) for _, c in cams]
     Es = torch.zeros(views, 3, 4)
@@ -123,15 +82,8 @@ if __name__ == "__main__":
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--evidence-steps", type=int, default=800)
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("exposure_bench.py needs a CUDA device")
-    dev = torch.device("cuda:0")
-    props = torch.cuda.get_device_properties(dev)
-    try:
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True).stdout.strip()
-    except Exception:  # noqa: BLE001
-        pl = "unknown"
-    res = {"gpu": props.name, "power_limit": pl, "cost": {cfg: cost(dev, cfg, a.steps, a.warmup, a.rounds) for cfg in a.configs}}
+    dev = harness.device()
+    res = {"card": harness.card(), "cost": {cfg: cost(dev, cfg, a.steps, a.warmup, a.rounds) for cfg in a.configs}}
     if a.evidence_steps > 0:
         res["evidence"] = evidence(dev, a.evidence_steps)
     print(json.dumps(res))

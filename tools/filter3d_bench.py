@@ -8,41 +8,27 @@ filter (recomputed from the 8 full-resolution cameras every 100 steps and after 
 against the targets (PSNR). Prints one JSON object with the card's name and power limit. Writes nothing."""
 import argparse
 import json
-import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import photo_slam_b200.synthetic as syn  # noqa: E402
-from photo_slam_b200 import _lib, trainer  # noqa: E402
-
-CONFIGS = {"B": (500_000, "replica"), "D": (3_000_000, "replica")}
-
-
-def _cam(dev, W, H, fx, fy, pose=None):
-    cam = syn.make_camera(W, H, fx, fy, *(pose or (None, None)))
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-    return cam, dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-                     tanfovy=float(cam["tanfovy"]), W=W, H=H)
+import harness
+import photo_slam_b200.synthetic as syn
+from photo_slam_b200 import _lib, trainer
 
 
 def _views(dev, K, W, H, f, seed=0):
     rng = np.random.default_rng(seed)
-    return [_cam(dev, W, H, f, f, syn.random_pose(rng, max_angle=0.3, max_trans=0.5))[1] for _ in range(K)]
+    return [syn.device_camera(syn.make_camera(W, H, f, f, *syn.random_pose(rng, max_angle=0.3, max_trans=0.5)), dev) for _ in range(K)]
 
 
 def filter_cost(dev):
     out = {}
     L = trainer._bind()
-    for P, camname in ((500_000, "replica"), (3_000_000, "replica")):
-        W, H, fx, fy = syn.CAMERAS[camname]
-        cam, c = _cam(dev, W, H, fx, fy)
-        m = trainer.GaussianModel.from_numpy(syn.make_scene(P, cam, seed=0), dev)
+    for config in ("B", "D"):
+        sc, _, _, c, _ = harness.workload(config, dev)
+        P, (W, H, fx, _) = len(sc["xyz"]), syn.CAMERAS[harness.CONFIGS[config][1]]
+        m = trainer.GaussianModel.from_numpy(sc, dev)
         f = torch.empty(P, device=dev)
         for K in (100, 300, 1000):
             views = _views(dev, K, W, H, fx)
@@ -50,62 +36,34 @@ def filter_cost(dev):
             packed = torch.tensor(np.stack([np.concatenate([v["viewmatrix"].cpu().numpy().reshape(-1), [W / (2 * v["tanfovx"]), H / (2 * v["tanfovy"]), W, H]])
                                             for v in views]), dtype=torch.float32, device=dev)
             s = torch.cuda.current_stream()
-            times = []
-            for i in range(7):
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record(s)
-                _lib.check(L.psb_filter3d(P, m.xyz_.data_ptr(), K, packed.data_ptr(), f.data_ptr(), None, s.cuda_stream), "psb_filter3d")
-                e1.record(s)
-                e1.synchronize()
-                if i >= 2:
-                    times.append(e0.elapsed_time(e1))
+            call = lambda: _lib.check(L.psb_filter3d(P, m.xyz_.data_ptr(), K, packed.data_ptr(), f.data_ptr(), None, s.cuda_stream), "psb_filter3d")
+            times = [harness.window_ms(call, 1) for _ in range(7)][2:]      # each call from an idle device, after 2 warm-up calls
             out[f"P={P},K={K}"] = {"ms": round(float(np.median(times)), 3), "rows_seen": m.computeFilter3D(views)}
     return out
 
 
-def _leg(sc, c, gt, dev, views, on, steps, warmup):
+def step_cost(dev, config, steps, warmup, rounds):
+    sc, _, _, c, gt = harness.workload(config, dev)
     m = trainer.GaussianModel.from_numpy(sc, dev)
     m.trainingSetup(trainer.GaussianOptimizationParams())
-    if on:
-        m.computeFilter3D(views)
-    tr = trainer.GaussianTrainer(m, filter3d=on)
-    tr.render(c)
+    W, H, fx, _ = syn.CAMERAS[harness.CONFIGS[config][1]]
+    m.computeFilter3D([c] + _views(dev, 31, W, H, fx))
+    trs = {"off": trainer.GaussianTrainer(m, filter3d=False), "on": trainer.GaussianTrainer(m, filter3d=True)}
+    rewind = harness.rewinder(m, *trs.values())   # every leg starts from the untrained model: the warm-up grows the arenas
     for _ in range(warmup):
-        tr.trainForOneIteration(c, gt)
-        tr.result()
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(steps):
-        tr.trainForOneIteration(c, gt)
-    tr.result()
-    torch.cuda.synchronize()
-    its = steps / (time.perf_counter() - t0)
-    tr.set_profiling(True)
-    st = {}
-    for _ in range(5):
-        tr.trainForOneIteration(c, gt)
-        tr.result()
-        for k, v in tr.stage_times().items():
-            st[k] = st.get(k, 0.0) + v / 5
-    return its, st, int(tr.result()[3])
-
-
-def step_cost(dev, config, steps, warmup, rounds):
-    P, camname = CONFIGS[config]
-    W, H, fx, fy = syn.CAMERAS[camname]
-    cam, c = _cam(dev, W, H, fx, fy)
-    sc = syn.make_scene(P, cam, seed=0)
-    gt = torch.from_numpy(syn.target_image(H, W)).to(dev)
-    views = [c] + _views(dev, 31, W, H, fx)
-    res = {"off": [], "on": []}
-    for _ in range(rounds):
-        for on in (False, True):
-            res["on" if on else "off"].append(_leg(sc, c, gt, dev, views, on, steps, warmup))
-    out = {}
-    for k, legs in res.items():
-        out[k] = {"it_s": [round(x[0], 1) for x in legs], "stage_ms": {s: round(float(np.mean([x[1][s] for x in legs])), 3) for s in legs[0][1]},
-                  "instances": legs[-1][2]}
-    return out
+        for tr in trs.values():
+            tr.trainForOneIteration(c, gt)
+            tr.result()
+    res = harness.alternate({k: (lambda tr=tr: harness.step_leg(tr, c, gt, steps, rewind)) for k, tr in trs.items()}, rounds, rewind)
+    instances = {}
+    for k, tr in trs.items():      # read after as many steps as a leg used to take: its warm-up, timed and 5 profiled steps
+        rewind()
+        for _ in range(warmup + steps + 5):
+            tr.trainForOneIteration(c, gt)
+        instances[k] = int(tr.result()[3])
+    rewind()
+    return {k: {"it_s": [round(x[0], 1) for x in legs], "stage_ms": {s: round(v, 3) for s, v in harness.mean_stages([x[1] for x in legs]).items()},
+                "instances": instances[k]} for k, legs in res.items()}
 
 
 def _psnr(a, b):
@@ -116,8 +74,8 @@ def evidence(dev, steps=600):
     Wf, Hf, ff = 1200, 680, 600.0
     rng = np.random.default_rng(1)
     poses = [syn.random_pose(rng, max_angle=0.1, max_trans=0.1) for _ in range(8)]
-    full = [_cam(dev, Wf, Hf, ff, ff, p) for p in poses]
-    half = [_cam(dev, Wf // 2, Hf // 2, ff / 2, ff / 2, p)[1] for p in poses]
+    full = [(cam, syn.device_camera(cam, dev)) for cam in (syn.make_camera(Wf, Hf, ff, ff, *p) for p in poses)]
+    half = [syn.device_camera(syn.make_camera(Wf // 2, Hf // 2, ff / 2, ff / 2, *p), dev) for p in poses]
     target = trainer.GaussianModel.from_numpy(syn.make_scene(100_000, full[0][0], seed=11, scale_px=1.5), dev)
     gts_full = [trainer.GaussianTrainer(target, antialiasing=True).render(c) for _, c in full]
     gts_half = [torch.nn.functional.avg_pool2d(g[None], 2)[0].contiguous() for g in gts_full]
@@ -154,10 +112,8 @@ if __name__ == "__main__":
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--evidence-steps", type=int, default=600)
     a = ap.parse_args()
-    dev = torch.device("cuda:0")
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
-    res = {"gpu": torch.cuda.get_device_name(dev), "nvidia_smi": q.stdout.strip(), "filter3d": filter_cost(dev),
-           "step": {cfg: step_cost(dev, cfg, a.steps, a.warmup, a.rounds) for cfg in a.configs}}
+    dev = harness.device()
+    res = {"card": harness.card(), "filter3d": filter_cost(dev), "step": {cfg: step_cost(dev, cfg, a.steps, a.warmup, a.rounds) for cfg in a.configs}}
     if a.evidence_steps > 0:
         res["evidence"] = evidence(dev, a.evidence_steps)
     print(json.dumps(res))

@@ -11,89 +11,41 @@ Prints one JSON object. Writes nothing."""
 import argparse
 import json
 import math
-import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import photo_slam_b200.synthetic as syn  # noqa: E402
-from photo_slam_b200 import trainer  # noqa: E402
-
-CONFIGS = {"B": (500_000, "replica"), "D": (3_000_000, "replica")}
-
-
-def _cam(dev, W, H, fx, fy, pose=None):
-    cam = syn.make_camera(W, H, fx, fy, *(pose or (None, None)))
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-    return cam, dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-                     tanfovy=float(cam["tanfovy"]), W=W, H=H)
-
-
-def _events(fn, n):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    a.record()
-    for _ in range(n):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / n
-
-
-def _leg(m, tr, snap, c, gt, steps, warmup):
-    m.restore(snap)
-    for _ in range(warmup):
-        tr.trainForOneIteration(c, gt)
-        tr.result()
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(steps):
-        tr.trainForOneIteration(c, gt)
-    tr.result()
-    torch.cuda.synchronize()
-    its = steps / (time.perf_counter() - t0)
-    tr.set_profiling(True)
-    st = {}
-    for _ in range(5):
-        tr.trainForOneIteration(c, gt)
-        tr.result()
-        for name, v in tr.stage_times().items():
-            st[name] = st.get(name, 0.0) + v / 5
-    tr.set_profiling(False)
-    return its, st
+import harness
+import photo_slam_b200.synthetic as syn
+from photo_slam_b200 import trainer
 
 
 def step_cost(dev, config, steps, warmup, rounds):
-    P, camname = CONFIGS[config]
-    W, H, fx, fy = syn.CAMERAS[camname]
-    cam, c = _cam(dev, W, H, fx, fy)
-    m = trainer.GaussianModel.from_numpy(syn.make_scene(P, cam, seed=0), dev)
+    sc, _, _, c, gt = harness.workload(config, dev)
+    P = len(sc["xyz"])
+    m = trainer.GaussianModel.from_numpy(sc, dev)
     opts = {"off": trainer.GaussianOptimizationParams(), "on": trainer.GaussianOptimizationParams(mcmc=True, cap_max=P)}
     m.trainingSetup(opts["off"])
-    gt = torch.from_numpy(syn.target_image(H, W)).to(dev)
     trs = {k: trainer.GaussianTrainer(m, o) for k, o in opts.items()}
-    for tr in trs.values():
-        tr.render(c)
-    snap = m.snapshot()
-    res = {"off": [], "on": []}
-    for _ in range(rounds):
-        for key in ("off", "on"):
-            res[key].append(_leg(m, trs[key], snap, c, gt, steps, warmup))
-    out = {}
-    for key, legs in res.items():
-        out[key] = {"it_s": [round(x[0], 1) for x in legs],
-                    "stage_ms": {s: round(float(np.mean([x[1][s] for x in legs])), 4) for s in legs[0][1]}}
-    # the noise kernel alone, behind a pass of the mcmc trainer
+    rewind = harness.rewinder(m, *trs.values())   # every leg starts from the untrained model: the warm-up grows the arenas
+    for _ in range(warmup):
+        for tr in trs.values():
+            tr.trainForOneIteration(c, gt)
+            tr.result()
+    res = harness.alternate({k: (lambda tr=tr: harness.step_leg(tr, c, gt, steps, rewind)) for k, tr in trs.items()}, rounds, rewind)
+    rewind()
+    out = {k: {"it_s": [round(x[0], 1) for x in legs], "stage_ms": {s: round(v, 4) for s, v in harness.mean_stages([x[1] for x in legs]).items()}}
+           for k, legs in res.items()}
+    # the noise kernel alone, behind a pass of the mcmc trainer, on the model as one "on" leg leaves it (its warm-up, timed and 5
+    # profiled steps); refine_cost then works on that model
     tr = trs["on"]
+    for _ in range(warmup + steps + 5):
+        tr.trainForOneIteration(c, gt)
+    tr.result()
     radii = torch.zeros(P, dtype=torch.int32, device=dev)
     tr.trainForOneIteration(c, gt, radii=radii)
     tr.result()
-    ms = _events(tr._inject_noise, 20)
+    ms = harness.window_ms(tr._inject_noise, 20)     # back to back: one launch is shorter than its host side
     visible = int((radii > 0).sum())
     out["noise_kernel"] = {"ms": round(ms, 4), "rows": P, "visible_rows": visible, "bytes": 16 * P + 56 * visible,
                            "GB_s": round((16 * P + 56 * visible) / ms / 1e6, 1)}
@@ -110,7 +62,7 @@ def refine_cost(dev, m, rounds=3):
     out = {"rows": P, "dead_rows": int(dead.sum()), "relocate_ms": [], "grow_ms": [], "densify_and_prune_ms": []}
     for _ in range(rounds):
         m.restore(snap)
-        out["relocate_ms"].append(round(_events(lambda: m.relocateGaussians(0.005, seed=1), 1), 3))
+        out["relocate_ms"].append(round(harness.window_ms(lambda: m.relocateGaussians(0.005, seed=1), 1), 3))
     keep = {k: [t.clone() for t in snap[k]] for k in ("p", "stats")}
     for fn, key in ((lambda mm: mm.addNewGaussians(2 * P, 1.05, seed=1), "grow_ms"),
                     (lambda mm: mm.densifyAndPrune(0.0019, 0.005, 5.0, 0, seed=1), "densify_and_prune_ms")):
@@ -119,27 +71,18 @@ def refine_cost(dev, m, rounds=3):
             mm._set([t.clone() for t in keep["p"]])
             mm.trainingSetup(trainer.GaussianOptimizationParams())
             mm.xyz_gradient_accum_, mm.denom_ = keep["stats"][0].clone(), keep["stats"][1].clone()
-            out[key].append(round(_events(lambda: fn(mm), 1), 3))
+            out[key].append(round(harness.window_ms(lambda: fn(mm), 1), 3))
             out[key + "_rows_after"] = mm.num_points()
             del mm
     return out
 
 
 def quality(dev, steps, cap=400_000):
-    P, W, H, fx = 200_000, 640, 480, 520.9
-    cam0 = syn.make_camera(W, H, fx, fx)
-    gt_scene = syn.make_scene(P, cam0, seed=21, scale_px=3.0)
-    views = [_cam(dev, W, H, fx, fx, None if k == 0 else syn.random_pose(np.random.default_rng(50 + k), max_angle=0.06, max_trans=0.12))[1] for k in range(6)]
+    gt_scene, cams = syn.quality_scene()
+    views = [syn.device_camera(cam, dev) for cam in cams]
     gt_tr = trainer.GaussianTrainer(trainer.GaussianModel.from_numpy(gt_scene, dev))
     gts = [gt_tr.render(c).clamp(0, 1).clone() for c in views]
-    rng = np.random.default_rng(3)
-    keep = rng.random(P) < 0.8
-    start = {k: v[keep].copy() for k, v in gt_scene.items()}
-    start["xyz"] += rng.normal(0, 0.01, start["xyz"].shape).astype(np.float32)
-    start["features_dc"] += rng.normal(0, 0.6, start["features_dc"].shape).astype(np.float32)
-    start["features_rest"] *= 0
-    start["opacity"] += rng.normal(0, 0.7, start["opacity"].shape).astype(np.float32)
-    start["scaling"] += np.float32(0.15)
+    start = syn.thinned_trainee(gt_scene)
     out = {}
     for mcmc in (False, True):
         opt = trainer.GaussianOptimizationParams(mcmc=mcmc, cap_max=cap, mcmc_grow_factor=1.2)
@@ -172,15 +115,8 @@ if __name__ == "__main__":
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--quality-steps", type=int, default=600)
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("mcmc_bench.py needs a CUDA device")
-    dev = torch.device("cuda:0")
-    props = torch.cuda.get_device_properties(dev)
-    try:
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True).stdout.strip()
-    except Exception:  # noqa: BLE001
-        pl = "unknown"
-    res = {"gpu": props.name, "power_limit": pl, "step": {}}
+    dev = harness.device()
+    res = {"card": harness.card(), "step": {}}
     m = None
     for cfg in a.configs:
         res["step"][cfg], m = step_cost(dev, cfg, a.steps, a.warmup, a.rounds)

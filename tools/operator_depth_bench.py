@@ -10,33 +10,17 @@ reference's, to size the binning scratch). Prints one JSON line with the per-rou
 each leg between rounds, the device name and its power limit; writes nothing."""
 import argparse
 import json
-import os
-import sys
 
 import numpy as np
 import torch
 import torch.nn.functional as F
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path[:0] = [ROOT, os.path.join(ROOT, "oracle")]
-import bench  # noqa: E402  (its workload: make_inputs)
-
-
-def power_limit_w(index):
-    try:
-        import pynvml
-        pynvml.nvmlInit()
-        h = pynvml.nvmlDeviceGetHandleByIndex(index)
-        return pynvml.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
-    except Exception:  # noqa: BLE001
-        return None
+import harness
 
 
 def run_config(config, a, dev):
     from photo_slam_b200 import rasterizer as R
-    args = argparse.Namespace(config=config)
-    args.points, args.camera = {"B": (500_000, "replica"), "D": (3_000_000, "replica")}[config]
-    scene, cam, host, c, gt = bench.make_inputs(args, 0, dev)
+    scene, cam, host, c, gt = harness.workload(config, dev)
     T = lambda k: torch.from_numpy(scene[k]).to(dev)
     means3D, opac = T("xyz"), torch.sigmoid(T("opacity"))
     scales, rots = torch.exp(T("scaling")), F.normalize(T("rotation"))
@@ -50,40 +34,32 @@ def run_config(config, a, dev):
     ddep = torch.randn((H, W), device=dev, generator=gen) / (H * W)
 
     def leg(depth):
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
         fwd = R.RasterizeGaussiansDepthCUDA if depth else R.RasterizeGaussiansCUDA
-        ev[0].record()
-        for _ in range(a.calls):
-            out = fwd(*fwd_args)
-        ev[1].record()
+        last = {}
+
+        def forward():
+            last["out"] = fwd(*fwd_args)
+        f_ms = harness.window_ms(forward, a.calls)
+        out = last["out"]
         nr, radii, bufs = out[0], out[-4], out[-3:]
         bwd_args = (bg, means3D, radii, e, scales, rots, 1.0, e, c["viewmatrix"], c["projmatrix"], c["tanfovx"], c["tanfovy"], dpix)
         tail = (shs, 3, c["campos"], bufs[0], nr, bufs[1], bufs[2])
-        ev[2].record()
-        for _ in range(a.calls):
-            if depth:
-                R.RasterizeGaussiansBackwardDepthCUDA(*bwd_args, ddep, *tail)
-            else:
-                R.RasterizeGaussiansBackwardCUDA(*bwd_args, *tail)
-        ev[3].record()
-        torch.cuda.synchronize()
-        return ev[0].elapsed_time(ev[1]) / a.calls, ev[2].elapsed_time(ev[3]) / a.calls, nr
+        if depth:
+            bwd = lambda: R.RasterizeGaussiansBackwardDepthCUDA(*bwd_args, ddep, *tail)
+        else:
+            bwd = lambda: R.RasterizeGaussiansBackwardCUDA(*bwd_args, *tail)
+        return f_ms, harness.window_ms(bwd, a.calls), nr
 
     for _ in range(a.warmup):
         leg(False)
         leg(True)
-    res = {k: dict(forward_ms=[], backward_ms=[]) for k in ("plain", "depth")}
-    for rnd in range(a.rounds):
-        for name in (("plain", "depth") if rnd % 2 == 0 else ("depth", "plain")):
-            f, b, nr = leg(name == "depth")
-            res[name]["forward_ms"].append(f)
-            res[name]["backward_ms"].append(b)
-    out = {"gaussians": args.points, "width": W, "height": H, "num_rendered": int(nr)}
-    for name, r in res.items():
-        out[name] = {k: v for k, v in r.items()}
+    legs = harness.alternate({"plain": lambda: leg(False), "depth": lambda: leg(True)}, a.rounds)
+    out = {"gaussians": len(scene["xyz"]), "width": W, "height": H, "num_rendered": int(legs["depth"][-1][2])}
+    for name, r in legs.items():
+        out[name] = {"forward_ms": [x[0] for x in r], "backward_ms": [x[1] for x in r]}
         for k in ("forward_ms", "backward_ms"):
-            out[name][k + "_mean"] = float(np.mean(r[k]))
-            out[name][k + "_spread"] = float(np.max(r[k]) - np.min(r[k]))
+            out[name][k + "_mean"] = float(np.mean(out[name][k]))
+            out[name][k + "_spread"] = float(np.max(out[name][k]) - np.min(out[name][k]))
     out["depth_cost_ms"] = {k: out["depth"][k + "_mean"] - out["plain"][k + "_mean"] for k in ("forward_ms", "backward_ms")}
     return out
 
@@ -95,9 +71,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--rounds", type=int, default=4)
     a = ap.parse_args()
-    dev = torch.device("cuda", 0)
-    out = {"device": torch.cuda.get_device_name(dev), "power_limit_w": power_limit_w(0), "calls": a.calls, "rounds": a.rounds,
-           "unit": "ms per call (CUDA events)"}
+    dev = harness.device()
+    out = {"card": harness.card(), "calls": a.calls, "rounds": a.rounds, "unit": "ms per call (CUDA events)"}
     for config in a.configs.split(","):
         out[config] = run_config(config, a, dev)
         torch.cuda.empty_cache()

@@ -11,34 +11,14 @@ the deterministic scratch size, the largest relative-norm difference between the
 its power limit; writes nothing."""
 import argparse
 import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
 import torch.nn.functional as F
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path[:0] = [ROOT, os.path.join(ROOT, "oracle")]
-import bench  # noqa: E402  (its workload: make_inputs)
+import harness
 
 LEGS = ("atomic", "deterministic", "atomic_depth", "deterministic_depth")
-
-
-def power_limit_w(index):
-    try:
-        import pynvml
-        pynvml.nvmlInit()
-        return pynvml.nvmlDeviceGetEnforcedPowerLimit(pynvml.nvmlDeviceGetHandleByIndex(index)) / 1000.0
-    except Exception:  # noqa: BLE001
-        pass
-    try:
-        out = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=power.limit", "--format=csv,noheader,nounits"], capture_output=True,
-                             text=True, timeout=30).stdout
-        return float(out.strip().splitlines()[0])
-    except Exception:  # noqa: BLE001
-        return None
 
 
 def _stats(v):
@@ -48,9 +28,8 @@ def _stats(v):
 def run_config(config, a, dev):
     from photo_slam_b200 import _lib
     from photo_slam_b200 import rasterizer as R
-    args = argparse.Namespace(config=config)
-    args.points, args.camera = {"B": (500_000, "replica"), "D": (3_000_000, "replica")}[config]
-    scene, cam, host, c, gt = bench.make_inputs(args, 0, dev)
+    scene, cam, host, c, gt = harness.workload(config, dev)
+    P = len(scene["xyz"])
     T = lambda k: torch.from_numpy(scene[k]).to(dev)
     means3D, opac = T("xyz"), torch.sigmoid(T("opacity"))
     scales, rots = torch.exp(T("scaling")), F.normalize(T("rotation"))
@@ -72,30 +51,19 @@ def run_config(config, a, dev):
             return R.RasterizeGaussiansBackwardDepthCUDA(*head, ddep, *tail, deterministic=det)
         return R.RasterizeGaussiansBackwardCUDA(*head, *tail, deterministic=det)
 
-    def timed(fn):
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
-        ev[0].record()
-        for _ in range(a.calls):
-            fn()
-        ev[1].record()
-        torch.cuda.synchronize()
-        return ev[0].elapsed_time(ev[1]) / a.calls
-
     forwards = {"colour": lambda: R.RasterizeGaussiansCUDA(*fwd_args), "depth": lambda: R.RasterizeGaussiansDepthCUDA(*fwd_args)}
     for _ in range(a.warmup):
         for f in forwards.values():
             f()
         for leg in LEGS:
             backward(leg)
-    torch.cuda.synchronize()
     fwd_ms = {k: [] for k in forwards}
     bwd_ms = {k: [] for k in LEGS}
     for rnd in range(a.rounds):
-        order = LEGS[rnd % len(LEGS):] + LEGS[:rnd % len(LEGS)]
         for k in (("colour", "depth") if rnd % 2 == 0 else ("depth", "colour")):
-            fwd_ms[k].append(timed(forwards[k]))
-        for leg in order:
-            bwd_ms[leg].append(timed(lambda: backward(leg)))
+            fwd_ms[k].append(harness.window_ms(forwards[k], a.calls))
+        for leg in LEGS[rnd % len(LEGS):] + LEGS[:rnd % len(LEGS)]:
+            bwd_ms[leg].append(harness.window_ms(lambda: backward(leg), a.calls))
     # the same gradients up to the order of the sums; the deterministic ones repeat bit for bit
     diff = {}
     for depth in (False, True):
@@ -104,8 +72,8 @@ def run_config(config, a, dev):
         diff["depth" if depth else "colour"] = {
             "max_relnorm_vs_atomic": max(((x - y).double().norm() / (y.double().norm() + 1e-30)).item() for x, y in zip(gd, ga) if y.numel()),
             "repeat_bit_identical": all(torch.equal(x, y) for x, y in zip(gd, gd2))}
-    out = {"gaussians": args.points, "width": W, "height": H, "num_rendered": int(nr),
-           "det_scratch_bytes": int(_lib.lib().psb_rasterize_backward_det_bytes(args.points, int(nr))),
+    out = {"gaussians": P, "width": W, "height": H, "num_rendered": int(nr),
+           "det_scratch_bytes": int(_lib.lib().psb_rasterize_backward_det_bytes(P, int(nr))),
            "forward_ms": {k: _stats(v) for k, v in fwd_ms.items()}, "backward_ms": {k: _stats(v) for k, v in bwd_ms.items()},
            "backward_rounds_ms": bwd_ms, "gradients": diff}
     out["forward_backward_ms"] = {leg: out["forward_ms"]["depth" if leg.endswith("depth") else "colour"]["median"] +
@@ -122,8 +90,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--rounds", type=int, default=4)
     a = ap.parse_args()
-    dev = torch.device("cuda", 0)
-    out = {"device": torch.cuda.get_device_name(dev), "power_limit_w": power_limit_w(0), "calls": a.calls, "rounds": a.rounds,
+    dev = harness.device()
+    out = {"card": harness.card(), "calls": a.calls, "rounds": a.rounds,
            "unit": "ms per call (CUDA events); median and range over the rounds"}
     for config in a.configs.split(","):
         out[config] = run_config(config, a, dev)

@@ -10,37 +10,16 @@ import argparse
 import ctypes as C
 import json
 import math
-import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-if ROOT not in sys.path:
-    sys.path.insert(0, ROOT)
-import photo_slam_b200.synthetic as syn  # noqa: E402
-from photo_slam_b200 import trainer  # noqa: E402
+import harness
+import photo_slam_b200.synthetic as syn
+from photo_slam_b200 import trainer
 
 LRS = [0.00016, 0.0025, 0.0025 / 20, 0.05, 0.005, 0.001]
-BOX = ((-0.6, 0.6), (-0.45, 0.45), (1.0, 4.0))   # world box (camera 0 is the identity) the trainee lacks
-
-
-def _dev_cam(cam, dev):
-    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-    return dict(viewmatrix=T(cam["viewmatrix"]), projmatrix=T(cam["projmatrix"]), campos=T(cam["campos"]), tanfovx=float(cam["tanfovx"]),
-                tanfovy=float(cam["tanfovy"]), W=int(cam["W"]), H=int(cam["H"]))
-
-
-def _time(fn, reps):
-    ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(reps)]
-    for a, b in ev:
-        a.record()
-        fn()
-        b.record()
-    torch.cuda.synchronize()
-    return float(np.median([a.elapsed_time(b) for a, b in ev]))
+BOX = ((-0.6, 0.6), (-0.45, 0.45), (1.0, 4.0))   # world box (the scene lies in front of the identity view) the trainee lacks
 
 
 def sensor_depth(tr, cam):
@@ -55,17 +34,12 @@ def sensor_depth(tr, cam):
 def payoff(dev, seeded, steps=300, stride=2):
     """The scene of tests/test_quality_gpu.py, a trainee without the rows in BOX, optionally seeded once per keyframe, `steps` fused steps.
     -> dict(psnr_start, psnr (mean over the 6 keyframes after the steps), rows_removed, seeded (rows added), points)."""
-    P, W, H, fx = 200_000, 640, 480, 520.9
-    cam0 = syn.make_camera(W, H, fx, fx)
-    gt_scene = syn.make_scene(P, cam0, seed=21, scale_px=3.0)
-    views = []
-    for k in range(6):
-        R, t = syn.random_pose(np.random.default_rng(50 + k), max_angle=0.06, max_trans=0.12)
-        views.append(_dev_cam(syn.make_camera(W, H, fx, fx, R, t), dev))
+    gt_scene, cams = syn.quality_scene()
+    views = [syn.device_camera(cam, dev) for cam in cams]
     gt_tr = trainer.GaussianTrainer(trainer.GaussianModel.from_numpy(gt_scene, dev))
     frames = [sensor_depth(gt_tr, c)[:2] for c in views]
     x = gt_scene["xyz"]
-    inside = np.ones(P, dtype=bool)
+    inside = np.ones(len(x), dtype=bool)
     for a, (lo, hi) in enumerate(BOX):
         inside &= (x[:, a] > lo) & (x[:, a] < hi)
     start = {k: v[~inside].copy() for k, v in gt_scene.items()}
@@ -93,13 +67,12 @@ def payoff(dev, seeded, steps=300, stride=2):
     return dict(psnr_start=p_start, psnr=psnr(), rows_removed=int(inside.sum()), seeded=int(added), points=model.num_points())
 
 
-def cost(dev, reps, P=500_000):
-    W, H, fx, fy = syn.CAMERAS["replica"]
-    cam = syn.make_camera(W, H, fx, fy)
-    m = trainer.GaussianModel.from_numpy(syn.make_scene(P, cam, seed=0), dev)
+def cost(dev, reps):
+    sc, _, _, c, _ = harness.workload("B", dev)
+    P, W, H = len(sc["xyz"]), c["W"], c["H"]
+    m = trainer.GaussianModel.from_numpy(sc, dev)
     m.trainingSetup(trainer.GaussianOptimizationParams())
     tr = trainer.GaussianTrainer(m)
-    c = _dev_cam(cam, dev)
     A = torch.empty((H, W), device=dev)
     D = torch.empty((H, W), device=dev)
     img = tr.render(c, out_depth=D, out_alpha=A).clamp(0, 1).clone()
@@ -125,12 +98,10 @@ def cost(dev, reps, P=500_000):
                                                stream), "psb_seed_plan")
             trainer._lib.check(L.psb_seed_apply(P, C.byref(src), C.byref(dst), n, C.byref(cc), img.data_ptr(), G.data_ptr(), C.byref(cfg),
                                                 ws.data_ptr(), 0, stream), "psb_seed_apply")
-        _time(call, 3)
-        out[f"stride{stride}"] = dict(ms=_time(call, reps), rows_added=n, holes=counts[1], in_front=counts[2])
+        out[f"stride{stride}"] = dict(ms=harness.cuda_ms(call, reps, warmup=3), rows_added=n, holes=counts[1], in_front=counts[2])
         del d
     step = lambda: tr.trainForOneIteration(c, img)
-    _time(step, 5)
-    out["fused_step_ms"] = _time(step, reps)
+    out["fused_step_ms"] = harness.cuda_ms(step, reps, warmup=5)
     out["P"] = P
     out["size"] = [W, H]
     return out
@@ -141,11 +112,8 @@ def main():
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--steps", type=int, default=300)
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("seed_bench needs a CUDA device")
-    dev = torch.device("cuda:0")
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    res = dict(gpu=q, cost=cost(dev, a.reps))
+    dev = harness.device()
+    res = dict(card=harness.card(), cost=cost(dev, a.reps))
     base, seeded = payoff(dev, False, a.steps), payoff(dev, True, a.steps)
     res["payoff"] = dict(steps=a.steps, unseeded=base, seeded=seeded, gain_db=seeded["psnr"] - base["psnr"])
     print(json.dumps(res))
