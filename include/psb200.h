@@ -375,6 +375,63 @@ int psb_trainer_backward_exposure(psb_trainer* t, int P, int M, const psb_model*
                                   const psb_exposure* exposure, float* exposure_grad, void* stream);
 /* psb_trainer_result with out4 = {loss, l1, ssim, depth_l1} (depth_l1 = 0 when the last step had no depth term). */
 int psb_trainer_result_depth(psb_trainer* t, float* out4, int* num_rendered, void* stream);
+/* ------------------------------------------------------------------------------------------------
+ * Rendered surface normals. Depth pins where a surface is, not which way it faces; the normal plane and its RGB-D term (DN-Splatter,
+ * GS-SLAM) supervise the orientation of each Gaussian's flattest axis.
+ * Per-Gaussian normal: q = the normalised (w, x, y, z) quaternion and R(q) the rotation the covariance is built from; k = argmin_c
+ *   scaling[c] (the raw log-scale; ties go to the lowest index); r = column k of R(q), the world-space shortest axis; V = the upper-left
+ *   3x3 of the view matrix, V[r][c] = viewmatrix[4 c + r]; m = V r and t = the view-space mean, formed as the forward forms it;
+ *   n_i = m if m . t <= 0, else -m (the normal faces the camera). The 3D filter widens Sigma by f^2 I, which keeps its eigenvectors and so
+ *   k; anti-aliasing changes only alpha: n_i is the same in every mode.
+ * Normal plane: N_c(p) = sum_i n_ic alpha_i T_i, c = 0, 1, 2, with alpha and T exactly those of the colour (same blend order, culls and
+ *   termination) and no background term. N is un-normalised, like D: N / |N| is the pixel's surface normal, in view space. Rendering it
+ *   leaves colour, depth, A, radii and the pass's scratch bit-identical.
+ * Backward: the three channels join the tile backward like z does for depth (alpha_i T_i dL/dN_c -> dL/dn_ic, and n_i . dL/dN joins
+ *   dL/dalpha, so the term reaches opacity, conic, mean2D and the densification statistics); dL/dr = +-V^T dL/dn, with the sign of the
+ *   flip, then through dR/dq and the quaternion normalisation into the rotation gradient. k and the flip are piecewise constant: no
+ *   gradient to the scales or the mean.
+ * Sensor normals (psb_depth_normals): fx = W / (2 tan_fovx), fy = H / (2 tan_fovy), X(u,v) = ((u + 0.5 - W/2) z / fx, (v + 0.5 - H/2) z / fy,
+ *   z) with z = depth(u,v) (the seeding rule's back-projection); c = (X(u+1,v) - X(u-1,v)) x (X(u,v+1) - X(u,v-1)); n = c / |c|, flipped
+ *   so that n . X(u,v) < 0. (0,0,0) on the image border, where any of the five depths is not finite or <= 0, where some neighbour has
+ *   |z_nb - z| > max_rel_jump z (a depth edge) and where |c| = 0. Output: view-space normals [3,H,W], the frame N is rendered in. No
+ *   atomics: bit-identical from run to run.
+ * Normal term of the built-in loss: valid(p) = G_n(p) != (0,0,0) and, with a mask, mask[0,p] != 0 (the depth loss's convention);
+ *   normal_l1 = sum_valid sum_c |N_c - G_c| / max(N_valid, 1); L += lambda_normal normal_l1; dL/dN_c = lambda_normal sign(N_c - G_c) /
+ *   max(N_valid, 1) on valid pixels (sign(0) = 0). N_valid is counted on the device (no host synchronisation); in deterministic mode the
+ *   sums are reduced in a fixed order. Comparing the un-normalised N with a unit G also pushes A towards 1 where normals are measured:
+ *   deliberate, as the depth term does with D. Exposure compensation acts on colour only and does not touch this term.
+ * The data-parallel calls, the _begin / _slab halves and the rasterizer operator take no normal term.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct psb_normal {
+	const float* gt_normal;  /* [3,H,W] device, view-space unit normals, (0,0,0) = no measurement (psb_depth_normals); NULL = no normal term */
+	float lambda_normal;     /* finite, >= 0; > 0 exactly when gt_normal is given */
+	float* out_normal;       /* [3,H,W] device or NULL: the normal plane N */
+} psb_normal;
+/* psb_trainer_forward plus out_normal [3,H,W] (device) = N; NULL is exactly psb_trainer_forward. The other outputs are bit-identical to
+ * psb_trainer_forward's. A pass with the plane may be followed by psb_trainer_backward_pixels_normal with a dL_dnormal. */
+int psb_trainer_forward_normal(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                               const float* background, int sh_degree, float* out_color, int* radii, float* out_depth, float* out_alpha,
+                               float* out_normal, unsigned* pass, void* stream);
+/* psb_trainer_backward_pixels plus dL_dnormal [3,H,W] (device), the gradient w.r.t. N; NULL is exactly psb_trainer_backward_pixels.
+ * PSB_ERR_ARG, before any CUDA call, for everything psb_trainer_backward_pixels rejects and for a dL_dnormal after a pass that rendered
+ * no normal plane. */
+int psb_trainer_backward_pixels_normal(psb_trainer* t, unsigned pass, int P, int M, const psb_model* model, const psb_camera* camera,
+                                       const float* background, const psb_pixel_grads* pixel_grads, const float* dL_dnormal,
+                                       const psb_step* step, float* const* grads, void* stream);
+/* psb_trainer_step_exposure plus the normal term (normal == NULL: exactly psb_trainer_step_exposure). PSB_ERR_ARG, before any CUDA call,
+ * for everything psb_trainer_step_exposure rejects, a negative or non-finite lambda_normal, and gt_normal without lambda_normal > 0 (or
+ * the reverse). An out_normal alone renders the plane and trains as without it. A step that overflows the binning arena is a no-op:
+ * repeating it applies the term once. */
+int psb_trainer_step_normal(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                            const float* background, const float* gt_image, const float* mask, const psb_step* step,
+                            float* out_color, int* radii, const psb_depth* depth, const psb_exposure* exposure, const psb_normal* normal,
+                            void* stream);
+/* psb_trainer_result with out5 = {loss, l1, ssim, depth_l1, normal_l1} (0 for a term the last step did not have). */
+int psb_trainer_result_normal(psb_trainer* t, float* out5, int* num_rendered, void* stream);
+/* Sensor normals of a depth image [H,W] (metres, <= 0 or not finite = no measurement) seen by `camera` (width, height, tan_fovx and
+ * tan_fovy are read) -> out_normal [3,H,W] device. PSB_ERR_ARG, before any CUDA call, for a NULL camera, depth or output, a size that is
+ * not positive, a tan_fov that is not finite and positive, and a max_rel_jump that is not finite and positive. Asynchronous. */
+int psb_depth_normals(const psb_camera* camera, const float* depth, float max_rel_jump, float* out_normal, void* stream);
 
 /* model->adam_live[i] = 1 if any of the 118 moments of row i is non-zero, else 0: one pass over the moments. Restores the
  * psb_model.adam_live contract after moments were written by anything but psb_trainer_step. Asynchronous on `stream`. */

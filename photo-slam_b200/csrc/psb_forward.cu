@@ -494,6 +494,23 @@ __global__ void __launch_bounds__(256) tile_ranges_kernel(const uint32_t* __rest
 	}
 }
 
+// The normal pass's n_i (normal_axis) of every visible row, from the raw trainer parameters, behind the preprocess: a kernel of its own,
+// so the preprocess variants keep their code. The quaternion is normalised and the view-space mean formed exactly as the preprocess does.
+__global__ void __launch_bounds__(256) normals_kernel(int P, const float* __restrict__ xyz, const float* __restrict__ scaling,
+                                                      const float4* __restrict__ rotation, const float* __restrict__ view,
+                                                      const uint4* __restrict__ tile_info, float4* __restrict__ normals)
+{
+	const int idx = blockIdx.x * 256 + threadIdx.x;
+	if (idx >= P || tile_info[idx].z == 0) return;
+	const float3 p = make_float3(xyz[3 * idx], xyz[3 * idx + 1], xyz[3 * idx + 2]);
+	const float3 sraw = make_float3(scaling[3 * idx], scaling[3 * idx + 1], scaling[3 * idx + 2]);
+	float4 q = rotation[idx];
+	const float n = fmaxf(sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w), 1e-12f);
+	q = make_float4(q.x / n, q.y / n, q.z / n, q.w / n);
+	const NormalAxis a = normal_axis(q, sraw, xform4x3(p, view), view);
+	normals[idx] = make_float4(a.n.x, a.n.y, a.n.z, 0.f);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Host orchestration
 // ------------------------------------------------------------------------------------------------
@@ -510,6 +527,15 @@ int launch_preprocess(const GaussIn& in, const Camera& cam, int* radii_out, cons
 	else if (aa) preprocess_fwd_kernel<false, true><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tt, nullptr);
 	else if (raw) preprocess_fwd_kernel<true><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tt, nullptr);
 	else preprocess_fwd_kernel<false><<<grid, PRE_TB, 0, stream>>>(in, cam, radii_out, geom, tt, nullptr);
+	PSB_LAUNCH_OK();
+	return 0;
+}
+
+int launch_normals(int P, const float* xyz, const float* scaling, const float* rotation, const Camera& cam, const uint4* tile_info, float4* normals,
+                   cudaStream_t stream)
+{
+	if (P == 0) return 0;
+	normals_kernel<<<cdiv(P, 256), 256, 0, stream>>>(P, xyz, scaling, reinterpret_cast<const float4*>(rotation), cam.view, tile_info, normals);
 	PSB_LAUNCH_OK();
 	return 0;
 }

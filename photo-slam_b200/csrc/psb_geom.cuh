@@ -96,6 +96,47 @@ __device__ __forceinline__ float filter3d_widen(float3& s, float f)
 	return sqrtf(r);
 }
 
+// Rendered normals (include/psb200.h): the camera-facing shortest axis n of a Gaussian in view space. q = the normalised (w, x, y, z)
+// quaternion the covariance is built from, sraw = the raw log-scales, t = the view-space mean (xform4x3 of the mean, as the forward forms
+// it), vm the view matrix. k = argmin_c sraw[c] (ties: lowest index), r = column k of R(q) (the world-space axis the covariance scales by
+// exp(sraw[k])), m = V r; n = m if m . t <= 0, else -m (sign = +1 / -1). The backward forms the same k and sign from the same inputs.
+struct NormalAxis {
+	float3 n;
+	int k;
+	float sign;
+};
+__device__ __forceinline__ NormalAxis normal_axis(const float4 q, const float3 sraw, const float3 t, const float* vm)
+{
+	const float w = q.x, x = q.y, y = q.z, z = q.w;
+	int k = 0;
+	float smin = sraw.x;
+	if (sraw.y < smin) { k = 1; smin = sraw.y; }
+	if (sraw.z < smin) k = 2;
+	float3 r;
+	if (k == 0) r = make_float3(1.f - 2.f * (y * y + z * z), 2.f * (x * y + w * z), 2.f * (x * z - w * y));
+	else if (k == 1) r = make_float3(2.f * (x * y - w * z), 1.f - 2.f * (x * x + z * z), 2.f * (y * z + w * x));
+	else r = make_float3(2.f * (x * z + w * y), 2.f * (y * z - w * x), 1.f - 2.f * (x * x + y * y));
+	const float3 m = make_float3(vm[0] * r.x + vm[4] * r.y + vm[8] * r.z, vm[1] * r.x + vm[5] * r.y + vm[9] * r.z,
+	                             vm[2] * r.x + vm[6] * r.y + vm[10] * r.z);
+	const float sign = (m.x * t.x + m.y * t.y + m.z * t.z <= 0.f) ? 1.f : -1.f;
+	return {make_float3(sign * m.x, sign * m.y, sign * m.z), k, sign};
+}
+
+// dL/dq (of the normalised quaternion) of n = sign V r_k(q), given dL/dn: dL/dr = sign V^T dL/dn, then the derivative of column k of R(q).
+// k and the sign are piecewise constant: they pass no gradient to the scales or the mean.
+__device__ __forceinline__ float4 normal_axis_backward(const float4 q, const NormalAxis& a, const float3 dL_dn, const float* vm)
+{
+	const float w = q.x, x = q.y, y = q.z, z = q.w;
+	const float g0 = a.sign * (vm[0] * dL_dn.x + vm[1] * dL_dn.y + vm[2] * dL_dn.z);
+	const float g1 = a.sign * (vm[4] * dL_dn.x + vm[5] * dL_dn.y + vm[6] * dL_dn.z);
+	const float g2 = a.sign * (vm[8] * dL_dn.x + vm[9] * dL_dn.y + vm[10] * dL_dn.z);
+	if (a.k == 0)
+		return make_float4(2.f * (z * g1 - y * g2), 2.f * (y * g1 + z * g2), 2.f * (x * g1 - w * g2) - 4.f * y * g0, 2.f * (w * g1 + x * g2) - 4.f * z * g0);
+	if (a.k == 1)
+		return make_float4(2.f * (x * g2 - z * g0), 2.f * (y * g0 + w * g2) - 4.f * x * g1, 2.f * (x * g0 + z * g2), 2.f * (y * g2 - w * g0) - 4.f * z * g1);
+	return make_float4(2.f * (y * g0 - x * g1), 2.f * (z * g0 - w * g1) - 4.f * x * g2, 2.f * (w * g0 + z * g1) - 4.f * y * g2, 2.f * (x * g0 + y * g1));
+}
+
 // SH (degree <= 3) -> RGB for one Gaussian, all three channels; sh points at this Gaussian's
 // [M][3] coefficient row (forward.cu:20-71). Returns colour after +0.5 and clamp at 0; `clamp_bits`
 // bit c set when channel c was clamped.

@@ -108,13 +108,21 @@ int launch_render_forward(const Camera& cam, const uint2* ranges, const uint32_t
                           float* out_color, float* final_T, uint32_t* n_contrib, cudaStream_t stream,
                           float* out_depth = nullptr /* [H,W]: also render the expected depth (depth variant of the kernel) */,
                           float* out_alpha = nullptr /* [H,W]: also write the accumulated opacity 1 - final_T (opacity variant) */,
-                          const ScoreSink* score = nullptr /* also add the contribution scores (score variant; no depth or opacity) */);
+                          const ScoreSink* score = nullptr /* also add the contribution scores (score variant; no depth or opacity) */,
+                          const float4* normals = nullptr /* [P] n_i of the pass (launch_normals); with out_normal only */,
+                          float* out_normal = nullptr /* [3,H,W]: also render the normal plane (normal variant; no score) */);
+// n_i of include/psb200.h (the camera-facing shortest axis in view space) of every visible row of the pass -> normals [P]; raw trainer
+// parameters (xyz, scaling, rotation), after launch_preprocess (tile_info says which rows are visible)
+int launch_normals(int P, const float* xyz, const float* scaling, const float* rotation, const Camera& cam, const uint4* tile_info, float4* normals,
+                   cudaStream_t stream);
 // dL_ddepth [H,W]: depth variant, dL/dz of every Gaussian lands in slot 11 of its packed sink row, or at sink.z (unpacked sink;
 // refused without either destination). det != null: the deterministic variant — slot stores, then the ordered gather, which WRITES the
 // sink rows (packed: gather_slots_kernel; unpacked: gather_slots_unpacked_kernel, dL/dz at sink.z with dL_ddepth). dL_dalpha [H,W]: opacity variant, the gradient of the accumulated opacity 1 - final_T joins dL/dalpha of every splat
 int launch_render_backward(const Camera& cam, const uint2* ranges, const uint32_t* point_list, const GaussRec* rec, const float* bg,
                            const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, const GradSink& sink,
-                           cudaStream_t stream, const float* dL_ddepth = nullptr, const DetSlots* det = nullptr, const float* dL_dalpha = nullptr);
+                           cudaStream_t stream, const float* dL_ddepth = nullptr, const DetSlots* det = nullptr, const float* dL_dalpha = nullptr,
+                           const float4* normals = nullptr /* [P] n_i of the forward pass; with dL_dnormal only */,
+                           const float* dL_dnormal = nullptr /* [3,H,W]: normal variant, packed 16-float sink rows, 64-byte deterministic slots */);
 // dL_dz [P] (non-null: depth variant): dL/dmean3D += dL/dz (V[2], V[6], V[10]) for every visible Gaussian
 // aa_dL_dopacity [P] (non-null: AA variant, after an anti-aliased forward): holds dL/do' on entry, dL/do on return
 int launch_preprocess_backward(const GaussIn& in, const Camera& cam, const GeomState& geom, const float* dL_dmean2D, int mean2D_stride,

@@ -324,7 +324,61 @@ __global__ void __launch_bounds__(256) depth_grad_scale_kernel(int n, float lamb
 	for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) dL_dD[i] *= scale;
 }
 
+// Normal L1, pass 1 (as depth_loss_kernel, over the three planes of N and G): a pixel is valid when G(p) != (0, 0, 0) and, with a mask,
+// mask[0, p] != 0; per valid pixel sum_c |N_c - G_c| and sign(N_c - G_c) (-> dL_dN, scaled by pass 2).
+template <bool DET>
+__global__ void __launch_bounds__(256) normal_loss_kernel(int n, const float* __restrict__ N, const float* __restrict__ G, const float* __restrict__ mask,
+                                                          float* __restrict__ dL_dN, double* __restrict__ sums)
+{
+	__shared__ float s_red[8];
+	float acc = 0.f, cnt = 0.f;
+	for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) {
+		const float g0 = G[i], g1 = G[n + i], g2 = G[2 * n + i];
+		const bool valid = (g0 != 0.f || g1 != 0.f || g2 != 0.f) && (!mask || mask[i] != 0.f);
+		float sg[3] = {0.f, 0.f, 0.f};
+		if (valid) {
+			const float d[3] = {N[i] - g0, N[n + i] - g1, N[2 * n + i] - g2};
+#pragma unroll
+			for (int c = 0; c < 3; c++) {
+				acc += fabsf(d[c]);
+				sg[c] = (d[c] > 0.f) ? 1.f : ((d[c] < 0.f) ? -1.f : 0.f);
+			}
+			cnt += 1.f;
+		}
+#pragma unroll
+		for (int c = 0; c < 3; c++) dL_dN[c * n + i] = sg[c];
+	}
+	const float tacc = block_sum_256(acc, s_red);
+	const float tcnt = block_sum_256(cnt, s_red);
+	block_sums_out<DET>(tacc, tcnt, sums);
+}
+
+// Normal L1, pass 2: dL_dN [3, n] *= lambda / max(N_valid, 1), N_valid read on the device.
+__global__ void __launch_bounds__(256) normal_grad_scale_kernel(int n, float lambda, const double* __restrict__ sums, float* __restrict__ dL_dN)
+{
+	const float scale = lambda / (float)fmax(sums[1], 1.0);
+	for (int i = blockIdx.x * 256 + threadIdx.x; i < 3 * n; i += gridDim.x * 256) dL_dN[i] *= scale;
+}
+
 }  // namespace
+
+int launch_normal_loss(int H, int W, const float* normal, const float* gt_normal, const float* mask, float lambda_normal, double* sums, float* dL_dN,
+                       cudaStream_t stream, double* partials)
+{
+	const int n = H * W;
+	const int grid = depth_loss_blocks(H, W);
+	const bool det = partials != nullptr;
+	if (!det) PSB_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), stream));
+	(det ? normal_loss_kernel<true> : normal_loss_kernel<false>)<<<grid, 256, 0, stream>>>(n, normal, gt_normal, mask, dL_dN, det ? partials : sums);
+	PSB_LAUNCH_OK();
+	if (det) {
+		reduce_partials_kernel<<<1, 256, 0, stream>>>(grid, partials, sums);
+		PSB_LAUNCH_OK();
+	}
+	normal_grad_scale_kernel<<<grid, 256, 0, stream>>>(n, lambda_normal, sums, dL_dN);
+	PSB_LAUNCH_OK();
+	return 0;
+}
 
 int launch_depth_loss(int H, int W, const float* depth, const float* gt_depth, const float* mask, float lambda_depth, double* sums, float* dL_dD,
                       cudaStream_t stream, double* partials)

@@ -52,6 +52,9 @@ constexpr int MODE_REG = 32;       // OR'd into MODE_GRADS / MODE_ADAM / MODE_AD
 constexpr int MODE_F3D = 64;       // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE (each optionally | MODE_DEPTH | MODE_AA | MODE_REG), not MODE_PUSH:
                                    // the forward applied the 3D smoothing filter f3d[idx] (preprocess_fwd_kernel<true, AA, true>): the covariance is
                                    // rebuilt from s' = sqrt(s^2 + f^2), and the filter's opacity factor c joins the scale and opacity gradients
+constexpr int MODE_NORMAL = 128;   // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE (each optionally | MODE_DEPTH | MODE_AA | MODE_REG | MODE_F3D),
+                                   // not MODE_PUSH: the sink rows are 16 floats (render_bwd_normal_kernel) and slots 12..14 hold dL/dn; the
+                                   // rotation gradient takes dL/dq of n = sign V r_k(q) (normal_axis_backward)
 
 // torch::optim::Adam single-tensor update (LibTorch adam.cpp): exp_avg.mul_(b1).add_(g, 1-b1);
 // exp_avg_sq.mul_(b2).addcmul_(g, g, 1-b2); denom = exp_avg_sq.sqrt()/sqrt(bc2) + eps; p.addcdiv_(exp_avg, denom, -lr/bc1).
@@ -172,6 +175,8 @@ __device__ __forceinline__ void adam_small(SmallRow& p, SmallRow& m, SmallRow& v
 // MODE_DEPTH: dL/dxyz += dL/dz (V[2], V[6], V[10]). A row whose only non-zero sum is slot 11 has a gradient (its parameters are loaded and
 // updated, its live byte set) but no SH gradient: the view-direction term depends on dL/dRGB only, so its f_rest row is not staged.
 //
+// MODE_NORMAL: a row whose only non-zero sums are slots 12..14 has a gradient (the rotation's) but no SH gradient, as with MODE_DEPTH.
+//
 // MODE_REG: `reg` is read by these instantiations only. The regularisers touch exactly the rows that have a gradient anyway (`reached`), so
 // the dirty / live decisions and the memory traffic are those of the variant without it.
 //
@@ -189,8 +194,11 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 	constexpr bool AA = (MODE & MODE_AA) != 0;
 	constexpr bool REG = (MODE & MODE_REG) != 0;
 	constexpr bool F3D = (MODE & MODE_F3D) != 0;
-	constexpr int BASE = MODE & ~(MODE_DEPTH | MODE_AA | MODE_REG | MODE_F3D);
+	constexpr bool NORMAL = (MODE & MODE_NORMAL) != 0;
+	constexpr int BASE = MODE & ~(MODE_DEPTH | MODE_AA | MODE_REG | MODE_F3D | MODE_NORMAL);
+	constexpr int SR = NORMAL ? 4 : 3;  // float4 lanes per sink row
 	static_assert(!F3D || BASE != MODE_PUSH, "no 3D filter on the NVLink step");
+	static_assert(!NORMAL || BASE != MODE_PUSH, "no normal term on the NVLink step");
 	constexpr bool LIVE = BASE == MODE_ADAM_LIVE;
 	constexpr bool ADAM = BASE == MODE_ADAM || LIVE;
 	__shared__ __align__(128) float s_p[TB * REST];  // f_rest parameter rows of this block (TMA destination; LIVE: compacted per warp)
@@ -244,14 +252,16 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 	bool staged = false;    // non-zero screen-space sums (LIVE: the f_rest row is staged)
 	bool reached = false;   // staged, or (DEPTH) a non-zero dL/dz: the sink row was added to and has a gradient
 	int rest_slot = tid;    // this row's f_rest row in s_p
-	float4 s0 = make_float4(0, 0, 0, 0), s1 = s0, s2 = s0;
+	float4 s0 = make_float4(0, 0, 0, 0), s1 = s0, s2 = s0, s3 = s0;
 	uint32_t meta = 0;
 	auto load_moments = [&]() { load_small(m, t.m, idx); load_small(v, t.v, idx); };
 	// rows nothing was added to (culled or hidden Gaussians) are zero since the last step: only the others are re-zeroed for the next one
 	auto take_sink = [&]() {
 		staged = s0.x != 0.f || s0.y != 0.f || s0.w != 0.f || s1.x != 0.f || s1.z != 0.f || s1.w != 0.f || s2.x != 0.f || s2.y != 0.f || s2.z != 0.f;
 		reached = staged || (DEPTH && s2.w != 0.f);
-		if (reached) { const float4 z = make_float4(0, 0, 0, 0); sink[3 * idx] = z; sink[3 * idx + 1] = z; sink[3 * idx + 2] = z; }
+		if constexpr (NORMAL) reached = reached || s3.x != 0.f || s3.y != 0.f || s3.z != 0.f;
+		if (reached) { const float4 z = make_float4(0, 0, 0, 0); sink[SR * idx] = z; sink[SR * idx + 1] = z; sink[SR * idx + 2] = z; }
+		if constexpr (NORMAL) if (reached) sink[SR * idx + 3] = make_float4(0, 0, 0, 0);
 	};
 	if (LIVE) {
 		if (valid) {
@@ -260,7 +270,8 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 			if (was_live) load_small(p, t.p, idx);  // (the moments are loaded after the backward: fewer registers held across it)
 			if (visible) {
 				if (st.enabled) { st_rad = st.max_radii2D[idx]; st_acc = st.xyz_gradient_accum[idx]; st_den = st.denom[idx]; }
-				s0 = sink[3 * idx]; s1 = sink[3 * idx + 1]; s2 = sink[3 * idx + 2];
+				s0 = sink[SR * idx]; s1 = sink[SR * idx + 1]; s2 = sink[SR * idx + 2];
+				if constexpr (NORMAL) s3 = sink[SR * idx + 3];
 				meta = __float_as_uint(geom.rec[idx].q2.w);
 				take_sink();  // (only visible rows were added to)
 				if (reached && !was_live) load_small(p, t.p, idx);  // first gradient of this row: its moments are zero by contract, not read
@@ -290,7 +301,8 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 			if (ADAM) load_moments();
 			if (st.enabled) { st_rad = st.max_radii2D[idx]; st_acc = st.xyz_gradient_accum[idx]; st_den = st.denom[idx]; }
 			tt = geom.tile_info[idx].z;
-			s0 = sink[3 * idx]; s1 = sink[3 * idx + 1]; s2 = sink[3 * idx + 2];
+			s0 = sink[SR * idx]; s1 = sink[SR * idx + 1]; s2 = sink[SR * idx + 2];
+			if constexpr (NORMAL) s3 = sink[SR * idx + 3];
 			meta = __float_as_uint(geom.rec[idx].q2.w);
 			load_small(p, t.p, idx);
 			visible = tt != 0 && !overflow;
@@ -328,6 +340,11 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 			float3 dL_dscale;
 			float4 dL_drot;
 			cov3d_backward(sf, 1.0f, q, dL_dcov, dL_dscale, dL_drot);
+			if constexpr (NORMAL) {  // n_i as the forward formed it (normals_kernel): same q, raw scales and view-space mean
+				const NormalAxis ax = normal_axis(q, sraw, xform4x3(mean, cam.view), cam.view);
+				const float4 dq = normal_axis_backward(q, ax, make_float3(s3.x, s3.y, s3.z), cam.view);
+				dL_drot.x += dq.x; dL_drot.y += dq.y; dL_drot.z += dq.z; dL_drot.w += dq.w;
+			}
 			if (F3D && f2 > 0.f) {  // (f = 0: s' = s and c = 1, nothing to add)
 				const float k = sig * f3d_c * (AA ? aa_h * dL_dopacity : dL_dopacity) * f2;   // o c dL/d(o c) f^2
 				dL_dscale.x = dL_dscale.x * (s.x / sf.x) + (k != 0.f ? k / (s.x * sf.x * sf.x) : 0.f);
@@ -716,7 +733,7 @@ void run_gaussian_backward(int first, int P, cudaStream_t stream, Args... args)
 }
 
 // Gaussians [first, P) in mode `mode` (MODE_GRADS, MODE_ADAM, MODE_ADAM_LIVE or MODE_PUSH, each optionally | MODE_DEPTH and | MODE_AA; all but
-// MODE_PUSH optionally | MODE_REG and | MODE_F3D)
+// MODE_PUSH optionally | MODE_REG, | MODE_F3D and | MODE_NORMAL)
 int launch_gaussian_backward(int mode, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink,
                              const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
                              float* seeds, const DpPush& dp, unsigned char* adam_live, cudaStream_t stream, const RegCoef& reg, const float* f3d)
@@ -728,7 +745,12 @@ int launch_gaussian_backward(int mode, int first, int P, const TrainTensors& t, 
 	case M: run_gaussian_backward<M>(first, P, stream, t, cam, geom, sink4, h, grads, st, counters, capacity, seeds4, dp, adam_live, reg, f3d); break
 #define PSB_BACKWARD_CASE_F3D(M) PSB_BACKWARD_CASE(M); PSB_BACKWARD_CASE(M | MODE_F3D)
 #define PSB_BACKWARD_CASE_REG(M) PSB_BACKWARD_CASE_F3D(M); PSB_BACKWARD_CASE_F3D(M | MODE_REG)
+#define PSB_BACKWARD_CASE_NRM(M) PSB_BACKWARD_CASE_REG(M | MODE_NORMAL); PSB_BACKWARD_CASE_REG(M | MODE_NORMAL | MODE_DEPTH); \
+	PSB_BACKWARD_CASE_REG(M | MODE_NORMAL | MODE_AA); PSB_BACKWARD_CASE_REG(M | MODE_NORMAL | MODE_DEPTH | MODE_AA)
 	switch (mode) {
+		PSB_BACKWARD_CASE_NRM(MODE_GRADS);
+		PSB_BACKWARD_CASE_NRM(MODE_ADAM);
+		PSB_BACKWARD_CASE_NRM(MODE_ADAM_LIVE);
 		PSB_BACKWARD_CASE_REG(MODE_GRADS);
 		PSB_BACKWARD_CASE_REG(MODE_ADAM);
 		PSB_BACKWARD_CASE_REG(MODE_ADAM_LIVE);
@@ -747,6 +769,7 @@ int launch_gaussian_backward(int mode, int first, int P, const TrainTensors& t, 
 		PSB_BACKWARD_CASE(MODE_PUSH | MODE_DEPTH | MODE_AA);
 		default: set_error_msg("launch_gaussian_backward: unknown mode"); return -1;
 	}
+#undef PSB_BACKWARD_CASE_NRM
 #undef PSB_BACKWARD_CASE_REG
 #undef PSB_BACKWARD_CASE_F3D
 #undef PSB_BACKWARD_CASE
@@ -780,7 +803,7 @@ int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, co
 	memset(&nodp, 0, sizeof(nodp));
 	unsigned char* live = adam ? adam_live : nullptr;
 	const int variant = (live ? MODE_ADAM_LIVE : adam ? MODE_ADAM : MODE_GRADS) | (mode.depth ? MODE_DEPTH : 0) | (mode.aa ? MODE_AA : 0) |
-	                    (reg.opacity != 0.f || reg.scale != 0.f ? MODE_REG : 0) | (mode.f3d ? MODE_F3D : 0);
+	                    (reg.opacity != 0.f || reg.scale != 0.f ? MODE_REG : 0) | (mode.f3d ? MODE_F3D : 0) | (mode.normal ? MODE_NORMAL : 0);
 	int rc;
 	if ((rc = launch_gaussian_backward(variant, first, P, t, cam, geom, sink, h, grads, st, counters, capacity, seeds, nodp, live, stream, reg, mode.f3d)))
 		return rc;
@@ -809,6 +832,7 @@ int launch_push_backward(int P, const TrainTensors& t, const Camera& cam, const 
 	const GradSegments nog = {};
 	int rc;
 	if (mode.f3d) { set_error_msg("launch_push_backward: the 3D filter is not wired into the NVLink step"); return -1; }
+	if (mode.normal) { set_error_msg("launch_push_backward: the normal term is not wired into the NVLink step"); return -1; }
 	if ((rc = launch_gaussian_backward(MODE_PUSH | (mode.depth ? MODE_DEPTH : 0) | (mode.aa ? MODE_AA : 0), 0, P, t, cam, geom, sink, h, nog, st, counters, capacity, nullptr, dp,
 	                                   nullptr, stream, RegCoef{0.f, 0.f}, nullptr)))
 		return rc;

@@ -36,6 +36,8 @@ struct PassMode {
 	bool depth;  // the sink rows carry dL/dz in slot 11 (render_bwd_kernel<true, ...>)
 	float reg_opacity, reg_scale;  // psb_trainer_set_regularizers: lambda_opacity, lambda_scale (both 0: the variants without MODE_REG)
 	const float* f3d;              // psb_trainer_set_filter3d: the 3D smoothing filter [P] the pass applies, or null (the variants without it)
+	bool normals = false;          // the forward wrote n_i of its visible rows (launch_normals): a normal gradient may follow it
+	bool normal = false;           // the sink rows are 16 floats and slots 12..14 hold dL/dn (render_bwd_normal_kernel, MODE_NORMAL)
 };
 // lambda / P of the opacity and scale regularisers for the rows a per-Gaussian backward updates; both 0 = no regulariser
 struct RegCoef {
@@ -113,6 +115,11 @@ constexpr size_t kExposurePartials = 12 * (size_t)kNumSMs * 8;   // doubles: eno
 int launch_depth_loss(int H, int W, const float* depth, const float* gt_depth, const float* mask, float lambda_depth, double* sums, float* dL_dD,
                       cudaStream_t stream, double* partials);
 inline int depth_loss_blocks(int H, int W) { return min(cdiv(H * W, 256), kNumSMs * 8); }
+// Normal L1 (include/psb200.h, psb_normal) over the valid pixels (gt_normal != (0, 0, 0) and, with a mask, mask[0, p] != 0), normal and
+// gt_normal [3,H,W]: sums[0] = sum_valid sum_c |N_c - G_c|, sums[1] = N_valid (zeroed here); dL_dN [3,H,W] = lambda sign(N - G) / max(N_valid, 1)
+// on valid pixels, 0 elsewhere. The launch geometry of launch_depth_loss (same partials).
+int launch_normal_loss(int H, int W, const float* normal, const float* gt_normal, const float* mask, float lambda_normal, double* sums, float* dL_dN,
+                       cudaStream_t stream, double* partials);
 // launch_loss runs one block per 16 x 16 tile and channel
 inline size_t loss_partials_doubles(int H, int W)
 {

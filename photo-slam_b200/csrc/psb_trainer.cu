@@ -27,10 +27,12 @@ struct psb_trainer {
 	ArenaChunk<ImgState> img;    // W*H pixels: reallocated whenever W*H changes
 	ArenaChunk<BinState> bin;    // its count is the binning capacity (instances)
 	ArenaBuffer<float> image, dL_dpix, dmap;  // [3][H*W], [3][H*W], [9][H*W]
-	ArenaBuffer<float> sink, seeds;           // [P][12] (zeroed when allocated), [P][20]
+	ArenaBuffer<float> sink, seeds;           // [P][12] ([P][16] once a normal pass has run; zeroed when allocated), [P][20]
 	ArenaBuffer<float> depth_buf;  // depth loss: [2][H*W] = rendered depth (when the caller passes no out_depth) | dL/dD
-	ArenaBuffer<double> sums;      // device [4]: sum |I - G|, sum SSIM | depth loss: sum |D - G|, N_valid
-	CudaBuffer<double, 0, true> h_sums;     // pinned [4]
+	ArenaBuffer<float4> normals;   // normal passes: n_i of the visible rows [P], made by the first one
+	ArenaBuffer<float> normal_buf; // normal loss: [6][H*W] = rendered normal plane (when the caller passes no out_normal) | dL/dN
+	ArenaBuffer<double> sums;      // device [6]: sum |I - G|, sum SSIM | depth loss: sum |D - G|, N_valid | normal loss: sum |N - G|, N_valid
+	CudaBuffer<double, 0, true> h_sums;     // pinned [6]
 	CudaBuffer<uint32_t, 0, true> h_count;  // pinned [4]: instance count of the last call | sticky overflow record {count, first seq, largest count}
 	ArenaBuffer<uint32_t> ovf;     // device [4]: the sticky overflow record (tile_ranges_kernel), collected by psb_trainer_result
 	// what the scratch was last carved for: set when ensure() succeeds, cleared (P = -1) when it fails or the binning chunk is lost
@@ -56,14 +58,16 @@ struct psb_trainer {
 	cudaEvent_t readback = nullptr;
 	float last_lambda = 0.2f;
 	float last_lambda_depth = 0.f;
+	float last_lambda_normal = 0.f;
 	bool have_loss = false;
 	bool have_depth_loss = false;  // the last step had a depth term (h_sums[2..3] belong to it)
+	bool have_normal_loss = false; // the last step had a normal term (h_sums[4..5] belong to it)
 	// tight instance lists: only the tiles a splat can reach get an instance (see preprocess_fwd_kernel); PSB_TIGHT=0 keeps the
 	// reference's full rectangles (A/B measurements only — images and gradients are the same either way)
 	bool tight = !(getenv("PSB_TIGHT") && atoi(getenv("PSB_TIGHT")) == 0);
 	// deterministic mode (psb_trainer_set_deterministic): its own scratch, made only while the mode is on and grown with the binning
 	// capacity — the instance slots [capacity][12] floats (zeroed when allocated: every tag reads "not this pass"), the emission offsets
-	// [P] and the loss partials
+	// [P] and the loss partials (a normal pass's slots are [capacity][16] floats)
 	bool deterministic = false;
 	ArenaBuffer<float> det_slots;
 	ArenaBuffer<uint32_t> det_base;
@@ -97,7 +101,8 @@ namespace {
 // The scratch of a pass of P Gaussians over W x H pixels, each buffer's need stated once (CudaBuffer::grow drains the stream before it
 // frees a buffer the last call's kernels may still use). Any failure leaves t->carved cleared: no call reads this scratch until an
 // ensure() succeeds.
-int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_loss)
+// normal: a normal pass (n_i, 16-float sink rows and 64-byte deterministic slots); normal_loss: the built-in normal term's planes.
+int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_loss, bool normal = false, bool normal_loss = false)
 {
 	const size_t N = (size_t)W * H;
 	// the binning arena grows to P * 6 + 64 Ki instances when it is empty, or when it is smaller and the last pass was over another P
@@ -109,11 +114,13 @@ int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_
 	PSB_CUDA_OK(t->dL_dpix.grow(3 * N, Fit::at_least, false, stream));
 	PSB_CUDA_OK(t->dmap.grow(9 * N, Fit::at_least, false, stream));
 	if (depth_loss) PSB_CUDA_OK(t->depth_buf.grow(2 * N, Fit::at_least, false, stream));
-	PSB_CUDA_OK(t->sink.grow((size_t)P * 12, Fit::at_least, true, stream));
+	if (normal) PSB_CUDA_OK(t->normals.grow((size_t)P, Fit::at_least, false, stream));
+	if (normal_loss) PSB_CUDA_OK(t->normal_buf.grow(6 * N, Fit::at_least, false, stream));
+	PSB_CUDA_OK(t->sink.grow((size_t)P * (normal ? 16 : 12), Fit::at_least, true, stream));
 	PSB_CUDA_OK(t->seeds.grow((size_t)P * 20, Fit::at_least, false, stream));
 	if (!t->readback) {
-		PSB_CUDA_OK(t->sums.grow(4, Fit::at_least, false, stream));
-		PSB_CUDA_OK(t->h_sums.grow(4, Fit::at_least, false, stream));
+		PSB_CUDA_OK(t->sums.grow(6, Fit::at_least, false, stream));
+		PSB_CUDA_OK(t->h_sums.grow(6, Fit::at_least, false, stream));
 		PSB_CUDA_OK(t->h_count.grow(4, Fit::at_least, true, stream));
 		PSB_CUDA_OK(t->ovf.grow(4, Fit::at_least, false, stream));
 		const uint32_t init[4] = {0u, 0xFFFFFFFFu, 0u, 0u};
@@ -122,7 +129,7 @@ int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_
 	}
 	PSB_CUDA_OK(t->bin.grow(bin_need, Fit::at_least, false, stream));
 	if (t->deterministic) {
-		PSB_CUDA_OK(t->det_slots.grow(t->bin.count() * 12, Fit::at_least, true, stream));
+		PSB_CUDA_OK(t->det_slots.grow(t->bin.count() * (normal ? 16 : 12), Fit::at_least, true, stream));
 		PSB_CUDA_OK(t->det_base.grow((size_t)P, Fit::at_least, false, stream));
 		PSB_CUDA_OK(t->det_partials.grow(loss_partials_doubles(H, W), Fit::at_least, false, stream));
 	}
@@ -218,6 +225,21 @@ int check_depth(const psb_depth* d, const char* fn)
 	return 0;
 }
 
+// NULL: no normal term. Otherwise lambda_normal finite and >= 0, and a target exactly when lambda_normal > 0.
+int check_normal(const psb_normal* n, const char* fn)
+{
+	if (!n) return 0;
+	if (!std::isfinite(n->lambda_normal) || n->lambda_normal < 0.f) {
+		set_error_msg(std::string(fn).append(": lambda_normal must be finite and >= 0").c_str());
+		return PSB_ERR_ARG;
+	}
+	if ((n->gt_normal != nullptr) != (n->lambda_normal > 0.f)) {
+		set_error_msg(std::string(fn).append(": gt_normal and lambda_normal > 0 must be given together").c_str());
+		return PSB_ERR_ARG;
+	}
+	return 0;
+}
+
 // NULL: no exposure. Otherwise a row (param), a finite lr >= 0 and, for a step (`adam`), the moments and the device step count; for the
 // gradient mode a gradient output.
 int check_exposure(const psb_exposure* e, bool adam, const float* grad, const char* fn)
@@ -277,15 +299,15 @@ int refuse_filter3d(const psb_trainer* t, const char* fn)
 // Stage 1 of every pass: forward of SH degree D from raw parameters into t->image (or out_color); out_depth != NULL: the depth variant
 // also writes the expected depth there; out_alpha != NULL: the opacity variant also writes 1 - final_T there. The pass is recorded as
 // `mode`, with D = -1 until it has been binned. score != NULL: the score variant also adds the contribution scores there (no depth or
-// opacity plane).
+// opacity plane). mode.normals: n_i of the visible rows -> t->normals, and the normal variant writes the normal plane to out_normal.
 int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, const psb_camera* camera, const float* background,
                 float* out_color, int* radii, Scratch& sc, Camera& cam, cudaStream_t stream, float* out_depth, float* out_alpha, const PassMode& mode,
-                const ScoreSink* score = nullptr)
+                const ScoreSink* score = nullptr, float* out_normal = nullptr)
 {
 	int rc;
 	t->pass = mode;
 	t->pass.D = -1;
-	if ((rc = ensure(t, P, camera->width, camera->height, stream, mode.depth))) return rc;
+	if ((rc = ensure(t, P, camera->width, camera->height, stream, mode.depth, mode.normals))) return rc;
 	cam = to_camera(camera);
 	sc = carve_scratch(t, P, camera->width, camera->height);
 	GeomState& geom = sc.geom;
@@ -294,6 +316,7 @@ int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, con
 	const GaussIn in = raw_input(P, D, M, model);
 	t->mark(0, stream);
 	if ((rc = launch_preprocess(in, cam, radii, geom, /*raw=*/true, t->tight, stream, mode.aa, mode.f3d))) return rc;
+	if (mode.normals && (rc = launch_normals(P, model->param[0], model->param[4], model->param[5], cam, geom.tile_info, t->normals.get(), stream))) return rc;
 	t->mark(1, stream);
 	if ((rc = launch_depth_sort_and_scan(P, geom, /*scan=*/false, stream))) return rc;
 	t->mark(2, stream);
@@ -306,15 +329,16 @@ int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, con
 	PSB_CUDA_OK(cudaMemcpyAsync(t->h_count.get() + 1, t->ovf.get(), 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
 	PSB_CUDA_OK(cudaEventRecord(t->readback, stream));
 	rc = launch_render_forward(cam, img.ranges, bin.inst[sorted_slot(cam.W, cam.H)], geom.rec, background, out_color ? out_color : t->image.get(), img.final_T,
-	                           img.n_contrib, stream, out_depth, out_alpha, score);
+	                           img.n_contrib, stream, out_depth, out_alpha, score, mode.normals ? t->normals.get() : nullptr, out_normal);
 	t->mark(4, stream);
 	return rc;
 }
 
 // Stage 3 of every pass: the tile backward of the context's last forward pass (scratch sc, camera cam, mode t->pass) on per-pixel
-// gradients -> the packed sink rows (dL_ddepth: also dL/dz in slot 11; dL_dalpha: the opacity variant). P > 0.
+// gradients -> the packed sink rows (dL_ddepth: also dL/dz in slot 11; dL_dalpha: the opacity variant; dL_dnormal: the normal variant,
+// 16-float rows with dL/dn in slots 12..14, after a pass with mode.normals). P > 0.
 int tile_backward(psb_trainer* t, int P, const Scratch& sc, const Camera& cam, const float* background, const float* dL_dpix, const float* dL_ddepth,
-                  const float* dL_dalpha, cudaStream_t stream)
+                  const float* dL_dalpha, cudaStream_t stream, const float* dL_dnormal = nullptr)
 {
 	float* const rows = t->sink.get();
 	GradSink sink;
@@ -335,7 +359,8 @@ int tile_backward(psb_trainer* t, int P, const Scratch& sc, const Camera& cam, c
 	// (the deterministic gather runs inside this call: stage "render bwd" covers it)
 	int rc;
 	if ((rc = launch_render_backward(cam, sc.img.ranges, sc.bin.inst[sorted_slot(cam.W, cam.H)], sc.geom.rec, background, sc.img.final_T, sc.img.n_contrib,
-	                                 dL_dpix, sink, stream, dL_ddepth, t->pass.det ? &det : nullptr, dL_dalpha)))
+	                                 dL_dpix, sink, stream, dL_ddepth, t->pass.det ? &det : nullptr, dL_dalpha, dL_dnormal ? t->normals.get() : nullptr,
+	                                 dL_dnormal)))
 		return rc;
 	t->mark(6, stream);
 	return 0;
@@ -353,7 +378,8 @@ struct TileBackward {
 // image through the row; exposure_grad == NULL: the row takes its Adam step (with step's betas and eps), else dL/dE -> exposure_grad.
 int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                          const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
-                         bool moments, cudaStream_t stream, TileBackward& out, const psb_exposure* exposure, float* exposure_grad)
+                         bool moments, cudaStream_t stream, TileBackward& out, const psb_exposure* exposure, float* exposure_grad,
+                         const psb_normal* normal = nullptr)
 {
 	int rc;
 	if (!t || !camera || !step || !background || !gt_image) { set_error_msg("psb_trainer_step: null argument"); return PSB_ERR_ARG; }
@@ -369,13 +395,26 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 		if (!depth_plane) depth_plane = t->depth_buf.get();
 		dL_ddepth = t->depth_buf.get() + (size_t)camera->width * camera->height;
 	}
+	// normal term: the plane is the caller's out_normal or the context's own; dL/dN lives in the context. An out_normal alone renders the
+	// plane and leaves the backward that of the step without it.
+	const bool normal_loss = normal && normal->gt_normal;
+	float* normal_plane = normal ? normal->out_normal : nullptr;
+	float* dL_dnormal = nullptr;
+	if (normal_loss) {
+		if ((rc = ensure(t, P, camera->width, camera->height, stream, depth_loss, true, true))) return rc;
+		if (!normal_plane) normal_plane = t->normal_buf.get();
+		dL_dnormal = t->normal_buf.get() + 3 * (size_t)camera->width * camera->height;
+	}
 	if (exposure) PSB_CUDA_OK(t->exp_partials.grow(kExposurePartials, Fit::at_least, false, stream));
 	Scratch sc;
 	Camera cam;
+	PassMode mode = pass_mode(t, -1, depth_loss);
+	mode.normals = normal_plane != nullptr;
+	mode.normal = normal_loss;
 	// this pass gets its own tile backward below and its sink rows belong to this call's per-Gaussian stage (or to the _slab calls
 	// that follow a _begin): psb_trainer_backward_pixels must not add a second backward of it (D = -1)
-	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, sc, cam, stream, depth_plane, nullptr,
-	                      pass_mode(t, -1, depth_loss))))
+	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, sc, cam, stream, depth_plane, nullptr, mode, nullptr,
+	                      normal_plane)))
 		return rc;
 	const float* image = out_color ? out_color : t->image.get();
 	double* partials = t->deterministic ? t->det_partials.get() : nullptr;
@@ -385,14 +424,19 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	if (depth_loss &&
 	    (rc = launch_depth_loss(cam.H, cam.W, depth_plane, depth->gt_depth, mask, depth->lambda_depth, t->sums.get() + 2, dL_ddepth, stream, partials)))
 		return rc;
+	if (normal_loss &&
+	    (rc = launch_normal_loss(cam.H, cam.W, normal_plane, normal->gt_normal, mask, normal->lambda_normal, t->sums.get() + 4, dL_dnormal, stream, partials)))
+		return rc;
 	// loss sums -> pinned memory right behind the loss kernel, so the host can read the loss of this iteration (and start
 	// enqueueing the next one) while the backward half is still running
-	PSB_CUDA_OK(cudaMemcpyAsync(t->h_sums.get(), t->sums.get(), (depth_loss ? 4 : 2) * sizeof(double), cudaMemcpyDeviceToHost, stream));
+	PSB_CUDA_OK(cudaMemcpyAsync(t->h_sums.get(), t->sums.get(), (normal_loss ? 6 : depth_loss ? 4 : 2) * sizeof(double), cudaMemcpyDeviceToHost, stream));
 	PSB_CUDA_OK(cudaEventRecord(t->readback, stream));
 	t->last_lambda = step->lambda_dssim;
 	t->last_lambda_depth = depth_loss ? depth->lambda_depth : 0.f;
+	t->last_lambda_normal = normal_loss ? normal->lambda_normal : 0.f;
 	t->have_loss = true;
 	t->have_depth_loss = depth_loss;
+	t->have_normal_loss = normal_loss;
 	if (exposure) {
 		// dL/dI for the tile backward and the row's update (or gradient), inside stage "loss"; the row moves only after every read of it
 		ExposureUpdate u{exposure->param, exposure->exp_avg, exposure->exp_avg_sq, exposure->step, exposure->lr, step->beta1, step->beta2, step->eps};
@@ -402,7 +446,7 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	}
 	t->mark(5, stream);
 	if (P == 0) return 0;
-	if ((rc = tile_backward(t, P, sc, cam, background, t->dL_dpix.get(), dL_ddepth, nullptr, stream))) return rc;
+	if ((rc = tile_backward(t, P, sc, cam, background, t->dL_dpix.get(), dL_ddepth, nullptr, stream, dL_dnormal))) return rc;
 	out.geom = sc.geom;
 	out.cam = cam;
 	return 0;
@@ -604,7 +648,8 @@ int psb_trainer_destroy(psb_trainer* t)
 }
 
 static int forward_impl(const char* fn, psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
-                        int sh_degree, float* out_color, int* radii, float* out_depth, float* out_alpha, unsigned* pass, cudaStream_t stream)
+                        int sh_degree, float* out_color, int* radii, float* out_depth, float* out_alpha, unsigned* pass, cudaStream_t stream,
+                        float* out_normal = nullptr)
 {
 	int rc;
 	if (!t || !camera || !background || !out_color) { set_error_msg(std::string(fn).append(": null argument").c_str()); return PSB_ERR_ARG; }
@@ -613,11 +658,20 @@ static int forward_impl(const char* fn, psb_trainer* t, int P, int M, const psb_
 	Scratch sc;
 	Camera cam;
 	t->have_loss = false;
-	if ((rc = forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, sc, cam, stream, out_depth, out_alpha,
-	                      pass_mode(t, sh_degree, false))))
+	PassMode mode = pass_mode(t, sh_degree, false);
+	mode.normals = out_normal != nullptr;
+	if ((rc = forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, sc, cam, stream, out_depth, out_alpha, mode, nullptr,
+	                      out_normal)))
 		return rc;
 	if (pass) *pass = t->seq;
 	return 0;
+}
+
+int psb_trainer_forward_normal(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
+                               float* out_color, int* radii, float* out_depth, float* out_alpha, float* out_normal, unsigned* pass, void* stream_)
+{
+	return forward_impl(out_normal ? "psb_trainer_forward_normal" : "psb_trainer_forward", t, P, M, model, camera, background, sh_degree, out_color, radii,
+	                    out_depth, out_alpha, pass, (cudaStream_t)stream_, out_normal);
 }
 
 int psb_trainer_forward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
@@ -663,6 +717,13 @@ int psb_trainer_contribution(psb_trainer* t, int P, int M, const psb_model* mode
 int psb_trainer_backward_pixels(psb_trainer* t, unsigned pass, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                                 const psb_pixel_grads* pixel_grads, const psb_step* step, float* const* grads, void* stream_)
 {
+	return psb_trainer_backward_pixels_normal(t, pass, P, M, model, camera, background, pixel_grads, nullptr, step, grads, stream_);
+}
+
+int psb_trainer_backward_pixels_normal(psb_trainer* t, unsigned pass, int P, int M, const psb_model* model, const psb_camera* camera,
+                                       const float* background, const psb_pixel_grads* pixel_grads, const float* dL_dnormal, const psb_step* step,
+                                       float* const* grads, void* stream_)
+{
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
 	const bool adam = grads == nullptr;
@@ -688,6 +749,10 @@ int psb_trainer_backward_pixels(psb_trainer* t, unsigned pass, int P, int M, con
 		set_error_msg("psb_trainer_backward_pixels: the 3D filter changed since the forward pass");
 		return PSB_ERR_ARG;
 	}
+	if (dL_dnormal && !t->pass.normals) {
+		set_error_msg("psb_trainer_backward_pixels_normal: dL_dnormal needs a pass that rendered the normal plane (psb_trainer_forward_normal)");
+		return PSB_ERR_ARG;
+	}
 	if (step->step < 1) { set_error_msg("psb_trainer_backward_pixels: step >= 1 required"); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, adam))) return rc;
 	if (!adam && (rc = check_grads(grads, P, "psb_trainer_backward_pixels"))) return rc;
@@ -697,7 +762,8 @@ int psb_trainer_backward_pixels(psb_trainer* t, unsigned pass, int P, int M, con
 	const Scratch sc = carve_scratch(t, P, camera->width, camera->height);
 	const Camera cam = to_camera(camera);
 	t->pass.depth = pixel_grads->dL_ddepth != nullptr;
-	if ((rc = tile_backward(t, P, sc, cam, background, pixel_grads->dL_dcolor, pixel_grads->dL_ddepth, pixel_grads->dL_dalpha, stream))) return rc;
+	t->pass.normal = dL_dnormal != nullptr;
+	if ((rc = tile_backward(t, P, sc, cam, background, pixel_grads->dL_dcolor, pixel_grads->dL_ddepth, pixel_grads->dL_dalpha, stream, dL_dnormal))) return rc;
 	GradSegments gs{};
 	if (!adam)
 		for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
@@ -724,14 +790,22 @@ int psb_trainer_step_exposure(psb_trainer* t, int P, int M, const psb_model* mod
                               const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
                               const psb_exposure* exposure, void* stream_)
 {
+	return psb_trainer_step_normal(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, exposure, nullptr, stream_);
+}
+
+int psb_trainer_step_normal(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                            const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
+                            const psb_exposure* exposure, const psb_normal* normal, void* stream_)
+{
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
-	const char* fn = exposure ? "psb_trainer_step_exposure" : "psb_trainer_step_depth";
+	const char* fn = normal ? "psb_trainer_step_normal" : exposure ? "psb_trainer_step_exposure" : "psb_trainer_step_depth";
 	if ((rc = check_depth(depth, fn))) return rc;
 	if ((rc = check_exposure(exposure, true, nullptr, fn))) return rc;
+	if ((rc = check_normal(normal, fn))) return rc;
 	TileBackward tb;
 	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, true, stream, tb, exposure,
-	                               nullptr)) ||
+	                               nullptr, normal)) ||
 	    P == 0)
 		return rc;
 	rc = launch_fused_backward(true, 0, P, train_tensors(model, true), tb.cam, tb.geom, t->sink.get(), t->seeds.get(), to_hyper(step), GradSegments{},
@@ -843,7 +917,7 @@ int psb_adam_flat(size_t n, float* param, float* exp_avg, float* exp_avg_sq, con
 	return launch_adam(n, param, exp_avg, exp_avg_sq, grad, lr, h, grad_scale, (cudaStream_t)stream_);
 }
 
-static int result_impl(psb_trainer* t, float* out, bool with_depth, int* num_rendered, void* stream_)
+static int result_impl(psb_trainer* t, float* out, int n_out, int* num_rendered, void* stream_)
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
 	if (!t || t->carved.P < 0) { set_error_msg("psb_trainer_result: no step has run"); return PSB_ERR_ARG; }
@@ -880,23 +954,31 @@ static int result_impl(psb_trainer* t, float* out, bool with_depth, int* num_ren
 		const double inv_n = 1.0 / (3.0 * (double)t->carved.W * (double)t->carved.H);
 		const float l1 = (float)(h_sums[0] * inv_n), ss = (float)(h_sums[1] * inv_n);
 		const float dl1 = t->have_depth_loss ? (float)(h_sums[2] / (h_sums[3] > 1.0 ? h_sums[3] : 1.0)) : 0.f;
+		const float nl1 = t->have_normal_loss ? (float)(h_sums[4] / (h_sums[5] > 1.0 ? h_sums[5] : 1.0)) : 0.f;
 		out[0] = (1.0f - t->last_lambda) * l1 + t->last_lambda * (1.0f - ss);
 		if (t->have_depth_loss) out[0] += t->last_lambda_depth * dl1;
+		if (t->have_normal_loss) out[0] += t->last_lambda_normal * nl1;
 		out[1] = l1;
 		out[2] = ss;
-		if (with_depth) out[3] = dl1;
+		if (n_out > 3) out[3] = dl1;
+		if (n_out > 4) out[4] = nl1;
 	}
 	return 0;
 }
 
 int psb_trainer_result(psb_trainer* t, float* out3, int* num_rendered, void* stream_)
 {
-	return result_impl(t, out3, false, num_rendered, stream_);
+	return result_impl(t, out3, 3, num_rendered, stream_);
 }
 
 int psb_trainer_result_depth(psb_trainer* t, float* out4, int* num_rendered, void* stream_)
 {
-	return result_impl(t, out4, true, num_rendered, stream_);
+	return result_impl(t, out4, 4, num_rendered, stream_);
+}
+
+int psb_trainer_result_normal(psb_trainer* t, float* out5, int* num_rendered, void* stream_)
+{
+	return result_impl(t, out5, 5, num_rendered, stream_);
 }
 
 // Parity/debug export (tests only): per pixel, the final transmittance and the Gaussian index of the last blended splat

@@ -89,6 +89,51 @@ def make_scene(P, cam, seed=0, sh_degree_max=3, culled_frac=0.05, scale_px=2.4):
                 rotation=f32(rotation), opacity=f32(opacity))
 
 
+def _quat_of(R):
+    """(w, x, y, z) unit quaternion of the rotation matrix R (Shoemake): the inverse of the covariance's R(q)"""
+    tr = np.trace(R)
+    if tr > 0:
+        s = 2.0 * math.sqrt(tr + 1.0)
+        return np.array([0.25 * s, (R[2, 1] - R[1, 2]) / s, (R[0, 2] - R[2, 0]) / s, (R[1, 0] - R[0, 1]) / s])
+    i = int(np.argmax(np.diag(R)))
+    j, k = (i + 1) % 3, (i + 2) % 3
+    s = 2.0 * math.sqrt(1.0 + R[i, i] - R[j, j] - R[k, k])
+    q = np.zeros(4)
+    q[0] = (R[k, j] - R[j, k]) / s
+    q[1 + i] = 0.25 * s
+    q[1 + j] = (R[j, i] + R[i, j]) / s
+    q[1 + k] = (R[k, i] + R[i, k]) / s
+    return q
+
+
+def planar_scene(per_wall=4000, seed=0, in_plane=0.04, thickness=0.004):
+    """A room corner seen from near the identity view: a back wall (z = 5), a left wall (x = -1.5) and a floor (y = 1, the image's y axis
+    points down), each covered by `per_wall` flat Gaussians (in-plane scale `in_plane`, scale `thickness` along the plane's normal, which
+    is the shortest axis, scaling[2]) with a checker texture. -> (scene, normals [P,3]: the world-space unit normal of each row's plane,
+    facing the room)."""
+    rng = np.random.default_rng(seed)
+    planes = [  # (normal facing the room, origin, in-plane axis a, axis b, extent a, extent b)
+        (np.array([0.0, 0.0, -1.0]), np.array([-1.5, -1.5, 5.0]), np.array([1.0, 0.0, 0.0]), np.array([0.0, 1.0, 0.0]), 4.0, 2.5),
+        (np.array([1.0, 0.0, 0.0]), np.array([-1.5, -1.5, 1.5]), np.array([0.0, 0.0, 1.0]), np.array([0.0, 1.0, 0.0]), 3.5, 2.5),
+        (np.array([0.0, -1.0, 0.0]), np.array([-1.5, 1.0, 1.5]), np.array([1.0, 0.0, 0.0]), np.array([0.0, 0.0, 1.0]), 4.0, 3.5)]
+    xyz, nrm, rot, rgb = [], [], [], []
+    for k, (n, o, a, b, ea, eb) in enumerate(planes):
+        u, v = rng.uniform(0, ea, per_wall), rng.uniform(0, eb, per_wall)
+        xyz.append(o + u[:, None] * a + v[:, None] * b)
+        nrm.append(np.repeat(n[None], per_wall, 0))
+        rot.append(np.repeat(_quat_of(np.stack([a, np.cross(n, a), n], 1))[None], per_wall, 0))   # a right-handed frame with n third
+        check = ((np.floor(u / 0.5) + np.floor(v / 0.5)) % 2)[:, None]
+        base = np.array([[0.8, 0.3, 0.2], [0.2, 0.7, 0.3], [0.3, 0.3, 0.8]])[k]
+        rgb.append(np.clip(base * (0.6 + 0.4 * check) + rng.normal(0, 0.03, (per_wall, 3)), 0, 1))
+    P = 3 * per_wall
+    rgb = np.concatenate(rgb)
+    f32 = lambda x: np.ascontiguousarray(x, dtype=np.float32)
+    scene = dict(xyz=f32(np.concatenate(xyz)), features_dc=f32(((rgb - 0.5) / C0)[:, None, :]), features_rest=f32(np.zeros((P, 15, 3))),
+                 scaling=f32(np.log(np.repeat([[in_plane, in_plane, thickness]], P, 0))), rotation=f32(np.concatenate(rot)),
+                 opacity=f32(np.full((P, 1), 3.0)))
+    return scene, f32(np.concatenate(nrm))
+
+
 def activate(scene):
     """The reference's activations (src/gaussian_model.cpp:48-71) in numpy float32: for CPU-side tests."""
     s = scene

@@ -66,6 +66,20 @@ def _cdepth(gt_depth, lambda_depth, out_depth):
                   out_depth.data_ptr() if out_depth is not None else None)
 
 
+class _Normal(C.Structure):
+    _fields_ = [("gt_normal", C.c_void_p), ("lambda_normal", C.c_float), ("out_normal", C.c_void_p)]
+
+
+def _cnormal(gt_normal, lambda_normal, out_normal, H, W):
+    """psb_normal for a call, or None when it has no normal argument (the call is then the one without the normal term)."""
+    if gt_normal is None and out_normal is None and not lambda_normal:
+        return None
+    _plane(gt_normal, (3, H, W), "gt_normal")
+    _plane(out_normal, (3, H, W), "out_normal")
+    return _Normal(gt_normal.data_ptr() if gt_normal is not None else None, float(lambda_normal),
+                   out_normal.data_ptr() if out_normal is not None else None)
+
+
 class _Exposure(C.Structure):
     _fields_ = [("param", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p), ("step", C.c_void_p), ("lr", C.c_float)]
 
@@ -158,10 +172,13 @@ def _bind():
         "psb_trainer_render": render + [vp],
         "psb_trainer_render_depth": render + [vp, vp],
         "psb_trainer_forward": render + [vp, vp, P(u), vp],
+        "psb_trainer_forward_normal": render + [vp, vp, vp, P(u), vp],
         "psb_trainer_backward_pixels": [vp, u, i, i, Model, Cam, vp, P(_PixelGrads), Step, P(vp), vp],
+        "psb_trainer_backward_pixels_normal": [vp, u, i, i, Model, Cam, vp, P(_PixelGrads), vp, Step, P(vp), vp],
         "psb_trainer_step": call + [vp],
         "psb_trainer_step_depth": call + [Depth, vp],
         "psb_trainer_step_exposure": call + [Depth, Exp, vp],
+        "psb_trainer_step_normal": call + [Depth, Exp, P(_Normal), vp],
         "psb_trainer_backward": call + [P(vp), vp],
         "psb_trainer_backward_depth": call + [P(vp), Depth, vp],
         "psb_trainer_backward_exposure": call + [P(vp), Depth, Exp, vp, vp],
@@ -170,6 +187,8 @@ def _bind():
         "psb_trainer_backward_slab": [vp, i, i, Model, Cam, Step, i, i, P(vp), vp],
         "psb_trainer_result": [vp, P(f), P(i), vp],
         "psb_trainer_result_depth": [vp, P(f), P(i), vp],
+        "psb_trainer_result_normal": [vp, P(f), P(i), vp],
+        "psb_depth_normals": [Cam, vp, f, vp, vp],
         "psb_trainer_overflow_info": [vp, P(u), P(u), P(u)],
         "psb_trainer_debug_state": [vp, i, i, vp, vp, P(i), vp],
         "psb_trainer_set_profiling": [vp, i],
@@ -965,34 +984,43 @@ class GaussianTrainer:
         s.update_densify_stats = int(densify_stats)
         return s
 
-    def render(self, cam, out=None, radii=None, check=True, out_depth=None, out_alpha=None):
+    def render(self, cam, out=None, radii=None, check=True, out_depth=None, out_alpha=None, out_normal=None):
         """Forward only. check=True waits for the instance count and renders again if the binning arena had to grow (an
         overflowing render leaves `out` blank); pass check=False to only enqueue (call result() yourself before using `out`).
         out_depth: [H,W] float32 tensor that receives the expected depth sum_i z_i alpha_i T_i; out_alpha: [H,W] float32 tensor that
-        receives the accumulated opacity 1 - T_final (psb_trainer_forward). backwardPixels() back-propagates through this render."""
+        receives the accumulated opacity 1 - T_final (psb_trainer_forward); out_normal: [3,H,W] float32 tensor that receives the
+        view-space normal plane sum_i n_i alpha_i T_i (psb_trainer_forward_normal; N / |N| is the surface normal).
+        backwardPixels() back-propagates through this render."""
         m = self.model
+        H, W = int(cam["H"]), int(cam["W"])
         out = out if out is not None else torch.empty((3, cam["H"], cam["W"]), device=m.device)
         for t in (out_depth, out_alpha):
             assert t is None or (t.is_contiguous() and t.dtype == torch.float32 and t.numel() == cam["H"] * cam["W"])
+        _plane(out_normal, (3, H, W), "out_normal")
         self._hand_filter3d()
         cm, cc = m._cmodel(False), _ccamera(cam)
         pass_no = C.c_uint()
-        _lib.check(self.L.psb_trainer_forward(self.h, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(), m.active_sh_degree_,
-                                              out.data_ptr(), radii.data_ptr() if radii is not None else None,
-                                              out_depth.data_ptr() if out_depth is not None else None,
-                                              out_alpha.data_ptr() if out_alpha is not None else None, C.byref(pass_no),
-                                              torch.cuda.current_stream().cuda_stream), "psb_trainer_forward")
+        args = (self.h, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(), m.active_sh_degree_, out.data_ptr(),
+                radii.data_ptr() if radii is not None else None, out_depth.data_ptr() if out_depth is not None else None,
+                out_alpha.data_ptr() if out_alpha is not None else None)
+        if out_normal is None:
+            _lib.check(self.L.psb_trainer_forward(*args, C.byref(pass_no), torch.cuda.current_stream().cuda_stream), "psb_trainer_forward")
+        else:
+            _lib.check(self.L.psb_trainer_forward_normal(*args, out_normal.data_ptr(), C.byref(pass_no), torch.cuda.current_stream().cuda_stream),
+                       "psb_trainer_forward_normal")
         self._pass = pass_no.value
-        self._last_render = (cam, out, radii, out_depth, out_alpha)
-        self._last = _Call(False, lambda: self.render(cam, out, radii, check=False, out_depth=out_depth, out_alpha=out_alpha), False)
+        self._last_render = (cam, out, radii, out_depth, out_alpha, out_normal)
+        self._last = _Call(False, lambda: self.render(cam, out, radii, check=False, out_depth=out_depth, out_alpha=out_alpha, out_normal=out_normal),
+                           False)
         if check:
             self.result()
         return out
 
-    def backwardPixels(self, dL_dcolor, dL_ddepth=None, dL_dalpha=None, grads=None, densify_stats=None):
+    def backwardPixels(self, dL_dcolor, dL_ddepth=None, dL_dalpha=None, grads=None, densify_stats=None, dL_dnormal=None):
         """Back-propagates per-pixel gradients of the caller's loss through the last render() (psb_trainer_backward_pixels).
         dL_dcolor [3,H,W] (required), dL_ddepth / dL_dalpha [H,W] or None: contiguous float32 gradients w.r.t. the image, the depth and
-        the accumulated opacity of that render. grads=None: the fused Adam step of trainForOneIteration (advances step_ and iteration);
+        the accumulated opacity of that render; dL_dnormal [3,H,W] or None: w.r.t. its normal plane (a render with out_normal;
+        psb_trainer_backward_pixels_normal). grads=None: the fused Adam step of trainForOneIteration (advances step_ and iteration);
         grads = six contiguous float32 tensors shaped like the model's parameters: they receive the raw-parameter gradients and the
         parameters stay as they are (for a caller's own optimizer or all-reduce). The model must not change between the render and
         this call. densify_stats as in trainForOneIteration (both modes fold the densification statistics in).
@@ -1008,6 +1036,9 @@ class GaussianTrainer:
             raise ValueError("dL_dcolor is required")
         _plane(dL_ddepth, (H, W), "dL_ddepth")
         _plane(dL_dalpha, (H, W), "dL_dalpha")
+        _plane(dL_dnormal, (3, H, W), "dL_dnormal")
+        if dL_dnormal is not None and (len(self._last_render) < 6 or self._last_render[5] is None):
+            raise ValueError("dL_dnormal: the last render() rendered no normal plane (pass out_normal)")
         if grads is not None:
             grads = list(grads)
             if len(grads) != 6:
@@ -1025,19 +1056,23 @@ class GaussianTrainer:
         px = _PixelGrads(dL_dcolor.data_ptr(), dL_ddepth.data_ptr() if dL_ddepth is not None else None,
                          dL_dalpha.data_ptr() if dL_dalpha is not None else None)
         ptrs = None if adam else (C.c_void_p * 6)(*[g.data_ptr() for g in grads])
-        rc = self.L.psb_trainer_backward_pixels(self.h, self._pass, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(),
-                                                C.byref(px), C.byref(cs), ptrs, torch.cuda.current_stream().cuda_stream)
+        head = (self.h, self._pass, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(), C.byref(px))
+        if dL_dnormal is None:
+            rc = self.L.psb_trainer_backward_pixels(*head, C.byref(cs), ptrs, torch.cuda.current_stream().cuda_stream)
+        else:
+            rc = self.L.psb_trainer_backward_pixels_normal(*head, dL_dnormal.data_ptr(), C.byref(cs), ptrs, torch.cuda.current_stream().cuda_stream)
         if rc < 0 and adam:
             self.iteration -= 1
-        _lib.check(rc, "psb_trainer_backward_pixels")
+        _lib.check(rc, "psb_trainer_backward_pixels_normal" if dL_dnormal is not None else "psb_trainer_backward_pixels")
         if adam:
             m.step_ += 1
         self._last = _Call(adam, None, False)     # (trainWithLoss replaces it with its own record)
 
-    def trainWithLoss(self, cam, loss_fn, depth=False, alpha=False, out_color=None, radii=None, densify_stats=None):
+    def trainWithLoss(self, cam, loss_fn, depth=False, alpha=False, out_color=None, radii=None, densify_stats=None, normal=False):
         """One training iteration against the caller's loss: enqueues the forward (no host synchronisation of its own), calls
-        loss = loss_fn(image[, depth][, alpha]) on leaf tensors that require grad (image [3,H,W]; depth [H,W] = sum z alpha T with
-        depth=True; alpha [H,W] = 1 - T_final with alpha=True), takes torch.autograd.grad of the loss w.r.t. those outputs only, and
+        loss = loss_fn(image[, depth][, alpha][, normal]) on leaf tensors that require grad (image [3,H,W]; depth [H,W] = sum z alpha T with
+        depth=True; alpha [H,W] = 1 - T_final with alpha=True; normal [3,H,W] = sum n alpha T, the view-space normal plane, with
+        normal=True), takes torch.autograd.grad of the loss w.r.t. those outputs only, and
         back-propagates it through the fused kernels into a fused Adam step (backwardPixels). The model tensors never enter autograd.
         Advances step_ / iteration like trainForOneIteration and returns the (detached) loss tensor; result() repeats the whole call
         if the forward overflowed the binning arena. out_color / radii: optional tensors that receive the image / radii."""
@@ -1049,9 +1084,10 @@ class GaussianTrainer:
         _plane(image, (3, H, W), "out_color")
         D = torch.empty((H, W), device=m.device) if depth else None
         A = torch.empty((H, W), device=m.device) if alpha else None
+        N = torch.empty((3, H, W), device=m.device) if normal else None
         self._apply_deterministic()
-        self.render(cam, image, radii, check=False, out_depth=D, out_alpha=A)
-        outs = [t for t in (image, D, A) if t is not None]
+        self.render(cam, image, radii, check=False, out_depth=D, out_alpha=A, out_normal=N)
+        outs = [t for t in (image, D, A, N) if t is not None]
         leaves = [t.detach().requires_grad_(True) for t in outs]
         with torch.enable_grad():
             loss = loss_fn(*leaves)
@@ -1061,22 +1097,27 @@ class GaussianTrainer:
         gc = gc if gc is not None else torch.zeros_like(image)
         gd = next(g) if depth else None
         ga = next(g) if alpha else None
-        self.backwardPixels(gc, gd, ga, densify_stats=densify_stats)
+        gn = next(g) if normal else None
+        self.backwardPixels(gc, gd, ga, densify_stats=densify_stats, dL_dnormal=gn)
         self._inject_noise()
-        self._last = _Call(True, lambda: self.trainWithLoss(cam, loss_fn, depth, alpha, out_color, radii, densify_stats), True)
+        self._last = _Call(True, lambda: self.trainWithLoss(cam, loss_fn, depth, alpha, out_color, radii, densify_stats, normal), True)
         self._last_loss = loss.detach()
         return self._last_loss
 
     def trainForOneIteration(self, cam, gt_image, mask=None, out_color=None, radii=None, densify_stats=None, gt_depth=None, lambda_depth=0.0,
-                             out_depth=None, exposure_id=None):
+                             out_depth=None, exposure_id=None, gt_normal=None, lambda_normal=0.0, out_normal=None):
         """Enqueues render -> loss -> backward -> Adam on the current stream (no host sync).
         gt_depth: [H,W] float32 target depth in metres (<= 0: no measurement) trained with weight lambda_depth (> 0) as an L1 term
         over the valid pixels; out_depth: [H,W] float32 tensor that receives the rendered depth.
         exposure_id: the keyframe id k of gt_image, or None. With an id, the loss compares gt_image with the render through exposure row
         k of the model (applyExposure; the table grows to k + 1 rows if needed) and that row takes one Adam step at
-        model.exposure_lr_. out_color stays the raw render; result() reports the compensated loss. One psb_trainer_step_exposure call."""
+        model.exposure_lr_. out_color stays the raw render; result() reports the compensated loss. One psb_trainer_step_exposure call.
+        gt_normal: [3,H,W] float32 view-space unit normals ((0,0,0): no measurement; normals_from_depth) trained with weight lambda_normal
+        (> 0) as an L1 term against the rendered normal plane; out_normal: [3,H,W] float32 tensor that receives that plane. With either,
+        the call is psb_trainer_step_normal; result_normal() reports the normal L1."""
         m = self.model
         depth = _cdepth(gt_depth, lambda_depth, out_depth)
+        normal = _cnormal(gt_normal, lambda_normal, out_normal, int(cam["H"]), int(cam["W"]))
         exposure = None
         if exposure_id is not None:
             k = int(exposure_id)
@@ -1091,14 +1132,17 @@ class GaussianTrainer:
         if densify_stats is None:
             densify_stats = self.iteration < self.opt.densify_until_iter
         cm, cc, cs = m._cmodel(live=m.adamLive()), _ccamera(cam), self._cstep(densify_stats)
-        _lib.check(self.L.psb_trainer_step_exposure(*self._call_args(m, cm, cc, cs, gt_image, mask, out_color, radii),
-                                                    C.byref(depth) if depth is not None else None,
-                                                    C.byref(exposure) if exposure is not None else None, torch.cuda.current_stream().cuda_stream),
-                   "psb_trainer_step_exposure")
+        args = (*self._call_args(m, cm, cc, cs, gt_image, mask, out_color, radii), C.byref(depth) if depth is not None else None,
+                C.byref(exposure) if exposure is not None else None)
+        if normal is None:
+            rc = self.L.psb_trainer_step_exposure(*args, torch.cuda.current_stream().cuda_stream)
+        else:
+            rc = self.L.psb_trainer_step_normal(*args, C.byref(normal), torch.cuda.current_stream().cuda_stream)
+        _lib.check(rc, "psb_trainer_step_normal" if normal is not None else "psb_trainer_step_exposure")
         m.step_ += 1
         self._inject_noise()
         self._last = _Call(True, lambda: self.trainForOneIteration(cam, gt_image, mask, out_color, radii, densify_stats, gt_depth, lambda_depth,
-                                                                   out_depth, exposure_id), False)
+                                                                   out_depth, exposure_id, gt_normal, lambda_normal, out_normal), False)
 
     def _call_args(self, m, cm, cc, cs, gt_image, mask, out_color, radii):
         """The leading arguments of a built-in-loss training call (t ... radii)."""
@@ -1116,15 +1160,21 @@ class GaussianTrainer:
         After trainWithLoss: (the caller's loss, nan, nan, num_rendered).
         The overflow record is sticky on the device: if an EARLIER queued step overflowed (it was a no-op on the model while
         step_ advanced), this raises instead of silently continuing. The loss includes the depth term of a depth step."""
-        return self._result(False)
+        return self._result(3)
 
     def result_depth(self):
         """result() with the depth L1 of the last step: -> (loss, l1, ssim, depth_l1, num_rendered); depth_l1 = 0 without a depth target."""
-        return self._result(True)
+        return self._result(4)
 
-    def _result(self, with_depth):
-        out, n = (C.c_float * 4)(), C.c_int()
-        rc = self.L.psb_trainer_result_depth(self.h, out, C.byref(n), torch.cuda.current_stream().cuda_stream)
+    def result_normal(self):
+        """result() with the depth and normal L1 of the last step: -> (loss, l1, ssim, depth_l1, normal_l1, num_rendered); a term the step did
+        not have reads 0 (psb_trainer_result_normal)."""
+        return self._result(5)
+
+    def _result(self, nterms):
+        out, n = (C.c_float * 5)(), C.c_int()
+        result_fn = self.L.psb_trainer_result_normal if nterms == 5 else self.L.psb_trainer_result_depth
+        rc = result_fn(self.h, out, C.byref(n), torch.cuda.current_stream().cuda_stream)
         if rc == -4:
             first, count, cur = self._overflow_info()
             last = self._last
@@ -1143,13 +1193,13 @@ class GaussianTrainer:
                                     "no-op; the arena has been grown. Render again (with check=True, or collect result() before computing the "
                                     "loss) and repeat the loss and backwardPixels.")
             last.repeat()
-            return self._result(with_depth)
-        _lib.check(rc, "psb_trainer_result_depth")
+            return self._result(nterms)
+        _lib.check(rc, "psb_trainer_result_normal" if nterms == 5 else "psb_trainer_result_depth")
         if self._last.callers_loss:
-            # the caller's loss: only its value is known (l1, ssim and depth_l1 are the built-in loss's terms)
+            # the caller's loss: only its value is known (l1, ssim, depth_l1 and normal_l1 are the built-in loss's terms)
             nan = float("nan")
-            out = (float(self._last_loss), nan, nan, nan)
-        return (*out[:4 if with_depth else 3], n.value)
+            out = (float(self._last_loss), nan, nan, nan, nan)
+        return (*out[:nterms], n.value)
 
     # ------------------------------------------------------------------------------------------------------------
     # Host-input front end: what the mapper thread does every iteration — `gt_image = original_image_.cuda()`
@@ -1391,10 +1441,15 @@ class DataParallelTrainer(GaussianTrainer):
         self.flat = self.grads.flat
 
     def trainForOneIteration(self, cam, gt_image, mask=None, out_color=None, radii=None, densify_stats=None, gt_depth=None, lambda_depth=0.0,
-                             out_depth=None, exposure_id=None):
+                             out_depth=None, exposure_id=None, gt_normal=None, lambda_normal=0.0, out_normal=None):
         """Depth arguments as in GaussianTrainer, on every path: "p2p" (psb_dp_step_depth), the slab pipeline
         (psb_trainer_backward_begin_depth) and the flat "nccl" path (psb_trainer_backward_depth). Each rank passes its own view's
-        target or none: ranks with and without a depth term may train in the same step. exposure_id must be None."""
+        target or none: ranks with and without a depth term may train in the same step. exposure_id and the normal arguments must be
+        None."""
+        if gt_normal is not None or out_normal is not None or lambda_normal:
+            raise NotImplementedError("DataParallelTrainer: the normal term is not wired into the data-parallel steps (the NVLink push "
+                                      "backward and the slab pipeline carry 12-float sink rows); train with normals on one GPU through "
+                                      "GaussianTrainer")
         if exposure_id is not None:
             raise NotImplementedError("DataParallelTrainer: exposure compensation is not wired into the data-parallel steps: the per-keyframe "
                                       "exposure table would have to be replicated across the ranks (each rank's row updates gathered to "
@@ -1478,6 +1533,26 @@ class DataParallelTrainer(GaussianTrainer):
         from .parallel import reduce_densify_stats
         m = self.model
         reduce_densify_stats(m.max_radii2D_, m.xyz_gradient_accum_, m.denom_, self.group)
+
+
+def normals_from_depth(cam, depth, max_rel_jump=0.05, out=None):
+    """View-space unit normals [3,H,W] of a depth image [H,W] (metres; <= 0 or not finite: no measurement) seen by `cam` (psb_depth_normals):
+    central differences of the back-projected neighbours, (0,0,0) on the border, at holes and across depth edges (a neighbour more than
+    max_rel_jump z away). The target of trainForOneIteration(gt_normal=...): compute it once per keyframe and pyramid level."""
+    H, W = int(cam["H"]), int(cam["W"])
+    _plane(depth, (H, W), "depth")
+    if depth is None:
+        raise ValueError("depth is required")
+    out = out if out is not None else torch.empty((3, H, W), device=depth.device)
+    _plane(out, (3, H, W), "out")
+    if not (math.isfinite(max_rel_jump) and max_rel_jump > 0):
+        raise ValueError(f"max_rel_jump must be finite and positive, got {max_rel_jump}")
+    c = _Camera()
+    c.tan_fovx, c.tan_fovy, c.width, c.height = float(cam["tanfovx"]), float(cam["tanfovy"]), W, H
+    L = _bind()
+    _lib.check(L.psb_depth_normals(C.byref(c), depth.data_ptr(), float(max_rel_jump), out.data_ptr(), torch.cuda.current_stream().cuda_stream),
+               "psb_depth_normals")
+    return out
 
 
 def fused_loss(image, gt, mask=None, lambda_dssim=0.2, want_grad=True):
