@@ -180,7 +180,10 @@ def RasterizeGaussiansBackwardCUDA(background, means3D, radii, colors, scales, r
                                    geomBuffer, R, binningBuffer, imageBuffer, *, deterministic=False, antialiasing=False):
     """-> (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations).
     deterministic=True: the same gradients, bit-identical from call to call (summed in a fixed order instead of with float atomics).
-    antialiasing=True: the backward of an anti-aliased forward (the same flag there); dL_dopacity is then dL/do."""
+    antialiasing=True: the backward of an anti-aliased forward (the same flag there); dL_dopacity is then dL/do.
+    dL_dmeans2D is in NDC units: dL/dpixel times (W/2, H/2). With scale_modifier != 1, dL_dscales is the gradient with respect to the
+    modified scale scale_modifier * scales, not with respect to `scales` (the reference's convention: the factor is not applied); the true
+    dL/dscales is dL_dscales * scale_modifier."""
     return _backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
                      tan_fovx, tan_fovy, dL_dout_color, None, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer, deterministic,
                      antialiasing)

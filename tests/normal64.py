@@ -15,16 +15,18 @@ def rotation_columns(q):
     return torch.stack([c0, c1, c2], 2)
 
 
-def gaussian_normals(raw, cam):
+def gaussian_normals(raw, cam, flip=True):
     """n_i [P,3] in view space of the trainer parameters raw (dict of s64.RAW) seen by cam (s64.camera64): k = argmin of the raw log-scales
     (the first on ties), r = column k of R(q / max(|q|, 1e-12)), m = V r, n = m if m . t <= 0 else -m (t = the view-space mean). The
-    argmin and the flip are constants of the pass."""
+    argmin and the flip are constants of the pass. flip=False: m itself, not turned towards the camera."""
     q = raw["rotation"]
     q = q / q.norm(dim=1, keepdim=True).clamp_min(1e-12)
     k = torch.argmin(raw["scaling"].detach(), dim=1)
     r = rotation_columns(q)[torch.arange(q.shape[0], device=q.device), :, k]
     V = cam["V"]                                      # V[c][r] = viewmatrix[4 c + r]: the math V is V.T
     m = r @ V[:3, :3]
+    if not flip:
+        return m
     t = raw["xyz"] @ V[:3, :3] + V[3, :3]
     sign = torch.where((m * t).sum(1).detach() <= 0, 1.0, -1.0).to(m.dtype)
     return m * sign[:, None]

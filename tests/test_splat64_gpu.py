@@ -3,7 +3,8 @@ kernels, with every decision of every scene at least splat64.MIN_MARGIN (relativ
 
   * operator forward (RasterizeGaussiansCUDA and RasterizeGaussiansDepthCUDA, plain and anti-aliased): colour, depth, radii,
     tiles_touched, tile-list lengths and per-pixel contributor counts; operator backward (atomic, deterministic, anti-aliased) against
-    float64 autograd on the activated leaves, with random weights on colour and depth;
+    float64 autograd on the activated leaves, with random weights on colour and depth, dL_dmeans2D (the densification signal, in NDC
+    units) included; at scale_modifier = 0.6 the forward and the backward, whose dL_dscales is the gradient with respect to 0.6 s;
   * trainer render (colour, depth, A, radii, last contributor and final T of psb_trainer_debug_state) and backwardPixels against
     float64 autograd on the raw parameters, default and deterministic modes, anti-aliasing on and off;
   * the built-in loss: psb_trainer_backward, _depth and _exposure in gradient mode (loss scalars, raw-parameter gradients, the 12
@@ -226,9 +227,9 @@ def _op_inputs(sc, dev):
     return {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in act.items()}
 
 
-def _op_forward(g, c, bg, D, aa):
+def _op_forward(g, c, bg, D, aa, mod=1.0):
     from photo_slam_b200 import rasterizer
-    return rasterizer.RasterizeGaussiansDepthCUDA(bg, g["means3D"], None, g["opacities"], g["scales"], g["rotations"], 1.0, None, c["viewmatrix"],
+    return rasterizer.RasterizeGaussiansDepthCUDA(bg, g["means3D"], None, g["opacities"], g["scales"], g["rotations"], mod, None, c["viewmatrix"],
                                                   c["projmatrix"], c["tanfovx"], c["tanfovy"], c["H"], c["W"], g["shs"], D, c["campos"], False,
                                                   antialiasing=aa)
 
@@ -245,9 +246,17 @@ def _export(P, R, W, H, geom, binning, img):
     return tt.long(), (ranges[:, 1] - ranges[:, 0]).long(), nc.long().reshape(H, W)
 
 
-def _truth_op(g, cam, bg, D, aa, conv=s64.CONV):
+def _truth_op(g, cam, bg, D, aa, conv=s64.CONV, mod=1.0):
+    """float64 leaves and the truth's render of them; the NDC mean2D is kept for its gradient (dL_dmeans2D)"""
     leaves = {k: v.double().clone().requires_grad_(True) for k, v in g.items()}
-    return leaves, s64.render(leaves, s64.camera64(cam, g["means3D"].device), bg, D=D, aa=aa, conv=conv)
+    tr = s64.render(leaves, s64.camera64(cam, g["means3D"].device), bg, D=D, aa=aa, scale_modifier=mod, conv=conv)
+    tr["geo"]["means2D"].retain_grad()
+    return leaves, tr
+
+
+def _ndc_mean2d_grad(tr, W, H):
+    """dL/dmean2D of the truth in the operator's NDC units: dL/dpixel * (W/2, H/2)"""
+    return tr["geo"]["means2D"].grad * torch.tensor([0.5 * W, 0.5 * H], dtype=torch.float64, device=tr["geo"]["means2D"].device)
 
 
 def _check_edge(s, name, tt, list_len, nc, radii, truth):
@@ -310,13 +319,57 @@ def test_operator_against_truth(cuda, name, aa):
         out = rasterizer.RasterizeGaussiansBackwardDepthCUDA(bgt, g["means3D"], radii, None, g["scales"], g["rotations"], 1.0, None, c["viewmatrix"],
                                                              c["projmatrix"], c["tanfovx"], c["tanfovy"], wc, wd, g["shs"], D, c["campos"], geom, R,
                                                              binning, img, deterministic=det, antialiasing=aa)
-        _, _, d_op, d_m3, _, d_sh, d_sc, d_rot = out
-        for k, a in (("means3D", d_m3), ("shs", d_sh), ("opacities", d_op), ("scales", d_sc), ("rotations", d_rot)):
-            errs[f"grad-{k}-{'det' if det else 'atomic'}"] = _relnorm(a, leaves[k].grad)
-            errs[f"gradmax-{k}-{'det' if det else 'atomic'}"] = _maxerr(a, leaves[k].grad, float(leaves[k].grad.abs().max()))
+        d_m2, _, d_op, d_m3, _, d_sh, d_sc, d_rot = out
+        m2 = _ndc_mean2d_grad(tr, W, H)
+        for k, a, ref in (("means3D", d_m3, leaves["means3D"].grad), ("shs", d_sh, leaves["shs"].grad), ("opacities", d_op, leaves["opacities"].grad),
+                          ("scales", d_sc, leaves["scales"].grad), ("rotations", d_rot, leaves["rotations"].grad), ("means2D", d_m2[:, :2], m2)):
+            errs[f"grad-{k}-{'det' if det else 'atomic'}"] = _relnorm(a, ref)
+            errs[f"gradmax-{k}-{'det' if det else 'atomic'}"] = _maxerr(a, ref, float(ref.abs().max()))
     torch.cuda.synchronize()
     print(f"MEASURED operator {name} aa={aa} margins={min(s['margins'].values()):.2e} {errs}")
     assert errs["color"] < GATE_COLOR and errs["color_plain_entry"] < GATE_COLOR and errs["depth"] < GATE_DEPTH, errs
+    _assert_grad_gates(errs)
+
+
+MOD = 0.6
+MOD_CASES = [(n, aa) for n in ("odd-P-129", "alpha-clamp", "terminate-mid-batch", "frustum-clamp") for aa in (False, True)]
+
+
+def _op_mod_pass(cuda, name, aa):
+    """forward and backward of the operator at scale_modifier = MOD, and the truth's render at MOD with its autograd"""
+    from photo_slam_b200 import rasterizer
+    s = _scene(name)
+    cam, D, bg = s["cam"], s["D"], _bg(name)
+    c, g = syn.device_camera(cam, cuda), _op_inputs(s["sc"], cuda)
+    bgt = torch.tensor(bg, device=cuda)
+    R, color, depth, radii, geom, binning, img = _op_forward(g, c, bgt, D, aa, mod=MOD)
+    leaves, tr = _truth_op(g, cam, bg, D, aa, mod=MOD)
+    wc, wd, _ = _weights(cam["H"], cam["W"], cuda)
+    ((tr["color"] * wc.double()).sum() + (tr["depth"] * wd.double()).sum()).backward()
+    out = rasterizer.RasterizeGaussiansBackwardDepthCUDA(bgt, g["means3D"], radii, None, g["scales"], g["rotations"], MOD, None, c["viewmatrix"],
+                                                         c["projmatrix"], c["tanfovx"], c["tanfovy"], wc, wd, g["shs"], D, c["campos"], geom, R,
+                                                         binning, img, antialiasing=aa)
+    torch.cuda.synchronize()
+    return s, (color, depth, radii), out, leaves, tr
+
+
+@pytest.mark.parametrize("name,aa", MOD_CASES, ids=[f"{n}-{'aa' if a else 'plain'}" for n, a in MOD_CASES])
+def test_operator_scale_modifier_against_truth(cuda, name, aa):
+    """scale_modifier = 0.6: the forward draws the splats at 0.6 s; the backward's dL_dscales is the gradient with respect to the modified
+    scale 0.6 s (the reference's convention, RasterizeGaussiansBackwardCUDA), i.e. the truth's dL/ds / 0.6"""
+    s, (color, depth, radii), out, leaves, tr = _op_mod_pass(cuda, name, aa)
+    W, H = s["cam"]["W"], s["cam"]["H"]
+    assert torch.equal(radii.long(), tr["radii"])
+    zmax = max(float(tr["depth"].detach().abs().max()), 1e-30)
+    errs = dict(color=_maxerr(color, tr["color"].detach()), depth=_maxerr(depth, tr["depth"].detach(), zmax))
+    d_m2, _, d_op, d_m3, _, d_sh, d_sc, d_rot = out
+    for k, a, ref in (("means3D", d_m3, leaves["means3D"].grad), ("shs", d_sh, leaves["shs"].grad), ("opacities", d_op, leaves["opacities"].grad),
+                      ("scales", d_sc, leaves["scales"].grad / MOD), ("rotations", d_rot, leaves["rotations"].grad),
+                      ("means2D", d_m2[:, :2], _ndc_mean2d_grad(tr, W, H))):
+        errs[f"grad-{k}"] = _relnorm(a, ref)
+        errs[f"gradmax-{k}"] = _maxerr(a, ref, float(ref.abs().max()))
+    print(f"MEASURED operator scale_modifier {name} aa={aa} {errs}")
+    assert errs["color"] < GATE_COLOR and errs["depth"] < GATE_DEPTH, errs
     _assert_grad_gates(errs)
 
 
@@ -624,6 +677,35 @@ def test_perturbed_truth_fails_the_gate(cuda, what):
         assert errmax > GATE_GRAD_MAX, errmax
     print(f"MEASURED perturbed {what}: {err:.2e} (gate {gate:.0e})")
     assert err > gate, f"{what}: the gate does not see the perturbation ({err} <= {gate})"
+
+
+def test_perturbed_scale_modifier_convention_fails_the_gate(cuda):
+    """dL_dscales at scale_modifier = 0.6 against the true dL/ds (the factor applied): the scales gates reject it"""
+    _, _, out, leaves, _ = _op_mod_pass(cuda, "odd-P-129", False)
+    d_sc, ref = out[6], leaves["scales"].grad
+    err, errmax = _relnorm(d_sc, ref), _maxerr(d_sc, ref, float(ref.abs().max()))
+    print(f"MEASURED perturbed scale_modifier convention: {err:.2e} (gate {GATE_GRAD:.0e}), max {errmax:.2e} (gate {GATE_GRAD_MAX:.0e})")
+    assert err > GATE_GRAD and errmax > GATE_GRAD_MAX
+
+
+def test_perturbed_ndc_mean2d_fails_the_gate(cuda):
+    """dL_dmeans2D against the truth's gradient in pixels instead of NDC: the means2D gate rejects it"""
+    name = "odd-P-129"
+    s = _scene(name)
+    cam, D, bg = s["cam"], s["D"], _bg(name)
+    c, g = syn.device_camera(cam, cuda), _op_inputs(s["sc"], cuda)
+    bgt = torch.tensor(bg, device=cuda)
+    R, color, depth, radii, geom, binning, img = _op_forward(g, c, bgt, D, False)
+    leaves, tr = _truth_op(g, cam, bg, D, False)
+    wc, wd, _ = _weights(cam["H"], cam["W"], cuda)
+    ((tr["color"] * wc.double()).sum() + (tr["depth"] * wd.double()).sum()).backward()
+    from photo_slam_b200 import rasterizer
+    d_m2 = rasterizer.RasterizeGaussiansBackwardDepthCUDA(bgt, g["means3D"], radii, None, g["scales"], g["rotations"], 1.0, None, c["viewmatrix"],
+                                                          c["projmatrix"], c["tanfovx"], c["tanfovy"], wc, wd, g["shs"], D, c["campos"], geom, R,
+                                                          binning, img)[0]
+    err = _relnorm(d_m2[:, :2], tr["geo"]["means2D"].grad)
+    print(f"MEASURED perturbed mean2D in pixels: {err:.2e} (gate {GATE_GRAD:.0e})")
+    assert err > GATE_GRAD
 
 
 @pytest.mark.parametrize("what", ["termination", "clamp-autograd"])
