@@ -432,6 +432,48 @@ int psb_trainer_result_normal(psb_trainer* t, float* out5, int* num_rendered, vo
  * tan_fovy are read) -> out_normal [3,H,W] device. PSB_ERR_ARG, before any CUDA call, for a NULL camera, depth or output, a size that is
  * not positive, a tan_fov that is not finite and positive, and a max_rel_jump that is not finite and positive. Asynchronous. */
 int psb_depth_normals(const psb_camera* camera, const float* depth, float max_rel_jump, float* out_normal, void* stream);
+/* ------------------------------------------------------------------------------------------------
+ * Depth-normal consistency (2DGS, PGSR): the normal of the map's own rendered depth should agree with its rendered normal plane. It
+ * needs no sensor and is invariant to the depth scale, so it trains surface orientation on monocular and stereo keyframes too.
+ * Inputs: D [H,W], A = 1 - T_final [H,W] and N [3,H,W] of one pass, seen by that pass's camera.
+ * Normalised depth: Dbar(p) = D(p) / A(p) (an IEEE division) where A(p) >= alpha_min, else 0 (a hole to psb_depth_normals).
+ * Depth normal: n_d = psb_depth_normals applied to Dbar with max_rel_jump (same back-projection, central differences, camera-facing
+ *   flip, border, hole and depth-edge rules); n_d = (0,0,0) marks an invalid pixel.
+ * Valid pixels: n_d(p) != 0 and, with a mask, mask[0,p] != 0 (the depth and normal terms' convention).
+ * Loss: dn = sum_valid (1 - n_d(p) . N(p)) / max(N_valid, 1); L += lambda_dn dn. N stays un-normalised, as in the normal term: since
+ *   |N| <= A <= 1 each summand is >= 0, and the term also pushes A towards 1 on valid pixels (deliberate, like the depth and normal terms).
+ * Gradients: dL/dN(p) = -lambda_dn n_d(p) / max(N_valid, 1) on valid p. dL/dDbar(q) gathers from the valid p whose stencil reads q,
+ *   through the normalisation (I - n n^T) / |c| and the cross product c = a x b, a = X(u+1) - X(u-1), b = X(v+1) - X(v-1),
+ *   X(q) = Dbar(q) ray(q); the centre depth, the flip and validity are piecewise constant and carry no gradient. Then
+ *   dL/dD = dL/dDbar / A and dL/dA = -dL/dDbar Dbar / A on pixels with A >= alpha_min. Both enter the tile backward with dL/dN, so the
+ *   term reaches rotations (through N), positions, opacity and shape, and the densification statistics.
+ * N_valid is counted on the device and the scale lambda_dn / max(N_valid, 1) read there; no float atomics on the planes, and in
+ * deterministic mode the loss sums are reduced in a fixed order. With a depth and/or normal term in the same step, their gradients are
+ * written first and this term adds into the same planes. Anti-aliasing, the 3D filter and exposure compose unchanged (exposure acts on
+ * colour only). The data-parallel calls, the _begin / _slab halves and the rasterizer operator take no consistency term.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct psb_dn {
+	float lambda_dn;          /* finite, > 0 */
+	float alpha_min;          /* (0, 1] */
+	float max_rel_jump;       /* finite, > 0: the depth-edge rule of psb_depth_normals */
+	float* out_depth_normal;  /* [3,H,W] device or NULL: n_d, (0,0,0) where psb_depth_normals of Dbar gives it */
+} psb_dn;
+/* psb_trainer_step_normal plus the consistency term (dn == NULL: exactly psb_trainer_step_normal). The pass renders D, A and N (in the
+ * context's own planes where the caller passes none). PSB_ERR_ARG, before any CUDA call and with the model untouched, for everything
+ * psb_trainer_step_normal rejects, a lambda_dn that is not finite and > 0, an alpha_min outside (0, 1] and a max_rel_jump that is not
+ * finite and > 0. A step that overflows the binning arena is a no-op: repeating it applies the term once. */
+int psb_trainer_step_dn(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                        const float* background, const float* gt_image, const float* mask, const psb_step* step,
+                        float* out_color, int* radii, const psb_depth* depth, const psb_exposure* exposure, const psb_normal* normal,
+                        const psb_dn* dn, void* stream);
+/* psb_trainer_result with out6 = {loss, l1, ssim, depth_l1, normal_l1, dn} (0 for a term the last step did not have). */
+int psb_trainer_result_dn(psb_trainer* t, float* out6, int* num_rendered, void* stream);
+/* The consistency term on a caller's planes (the two kernels of the built-in step): depth, alpha [H,W] and normal [3,H,W] device, mask
+ * [H,W] device or NULL, seen by `camera` (width, height, tan_fovx and tan_fovy are read). dL_ddepth, dL_dalpha [H,W] and dL_dnormal [3,H,W]
+ * are ADDED into; out2_host (or NULL) <- {dn, N_valid}. PSB_ERR_ARG, before any CUDA call, for a NULL camera, plane or dn, the camera
+ * psb_depth_normals rejects and the dn values psb_trainer_step_dn rejects. Synchronises the stream; the same result every run. */
+int psb_dn_loss(const psb_camera* camera, const float* depth, const float* alpha, const float* normal, const float* mask, const psb_dn* dn,
+                float* dL_ddepth, float* dL_dalpha, float* dL_dnormal, float* out2_host, void* stream);
 
 /* model->adam_live[i] = 1 if any of the 118 moments of row i is non-zero, else 0: one pass over the moments. Restores the
  * psb_model.adam_live contract after moments were written by anything but psb_trainer_step. Asynchronous on `stream`. */

@@ -7,6 +7,7 @@
 // needs; backward filters those three maps (the window is symmetric, so the adjoint of the zero-padded
 // convolution is the same convolution) and writes dL/d(rendered) directly.
 #include "psb_common.cuh"
+#include "psb_normals.cuh"
 #include "psb_train.h"
 
 namespace psb {
@@ -360,7 +361,141 @@ __global__ void __launch_bounds__(256) normal_grad_scale_kernel(int n, float lam
 	for (int i = blockIdx.x * 256 + threadIdx.x; i < 3 * n; i += gridDim.x * 256) dL_dN[i] *= scale;
 }
 
+// Depth-normal consistency (include/psb200.h, psb_dn). The planes of one pass and its camera; D-bar(q) = D(q) / A(q) where
+// A(q) >= alpha_min, else 0 (a hole to the stencil).
+struct DnPlanes {
+	NormalCam c;
+	const float* __restrict__ D;
+	const float* __restrict__ A;
+	const float* __restrict__ N;
+	const float* __restrict__ mask;
+	float alpha_min, max_rel_jump;
+};
+
+__device__ __forceinline__ float dn_dbar(const DnPlanes& p, int q)
+{
+	const float a = p.A[q];
+	return a >= p.alpha_min ? p.D[q] / a : 0.f;
+}
+
+// n_d at pixel (u, v), which may lie outside the image ((0,0,0) there and on the border); its stencil -> st (st.s = 0 where n_d = 0)
+__device__ __forceinline__ float3 dn_normal(const DnPlanes& p, int u, int v, Stencil& st)
+{
+	float3 nrm = make_float3(0.f, 0.f, 0.f);
+	st.s = 0.f;
+	if (u > 0 && v > 0 && u < p.c.W - 1 && v < p.c.H - 1) {
+		const int i = v * p.c.W + u;
+		stencil_normal(p.c, u, v, dn_dbar(p, i), dn_dbar(p, i - 1), dn_dbar(p, i + 1), dn_dbar(p, i - p.c.W), dn_dbar(p, i + p.c.W), p.max_rel_jump,
+		               nrm, st);
+	}
+	return nrm;
+}
+
+__device__ __forceinline__ bool dn_valid(const DnPlanes& p, int i, float3 nd)
+{
+	return (nd.x != 0.f || nd.y != 0.f || nd.z != 0.f) && (!p.mask || p.mask[i] != 0.f);
+}
+
+// Pass 1 (the geometry of depth_loss_kernel): per valid pixel 1 - n_d . N; block sums of it and of the valid count -> sums[0..1]
+// (DET: the block's partials); n_d -> out_dn when given. (The minimum of 4 blocks lets ptxas keep the DET variant out of local memory:
+// without it it picks 32 registers and spills.)
+template <bool DET>
+__global__ void __launch_bounds__(256, 4) dn_loss_kernel(DnPlanes p, float* __restrict__ out_dn, double* __restrict__ sums)
+{
+	__shared__ float s_red[8];
+	const int n = p.c.W * p.c.H;
+	float acc = 0.f, cnt = 0.f;
+	for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) {
+		Stencil st;
+		const float3 nd = dn_normal(p, i % p.c.W, i / p.c.W, st);
+		if (dn_valid(p, i, nd)) {
+			acc += 1.f - (nd.x * p.N[i] + nd.y * p.N[n + i] + nd.z * p.N[2 * n + i]);
+			cnt += 1.f;
+		}
+		if (out_dn) {
+			out_dn[i] = nd.x;
+			out_dn[n + i] = nd.y;
+			out_dn[2 * n + i] = nd.z;
+		}
+	}
+	const float tacc = block_sum_256(acc, s_red);
+	const float tcnt = block_sum_256(cnt, s_red);
+	block_sums_out<DET>(tacc, tcnt, sums);
+}
+
+// dL/dc of the stencil of pixel (u, v) per unit of lambda / max(N_valid, 1), for n_d = s c and the term -n_d . N:
+// -s (N - n_d (n_d . N)). False where (u, v) is not a valid pixel.
+__device__ __forceinline__ bool dn_dc(const DnPlanes& p, int u, int v, Stencil& st, float3& g)
+{
+	const float3 nd = dn_normal(p, u, v, st);
+	const int n = p.c.W * p.c.H, i = v * p.c.W + u;
+	if (!dn_valid(p, i, nd)) return false;
+	const float N0 = p.N[i], N1 = p.N[n + i], N2 = p.N[2 * n + i];
+	const float nN = nd.x * N0 + nd.y * N1 + nd.z * N2;
+	g = make_float3(-st.s * (N0 - nd.x * nN), -st.s * (N1 - nd.y * nN), -st.s * (N2 - nd.z * nN));
+	return true;
+}
+
+__device__ __forceinline__ float3 cross3(float3 a, float3 b)
+{
+	return make_float3(a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x);
+}
+
+// Pass 2, one thread per pixel q, no atomics: with k = lambda / max(N_valid, 1) read on the device, dL/dN(q) += -k n_d(q) on a valid q;
+// dL/dD-bar(q) gathers, in a fixed order, the dL/dX(q) of the four stencils that read q (c = a x b: dL/da = b x dL/dc, dL/db = dL/dc x a;
+// q is X(u-1) of its right neighbour, X(u+1) of its left one, X(v-1) of the one below and X(v+1) of the one above), each recomputed
+// here, times dX/dD-bar = the ray of q. Then dL/dD(q) += dL/dD-bar / A and dL/dA(q) += -dL/dD-bar D-bar / A where A >= alpha_min.
+__global__ void __launch_bounds__(256) dn_grad_kernel(DnPlanes p, float lambda, const double* __restrict__ sums, float* __restrict__ dL_dD,
+                                                      float* __restrict__ dL_dA, float* __restrict__ dL_dN)
+{
+	const int n = p.c.W * p.c.H;
+	const int i = blockIdx.x * 256 + threadIdx.x;
+	if (i >= n) return;
+	const int u = i % p.c.W, v = i / p.c.W;
+	const float k = lambda / (float)fmax(sums[1], 1.0);
+	Stencil st;
+	const float3 nd = dn_normal(p, u, v, st);
+	if (dn_valid(p, i, nd)) {
+		dL_dN[i] += -k * nd.x;
+		dL_dN[n + i] += -k * nd.y;
+		dL_dN[2 * n + i] += -k * nd.z;
+	}
+	const float a = p.A[i];
+	if (!(a >= p.alpha_min)) return;
+	const float rx = ((float)u + 0.5f - p.c.half_w) / p.c.fx, ry = ((float)v + 0.5f - p.c.half_h) / p.c.fy;
+	float g = 0.f;
+	float3 gc;
+	if (dn_dc(p, u + 1, v, st, gc)) { const float3 d = cross3(st.b, gc); g -= rx * d.x + ry * d.y + d.z; }
+	if (dn_dc(p, u - 1, v, st, gc)) { const float3 d = cross3(st.b, gc); g += rx * d.x + ry * d.y + d.z; }
+	if (dn_dc(p, u, v + 1, st, gc)) { const float3 d = cross3(gc, st.a); g -= rx * d.x + ry * d.y + d.z; }
+	if (dn_dc(p, u, v - 1, st, gc)) { const float3 d = cross3(gc, st.a); g += rx * d.x + ry * d.y + d.z; }
+	g *= k;
+	const float dbar = p.D[i] / a;
+	dL_dD[i] += g / a;
+	dL_dA[i] += -g * dbar / a;
+}
+
 }  // namespace
+
+int launch_dn_loss(int W, int H, float tan_fovx, float tan_fovy, const float* depth, const float* alpha, const float* normal, const float* mask,
+                   float lambda, float alpha_min, float max_rel_jump, float* out_dn, double* sums, float* dL_dD, float* dL_dA, float* dL_dN,
+                   cudaStream_t stream, double* partials)
+{
+	const DnPlanes p{normal_cam(W, H, tan_fovx, tan_fovy), depth, alpha, normal, mask, alpha_min, max_rel_jump};
+	const int n = H * W;
+	const int grid = depth_loss_blocks(H, W);
+	const bool det = partials != nullptr;
+	if (!det) PSB_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), stream));
+	(det ? dn_loss_kernel<true> : dn_loss_kernel<false>)<<<grid, 256, 0, stream>>>(p, out_dn, det ? partials : sums);
+	PSB_LAUNCH_OK();
+	if (det) {
+		reduce_partials_kernel<<<1, 256, 0, stream>>>(grid, partials, sums);
+		PSB_LAUNCH_OK();
+	}
+	dn_grad_kernel<<<cdiv(n, 256), 256, 0, stream>>>(p, lambda, sums, dL_dD, dL_dA, dL_dN);
+	PSB_LAUNCH_OK();
+	return 0;
+}
 
 int launch_normal_loss(int H, int W, const float* normal, const float* gt_normal, const float* mask, float lambda_normal, double* sums, float* dL_dN,
                        cudaStream_t stream, double* partials)

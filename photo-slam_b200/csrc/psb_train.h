@@ -120,6 +120,13 @@ inline int depth_loss_blocks(int H, int W) { return min(cdiv(H * W, 256), kNumSM
 // on valid pixels, 0 elsewhere. The launch geometry of launch_depth_loss (same partials).
 int launch_normal_loss(int H, int W, const float* normal, const float* gt_normal, const float* mask, float lambda_normal, double* sums, float* dL_dN,
                        cudaStream_t stream, double* partials);
+// Depth-normal consistency (include/psb200.h, psb_dn) over the depth, opacity and normal planes of one pass whose camera is W x H pixels
+// with tan_fovx / tan_fovy: sums[0] = sum_valid (1 - n_d . N), sums[1] = N_valid (zeroed here); out_dn [3,H,W] or null: n_d; dL_dD,
+// dL_dA [H,W] and dL_dN [3,H,W] are ADDED into (no atomics). The loss pass has the launch geometry of launch_depth_loss (same partials);
+// the gradient pass runs one thread per pixel. No host synchronisation.
+int launch_dn_loss(int W, int H, float tan_fovx, float tan_fovy, const float* depth, const float* alpha, const float* normal, const float* mask,
+                   float lambda, float alpha_min, float max_rel_jump, float* out_dn, double* sums, float* dL_dD, float* dL_dA, float* dL_dN,
+                   cudaStream_t stream, double* partials);
 // launch_loss runs one block per 16 x 16 tile and channel
 inline size_t loss_partials_doubles(int H, int W)
 {

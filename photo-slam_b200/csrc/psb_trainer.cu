@@ -31,8 +31,10 @@ struct psb_trainer {
 	ArenaBuffer<float> depth_buf;  // depth loss: [2][H*W] = rendered depth (when the caller passes no out_depth) | dL/dD
 	ArenaBuffer<float4> normals;   // normal passes: n_i of the visible rows [P], made by the first one
 	ArenaBuffer<float> normal_buf; // normal loss: [6][H*W] = rendered normal plane (when the caller passes no out_normal) | dL/dN
-	ArenaBuffer<double> sums;      // device [6]: sum |I - G|, sum SSIM | depth loss: sum |D - G|, N_valid | normal loss: sum |N - G|, N_valid
-	CudaBuffer<double, 0, true> h_sums;     // pinned [6]
+	ArenaBuffer<float> alpha_buf;  // depth-normal consistency: [2][H*W] = rendered opacity A | dL/dA
+	// device [8]: sum |I - G|, sum SSIM | depth loss: sum |D - G|, N_valid | normal loss: sum |N - G|, N_valid | consistency: sum (1 - n_d . N), N_valid
+	ArenaBuffer<double> sums;
+	CudaBuffer<double, 0, true> h_sums;     // pinned [8]
 	CudaBuffer<uint32_t, 0, true> h_count;  // pinned [4]: instance count of the last call | sticky overflow record {count, first seq, largest count}
 	ArenaBuffer<uint32_t> ovf;     // device [4]: the sticky overflow record (tile_ranges_kernel), collected by psb_trainer_result
 	// what the scratch was last carved for: set when ensure() succeeds, cleared (P = -1) when it fails or the binning chunk is lost
@@ -59,9 +61,11 @@ struct psb_trainer {
 	float last_lambda = 0.2f;
 	float last_lambda_depth = 0.f;
 	float last_lambda_normal = 0.f;
+	float last_lambda_dn = 0.f;
 	bool have_loss = false;
 	bool have_depth_loss = false;  // the last step had a depth term (h_sums[2..3] belong to it)
 	bool have_normal_loss = false; // the last step had a normal term (h_sums[4..5] belong to it)
+	bool have_dn_loss = false;     // the last step had a depth-normal consistency term (h_sums[6..7] belong to it)
 	// tight instance lists: only the tiles a splat can reach get an instance (see preprocess_fwd_kernel); PSB_TIGHT=0 keeps the
 	// reference's full rectangles (A/B measurements only — images and gradients are the same either way)
 	bool tight = !(getenv("PSB_TIGHT") && atoi(getenv("PSB_TIGHT")) == 0);
@@ -101,8 +105,10 @@ namespace {
 // The scratch of a pass of P Gaussians over W x H pixels, each buffer's need stated once (CudaBuffer::grow drains the stream before it
 // frees a buffer the last call's kernels may still use). Any failure leaves t->carved cleared: no call reads this scratch until an
 // ensure() succeeds.
-// normal: a normal pass (n_i, 16-float sink rows and 64-byte deterministic slots); normal_loss: the built-in normal term's planes.
-int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_loss, bool normal = false, bool normal_loss = false)
+// normal: a normal pass (n_i, 16-float sink rows and 64-byte deterministic slots); normal_loss: the built-in normal term's planes;
+// dn_loss: the consistency term's opacity planes.
+int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_loss, bool normal = false, bool normal_loss = false,
+           bool dn_loss = false)
 {
 	const size_t N = (size_t)W * H;
 	// the binning arena grows to P * 6 + 64 Ki instances when it is empty, or when it is smaller and the last pass was over another P
@@ -116,11 +122,12 @@ int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_
 	if (depth_loss) PSB_CUDA_OK(t->depth_buf.grow(2 * N, Fit::at_least, false, stream));
 	if (normal) PSB_CUDA_OK(t->normals.grow((size_t)P, Fit::at_least, false, stream));
 	if (normal_loss) PSB_CUDA_OK(t->normal_buf.grow(6 * N, Fit::at_least, false, stream));
+	if (dn_loss) PSB_CUDA_OK(t->alpha_buf.grow(2 * N, Fit::at_least, false, stream));
 	PSB_CUDA_OK(t->sink.grow((size_t)P * (normal ? 16 : 12), Fit::at_least, true, stream));
 	PSB_CUDA_OK(t->seeds.grow((size_t)P * 20, Fit::at_least, false, stream));
 	if (!t->readback) {
-		PSB_CUDA_OK(t->sums.grow(6, Fit::at_least, false, stream));
-		PSB_CUDA_OK(t->h_sums.grow(6, Fit::at_least, false, stream));
+		PSB_CUDA_OK(t->sums.grow(8, Fit::at_least, false, stream));
+		PSB_CUDA_OK(t->h_sums.grow(8, Fit::at_least, false, stream));
 		PSB_CUDA_OK(t->h_count.grow(4, Fit::at_least, true, stream));
 		PSB_CUDA_OK(t->ovf.grow(4, Fit::at_least, false, stream));
 		const uint32_t init[4] = {0u, 0xFFFFFFFFu, 0u, 0u};
@@ -235,6 +242,25 @@ int check_normal(const psb_normal* n, const char* fn)
 	}
 	if ((n->gt_normal != nullptr) != (n->lambda_normal > 0.f)) {
 		set_error_msg(std::string(fn).append(": gt_normal and lambda_normal > 0 must be given together").c_str());
+		return PSB_ERR_ARG;
+	}
+	return 0;
+}
+
+// NULL: no consistency term. Otherwise lambda_dn finite and > 0, alpha_min in (0, 1] and max_rel_jump finite and > 0.
+int check_dn(const psb_dn* d, const char* fn)
+{
+	if (!d) return 0;
+	if (!std::isfinite(d->lambda_dn) || !(d->lambda_dn > 0.f)) {
+		set_error_msg(std::string(fn).append(": lambda_dn must be finite and > 0").c_str());
+		return PSB_ERR_ARG;
+	}
+	if (!(d->alpha_min > 0.f && d->alpha_min <= 1.f)) {
+		set_error_msg(std::string(fn).append(": alpha_min must lie in (0, 1]").c_str());
+		return PSB_ERR_ARG;
+	}
+	if (!std::isfinite(d->max_rel_jump) || !(d->max_rel_jump > 0.f)) {
+		set_error_msg(std::string(fn).append(": max_rel_jump must be finite and > 0").c_str());
 		return PSB_ERR_ARG;
 	}
 	return 0;
@@ -379,42 +405,49 @@ struct TileBackward {
 int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                          const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
                          bool moments, cudaStream_t stream, TileBackward& out, const psb_exposure* exposure, float* exposure_grad,
-                         const psb_normal* normal = nullptr)
+                         const psb_normal* normal = nullptr, const psb_dn* dn = nullptr)
 {
 	int rc;
 	if (!t || !camera || !step || !background || !gt_image) { set_error_msg("psb_trainer_step: null argument"); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, moments))) return rc;
 	if ((rc = check_filter3d(t, P, "psb_trainer_step"))) return rc;
 	if (step->sh_degree < 0 || step->sh_degree > 3 || step->step < 1) { set_error_msg("psb_trainer_step: sh_degree in 0..3 and step >= 1 required"); return PSB_ERR_ARG; }
+	const size_t npix = (size_t)camera->width * camera->height;
+	// the depth-normal consistency term reads D, A and N of this pass and adds into dL/dD, dL/dA and dL/dN: it forces all three planes
+	const bool dn_loss = dn != nullptr;
 	// depth loss: the depth plane is the caller's out_depth or the context's own; dL/dD lives in the context
 	const bool depth_loss = depth && depth->gt_depth;
+	const bool depth_pass = depth_loss || dn_loss;
 	float* depth_plane = depth ? depth->out_depth : nullptr;
 	float* dL_ddepth = nullptr;
-	if (depth_loss) {
+	if (depth_pass) {
 		if ((rc = ensure(t, P, camera->width, camera->height, stream, true))) return rc;
 		if (!depth_plane) depth_plane = t->depth_buf.get();
-		dL_ddepth = t->depth_buf.get() + (size_t)camera->width * camera->height;
+		dL_ddepth = t->depth_buf.get() + npix;
 	}
 	// normal term: the plane is the caller's out_normal or the context's own; dL/dN lives in the context. An out_normal alone renders the
 	// plane and leaves the backward that of the step without it.
 	const bool normal_loss = normal && normal->gt_normal;
+	const bool normal_grad = normal_loss || dn_loss;
 	float* normal_plane = normal ? normal->out_normal : nullptr;
 	float* dL_dnormal = nullptr;
-	if (normal_loss) {
-		if ((rc = ensure(t, P, camera->width, camera->height, stream, depth_loss, true, true))) return rc;
+	if (normal_grad) {
+		if ((rc = ensure(t, P, camera->width, camera->height, stream, depth_pass, true, true, dn_loss))) return rc;
 		if (!normal_plane) normal_plane = t->normal_buf.get();
-		dL_dnormal = t->normal_buf.get() + 3 * (size_t)camera->width * camera->height;
+		dL_dnormal = t->normal_buf.get() + 3 * npix;
 	}
+	float* alpha_plane = dn_loss ? t->alpha_buf.get() : nullptr;
+	float* dL_dalpha = dn_loss ? t->alpha_buf.get() + npix : nullptr;
 	if (exposure) PSB_CUDA_OK(t->exp_partials.grow(kExposurePartials, Fit::at_least, false, stream));
 	Scratch sc;
 	Camera cam;
-	PassMode mode = pass_mode(t, -1, depth_loss);
+	PassMode mode = pass_mode(t, -1, depth_pass);
 	mode.normals = normal_plane != nullptr;
-	mode.normal = normal_loss;
+	mode.normal = normal_grad;
 	// this pass gets its own tile backward below and its sink rows belong to this call's per-Gaussian stage (or to the _slab calls
 	// that follow a _begin): psb_trainer_backward_pixels must not add a second backward of it (D = -1)
-	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, sc, cam, stream, depth_plane, nullptr, mode, nullptr,
-	                      normal_plane)))
+	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, sc, cam, stream, depth_plane, alpha_plane, mode,
+	                      nullptr, normal_plane)))
 		return rc;
 	const float* image = out_color ? out_color : t->image.get();
 	double* partials = t->deterministic ? t->det_partials.get() : nullptr;
@@ -427,16 +460,28 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	if (normal_loss &&
 	    (rc = launch_normal_loss(cam.H, cam.W, normal_plane, normal->gt_normal, mask, normal->lambda_normal, t->sums.get() + 4, dL_dnormal, stream, partials)))
 		return rc;
+	// the consistency term adds into the gradient planes after the depth and normal terms wrote theirs; planes no term wrote start at 0
+	if (dn_loss) {
+		if (!depth_loss) PSB_CUDA_OK(cudaMemsetAsync(dL_ddepth, 0, npix * sizeof(float), stream));
+		if (!normal_loss) PSB_CUDA_OK(cudaMemsetAsync(dL_dnormal, 0, 3 * npix * sizeof(float), stream));
+		PSB_CUDA_OK(cudaMemsetAsync(dL_dalpha, 0, npix * sizeof(float), stream));
+		if ((rc = launch_dn_loss(cam.W, cam.H, camera->tan_fovx, camera->tan_fovy, depth_plane, alpha_plane, normal_plane, mask, dn->lambda_dn, dn->alpha_min,
+		                         dn->max_rel_jump, dn->out_depth_normal, t->sums.get() + 6, dL_ddepth, dL_dalpha, dL_dnormal, stream, partials)))
+			return rc;
+	}
 	// loss sums -> pinned memory right behind the loss kernel, so the host can read the loss of this iteration (and start
 	// enqueueing the next one) while the backward half is still running
-	PSB_CUDA_OK(cudaMemcpyAsync(t->h_sums.get(), t->sums.get(), (normal_loss ? 6 : depth_loss ? 4 : 2) * sizeof(double), cudaMemcpyDeviceToHost, stream));
+	PSB_CUDA_OK(cudaMemcpyAsync(t->h_sums.get(), t->sums.get(), (dn_loss ? 8 : normal_loss ? 6 : depth_loss ? 4 : 2) * sizeof(double),
+	                            cudaMemcpyDeviceToHost, stream));
 	PSB_CUDA_OK(cudaEventRecord(t->readback, stream));
 	t->last_lambda = step->lambda_dssim;
 	t->last_lambda_depth = depth_loss ? depth->lambda_depth : 0.f;
 	t->last_lambda_normal = normal_loss ? normal->lambda_normal : 0.f;
+	t->last_lambda_dn = dn_loss ? dn->lambda_dn : 0.f;
 	t->have_loss = true;
 	t->have_depth_loss = depth_loss;
 	t->have_normal_loss = normal_loss;
+	t->have_dn_loss = dn_loss;
 	if (exposure) {
 		// dL/dI for the tile backward and the row's update (or gradient), inside stage "loss"; the row moves only after every read of it
 		ExposureUpdate u{exposure->param, exposure->exp_avg, exposure->exp_avg_sq, exposure->step, exposure->lr, step->beta1, step->beta2, step->eps};
@@ -446,7 +491,7 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	}
 	t->mark(5, stream);
 	if (P == 0) return 0;
-	if ((rc = tile_backward(t, P, sc, cam, background, t->dL_dpix.get(), dL_ddepth, nullptr, stream, dL_dnormal))) return rc;
+	if ((rc = tile_backward(t, P, sc, cam, background, t->dL_dpix.get(), dL_ddepth, dL_dalpha, stream, dL_dnormal))) return rc;
 	out.geom = sc.geom;
 	out.cam = cam;
 	return 0;
@@ -797,15 +842,23 @@ int psb_trainer_step_normal(psb_trainer* t, int P, int M, const psb_model* model
                             const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
                             const psb_exposure* exposure, const psb_normal* normal, void* stream_)
 {
+	return psb_trainer_step_dn(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, exposure, normal, nullptr, stream_);
+}
+
+int psb_trainer_step_dn(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                        const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
+                        const psb_exposure* exposure, const psb_normal* normal, const psb_dn* dn, void* stream_)
+{
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
-	const char* fn = normal ? "psb_trainer_step_normal" : exposure ? "psb_trainer_step_exposure" : "psb_trainer_step_depth";
+	const char* fn = dn ? "psb_trainer_step_dn" : normal ? "psb_trainer_step_normal" : exposure ? "psb_trainer_step_exposure" : "psb_trainer_step_depth";
 	if ((rc = check_depth(depth, fn))) return rc;
 	if ((rc = check_exposure(exposure, true, nullptr, fn))) return rc;
 	if ((rc = check_normal(normal, fn))) return rc;
+	if ((rc = check_dn(dn, fn))) return rc;
 	TileBackward tb;
 	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, true, stream, tb, exposure,
-	                               nullptr, normal)) ||
+	                               nullptr, normal, dn)) ||
 	    P == 0)
 		return rc;
 	rc = launch_fused_backward(true, 0, P, train_tensors(model, true), tb.cam, tb.geom, t->sink.get(), t->seeds.get(), to_hyper(step), GradSegments{},
@@ -955,13 +1008,16 @@ static int result_impl(psb_trainer* t, float* out, int n_out, int* num_rendered,
 		const float l1 = (float)(h_sums[0] * inv_n), ss = (float)(h_sums[1] * inv_n);
 		const float dl1 = t->have_depth_loss ? (float)(h_sums[2] / (h_sums[3] > 1.0 ? h_sums[3] : 1.0)) : 0.f;
 		const float nl1 = t->have_normal_loss ? (float)(h_sums[4] / (h_sums[5] > 1.0 ? h_sums[5] : 1.0)) : 0.f;
+		const float dn = t->have_dn_loss ? (float)(h_sums[6] / (h_sums[7] > 1.0 ? h_sums[7] : 1.0)) : 0.f;
 		out[0] = (1.0f - t->last_lambda) * l1 + t->last_lambda * (1.0f - ss);
 		if (t->have_depth_loss) out[0] += t->last_lambda_depth * dl1;
 		if (t->have_normal_loss) out[0] += t->last_lambda_normal * nl1;
+		if (t->have_dn_loss) out[0] += t->last_lambda_dn * dn;
 		out[1] = l1;
 		out[2] = ss;
 		if (n_out > 3) out[3] = dl1;
 		if (n_out > 4) out[4] = nl1;
+		if (n_out > 5) out[5] = dn;
 	}
 	return 0;
 }
@@ -979,6 +1035,11 @@ int psb_trainer_result_depth(psb_trainer* t, float* out4, int* num_rendered, voi
 int psb_trainer_result_normal(psb_trainer* t, float* out5, int* num_rendered, void* stream_)
 {
 	return result_impl(t, out5, 5, num_rendered, stream_);
+}
+
+int psb_trainer_result_dn(psb_trainer* t, float* out6, int* num_rendered, void* stream_)
+{
+	return result_impl(t, out6, 6, num_rendered, stream_);
 }
 
 // Parity/debug export (tests only): per pixel, the final transmittance and the Gaussian index of the last blended splat

@@ -70,6 +70,19 @@ class _Normal(C.Structure):
     _fields_ = [("gt_normal", C.c_void_p), ("lambda_normal", C.c_float), ("out_normal", C.c_void_p)]
 
 
+class _Dn(C.Structure):
+    _fields_ = [("lambda_dn", C.c_float), ("alpha_min", C.c_float), ("max_rel_jump", C.c_float), ("out_depth_normal", C.c_void_p)]
+
+
+def _cdn(lambda_dn, alpha_min, max_rel_jump, out_depth_normal, H, W):
+    """psb_dn for a call, or None when lambda_dn == 0 and there is no out_depth_normal (the call is then the one without the term); the
+    library refuses a lambda_dn, alpha_min or max_rel_jump out of range."""
+    if lambda_dn == 0 and out_depth_normal is None:
+        return None
+    _plane(out_depth_normal, (3, H, W), "out_depth_normal")
+    return _Dn(float(lambda_dn), float(alpha_min), float(max_rel_jump), out_depth_normal.data_ptr() if out_depth_normal is not None else None)
+
+
 def _cnormal(gt_normal, lambda_normal, out_normal, H, W):
     """psb_normal for a call, or None when it has no normal argument (the call is then the one without the normal term)."""
     if gt_normal is None and out_normal is None and not lambda_normal:
@@ -179,6 +192,7 @@ def _bind():
         "psb_trainer_step_depth": call + [Depth, vp],
         "psb_trainer_step_exposure": call + [Depth, Exp, vp],
         "psb_trainer_step_normal": call + [Depth, Exp, P(_Normal), vp],
+        "psb_trainer_step_dn": call + [Depth, Exp, P(_Normal), P(_Dn), vp],
         "psb_trainer_backward": call + [P(vp), vp],
         "psb_trainer_backward_depth": call + [P(vp), Depth, vp],
         "psb_trainer_backward_exposure": call + [P(vp), Depth, Exp, vp, vp],
@@ -188,7 +202,9 @@ def _bind():
         "psb_trainer_result": [vp, P(f), P(i), vp],
         "psb_trainer_result_depth": [vp, P(f), P(i), vp],
         "psb_trainer_result_normal": [vp, P(f), P(i), vp],
+        "psb_trainer_result_dn": [vp, P(f), P(i), vp],
         "psb_depth_normals": [Cam, vp, f, vp, vp],
+        "psb_dn_loss": [Cam, vp, vp, vp, vp, P(_Dn), vp, vp, vp, P(f), vp],
         "psb_trainer_overflow_info": [vp, P(u), P(u), P(u)],
         "psb_trainer_debug_state": [vp, i, i, vp, vp, P(i), vp],
         "psb_trainer_set_profiling": [vp, i],
@@ -1105,7 +1121,8 @@ class GaussianTrainer:
         return self._last_loss
 
     def trainForOneIteration(self, cam, gt_image, mask=None, out_color=None, radii=None, densify_stats=None, gt_depth=None, lambda_depth=0.0,
-                             out_depth=None, exposure_id=None, gt_normal=None, lambda_normal=0.0, out_normal=None):
+                             out_depth=None, exposure_id=None, gt_normal=None, lambda_normal=0.0, out_normal=None, lambda_dn=0.0, dn_alpha_min=0.5,
+                             dn_max_rel_jump=0.05, out_depth_normal=None):
         """Enqueues render -> loss -> backward -> Adam on the current stream (no host sync).
         gt_depth: [H,W] float32 target depth in metres (<= 0: no measurement) trained with weight lambda_depth (> 0) as an L1 term
         over the valid pixels; out_depth: [H,W] float32 tensor that receives the rendered depth.
@@ -1114,10 +1131,15 @@ class GaussianTrainer:
         model.exposure_lr_. out_color stays the raw render; result() reports the compensated loss. One psb_trainer_step_exposure call.
         gt_normal: [3,H,W] float32 view-space unit normals ((0,0,0): no measurement; normals_from_depth) trained with weight lambda_normal
         (> 0) as an L1 term against the rendered normal plane; out_normal: [3,H,W] float32 tensor that receives that plane. With either,
-        the call is psb_trainer_step_normal; result_normal() reports the normal L1."""
+        the call is psb_trainer_step_normal; result_normal() reports the normal L1.
+        lambda_dn > 0: the depth-normal consistency term (psb_dn; no sensor needed, so monocular and stereo keyframes can use it) with
+        weight lambda_dn: the normal of the rendered depth D / A (where A >= dn_alpha_min; dn_max_rel_jump: the depth-edge rule of
+        normals_from_depth) against the rendered normal plane. out_depth_normal: [3,H,W] float32 tensor that receives that depth normal.
+        The call is then psb_trainer_step_dn; result_dn() reports the term. lambda_dn = 0 without out_depth_normal makes the call without it."""
         m = self.model
         depth = _cdepth(gt_depth, lambda_depth, out_depth)
         normal = _cnormal(gt_normal, lambda_normal, out_normal, int(cam["H"]), int(cam["W"]))
+        dn = _cdn(lambda_dn, dn_alpha_min, dn_max_rel_jump, out_depth_normal, int(cam["H"]), int(cam["W"]))
         exposure = None
         if exposure_id is not None:
             k = int(exposure_id)
@@ -1134,15 +1156,22 @@ class GaussianTrainer:
         cm, cc, cs = m._cmodel(live=m.adamLive()), _ccamera(cam), self._cstep(densify_stats)
         args = (*self._call_args(m, cm, cc, cs, gt_image, mask, out_color, radii), C.byref(depth) if depth is not None else None,
                 C.byref(exposure) if exposure is not None else None)
-        if normal is None:
-            rc = self.L.psb_trainer_step_exposure(*args, torch.cuda.current_stream().cuda_stream)
+        stream = torch.cuda.current_stream().cuda_stream
+        if dn is not None:
+            rc = self.L.psb_trainer_step_dn(*args, C.byref(normal) if normal is not None else None, C.byref(dn), stream)
+            fn = "psb_trainer_step_dn"
+        elif normal is not None:
+            rc = self.L.psb_trainer_step_normal(*args, C.byref(normal), stream)
+            fn = "psb_trainer_step_normal"
         else:
-            rc = self.L.psb_trainer_step_normal(*args, C.byref(normal), torch.cuda.current_stream().cuda_stream)
-        _lib.check(rc, "psb_trainer_step_normal" if normal is not None else "psb_trainer_step_exposure")
+            rc = self.L.psb_trainer_step_exposure(*args, stream)
+            fn = "psb_trainer_step_exposure"
+        _lib.check(rc, fn)
         m.step_ += 1
         self._inject_noise()
         self._last = _Call(True, lambda: self.trainForOneIteration(cam, gt_image, mask, out_color, radii, densify_stats, gt_depth, lambda_depth,
-                                                                   out_depth, exposure_id, gt_normal, lambda_normal, out_normal), False)
+                                                                   out_depth, exposure_id, gt_normal, lambda_normal, out_normal, lambda_dn,
+                                                                   dn_alpha_min, dn_max_rel_jump, out_depth_normal), False)
 
     def _call_args(self, m, cm, cc, cs, gt_image, mask, out_color, radii):
         """The leading arguments of a built-in-loss training call (t ... radii)."""
@@ -1171,9 +1200,15 @@ class GaussianTrainer:
         not have reads 0 (psb_trainer_result_normal)."""
         return self._result(5)
 
+    def result_dn(self):
+        """result() with the depth L1, normal L1 and depth-normal consistency of the last step: -> (loss, l1, ssim, depth_l1, normal_l1, dn,
+        num_rendered); a term the step did not have reads 0 (psb_trainer_result_dn)."""
+        return self._result(6)
+
     def _result(self, nterms):
-        out, n = (C.c_float * 5)(), C.c_int()
-        result_fn = self.L.psb_trainer_result_normal if nterms == 5 else self.L.psb_trainer_result_depth
+        out, n = (C.c_float * 6)(), C.c_int()
+        name = {6: "psb_trainer_result_dn", 5: "psb_trainer_result_normal"}.get(nterms, "psb_trainer_result_depth")
+        result_fn = getattr(self.L, name)
         rc = result_fn(self.h, out, C.byref(n), torch.cuda.current_stream().cuda_stream)
         if rc == -4:
             first, count, cur = self._overflow_info()
@@ -1194,11 +1229,11 @@ class GaussianTrainer:
                                     "loss) and repeat the loss and backwardPixels.")
             last.repeat()
             return self._result(nterms)
-        _lib.check(rc, "psb_trainer_result_normal" if nterms == 5 else "psb_trainer_result_depth")
+        _lib.check(rc, name)
         if self._last.callers_loss:
             # the caller's loss: only its value is known (l1, ssim, depth_l1 and normal_l1 are the built-in loss's terms)
             nan = float("nan")
-            out = (float(self._last_loss), nan, nan, nan, nan)
+            out = (float(self._last_loss), nan, nan, nan, nan, nan)
         return (*out[:nterms], n.value)
 
     # ------------------------------------------------------------------------------------------------------------
@@ -1441,15 +1476,19 @@ class DataParallelTrainer(GaussianTrainer):
         self.flat = self.grads.flat
 
     def trainForOneIteration(self, cam, gt_image, mask=None, out_color=None, radii=None, densify_stats=None, gt_depth=None, lambda_depth=0.0,
-                             out_depth=None, exposure_id=None, gt_normal=None, lambda_normal=0.0, out_normal=None):
+                             out_depth=None, exposure_id=None, gt_normal=None, lambda_normal=0.0, out_normal=None, lambda_dn=0.0, dn_alpha_min=0.5,
+                             dn_max_rel_jump=0.05, out_depth_normal=None):
         """Depth arguments as in GaussianTrainer, on every path: "p2p" (psb_dp_step_depth), the slab pipeline
         (psb_trainer_backward_begin_depth) and the flat "nccl" path (psb_trainer_backward_depth). Each rank passes its own view's
         target or none: ranks with and without a depth term may train in the same step. exposure_id and the normal arguments must be
-        None."""
+        None, and lambda_dn 0."""
         if gt_normal is not None or out_normal is not None or lambda_normal:
             raise NotImplementedError("DataParallelTrainer: the normal term is not wired into the data-parallel steps (the NVLink push "
                                       "backward and the slab pipeline carry 12-float sink rows); train with normals on one GPU through "
                                       "GaussianTrainer")
+        if lambda_dn or out_depth_normal is not None:
+            raise NotImplementedError("DataParallelTrainer: the depth-normal consistency term is not wired into the data-parallel steps (it "
+                                      "needs the normal plane and its 16-float sink rows); train with it on one GPU through GaussianTrainer")
         if exposure_id is not None:
             raise NotImplementedError("DataParallelTrainer: exposure compensation is not wired into the data-parallel steps: the per-keyframe "
                                       "exposure table would have to be replicated across the ranks (each rank's row updates gathered to "
@@ -1553,6 +1592,28 @@ def normals_from_depth(cam, depth, max_rel_jump=0.05, out=None):
     _lib.check(L.psb_depth_normals(C.byref(c), depth.data_ptr(), float(max_rel_jump), out.data_ptr(), torch.cuda.current_stream().cuda_stream),
                "psb_depth_normals")
     return out
+
+
+def _dn_loss(cam, depth, alpha, normal, mask=None, lambda_dn=1.0, alpha_min=0.5, max_rel_jump=0.05, grads=None, out_depth_normal=None):
+    """The depth-normal consistency term on caller planes through psb_dn_loss (synchronises): depth, alpha [H,W], normal [3,H,W] and mask
+    [H,W] or None seen by `cam`. grads = (dL_ddepth, dL_dalpha, dL_dnormal) are added into (zeros when None); out_depth_normal [3,H,W]
+    receives n_d. -> (dn, N_valid, grads)."""
+    H, W = int(cam["H"]), int(cam["W"])
+    for t, shape, name in ((depth, (H, W), "depth"), (alpha, (H, W), "alpha"), (normal, (3, H, W), "normal"), (mask, (H, W), "mask"),
+                           (out_depth_normal, (3, H, W), "out_depth_normal")):
+        _plane(t, shape, name)
+    if grads is None:
+        grads = (torch.zeros_like(depth), torch.zeros_like(alpha), torch.zeros_like(normal))
+    for t, shape, name in zip(grads, ((H, W), (H, W), (3, H, W)), ("dL_ddepth", "dL_dalpha", "dL_dnormal")):
+        _plane(t, shape, name)
+    c = _Camera()
+    c.tan_fovx, c.tan_fovy, c.width, c.height = float(cam["tanfovx"]), float(cam["tanfovy"]), W, H
+    dn = _cdn(lambda_dn, alpha_min, max_rel_jump, out_depth_normal, H, W)
+    out = (C.c_float * 2)()
+    L = _bind()
+    _lib.check(L.psb_dn_loss(C.byref(c), depth.data_ptr(), alpha.data_ptr(), normal.data_ptr(), mask.data_ptr() if mask is not None else None,
+                             C.byref(dn), *(g.data_ptr() for g in grads), out, torch.cuda.current_stream().cuda_stream), "psb_dn_loss")
+    return float(out[0]), int(out[1]), grads
 
 
 def fused_loss(image, gt, mask=None, lambda_dssim=0.2, want_grad=True):
