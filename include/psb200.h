@@ -474,6 +474,56 @@ int psb_trainer_result_dn(psb_trainer* t, float* out6, int* num_rendered, void* 
  * psb_depth_normals rejects and the dn values psb_trainer_step_dn rejects. Synchronises the stream; the same result every run. */
 int psb_dn_loss(const psb_camera* camera, const float* depth, const float* alpha, const float* normal, const float* mask, const psb_dn* dn,
                 float* dL_ddepth, float* dL_dalpha, float* dL_dnormal, float* out2_host, void* stream);
+/* ------------------------------------------------------------------------------------------------
+ * Depth distortion (2DGS): how many Gaussians along a ray share a pixel's weight. Colour alone can explain a view with a haze of
+ * half-transparent Gaussians spread in depth; this term pulls each ray's weight onto one depth. It needs no sensor and no target.
+ * Second depth moment: M(p) = sum_i z_i^2 alpha_i T_i, with z_i the view-space depth D uses and alpha_i, T_i exactly those of the colour
+ *   (same blend order, culls and termination), no background term; un-normalised like D. Rendering it leaves colour, D, A, N, radii and
+ *   the pass's scratch bit-identical. With A = 1 - T_final and D = sum_i z_i alpha_i T_i, sqrt(max(M / A - (D / A)^2, 0)) is the pixel's
+ *   depth spread: a per-pixel uncertainty of the rendered depth.
+ * Distortion of a pixel: dist_p = A M - D^2. With A = sum_i w_i (w_i = alpha_i T_i) this is (1/2) sum_i sum_j w_i w_j (z_i - z_j)^2, 2DGS's
+ *   pairwise term in its squared form with a pair counted once. 2DGS measures z in NDC; this term uses view-space z (it reuses D and needs
+ *   one accumulator, not two), so its units are depth^2 and its weight scales with the square of the scene's depth.
+ *   dist_p is formed in double from the float planes (the products are exact; one rounding). The planes themselves carry float32
+ *   rounding, and A M - D^2 cancels: relative to the spread sigma^2 = dist_p / A^2, the error is of order eps_float (Dbar / sigma)^2,
+ *   Dbar = D / A: for Gaussians within 1e-3 Dbar of each other a pixel's distortion is known to about 6 %.
+ * Loss: valid(p) = mask[0,p] != 0 with a mask, every pixel without one; dist = sum_valid dist_p / max(N_valid, 1); L += lambda_dist dist.
+ * Gradients: k = lambda_dist / max(N_valid, 1) (a float32 IEEE division on the device; N_valid counted there); on valid pixels
+ *   dL/dA += k M, dL/dD += (-2k) D and dL/dM = k A (0 elsewhere), each one float32 product and one sum, no contraction. The term adds after
+ *   the depth, normal and consistency terms have written their gradients; planes no term wrote start at 0. In the tile backward M is one
+ *   more channel with per-Gaussian value z_i^2: z_i^2 dL/dM joins dL/dalpha_i, and dL/dz_i gains sum_p alpha_i T_i 2 z_i dL/dM, so per
+ *   Gaussian dL/dz_i = 2k sum_p w_i (A z_i - D) (2DGS's gradient). The term reaches positions, opacity and shape, and the densification
+ *   statistics. No float atomics on the planes; in deterministic mode the loss sums are reduced in a fixed order. Anti-aliasing, the 3D
+ *   filter and exposure compose unchanged (exposure acts on colour only). The data-parallel calls, the _begin / _slab halves and the
+ *   rasterizer operator take no distortion term.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct psb_dist {
+	float lambda_dist;   /* finite, >= 0; 0 with out_depth2: the plane alone */
+	float* out_depth2;   /* [H,W] device or NULL: the second depth moment M */
+} psb_dist;
+/* psb_trainer_forward_normal plus out_depth2 [H,W] (device) = M; NULL is exactly psb_trainer_forward_normal. The other outputs are
+ * bit-identical to psb_trainer_forward_normal's; out_depth may be NULL. A pass with the plane may be followed by
+ * psb_trainer_backward_pixels_moment with a dL_ddepth2. */
+int psb_trainer_forward_moment(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                               const float* background, int sh_degree, float* out_color, int* radii, float* out_depth, float* out_alpha,
+                               float* out_normal, float* out_depth2, unsigned* pass, void* stream);
+/* psb_trainer_backward_pixels_normal plus dL_ddepth2 [H,W] (device), the gradient w.r.t. M; NULL is exactly
+ * psb_trainer_backward_pixels_normal. pixel_grads->dL_ddepth may be NULL alongside it. PSB_ERR_ARG, before any CUDA call, for everything
+ * psb_trainer_backward_pixels_normal rejects and for a dL_ddepth2 after a pass that rendered no second depth moment. */
+int psb_trainer_backward_pixels_moment(psb_trainer* t, unsigned pass, int P, int M, const psb_model* model, const psb_camera* camera,
+                                       const float* background, const psb_pixel_grads* pixel_grads, const float* dL_dnormal,
+                                       const float* dL_ddepth2, const psb_step* step, float* const* grads, void* stream);
+/* psb_trainer_step_dn plus the distortion term (dist == NULL: exactly psb_trainer_step_dn). With lambda_dist > 0 the pass renders D, A
+ * and M (in the context's own planes where the caller passes none), and N too when a normal or consistency term is on. An out_depth2
+ * alone (lambda_dist = 0) renders the plane and trains as without it. PSB_ERR_ARG, before any CUDA call and with the model untouched, for
+ * everything psb_trainer_step_dn rejects and a lambda_dist that is negative or not finite. A step that overflows the binning arena is a
+ * no-op: repeating it applies the term once. */
+int psb_trainer_step_dist(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                          const float* background, const float* gt_image, const float* mask, const psb_step* step,
+                          float* out_color, int* radii, const psb_depth* depth, const psb_exposure* exposure, const psb_normal* normal,
+                          const psb_dn* dn, const psb_dist* dist, void* stream);
+/* psb_trainer_result with out7 = {loss, l1, ssim, depth_l1, normal_l1, dn, dist} (0 for a term the last step did not have). */
+int psb_trainer_result_dist(psb_trainer* t, float* out7, int* num_rendered, void* stream);
 
 /* model->adam_live[i] = 1 if any of the 118 moments of row i is non-zero, else 0: one pass over the moments. Restores the
  * psb_model.adam_live contract after moments were written by anything but psb_trainer_step. Asynchronous on `stream`. */

@@ -110,7 +110,9 @@ int launch_render_forward(const Camera& cam, const uint2* ranges, const uint32_t
                           float* out_alpha = nullptr /* [H,W]: also write the accumulated opacity 1 - final_T (opacity variant) */,
                           const ScoreSink* score = nullptr /* also add the contribution scores (score variant; no depth or opacity) */,
                           const float4* normals = nullptr /* [P] n_i of the pass (launch_normals); with out_normal only */,
-                          float* out_normal = nullptr /* [3,H,W]: also render the normal plane (normal variant; no score) */);
+                          float* out_normal = nullptr /* [3,H,W]: also render the normal plane (normal variant; no score) */,
+                          float* out_depth2 = nullptr /* [H,W]: also render the second depth moment sum z^2 alpha T (moment variant, which
+                                                         is a depth variant: out_depth may then be null; no score) */);
 // n_i of include/psb200.h (the camera-facing shortest axis in view space) of every visible row of the pass -> normals [P]; raw trainer
 // parameters (xyz, scaling, rotation), after launch_preprocess (tile_info says which rows are visible)
 int launch_normals(int P, const float* xyz, const float* scaling, const float* rotation, const Camera& cam, const uint4* tile_info, float4* normals,
@@ -122,7 +124,9 @@ int launch_render_backward(const Camera& cam, const uint2* ranges, const uint32_
                            const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, const GradSink& sink,
                            cudaStream_t stream, const float* dL_ddepth = nullptr, const DetSlots* det = nullptr, const float* dL_dalpha = nullptr,
                            const float4* normals = nullptr /* [P] n_i of the forward pass; with dL_dnormal only */,
-                           const float* dL_dnormal = nullptr /* [3,H,W]: normal variant, packed 16-float sink rows, 64-byte deterministic slots */);
+                           const float* dL_dnormal = nullptr /* [3,H,W]: normal variant, packed 16-float sink rows, 64-byte deterministic slots */,
+                           const float* dL_ddepth2 = nullptr /* [H,W]: moment variant (a depth variant; dL_ddepth may be null), packed sink
+                                                                only; its dL/dz (slot 11) includes 2 z dL/dM */);
 // dL_dz [P] (non-null: depth variant): dL/dmean3D += dL/dz (V[2], V[6], V[10]) for every visible Gaussian
 // aa_dL_dopacity [P] (non-null: AA variant, after an anti-aliased forward): holds dL/do' on entry, dL/do on return
 int launch_preprocess_backward(const GaussIn& in, const Camera& cam, const GeomState& geom, const float* dL_dmean2D, int mean2D_stride,

@@ -152,6 +152,35 @@ __global__ void __launch_bounds__(256) reduce_partials_kernel(int n, const doubl
 	if (tid == 0) { sums[0] = s[0][0]; sums[1] = s[1][0]; }
 }
 
+// The double sums of a block (the distortion term): as above, with the block's value in double.
+template <bool DET>
+__device__ __forceinline__ void block_sums_out(double a, double b, double* __restrict__ sums)
+{
+	if (threadIdx.x != 0) return;
+	if (DET) {
+		const size_t blk = ((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+		sums[2 * blk] = a;
+		sums[2 * blk + 1] = b;
+	} else {
+		atomicAdd(&sums[0], a);
+		atomicAdd(&sums[1], b);
+	}
+}
+
+__device__ __forceinline__ double block_sum_256(double v, double* s_red)
+{
+#pragma unroll
+	for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	__syncthreads();
+	if (lane == 0) s_red[warp] = v;
+	__syncthreads();
+	double t = 0.0;
+#pragma unroll
+	for (int i = 0; i < 8; i++) t += s_red[i];
+	return t;
+}
+
 // EXP: evaluated at x = X = mask * I' (see loss_fwd_kernel); dL_dimg then receives g = dL/dI' (mask factor applied), which
 // exposure_mix_kernel turns into dL/dI.
 template <bool EXP>
@@ -475,7 +504,64 @@ __global__ void __launch_bounds__(256) dn_grad_kernel(DnPlanes p, float lambda, 
 	dL_dA[i] += -g * dbar / a;
 }
 
+// Depth distortion, pass 1 (the geometry of depth_loss_kernel): per valid pixel A M - D^2 in double (the products of two floats are
+// exact there, so the difference is rounded once); block sums of it and of the valid count -> sums[0..1] (DET: the block's partials).
+template <bool DET>
+__global__ void __launch_bounds__(256) dist_loss_kernel(int n, const float* __restrict__ D, const float* __restrict__ A, const float* __restrict__ M,
+                                                        const float* __restrict__ mask, double* __restrict__ sums)
+{
+	__shared__ double s_red[8];
+	double acc = 0.0, cnt = 0.0;
+	for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) {
+		if (!mask || mask[i] != 0.f) {
+			const double d = (double)D[i];
+			acc += __dadd_rn(__dmul_rn((double)A[i], (double)M[i]), -__dmul_rn(d, d));
+			cnt += 1.0;
+		}
+	}
+	const double tacc = block_sum_256(acc, s_red);
+	const double tcnt = block_sum_256(cnt, s_red);
+	block_sums_out<DET>(tacc, tcnt, sums);
+}
+
+// Depth distortion, pass 2: k = lambda / max(N_valid, 1) read on the device (an IEEE float division); on valid pixels dL/dA += k M and
+// dL/dD += (-2k) D, and dL/dM = k A (0 elsewhere). Explicit roundings, no contraction: torch float32 reproduces the planes bit for bit.
+__global__ void __launch_bounds__(256) dist_grad_kernel(int n, float lambda, const double* __restrict__ sums, const float* __restrict__ D,
+                                                        const float* __restrict__ A, const float* __restrict__ M, const float* __restrict__ mask,
+                                                        float* __restrict__ dL_dD, float* __restrict__ dL_dA, float* __restrict__ dL_dM)
+{
+	const float k = __fdiv_rn(lambda, (float)fmax(sums[1], 1.0));
+	const float m2k = __fmul_rn(-2.f, k);
+	for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) {
+		float gM = 0.f;
+		if (!mask || mask[i] != 0.f) {
+			dL_dA[i] = __fadd_rn(dL_dA[i], __fmul_rn(k, M[i]));
+			dL_dD[i] = __fadd_rn(dL_dD[i], __fmul_rn(m2k, D[i]));
+			gM = __fmul_rn(k, A[i]);
+		}
+		dL_dM[i] = gM;
+	}
+}
+
 }  // namespace
+
+int launch_dist_loss(int H, int W, const float* depth, const float* alpha, const float* depth2, const float* mask, float lambda, double* sums,
+                     float* dL_dD, float* dL_dA, float* dL_dM, cudaStream_t stream, double* partials)
+{
+	const int n = H * W;
+	const int grid = depth_loss_blocks(H, W);
+	const bool det = partials != nullptr;
+	if (!det) PSB_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), stream));
+	(det ? dist_loss_kernel<true> : dist_loss_kernel<false>)<<<grid, 256, 0, stream>>>(n, depth, alpha, depth2, mask, det ? partials : sums);
+	PSB_LAUNCH_OK();
+	if (det) {
+		reduce_partials_kernel<<<1, 256, 0, stream>>>(grid, partials, sums);
+		PSB_LAUNCH_OK();
+	}
+	dist_grad_kernel<<<grid, 256, 0, stream>>>(n, lambda, sums, depth, alpha, depth2, mask, dL_dD, dL_dA, dL_dM);
+	PSB_LAUNCH_OK();
+	return 0;
+}
 
 int launch_dn_loss(int W, int H, float tan_fovx, float tan_fovy, const float* depth, const float* alpha, const float* normal, const float* mask,
                    float lambda, float alpha_min, float max_rel_jump, float* out_dn, double* sums, float* dL_dD, float* dL_dA, float* dL_dN,

@@ -38,6 +38,7 @@ struct PassMode {
 	const float* f3d;              // psb_trainer_set_filter3d: the 3D smoothing filter [P] the pass applies, or null (the variants without it)
 	bool normals = false;          // the forward wrote n_i of its visible rows (launch_normals): a normal gradient may follow it
 	bool normal = false;           // the sink rows are 16 floats and slots 12..14 hold dL/dn (render_bwd_normal_kernel, MODE_NORMAL)
+	bool moment = false;           // the forward wrote the second depth moment M (render_fwd_moment_kernel): a dL/dM may follow it
 };
 // lambda / P of the opacity and scale regularisers for the rows a per-Gaussian backward updates; both 0 = no regulariser
 struct RegCoef {
@@ -127,6 +128,12 @@ int launch_normal_loss(int H, int W, const float* normal, const float* gt_normal
 int launch_dn_loss(int W, int H, float tan_fovx, float tan_fovy, const float* depth, const float* alpha, const float* normal, const float* mask,
                    float lambda, float alpha_min, float max_rel_jump, float* out_dn, double* sums, float* dL_dD, float* dL_dA, float* dL_dN,
                    cudaStream_t stream, double* partials);
+// Depth distortion (include/psb200.h, psb_dist) over the depth D, opacity A and second-moment M planes [H,W] of one pass, mask [H,W] or
+// null: sums[0] = sum_valid (A M - D^2) (each term formed in double), sums[1] = N_valid (zeroed here). With k = lambda / max(N_valid, 1)
+// (a float division on the device): dL_dA += k M and dL_dD += -2k D on valid pixels (added into, no atomics), and dL_dM = k A there, 0
+// elsewhere (written). The launch geometry of launch_depth_loss (same partials). No host synchronisation.
+int launch_dist_loss(int H, int W, const float* depth, const float* alpha, const float* depth2, const float* mask, float lambda, double* sums,
+                     float* dL_dD, float* dL_dA, float* dL_dM, cudaStream_t stream, double* partials);
 // launch_loss runs one block per 16 x 16 tile and channel
 inline size_t loss_partials_doubles(int H, int W)
 {

@@ -31,10 +31,12 @@ struct psb_trainer {
 	ArenaBuffer<float> depth_buf;  // depth loss: [2][H*W] = rendered depth (when the caller passes no out_depth) | dL/dD
 	ArenaBuffer<float4> normals;   // normal passes: n_i of the visible rows [P], made by the first one
 	ArenaBuffer<float> normal_buf; // normal loss: [6][H*W] = rendered normal plane (when the caller passes no out_normal) | dL/dN
-	ArenaBuffer<float> alpha_buf;  // depth-normal consistency: [2][H*W] = rendered opacity A | dL/dA
-	// device [8]: sum |I - G|, sum SSIM | depth loss: sum |D - G|, N_valid | normal loss: sum |N - G|, N_valid | consistency: sum (1 - n_d . N), N_valid
+	ArenaBuffer<float> alpha_buf;  // depth-normal consistency, depth distortion: [2][H*W] = rendered opacity A | dL/dA
+	ArenaBuffer<float> moment_buf; // depth distortion: [2][H*W] = second depth moment M (when the caller passes no out_depth2) | dL/dM
+	// device [10]: sum |I - G|, sum SSIM | depth loss: sum |D - G|, N_valid | normal loss: sum |N - G|, N_valid | consistency: sum (1 - n_d . N), N_valid
+	//   | distortion: sum (A M - D^2), N_valid
 	ArenaBuffer<double> sums;
-	CudaBuffer<double, 0, true> h_sums;     // pinned [8]
+	CudaBuffer<double, 0, true> h_sums;     // pinned [10]
 	CudaBuffer<uint32_t, 0, true> h_count;  // pinned [4]: instance count of the last call | sticky overflow record {count, first seq, largest count}
 	ArenaBuffer<uint32_t> ovf;     // device [4]: the sticky overflow record (tile_ranges_kernel), collected by psb_trainer_result
 	// what the scratch was last carved for: set when ensure() succeeds, cleared (P = -1) when it fails or the binning chunk is lost
@@ -62,10 +64,12 @@ struct psb_trainer {
 	float last_lambda_depth = 0.f;
 	float last_lambda_normal = 0.f;
 	float last_lambda_dn = 0.f;
+	float last_lambda_dist = 0.f;
 	bool have_loss = false;
 	bool have_depth_loss = false;  // the last step had a depth term (h_sums[2..3] belong to it)
 	bool have_normal_loss = false; // the last step had a normal term (h_sums[4..5] belong to it)
 	bool have_dn_loss = false;     // the last step had a depth-normal consistency term (h_sums[6..7] belong to it)
+	bool have_dist_loss = false;   // the last step had a depth distortion term (h_sums[8..9] belong to it)
 	// tight instance lists: only the tiles a splat can reach get an instance (see preprocess_fwd_kernel); PSB_TIGHT=0 keeps the
 	// reference's full rectangles (A/B measurements only — images and gradients are the same either way)
 	bool tight = !(getenv("PSB_TIGHT") && atoi(getenv("PSB_TIGHT")) == 0);
@@ -106,9 +110,9 @@ namespace {
 // frees a buffer the last call's kernels may still use). Any failure leaves t->carved cleared: no call reads this scratch until an
 // ensure() succeeds.
 // normal: a normal pass (n_i, 16-float sink rows and 64-byte deterministic slots); normal_loss: the built-in normal term's planes;
-// dn_loss: the consistency term's opacity planes.
+// dn_loss: the opacity planes of the consistency and distortion terms; dist_loss: the distortion term's moment planes.
 int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_loss, bool normal = false, bool normal_loss = false,
-           bool dn_loss = false)
+           bool dn_loss = false, bool dist_loss = false)
 {
 	const size_t N = (size_t)W * H;
 	// the binning arena grows to P * 6 + 64 Ki instances when it is empty, or when it is smaller and the last pass was over another P
@@ -123,11 +127,12 @@ int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_
 	if (normal) PSB_CUDA_OK(t->normals.grow((size_t)P, Fit::at_least, false, stream));
 	if (normal_loss) PSB_CUDA_OK(t->normal_buf.grow(6 * N, Fit::at_least, false, stream));
 	if (dn_loss) PSB_CUDA_OK(t->alpha_buf.grow(2 * N, Fit::at_least, false, stream));
+	if (dist_loss) PSB_CUDA_OK(t->moment_buf.grow(2 * N, Fit::at_least, false, stream));
 	PSB_CUDA_OK(t->sink.grow((size_t)P * (normal ? 16 : 12), Fit::at_least, true, stream));
 	PSB_CUDA_OK(t->seeds.grow((size_t)P * 20, Fit::at_least, false, stream));
 	if (!t->readback) {
-		PSB_CUDA_OK(t->sums.grow(8, Fit::at_least, false, stream));
-		PSB_CUDA_OK(t->h_sums.grow(8, Fit::at_least, false, stream));
+		PSB_CUDA_OK(t->sums.grow(10, Fit::at_least, false, stream));
+		PSB_CUDA_OK(t->h_sums.grow(10, Fit::at_least, false, stream));
 		PSB_CUDA_OK(t->h_count.grow(4, Fit::at_least, true, stream));
 		PSB_CUDA_OK(t->ovf.grow(4, Fit::at_least, false, stream));
 		const uint32_t init[4] = {0u, 0xFFFFFFFFu, 0u, 0u};
@@ -266,6 +271,17 @@ int check_dn(const psb_dn* d, const char* fn)
 	return 0;
 }
 
+// NULL: no distortion term. Otherwise lambda_dist finite and >= 0 (0: the plane alone, when out_depth2 is given).
+int check_dist(const psb_dist* d, const char* fn)
+{
+	if (!d) return 0;
+	if (!std::isfinite(d->lambda_dist) || d->lambda_dist < 0.f) {
+		set_error_msg(std::string(fn).append(": lambda_dist must be finite and >= 0").c_str());
+		return PSB_ERR_ARG;
+	}
+	return 0;
+}
+
 // NULL: no exposure. Otherwise a row (param), a finite lr >= 0 and, for a step (`adam`), the moments and the device step count; for the
 // gradient mode a gradient output.
 int check_exposure(const psb_exposure* e, bool adam, const float* grad, const char* fn)
@@ -326,9 +342,10 @@ int refuse_filter3d(const psb_trainer* t, const char* fn)
 // also writes the expected depth there; out_alpha != NULL: the opacity variant also writes 1 - final_T there. The pass is recorded as
 // `mode`, with D = -1 until it has been binned. score != NULL: the score variant also adds the contribution scores there (no depth or
 // opacity plane). mode.normals: n_i of the visible rows -> t->normals, and the normal variant writes the normal plane to out_normal.
+// out_depth2 != NULL (mode.moment): the moment variant also writes the second depth moment there (out_depth may then be NULL).
 int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, const psb_camera* camera, const float* background,
                 float* out_color, int* radii, Scratch& sc, Camera& cam, cudaStream_t stream, float* out_depth, float* out_alpha, const PassMode& mode,
-                const ScoreSink* score = nullptr, float* out_normal = nullptr)
+                const ScoreSink* score = nullptr, float* out_normal = nullptr, float* out_depth2 = nullptr)
 {
 	int rc;
 	t->pass = mode;
@@ -355,16 +372,17 @@ int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, con
 	PSB_CUDA_OK(cudaMemcpyAsync(t->h_count.get() + 1, t->ovf.get(), 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
 	PSB_CUDA_OK(cudaEventRecord(t->readback, stream));
 	rc = launch_render_forward(cam, img.ranges, bin.inst[sorted_slot(cam.W, cam.H)], geom.rec, background, out_color ? out_color : t->image.get(), img.final_T,
-	                           img.n_contrib, stream, out_depth, out_alpha, score, mode.normals ? t->normals.get() : nullptr, out_normal);
+	                           img.n_contrib, stream, out_depth, out_alpha, score, mode.normals ? t->normals.get() : nullptr, out_normal, out_depth2);
 	t->mark(4, stream);
 	return rc;
 }
 
 // Stage 3 of every pass: the tile backward of the context's last forward pass (scratch sc, camera cam, mode t->pass) on per-pixel
 // gradients -> the packed sink rows (dL_ddepth: also dL/dz in slot 11; dL_dalpha: the opacity variant; dL_dnormal: the normal variant,
-// 16-float rows with dL/dn in slots 12..14, after a pass with mode.normals). P > 0.
+// 16-float rows with dL/dn in slots 12..14, after a pass with mode.normals; dL_ddepth2: the moment variant, its 2 z dL/dM in slot 11, after
+// a pass with mode.moment). P > 0.
 int tile_backward(psb_trainer* t, int P, const Scratch& sc, const Camera& cam, const float* background, const float* dL_dpix, const float* dL_ddepth,
-                  const float* dL_dalpha, cudaStream_t stream, const float* dL_dnormal = nullptr)
+                  const float* dL_dalpha, cudaStream_t stream, const float* dL_dnormal = nullptr, const float* dL_ddepth2 = nullptr)
 {
 	float* const rows = t->sink.get();
 	GradSink sink;
@@ -386,7 +404,7 @@ int tile_backward(psb_trainer* t, int P, const Scratch& sc, const Camera& cam, c
 	int rc;
 	if ((rc = launch_render_backward(cam, sc.img.ranges, sc.bin.inst[sorted_slot(cam.W, cam.H)], sc.geom.rec, background, sc.img.final_T, sc.img.n_contrib,
 	                                 dL_dpix, sink, stream, dL_ddepth, t->pass.det ? &det : nullptr, dL_dalpha, dL_dnormal ? t->normals.get() : nullptr,
-	                                 dL_dnormal)))
+	                                 dL_dnormal, dL_ddepth2)))
 		return rc;
 	t->mark(6, stream);
 	return 0;
@@ -405,7 +423,7 @@ struct TileBackward {
 int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                          const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
                          bool moments, cudaStream_t stream, TileBackward& out, const psb_exposure* exposure, float* exposure_grad,
-                         const psb_normal* normal = nullptr, const psb_dn* dn = nullptr)
+                         const psb_normal* normal = nullptr, const psb_dn* dn = nullptr, const psb_dist* dist = nullptr)
 {
 	int rc;
 	if (!t || !camera || !step || !background || !gt_image) { set_error_msg("psb_trainer_step: null argument"); return PSB_ERR_ARG; }
@@ -415,9 +433,11 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	const size_t npix = (size_t)camera->width * camera->height;
 	// the depth-normal consistency term reads D, A and N of this pass and adds into dL/dD, dL/dA and dL/dN: it forces all three planes
 	const bool dn_loss = dn != nullptr;
+	// the distortion term reads D, A and M of this pass, adds into dL/dD and dL/dA and writes dL/dM: it forces those three planes
+	const bool dist_loss = dist && dist->lambda_dist > 0.f;
 	// depth loss: the depth plane is the caller's out_depth or the context's own; dL/dD lives in the context
 	const bool depth_loss = depth && depth->gt_depth;
-	const bool depth_pass = depth_loss || dn_loss;
+	const bool depth_pass = depth_loss || dn_loss || dist_loss;
 	float* depth_plane = depth ? depth->out_depth : nullptr;
 	float* dL_ddepth = nullptr;
 	if (depth_pass) {
@@ -436,18 +456,28 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 		if (!normal_plane) normal_plane = t->normal_buf.get();
 		dL_dnormal = t->normal_buf.get() + 3 * npix;
 	}
-	float* alpha_plane = dn_loss ? t->alpha_buf.get() : nullptr;
-	float* dL_dalpha = dn_loss ? t->alpha_buf.get() + npix : nullptr;
+	// distortion term: the moment plane is the caller's out_depth2 or the context's own; dL/dM lives in the context. An out_depth2 alone
+	// renders the plane and leaves the backward that of the step without it.
+	float* depth2_plane = dist ? dist->out_depth2 : nullptr;
+	float* dL_ddepth2 = nullptr;
+	if (dist_loss) {
+		if ((rc = ensure(t, P, camera->width, camera->height, stream, true, normal_grad, normal_grad, true, true))) return rc;
+		if (!depth2_plane) depth2_plane = t->moment_buf.get();
+		dL_ddepth2 = t->moment_buf.get() + npix;
+	}
+	float* alpha_plane = dn_loss || dist_loss ? t->alpha_buf.get() : nullptr;
+	float* dL_dalpha = dn_loss || dist_loss ? t->alpha_buf.get() + npix : nullptr;
 	if (exposure) PSB_CUDA_OK(t->exp_partials.grow(kExposurePartials, Fit::at_least, false, stream));
 	Scratch sc;
 	Camera cam;
 	PassMode mode = pass_mode(t, -1, depth_pass);
 	mode.normals = normal_plane != nullptr;
 	mode.normal = normal_grad;
+	mode.moment = depth2_plane != nullptr;
 	// this pass gets its own tile backward below and its sink rows belong to this call's per-Gaussian stage (or to the _slab calls
 	// that follow a _begin): psb_trainer_backward_pixels must not add a second backward of it (D = -1)
 	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, sc, cam, stream, depth_plane, alpha_plane, mode,
-	                      nullptr, normal_plane)))
+	                      nullptr, normal_plane, depth2_plane)))
 		return rc;
 	const float* image = out_color ? out_color : t->image.get();
 	double* partials = t->deterministic ? t->det_partials.get() : nullptr;
@@ -469,19 +499,30 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 		                         dn->max_rel_jump, dn->out_depth_normal, t->sums.get() + 6, dL_ddepth, dL_dalpha, dL_dnormal, stream, partials)))
 			return rc;
 	}
+	// the distortion term adds into dL/dD and dL/dA after the depth, normal and consistency terms wrote theirs (planes no term wrote start
+	// at 0) and writes dL/dM
+	if (dist_loss) {
+		if (!depth_loss && !dn_loss) PSB_CUDA_OK(cudaMemsetAsync(dL_ddepth, 0, npix * sizeof(float), stream));
+		if (!dn_loss) PSB_CUDA_OK(cudaMemsetAsync(dL_dalpha, 0, npix * sizeof(float), stream));
+		if ((rc = launch_dist_loss(cam.H, cam.W, depth_plane, alpha_plane, depth2_plane, mask, dist->lambda_dist, t->sums.get() + 8, dL_ddepth, dL_dalpha,
+		                           dL_ddepth2, stream, partials)))
+			return rc;
+	}
 	// loss sums -> pinned memory right behind the loss kernel, so the host can read the loss of this iteration (and start
 	// enqueueing the next one) while the backward half is still running
-	PSB_CUDA_OK(cudaMemcpyAsync(t->h_sums.get(), t->sums.get(), (dn_loss ? 8 : normal_loss ? 6 : depth_loss ? 4 : 2) * sizeof(double),
+	PSB_CUDA_OK(cudaMemcpyAsync(t->h_sums.get(), t->sums.get(), (dist_loss ? 10 : dn_loss ? 8 : normal_loss ? 6 : depth_loss ? 4 : 2) * sizeof(double),
 	                            cudaMemcpyDeviceToHost, stream));
 	PSB_CUDA_OK(cudaEventRecord(t->readback, stream));
 	t->last_lambda = step->lambda_dssim;
 	t->last_lambda_depth = depth_loss ? depth->lambda_depth : 0.f;
 	t->last_lambda_normal = normal_loss ? normal->lambda_normal : 0.f;
 	t->last_lambda_dn = dn_loss ? dn->lambda_dn : 0.f;
+	t->last_lambda_dist = dist_loss ? dist->lambda_dist : 0.f;
 	t->have_loss = true;
 	t->have_depth_loss = depth_loss;
 	t->have_normal_loss = normal_loss;
 	t->have_dn_loss = dn_loss;
+	t->have_dist_loss = dist_loss;
 	if (exposure) {
 		// dL/dI for the tile backward and the row's update (or gradient), inside stage "loss"; the row moves only after every read of it
 		ExposureUpdate u{exposure->param, exposure->exp_avg, exposure->exp_avg_sq, exposure->step, exposure->lr, step->beta1, step->beta2, step->eps};
@@ -491,7 +532,7 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	}
 	t->mark(5, stream);
 	if (P == 0) return 0;
-	if ((rc = tile_backward(t, P, sc, cam, background, t->dL_dpix.get(), dL_ddepth, dL_dalpha, stream, dL_dnormal))) return rc;
+	if ((rc = tile_backward(t, P, sc, cam, background, t->dL_dpix.get(), dL_ddepth, dL_dalpha, stream, dL_dnormal, dL_ddepth2))) return rc;
 	out.geom = sc.geom;
 	out.cam = cam;
 	return 0;
@@ -694,7 +735,7 @@ int psb_trainer_destroy(psb_trainer* t)
 
 static int forward_impl(const char* fn, psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                         int sh_degree, float* out_color, int* radii, float* out_depth, float* out_alpha, unsigned* pass, cudaStream_t stream,
-                        float* out_normal = nullptr)
+                        float* out_normal = nullptr, float* out_depth2 = nullptr)
 {
 	int rc;
 	if (!t || !camera || !background || !out_color) { set_error_msg(std::string(fn).append(": null argument").c_str()); return PSB_ERR_ARG; }
@@ -705,8 +746,9 @@ static int forward_impl(const char* fn, psb_trainer* t, int P, int M, const psb_
 	t->have_loss = false;
 	PassMode mode = pass_mode(t, sh_degree, false);
 	mode.normals = out_normal != nullptr;
+	mode.moment = out_depth2 != nullptr;
 	if ((rc = forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, sc, cam, stream, out_depth, out_alpha, mode, nullptr,
-	                      out_normal)))
+	                      out_normal, out_depth2)))
 		return rc;
 	if (pass) *pass = t->seq;
 	return 0;
@@ -717,6 +759,15 @@ int psb_trainer_forward_normal(psb_trainer* t, int P, int M, const psb_model* mo
 {
 	return forward_impl(out_normal ? "psb_trainer_forward_normal" : "psb_trainer_forward", t, P, M, model, camera, background, sh_degree, out_color, radii,
 	                    out_depth, out_alpha, pass, (cudaStream_t)stream_, out_normal);
+}
+
+int psb_trainer_forward_moment(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
+                               float* out_color, int* radii, float* out_depth, float* out_alpha, float* out_normal, float* out_depth2, unsigned* pass,
+                               void* stream_)
+{
+	const char* fn = out_depth2 ? "psb_trainer_forward_moment" : out_normal ? "psb_trainer_forward_normal" : "psb_trainer_forward";
+	return forward_impl(fn, t, P, M, model, camera, background, sh_degree, out_color, radii, out_depth, out_alpha, pass, (cudaStream_t)stream_, out_normal,
+	                    out_depth2);
 }
 
 int psb_trainer_forward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
@@ -769,6 +820,13 @@ int psb_trainer_backward_pixels_normal(psb_trainer* t, unsigned pass, int P, int
                                        const float* background, const psb_pixel_grads* pixel_grads, const float* dL_dnormal, const psb_step* step,
                                        float* const* grads, void* stream_)
 {
+	return psb_trainer_backward_pixels_moment(t, pass, P, M, model, camera, background, pixel_grads, dL_dnormal, nullptr, step, grads, stream_);
+}
+
+int psb_trainer_backward_pixels_moment(psb_trainer* t, unsigned pass, int P, int M, const psb_model* model, const psb_camera* camera,
+                                       const float* background, const psb_pixel_grads* pixel_grads, const float* dL_dnormal, const float* dL_ddepth2,
+                                       const psb_step* step, float* const* grads, void* stream_)
+{
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
 	const bool adam = grads == nullptr;
@@ -798,6 +856,10 @@ int psb_trainer_backward_pixels_normal(psb_trainer* t, unsigned pass, int P, int
 		set_error_msg("psb_trainer_backward_pixels_normal: dL_dnormal needs a pass that rendered the normal plane (psb_trainer_forward_normal)");
 		return PSB_ERR_ARG;
 	}
+	if (dL_ddepth2 && !t->pass.moment) {
+		set_error_msg("psb_trainer_backward_pixels_moment: dL_ddepth2 needs a pass that rendered the second depth moment (psb_trainer_forward_moment)");
+		return PSB_ERR_ARG;
+	}
 	if (step->step < 1) { set_error_msg("psb_trainer_backward_pixels: step >= 1 required"); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, adam))) return rc;
 	if (!adam && (rc = check_grads(grads, P, "psb_trainer_backward_pixels"))) return rc;
@@ -806,9 +868,12 @@ int psb_trainer_backward_pixels_normal(psb_trainer* t, unsigned pass, int P, int
 	if (P == 0) return 0;
 	const Scratch sc = carve_scratch(t, P, camera->width, camera->height);
 	const Camera cam = to_camera(camera);
-	t->pass.depth = pixel_grads->dL_ddepth != nullptr;
+	// (a moment gradient leaves 2 z dL/dM in slot 11: the per-Gaussian stage consumes dL/dz)
+	t->pass.depth = pixel_grads->dL_ddepth != nullptr || dL_ddepth2 != nullptr;
 	t->pass.normal = dL_dnormal != nullptr;
-	if ((rc = tile_backward(t, P, sc, cam, background, pixel_grads->dL_dcolor, pixel_grads->dL_ddepth, pixel_grads->dL_dalpha, stream, dL_dnormal))) return rc;
+	if ((rc = tile_backward(t, P, sc, cam, background, pixel_grads->dL_dcolor, pixel_grads->dL_ddepth, pixel_grads->dL_dalpha, stream, dL_dnormal,
+	                        dL_ddepth2)))
+		return rc;
 	GradSegments gs{};
 	if (!adam)
 		for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
@@ -849,16 +914,26 @@ int psb_trainer_step_dn(psb_trainer* t, int P, int M, const psb_model* model, co
                         const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
                         const psb_exposure* exposure, const psb_normal* normal, const psb_dn* dn, void* stream_)
 {
+	return psb_trainer_step_dist(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, exposure, normal, dn, nullptr,
+	                             stream_);
+}
+
+int psb_trainer_step_dist(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                          const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
+                          const psb_exposure* exposure, const psb_normal* normal, const psb_dn* dn, const psb_dist* dist, void* stream_)
+{
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
-	const char* fn = dn ? "psb_trainer_step_dn" : normal ? "psb_trainer_step_normal" : exposure ? "psb_trainer_step_exposure" : "psb_trainer_step_depth";
+	const char* fn = dist ? "psb_trainer_step_dist"
+	                 : dn ? "psb_trainer_step_dn" : normal ? "psb_trainer_step_normal" : exposure ? "psb_trainer_step_exposure" : "psb_trainer_step_depth";
 	if ((rc = check_depth(depth, fn))) return rc;
 	if ((rc = check_exposure(exposure, true, nullptr, fn))) return rc;
 	if ((rc = check_normal(normal, fn))) return rc;
 	if ((rc = check_dn(dn, fn))) return rc;
+	if ((rc = check_dist(dist, fn))) return rc;
 	TileBackward tb;
 	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, true, stream, tb, exposure,
-	                               nullptr, normal, dn)) ||
+	                               nullptr, normal, dn, dist)) ||
 	    P == 0)
 		return rc;
 	rc = launch_fused_backward(true, 0, P, train_tensors(model, true), tb.cam, tb.geom, t->sink.get(), t->seeds.get(), to_hyper(step), GradSegments{},
@@ -1009,15 +1084,18 @@ static int result_impl(psb_trainer* t, float* out, int n_out, int* num_rendered,
 		const float dl1 = t->have_depth_loss ? (float)(h_sums[2] / (h_sums[3] > 1.0 ? h_sums[3] : 1.0)) : 0.f;
 		const float nl1 = t->have_normal_loss ? (float)(h_sums[4] / (h_sums[5] > 1.0 ? h_sums[5] : 1.0)) : 0.f;
 		const float dn = t->have_dn_loss ? (float)(h_sums[6] / (h_sums[7] > 1.0 ? h_sums[7] : 1.0)) : 0.f;
+		const float dist = t->have_dist_loss ? (float)(h_sums[8] / (h_sums[9] > 1.0 ? h_sums[9] : 1.0)) : 0.f;
 		out[0] = (1.0f - t->last_lambda) * l1 + t->last_lambda * (1.0f - ss);
 		if (t->have_depth_loss) out[0] += t->last_lambda_depth * dl1;
 		if (t->have_normal_loss) out[0] += t->last_lambda_normal * nl1;
 		if (t->have_dn_loss) out[0] += t->last_lambda_dn * dn;
+		if (t->have_dist_loss) out[0] += t->last_lambda_dist * dist;
 		out[1] = l1;
 		out[2] = ss;
 		if (n_out > 3) out[3] = dl1;
 		if (n_out > 4) out[4] = nl1;
 		if (n_out > 5) out[5] = dn;
+		if (n_out > 6) out[6] = dist;
 	}
 	return 0;
 }
@@ -1040,6 +1118,11 @@ int psb_trainer_result_normal(psb_trainer* t, float* out5, int* num_rendered, vo
 int psb_trainer_result_dn(psb_trainer* t, float* out6, int* num_rendered, void* stream_)
 {
 	return result_impl(t, out6, 6, num_rendered, stream_);
+}
+
+int psb_trainer_result_dist(psb_trainer* t, float* out7, int* num_rendered, void* stream_)
+{
+	return result_impl(t, out7, 7, num_rendered, stream_);
 }
 
 // Parity/debug export (tests only): per pixel, the final transmittance and the Gaussian index of the last blended splat

@@ -178,3 +178,14 @@ def thinned_trainee(scene, seed=3):
     start["opacity"] += rng.normal(0, 0.7, start["opacity"].shape).astype(np.float32)
     start["scaling"] += np.float32(0.15)
     return start
+
+
+def distortion_trainee(scene, normals, seed=1, sigma=0.1, opacity=0.3):
+    """A trainee for the depth distortion payoff: the rows of planar_scene's (scene, normals) with positions moved along their plane's
+    normal by N(0, sigma) metres and every opacity set to `opacity`, so that several half-transparent rows at different depths share each
+    pixel."""
+    rng = np.random.default_rng(seed)
+    start = {k: v.copy() for k, v in scene.items()}
+    start["xyz"] += (normals * rng.normal(0.0, sigma, (len(normals), 1))).astype(np.float32)
+    start["opacity"][:] = np.float32(math.log(opacity / (1.0 - opacity)))
+    return start

@@ -83,6 +83,19 @@ def _cdn(lambda_dn, alpha_min, max_rel_jump, out_depth_normal, H, W):
     return _Dn(float(lambda_dn), float(alpha_min), float(max_rel_jump), out_depth_normal.data_ptr() if out_depth_normal is not None else None)
 
 
+class _Dist(C.Structure):
+    _fields_ = [("lambda_dist", C.c_float), ("out_depth2", C.c_void_p)]
+
+
+def _cdist(lambda_dist, out_depth2, H, W):
+    """psb_dist for a call, or None when lambda_dist == 0 and there is no out_depth2 (the call is then the one without the term); the
+    library refuses a lambda_dist out of range."""
+    if lambda_dist == 0 and out_depth2 is None:
+        return None
+    _plane(out_depth2, (H, W), "out_depth2")
+    return _Dist(float(lambda_dist), out_depth2.data_ptr() if out_depth2 is not None else None)
+
+
 def _cnormal(gt_normal, lambda_normal, out_normal, H, W):
     """psb_normal for a call, or None when it has no normal argument (the call is then the one without the normal term)."""
     if gt_normal is None and out_normal is None and not lambda_normal:
@@ -186,13 +199,16 @@ def _bind():
         "psb_trainer_render_depth": render + [vp, vp],
         "psb_trainer_forward": render + [vp, vp, P(u), vp],
         "psb_trainer_forward_normal": render + [vp, vp, vp, P(u), vp],
+        "psb_trainer_forward_moment": render + [vp, vp, vp, vp, P(u), vp],
         "psb_trainer_backward_pixels": [vp, u, i, i, Model, Cam, vp, P(_PixelGrads), Step, P(vp), vp],
         "psb_trainer_backward_pixels_normal": [vp, u, i, i, Model, Cam, vp, P(_PixelGrads), vp, Step, P(vp), vp],
+        "psb_trainer_backward_pixels_moment": [vp, u, i, i, Model, Cam, vp, P(_PixelGrads), vp, vp, Step, P(vp), vp],
         "psb_trainer_step": call + [vp],
         "psb_trainer_step_depth": call + [Depth, vp],
         "psb_trainer_step_exposure": call + [Depth, Exp, vp],
         "psb_trainer_step_normal": call + [Depth, Exp, P(_Normal), vp],
         "psb_trainer_step_dn": call + [Depth, Exp, P(_Normal), P(_Dn), vp],
+        "psb_trainer_step_dist": call + [Depth, Exp, P(_Normal), P(_Dn), P(_Dist), vp],
         "psb_trainer_backward": call + [P(vp), vp],
         "psb_trainer_backward_depth": call + [P(vp), Depth, vp],
         "psb_trainer_backward_exposure": call + [P(vp), Depth, Exp, vp, vp],
@@ -203,6 +219,7 @@ def _bind():
         "psb_trainer_result_depth": [vp, P(f), P(i), vp],
         "psb_trainer_result_normal": [vp, P(f), P(i), vp],
         "psb_trainer_result_dn": [vp, P(f), P(i), vp],
+        "psb_trainer_result_dist": [vp, P(f), P(i), vp],
         "psb_depth_normals": [Cam, vp, f, vp, vp],
         "psb_dn_loss": [Cam, vp, vp, vp, vp, P(_Dn), vp, vp, vp, P(f), vp],
         "psb_trainer_overflow_info": [vp, P(u), P(u), P(u)],
@@ -1000,12 +1017,14 @@ class GaussianTrainer:
         s.update_densify_stats = int(densify_stats)
         return s
 
-    def render(self, cam, out=None, radii=None, check=True, out_depth=None, out_alpha=None, out_normal=None):
+    def render(self, cam, out=None, radii=None, check=True, out_depth=None, out_alpha=None, out_normal=None, out_depth2=None):
         """Forward only. check=True waits for the instance count and renders again if the binning arena had to grow (an
         overflowing render leaves `out` blank); pass check=False to only enqueue (call result() yourself before using `out`).
         out_depth: [H,W] float32 tensor that receives the expected depth sum_i z_i alpha_i T_i; out_alpha: [H,W] float32 tensor that
         receives the accumulated opacity 1 - T_final (psb_trainer_forward); out_normal: [3,H,W] float32 tensor that receives the
-        view-space normal plane sum_i n_i alpha_i T_i (psb_trainer_forward_normal; N / |N| is the surface normal).
+        view-space normal plane sum_i n_i alpha_i T_i (psb_trainer_forward_normal; N / |N| is the surface normal); out_depth2: [H,W]
+        float32 tensor that receives the second depth moment M = sum_i z_i^2 alpha_i T_i (psb_trainer_forward_moment; with A and D,
+        sqrt(max(M / A - (D / A)^2, 0)) is the pixel's depth spread).
         backwardPixels() back-propagates through this render."""
         m = self.model
         H, W = int(cam["H"]), int(cam["W"])
@@ -1013,30 +1032,35 @@ class GaussianTrainer:
         for t in (out_depth, out_alpha):
             assert t is None or (t.is_contiguous() and t.dtype == torch.float32 and t.numel() == cam["H"] * cam["W"])
         _plane(out_normal, (3, H, W), "out_normal")
+        _plane(out_depth2, (H, W), "out_depth2")
         self._hand_filter3d()
         cm, cc = m._cmodel(False), _ccamera(cam)
         pass_no = C.c_uint()
         args = (self.h, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(), m.active_sh_degree_, out.data_ptr(),
                 radii.data_ptr() if radii is not None else None, out_depth.data_ptr() if out_depth is not None else None,
                 out_alpha.data_ptr() if out_alpha is not None else None)
-        if out_normal is None:
+        if out_depth2 is not None:
+            _lib.check(self.L.psb_trainer_forward_moment(*args, out_normal.data_ptr() if out_normal is not None else None, out_depth2.data_ptr(),
+                                                         C.byref(pass_no), torch.cuda.current_stream().cuda_stream), "psb_trainer_forward_moment")
+        elif out_normal is None:
             _lib.check(self.L.psb_trainer_forward(*args, C.byref(pass_no), torch.cuda.current_stream().cuda_stream), "psb_trainer_forward")
         else:
             _lib.check(self.L.psb_trainer_forward_normal(*args, out_normal.data_ptr(), C.byref(pass_no), torch.cuda.current_stream().cuda_stream),
                        "psb_trainer_forward_normal")
         self._pass = pass_no.value
-        self._last_render = (cam, out, radii, out_depth, out_alpha, out_normal)
-        self._last = _Call(False, lambda: self.render(cam, out, radii, check=False, out_depth=out_depth, out_alpha=out_alpha, out_normal=out_normal),
-                           False)
+        self._last_render = (cam, out, radii, out_depth, out_alpha, out_normal, out_depth2)
+        self._last = _Call(False, lambda: self.render(cam, out, radii, check=False, out_depth=out_depth, out_alpha=out_alpha, out_normal=out_normal,
+                                                      out_depth2=out_depth2), False)
         if check:
             self.result()
         return out
 
-    def backwardPixels(self, dL_dcolor, dL_ddepth=None, dL_dalpha=None, grads=None, densify_stats=None, dL_dnormal=None):
+    def backwardPixels(self, dL_dcolor, dL_ddepth=None, dL_dalpha=None, grads=None, densify_stats=None, dL_dnormal=None, dL_ddepth2=None):
         """Back-propagates per-pixel gradients of the caller's loss through the last render() (psb_trainer_backward_pixels).
         dL_dcolor [3,H,W] (required), dL_ddepth / dL_dalpha [H,W] or None: contiguous float32 gradients w.r.t. the image, the depth and
         the accumulated opacity of that render; dL_dnormal [3,H,W] or None: w.r.t. its normal plane (a render with out_normal;
-        psb_trainer_backward_pixels_normal). grads=None: the fused Adam step of trainForOneIteration (advances step_ and iteration);
+        psb_trainer_backward_pixels_normal); dL_ddepth2 [H,W] or None: w.r.t. its second depth moment (a render with out_depth2;
+        psb_trainer_backward_pixels_moment). grads=None: the fused Adam step of trainForOneIteration (advances step_ and iteration);
         grads = six contiguous float32 tensors shaped like the model's parameters: they receive the raw-parameter gradients and the
         parameters stay as they are (for a caller's own optimizer or all-reduce). The model must not change between the render and
         this call. densify_stats as in trainForOneIteration (both modes fold the densification statistics in).
@@ -1055,6 +1079,9 @@ class GaussianTrainer:
         _plane(dL_dnormal, (3, H, W), "dL_dnormal")
         if dL_dnormal is not None and (len(self._last_render) < 6 or self._last_render[5] is None):
             raise ValueError("dL_dnormal: the last render() rendered no normal plane (pass out_normal)")
+        _plane(dL_ddepth2, (H, W), "dL_ddepth2")
+        if dL_ddepth2 is not None and (len(self._last_render) < 7 or self._last_render[6] is None):
+            raise ValueError("dL_ddepth2: the last render() rendered no second depth moment (pass out_depth2)")
         if grads is not None:
             grads = list(grads)
             if len(grads) != 6:
@@ -1073,22 +1100,28 @@ class GaussianTrainer:
                          dL_dalpha.data_ptr() if dL_dalpha is not None else None)
         ptrs = None if adam else (C.c_void_p * 6)(*[g.data_ptr() for g in grads])
         head = (self.h, self._pass, m.num_points(), 16, C.byref(cm), C.byref(cc), self.background.data_ptr(), C.byref(px))
-        if dL_dnormal is None:
+        if dL_ddepth2 is not None:
+            fn = "psb_trainer_backward_pixels_moment"
+            rc = self.L.psb_trainer_backward_pixels_moment(*head, dL_dnormal.data_ptr() if dL_dnormal is not None else None, dL_ddepth2.data_ptr(),
+                                                           C.byref(cs), ptrs, torch.cuda.current_stream().cuda_stream)
+        elif dL_dnormal is None:
+            fn = "psb_trainer_backward_pixels"
             rc = self.L.psb_trainer_backward_pixels(*head, C.byref(cs), ptrs, torch.cuda.current_stream().cuda_stream)
         else:
+            fn = "psb_trainer_backward_pixels_normal"
             rc = self.L.psb_trainer_backward_pixels_normal(*head, dL_dnormal.data_ptr(), C.byref(cs), ptrs, torch.cuda.current_stream().cuda_stream)
         if rc < 0 and adam:
             self.iteration -= 1
-        _lib.check(rc, "psb_trainer_backward_pixels_normal" if dL_dnormal is not None else "psb_trainer_backward_pixels")
+        _lib.check(rc, fn)
         if adam:
             m.step_ += 1
         self._last = _Call(adam, None, False)     # (trainWithLoss replaces it with its own record)
 
-    def trainWithLoss(self, cam, loss_fn, depth=False, alpha=False, out_color=None, radii=None, densify_stats=None, normal=False):
+    def trainWithLoss(self, cam, loss_fn, depth=False, alpha=False, out_color=None, radii=None, densify_stats=None, normal=False, depth2=False):
         """One training iteration against the caller's loss: enqueues the forward (no host synchronisation of its own), calls
-        loss = loss_fn(image[, depth][, alpha][, normal]) on leaf tensors that require grad (image [3,H,W]; depth [H,W] = sum z alpha T with
-        depth=True; alpha [H,W] = 1 - T_final with alpha=True; normal [3,H,W] = sum n alpha T, the view-space normal plane, with
-        normal=True), takes torch.autograd.grad of the loss w.r.t. those outputs only, and
+        loss = loss_fn(image[, depth][, alpha][, normal][, depth2]) on leaf tensors that require grad (image [3,H,W]; depth [H,W] = sum z
+        alpha T with depth=True; alpha [H,W] = 1 - T_final with alpha=True; normal [3,H,W] = sum n alpha T, the view-space normal plane, with
+        normal=True; depth2 [H,W] = sum z^2 alpha T, the second depth moment, with depth2=True), takes torch.autograd.grad of the loss w.r.t. those outputs only, and
         back-propagates it through the fused kernels into a fused Adam step (backwardPixels). The model tensors never enter autograd.
         Advances step_ / iteration like trainForOneIteration and returns the (detached) loss tensor; result() repeats the whole call
         if the forward overflowed the binning arena. out_color / radii: optional tensors that receive the image / radii."""
@@ -1101,9 +1134,10 @@ class GaussianTrainer:
         D = torch.empty((H, W), device=m.device) if depth else None
         A = torch.empty((H, W), device=m.device) if alpha else None
         N = torch.empty((3, H, W), device=m.device) if normal else None
+        M2 = torch.empty((H, W), device=m.device) if depth2 else None
         self._apply_deterministic()
-        self.render(cam, image, radii, check=False, out_depth=D, out_alpha=A, out_normal=N)
-        outs = [t for t in (image, D, A, N) if t is not None]
+        self.render(cam, image, radii, check=False, out_depth=D, out_alpha=A, out_normal=N, out_depth2=M2)
+        outs = [t for t in (image, D, A, N, M2) if t is not None]
         leaves = [t.detach().requires_grad_(True) for t in outs]
         with torch.enable_grad():
             loss = loss_fn(*leaves)
@@ -1114,15 +1148,18 @@ class GaussianTrainer:
         gd = next(g) if depth else None
         ga = next(g) if alpha else None
         gn = next(g) if normal else None
-        self.backwardPixels(gc, gd, ga, densify_stats=densify_stats, dL_dnormal=gn)
+        gm = next(g) if depth2 else None
+        if depth2 and gm is None:
+            gm = torch.zeros((H, W), device=m.device)
+        self.backwardPixels(gc, gd, ga, densify_stats=densify_stats, dL_dnormal=gn, dL_ddepth2=gm)
         self._inject_noise()
-        self._last = _Call(True, lambda: self.trainWithLoss(cam, loss_fn, depth, alpha, out_color, radii, densify_stats, normal), True)
+        self._last = _Call(True, lambda: self.trainWithLoss(cam, loss_fn, depth, alpha, out_color, radii, densify_stats, normal, depth2), True)
         self._last_loss = loss.detach()
         return self._last_loss
 
     def trainForOneIteration(self, cam, gt_image, mask=None, out_color=None, radii=None, densify_stats=None, gt_depth=None, lambda_depth=0.0,
                              out_depth=None, exposure_id=None, gt_normal=None, lambda_normal=0.0, out_normal=None, lambda_dn=0.0, dn_alpha_min=0.5,
-                             dn_max_rel_jump=0.05, out_depth_normal=None):
+                             dn_max_rel_jump=0.05, out_depth_normal=None, lambda_dist=0.0, out_depth2=None):
         """Enqueues render -> loss -> backward -> Adam on the current stream (no host sync).
         gt_depth: [H,W] float32 target depth in metres (<= 0: no measurement) trained with weight lambda_depth (> 0) as an L1 term
         over the valid pixels; out_depth: [H,W] float32 tensor that receives the rendered depth.
@@ -1135,11 +1172,16 @@ class GaussianTrainer:
         lambda_dn > 0: the depth-normal consistency term (psb_dn; no sensor needed, so monocular and stereo keyframes can use it) with
         weight lambda_dn: the normal of the rendered depth D / A (where A >= dn_alpha_min; dn_max_rel_jump: the depth-edge rule of
         normals_from_depth) against the rendered normal plane. out_depth_normal: [3,H,W] float32 tensor that receives that depth normal.
-        The call is then psb_trainer_step_dn; result_dn() reports the term. lambda_dn = 0 without out_depth_normal makes the call without it."""
+        The call is then psb_trainer_step_dn; result_dn() reports the term. lambda_dn = 0 without out_depth_normal makes the call without it.
+        lambda_dist > 0: the depth distortion term (psb_dist; no sensor or target needed) with weight lambda_dist: the mean over the (mask's)
+        pixels of A M - D^2, which pulls each ray's blending weight onto one depth. out_depth2: [H,W] float32 tensor that receives the second
+        depth moment M. The call is then psb_trainer_step_dist; result_dist() reports the term. lambda_dist = 0 without out_depth2 makes
+        the call without it."""
         m = self.model
         depth = _cdepth(gt_depth, lambda_depth, out_depth)
         normal = _cnormal(gt_normal, lambda_normal, out_normal, int(cam["H"]), int(cam["W"]))
         dn = _cdn(lambda_dn, dn_alpha_min, dn_max_rel_jump, out_depth_normal, int(cam["H"]), int(cam["W"]))
+        dist = _cdist(lambda_dist, out_depth2, int(cam["H"]), int(cam["W"]))
         exposure = None
         if exposure_id is not None:
             k = int(exposure_id)
@@ -1157,7 +1199,11 @@ class GaussianTrainer:
         args = (*self._call_args(m, cm, cc, cs, gt_image, mask, out_color, radii), C.byref(depth) if depth is not None else None,
                 C.byref(exposure) if exposure is not None else None)
         stream = torch.cuda.current_stream().cuda_stream
-        if dn is not None:
+        if dist is not None:
+            rc = self.L.psb_trainer_step_dist(*args, C.byref(normal) if normal is not None else None, C.byref(dn) if dn is not None else None,
+                                              C.byref(dist), stream)
+            fn = "psb_trainer_step_dist"
+        elif dn is not None:
             rc = self.L.psb_trainer_step_dn(*args, C.byref(normal) if normal is not None else None, C.byref(dn), stream)
             fn = "psb_trainer_step_dn"
         elif normal is not None:
@@ -1171,7 +1217,8 @@ class GaussianTrainer:
         self._inject_noise()
         self._last = _Call(True, lambda: self.trainForOneIteration(cam, gt_image, mask, out_color, radii, densify_stats, gt_depth, lambda_depth,
                                                                    out_depth, exposure_id, gt_normal, lambda_normal, out_normal, lambda_dn,
-                                                                   dn_alpha_min, dn_max_rel_jump, out_depth_normal), False)
+                                                                   dn_alpha_min, dn_max_rel_jump, out_depth_normal, lambda_dist, out_depth2),
+                           False)
 
     def _call_args(self, m, cm, cc, cs, gt_image, mask, out_color, radii):
         """The leading arguments of a built-in-loss training call (t ... radii)."""
@@ -1205,9 +1252,14 @@ class GaussianTrainer:
         num_rendered); a term the step did not have reads 0 (psb_trainer_result_dn)."""
         return self._result(6)
 
+    def result_dist(self):
+        """result() with the depth L1, normal L1, depth-normal consistency and depth distortion of the last step: -> (loss, l1, ssim,
+        depth_l1, normal_l1, dn, dist, num_rendered); a term the step did not have reads 0 (psb_trainer_result_dist)."""
+        return self._result(7)
+
     def _result(self, nterms):
-        out, n = (C.c_float * 6)(), C.c_int()
-        name = {6: "psb_trainer_result_dn", 5: "psb_trainer_result_normal"}.get(nterms, "psb_trainer_result_depth")
+        out, n = (C.c_float * 7)(), C.c_int()
+        name = {7: "psb_trainer_result_dist", 6: "psb_trainer_result_dn", 5: "psb_trainer_result_normal"}.get(nterms, "psb_trainer_result_depth")
         result_fn = getattr(self.L, name)
         rc = result_fn(self.h, out, C.byref(n), torch.cuda.current_stream().cuda_stream)
         if rc == -4:
@@ -1233,7 +1285,7 @@ class GaussianTrainer:
         if self._last.callers_loss:
             # the caller's loss: only its value is known (l1, ssim, depth_l1 and normal_l1 are the built-in loss's terms)
             nan = float("nan")
-            out = (float(self._last_loss), nan, nan, nan, nan, nan)
+            out = (float(self._last_loss), nan, nan, nan, nan, nan, nan)
         return (*out[:nterms], n.value)
 
     # ------------------------------------------------------------------------------------------------------------
@@ -1477,11 +1529,11 @@ class DataParallelTrainer(GaussianTrainer):
 
     def trainForOneIteration(self, cam, gt_image, mask=None, out_color=None, radii=None, densify_stats=None, gt_depth=None, lambda_depth=0.0,
                              out_depth=None, exposure_id=None, gt_normal=None, lambda_normal=0.0, out_normal=None, lambda_dn=0.0, dn_alpha_min=0.5,
-                             dn_max_rel_jump=0.05, out_depth_normal=None):
+                             dn_max_rel_jump=0.05, out_depth_normal=None, lambda_dist=0.0, out_depth2=None):
         """Depth arguments as in GaussianTrainer, on every path: "p2p" (psb_dp_step_depth), the slab pipeline
         (psb_trainer_backward_begin_depth) and the flat "nccl" path (psb_trainer_backward_depth). Each rank passes its own view's
-        target or none: ranks with and without a depth term may train in the same step. exposure_id and the normal arguments must be
-        None, and lambda_dn 0."""
+        target or none: ranks with and without a depth term may train in the same step. exposure_id, the normal arguments and out_depth2
+        must be None, and lambda_dn and lambda_dist 0."""
         if gt_normal is not None or out_normal is not None or lambda_normal:
             raise NotImplementedError("DataParallelTrainer: the normal term is not wired into the data-parallel steps (the NVLink push "
                                       "backward and the slab pipeline carry 12-float sink rows); train with normals on one GPU through "
@@ -1489,6 +1541,9 @@ class DataParallelTrainer(GaussianTrainer):
         if lambda_dn or out_depth_normal is not None:
             raise NotImplementedError("DataParallelTrainer: the depth-normal consistency term is not wired into the data-parallel steps (it "
                                       "needs the normal plane and its 16-float sink rows); train with it on one GPU through GaussianTrainer")
+        if lambda_dist or out_depth2 is not None:
+            raise NotImplementedError("DataParallelTrainer: the depth distortion term is not wired into the data-parallel steps (their "
+                                      "forward renders no second depth moment); train with it on one GPU through GaussianTrainer")
         if exposure_id is not None:
             raise NotImplementedError("DataParallelTrainer: exposure compensation is not wired into the data-parallel steps: the per-keyframe "
                                       "exposure table would have to be replicated across the ranks (each rank's row updates gathered to "

@@ -28,15 +28,16 @@ def _si_depth_error(D, A, D_true):
     return float(torch.sqrt((d * d).mean() - d.mean() ** 2))
 
 
-def planar_payoff(dev, per_wall=3000, steps=300, W=160, H=120, lambda_dn=0.05, alpha_min=0.5, max_rel_jump=0.05, seed=0):
-    """-> {"colour": dict(psnr, angle, si_depth), "colour+dn": ...} (see the module docstring); deterministic mode."""
+def planar_views(dev, per_wall=3000, W=160, H=120, seed=0):
+    """The planar payoff's setup: synthetic.planar_scene(per_wall) seen at W x H (f = 0.7 W) from 9 poses, the first 6 for training and
+    the last 3 held out. -> (scene, normals, train cams, held-out cams, targets: per camera (image, true depth D / A where A > 0.5 else 0,
+    normal plane N) rendered from the true scene)."""
     import photo_slam_b200.synthetic as syn
     from photo_slam_b200 import trainer
-    sc, _ = syn.planar_scene(per_wall, seed=seed)
+    sc, normals = syn.planar_scene(per_wall, seed=seed)
     f = 0.7 * W
     cams = [syn.device_camera(syn.make_camera(W, H, f, f, *syn.random_pose(np.random.default_rng(100 + k), max_angle=0.12, max_trans=0.25)), dev)
             for k in range(9)]
-    train, held = cams[:6], cams[6:]
     truth = trainer.GaussianTrainer(_model(sc, dev))
     targets = []
     for c in cams:
@@ -44,6 +45,13 @@ def planar_payoff(dev, per_wall=3000, steps=300, W=160, H=120, lambda_dn=0.05, a
                         torch.empty((3, H, W), device=dev))
         truth.render(c, img, out_depth=D, out_alpha=A, out_normal=N)
         targets.append((img, torch.where(A > 0.5, D / A.clamp_min(1e-6), torch.zeros_like(D)), N))
+    return sc, normals, cams[:6], cams[6:], targets
+
+
+def planar_payoff(dev, per_wall=3000, steps=300, W=160, H=120, lambda_dn=0.05, alpha_min=0.5, max_rel_jump=0.05, seed=0):
+    """-> {"colour": dict(psnr, angle, si_depth), "colour+dn": ...} (see the module docstring); deterministic mode."""
+    from photo_slam_b200 import trainer
+    sc, _, train, held, targets = planar_views(dev, per_wall, W, H, seed)
     rng = np.random.default_rng(seed + 1)
     start = dict(sc, rotation=rng.normal(size=sc["rotation"].shape).astype(np.float32),
                  scaling=(np.full(sc["scaling"].shape, math.log(0.02)) + rng.normal(0, 0.1, sc["scaling"].shape)).astype(np.float32))
