@@ -20,7 +20,7 @@ def build_rotation(r):
     norm = torch.sqrt(r0 * r0 + r1 * r1 + r2 * r2 + r3 * r3)
     q = r / norm.unsqueeze(1)
     w, x, y, z = q[:, 0], q[:, 1], q[:, 2], q[:, 3]
-    R = torch.zeros((q.size(0), 3, 3), device=r.device)
+    R = torch.zeros((q.size(0), 3, 3), dtype=r.dtype, device=r.device)
     R[:, 0, 0] = 1 - 2 * (y * y + z * z); R[:, 0, 1] = 2 * (x * y - w * z); R[:, 0, 2] = 2 * (x * z + w * y)
     R[:, 1, 0] = 2 * (x * y + w * z); R[:, 1, 1] = 1 - 2 * (x * x + z * z); R[:, 1, 2] = 2 * (y * z - w * x)
     R[:, 2, 0] = 2 * (x * z - w * y); R[:, 2, 1] = 2 * (y * z + w * x); R[:, 2, 2] = 1 - 2 * (x * x + y * y)
@@ -56,7 +56,7 @@ def densify_and_split(st, grads, grad_threshold, scene_extent, percent_dense, z,
     """:716-761; z: [N * n_selected, 3] standard-normal draw (None -> torch.randn)"""
     n_init = st["p"][0].size(0)
     dev = st["p"][0].device
-    padded = torch.zeros(n_init, device=dev)
+    padded = torch.zeros(n_init, dtype=grads.dtype, device=dev)
     padded[:grads.size(0)] = grads.squeeze()
     sel = torch.where(padded >= grad_threshold, True, False)
     sel = torch.logical_and(sel, torch.max(_exp(st["p"][4]), dim=1).values > percent_dense * scene_extent)

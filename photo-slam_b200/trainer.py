@@ -1420,6 +1420,7 @@ class DataParallelTrainer(GaussianTrainer):
         h = C.c_void_p()
         _lib.check(L.psb_dp_create(C.byref(h), self.rank, self.world, P), "psb_dp_create")
         self.dp = h
+        self._dp_P = P
         nb = L.psb_dp_handle_bytes()
         if self.world > 1:
             mine = (C.c_char * nb)()
@@ -1549,6 +1550,10 @@ class DataParallelTrainer(GaussianTrainer):
                                       "exposure table would have to be replicated across the ranks (each rank's row updates gathered to "
                                       "every rank every step); train with exposure on one GPU through GaussianTrainer")
         m = self.model
+        built = self._dp_P if self.mode == "p2p" else self.grads.P
+        if built != m.num_points():
+            raise ValueError(f"DataParallelTrainer: the model has {m.num_points()} rows, the trainer was built for {built}: call rebuild() "
+                             "after densify, prune or insertion")
         depth = _cdepth(gt_depth, lambda_depth, out_depth)
         self._apply_deterministic()
         self.iteration += 1
@@ -1563,13 +1568,11 @@ class DataParallelTrainer(GaussianTrainer):
         if self.mode == "p2p":
             _lib.check(self.L.psb_dp_step_depth(self.h, self.dp, *args[1:], cdepth, stream), "psb_dp_step_depth")
         elif not self.pipeline:
-            assert self.grads.P == P, "gradient buffer was built for a different model size: call rebuild() after densify/prune"
             ptrs = (C.c_void_p * 6)(*[s.data_ptr() for s in self.segs])
             _lib.check(self.L.psb_trainer_backward_depth(*args, ptrs, cdepth, stream), "psb_trainer_backward_depth")
             scale = self.grads.all_reduce(self.group)   # ONE collective per step: 59 floats per Gaussian
             _lib.check(self.L.psb_adam_update(P, 16, C.byref(cm), ptrs, C.byref(cs), scale, stream), "psb_adam_update")
         else:
-            assert self.grads.P == P, "gradient buffer was built for a different model size: call rebuild() after densify/prune"
             _lib.check(self.L.psb_trainer_backward_begin_depth(*args, cdepth, stream), "psb_trainer_backward_begin_depth")
             scale = 1.0 / self.world
             for s, (first, count) in enumerate(self.grads.slabs):
