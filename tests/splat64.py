@@ -181,11 +181,16 @@ def _alpha(a_raw, conv):
     return torch.clamp_max(a_raw, ALPHA_MAX)
 
 
-def composite(geo, W, H, bg, conv=CONV, want_margins=False):
+def composite(geo, W, H, bg, conv=CONV, want_margins=False, tiles=None):
     """Per pixel, over the Gaussians whose rectangle holds the pixel's tile, in depth order (psb_render.cu render_fwd_body).
     -> dict(color [3,H,W], depth [H,W], alpha [H,W] = 1 - T_final, n_contrib [H,W] (1-based list position of the last blended
     splat, 0 = none), last [H,W] (the Gaussian index of that splat, -1 = none), stopped [H,W] (the T test ended the pixel's list), clamped [H,W] (a blended alpha was clamped at 0.99),
-    list_len [tiles]) and with want_margins the pair decisions' margins."""
+    list_len [tiles]) and with want_margins the pair decisions' margins.
+
+    tiles: a list of (tx, ty) composites only those tiles and returns the same keys over their pixels, flattened in the order of the
+    list (color [3,N], the others [N]), with pix [N] (y W + x) and, with want_margins, pix_margins: per pixel and decision the smallest
+    margin of its pairs (inf for none), T_ulp (the T test's margin over 2^-24 sum 1 / (1 - alpha) of the factors blended up to the
+    test) and depth_tie (the relative depth gap of two successive splats of the pixel that pass the alpha test)."""
     dev = geo["z"].device
     bg = _t(bg, dev).reshape(3)
     gx, gy = geo["gx"], geo["gy"]
@@ -195,60 +200,83 @@ def composite(geo, W, H, bg, conv=CONV, want_margins=False):
     m2, con, o, rgb, z = geo["means2D"][order], geo["conic"][order], geo["o"][order], geo["rgb"][order], geo["z"][order]
     outs, pix_ids, list_len = [], [], []
     mg = {k: [] for k in ("power", "alpha_min", "alpha_max", "T", "depth_tie")}
-    for ty in range(gy):
-        for tx in range(gx):
-            sel = ((rect[:, 0] <= tx) & (tx < rect[:, 2]) & (rect[:, 1] <= ty) & (ty < rect[:, 3])).nonzero().reshape(-1)
-            list_len.append(int(sel.numel()))
-            ys, xs = torch.meshgrid(torch.arange(ty * TILE, min(ty * TILE + TILE, H), device=dev),
-                                    torch.arange(tx * TILE, min(tx * TILE + TILE, W), device=dev), indexing="ij")
-            ys, xs = ys.reshape(-1), xs.reshape(-1)
-            pix_ids.append(ys * W + xs)
-            n = sel.numel()
-            if n == 0:
-                npx = xs.numel()
-                outs.append(torch.cat([bg.expand(npx, 3), torch.zeros(npx, 5, dtype=torch.float64, device=dev),
-                                       torch.full((npx, 1), -1.0, dtype=torch.float64, device=dev)], 1))
-                continue
-            dx = m2[sel, 0][None, :] - xs[:, None].double()
-            dy = m2[sel, 1][None, :] - ys[:, None].double()
-            A, B, C = con[sel, 0][None, :], con[sel, 1][None, :], con[sel, 2][None, :]
-            power = -0.5 * (A * dx * dx + C * dy * dy) - B * dx * dy      # psb_geom.cuh splat_power
-            pw = power.detach()
-            a_raw = o[sel][None, :] * torch.exp(power)
-            ad = a_raw.detach()
-            valid = (pw <= 0) & (torch.clamp_max(ad, ALPHA_MAX) >= conv.alpha_min)
-            alpha = _alpha(a_raw, conv)
-            f_all = torch.where(valid, 1.0 - alpha.detach(), torch.ones_like(ad))
-            t_after = torch.cumprod(f_all, 1)
-            include = valid & (t_after >= conv.t_min)
-            fi = torch.where(include, 1.0 - alpha, torch.ones_like(alpha))
-            cp = torch.cumprod(fi, 1)
-            Tb = torch.cat([torch.ones_like(cp[:, :1]), cp[:, :-1]], 1)
-            w = torch.where(include, alpha * Tb, torch.zeros_like(alpha))
-            Tf = cp[:, -1:]
-            col = w @ rgb[sel] + Tf * bg
-            dep = (w @ z[sel]) if conv.depth_weighted else (include.double() @ z[sel])
-            pos = torch.arange(1, n + 1, device=dev, dtype=torch.float64)
-            nc = (include.double() * pos).amax(1)
-            stopped = (valid & ~include).any(1).double()
-            clamped = (include & (ad > ALPHA_MAX)).any(1).double()
-            last = torch.where(nc > 0, order[sel].double()[(nc.long() - 1).clamp_min(0)], torch.full_like(nc, -1.0))
-            outs.append(torch.cat([col, dep[:, None], (1.0 - Tf), nc[:, None], stopped[:, None], clamped[:, None], last[:, None]], 1))
-            if want_margins:
-                gid = order[sel][None, :].expand_as(pw)
-                mag = 0.5 * (A.abs() * dx * dx + C.abs() * dy * dy).detach() + (B * dx * dy).abs().detach()
-                nz = mag > 0
-                mg["power"].append(((pw.abs() / mag)[nz], gid[nz]))
-                tested = pw <= 0
-                mg["alpha_min"].append(((ad - conv.alpha_min).abs()[tested] / conv.alpha_min, gid[tested]))
-                mg["alpha_max"].append(((ad - ALPHA_MAX).abs()[tested] / ALPHA_MAX, gid[tested]))
-                t_before = torch.cat([torch.ones_like(t_after[:, :1]), t_after[:, :-1]], 1)
-                ev = valid & (t_before >= conv.t_min)
-                mg["T"].append(((t_before * f_all - conv.t_min).abs()[ev] / conv.t_min, gid[ev]))
-                zs = geo["zd"][order[sel]]
-                if n > 1:
-                    mg["depth_tie"].append(((zs[1:] - zs[:-1]) / zs[1:], order[sel][1:]))
+    pm = []
+    for ty, tx in ([(ty, tx) for ty in range(gy) for tx in range(gx)] if tiles is None else [(ty, tx) for tx, ty in tiles]):
+        sel = ((rect[:, 0] <= tx) & (tx < rect[:, 2]) & (rect[:, 1] <= ty) & (ty < rect[:, 3])).nonzero().reshape(-1)
+        list_len.append(int(sel.numel()))
+        ys, xs = torch.meshgrid(torch.arange(ty * TILE, min(ty * TILE + TILE, H), device=dev),
+                                torch.arange(tx * TILE, min(tx * TILE + TILE, W), device=dev), indexing="ij")
+        ys, xs = ys.reshape(-1), xs.reshape(-1)
+        pix_ids.append(ys * W + xs)
+        n = sel.numel()
+        if n == 0:
+            npx = xs.numel()
+            outs.append(torch.cat([bg.expand(npx, 3), torch.zeros(npx, 5, dtype=torch.float64, device=dev),
+                                   torch.full((npx, 1), -1.0, dtype=torch.float64, device=dev)], 1))
+            if want_margins and tiles is not None:
+                pm.append({k: torch.full((npx,), math.inf, dtype=torch.float64, device=dev)
+                           for k in ("power", "alpha_min", "alpha_max", "T", "T_ulp", "depth_tie")})
+            continue
+        dx = m2[sel, 0][None, :] - xs[:, None].double()
+        dy = m2[sel, 1][None, :] - ys[:, None].double()
+        A, B, C = con[sel, 0][None, :], con[sel, 1][None, :], con[sel, 2][None, :]
+        power = -0.5 * (A * dx * dx + C * dy * dy) - B * dx * dy      # psb_geom.cuh splat_power
+        pw = power.detach()
+        a_raw = o[sel][None, :] * torch.exp(power)
+        ad = a_raw.detach()
+        valid = (pw <= 0) & (torch.clamp_max(ad, ALPHA_MAX) >= conv.alpha_min)
+        alpha = _alpha(a_raw, conv)
+        f_all = torch.where(valid, 1.0 - alpha.detach(), torch.ones_like(ad))
+        t_after = torch.cumprod(f_all, 1)
+        include = valid & (t_after >= conv.t_min)
+        fi = torch.where(include, 1.0 - alpha, torch.ones_like(alpha))
+        cp = torch.cumprod(fi, 1)
+        Tb = torch.cat([torch.ones_like(cp[:, :1]), cp[:, :-1]], 1)
+        w = torch.where(include, alpha * Tb, torch.zeros_like(alpha))
+        Tf = cp[:, -1:]
+        col = w @ rgb[sel] + Tf * bg
+        dep = (w @ z[sel]) if conv.depth_weighted else (include.double() @ z[sel])
+        pos = torch.arange(1, n + 1, device=dev, dtype=torch.float64)
+        nc = (include.double() * pos).amax(1)
+        stopped = (valid & ~include).any(1).double()
+        clamped = (include & (ad > ALPHA_MAX)).any(1).double()
+        last = torch.where(nc > 0, order[sel].double()[(nc.long() - 1).clamp_min(0)], torch.full_like(nc, -1.0))
+        outs.append(torch.cat([col, dep[:, None], (1.0 - Tf), nc[:, None], stopped[:, None], clamped[:, None], last[:, None]], 1))
+        if want_margins:
+            gid = order[sel][None, :].expand_as(pw)
+            mag = 0.5 * (A.abs() * dx * dx + C.abs() * dy * dy).detach() + (B * dx * dy).abs().detach()
+            nz = mag > 0
+            mg["power"].append(((pw.abs() / mag)[nz], gid[nz]))
+            tested = pw <= 0
+            mg["alpha_min"].append(((ad - conv.alpha_min).abs()[tested] / conv.alpha_min, gid[tested]))
+            mg["alpha_max"].append(((ad - ALPHA_MAX).abs()[tested] / ALPHA_MAX, gid[tested]))
+            t_before = torch.cat([torch.ones_like(t_after[:, :1]), t_after[:, :-1]], 1)
+            ev = valid & (t_before >= conv.t_min)
+            mg["T"].append(((t_before * f_all - conv.t_min).abs()[ev] / conv.t_min, gid[ev]))
+            zs = geo["zd"][order[sel]]
+            if n > 1:
+                mg["depth_tie"].append(((zs[1:] - zs[:-1]) / zs[1:], order[sel][1:]))
+            if tiles is not None:
+                inf = torch.full_like(pw, math.inf)
+                t_rel = (t_before * f_all - conv.t_min).abs() / conv.t_min
+                ulps = torch.cumsum(torch.where(valid, 1.0 / f_all, torch.zeros_like(f_all)), 1) * 2.0 ** -24
+                idx = torch.arange(n, device=dev).expand_as(pw)
+                prev = torch.cummax(torch.where(ev, idx, torch.full_like(idx, -1)), 1).values
+                prev = torch.cat([torch.full_like(prev[:, :1], -1), prev[:, :-1]], 1)
+                gap = (zs[None, :] - zs[prev.clamp_min(0)]) / zs[None, :].abs()
+                pm.append(dict(power=torch.where(nz, pw.abs() / mag, inf).amin(1),
+                               alpha_min=torch.where(tested, (ad - conv.alpha_min).abs() / conv.alpha_min, inf).amin(1),
+                               alpha_max=torch.where(tested, (ad - ALPHA_MAX).abs() / ALPHA_MAX, inf).amin(1),
+                               T=torch.where(ev, t_rel, inf).amin(1), T_ulp=torch.where(ev, t_rel / ulps, inf).amin(1),
+                               depth_tie=torch.where(ev & (prev >= 0), gap, inf).amin(1)))
     vals = torch.cat(outs, 0)
+    if tiles is not None:
+        out = dict(pix=torch.cat(pix_ids), color=vals[:, :3].T, depth=vals[:, 3], alpha=vals[:, 4], n_contrib=vals[:, 5].detach().round().long(),
+                   stopped=vals[:, 6].detach().bool(), clamped=vals[:, 7].detach().bool(), last=vals[:, 8].detach().round().long(),
+                   list_len=torch.tensor(list_len, device=dev))
+        if want_margins:
+            out["pix_margins"] = {k: torch.cat([d[k] for d in pm]) for k in pm[0]}
+        return out
     inv = torch.argsort(torch.cat(pix_ids))
     vals = vals[inv]
     out = dict(color=vals[:, :3].T.reshape(3, H, W), depth=vals[:, 3].reshape(H, W), alpha=vals[:, 4].reshape(H, W),
