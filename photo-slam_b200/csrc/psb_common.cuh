@@ -417,6 +417,11 @@ __device__ __forceinline__ void cp_async4(void* smem_dst, const void* gmem_src)
 {
 	asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
 }
+// brings the 128-byte line holding `gmem` into L2 with the evict-last priority (a later load of it hits L2); no register, no wait
+__device__ __forceinline__ void prefetch_l2_evict_last(const void* gmem)
+{
+	asm volatile("prefetch.global.L2::evict_last [%0];" ::"l"(gmem));
+}
 __device__ __forceinline__ void cp_async_wait_all()
 {
 	asm volatile("cp.async.wait_all;" ::: "memory");

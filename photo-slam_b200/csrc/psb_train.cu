@@ -8,6 +8,8 @@
 //                             parameter rows it has to read arrive by one TMA bulk copy per block);
 //   frest_stream_kernel       Adam over the [P,15,3] SH rows (76 % of the parameter bytes), one float4 per thread,
 //                             gradient = seed products; runs at the HBM copy rate.
+// With the caller's live byte (MODE_ADAM_LIVE) the per-Gaussian kernel applies the f_rest Adam to the rows it staged, and
+//   frest_momentum_kernel     applies it (g = 0) to the live rows it did not stage, from a list that kernel leaves.
 //
 // Replaces, per iteration of reference GaussianMapper::trainForOneIteration (src/gaussian_mapper.cpp:614-774):
 //   computeCov2DCUDA + preprocessCUDA backward (cuda_rasterizer/backward.cu:144-396),
@@ -81,11 +83,12 @@ __device__ __forceinline__ void adam4(float4& p, float4& m, float4& v, const flo
 // (m' = v' = 0, p' = p - lr * 0 / (0 + eps) = p): such elements (Gaussians no view has reached since their moments were created) are
 // neither read beyond their moments nor rewritten, and false is returned. Otherwise the moments are stored back and the new
 // parameters are returned in `pp` for the caller to store.
+__device__ __forceinline__ bool adam_noop(float g, float m, float v) { return g == 0.f && m == 0.f && v == 0.f; }
+
 __device__ __forceinline__ bool adam4_unless_noop(const float* p, float* m, float* v, const float4 g, float lr_eff, const AdamCoef& c, float4& pp)
 {
 	float4 mm = __ldcs(reinterpret_cast<const float4*>(m)), vv = __ldcs(reinterpret_cast<const float4*>(v));
-	if (g.x == 0.f && g.y == 0.f && g.z == 0.f && g.w == 0.f && mm.x == 0.f && mm.y == 0.f && mm.z == 0.f && mm.w == 0.f &&
-	    vv.x == 0.f && vv.y == 0.f && vv.z == 0.f && vv.w == 0.f) return false;
+	if (adam_noop(g.x, mm.x, vv.x) && adam_noop(g.y, mm.y, vv.y) && adam_noop(g.z, mm.z, vv.z) && adam_noop(g.w, mm.w, vv.w)) return false;
 	pp = __ldcs(reinterpret_cast<const float4*>(p));
 	adam4(pp, mm, vv, g, lr_eff, c);
 	__stcs(reinterpret_cast<float4*>(m), mm); __stcs(reinterpret_cast<float4*>(v), vv);
@@ -114,6 +117,14 @@ __device__ __forceinline__ void store_small(float* const* ts, int idx, const Sma
 	ts[3][idx] = r.op;
 	reinterpret_cast<float4*>(ts[5])[idx] = r.rot;
 }
+
+// MODE_ADAM_LIVE: rows that are live after the step but had no f_rest row staged (hidden, out of view, or reached through dL/dz /
+// dL/dn only). Their f_rest gradient is zero, but their moments still move the parameters: frest_momentum_kernel updates them.
+// rows[0 .. *count) in no particular order (every row's update is independent of the others); *count is zeroed before the step.
+struct MomentumList {
+	uint32_t* rows;   // [P]
+	uint32_t* count;
+};
 
 // any of the 14 values is non-zero
 __device__ __forceinline__ bool any_nonzero(const SmallRow& r)
@@ -169,8 +180,9 @@ __device__ __forceinline__ void adam_small(SmallRow& p, SmallRow& m, SmallRow& v
 // moments (a row reached for the first time starts from the zero moments the contract guarantees). The f_rest rows are staged
 // only for rows with non-zero sums — the only rows whose view-direction term of dL/dxyz can be non-zero — each warp copying its
 // own rows with 4-byte async copies into a compacted region of s_p (one coalesced 180-byte run per row; the whole-block TMA copy
-// would move every row, since nearly every block holds some live row). Seed rows are written, and updated by
-// frest_stream_kernel, only for rows that are live after this step; the live byte is set for every row that received a gradient.
+// would move every row, since nearly every block holds some live row). No seed row is written: a last phase applies the f_rest
+// Adam to the staged rows (phase 2 below), and the rows that are live after this step without a staged row go to `mom` for
+// frest_momentum_kernel. The live byte is set for every row that received a gradient.
 //
 // MODE_DEPTH: dL/dxyz += dL/dz (V[2], V[6], V[10]). A row whose only non-zero sum is slot 11 has a gradient (its parameters are loaded and
 // updated, its live byte set) but no SH gradient: the view-direction term depends on dL/dRGB only, so its f_rest row is not staged.
@@ -188,7 +200,7 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
                                                             StepHyper h, GradSegments grads, DensifyStats st,
                                                             const uint32_t* __restrict__ counters, uint32_t capacity, float4* __restrict__ seeds,
                                                             DpPush dp, unsigned char* __restrict__ adam_live, RegCoef reg,
-                                                            const float* __restrict__ f3d)
+                                                            const float* __restrict__ f3d, MomentumList mom)
 {
 	constexpr bool DEPTH = (MODE & MODE_DEPTH) != 0;
 	constexpr bool AA = (MODE & MODE_AA) != 0;
@@ -202,9 +214,9 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 	constexpr bool LIVE = BASE == MODE_ADAM_LIVE;
 	constexpr bool ADAM = BASE == MODE_ADAM || LIVE;
 	__shared__ __align__(128) float s_p[TB * REST];  // f_rest parameter rows of this block (TMA destination; LIVE: compacted per warp)
-	__shared__ __align__(16) float s_w[TB][SEED];    // seed rows of this block (copied out 128-bit coalesced at the end)
+	__shared__ __align__(16) float s_w[TB][SEED];    // seed rows of this block (copied out 128-bit coalesced at the end; LIVE: read by
+	                                                 // the f_rest Adam phase instead)
 	__shared__ __align__(8) uint64_t s_bar;
-	__shared__ bool s_live[LIVE ? TB : 1];           // LIVE: the row is live after this step (its seed row is written)
 
 	// A binning arena that turned out too small leaves the tile lists incomplete. Fused step: no-op (the host sees the
 	// same counter, grows the arena and repeats the step). Data-parallel modes: this view contributes a ZERO gradient to
@@ -283,15 +295,18 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 			}
 		}
 		// f_rest rows of the rows with non-zero sums -> this warp's 32-row region of s_p, compacted; the copies land while the
-		// geometry backward below runs
+		// geometry backward below runs. Their f_rest moments, which phase 2 reads, are prefetched into L2 at the same time (lanes 0-2:
+		// m, 3-5: v; floats 0, 32 and 44 of a 180-byte row touch each 128-byte line it spans), so that phase 2 waits on L2, not HBM.
 		const int lane = tid & 31, wbase = tid & ~31;
 		const uint32_t ball = __ballot_sync(0xffffffffu, staged);
 		uint32_t b = ball;
 		for (int r = wbase; b != 0u; r++, b &= b - 1u) {
-			const float* src = t.p[2] + (size_t)(base + wbase + __ffs(b) - 1) * REST;
+			const size_t e = (size_t)(base + wbase + __ffs(b) - 1) * REST;
+			const float* src = t.p[2] + e;
 			float* dst = s_p + r * REST;
 			cp_async4(dst + lane, src + lane);
 			if (lane < REST - 32) cp_async4(dst + 32 + lane, src + 32 + lane);
+			if (lane < 6) prefetch_l2_evict_last((lane < 3 ? t.m[2] : t.v[2]) + e + (lane % 3 == 0 ? 0 : lane % 3 == 1 ? 32 : REST - 1));
 		}
 		rest_slot = wbase + __popc(ball & ((1u << lane) - 1u));
 	}
@@ -427,13 +442,14 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 	}
 
 	// ---- the 14 small parameters of this Gaussian
+	bool momentum_only = false;  // LIVE: live after this step, no f_rest row staged
 	if (valid) {
 		// a zero gradient on zero moments is an exact no-op of Adam (see adam4_unless_noop): hidden / never-reached Gaussians are not rewritten
 		bool idle = false;
 		if (LIVE) {
 			if (gnz && !was_live) adam_live[idx] = 1;
 			idle = !(gnz || was_live);
-			s_live[tid] = !idle;
+			momentum_only = !idle && !staged;
 			if (was_live) load_moments();
 		} else if (ADAM) {
 			idle = !(any_nonzero(g) || any_nonzero(m, v));
@@ -445,14 +461,64 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 			store_small(grads.g, idx, g);
 		}
 	}
+
+	if (LIVE) {
+		const int lane = tid & 31, wbase = tid & ~31;
+		// momentum-only rows -> the list, one atomic per warp
+		const uint32_t mball = __ballot_sync(0xffffffffu, momentum_only);
+		if (mball != 0u) {
+			uint32_t at = 0;
+			if (lane == 0) at = atomicAdd(mom.count, (uint32_t)__popc(mball));
+			at = __shfl_sync(0xffffffffu, at, 0);
+			if (momentum_only) mom.rows[at + __popc(mball & ((1u << lane) - 1u))] = (uint32_t)idx;
+		}
+		// ---- phase 2 (LIVE): Adam over this warp's staged f_rest rows, walked as one flat array of n x 45 elements so that no lane
+		// idles on a row's 13-element tail. Parameters from s_p, gradient w_k * gm[ch] from s_w, moments from global memory; a
+		// per-element no-op skip gives the bits of frest_stream_kernel's per-float4 one (g = m = v = 0 leaves p unchanged). The r-th
+		// staged row of the warp is that of lane __fns(sball, 0, r + 1): its seeds are that thread's s_w row, its parameters s_p's row
+		// wbase + r.
+		__syncwarp();  // this warp's s_w rows are written
+		const uint32_t sball = __ballot_sync(0xffffffffu, staged);
+		const int n = __popc(sball) * REST;
+		const float lr_eff = h.lr[2] * ac.inv_bc1;
+		constexpr int U = 2;  // elements per lane in flight (more raise the spills of the variants)
+		for (int f0 = lane; f0 < n; f0 += 32 * U) {
+			uint32_t ge[U], rl[U];  // element index in the f_rest tensors | the row's lane
+			float mm[U], vv[U];
+#pragma unroll
+			for (int u = 0; u < U; u++) {
+				const int f = f0 + 32 * u;
+				if (f < n) {
+					const int r = f / REST;
+					rl[u] = __fns(sball, 0, r + 1);
+					ge[u] = (uint32_t)(base + wbase + rl[u]) * REST + (uint32_t)(f - r * REST);
+					mm[u] = __ldcs(t.m[2] + ge[u]); vv[u] = __ldcs(t.v[2] + ge[u]);
+				}
+			}
+#pragma unroll
+			for (int u = 0; u < U; u++) {
+				const int f = f0 + 32 * u;
+				if (f < n) {
+					const int r = f / REST, e = f - r * REST, k = e / 3;
+					const float* sw = s_w[wbase + rl[u]];
+					const float g = sw[k] * sw[16 + (e - 3 * k)];
+					if (!adam_noop(g, mm[u], vv[u])) {
+						float pp = s_p[(wbase + r) * REST + e];
+						adam1(pp, mm[u], vv[u], g, lr_eff, ac);
+						__stcs(t.p[2] + ge[u], pp); __stcs(t.m[2] + ge[u], mm[u]); __stcs(t.v[2] + ge[u], vv[u]);
+					}
+				}
+			}
+		}
+		return;
+	}
 	__syncthreads();
 
 	if (BASE != MODE_PUSH) {
 		// seed rows of this block -> global, 128-bit coalesced
 		const float4* src = reinterpret_cast<const float4*>(&s_w[0][0]);
 		float4* dst = seeds + (size_t)base * (SEED / 4);
-		for (int i = tid; i < rows * (SEED / 4); i += TB)
-			if (!LIVE || s_live[i / (SEED / 4)]) dst[i] = src[i];  // (LIVE: frest_stream_kernel reads no seed row of a row that is not live)
+		for (int i = tid; i < rows * (SEED / 4); i += TB) dst[i] = src[i];
 		return;
 	}
 	// MODE_PUSH: the block's records go straight into the inbox of the rank that owns this 128-Gaussian chunk (remote
@@ -473,31 +539,24 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 
 // Adam over the f_rest rows of Gaussians [first, P) (ADAM) or their gradient written out
 // (!ADAM), one float4 per thread. The gradient of element (row, k, ch) is seed[row][k-1] * seed[row][16+ch].
-// ADAM with `live` (psb_model.adam_live, as left by gaussian_backward_kernel<MODE_ADAM_LIVE>): a row whose byte is 0 has zero
-// moments and no gradient (and no seed row written in this step): its elements are a no-op, the thread reads nothing else for them.
+// (MODE_ADAM_LIVE updates the f_rest rows in gaussian_backward_kernel and frest_momentum_kernel instead.)
 template <bool ADAM>
 __global__ void __launch_bounds__(256) frest_stream_kernel(uint32_t e_first, uint32_t e_end, float* __restrict__ p, float* __restrict__ m, float* __restrict__ v,
                                                            float* __restrict__ gout, const float* __restrict__ seeds, float lr_eff, AdamCoef ac,
-                                                           const uint32_t* __restrict__ counters, uint32_t capacity, const unsigned char* __restrict__ live)
+                                                           const uint32_t* __restrict__ counters, uint32_t capacity)
 {
 	if (ADAM && counters[0] > capacity) return;  // overflowing fused step: no-op (see gaussian_backward_kernel; !ADAM: the seeds are zero)
 	const uint32_t e = e_first + 4u * (blockIdx.x * 256u + threadIdx.x);
 	if (e >= e_end) return;
 	uint32_t row = e / REST;
 	int c = (int)(e - row * REST);
-	bool lv = true, lv_next = true;  // the float4 covers one row or the end of one and the start of the next
-	if (ADAM && live) {
-		lv = live[row] != 0;
-		lv_next = live[min(e + 3u, e_end - 1u) / REST] != 0;
-		if (!lv && !lv_next) return;
-	}
 	const float* sd = seeds + (size_t)row * SEED;
 	float g[4];
 #pragma unroll
 	for (int j = 0; j < 4; j++) {
 		const int k = c / 3, ch = c - 3 * k;
-		g[j] = lv ? sd[k] * sd[16 + ch] : 0.f;
-		if (++c == REST) { c = 0; sd += SEED; lv = lv_next; }
+		g[j] = sd[k] * sd[16 + ch];
+		if (++c == REST) { c = 0; sd += SEED; }
 	}
 	if (e + 4 <= e_end) {
 		if (ADAM) {
@@ -510,6 +569,32 @@ __global__ void __launch_bounds__(256) frest_stream_kernel(uint32_t e_first, uin
 		for (uint32_t j = 0; e + j < e_end; j++) {
 			if (ADAM) adam1(p[e + j], m[e + j], v[e + j], g[j], lr_eff, ac);
 			else gout[e + j] = g[j];
+		}
+	}
+}
+
+// MODE_ADAM_LIVE: Adam with a zero gradient over the f_rest rows of the momentum-only rows gaussian_backward_kernel listed (see
+// MomentumList), one warp per row over a fixed grid; lanes take elements lane and lane + 32 of the 45. An overflowing step is a no-op.
+constexpr int MOM_THREADS = 256;
+__global__ void __launch_bounds__(MOM_THREADS) frest_momentum_kernel(MomentumList mom, float* __restrict__ p, float* __restrict__ m, float* __restrict__ v,
+                                                                     float lr_eff, AdamCoef ac, const uint32_t* __restrict__ counters, uint32_t capacity)
+{
+	if (counters[0] > capacity) return;
+	const uint32_t n = *mom.count;
+	const int lane = threadIdx.x & 31;
+	const uint32_t nwarps = gridDim.x * (MOM_THREADS / 32);
+	for (uint32_t i = blockIdx.x * (MOM_THREADS / 32) + threadIdx.x / 32; i < n; i += nwarps) {
+		const uint32_t e0 = mom.rows[i] * REST + lane, e1 = e0 + 32;
+		const bool two = lane < REST - 32;
+		float p0 = __ldcs(p + e0), m0 = __ldcs(m + e0), v0 = __ldcs(v + e0), p1 = 0.f, m1 = 0.f, v1 = 0.f;
+		if (two) { p1 = __ldcs(p + e1); m1 = __ldcs(m + e1); v1 = __ldcs(v + e1); }
+		if (!adam_noop(0.f, m0, v0)) {
+			adam1(p0, m0, v0, 0.f, lr_eff, ac);
+			__stcs(p + e0, p0); __stcs(m + e0, m0); __stcs(v + e0, v0);
+		}
+		if (two && !adam_noop(0.f, m1, v1)) {
+			adam1(p1, m1, v1, 0.f, lr_eff, ac);
+			__stcs(p + e1, p1); __stcs(m + e1, m1); __stcs(v + e1, v1);
 		}
 	}
 }
@@ -736,13 +821,14 @@ void run_gaussian_backward(int first, int P, cudaStream_t stream, Args... args)
 // MODE_PUSH optionally | MODE_REG, | MODE_F3D and | MODE_NORMAL)
 int launch_gaussian_backward(int mode, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink,
                              const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
-                             float* seeds, const DpPush& dp, unsigned char* adam_live, cudaStream_t stream, const RegCoef& reg, const float* f3d)
+                             float* seeds, const DpPush& dp, unsigned char* adam_live, cudaStream_t stream, const RegCoef& reg, const float* f3d,
+                             const MomentumList& mom)
 {
 	if (P - first <= 0) return 0;
 	float4* sink4 = reinterpret_cast<float4*>(sink);
 	float4* seeds4 = reinterpret_cast<float4*>(seeds);
 #define PSB_BACKWARD_CASE(M) \
-	case M: run_gaussian_backward<M>(first, P, stream, t, cam, geom, sink4, h, grads, st, counters, capacity, seeds4, dp, adam_live, reg, f3d); break
+	case M: run_gaussian_backward<M>(first, P, stream, t, cam, geom, sink4, h, grads, st, counters, capacity, seeds4, dp, adam_live, reg, f3d, mom); break
 #define PSB_BACKWARD_CASE_F3D(M) PSB_BACKWARD_CASE(M); PSB_BACKWARD_CASE(M | MODE_F3D)
 #define PSB_BACKWARD_CASE_REG(M) PSB_BACKWARD_CASE_F3D(M); PSB_BACKWARD_CASE_F3D(M | MODE_REG)
 #define PSB_BACKWARD_CASE_NRM(M) PSB_BACKWARD_CASE_REG(M | MODE_NORMAL); PSB_BACKWARD_CASE_REG(M | MODE_NORMAL | MODE_DEPTH); \
@@ -804,15 +890,27 @@ int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, co
 	unsigned char* live = adam ? adam_live : nullptr;
 	const int variant = (live ? MODE_ADAM_LIVE : adam ? MODE_ADAM : MODE_GRADS) | (mode.depth ? MODE_DEPTH : 0) | (mode.aa ? MODE_AA : 0) |
 	                    (reg.opacity != 0.f || reg.scale != 0.f ? MODE_REG : 0) | (mode.f3d ? MODE_F3D : 0) | (mode.normal ? MODE_NORMAL : 0);
+	// LIVE writes no seed rows: the seed scratch ([P][20] floats) holds the momentum-only list instead
+	const MomentumList mom = {reinterpret_cast<uint32_t*>(seeds), reinterpret_cast<uint32_t*>(seeds) + P};
+	if (live) PSB_CUDA_OK(cudaMemsetAsync(mom.count, 0, sizeof(uint32_t), stream));
 	int rc;
-	if ((rc = launch_gaussian_backward(variant, first, P, t, cam, geom, sink, h, grads, st, counters, capacity, seeds, nodp, live, stream, reg, mode.f3d)))
+	if ((rc = launch_gaussian_backward(variant, first, P, t, cam, geom, sink, h, grads, st, counters, capacity, seeds, nodp, live, stream, reg, mode.f3d,
+	                                   mom)))
 		return rc;
 	if (between) cudaEventRecord(between, stream);
 	const AdamCoef ac(h);
+	if (live) {
+		int dev = 0, sms = 0;  // grid: a full SM's worth of threads on every SM (the list length is known on the device only)
+		PSB_CUDA_OK(cudaGetDevice(&dev));
+		PSB_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+		frest_momentum_kernel<<<sms * (2048 / MOM_THREADS), MOM_THREADS, 0, stream>>>(mom, t.p[2], t.m[2], t.v[2], h.lr[2] * ac.inv_bc1, ac, counters, capacity);
+		PSB_LAUNCH_OK();
+		return 0;
+	}
 	const uint32_t e0 = (uint32_t)first * REST, e1 = (uint32_t)P * REST;
 	const unsigned gridB = (unsigned)(((size_t)(e1 - e0) + 1023) / 1024);
-	if (adam) frest_stream_kernel<true><<<gridB, 256, 0, stream>>>(e0, e1, t.p[2], t.m[2], t.v[2], nullptr, seeds, h.lr[2] * ac.inv_bc1, ac, counters, capacity, live);
-	else frest_stream_kernel<false><<<gridB, 256, 0, stream>>>(e0, e1, nullptr, nullptr, nullptr, grads.g[2], seeds, 0.f, ac, counters, capacity, nullptr);
+	if (adam) frest_stream_kernel<true><<<gridB, 256, 0, stream>>>(e0, e1, t.p[2], t.m[2], t.v[2], nullptr, seeds, h.lr[2] * ac.inv_bc1, ac, counters, capacity);
+	else frest_stream_kernel<false><<<gridB, 256, 0, stream>>>(e0, e1, nullptr, nullptr, nullptr, grads.g[2], seeds, 0.f, ac, counters, capacity);
 	PSB_LAUNCH_OK();
 	return 0;
 }
@@ -834,7 +932,7 @@ int launch_push_backward(int P, const TrainTensors& t, const Camera& cam, const 
 	if (mode.f3d) { set_error_msg("launch_push_backward: the 3D filter is not wired into the NVLink step"); return -1; }
 	if (mode.normal) { set_error_msg("launch_push_backward: the normal term is not wired into the NVLink step"); return -1; }
 	if ((rc = launch_gaussian_backward(MODE_PUSH | (mode.depth ? MODE_DEPTH : 0) | (mode.aa ? MODE_AA : 0), 0, P, t, cam, geom, sink, h, nog, st, counters, capacity, nullptr, dp,
-	                                   nullptr, stream, RegCoef{0.f, 0.f}, nullptr)))
+	                                   nullptr, stream, RegCoef{0.f, 0.f}, nullptr, MomentumList{})))
 		return rc;
 	return launch_signal(dp.grad_flag, dp.meta, cam.campos, h.D, dp.world, dp.rank, dp.epoch, stream);
 }

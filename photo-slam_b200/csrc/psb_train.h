@@ -76,7 +76,8 @@ int launch_shard_adam(const DpShard& d, const TrainTensors& t, const StepHyper& 
 int launch_wait_flags(const uint32_t* flags, int world, uint32_t epoch, uint32_t* status, cudaStream_t stream);
 
 // Gaussians [first, P) (first must be a multiple of 128 so f_rest chunks stay 16-byte aligned)
-// seeds: scratch [P][20] floats (per-Gaussian SH gradient seeds handed from the per-Gaussian kernel to the f_rest stream kernel)
+// seeds: scratch [P][20] floats (per-Gaussian SH gradient seeds handed from the per-Gaussian kernel to the f_rest stream kernel; with
+// adam_live, the momentum-only row list of frest_momentum_kernel and its length instead)
 int launch_fused_backward(bool adam, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, float* seeds,
                           const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
                           cudaStream_t stream, cudaEvent_t between /* recorded between the two kernels (stage timing), or null */,
