@@ -190,6 +190,81 @@ int psb_rasterize_backward_aa(int P, int D, int M, int R,
                               const float* dL_ddepth, float* dL_dz, void* det_scratch, size_t det_scratch_bytes,
                               int antialiasing, void* stream);
 
+/*
+ * Opacity, normals and the second depth moment on the operator path: the planes the fused training step renders
+ * (psb_trainer_forward, psb_trainer_forward_normal, psb_trainer_forward_moment), formed from the operator's inputs, culls, full-rectangle
+ * instance lists and blend order. Per pixel p, over the Gaussians i that blend there with alpha_i and transmittance T_i:
+ *   A(p)   = 1 - T_final(p)                the accumulated opacity; no background term (the colour keeps its own)
+ *   N_c(p) = sum_i n_ic alpha_i T_i        [3,H,W], no background term
+ *   M(p)   = sum_i z_i^2 alpha_i T_i       the second depth moment, with the z and alpha of D; no background term
+ * n_i = +-V r_k: r_k is the column of R(q) belonging to the smallest of the three activated scales (ties: the lowest index), q the
+ * rotation input as given (neither the operator's covariance nor the reference's computeCov3D normalises it; scale_modifier does not
+ * change the arg-min), V the view rotation; the sign makes n_i . t_i <= 0, t_i the view-space mean. With antialiasing = 1 every plane
+ * blends with o h, as the colour does. dL/dn reaches `rotations` only: the arg-min and the sign are piecewise constant. N needs scales
+ * and rotations; A and M work for every input combination.
+ *
+ * psb_rasterize_planes_bytes: the plane_scratch that the normal plane needs, a pure function of (P, R): 16 B per Gaussian for n_i,
+ * 12 B per Gaussian for dL/dn and, for the deterministic backward, 64 B per instance (pass R = 0 for the forward and the atomic
+ * backward), plus alignment. Only calls that render N or take dL/dN read plane_scratch; its contents are irrelevant.
+ *
+ * psb_rasterize_forward_planes: the argument list of psb_rasterize_forward_aa with out_depth moved into `planes` (NULL record or NULL
+ * field = not rendered), plus plane_scratch, plane_scratch_bytes (device, at least psb_rasterize_planes_bytes(P, 0) bytes with
+ * out_normal). Without planes it is psb_rasterize_forward_aa bit for bit; with them, colour, radii, num_rendered, the scratch
+ * contents and D are bit-identical to it.
+ *
+ * psb_rasterize_backward_planes: the argument list of psb_rasterize_backward_aa with dL_ddepth moved into `grads` (NULL record or NULL
+ * field = no gradient), plus plane_scratch, plane_scratch_bytes (at least psb_rasterize_planes_bytes(P, deterministic ? R : 0) bytes
+ * with dL_dnormal) and `deterministic` (0 or 1; 1 needs det_scratch as in psb_rasterize_backward_deterministic and is bit-identical
+ * from call to call; 0 ignores det_scratch). dL_dz [P], caller-allocated and zeroed, is required with dL_ddepth or dL_ddepth2: dM/dz =
+ * 2 z alpha T joins dL/dz, which is folded into dL_dmean3D. dL/dA and the alpha-part of dL/dM join every splat's dL/dalpha, so they
+ * reach dL_dopacity, dL_dmean2D, dL_dconic and through them the covariance inputs. dL/dn is folded into dL_drot. Without gradients it is
+ * psb_rasterize_backward_aa bit for bit (with det_scratch only when deterministic = 1).
+ *
+ * Both return PSB_ERR_ARG, before any CUDA call, for everything the calls they extend reject, an antialiasing or deterministic value
+ * other than 0 or 1, N or dL/dN with cov3D_precomp, a missing or too small plane_scratch with N or dL/dN, dL_ddepth or dL_ddepth2
+ * without dL_dz, and dL_dnormal without dL_drot. The scratch sizes psb_geometry_bytes, psb_binning_bytes, psb_image_bytes and
+ * psb_rasterize_backward_det_bytes do not change.
+ */
+typedef struct psb_raster_planes {
+	float* out_depth;   /* [H,W] D, as psb_rasterize_forward_depth */
+	float* out_alpha;   /* [H,W] A */
+	float* out_normal;  /* [3,H,W] N */
+	float* out_depth2;  /* [H,W] M */
+} psb_raster_planes;
+typedef struct psb_raster_plane_grads {
+	const float* dL_ddepth;   /* [H,W] */
+	const float* dL_dalpha;   /* [H,W] */
+	const float* dL_dnormal;  /* [3,H,W] */
+	const float* dL_ddepth2;  /* [H,W] */
+} psb_raster_plane_grads;
+size_t psb_rasterize_planes_bytes(int P, int R);
+int psb_rasterize_forward_planes(psb_alloc_fn geometry_buffer, void* geometry_user,
+                                 psb_alloc_fn binning_buffer, void* binning_user,
+                                 psb_alloc_fn image_buffer, void* image_user,
+                                 int P, int D, int M,
+                                 const float* background, int width, int height,
+                                 const float* means3D, const float* shs, const float* colors_precomp,
+                                 const float* opacities, const float* scales, float scale_modifier,
+                                 const float* rotations, const float* cov3D_precomp,
+                                 const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+                                 float tan_fovx, float tan_fovy, int prefiltered,
+                                 float* out_color, int* radii, const psb_raster_planes* planes,
+                                 void* plane_scratch, size_t plane_scratch_bytes, int antialiasing, void* stream);
+int psb_rasterize_backward_planes(int P, int D, int M, int R,
+                                  const float* background, int width, int height,
+                                  const float* means3D, const float* shs, const float* colors_precomp,
+                                  const float* scales, float scale_modifier, const float* rotations,
+                                  const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix,
+                                  const float* campos, float tan_fovx, float tan_fovy, const int* radii,
+                                  char* geom_buffer, char* binning_buffer, char* image_buffer,
+                                  const float* dL_dpix,
+                                  float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
+                                  float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
+                                  const psb_raster_plane_grads* grads, float* dL_dz,
+                                  void* det_scratch, size_t det_scratch_bytes,
+                                  void* plane_scratch, size_t plane_scratch_bytes,
+                                  int antialiasing, int deterministic, void* stream);
+
 /* Near-plane visibility (view z > 0.2). Replaces CudaRasterizer::Rasterizer::markVisible
  * (cuda_rasterizer/rasterizer.h:24-29, rasterizer_impl.cu:141-153). present: [P] bytes (bool), device. */
 int psb_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,

@@ -10,6 +10,16 @@ ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_size_t, C.c_void_p)
 _lib = None
 
 
+class RasterPlanes(C.Structure):
+    """psb_raster_planes: the planes psb_rasterize_forward_planes renders beside colour (device pointers; None = not rendered)."""
+    _fields_ = [("out_depth", C.c_void_p), ("out_alpha", C.c_void_p), ("out_normal", C.c_void_p), ("out_depth2", C.c_void_p)]
+
+
+class RasterPlaneGrads(C.Structure):
+    """psb_raster_plane_grads: the plane gradients psb_rasterize_backward_planes takes (device pointers; None = no gradient)."""
+    _fields_ = [("dL_ddepth", C.c_void_p), ("dL_dalpha", C.c_void_p), ("dL_dnormal", C.c_void_p), ("dL_ddepth2", C.c_void_p)]
+
+
 class PsbError(RuntimeError):
     pass
 
@@ -52,6 +62,15 @@ def lib():
     L.psb_rasterize_forward_aa.argtypes = L.psb_rasterize_forward_depth.argtypes[:-1] + [C.c_int, vp]
     L.psb_rasterize_backward_aa.restype = C.c_int
     L.psb_rasterize_backward_aa.argtypes = L.psb_rasterize_backward_deterministic.argtypes[:-1] + [C.c_int, vp]
+    # opacity, normals and the second depth moment: the _aa argument lists with out_depth / dL_ddepth moved into a record (passed by
+    # pointer), plus plane_scratch, plane_scratch_bytes (and `deterministic` on the backward)
+    L.psb_rasterize_planes_bytes.restype = C.c_size_t
+    L.psb_rasterize_planes_bytes.argtypes = [C.c_int, C.c_int]
+    L.psb_rasterize_forward_planes.restype = C.c_int
+    L.psb_rasterize_forward_planes.argtypes = L.psb_rasterize_forward.argtypes[:-1] + [C.POINTER(RasterPlanes), vp, C.c_size_t, C.c_int, vp]
+    L.psb_rasterize_backward_planes.restype = C.c_int
+    L.psb_rasterize_backward_planes.argtypes = L.psb_rasterize_backward.argtypes[:-1] + [
+        C.POINTER(RasterPlaneGrads), fp, vp, C.c_size_t, vp, C.c_size_t, C.c_int, C.c_int, vp]
     L.psb_mark_visible.restype = C.c_int
     L.psb_mark_visible.argtypes = [C.c_int, fp, fp, fp, u8p, vp]
     L.psb_debug_export.restype = C.c_int

@@ -66,13 +66,25 @@ static int arg_error(const char* fn, const char* what)
 	return PSB_ERR_ARG;
 }
 
-// Body of psb_rasterize_forward[_depth|_aa]; fn names the entry point in error messages. out_depth [H,W] or NULL; aa: the 2D Mip filter.
+// Planes of the operator forward beyond colour (include/psb200.h psb_raster_planes; NULL = not rendered). normal_scratch / normal_bytes:
+// the caller's scratch of psb_rasterize_planes_bytes(P, 0) bytes, read only with the normal plane.
+struct FwdPlanes {
+	float *depth, *alpha, *normal, *depth2;
+	void* normal_scratch;
+	size_t normal_bytes;
+};
+
+// Scratch bytes of the operator's normal plane; 0 for a negative size.
+static size_t op_plane_bytes(int P, int R) { return (P < 0 || R < 0) ? 0 : OpPlaneState::required_bytes((size_t)P, (size_t)R); }
+
+// Body of psb_rasterize_forward[_depth|_aa|_planes]; fn names the entry point in error messages. pl: the planes beyond colour; aa: the
+// 2D Mip filter.
 static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void* geometry_user, psb_alloc_fn binning_buffer, void* binning_user,
                              psb_alloc_fn image_buffer, void* image_user, int P, int D, int M, const float* background, int width, int height,
                              const float* means3D, const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
                              float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
                              const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered, float* out_color,
-                             int* radii, float* out_depth, bool aa, void* stream_)
+                             int* radii, const FwdPlanes& pl, bool aa, void* stream_)
 {
 	(void)prefiltered;  // the reference only uses it for a device-side assert (auxiliary.h:156-160)
 	cudaStream_t stream = (cudaStream_t)stream_;
@@ -83,6 +95,10 @@ static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void*
 	if (P > 0 && shs && (M < (D + 1) * (D + 1) || D > 3 || D < 0)) return arg_error(fn, "SH degree / coefficient count mismatch");
 	if (P > 0 && shs && !cam_pos) return arg_error(fn, "cam_pos required with shs");
 	if (width > 65535 * 16 || height > 65535 * 16) return arg_error(fn, "image too large");
+	if (pl.normal && cov3D_precomp) return arg_error(fn, "the normal plane needs scales and rotations, not cov3D_precomp");
+	if (pl.normal && (!pl.normal_scratch || pl.normal_bytes < op_plane_bytes(P, 0)))
+		return arg_error(fn, ("the normal plane needs a plane_scratch of psb_rasterize_planes_bytes(P, 0) = " + std::to_string(op_plane_bytes(P, 0)) +
+		                      " bytes").c_str());
 
 	const Camera cam = make_camera(width, height, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy);
 	if ((size_t)cam.grid_x * cam.grid_y >= (1u << 24)) return arg_error(fn, "more than 2^24 tiles");
@@ -96,6 +112,12 @@ static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void*
 	const GaussIn in = make_input(P, D, M, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp);
 	int rc;
 	if ((rc = launch_preprocess(in, cam, radii, geom, /*raw=*/false, /*tight=*/false, stream, aa))) return rc;
+	float4* normals = nullptr;
+	if (pl.normal) {
+		char* chunk = static_cast<char*>(pl.normal_scratch);
+		normals = OpPlaneState::from_chunk(chunk, (size_t)P, 0).normals;
+		if ((rc = launch_op_normals(in, cam, geom.tile_info, normals, stream))) return rc;
+	}
 	if ((rc = launch_depth_sort_and_scan(P, geom, /*scan=*/true, stream))) return rc;
 
 	uint32_t num_rendered = 0;
@@ -110,7 +132,8 @@ static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void*
 	BinState bin = BinState::from_chunk(bin_chunk, (size_t)num_rendered);
 	if ((rc = launch_binning(P, cam, geom, bin, img, (size_t)num_rendered, stream))) return rc;
 
-	if ((rc = launch_render_forward(cam, img.ranges, bin.inst[sorted_slot(width, height)], geom.rec, background, out_color, img.final_T, img.n_contrib, stream, out_depth)))
+	if ((rc = launch_render_forward(cam, img.ranges, bin.inst[sorted_slot(width, height)], geom.rec, background, out_color, img.final_T, img.n_contrib, stream,
+	                                pl.depth, pl.alpha, /*score=*/nullptr, normals, pl.normal, pl.depth2)))
 		return rc;
 	return (int)num_rendered;
 }
@@ -119,16 +142,21 @@ static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void*
 static size_t op_det_bytes(int P, int R) { return (P < 0 || R < 0) ? 0 : OpDetState::required_bytes((size_t)P, (size_t)R); }
 
 // What an entry point adds to the plain backward. dL_ddepth [H,W] or NULL; with it, dL_dz [P] receives dL/dz and the depth variants
-// run. det: the deterministic variant over det_scratch (det_bytes: its size). aa: the forward was anti-aliased.
+// run. det: the deterministic variant over det_scratch (det_bytes: its size). aa: the forward was anti-aliased. dL_dalpha, dL_dnormal,
+// dL_ddepth2: the gradients of the other planes (psb_raster_plane_grads); dL_ddepth2 also needs dL_dz, dL_dnormal a plane_scratch of
+// psb_rasterize_planes_bytes(P, det ? R : 0) bytes (plane_bytes: its size).
 struct BwdVariant {
 	const float* dL_ddepth;
 	float* dL_dz;
 	void* det_scratch;
 	size_t det_bytes;
 	bool det, aa;
+	const float *dL_dalpha, *dL_dnormal, *dL_ddepth2;
+	void* plane_scratch;
+	size_t plane_bytes;
 };
 
-// Body of psb_rasterize_backward[_depth|_deterministic|_aa]; fn names the entry point in error messages. Every argument check comes
+// Body of psb_rasterize_backward[_depth|_deterministic|_aa|_planes]; fn names the entry point in error messages. Every argument check comes
 // before any CUDA call.
 static int rasterize_backward(const char* fn, int P, int D, int M, int R, const float* background, int width, int height, const float* means3D,
                               const float* shs, const float* colors_precomp, const float* scales, float scale_modifier, const float* rotations,
@@ -141,10 +169,19 @@ static int rasterize_backward(const char* fn, int P, int D, int M, int R, const 
 	cudaStream_t stream = (cudaStream_t)stream_;
 	const float* dL_ddepth = v.dL_ddepth;
 	float* dL_dz = v.dL_dz;
+	const bool normal = v.dL_dnormal != nullptr;
 	if (dL_ddepth && !dL_dz) return arg_error(fn, "dL_ddepth needs a dL_dz array");
+	if (v.dL_ddepth2 && !dL_dz) return arg_error(fn, "dL_ddepth2 needs a dL_dz array");
+	if (normal && cov3D_precomp) return arg_error(fn, "dL_dnormal needs scales and rotations, not cov3D_precomp");
+	if (normal && !dL_drot) return arg_error(fn, "dL_dnormal needs a dL_drot array");
 	if (P == 0) return 0;
 	if (P < 0 || R < 0 || !geom_buffer || !binning_buffer || !image_buffer || !dL_dpix || !dL_dmean2D || !dL_dconic || !dL_dopacity || !dL_dcolor)
 		return arg_error(fn, "bad argument");
+	if (normal && (!scales || !rotations)) return arg_error(fn, "dL_dnormal needs scales and rotations");
+	const int plane_R = v.det ? R : 0;
+	if (normal && (!v.plane_scratch || v.plane_bytes < op_plane_bytes(P, plane_R)))
+		return arg_error(fn, ("dL_dnormal needs a plane_scratch of psb_rasterize_planes_bytes(P, " + std::string(v.det ? "R" : "0") + ") = " +
+		                      std::to_string(op_plane_bytes(P, plane_R)) + " bytes").c_str());
 	if (v.det && !v.det_scratch) return arg_error(fn, "det_scratch is NULL");
 	if (v.det && v.det_bytes < op_det_bytes(P, R))
 		return arg_error(fn, ("det_scratch holds " + std::to_string(v.det_bytes) + " bytes, psb_rasterize_backward_det_bytes(P, R) = " +
@@ -160,8 +197,18 @@ static int rasterize_backward(const char* fn, int P, int D, int M, int R, const 
 	sink.opacity = dL_dopacity; sink.opacity_stride = 1;
 	sink.color = dL_dcolor; sink.color_stride = 3;
 	sink.packed = 0;
-	if (dL_ddepth) { sink.z = dL_dz; sink.z_stride = 1; }
+	const bool depth = dL_ddepth || v.dL_ddepth2;
+	if (depth) { sink.z = dL_dz; sink.z_stride = 1; }
+	const GaussIn in = make_input(P, D, M, means3D, shs, colors_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp);
+	OpPlaneState ps{};
 	int rc;
+	if (normal) {
+		// n_i is a function of the inputs: recomputed here rather than kept from the forward (the scratch sizes stay functions of P / R / W H)
+		char* chunk = static_cast<char*>(v.plane_scratch);
+		ps = OpPlaneState::from_chunk(chunk, (size_t)P, (size_t)plane_R);
+		PSB_CUDA_OK(cudaMemsetAsync(ps.dn, 0, (size_t)P * 3 * sizeof(float), stream));
+		if ((rc = launch_op_normals(in, cam, geom.tile_info, ps.normals, stream))) return rc;
+	}
 	if (R > 0) {
 		DetSlots slots{};
 		if (v.det) {
@@ -170,22 +217,23 @@ static int rasterize_backward(const char* fn, int P, int D, int M, int R, const 
 			// every call: a block handed back by the caller's allocator may hold tags of an earlier call, which the fixed seq would accept.
 			char* chunk = static_cast<char*>(v.det_scratch);
 			const OpDetState ds = OpDetState::from_chunk(chunk, (size_t)P, (size_t)R);
-			PSB_CUDA_OK(cudaMemsetAsync(ds.slots, 0, (size_t)R * 3 * sizeof(float4), stream));
+			// (the normal variant's 64-byte slots live in the plane scratch; ds.slots is then unused)
+			float4* slot_rows = normal ? ps.slots : ds.slots;
+			PSB_CUDA_OK(cudaMemsetAsync(slot_rows, 0, (size_t)R * (normal ? 4 : 3) * sizeof(float4), stream));
 			if ((rc = launch_det_base(P, geom, ds.base, stream))) return rc;
-			slots.slots = ds.slots; slots.base = ds.base; slots.tile_info = geom.tile_info; slots.counters = geom.counters;
+			slots.slots = slot_rows; slots.base = ds.base; slots.tile_info = geom.tile_info; slots.counters = geom.counters;
 			slots.capacity = (uint32_t)R; slots.seq = 1u; slots.P = P; slots.tight = 0;
 		}
 		if ((rc = launch_render_backward(cam, img.ranges, bin.inst[sorted_slot(width, height)], geom.rec, background, img.final_T, img.n_contrib, dL_dpix,
-		                                 sink, stream, dL_ddepth, v.det ? &slots : nullptr)))
+		                                 sink, stream, dL_ddepth, v.det ? &slots : nullptr, v.dL_dalpha, ps.normals, v.dL_dnormal, v.dL_ddepth2, ps.dn)))
 			return rc;
 	}
 
-	const GaussIn in = make_input(P, D, M, means3D, shs, colors_precomp, nullptr, scales, scale_modifier, rotations, cov3D_precomp);
 	GaussGradOut out;
 	out.dL_dmeans3D = dL_dmean3D; out.dL_dcov3D = dL_dcov3D; out.dL_dsh = dL_dsh; out.dL_dscales = dL_dscale; out.dL_drots = dL_drot;
 	// (AA: dL_dopacity holds dL/do' here, the per-Gaussian kernel turns it into dL/do)
-	if ((rc = launch_preprocess_backward(in, cam, geom, dL_dmean2D, 3, dL_dconic, 4, dL_dcolor, 3, out, stream, dL_ddepth ? dL_dz : nullptr,
-	                                     v.aa ? dL_dopacity : nullptr)))
+	if ((rc = launch_preprocess_backward(in, cam, geom, dL_dmean2D, 3, dL_dconic, 4, dL_dcolor, 3, out, stream, depth ? dL_dz : nullptr,
+	                                     v.aa ? dL_dopacity : nullptr, normal ? ps.dn : nullptr)))
 		return rc;
 	return 0;
 }
@@ -212,7 +260,7 @@ int psb_rasterize_forward(psb_alloc_fn geometry_buffer, void* geometry_user, psb
 {
 	return rasterize_forward("psb_rasterize_forward", geometry_buffer, geometry_user, binning_buffer, binning_user, image_buffer, image_user, P, D, M,
 	                         background, width, height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp,
-	                         viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, /*out_depth=*/nullptr, /*aa=*/false, stream);
+	                         viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, FwdPlanes{}, /*aa=*/false, stream);
 }
 
 int psb_rasterize_forward_depth(psb_alloc_fn geometry_buffer, void* geometry_user, psb_alloc_fn binning_buffer, void* binning_user,
@@ -224,7 +272,7 @@ int psb_rasterize_forward_depth(psb_alloc_fn geometry_buffer, void* geometry_use
 {
 	return rasterize_forward("psb_rasterize_forward_depth", geometry_buffer, geometry_user, binning_buffer, binning_user, image_buffer, image_user, P,
 	                         D, M, background, width, height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations,
-	                         cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, out_depth, /*aa=*/false, stream);
+	                         cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, FwdPlanes{out_depth}, /*aa=*/false, stream);
 }
 
 int psb_rasterize_backward(int P, int D, int M, int R, const float* background, int width, int height, const float* means3D, const float* shs,
@@ -286,7 +334,7 @@ int psb_rasterize_forward_aa(psb_alloc_fn geometry_buffer, void* geometry_user, 
 	if (antialiasing != 0 && antialiasing != 1) return arg_error("psb_rasterize_forward_aa", "antialiasing must be 0 or 1");
 	return rasterize_forward("psb_rasterize_forward_aa", geometry_buffer, geometry_user, binning_buffer, binning_user, image_buffer, image_user, P, D,
 	                         M, background, width, height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp,
-	                         viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, out_depth, antialiasing != 0, stream);
+	                         viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, FwdPlanes{out_depth}, antialiasing != 0, stream);
 }
 
 int psb_rasterize_backward_aa(int P, int D, int M, int R, const float* background, int width, int height, const float* means3D, const float* shs,
@@ -303,6 +351,49 @@ int psb_rasterize_backward_aa(int P, int D, int M, int R, const float* backgroun
 	v.dL_ddepth = dL_ddepth; v.dL_dz = dL_dz;
 	v.det = det_scratch != nullptr; v.det_scratch = det_scratch; v.det_bytes = det_scratch_bytes;
 	v.aa = antialiasing != 0;
+	return rasterize_backward(fn, P, D, M, R, background, width, height, means3D, shs, colors_precomp, scales, scale_modifier, rotations, cov3D_precomp,
+	                          viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dmean2D,
+	                          dL_dconic, dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, v, stream);
+}
+
+size_t psb_rasterize_planes_bytes(int P, int R) { return op_plane_bytes(P, R); }
+
+int psb_rasterize_forward_planes(psb_alloc_fn geometry_buffer, void* geometry_user, psb_alloc_fn binning_buffer, void* binning_user,
+                                 psb_alloc_fn image_buffer, void* image_user, int P, int D, int M, const float* background, int width, int height,
+                                 const float* means3D, const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
+                                 float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
+                                 const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered, float* out_color,
+                                 int* radii, const psb_raster_planes* planes, void* plane_scratch, size_t plane_scratch_bytes, int antialiasing,
+                                 void* stream)
+{
+	const char* fn = "psb_rasterize_forward_planes";
+	if (antialiasing != 0 && antialiasing != 1) return arg_error(fn, "antialiasing must be 0 or 1");
+	FwdPlanes pl{};
+	if (planes) { pl.depth = planes->out_depth; pl.alpha = planes->out_alpha; pl.normal = planes->out_normal; pl.depth2 = planes->out_depth2; }
+	pl.normal_scratch = plane_scratch; pl.normal_bytes = plane_scratch_bytes;
+	return rasterize_forward(fn, geometry_buffer, geometry_user, binning_buffer, binning_user, image_buffer, image_user, P, D, M, background, width,
+	                         height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix,
+	                         cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, pl, antialiasing != 0, stream);
+}
+
+int psb_rasterize_backward_planes(int P, int D, int M, int R, const float* background, int width, int height, const float* means3D, const float* shs,
+                                  const float* colors_precomp, const float* scales, float scale_modifier, const float* rotations,
+                                  const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix, const float* campos, float tan_fovx,
+                                  float tan_fovy, const int* radii, char* geom_buffer, char* binning_buffer, char* image_buffer, const float* dL_dpix,
+                                  float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dmean3D, float* dL_dcov3D,
+                                  float* dL_dsh, float* dL_dscale, float* dL_drot, const psb_raster_plane_grads* grads, float* dL_dz,
+                                  void* det_scratch, size_t det_scratch_bytes, void* plane_scratch, size_t plane_scratch_bytes, int antialiasing,
+                                  int deterministic, void* stream)
+{
+	const char* fn = "psb_rasterize_backward_planes";
+	if (antialiasing != 0 && antialiasing != 1) return arg_error(fn, "antialiasing must be 0 or 1");
+	if (deterministic != 0 && deterministic != 1) return arg_error(fn, "deterministic must be 0 or 1");
+	BwdVariant v{};
+	if (grads) { v.dL_ddepth = grads->dL_ddepth; v.dL_dalpha = grads->dL_dalpha; v.dL_dnormal = grads->dL_dnormal; v.dL_ddepth2 = grads->dL_ddepth2; }
+	v.dL_dz = dL_dz;
+	v.det = deterministic != 0; v.det_scratch = det_scratch; v.det_bytes = det_scratch_bytes;
+	v.aa = antialiasing != 0;
+	v.plane_scratch = plane_scratch; v.plane_bytes = plane_scratch_bytes;
 	return rasterize_backward(fn, P, D, M, R, background, width, height, means3D, shs, colors_precomp, scales, scale_modifier, rotations, cov3D_precomp,
 	                          viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, radii, geom_buffer, binning_buffer, image_buffer, dL_dpix, dL_dmean2D,
 	                          dL_dconic, dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, v, stream);

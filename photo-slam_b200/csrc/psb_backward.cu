@@ -12,11 +12,15 @@ namespace psb {
 // z = V[2] x + V[6] y + V[10] z + V[14] (column-major), as in gaussian_backward_kernel<MODE_DEPTH>.
 // AA: the forward blended o' = o h (preprocess_fwd_kernel<false, true>, o' in the record). dL_dopacity [P] holds dL/do' from the tile
 // backward (atomic or gathered); the h-term joins the covariance gradient and dL_dopacity[g] is rescaled in place to dL/do = h dL/do'.
-template <bool DEPTH, bool AA = false>
+// NORMAL (scales + rotations): dL_dn [P,3] holds dL/dn of the operator's n_i (op_normals_kernel: activated scales, the rotation as given);
+// its rotation gradient, through column k of R(q), the sign and V (normal_axis_backward), joins dL/drot. The arg-min k and the sign are
+// piecewise constant, so nothing reaches the scales or the mean.
+template <bool DEPTH, bool AA = false, bool NORMAL = false>
 __device__ __forceinline__ void preprocess_bwd_body(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
                                                     int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
                                                     const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out,
-                                                    const float* __restrict__ dL_dz, float* __restrict__ dL_dopacity = nullptr)
+                                                    const float* __restrict__ dL_dz, float* __restrict__ dL_dopacity = nullptr,
+                                                    const float* __restrict__ dL_dn = nullptr)
 {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	if (idx >= in.P || geom.tile_info[idx].z == 0) return;
@@ -54,6 +58,12 @@ __device__ __forceinline__ void preprocess_bwd_body(GaussIn in, Camera cam, Geom
 		const float dz = dL_dz[idx];
 		dL_dmean.x += dz * cam.view[2]; dL_dmean.y += dz * cam.view[6]; dL_dmean.z += dz * cam.view[10];
 	}
+	if constexpr (NORMAL) {
+		const NormalAxis a = normal_axis(rot, scale, xform4x3(mean, cam.view), cam.view);
+		const float3 gn = make_float3(dL_dn[3 * idx], dL_dn[3 * idx + 1], dL_dn[3 * idx + 2]);
+		const float4 gq = normal_axis_backward(rot, a, gn, cam.view);
+		dL_drot.x += gq.x; dL_drot.y += gq.y; dL_drot.z += gq.z; dL_drot.w += gq.w;
+	}
 
 	if (out.dL_dmeans3D) { out.dL_dmeans3D[3 * idx] = dL_dmean.x; out.dL_dmeans3D[3 * idx + 1] = dL_dmean.y; out.dL_dmeans3D[3 * idx + 2] = dL_dmean.z; }
 	if (out.dL_dcov3D) {
@@ -77,11 +87,33 @@ __global__ void __launch_bounds__(128) preprocess_bwd_kernel(GaussIn in, Camera 
 	                               dL_dopacity);
 }
 
+// The operator's normal variants (psb_rasterize_backward_planes with a normal gradient): the four (DEPTH, AA) variants plus dL/dn. An
+// entry of its own, so the preprocess_bwd_kernel variants keep their names, parameters and code.
+template <bool DEPTH, bool AA>
+__global__ void __launch_bounds__(128) preprocess_bwd_normal_kernel(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
+                                                                    int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
+                                                                    const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out,
+                                                                    const float* __restrict__ dL_dz, float* __restrict__ dL_dopacity,
+                                                                    const float* __restrict__ dL_dn)
+{
+	preprocess_bwd_body<DEPTH, AA, true>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out, dL_dz,
+	                                     dL_dopacity, dL_dn);
+}
+
 int launch_preprocess_backward(const GaussIn& in, const Camera& cam, const GeomState& geom, const float* dL_dmean2D, int mean2D_stride,
                                const float* dL_dconic, int conic_stride, const float* dL_dcolor, int color_stride,
-                               const GaussGradOut& out, cudaStream_t stream, const float* dL_dz, float* aa_dL_dopacity)
+                               const GaussGradOut& out, cudaStream_t stream, const float* dL_dz, float* aa_dL_dopacity, const float* dL_dn)
 {
 	if (in.P == 0) return 0;
+	if (dL_dn) {
+		if (!in.scales || !in.rotations) { set_error_msg("launch_preprocess_backward: the normal gradient needs scales and rotations"); return -1; }
+		auto kernel = aa_dL_dopacity ? (dL_dz ? preprocess_bwd_normal_kernel<true, true> : preprocess_bwd_normal_kernel<false, true>)
+		                             : (dL_dz ? preprocess_bwd_normal_kernel<true, false> : preprocess_bwd_normal_kernel<false, false>);
+		kernel<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out,
+		                                            dL_dz, aa_dL_dopacity, dL_dn);
+		PSB_LAUNCH_OK();
+		return 0;
+	}
 	auto kernel = aa_dL_dopacity ? (dL_dz ? preprocess_bwd_kernel<true, true> : preprocess_bwd_kernel<false, true>)
 	                             : (dL_dz ? preprocess_bwd_kernel<true, false> : preprocess_bwd_kernel<false, false>);
 	kernel<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out,

@@ -494,21 +494,41 @@ __global__ void __launch_bounds__(256) tile_ranges_kernel(const uint32_t* __rest
 	}
 }
 
-// The normal pass's n_i (normal_axis) of every visible row, from the raw trainer parameters, behind the preprocess: a kernel of its own,
-// so the preprocess variants keep their code. The quaternion is normalised and the view-space mean formed exactly as the preprocess does.
-__global__ void __launch_bounds__(256) normals_kernel(int P, const float* __restrict__ xyz, const float* __restrict__ scaling,
-                                                      const float4* __restrict__ rotation, const float* __restrict__ view,
-                                                      const uint4* __restrict__ tile_info, float4* __restrict__ normals)
+// n_i (normal_axis) of every visible row behind the preprocess. RAW: the trainer's raw parameters (log-scales; the quaternion normalised
+// as the preprocess does); otherwise the operator's inputs (activated scales, whose arg-min is that of the log-scales and of the
+// modified scales; the rotation as given). The view-space mean is formed exactly as the preprocess does.
+template <bool RAW>
+__device__ __forceinline__ void normals_body(int P, const float* __restrict__ xyz, const float* __restrict__ scaling,
+                                             const float4* __restrict__ rotation, const float* __restrict__ view,
+                                             const uint4* __restrict__ tile_info, float4* __restrict__ normals)
 {
 	const int idx = blockIdx.x * 256 + threadIdx.x;
 	if (idx >= P || tile_info[idx].z == 0) return;
 	const float3 p = make_float3(xyz[3 * idx], xyz[3 * idx + 1], xyz[3 * idx + 2]);
 	const float3 sraw = make_float3(scaling[3 * idx], scaling[3 * idx + 1], scaling[3 * idx + 2]);
 	float4 q = rotation[idx];
-	const float n = fmaxf(sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w), 1e-12f);
-	q = make_float4(q.x / n, q.y / n, q.z / n, q.w / n);
+	if (RAW) {
+		const float n = fmaxf(sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w), 1e-12f);
+		q = make_float4(q.x / n, q.y / n, q.z / n, q.w / n);
+	}
 	const NormalAxis a = normal_axis(q, sraw, xform4x3(p, view), view);
 	normals[idx] = make_float4(a.n.x, a.n.y, a.n.z, 0.f);
+}
+
+// The normal pass's n_i from the raw trainer parameters: a kernel of its own, so the preprocess variants keep their code.
+__global__ void __launch_bounds__(256) normals_kernel(int P, const float* __restrict__ xyz, const float* __restrict__ scaling,
+                                                      const float4* __restrict__ rotation, const float* __restrict__ view,
+                                                      const uint4* __restrict__ tile_info, float4* __restrict__ normals)
+{
+	normals_body<true>(P, xyz, scaling, rotation, view, tile_info, normals);
+}
+
+// The operator's n_i (psb_rasterize_forward_planes / psb_rasterize_backward_planes) from its activated scales and rotations.
+__global__ void __launch_bounds__(256) op_normals_kernel(int P, const float* __restrict__ means3D, const float* __restrict__ scales,
+                                                         const float4* __restrict__ rotations, const float* __restrict__ view,
+                                                         const uint4* __restrict__ tile_info, float4* __restrict__ normals)
+{
+	normals_body<false>(P, means3D, scales, rotations, view, tile_info, normals);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -536,6 +556,15 @@ int launch_normals(int P, const float* xyz, const float* scaling, const float* r
 {
 	if (P == 0) return 0;
 	normals_kernel<<<cdiv(P, 256), 256, 0, stream>>>(P, xyz, scaling, reinterpret_cast<const float4*>(rotation), cam.view, tile_info, normals);
+	PSB_LAUNCH_OK();
+	return 0;
+}
+
+int launch_op_normals(const GaussIn& in, const Camera& cam, const uint4* tile_info, float4* normals, cudaStream_t stream)
+{
+	if (in.P == 0) return 0;
+	op_normals_kernel<<<cdiv(in.P, 256), 256, 0, stream>>>(in.P, in.means3D, in.scales, reinterpret_cast<const float4*>(in.rotations), cam.view,
+	                                                      tile_info, normals);
 	PSB_LAUNCH_OK();
 	return 0;
 }

@@ -33,6 +33,12 @@ struct GradSink {
 	float* z = nullptr; int z_stride = 0;  // unpacked sink with a depth gradient: the tenth sum, dL/dz (the packed row keeps it in slot 11)
 };
 
+// The operator's unpacked sink with a normal gradient: GradSink plus the dL/dn destination (three sums at +0..2). A type of its own
+// rather than two more GradSink fields, so that the kernels taking a GradSink keep their parameter layout and code.
+struct GradSinkN : GradSink {
+	float* n = nullptr; int n_stride = 0;
+};
+
 // Deterministic mode of the tile backward (the trainer's packed sink, or the operator's unpacked one). Float atomics from tiles that finish in any order would
 // sum a Gaussian's (Gaussian, tile) flushes in a different order every run; instead each flush is STORED in the slot of its
 // instance's emission index, base[g] + (rank of the tile among g's instances, InstRect), and gather_slots_kernel then sums every
@@ -117,6 +123,9 @@ int launch_render_forward(const Camera& cam, const uint2* ranges, const uint32_t
 // parameters (xyz, scaling, rotation), after launch_preprocess (tile_info says which rows are visible)
 int launch_normals(int P, const float* xyz, const float* scaling, const float* rotation, const Camera& cam, const uint4* tile_info, float4* normals,
                    cudaStream_t stream);
+// The same n_i from the operator's inputs: activated scales (the arg-min ignores the scale modifier) and the rotation as given, not
+// normalised (the operator's covariance does not normalise it either)
+int launch_op_normals(const GaussIn& in, const Camera& cam, const uint4* tile_info, float4* normals, cudaStream_t stream);
 // dL_ddepth [H,W]: depth variant, dL/dz of every Gaussian lands in slot 11 of its packed sink row, or at sink.z (unpacked sink;
 // refused without either destination). det != null: the deterministic variant — slot stores, then the ordered gather, which WRITES the
 // sink rows (packed: gather_slots_kernel; unpacked: gather_slots_unpacked_kernel, dL/dz at sink.z with dL_ddepth). dL_dalpha [H,W]: opacity variant, the gradient of the accumulated opacity 1 - final_T joins dL/dalpha of every splat
@@ -125,12 +134,17 @@ int launch_render_backward(const Camera& cam, const uint2* ranges, const uint32_
                            cudaStream_t stream, const float* dL_ddepth = nullptr, const DetSlots* det = nullptr, const float* dL_dalpha = nullptr,
                            const float4* normals = nullptr /* [P] n_i of the forward pass; with dL_dnormal only */,
                            const float* dL_dnormal = nullptr /* [3,H,W]: normal variant, packed 16-float sink rows, 64-byte deterministic slots */,
-                           const float* dL_ddepth2 = nullptr /* [H,W]: moment variant (a depth variant; dL_ddepth may be null), packed sink
-                                                                only; its dL/dz (slot 11) includes 2 z dL/dM */);
+                           const float* dL_ddepth2 = nullptr /* [H,W]: moment variant (a depth variant; dL_ddepth may be null); its dL/dz
+                                                                (slot 11 of a packed sink, sink.z of an unpacked one) includes 2 z dL/dM */,
+                           float* dL_dn = nullptr /* [P,3] (unpacked sink with dL_dnormal, operator path): receives dL/dn; the
+                                                     operator's normal variant (render_bwd_op_normal_kernel; deterministic: 64-byte
+                                                     slots and gather_slots_unpacked_normal_kernel) */);
 // dL_dz [P] (non-null: depth variant): dL/dmean3D += dL/dz (V[2], V[6], V[10]) for every visible Gaussian
 // aa_dL_dopacity [P] (non-null: AA variant, after an anti-aliased forward): holds dL/do' on entry, dL/do on return
+// dL_dn [P,3] (non-null: normal variant, scales + rotations only): dL/drot += the rotation gradient of n_i (launch_op_normals' n_i)
 int launch_preprocess_backward(const GaussIn& in, const Camera& cam, const GeomState& geom, const float* dL_dmean2D, int mean2D_stride,
                                const float* dL_dconic, int conic_stride, const float* dL_dcolor, int color_stride,
-                               const GaussGradOut& out, cudaStream_t stream, const float* dL_dz = nullptr, float* aa_dL_dopacity = nullptr);
+                               const GaussGradOut& out, cudaStream_t stream, const float* dL_dz = nullptr, float* aa_dL_dopacity = nullptr,
+                               const float* dL_dn = nullptr);
 
 }  // namespace psb

@@ -114,6 +114,29 @@ struct OpDetState {
 	}
 };
 
+// Scratch of the operator's normal plane (psb_rasterize_planes_bytes): n_i of every Gaussian, which the forward renders and the backward
+// recomputes, the unpacked sink's dL/dn and, for the deterministic backward only (R > 0), the 64-byte slots of its normal variant.
+struct OpPlaneState {
+	float4* normals;  // [P]
+	float* dn;        // [P][3]
+	float4* slots;    // [R][4]: one 16-float sink row per instance (DetSlots::slots of a normal pass)
+
+	static OpPlaneState from_chunk(char*& chunk, size_t P, size_t R)
+	{
+		OpPlaneState s;
+		s.normals = carve<float4>(chunk, P);
+		s.dn = carve<float>(chunk, 3 * P);
+		s.slots = carve<float4>(chunk, 4 * R);
+		return s;
+	}
+	static size_t required_bytes(size_t P, size_t R)
+	{
+		char* p = nullptr;
+		from_chunk(p, P, R);
+		return reinterpret_cast<size_t>(p) + 128;
+	}
+};
+
 template <typename S>
 static inline size_t required_bytes(size_t n)
 {

@@ -9,7 +9,8 @@
 // libgaussian_mapper.so links against exactly these symbols (SURVEY.md §8b); building this file into
 // libcuda_rasterizer.so (+ libpsb200.so) swaps the rasterizer without touching any caller. Pure C++/LibTorch host
 // code: no kernels here. Every RasterizeGaussians*CUDA forward is forward_impl and every backward is backward_impl (below), which
-// differ per export only in the C entry point they call. The TORCH_LIBRARY block at the end only exists so the Python test-suite can call the
+// differ per export only in the C entry point they call; the planes pair (RasterizeGaussians[Backward]PlanesCUDA) calls the one C entry
+// point that takes every plane in a record. The TORCH_LIBRARY block at the end only exists so the Python test-suite can call the
 // C++ entry points (torch.ops.psb200.*).
 #include <functional>
 #include <optional>
@@ -262,6 +263,119 @@ RasterizeGaussiansBackwardAntialiasedCUDA(const torch::Tensor& background, const
 	                     dL_dout_color, dL_dout_depth, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer, Bwd::Antialiased, deterministic);
 }
 
+// ---- opacity, normals and the second depth moment (include/psb200.h psb_rasterize_forward_planes): A = 1 - T_final, N = sum n alpha T,
+// M = sum z^2 alpha T beside colour and depth, for a GaussianRasterizerFunction that returns and back-propagates them (INTEGRATION.md §1).
+// -> (rendered, out_color, out_depth, out_alpha, out_normal, out_depth2, radii, geomBuffer, binningBuffer, imgBuffer); a plane that is not
+// requested comes back undefined. Colour, depth, radii and the buffers are bit-identical to RasterizeGaussiansAntialiasedCUDA's (with the
+// same antialiasing flag). The normal plane needs scales and rotations.
+std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
+RasterizeGaussiansPlanesCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors, const torch::Tensor& opacity,
+                             const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier, const torch::Tensor& cov3D_precomp,
+                             const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx, const float tan_fovy,
+                             const int image_height, const int image_width, const torch::Tensor& sh, const int degree, const torch::Tensor& campos,
+                             const bool prefiltered, const bool depth, const bool alpha, const bool normal, const bool depth2, const bool antialiasing)
+{
+	if (means3D.ndimension() != 2 || means3D.size(1) != 3) { AT_ERROR("means3D must have dimensions (num_points, 3)"); }
+	if (normal && cov3D_precomp.defined() && cov3D_precomp.numel() != 0) { AT_ERROR("the normal plane needs scales and rotations, not cov3D_precomp"); }
+	const int P = means3D.size(0);
+	const int H = image_height, W = image_width;
+	auto float_opts = means3D.options().dtype(torch::kFloat32);
+	torch::Tensor out_color = torch::full({3, H, W}, 0.0, float_opts);
+	torch::Tensor out_depth, out_alpha, out_normal, out_depth2;
+	if (depth) out_depth = torch::full({H, W}, 0.0, float_opts);
+	if (alpha) out_alpha = torch::full({H, W}, 0.0, float_opts);
+	if (normal) out_normal = torch::full({3, H, W}, 0.0, float_opts);
+	if (depth2) out_depth2 = torch::full({H, W}, 0.0, float_opts);
+	torch::Tensor radii = torch::full({P}, 0, means3D.options().dtype(torch::kInt32));
+	torch::TensorOptions options(torch::kByte);
+	torch::Tensor geomBuffer = torch::empty({0}, options.device(means3D.device()));
+	torch::Tensor binningBuffer = torch::empty({0}, options.device(means3D.device()));
+	torch::Tensor imgBuffer = torch::empty({0}, options.device(means3D.device()));
+	int rendered = 0;
+	if (P != 0) {
+		int M = 0;
+		if (sh.size(0) != 0) M = sh.size(1);
+		const auto bg = background.contiguous(), m3 = means3D.contiguous(), shc = sh.contiguous(), col = colors.contiguous(), op = opacity.contiguous(),
+		           sc = scales.contiguous(), rot = rotations.contiguous(), cov = cov3D_precomp.contiguous(), vm = viewmatrix.contiguous(),
+		           pm = projmatrix.contiguous(), cp = campos.contiguous();
+		psb_raster_planes planes{depth ? out_depth.data_ptr<float>() : nullptr, alpha ? out_alpha.data_ptr<float>() : nullptr,
+		                         normal ? out_normal.data_ptr<float>() : nullptr, depth2 ? out_depth2.data_ptr<float>() : nullptr};
+		const size_t plane_bytes = normal ? psb_rasterize_planes_bytes(P, 0) : 0;
+		torch::Tensor plane_t;
+		if (normal) plane_t = torch::empty({(long long)plane_bytes}, means3D.options().dtype(torch::kByte));
+		rendered = psb_rasterize_forward_planes(resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer, P, degree, M, fptr(bg), W, H,
+		                                        fptr(m3), fptr(shc), fptr(col), fptr(op), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm),
+		                                        fptr(cp), tan_fovx, tan_fovy, prefiltered ? 1 : 0, out_color.data_ptr<float>(), radii.data_ptr<int>(),
+		                                        &planes, normal ? plane_t.data_ptr() : nullptr, plane_bytes, antialiasing ? 1 : 0, current_stream());
+		if (rendered < 0) { AT_ERROR("psb_rasterize_forward_planes: ", psb_last_error()); }
+	}
+	return std::make_tuple(rendered, out_color, out_depth, out_alpha, out_normal, out_depth2, radii, geomBuffer, binningBuffer, imgBuffer);
+}
+
+// The backward of RasterizeGaussiansPlanesCUDA: the signature of RasterizeGaussiansBackwardAntialiasedCUDA plus the gradients of the
+// opacity, normal and second-moment planes after dL_dout_depth, and `antialiasing` (the forward's flag) before `deterministic`. An
+// undefined or empty gradient is none; without any it is RasterizeGaussiansBackwardAntialiasedCUDA's backward. Returns the same 8-tuple;
+// dL/dz (depth and second moment) is folded into dL_dmeans3D and dL/dn into dL_drotations.
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
+RasterizeGaussiansBackwardPlanesCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& radii, const torch::Tensor& colors,
+                                     const torch::Tensor& scales, const torch::Tensor& rotations, const float scale_modifier,
+                                     const torch::Tensor& cov3D_precomp, const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix,
+                                     const float tan_fovx, const float tan_fovy, const torch::Tensor& dL_dout_color, const torch::Tensor& dL_dout_depth,
+                                     const torch::Tensor& dL_dout_alpha, const torch::Tensor& dL_dout_normal, const torch::Tensor& dL_dout_depth2,
+                                     const torch::Tensor& sh, const int degree, const torch::Tensor& campos, const torch::Tensor& geomBuffer, const int R,
+                                     const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const bool antialiasing,
+                                     const bool deterministic)
+{
+	const int P = means3D.size(0);
+	const int H = dL_dout_color.size(1), W = dL_dout_color.size(2);
+	auto given = [&](const torch::Tensor& t, int C, const char* name) {
+		if (!t.defined() || t.numel() == 0) return false;
+		const bool ok = C == 1 ? (t.ndimension() == 2 && t.size(0) == H && t.size(1) == W)
+		                       : (t.ndimension() == 3 && t.size(0) == C && t.size(1) == H && t.size(2) == W);
+		if (!ok) { AT_ERROR(name, " must have dimensions (", C == 1 ? "" : "3, ", H, ", ", W, ")"); }
+		return true;
+	};
+	const bool depth = given(dL_dout_depth, 1, "dL_dout_depth"), alpha = given(dL_dout_alpha, 1, "dL_dout_alpha");
+	const bool normal = given(dL_dout_normal, 3, "dL_dout_normal"), depth2 = given(dL_dout_depth2, 1, "dL_dout_depth2");
+	if (normal && cov3D_precomp.defined() && cov3D_precomp.numel() != 0) { AT_ERROR("dL_dout_normal needs scales and rotations, not cov3D_precomp"); }
+	int M = 0;
+	if (sh.size(0) != 0) M = sh.size(1);
+	torch::Tensor dL_dmeans3D = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_dmeans2D = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_dcolors = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_dconic = torch::zeros({P, 2, 2}, means3D.options());
+	torch::Tensor dL_dopacity = torch::zeros({P, 1}, means3D.options());
+	torch::Tensor dL_dcov3D = torch::zeros({P, 6}, means3D.options());
+	torch::Tensor dL_dsh = torch::zeros({P, M, 3}, means3D.options());
+	torch::Tensor dL_dscales = torch::zeros({P, 3}, means3D.options());
+	torch::Tensor dL_drotations = torch::zeros({P, 4}, means3D.options());
+	if (P != 0) {
+		const auto bg = background.contiguous(), m3 = means3D.contiguous(), shc = sh.contiguous(), col = colors.contiguous(), sc = scales.contiguous(),
+		           rot = rotations.contiguous(), cov = cov3D_precomp.contiguous(), vm = viewmatrix.contiguous(), pm = projmatrix.contiguous(),
+		           cp = campos.contiguous(), dpix = dL_dout_color.contiguous(), rad = radii.contiguous();
+		const torch::Tensor gd = depth ? dL_dout_depth.contiguous() : torch::Tensor(), ga = alpha ? dL_dout_alpha.contiguous() : torch::Tensor(),
+		                    gn = normal ? dL_dout_normal.contiguous() : torch::Tensor(), gm = depth2 ? dL_dout_depth2.contiguous() : torch::Tensor();
+		const psb_raster_plane_grads grads{depth ? gd.data_ptr<float>() : nullptr, alpha ? ga.data_ptr<float>() : nullptr,
+		                                   normal ? gn.data_ptr<float>() : nullptr, depth2 ? gm.data_ptr<float>() : nullptr};
+		torch::Tensor dL_dz, det_t, plane_t;
+		if (depth || depth2) dL_dz = torch::zeros({P}, means3D.options());
+		const size_t det_bytes = deterministic ? psb_rasterize_backward_det_bytes(P, R) : 0;
+		if (deterministic) det_t = torch::empty({(long long)det_bytes}, means3D.options().dtype(torch::kByte));
+		const size_t plane_bytes = normal ? psb_rasterize_planes_bytes(P, deterministic ? R : 0) : 0;
+		if (normal) plane_t = torch::empty({(long long)plane_bytes}, means3D.options().dtype(torch::kByte));
+		const int rc = psb_rasterize_backward_planes(
+			P, degree, M, R, fptr(bg), W, H, fptr(m3), fptr(shc), fptr(col), fptr(sc), scale_modifier, fptr(rot), fptr(cov), fptr(vm), fptr(pm), fptr(cp),
+			tan_fovx, tan_fovy, rad.data_ptr<int>(), reinterpret_cast<char*>(geomBuffer.contiguous().data_ptr()),
+			reinterpret_cast<char*>(binningBuffer.contiguous().data_ptr()), reinterpret_cast<char*>(imageBuffer.contiguous().data_ptr()), fptr(dpix),
+			dL_dmeans2D.data_ptr<float>(), dL_dconic.data_ptr<float>(), dL_dopacity.data_ptr<float>(), dL_dcolors.data_ptr<float>(),
+			dL_dmeans3D.data_ptr<float>(), dL_dcov3D.data_ptr<float>(), M ? dL_dsh.data_ptr<float>() : nullptr, dL_dscales.data_ptr<float>(),
+			dL_drotations.data_ptr<float>(), &grads, (depth || depth2) ? dL_dz.data_ptr<float>() : nullptr, deterministic ? det_t.data_ptr() : nullptr,
+			det_bytes, normal ? plane_t.data_ptr() : nullptr, plane_bytes, antialiasing ? 1 : 0, deterministic ? 1 : 0, current_stream());
+		if (rc < 0) { AT_ERROR("psb_rasterize_backward_planes: ", psb_last_error()); }
+	}
+	return std::make_tuple(dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations);
+}
+
 torch::Tensor markVisible(torch::Tensor& means3D, torch::Tensor& viewmatrix, torch::Tensor& projmatrix)
 {
 	const int P = means3D.size(0);
@@ -473,6 +587,26 @@ std::tuple<T, T, T, T, T, T, T, T> op_bwd_aa(const T& bg, const T& m3, const T& 
 	return RasterizeGaussiansBackwardAntialiasedCUDA(bg, m3, radii, col, sc, rot, (float)smod, cov, vm, pm, (float)tfx, (float)tfy, dpix, ddep.value_or(T()),
 	                                                 sh, (int)deg, cp, gb, (int)R, bb, ib, deterministic);
 }
+std::tuple<int64_t, T, T, T, T, T, T, T, T, T> op_fwd_planes(const T& bg, const T& m3, const T& col, const T& op, const T& sc, const T& rot, double smod,
+                                                            const T& cov, const T& vm, const T& pm, double tfx, double tfy, int64_t H, int64_t W,
+                                                            const T& sh, int64_t deg, const T& cp, bool pre, bool depth, bool alpha, bool normal,
+                                                            bool depth2, bool aa)
+{
+	auto r = RasterizeGaussiansPlanesCUDA(bg, m3, col, op, sc, rot, (float)smod, cov, vm, pm, (float)tfx, (float)tfy, (int)H, (int)W, sh, (int)deg, cp, pre,
+	                                      depth, alpha, normal, depth2, aa);
+	return std::make_tuple((int64_t)std::get<0>(r), std::get<1>(r), std::get<2>(r), std::get<3>(r), std::get<4>(r), std::get<5>(r), std::get<6>(r),
+	                       std::get<7>(r), std::get<8>(r), std::get<9>(r));
+}
+std::tuple<T, T, T, T, T, T, T, T> op_bwd_planes(const T& bg, const T& m3, const T& radii, const T& col, const T& sc, const T& rot, double smod,
+                                                 const T& cov, const T& vm, const T& pm, double tfx, double tfy, const T& dpix,
+                                                 const std::optional<T>& ddep, const std::optional<T>& dalpha, const std::optional<T>& dnormal,
+                                                 const std::optional<T>& ddep2, const T& sh, int64_t deg, const T& cp, const T& gb, int64_t R,
+                                                 const T& bb, const T& ib, bool aa, bool deterministic)
+{
+	return RasterizeGaussiansBackwardPlanesCUDA(bg, m3, radii, col, sc, rot, (float)smod, cov, vm, pm, (float)tfx, (float)tfy, dpix, ddep.value_or(T()),
+	                                            dalpha.value_or(T()), dnormal.value_or(T()), ddep2.value_or(T()), sh, (int)deg, cp, gb, (int)R, bb, ib, aa,
+	                                            deterministic);
+}
 T op_vis(T m3, T vm, T pm) { return markVisible(m3, vm, pm); }
 T op_dist(const T& p) { return distCUDA2(p); }
 T op_xform(T p, T m) { transformPoints(p, m); return p; }
@@ -511,6 +645,8 @@ TORCH_LIBRARY(psb200, m)
 	m.def("rasterize_gaussians_backward_deterministic", &op_bwd_det);
 	m.def("rasterize_gaussians_antialiased", &op_fwd_aa);
 	m.def("rasterize_gaussians_backward_antialiased", &op_bwd_aa);
+	m.def("rasterize_gaussians_planes", &op_fwd_planes);
+	m.def("rasterize_gaussians_backward_planes", &op_bwd_planes);
 	m.def("mark_visible", &op_vis);
 	m.def("b2_forward", &op_b2_fwd);
 	m.def("dist_cuda2", &op_dist);

@@ -7,7 +7,8 @@ EVERY pipeline branch, on top of the psb200 rasterizer operator (rasterizer.Gaus
   default              raw SH rows to the rasterizer                                               (:114-117)
 
 and any SH storage size M = (max_sh_degree + 1)^2 (the operator-level path takes M from the tensor). The result tuple is the
-reference's: (rendered_image, viewspace_points, visibility_filter, radii), plus the depth image with return_depth=True; gradients
+reference's: (rendered_image, viewspace_points, visibility_filter, radii), plus the depth image with return_depth=True and the opacity,
+normal and second-moment planes with return_alpha / return_normal / return_depth2; gradients
 flow through torch autograd into the model tensors, and viewspace_points.grad[:, :2] feeds addDensificationStats like in the reference.
 
 This is the general, differentiable path. The trainer's hot loop does not come through here: psb_trainer_step / psb_trainer_render fuse
@@ -60,13 +61,17 @@ def get_covariance_activation(model, scaling_modifier=1.0, scales=None):
 
 
 def render(viewpoint_camera, image_height, image_width, pc, pipe=None, bg_color=None, override_color=None, scaling_modifier=1.0,
-           use_override_color=False, return_depth=False, deterministic=False):
+           use_override_color=False, return_depth=False, deterministic=False, return_alpha=False, return_normal=False, return_depth2=False):
     """viewpoint_camera: dict(viewmatrix, projmatrix, campos: device tensors; tanfovx, tanfovy) — the fields of GaussianKeyframe the
     reference reads (world_view_transform_, full_proj_transform_, camera_center_, FoVx_/FoVy_ as tangents). pc: trainer.GaussianModel.
     return_depth=True appends the rendered depth [H,W] (include/psb200.h: sum z alpha T, no background term) to the tuple, in every
-    branch; gradients flow through it like through the image. deterministic=True: the rasterizer's backward is bit-identical from run to
+    branch; gradients flow through it like through the image. return_alpha / return_normal / return_depth2 append, in that order after
+    depth, the accumulated opacity A [H,W], the normal plane N [3,H,W] and the second depth moment M [H,W] (include/psb200.h), in every
+    branch except N with pipe.compute_cov3D, which is refused (N needs the scales and rotations). deterministic=True: the rasterizer's backward is bit-identical from run to
     run (GaussianRasterizer.forward), so are the gradients it sends into the model tensors and viewspace_points."""
     pipe = pipe or GaussianPipelineParams()
+    if return_normal and pipe.compute_cov3D:
+        raise RuntimeError("render: return_normal needs scales and rotations; pipe.compute_cov3D passes a covariance instead")
     dev = pc.xyz_.device
     bg_color = bg_color if bg_color is not None else torch.zeros(3, device=dev)
     screenspace_points = torch.zeros_like(pc.xyz_, requires_grad=True)
@@ -94,6 +99,12 @@ def render(viewpoint_camera, image_height, image_width, pc, pipe=None, bg_color=
         colors_precomp = torch.clamp_min(sh_utils.eval_sh(pc.active_sh_degree_, shs_view, dir_pp) + 0.5, 0.0)
     else:
         shs = get_features(pc)
+    if return_alpha or return_normal or return_depth2:
+        rendered_image, radii, *planes = rasterizer(means3D, means2D, opacity, shs=shs, colors_precomp=colors_precomp, scales=scales,
+                                                    rotations=rotations, cov3D_precomp=cov3D_precomp, return_depth=return_depth,
+                                                    deterministic=deterministic, return_alpha=return_alpha, return_normal=return_normal,
+                                                    return_depth2=return_depth2)
+        return (rendered_image, screenspace_points, radii > 0, radii, *planes)
     if return_depth:
         rendered_image, radii, depth = rasterizer(means3D, means2D, opacity, shs=shs, colors_precomp=colors_precomp, scales=scales,
                                                   rotations=rotations, cov3D_precomp=cov3D_precomp, return_depth=True,
