@@ -475,7 +475,8 @@ int psb_trainer_result_depth(psb_trainer* t, float* out4, int* num_rendered, voi
  *   max(N_valid, 1) on valid pixels (sign(0) = 0). N_valid is counted on the device (no host synchronisation); in deterministic mode the
  *   sums are reduced in a fixed order. Comparing the un-normalised N with a unit G also pushes A towards 1 where normals are measured:
  *   deliberate, as the depth term does with D. Exposure compensation acts on colour only and does not touch this term.
- * The data-parallel calls, the _begin / _slab halves and the rasterizer operator take no normal term.
+ * The data-parallel calls take it through psb_dp_step_dist, psb_trainer_backward_begin_dist (+ _slab) and psb_trainer_backward_dist;
+ * the rasterizer operator takes no normal term.
  * ------------------------------------------------------------------------------------------------ */
 typedef struct psb_normal {
 	const float* gt_normal;  /* [3,H,W] device, view-space unit normals, (0,0,0) = no measurement (psb_depth_normals); NULL = no normal term */
@@ -525,7 +526,8 @@ int psb_depth_normals(const psb_camera* camera, const float* depth, float max_re
  * N_valid is counted on the device and the scale lambda_dn / max(N_valid, 1) read there; no float atomics on the planes, and in
  * deterministic mode the loss sums are reduced in a fixed order. With a depth and/or normal term in the same step, their gradients are
  * written first and this term adds into the same planes. Anti-aliasing, the 3D filter and exposure compose unchanged (exposure acts on
- * colour only). The data-parallel calls, the _begin / _slab halves and the rasterizer operator take no consistency term.
+ * colour only). The data-parallel calls take it through psb_dp_step_dist, psb_trainer_backward_begin_dist (+ _slab) and
+ * psb_trainer_backward_dist; the rasterizer operator takes no consistency term.
  * ------------------------------------------------------------------------------------------------ */
 typedef struct psb_dn {
 	float lambda_dn;          /* finite, > 0 */
@@ -569,8 +571,8 @@ int psb_dn_loss(const psb_camera* camera, const float* depth, const float* alpha
  *   more channel with per-Gaussian value z_i^2: z_i^2 dL/dM joins dL/dalpha_i, and dL/dz_i gains sum_p alpha_i T_i 2 z_i dL/dM, so per
  *   Gaussian dL/dz_i = 2k sum_p w_i (A z_i - D) (2DGS's gradient). The term reaches positions, opacity and shape, and the densification
  *   statistics. No float atomics on the planes; in deterministic mode the loss sums are reduced in a fixed order. Anti-aliasing, the 3D
- *   filter and exposure compose unchanged (exposure acts on colour only). The data-parallel calls, the _begin / _slab halves and the
- *   rasterizer operator take no distortion term.
+ *   filter and exposure compose unchanged (exposure acts on colour only). The data-parallel calls take it through psb_dp_step_dist,
+ *   psb_trainer_backward_begin_dist (+ _slab) and psb_trainer_backward_dist; the rasterizer operator takes no distortion term.
  * ------------------------------------------------------------------------------------------------ */
 typedef struct psb_dist {
 	float lambda_dist;   /* finite, >= 0; 0 with out_depth2: the plane alone */
@@ -597,8 +599,18 @@ int psb_trainer_step_dist(psb_trainer* t, int P, int M, const psb_model* model, 
                           const float* background, const float* gt_image, const float* mask, const psb_step* step,
                           float* out_color, int* radii, const psb_depth* depth, const psb_exposure* exposure, const psb_normal* normal,
                           const psb_dn* dn, const psb_dist* dist, void* stream);
-/* psb_trainer_result with out7 = {loss, l1, ssim, depth_l1, normal_l1, dn, dist} (0 for a term the last step did not have). */
+/* psb_trainer_result with out7 = {loss, l1, ssim, depth_l1, normal_l1, dn, dist} (0 for a term the last step did not have). After
+ * psb_dp_step_dist, psb_trainer_backward_begin_dist and psb_trainer_backward_dist it reports this context's (this rank's) terms. */
 int psb_trainer_result_dist(psb_trainer* t, float* out7, int* num_rendered, void* stream);
+/* psb_trainer_backward_exposure plus the normal, consistency and distortion terms (all three NULL: exactly psb_trainer_backward_exposure):
+ * the raw-parameter gradients of the loss psb_trainer_step_dist would train on, written to grads; the parameters do not move. The
+ * rotation gradient takes dL/dn, and the distortion's dL/dz joins the xyz gradient. PSB_ERR_ARG, before any CUDA call, for everything
+ * psb_trainer_backward_exposure rejects and the normal, dn and dist records psb_trainer_step_dist rejects. */
+int psb_trainer_backward_dist(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                              const float* background, const float* gt_image, const float* mask, const psb_step* step,
+                              float* out_color, int* radii, float* const* grads, const psb_depth* depth,
+                              const psb_exposure* exposure, float* exposure_grad, const psb_normal* normal, const psb_dn* dn,
+                              const psb_dist* dist, void* stream);
 
 /* model->adam_live[i] = 1 if any of the 118 moments of row i is non-zero, else 0: one pass over the moments. Restores the
  * psb_model.adam_live contract after moments were written by anything but psb_trainer_step. Asynchronous on `stream`. */
@@ -631,6 +643,16 @@ int psb_trainer_backward_slab(psb_trainer* t, int P, int M, const psb_model* mod
 int psb_trainer_backward_begin_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
                                      const float* background, const float* gt_image, const float* mask, const psb_step* step,
                                      float* out_color, int* radii, const psb_depth* depth, void* stream);
+/* psb_trainer_backward_begin_depth plus the normal, consistency and distortion terms (all three NULL: exactly
+ * psb_trainer_backward_begin_depth). The context records, before the pass and whether or not the call succeeds, which gradients the
+ * pass leaves in its rows (dL/dz with a depth, consistency or distortion term; dL/dn with a normal or consistency term), and every _slab
+ * that follows takes them into its gradients; a plain _begin or _begin_depth clears that again. A _slab after a _begin_dist that failed
+ * before its pass returns PSB_ERR_ARG. PSB_ERR_ARG, before any CUDA call, for everything _begin_depth rejects and the normal, dn and dist
+ * records psb_trainer_step_dist rejects. psb_trainer_result_dist reports this rank's terms. */
+int psb_trainer_backward_begin_dist(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                                    const float* background, const float* gt_image, const float* mask, const psb_step* step,
+                                    float* out_color, int* radii, const psb_depth* depth, const psb_normal* normal, const psb_dn* dn,
+                                    const psb_dist* dist, void* stream);
 /* Same update on one flat range of n floats (any slice of a parameter tensor and the matching slices of its moments and
  * gradient) with an explicit learning rate: lets the caller pipeline chunked all-reduces with the optimizer. */
 int psb_adam_flat(size_t n, float* param, float* exp_avg, float* exp_avg_sq, const float* grad, float lr,
@@ -671,6 +693,16 @@ int psb_dp_step(psb_trainer* t, psb_dp* dp, int P, int M, const psb_model* model
 int psb_dp_step_depth(psb_trainer* t, psb_dp* dp, int P, int M, const psb_model* model, const psb_camera* camera,
                       const float* background, const float* gt_image, const float* mask, const psb_step* step,
                       float* out_color, int* radii, const psb_depth* depth, void* stream);
+/* psb_dp_step_depth plus this rank's normal, consistency and distortion terms (all three NULL: exactly psb_dp_step_depth; the records as
+ * in psb_trainer_step_dist). dL/dn joins this rank's rotation gradient and the distortion's dL/dz its xyz gradient before the records
+ * are built, so the record format and the owner-side Adam are those of psb_dp_step: the ranks of one step may mix views with different
+ * terms. A row that only the terms reach sends a record. psb_trainer_result_dist reports this rank's terms; a view that overflows the
+ * binning arena contributes a zero gradient, as in psb_dp_step. PSB_ERR_ARG, before any CUDA call, for everything psb_dp_step_depth
+ * rejects and the normal, dn and dist records psb_trainer_step_dist rejects. */
+int psb_dp_step_dist(psb_trainer* t, psb_dp* dp, int P, int M, const psb_model* model, const psb_camera* camera,
+                     const float* background, const float* gt_image, const float* mask, const psb_step* step,
+                     float* out_color, int* radii, const psb_depth* depth, const psb_normal* normal, const psb_dn* dn,
+                     const psb_dist* dist, void* stream);
 /* Enqueues a device-side wait until every rank's rows of the last psb_dp_step have landed in this rank's tensors. */
 int psb_dp_sync(psb_dp* dp, void* stream);
 /* 0 = healthy, 1 = a cross-rank wait timed out (PSB_DP_TIMEOUT_MS, default 20 s). Synchronises the stream. */

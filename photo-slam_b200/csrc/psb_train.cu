@@ -54,9 +54,9 @@ constexpr int MODE_REG = 32;       // OR'd into MODE_GRADS / MODE_ADAM / MODE_AD
 constexpr int MODE_F3D = 64;       // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE (each optionally | MODE_DEPTH | MODE_AA | MODE_REG), not MODE_PUSH:
                                    // the forward applied the 3D smoothing filter f3d[idx] (preprocess_fwd_kernel<true, AA, true>): the covariance is
                                    // rebuilt from s' = sqrt(s^2 + f^2), and the filter's opacity factor c joins the scale and opacity gradients
-constexpr int MODE_NORMAL = 128;   // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE (each optionally | MODE_DEPTH | MODE_AA | MODE_REG | MODE_F3D),
-                                   // not MODE_PUSH: the sink rows are 16 floats (render_bwd_normal_kernel) and slots 12..14 hold dL/dn; the
-                                   // rotation gradient takes dL/dq of n = sign V r_k(q) (normal_axis_backward)
+constexpr int MODE_NORMAL = 128;   // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE (each optionally | MODE_DEPTH | MODE_AA | MODE_REG | MODE_F3D)
+                                   // and into MODE_PUSH (optionally | MODE_DEPTH | MODE_AA): the sink rows are 16 floats (render_bwd_normal_kernel) and
+                                   // slots 12..14 hold dL/dn; the rotation gradient takes dL/dq of n = sign V r_k(q) (normal_axis_backward)
 
 // torch::optim::Adam single-tensor update (LibTorch adam.cpp): exp_avg.mul_(b1).add_(g, 1-b1);
 // exp_avg_sq.mul_(b2).addcmul_(g, g, 1-b2); denom = exp_avg_sq.sqrt()/sqrt(bc2) + eps; p.addcdiv_(exp_avg, denom, -lr/bc1).
@@ -187,7 +187,8 @@ __device__ __forceinline__ void adam_small(SmallRow& p, SmallRow& m, SmallRow& v
 // MODE_DEPTH: dL/dxyz += dL/dz (V[2], V[6], V[10]). A row whose only non-zero sum is slot 11 has a gradient (its parameters are loaded and
 // updated, its live byte set) but no SH gradient: the view-direction term depends on dL/dRGB only, so its f_rest row is not staged.
 //
-// MODE_NORMAL: a row whose only non-zero sums are slots 12..14 has a gradient (the rotation's) but no SH gradient, as with MODE_DEPTH.
+// MODE_NORMAL: a row whose only non-zero sums are slots 12..14 has a gradient (the rotation's) but no SH gradient, as with MODE_DEPTH. Under
+// MODE_PUSH such a row sends a record: its g_rot is non-zero.
 //
 // MODE_REG: `reg` is read by these instantiations only. The regularisers touch exactly the rows that have a gradient anyway (`reached`), so
 // the dirty / live decisions and the memory traffic are those of the variant without it.
@@ -210,7 +211,6 @@ __global__ void __launch_bounds__(TB, A_MINBLOCKS) gaussian_backward_kernel(int 
 	constexpr int BASE = MODE & ~(MODE_DEPTH | MODE_AA | MODE_REG | MODE_F3D | MODE_NORMAL);
 	constexpr int SR = NORMAL ? 4 : 3;  // float4 lanes per sink row
 	static_assert(!F3D || BASE != MODE_PUSH, "no 3D filter on the NVLink step");
-	static_assert(!NORMAL || BASE != MODE_PUSH, "no normal term on the NVLink step");
 	constexpr bool LIVE = BASE == MODE_ADAM_LIVE;
 	constexpr bool ADAM = BASE == MODE_ADAM || LIVE;
 	__shared__ __align__(128) float s_p[TB * REST];  // f_rest parameter rows of this block (TMA destination; LIVE: compacted per warp)
@@ -817,8 +817,8 @@ void run_gaussian_backward(int first, int P, cudaStream_t stream, Args... args)
 	gaussian_backward_kernel<MODE><<<cdiv(P - first, TB), TB, 0, stream>>>(first, P, args...);
 }
 
-// Gaussians [first, P) in mode `mode` (MODE_GRADS, MODE_ADAM, MODE_ADAM_LIVE or MODE_PUSH, each optionally | MODE_DEPTH and | MODE_AA; all but
-// MODE_PUSH optionally | MODE_REG, | MODE_F3D and | MODE_NORMAL)
+// Gaussians [first, P) in mode `mode` (MODE_GRADS, MODE_ADAM, MODE_ADAM_LIVE or MODE_PUSH, each optionally | MODE_DEPTH, | MODE_AA and
+// | MODE_NORMAL; all but MODE_PUSH optionally | MODE_REG and | MODE_F3D)
 int launch_gaussian_backward(int mode, int first, int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink,
                              const StepHyper& h, const GradSegments& grads, const DensifyStats& st, const uint32_t* counters, uint32_t capacity,
                              float* seeds, const DpPush& dp, unsigned char* adam_live, cudaStream_t stream, const RegCoef& reg, const float* f3d,
@@ -853,6 +853,10 @@ int launch_gaussian_backward(int mode, int first, int P, const TrainTensors& t, 
 		PSB_BACKWARD_CASE_REG(MODE_ADAM | MODE_DEPTH | MODE_AA);
 		PSB_BACKWARD_CASE_REG(MODE_ADAM_LIVE | MODE_DEPTH | MODE_AA);
 		PSB_BACKWARD_CASE(MODE_PUSH | MODE_DEPTH | MODE_AA);
+		PSB_BACKWARD_CASE(MODE_PUSH | MODE_NORMAL);
+		PSB_BACKWARD_CASE(MODE_PUSH | MODE_NORMAL | MODE_DEPTH);
+		PSB_BACKWARD_CASE(MODE_PUSH | MODE_NORMAL | MODE_AA);
+		PSB_BACKWARD_CASE(MODE_PUSH | MODE_NORMAL | MODE_DEPTH | MODE_AA);
 		default: set_error_msg("launch_gaussian_backward: unknown mode"); return -1;
 	}
 #undef PSB_BACKWARD_CASE_NRM
@@ -930,8 +934,7 @@ int launch_push_backward(int P, const TrainTensors& t, const Camera& cam, const 
 	const GradSegments nog = {};
 	int rc;
 	if (mode.f3d) { set_error_msg("launch_push_backward: the 3D filter is not wired into the NVLink step"); return -1; }
-	if (mode.normal) { set_error_msg("launch_push_backward: the normal term is not wired into the NVLink step"); return -1; }
-	if ((rc = launch_gaussian_backward(MODE_PUSH | (mode.depth ? MODE_DEPTH : 0) | (mode.aa ? MODE_AA : 0), 0, P, t, cam, geom, sink, h, nog, st, counters, capacity, nullptr, dp,
+	if ((rc = launch_gaussian_backward(MODE_PUSH | (mode.depth ? MODE_DEPTH : 0) | (mode.aa ? MODE_AA : 0) | (mode.normal ? MODE_NORMAL : 0), 0, P, t, cam, geom, sink, h, nog, st, counters, capacity, nullptr, dp,
 	                                   nullptr, stream, RegCoef{0.f, 0.f}, nullptr, MomentumList{})))
 		return rc;
 	return launch_signal(dp.grad_flag, dp.meta, cam.campos, h.D, dp.world, dp.rank, dp.epoch, stream);

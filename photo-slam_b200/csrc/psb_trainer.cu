@@ -660,10 +660,21 @@ int psb_dp_step_depth(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* 
                       const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
                       void* stream_)
 {
+	return psb_dp_step_dist(t, d, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, nullptr, nullptr, nullptr, stream_);
+}
+
+int psb_dp_step_dist(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                     const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
+                     const psb_normal* normal, const psb_dn* dn, const psb_dist* dist, void* stream_)
+{
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
-	if ((rc = check_depth(depth, "psb_dp_step_depth"))) return rc;
-	if ((rc = refuse_filter3d(t, "psb_dp_step_depth"))) return rc;
+	const char* fn = normal || dn || dist ? "psb_dp_step_dist" : "psb_dp_step_depth";
+	if ((rc = check_depth(depth, fn))) return rc;
+	if ((rc = check_normal(normal, fn))) return rc;
+	if ((rc = check_dn(dn, fn))) return rc;
+	if ((rc = check_dist(dist, fn))) return rc;
+	if ((rc = refuse_filter3d(t, fn))) return rc;
 	if (!d || !d->connected || P != d->P || !model) { set_error_msg("psb_dp_step: context not connected or built for a different P"); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, true))) return rc;
 	for (int i = 0; i < 6; i++)
@@ -676,11 +687,12 @@ int psb_dp_step_depth(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* 
 	// every rank's updated rows of the previous step must have landed here before this step reads the parameters
 	if (epoch > 1 && P > 0 && d->world > 1)
 		if ((rc = launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base.get() + d->off_pflag), d->world, epoch - 1, d->status.get(), stream))) return rc;
-	// render, loss, tile backward (the 9 screen-space sums per Gaussian; with a depth term also dL/dz in slot 11, which the push
-	// backward below must consume: a plain push backward would leave it in the sink for the next depth step)
+	// render, loss, tile backward (the 9 screen-space sums per Gaussian; with a depth, consistency or distortion term also dL/dz in slot 11,
+	// with a normal or consistency term 16-float rows with dL/dn in slots 12..14: the push backward below runs the variant t->pass names and
+	// consumes them, where a plain one would leave them in the sink for the next step)
 	TileBackward tb;
 	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, stream, tb, nullptr,
-	                               nullptr)) ||
+	                               nullptr, normal, dn, dist)) ||
 	    P == 0)
 		return rc;
 	const TrainTensors tt = train_tensors(model, true);
@@ -962,14 +974,27 @@ int psb_trainer_backward_exposure(psb_trainer* t, int P, int M, const psb_model*
                                   const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, float* const* grads,
                                   const psb_depth* depth, const psb_exposure* exposure, float* exposure_grad, void* stream_)
 {
+	return psb_trainer_backward_dist(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, grads, depth, exposure, exposure_grad,
+	                                 nullptr, nullptr, nullptr, stream_);
+}
+
+int psb_trainer_backward_dist(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                              const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, float* const* grads,
+                              const psb_depth* depth, const psb_exposure* exposure, float* exposure_grad, const psb_normal* normal, const psb_dn* dn,
+                              const psb_dist* dist, void* stream_)
+{
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
-	if ((rc = check_depth(depth, exposure ? "psb_trainer_backward_exposure" : "psb_trainer_backward_depth"))) return rc;
-	if ((rc = check_exposure(exposure, false, exposure_grad, "psb_trainer_backward_exposure"))) return rc;
-	if ((rc = check_grads(grads, P, "psb_trainer_backward"))) return rc;
+	const bool terms = normal || dn || dist;
+	if ((rc = check_depth(depth, terms ? "psb_trainer_backward_dist" : exposure ? "psb_trainer_backward_exposure" : "psb_trainer_backward_depth"))) return rc;
+	if ((rc = check_exposure(exposure, false, exposure_grad, terms ? "psb_trainer_backward_dist" : "psb_trainer_backward_exposure"))) return rc;
+	if ((rc = check_normal(normal, "psb_trainer_backward_dist"))) return rc;
+	if ((rc = check_dn(dn, "psb_trainer_backward_dist"))) return rc;
+	if ((rc = check_dist(dist, "psb_trainer_backward_dist"))) return rc;
+	if ((rc = check_grads(grads, P, terms ? "psb_trainer_backward_dist" : "psb_trainer_backward"))) return rc;
 	TileBackward tb;
 	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, stream, tb, exposure,
-	                               exposure ? exposure_grad : nullptr)) ||
+	                               exposure ? exposure_grad : nullptr, normal, dn, dist)) ||
 	    P == 0)
 		return rc;
 	GradSegments gs;
@@ -991,14 +1016,31 @@ int psb_trainer_backward_begin_depth(psb_trainer* t, int P, int M, const psb_mod
                                      const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii,
                                      const psb_depth* depth, void* stream_)
 {
+	return psb_trainer_backward_begin_dist(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, nullptr, nullptr, nullptr,
+	                                       stream_);
+}
+
+int psb_trainer_backward_begin_dist(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                                    const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii,
+                                    const psb_depth* depth, const psb_normal* normal, const psb_dn* dn, const psb_dist* dist, void* stream_)
+{
 	int rc;
-	if ((rc = check_depth(depth, "psb_trainer_backward_begin_depth"))) return rc;
-	if ((rc = refuse_filter3d(t, "psb_trainer_backward_begin_depth"))) return rc;
-	// recorded whether or not the call below succeeds: the depth variant of _slab gives the plain result on rows without dL/dz
-	if (t) t->pass = pass_mode(t, -1, depth && depth->gt_depth);
+	const char* fn = normal || dn || dist ? "psb_trainer_backward_begin_dist" : "psb_trainer_backward_begin_depth";
+	if ((rc = check_depth(depth, fn))) return rc;
+	if ((rc = check_normal(normal, fn))) return rc;
+	if ((rc = check_dn(dn, fn))) return rc;
+	if ((rc = check_dist(dist, fn))) return rc;
+	if ((rc = refuse_filter3d(t, fn))) return rc;
+	// recorded whether or not the call below succeeds (render_loss_backward records the same rows again): dL/dz in slot 11 with a depth,
+	// consistency or distortion term, 16-float rows with dL/dn with a normal or consistency term. The variants that read them give the
+	// plain result on rows without those gradients.
+	if (t) {
+		t->pass = pass_mode(t, -1, (depth && depth->gt_depth) || dn || (dist && dist->lambda_dist > 0.f));
+		t->pass.normal = (normal && normal->gt_normal) || dn;
+	}
 	TileBackward tb;
 	return render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, (cudaStream_t)stream_, tb,
-	                            nullptr, nullptr);
+	                            nullptr, nullptr, normal, dn, dist);
 }
 
 int psb_trainer_backward_begin(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
@@ -1017,6 +1059,8 @@ int psb_trainer_backward_slab(psb_trainer* t, int P, int M, const psb_model* mod
 	if (first < 0 || count < 0 || first + count > P || (first % 128) != 0) { set_error_msg("psb_trainer_backward_slab: slab must start at a multiple of 128"); return PSB_ERR_ARG; }
 	if (count == 0) return 0;
 	if ((rc = check_grads(grads, count, "psb_trainer_backward_slab"))) return rc;
+	// a _begin_dist that failed before its pass made the 16-float rows it recorded: there is nothing of that pass to read
+	if (t->pass.normal && t->sink.count() < (size_t)P * 16) { set_error_msg("psb_trainer_backward_slab: no matching backward_begin"); return PSB_ERR_ARG; }
 	const GeomState geom = carve_scratch(t, P, t->carved.W, t->carved.H).geom;
 	GradSegments gs;
 	for (int i = 0; i < 6; i++) gs.g[i] = grads[i];

@@ -212,8 +212,10 @@ def _bind():
         "psb_trainer_backward": call + [P(vp), vp],
         "psb_trainer_backward_depth": call + [P(vp), Depth, vp],
         "psb_trainer_backward_exposure": call + [P(vp), Depth, Exp, vp, vp],
+        "psb_trainer_backward_dist": call + [P(vp), Depth, Exp, vp, P(_Normal), P(_Dn), P(_Dist), vp],
         "psb_trainer_backward_begin": call + [vp],
         "psb_trainer_backward_begin_depth": call + [Depth, vp],
+        "psb_trainer_backward_begin_dist": call + [Depth, P(_Normal), P(_Dn), P(_Dist), vp],
         "psb_trainer_backward_slab": [vp, i, i, Model, Cam, Step, i, i, P(vp), vp],
         "psb_trainer_result": [vp, P(f), P(i), vp],
         "psb_trainer_result_depth": [vp, P(f), P(i), vp],
@@ -244,6 +246,7 @@ def _bind():
         "psb_dp_params": [vp, P(vp)],
         "psb_dp_step": [vp] + call + [vp],
         "psb_dp_step_depth": [vp] + call + [Depth, vp],
+        "psb_dp_step_dist": [vp] + call + [Depth, P(_Normal), P(_Dn), P(_Dist), vp],
         "psb_dp_sync": [vp, vp],
         "psb_dp_status": [vp, vp],
         "psb_dp_destroy": [vp],
@@ -1371,10 +1374,16 @@ class DataParallelTrainer(GaussianTrainer):
     world == 1 and mode=None: backward -> Adam split path on one GPU (tests).
     deterministic: as in GaussianTrainer, kept across rebuild(). "p2p" is then bit-identical run to run at any world size; "nccl"
     gives deterministic per-rank gradients, but the all-reduce's summation order is NCCL's.
-    antialiasing: as in GaussianTrainer, in every mode. Every rank must pass the same value."""
+    antialiasing: as in GaussianTrainer, in every mode. Every rank must pass the same value.
+    geometry_terms=True: trainForOneIteration takes the normal, depth-normal consistency and distortion arguments in every mode
+        (psb_dp_step_dist, psb_trainer_backward_begin_dist, psb_trainer_backward_dist); each rank passes its own view's terms or none.
+        Off (the default), those arguments raise NotImplementedError, as they always have, and every step makes the calls it made
+        before the terms existed."""
+
+    geometry_terms = False
 
     def __init__(self, model, opt=None, background=None, group=None, pipeline=None, nslabs=4, mode=None, deterministic=None,
-                 antialiasing=False, filter3d=False):
+                 antialiasing=False, filter3d=False, geometry_terms=False):
         if filter3d:
             raise NotImplementedError("DataParallelTrainer: the 3D filter is not wired into the data-parallel steps (the NVLink push backward and "
                                       "the slab pipeline have no filtered variant); train with it on one GPU through GaussianTrainer(filter3d=True)")
@@ -1383,6 +1392,7 @@ class DataParallelTrainer(GaussianTrainer):
                                       "regularisers, every rank the noise, and a refinement gather_moments() first); train with it on one GPU "
                                       "through GaussianTrainer")
         super().__init__(model, opt, background, deterministic=deterministic, antialiasing=antialiasing)
+        self.geometry_terms = bool(geometry_terms)
         import os
         import torch.distributed as dist
         self.dist = dist
@@ -1472,11 +1482,11 @@ class DataParallelTrainer(GaussianTrainer):
     def status(self):
         return self.L.psb_dp_status(self.dp, torch.cuda.current_stream().cuda_stream) if self.mode == "p2p" else 0
 
-    def render(self, cam, out=None, radii=None, check=True, out_depth=None, out_alpha=None):
+    def render(self, cam, out=None, radii=None, check=True, out_depth=None, out_alpha=None, out_normal=None, out_depth2=None):
         """Forward only, on the complete replica: the peers store their rows of the last step asynchronously, so the render is
         ordered behind every rank's rows (device-side wait)."""
         self.sync()
-        return super().render(cam, out, radii, check, out_depth, out_alpha)
+        return super().render(cam, out, radii, check, out_depth, out_alpha, out_normal, out_depth2)
 
     def contributionScores(self, cams):
         """As in GaussianTrainer, on the complete replica (ordered behind every rank's rows, like render)."""
@@ -1532,19 +1542,18 @@ class DataParallelTrainer(GaussianTrainer):
                              out_depth=None, exposure_id=None, gt_normal=None, lambda_normal=0.0, out_normal=None, lambda_dn=0.0, dn_alpha_min=0.5,
                              dn_max_rel_jump=0.05, out_depth_normal=None, lambda_dist=0.0, out_depth2=None):
         """Depth arguments as in GaussianTrainer, on every path: "p2p" (psb_dp_step_depth), the slab pipeline
-        (psb_trainer_backward_begin_depth) and the flat "nccl" path (psb_trainer_backward_depth). Each rank passes its own view's
-        target or none: ranks with and without a depth term may train in the same step. exposure_id, the normal arguments and out_depth2
-        must be None, and lambda_dn and lambda_dist 0."""
-        if gt_normal is not None or out_normal is not None or lambda_normal:
-            raise NotImplementedError("DataParallelTrainer: the normal term is not wired into the data-parallel steps (the NVLink push "
-                                      "backward and the slab pipeline carry 12-float sink rows); train with normals on one GPU through "
-                                      "GaussianTrainer")
-        if lambda_dn or out_depth_normal is not None:
-            raise NotImplementedError("DataParallelTrainer: the depth-normal consistency term is not wired into the data-parallel steps (it "
-                                      "needs the normal plane and its 16-float sink rows); train with it on one GPU through GaussianTrainer")
-        if lambda_dist or out_depth2 is not None:
-            raise NotImplementedError("DataParallelTrainer: the depth distortion term is not wired into the data-parallel steps (their "
-                                      "forward renders no second depth moment); train with it on one GPU through GaussianTrainer")
+        (psb_trainer_backward_begin_depth) and the flat "nccl" path (psb_trainer_backward_depth). With geometry_terms=True also the normal,
+        depth-normal consistency and distortion arguments, on every path: "p2p" (psb_dp_step_dist), the slab pipeline
+        (psb_trainer_backward_begin_dist) and the flat "nccl" path (psb_trainer_backward_dist). Each rank passes its own view's terms or
+        none: ranks with different terms may train in the same step. exposure_id must be None."""
+        if not self.geometry_terms:
+            how = "; construct DataParallelTrainer(..., geometry_terms=True) to train it on the data-parallel steps"
+            if gt_normal is not None or out_normal is not None or lambda_normal:
+                raise NotImplementedError("DataParallelTrainer: the normal term is off on this trainer" + how)
+            if lambda_dn or out_depth_normal is not None:
+                raise NotImplementedError("DataParallelTrainer: the depth-normal consistency term is off on this trainer" + how)
+            if lambda_dist or out_depth2 is not None:
+                raise NotImplementedError("DataParallelTrainer: the depth distortion term is off on this trainer" + how)
         if exposure_id is not None:
             raise NotImplementedError("DataParallelTrainer: exposure compensation is not wired into the data-parallel steps: the per-keyframe "
                                       "exposure table would have to be replicated across the ranks (each rank's row updates gathered to "
@@ -1554,7 +1563,11 @@ class DataParallelTrainer(GaussianTrainer):
         if built != m.num_points():
             raise ValueError(f"DataParallelTrainer: the model has {m.num_points()} rows, the trainer was built for {built}: call rebuild() "
                              "after densify, prune or insertion")
+        H, W = int(cam["H"]), int(cam["W"])
         depth = _cdepth(gt_depth, lambda_depth, out_depth)
+        normal = _cnormal(gt_normal, lambda_normal, out_normal, H, W)
+        dn = _cdn(lambda_dn, dn_alpha_min, dn_max_rel_jump, out_depth_normal, H, W)
+        dist = _cdist(lambda_dist, out_depth2, H, W)
         self._apply_deterministic()
         self.iteration += 1
         if densify_stats is None:
@@ -1564,16 +1577,28 @@ class DataParallelTrainer(GaussianTrainer):
         stream = main.cuda_stream
         P = m.num_points()
         args = self._call_args(m, cm, cc, cs, gt_image, mask, out_color, radii)
-        cdepth = C.byref(depth) if depth is not None else None
+        byref = lambda x: C.byref(x) if x is not None else None
+        cdepth = byref(depth)
+        terms = (byref(normal), byref(dn), byref(dist))
+        geo = self.geometry_terms
         if self.mode == "p2p":
-            _lib.check(self.L.psb_dp_step_depth(self.h, self.dp, *args[1:], cdepth, stream), "psb_dp_step_depth")
+            if geo:
+                _lib.check(self.L.psb_dp_step_dist(self.h, self.dp, *args[1:], cdepth, *terms, stream), "psb_dp_step_dist")
+            else:
+                _lib.check(self.L.psb_dp_step_depth(self.h, self.dp, *args[1:], cdepth, stream), "psb_dp_step_depth")
         elif not self.pipeline:
             ptrs = (C.c_void_p * 6)(*[s.data_ptr() for s in self.segs])
-            _lib.check(self.L.psb_trainer_backward_depth(*args, ptrs, cdepth, stream), "psb_trainer_backward_depth")
+            if geo:
+                _lib.check(self.L.psb_trainer_backward_dist(*args, ptrs, cdepth, None, None, *terms, stream), "psb_trainer_backward_dist")
+            else:
+                _lib.check(self.L.psb_trainer_backward_depth(*args, ptrs, cdepth, stream), "psb_trainer_backward_depth")
             scale = self.grads.all_reduce(self.group)   # ONE collective per step: 59 floats per Gaussian
             _lib.check(self.L.psb_adam_update(P, 16, C.byref(cm), ptrs, C.byref(cs), scale, stream), "psb_adam_update")
         else:
-            _lib.check(self.L.psb_trainer_backward_begin_depth(*args, cdepth, stream), "psb_trainer_backward_begin_depth")
+            if geo:
+                _lib.check(self.L.psb_trainer_backward_begin_dist(*args, cdepth, *terms, stream), "psb_trainer_backward_begin_dist")
+            else:
+                _lib.check(self.L.psb_trainer_backward_begin_depth(*args, cdepth, stream), "psb_trainer_backward_begin_depth")
             scale = 1.0 / self.world
             for s, (first, count) in enumerate(self.grads.slabs):
                 ptrs = (C.c_void_p * 6)(*self.grads.kernel_pointers(s))
@@ -1599,31 +1624,33 @@ class DataParallelTrainer(GaussianTrainer):
     def result(self):
         """-> (loss, l1, ssim, num_rendered) of this rank's view. A view whose binning arena overflowed contributed a zero
         gradient to the step (every rank still stepped, replicas identical); it is counted in `dropped_views`, the arena
-        has been grown, and the step is NOT repeated (a one-rank retry would desynchronise the group). result_depth() adds this
-        rank's depth_l1; all four terms are NaN for a dropped view."""
-        return self._result(False)
+        has been grown, and the step is NOT repeated (a one-rank retry would desynchronise the group). result_depth(),
+        result_normal(), result_dn() and result_dist() add this rank's terms as GaussianTrainer's do; every term is NaN for a
+        dropped view."""
+        return self._result(3)
 
-    def _result(self, with_depth):
-        out, n = (C.c_float * 4)(), C.c_int()
-        rc = self.L.psb_trainer_result_depth(self.h, out, C.byref(n), torch.cuda.current_stream().cuda_stream)
+    def _result(self, nterms):
+        out, n = (C.c_float * 7)(), C.c_int()
+        rc = self.L.psb_trainer_result_dist(self.h, out, C.byref(n), torch.cuda.current_stream().cuda_stream)
         if rc == -4:
             self.dropped_views += 1
-            out = (float("nan"),) * 4
+            out = (float("nan"),) * 7
         else:
-            _lib.check(rc, "psb_trainer_result_depth")
-        return (*out[:4 if with_depth else 3], n.value)
+            _lib.check(rc, "psb_trainer_result_dist")
+        return (*out[:nterms], n.value)
 
     def trainWithLoss(self, *args, **kwargs):
         raise NotImplementedError("DataParallelTrainer.trainWithLoss: a caller's loss is not wired into the data-parallel steps (the "
                                   "fused Adam of one rank would desynchronise the replicas); use GaussianTrainer.trainWithLoss on one GPU, or "
                                   "render() + backwardPixels(..., grads=...) + your own all-reduce + psb_adam_update")
 
-    def backwardPixels(self, dL_dcolor, dL_ddepth=None, dL_dalpha=None, grads=None, densify_stats=None):
+    def backwardPixels(self, dL_dcolor, dL_ddepth=None, dL_dalpha=None, grads=None, densify_stats=None, dL_dnormal=None, dL_ddepth2=None):
         """Gradient mode only (grads= required): a one-rank Adam step would desynchronise the replicas."""
         if grads is None:
             raise NotImplementedError("DataParallelTrainer.backwardPixels: pass grads= (the gradient mode); a one-rank Adam step would "
                                       "desynchronise the replicas")
-        return super().backwardPixels(dL_dcolor, dL_ddepth, dL_dalpha, grads=grads, densify_stats=densify_stats)
+        return super().backwardPixels(dL_dcolor, dL_ddepth, dL_dalpha, grads=grads, densify_stats=densify_stats, dL_dnormal=dL_dnormal,
+                                      dL_ddepth2=dL_ddepth2)
 
     def sync_densify_stats(self):
         """Reduce the rank-local densification statistics (call right before densify/prune)."""
