@@ -1,11 +1,13 @@
 """A float64 restatement of one whole training iteration of the fused step (include/psb200.h): the forward with the 3D filter, the
-anti-aliasing factor and the normal plane, the built-in loss with exposure, depth and normal terms, the 3DGS-MCMC regularisers, the
-densification statistics and the Adam update of every parameter, its moments and the exposure row. The arbiter the per-Gaussian stage
-(gaussian_backward_kernel<MODE> and frest_stream_kernel) is measured against, in every flag set and base.
+anti-aliasing factor, the normal plane and the second depth moment, the built-in loss with exposure, depth, normal, depth-normal consistency
+and distortion terms, the 3DGS-MCMC regularisers, the densification statistics and the Adam update of every parameter, its moments and the
+exposure row. The arbiter the per-Gaussian stage (gaussian_backward_kernel<MODE> and frest_stream_kernel) is measured against, in every
+flag set and base.
 
-Plain torch, differentiable with autograd, on any device. Built on splat64 (render, loss) and normal64 (per-Gaussian normals, normal L1)
-without changing their behaviour (normal64.gaussian_normals takes flip=False for the perturbed truth). Decisions this module adds (the normal's axis and flip, the kinks of the depth and normal L1) are constants of the
-pass; `margins` reports how far each lies from its threshold, next to splat64.margins'.
+Plain torch, differentiable with autograd, on any device. Built on splat64 (render, loss), normal64 (per-Gaussian normals, normal L1),
+dn64 (consistency) and dist64 (distortion) without changing their behaviour (normal64.gaussian_normals takes flip=False for the perturbed
+truth). Decisions this module adds (the normal's axis and flip, the kinks of the depth and normal L1, the consistency term's alpha and
+depth-jump tests) are constants of the pass; `margins` reports how far each lies from its threshold, next to splat64.margins'.
 
 Conventions the perturbation tests alter live in `StepConv`.
 """
@@ -14,6 +16,8 @@ import math
 
 import torch
 
+import dist64
+import dn64
 import normal64 as n64
 import splat64 as s64
 
@@ -29,6 +33,7 @@ class StepConv:
     reg_reached_only: bool = True      # the regularisers act on the rows the pass reaches, not on all P rows
     f3d_opacity: bool = True           # the 3D filter multiplies the opacity by c
     normal_flip: bool = True           # the normal faces the camera (n = -m when m . t > 0)
+    dist_dz: bool = True               # the second moment's z_i^2 carries its gradient 2 z_i dL/dM into dL/dz_i
 
 
 STEP_CONV = StepConv()
@@ -36,12 +41,16 @@ STEP_CONV = StepConv()
 
 @dataclasses.dataclass(frozen=True)
 class Flags:
-    """the per-Gaussian stage's flags (psb_train.cu MODE_DEPTH / _AA / _REG / _F3D / _NORMAL) and the regularisers' lambdas"""
+    """the per-Gaussian stage's flags (psb_train.cu MODE_DEPTH / _AA / _REG / _F3D / _NORMAL), the optional consistency (dn) and
+    distortion (dist) terms of the loss, and the regularisers' lambdas. normal: the normal L1 against targets["normal"]; dn renders the
+    normal plane too (the kernels' MODE_NORMAL), dn and dist the depth's dL/dz (MODE_DEPTH) whether or not depth is set."""
     depth: bool = False
     aa: bool = False
     reg: bool = False
     f3d: bool = False
     normal: bool = False
+    dn: bool = False
+    dist: bool = False
     lambda_opacity: float = 0.01       # GaussianOptimizationParams.opacity_reg
     lambda_scale: float = 0.01         # GaussianOptimizationParams.scale_reg
 
@@ -50,7 +59,7 @@ ALL_FLAGS = [Flags(depth=bool(k & 1), aa=bool(k & 2), reg=bool(k & 4), f3d=bool(
 
 
 def flag_name(fl):
-    return "+".join(n for n in ("depth", "aa", "reg", "f3d", "normal") if getattr(fl, n)) or "plain"
+    return "+".join(n for n in ("depth", "aa", "reg", "f3d", "normal", "dn", "dist") if getattr(fl, n)) or "plain"
 
 
 # ---- the forward --------------------------------------------------------------------------------------------------------------------
@@ -82,27 +91,48 @@ def splat_inputs(raw, flags, f=None, conv=STEP_CONV):
 
 
 def forward(raw, cam, flags, D, bg, f=None, conv=STEP_CONV):
-    """-> (s64.composite's dict plus radii and geo, N [3,H,W] or None, n [P,3] or None): the trainer's forward of one pass"""
+    """-> (s64.composite's dict plus radii and geo, N [3,H,W] or None, n [P,3] or None): the trainer's forward of one pass. The dict
+    holds the accumulated opacity A = 1 - T_final under "alpha" and, with flags.dist, the second depth moment M = sum_i z_i^2 alpha_i T_i
+    under "depth2" (the blend with the colour replaced by (z^2, 0, 0) and no background, as dist64.render_moment)."""
     g = splat_inputs(raw, flags, f, conv)
     geo = s64.geometry(g, cam, D, flags.aa)
     out = s64.composite(geo, cam["W"], cam["H"], bg)
     out.update(radii=geo["radius"], geo=geo)
     N = n = None
-    if flags.normal:
+    if flags.normal or flags.dn:
         n = normals(raw, cam, conv.normal_flip)
         N = s64.composite(dict(geo, rgb=n), cam["W"], cam["H"], (0.0, 0.0, 0.0))["color"]
+    if flags.dist:
+        z = geo["z"] if conv.dist_dz else geo["z"].detach()
+        zero = torch.zeros_like(z)
+        out["depth2"] = s64.composite(dict(geo, rgb=torch.stack([z * z, zero, zero], 1)), cam["W"], cam["H"], (0.0, 0.0, 0.0))["color"][0]
     return out, N, n
 
 
-def image_loss(out, N, targets, flags, E=None):
-    """-> (total, dict of the scalars): loss64 (mask, exposure row E) + lambda_depth depth_l1_64 + lambda_normal normal_l1_64"""
+def image_loss(out, N, targets, flags, E=None, cam=None):
+    """-> (total, dict of the scalars): loss64 (mask, exposure row E) + lambda_depth depth_l1_64 + lambda_normal normal_l1_64, and with
+    flags.dn / flags.dist + lambda_dn dn64 (of D, A and N seen by cam; dn_alpha_min, dn_max_rel_jump) + lambda_dist dist64 (of D, A, M),
+    both with the mask. targets["colour"] = False drops loss64: the loss of a colour target equal to the render with lambda_dssim = 0,
+    whose photometric gradient is exactly zero (l1 reads 0 and ssim 1 then)."""
     mask = targets.get("mask")
-    L, l1, ssim = s64.loss64(out["color"], targets["gt"], mask, targets.get("lambda_dssim", 0.2), E)
-    zero = torch.zeros((), dtype=torch.float64, device=L.device)
+    dev = out["depth"].device
+    zero = torch.zeros((), dtype=torch.float64, device=dev)
+    if targets.get("colour", True):
+        L, l1, ssim = s64.loss64(out["color"], targets["gt"], mask, targets.get("lambda_dssim", 0.2), E)
+    else:
+        L, l1, ssim = zero, zero, torch.ones((), dtype=torch.float64, device=dev)
     dl1 = s64.depth_l1_64(out["depth"], targets["depth"], mask) if flags.depth else zero
     nl1 = n64.normal_l1_64(N, targets["normal"], mask) if flags.normal else zero
     total = L + targets.get("lambda_depth", 0.0) * dl1 + targets.get("lambda_normal", 0.0) * nl1
-    return total, dict(l1=l1, ssim=ssim, depth_l1=dl1, normal_l1=nl1)
+    dn = dist = zero
+    if flags.dn:
+        dn = dn64.dn64(out["depth"], out["alpha"], N, cam["W"], cam["H"], cam["tanfovx"], cam["tanfovy"], targets.get("dn_alpha_min", 0.5),
+                       targets.get("dn_max_rel_jump", 0.05), mask)[0]
+        total = total + targets["lambda_dn"] * dn
+    if flags.dist:
+        dist = dist64.dist64(out["depth"], out["alpha"], out["depth2"], mask)[0]
+        total = total + targets["lambda_dist"] * dist
+    return total, dict(l1=l1, ssim=ssim, depth_l1=dl1, normal_l1=nl1, dn=dn, dist=dist)
 
 
 def regularizer(raw, rows, flags):
@@ -129,8 +159,10 @@ def _nz_rows(t, P):
 
 def grads64(state, cam, targets, flags, conv=STEP_CONV):
     """The gradients of one pass: -> dict(grads {group: dL/dparam, reg included}, E (dL/dE or None), loss scalars, reached [P],
-    visible [P], radii [P], mean2D [P,2] (dL/dmean2D in the statistics' units), pixel (dL/dI [3,H,W], dL/dD [H,W], dL/dN [3,H,W] or None:
-    the per-pixel gradients of the loss w.r.t. the raw render))"""
+    visible [P], radii [P], mean2D [P,2] (dL/dmean2D in the statistics' units), pixel (dL/dI [3,H,W], dL/dD [H,W], dL/dA [H,W],
+    dL/dN [3,H,W] or None, dL/dM [H,W] or None: the per-pixel gradients of the loss w.r.t. the raw render), inter ({means2D, conic, o,
+    rgb, z, n}: the per-Gaussian gradients w.r.t. the screen-space record, zeros where the loss does not depend on it; n only with a normal
+    plane))"""
     raw = {k: state["params"][k].detach().clone().requires_grad_(True) for k in GROUPS}
     E = state.get("E")
     E = E.detach().clone().requires_grad_(True) if E is not None else None
@@ -139,10 +171,12 @@ def grads64(state, cam, targets, flags, conv=STEP_CONV):
     inter = dict(means2D=geo["means2D"], conic=geo["conic"], o=geo["o"], rgb=geo["rgb"], z=geo["z"])
     if n is not None:
         inter["n"] = n
-    pix = dict(color=out["color"], depth=out["depth"])
+    pix = dict(color=out["color"], depth=out["depth"], alpha=out["alpha"])
     if N is not None:
         pix["normal"] = N
-    total, scal = image_loss(out, N, targets, flags, E)
+    if "depth2" in out:
+        pix["depth2"] = out["depth2"]
+    total, scal = image_loss(out, N, targets, flags, E, cam)
     leaves = [raw[k] for k in GROUPS] + ([E] if E is not None else [])
     keys = list(inter) + list(pix)
     res = torch.autograd.grad(total, leaves + [inter[k] for k in inter] + [pix[k] for k in pix], allow_unused=True)
@@ -165,9 +199,11 @@ def grads64(state, cam, targets, flags, conv=STEP_CONV):
     if conv.mean2d_ndc:
         m2 = m2 * torch.tensor([0.5 * cam["W"], 0.5 * cam["H"]], dtype=torch.float64, device=dev)
     z = lambda t, like: t if t is not None else torch.zeros_like(like)
-    pixel = dict(color=z(rest["color"], out["color"]), depth=z(rest["depth"], out["depth"]),
-                 normal=z(rest["normal"], N) if N is not None else None)
+    pixel = dict(color=z(rest["color"], out["color"]), depth=z(rest["depth"], out["depth"]), alpha=z(rest["alpha"], out["alpha"]),
+                 normal=z(rest["normal"], N) if N is not None else None,
+                 depth2=z(rest["depth2"], out["depth2"]) if "depth2" in out else None)
     return dict(grads=grads, E=gE, reached=reached, visible=out["radii"] > 0, radii=out["radii"], mean2D=m2, pixel=pixel,
+                inter={k: z(rest[k], inter[k]) for k in inter},
                 loss=dict(loss=float(total.detach()), **{k: float(v.detach()) for k, v in scal.items()}), out=out, N=N)
 
 
@@ -177,7 +213,8 @@ def step64(state, cam, targets, flags, conv=STEP_CONV, stats=True):
       Adam step step + 1), lr [6] (the model's lr_, f_rest at lr / 20 already), D (active SH degree), f [P] (the 3D filter, with
       flags.f3d), and optionally the exposure row E [3,4], E_m, E_v, E_step (its step count before this update), E_lr).
     cam: splat64.camera64; targets: dict(gt [3,H,W], mask [3,H,W] or None, depth [H,W], normal [3,H,W], lambda_depth, lambda_normal,
-      bg, lambda_dssim).
+      bg, lambda_dssim, and with flags.dn / flags.dist lambda_dn, dn_alpha_min, dn_max_rel_jump / lambda_dist; colour = False drops the
+      photometric term).
     -> dict(state = the next state, and grads64's entries: loss scalars, reached and visible masks, gradients)."""
     r = grads64(state, cam, targets, flags, conv)
     t = state["step"] + 1
@@ -200,13 +237,17 @@ def step64(state, cam, targets, flags, conv=STEP_CONV, stats=True):
 # ---- margins ------------------------------------------------------------------------------------------------------------------------
 def margins(state, cam, targets, flags, conv=STEP_CONV):
     """splat64.margins of the splat the pass draws (3D filter and anti-aliasing as flagged), plus the decisions this module adds:
-    axis (gap between the two smallest raw log-scales of a live row) and flip (|m . t| / (|m| |t|)) with the normal term; depth_kink
-    (|D - G| / G) and normal_kink (|N_c - G_c|) at the valid pixels some splat reaches, charged to the pixel's last blended Gaussian."""
+    axis (gap between the two smallest raw log-scales of a live row) and flip (|m . t| / (|m| |t|)) with a normal plane; depth_kink
+    (|D - G| / G) and normal_kink (|N_c - G_c|) at the valid pixels some splat reaches, charged to the pixel's last blended Gaussian.
+    With the consistency term: dn_alpha (|A - alpha_min| / alpha_min at every pixel some splat reaches: A >= alpha_min decides whether
+    D / A exists there) and dn_jump (| |z_nb - z| - j z | / (j z), j = max_rel_jump, for each stencil pair of a mask-valid interior pixel
+    whose normalised depths z, z_nb both exist), charged to the last blended Gaussian of the pixel and, for a pair, of its neighbour too.
+    The distortion's validity is the mask alone, a constant of the targets: it adds no decision."""
     with torch.no_grad():
         raw = {k: state["params"][k] for k in GROUPS}
         g = splat_inputs(raw, flags, state.get("f"), conv)
         res = s64.margins(g, cam, state["D"], flags.aa, targets["bg"])
-        if not (flags.normal or flags.depth):
+        if not (flags.normal or flags.depth or flags.dn):
             return res
         out, N, n = forward(raw, cam, flags, state["D"], targets["bg"], state.get("f"), conv)
         alive = out["geo"]["alive"]
@@ -221,7 +262,7 @@ def margins(state, cam, targets, flags, conv=STEP_CONV):
             G = targets["depth"].reshape(-1)
             sel = keep & (G > 0)
             res["depth_kink"] = _charge(((out["depth"].reshape(-1) - G).abs() / G.clamp_min(1e-30))[sel], sel.nonzero().reshape(-1), last, cover)
-        if flags.normal:
+        if flags.normal or flags.dn:
             sc = torch.sort(raw["scaling"], dim=1).values
             res["axis"] = ((sc[:, 1] - sc[:, 0])[alive], ids[alive])
             V = cam["V"]
@@ -229,10 +270,38 @@ def margins(state, cam, targets, flags, conv=STEP_CONV):
             tv = raw["xyz"] @ V[:3, :3] + V[3, :3]
             cosang = (mvec * tv).sum(1).abs() / (mvec.norm(dim=1) * tv.norm(dim=1)).clamp_min(1e-300)
             res["flip"] = (cosang[alive], ids[alive])
+        if flags.normal:
             G = targets["normal"].reshape(3, -1)
             sel = keep & (G != 0).any(0)
             d = (N.reshape(3, -1) - G).abs()[:, sel].amin(0)
             res["normal_kink"] = _charge(d, sel.nonzero().reshape(-1), last, cover)
+        if flags.dn:
+            res.update(_dn_margins(out, cam, targets, last, cover))
+    return res
+
+
+def _dn_margins(out, cam, targets, last, cover):
+    W, H = cam["W"], cam["H"]
+    amin, jump = targets.get("dn_alpha_min", 0.5), targets.get("dn_max_rel_jump", 0.05)
+    A = out["alpha"].reshape(-1)
+    sel = last >= 0
+    res = dict(dn_alpha=_charge(((A - amin).abs() / amin)[sel], sel.nonzero().reshape(-1), last, cover))
+    z = dn64.normalised_depth(out["depth"], out["alpha"], amin)
+    pix = torch.arange(H * W, device=z.device).reshape(H, W)
+    centre = (z > 0)[1:-1, 1:-1]
+    mask = targets.get("mask")
+    if mask is not None:
+        centre &= (mask[0] != 0)[1:-1, 1:-1]
+    zc, pc = z[1:-1, 1:-1], pix[1:-1, 1:-1]
+    vals, pa, pb = [], [], []
+    for zn, pn in ((z[1:-1, :-2], pix[1:-1, :-2]), (z[1:-1, 2:], pix[1:-1, 2:]), (z[:-2, 1:-1], pix[:-2, 1:-1]), (z[2:, 1:-1], pix[2:, 1:-1])):
+        both = centre & (zn > 0)
+        vals.append((((zn - zc).abs() - jump * zc).abs() / (jump * zc))[both])
+        pa.append(pc[both])
+        pb.append(pn[both])
+    vals, pa, pb = torch.cat(vals), torch.cat(pa), torch.cat(pb)
+    ca, cb = _charge(vals, pa, last, cover), _charge(vals, pb, last, cover)
+    res["dn_jump"] = (torch.cat([ca[0], cb[0]]), torch.cat([ca[1], cb[1]]))
     return res
 
 

@@ -505,9 +505,9 @@ DP_CASES = [("p2p", d, a) for d in (False, True) for a in (False, True)] + [("sl
 
 @pytest.mark.parametrize("mode,depth,aa", DP_CASES, ids=[f"{m}-{'depth' if d else 'nodepth'}-{'aa' if a else 'plain'}" for m, d, a in DP_CASES])
 def test_dp_step(cuda, mode, depth, aa):
-    """one DataParallelTrainer step at world 1 against step64 (no exposure, normal, regulariser or filter: the data-parallel steps take
-    none): p2p runs gaussian_backward_kernel<MODE_PUSH | flags> and the owner-side Adam, the slab pipeline the per-slab gradient kernels and
-    the flat Adam with its scalar tail"""
+    """one DataParallelTrainer step at world 1 against step64 with {depth, aa} (the data-parallel steps take no exposure, regulariser or
+    filter; their normal, consistency and distortion terms are checked in test_dp64_gpu): p2p runs gaussian_backward_kernel<MODE_PUSH |
+    flags> and the owner-side Adam, the slab pipeline the per-slab gradient kernels and the flat Adam with its scalar tail"""
     from photo_slam_b200 import trainer
     fl = step64.Flags(depth=depth, aa=aa)
     k = int(depth) + 2 * int(aa)
