@@ -66,25 +66,18 @@ static int arg_error(const char* fn, const char* what)
 	return PSB_ERR_ARG;
 }
 
-// Planes of the operator forward beyond colour (include/psb200.h psb_raster_planes; NULL = not rendered). normal_scratch / normal_bytes:
-// the caller's scratch of psb_rasterize_planes_bytes(P, 0) bytes, read only with the normal plane.
-struct FwdPlanes {
-	float *depth, *alpha, *normal, *depth2;
-	void* normal_scratch;
-	size_t normal_bytes;
-};
-
 // Scratch bytes of the operator's normal plane; 0 for a negative size.
 static size_t op_plane_bytes(int P, int R) { return (P < 0 || R < 0) ? 0 : OpPlaneState::required_bytes((size_t)P, (size_t)R); }
 
-// Body of psb_rasterize_forward[_depth|_aa|_planes]; fn names the entry point in error messages. pl: the planes beyond colour; aa: the
-// 2D Mip filter.
+// Body of psb_rasterize_forward[_depth|_aa|_planes]; fn names the entry point in error messages. pl: the planes beyond colour
+// (include/psb200.h psb_raster_planes; pl.normals is filled in here); plane_scratch / plane_bytes: the caller's scratch of
+// psb_rasterize_planes_bytes(P, 0) bytes, read only with the normal plane; aa: the 2D Mip filter.
 static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void* geometry_user, psb_alloc_fn binning_buffer, void* binning_user,
                              psb_alloc_fn image_buffer, void* image_user, int P, int D, int M, const float* background, int width, int height,
                              const float* means3D, const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
                              float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
                              const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered, float* out_color,
-                             int* radii, const FwdPlanes& pl, bool aa, void* stream_)
+                             int* radii, FwdPlanes pl, void* plane_scratch, size_t plane_bytes, bool aa, void* stream_)
 {
 	(void)prefiltered;  // the reference only uses it for a device-side assert (auxiliary.h:156-160)
 	cudaStream_t stream = (cudaStream_t)stream_;
@@ -95,8 +88,8 @@ static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void*
 	if (P > 0 && shs && (M < (D + 1) * (D + 1) || D > 3 || D < 0)) return arg_error(fn, "SH degree / coefficient count mismatch");
 	if (P > 0 && shs && !cam_pos) return arg_error(fn, "cam_pos required with shs");
 	if (width > 65535 * 16 || height > 65535 * 16) return arg_error(fn, "image too large");
-	if (pl.normal && cov3D_precomp) return arg_error(fn, "the normal plane needs scales and rotations, not cov3D_precomp");
-	if (pl.normal && (!pl.normal_scratch || pl.normal_bytes < op_plane_bytes(P, 0)))
+	if (pl.out_normal && cov3D_precomp) return arg_error(fn, "the normal plane needs scales and rotations, not cov3D_precomp");
+	if (pl.out_normal && (!plane_scratch || plane_bytes < op_plane_bytes(P, 0)))
 		return arg_error(fn, ("the normal plane needs a plane_scratch of psb_rasterize_planes_bytes(P, 0) = " + std::to_string(op_plane_bytes(P, 0)) +
 		                      " bytes").c_str());
 
@@ -112,11 +105,12 @@ static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void*
 	const GaussIn in = make_input(P, D, M, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp);
 	int rc;
 	if ((rc = launch_preprocess(in, cam, radii, geom, /*raw=*/false, /*tight=*/false, stream, aa))) return rc;
-	float4* normals = nullptr;
-	if (pl.normal) {
-		char* chunk = static_cast<char*>(pl.normal_scratch);
-		normals = OpPlaneState::from_chunk(chunk, (size_t)P, 0).normals;
+	pl.normals = nullptr;
+	if (pl.out_normal) {
+		char* chunk = static_cast<char*>(plane_scratch);
+		float4* normals = OpPlaneState::from_chunk(chunk, (size_t)P, 0).normals;
 		if ((rc = launch_op_normals(in, cam, geom.tile_info, normals, stream))) return rc;
+		pl.normals = normals;
 	}
 	if ((rc = launch_depth_sort_and_scan(P, geom, /*scan=*/true, stream))) return rc;
 
@@ -132,8 +126,8 @@ static int rasterize_forward(const char* fn, psb_alloc_fn geometry_buffer, void*
 	BinState bin = BinState::from_chunk(bin_chunk, (size_t)num_rendered);
 	if ((rc = launch_binning(P, cam, geom, bin, img, (size_t)num_rendered, stream))) return rc;
 
-	if ((rc = launch_render_forward(cam, img.ranges, bin.inst[sorted_slot(width, height)], geom.rec, background, out_color, img.final_T, img.n_contrib, stream,
-	                                pl.depth, pl.alpha, /*score=*/nullptr, normals, pl.normal, pl.depth2)))
+	if ((rc = launch_render_forward(cam, img.ranges, bin.inst[sorted_slot(width, height)], geom.rec, background, out_color, img.final_T, img.n_contrib, pl,
+	                                stream)))
 		return rc;
 	return (int)num_rendered;
 }
@@ -224,8 +218,9 @@ static int rasterize_backward(const char* fn, int P, int D, int M, int R, const 
 			slots.slots = slot_rows; slots.base = ds.base; slots.tile_info = geom.tile_info; slots.counters = geom.counters;
 			slots.capacity = (uint32_t)R; slots.seq = 1u; slots.P = P; slots.tight = 0;
 		}
+		const BwdPlanes planes{dL_ddepth, v.det ? &slots : nullptr, v.dL_dalpha, ps.normals, v.dL_dnormal, v.dL_ddepth2, ps.dn};
 		if ((rc = launch_render_backward(cam, img.ranges, bin.inst[sorted_slot(width, height)], geom.rec, background, img.final_T, img.n_contrib, dL_dpix,
-		                                 sink, stream, dL_ddepth, v.det ? &slots : nullptr, v.dL_dalpha, ps.normals, v.dL_dnormal, v.dL_ddepth2, ps.dn)))
+		                                 sink, planes, stream)))
 			return rc;
 	}
 
@@ -260,7 +255,7 @@ int psb_rasterize_forward(psb_alloc_fn geometry_buffer, void* geometry_user, psb
 {
 	return rasterize_forward("psb_rasterize_forward", geometry_buffer, geometry_user, binning_buffer, binning_user, image_buffer, image_user, P, D, M,
 	                         background, width, height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp,
-	                         viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, FwdPlanes{}, /*aa=*/false, stream);
+	                         viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, FwdPlanes{}, nullptr, 0, /*aa=*/false, stream);
 }
 
 int psb_rasterize_forward_depth(psb_alloc_fn geometry_buffer, void* geometry_user, psb_alloc_fn binning_buffer, void* binning_user,
@@ -272,7 +267,7 @@ int psb_rasterize_forward_depth(psb_alloc_fn geometry_buffer, void* geometry_use
 {
 	return rasterize_forward("psb_rasterize_forward_depth", geometry_buffer, geometry_user, binning_buffer, binning_user, image_buffer, image_user, P,
 	                         D, M, background, width, height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations,
-	                         cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, FwdPlanes{out_depth}, /*aa=*/false, stream);
+	                         cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, FwdPlanes{out_depth}, nullptr, 0, /*aa=*/false, stream);
 }
 
 int psb_rasterize_backward(int P, int D, int M, int R, const float* background, int width, int height, const float* means3D, const float* shs,
@@ -334,7 +329,7 @@ int psb_rasterize_forward_aa(psb_alloc_fn geometry_buffer, void* geometry_user, 
 	if (antialiasing != 0 && antialiasing != 1) return arg_error("psb_rasterize_forward_aa", "antialiasing must be 0 or 1");
 	return rasterize_forward("psb_rasterize_forward_aa", geometry_buffer, geometry_user, binning_buffer, binning_user, image_buffer, image_user, P, D,
 	                         M, background, width, height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp,
-	                         viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, FwdPlanes{out_depth}, antialiasing != 0, stream);
+	                         viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, FwdPlanes{out_depth}, nullptr, 0, antialiasing != 0, stream);
 }
 
 int psb_rasterize_backward_aa(int P, int D, int M, int R, const float* background, int width, int height, const float* means3D, const float* shs,
@@ -369,11 +364,10 @@ int psb_rasterize_forward_planes(psb_alloc_fn geometry_buffer, void* geometry_us
 	const char* fn = "psb_rasterize_forward_planes";
 	if (antialiasing != 0 && antialiasing != 1) return arg_error(fn, "antialiasing must be 0 or 1");
 	FwdPlanes pl{};
-	if (planes) { pl.depth = planes->out_depth; pl.alpha = planes->out_alpha; pl.normal = planes->out_normal; pl.depth2 = planes->out_depth2; }
-	pl.normal_scratch = plane_scratch; pl.normal_bytes = plane_scratch_bytes;
+	if (planes) { pl.out_depth = planes->out_depth; pl.out_alpha = planes->out_alpha; pl.out_normal = planes->out_normal; pl.out_depth2 = planes->out_depth2; }
 	return rasterize_forward(fn, geometry_buffer, geometry_user, binning_buffer, binning_user, image_buffer, image_user, P, D, M, background, width,
 	                         height, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix,
-	                         cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, pl, antialiasing != 0, stream);
+	                         cam_pos, tan_fovx, tan_fovy, prefiltered, out_color, radii, pl, plane_scratch, plane_scratch_bytes, antialiasing != 0, stream);
 }
 
 int psb_rasterize_backward_planes(int P, int D, int M, int R, const float* background, int width, int height, const float* means3D, const float* shs,

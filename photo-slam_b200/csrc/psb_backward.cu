@@ -15,12 +15,13 @@ namespace psb {
 // NORMAL (scales + rotations): dL_dn [P,3] holds dL/dn of the operator's n_i (op_normals_kernel: activated scales, the rotation as given);
 // its rotation gradient, through column k of R(q), the sign and V (normal_axis_backward), joins dL/drot. The arg-min k and the sign are
 // piecewise constant, so nothing reaches the scales or the mean.
-template <bool DEPTH, bool AA = false, bool NORMAL = false>
-__device__ __forceinline__ void preprocess_bwd_body(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
-                                                    int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
-                                                    const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out,
-                                                    const float* __restrict__ dL_dz, float* __restrict__ dL_dopacity = nullptr,
-                                                    const float* __restrict__ dL_dn = nullptr)
+// One entry for the eight variants: dL_dz is read only when DEPTH, dL_dopacity only when AA, dL_dn only when NORMAL.
+template <bool DEPTH, bool AA, bool NORMAL>
+__global__ void __launch_bounds__(128) preprocess_bwd_kernel(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
+                                                             int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
+                                                             const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out,
+                                                             const float* __restrict__ dL_dz, float* __restrict__ dL_dopacity,
+                                                             const float* __restrict__ dL_dn)
 {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	if (idx >= in.P || geom.tile_info[idx].z == 0) return;
@@ -76,48 +77,20 @@ __device__ __forceinline__ void preprocess_bwd_body(GaussIn in, Camera cam, Geom
 	}
 }
 
-// One entry for the four (DEPTH, AA) variants: dL_dz is read only when DEPTH, dL_dopacity only when AA.
-template <bool DEPTH, bool AA>
-__global__ void __launch_bounds__(128) preprocess_bwd_kernel(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
-                                                             int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
-                                                             const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out,
-                                                             const float* __restrict__ dL_dz, float* __restrict__ dL_dopacity)
-{
-	preprocess_bwd_body<DEPTH, AA>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out, dL_dz,
-	                               dL_dopacity);
-}
-
-// The operator's normal variants (psb_rasterize_backward_planes with a normal gradient): the four (DEPTH, AA) variants plus dL/dn. An
-// entry of its own, so the preprocess_bwd_kernel variants keep their names, parameters and code.
-template <bool DEPTH, bool AA>
-__global__ void __launch_bounds__(128) preprocess_bwd_normal_kernel(GaussIn in, Camera cam, GeomState geom, const float* __restrict__ dL_dmean2D,
-                                                                    int mean2D_stride, const float* __restrict__ dL_dconic, int conic_stride,
-                                                                    const float* __restrict__ dL_dcolor, int color_stride, GaussGradOut out,
-                                                                    const float* __restrict__ dL_dz, float* __restrict__ dL_dopacity,
-                                                                    const float* __restrict__ dL_dn)
-{
-	preprocess_bwd_body<DEPTH, AA, true>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out, dL_dz,
-	                                     dL_dopacity, dL_dn);
-}
-
 int launch_preprocess_backward(const GaussIn& in, const Camera& cam, const GeomState& geom, const float* dL_dmean2D, int mean2D_stride,
                                const float* dL_dconic, int conic_stride, const float* dL_dcolor, int color_stride,
                                const GaussGradOut& out, cudaStream_t stream, const float* dL_dz, float* aa_dL_dopacity, const float* dL_dn)
 {
 	if (in.P == 0) return 0;
-	if (dL_dn) {
-		if (!in.scales || !in.rotations) { set_error_msg("launch_preprocess_backward: the normal gradient needs scales and rotations"); return -1; }
-		auto kernel = aa_dL_dopacity ? (dL_dz ? preprocess_bwd_normal_kernel<true, true> : preprocess_bwd_normal_kernel<false, true>)
-		                             : (dL_dz ? preprocess_bwd_normal_kernel<true, false> : preprocess_bwd_normal_kernel<false, false>);
-		kernel<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out,
-		                                            dL_dz, aa_dL_dopacity, dL_dn);
-		PSB_LAUNCH_OK();
-		return 0;
-	}
-	auto kernel = aa_dL_dopacity ? (dL_dz ? preprocess_bwd_kernel<true, true> : preprocess_bwd_kernel<false, true>)
-	                             : (dL_dz ? preprocess_bwd_kernel<true, false> : preprocess_bwd_kernel<false, false>);
-	kernel<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out,
-	                                            dL_dz, aa_dL_dopacity);
+	if (dL_dn && (!in.scales || !in.rotations)) { set_error_msg("launch_preprocess_backward: the normal gradient needs scales and rotations"); return -1; }
+	const int v = (dL_dz ? 1 : 0) | (aa_dL_dopacity ? 2 : 0) | (dL_dn ? 4 : 0);
+	using Kernel = decltype(&preprocess_bwd_kernel<false, false, false>);
+	static const Kernel VARIANTS[8] = {preprocess_bwd_kernel<false, false, false>, preprocess_bwd_kernel<true, false, false>,
+	                                   preprocess_bwd_kernel<false, true, false>,  preprocess_bwd_kernel<true, true, false>,
+	                                   preprocess_bwd_kernel<false, false, true>,  preprocess_bwd_kernel<true, false, true>,
+	                                   preprocess_bwd_kernel<false, true, true>,   preprocess_bwd_kernel<true, true, true>};
+	VARIANTS[v]<<<cdiv(in.P, 128), 128, 0, stream>>>(in, cam, geom, dL_dmean2D, mean2D_stride, dL_dconic, conic_stride, dL_dcolor, color_stride, out, dL_dz,
+	                                                 aa_dL_dopacity, dL_dn);
 	PSB_LAUNCH_OK();
 	return 0;
 }

@@ -61,6 +61,32 @@ struct ScoreSink {
 constexpr int kScoreFracBits = 26;   // PSB_CONTRIB_SUM_FRAC_BITS
 constexpr float kScoreUnitsPerWeight = (float)(1u << kScoreFracBits);
 
+// What the forward tile pass renders beyond colour, final T and n_contrib (launch_render_forward); a null pointer leaves its plane out.
+// The set of planes picks the render_fwd_kernel<F> instantiation.
+struct FwdPlanes {
+	float* out_depth;       // [H,W] the expected depth D
+	float* out_alpha;       // [H,W] the accumulated opacity 1 - final_T
+	const float4* normals;  // [P] n_i of the pass (launch_normals); read with out_normal only
+	float* out_normal;      // [3,H,W] the normal plane
+	float* out_depth2;      // [H,W] the second depth moment sum z^2 alpha T; a depth variant, in which out_depth may be null
+	ScoreSink score;        // score.max != null: also add the contribution scores (colour only: no other plane)
+};
+
+// What the tile backward takes beyond dL/dpix (launch_render_backward); a null pointer leaves its plane out. The set of planes and the sink
+// pick the render_bwd_kernel<F, Sink> instantiation.
+struct BwdPlanes {
+	const float* dL_ddepth;   // [H,W] depth variant: dL/dz of every Gaussian lands in slot 11 of its packed sink row, or at sink.z
+	                          // (unpacked sink; refused without either destination)
+	const DetSlots* det;      // the deterministic variant: slot stores, then the ordered gather, which WRITES the sink rows
+	const float* dL_dalpha;   // [H,W] opacity variant: the gradient of the accumulated opacity 1 - final_T joins dL/dalpha of every splat
+	const float4* normals;    // [P] n_i of the forward pass; with dL_dnormal only
+	const float* dL_dnormal;  // [3,H,W] normal variant: packed 16-float sink rows and 64-byte deterministic slots, or with an unpacked sink
+	                          // (the operator) the GradSinkN variant, which sends dL/dn to dL_dn
+	const float* dL_ddepth2;  // [H,W] moment variant (a depth variant; dL_ddepth may be null): its dL/dz (slot 11 of a packed sink, sink.z
+	                          // of an unpacked one) includes 2 z dL/dM
+	float* dL_dn;             // [P,3] (unpacked sink with dL_dnormal) receives dL/dn
+};
+
 // Outputs of the per-Gaussian backward (any pointer may be null = not wanted).
 struct GaussGradOut {
 	float* dL_dmeans3D;  // [P,3]
@@ -111,14 +137,7 @@ int launch_det_base(int P, const GeomState& geom, uint32_t* base, cudaStream_t s
 int launch_scan_binning(int P, const Camera& cam, const GeomState& geom, BinState& bin, const ImgState& img, size_t capacity, bool tight,
                         uint32_t* ovf, uint32_t seq, cudaStream_t stream, uint32_t* base = nullptr);
 int launch_render_forward(const Camera& cam, const uint2* ranges, const uint32_t* point_list, const GaussRec* rec, const float* bg,
-                          float* out_color, float* final_T, uint32_t* n_contrib, cudaStream_t stream,
-                          float* out_depth = nullptr /* [H,W]: also render the expected depth (depth variant of the kernel) */,
-                          float* out_alpha = nullptr /* [H,W]: also write the accumulated opacity 1 - final_T (opacity variant) */,
-                          const ScoreSink* score = nullptr /* also add the contribution scores (score variant; no depth or opacity) */,
-                          const float4* normals = nullptr /* [P] n_i of the pass (launch_normals); with out_normal only */,
-                          float* out_normal = nullptr /* [3,H,W]: also render the normal plane (normal variant; no score) */,
-                          float* out_depth2 = nullptr /* [H,W]: also render the second depth moment sum z^2 alpha T (moment variant, which
-                                                         is a depth variant: out_depth may then be null; no score) */);
+                          float* out_color, float* final_T, uint32_t* n_contrib, const FwdPlanes& planes, cudaStream_t stream);
 // n_i of include/psb200.h (the camera-facing shortest axis in view space) of every visible row of the pass -> normals [P]; raw trainer
 // parameters (xyz, scaling, rotation), after launch_preprocess (tile_info says which rows are visible)
 int launch_normals(int P, const float* xyz, const float* scaling, const float* rotation, const Camera& cam, const uint4* tile_info, float4* normals,
@@ -126,19 +145,9 @@ int launch_normals(int P, const float* xyz, const float* scaling, const float* r
 // The same n_i from the operator's inputs: activated scales (the arg-min ignores the scale modifier) and the rotation as given, not
 // normalised (the operator's covariance does not normalise it either)
 int launch_op_normals(const GaussIn& in, const Camera& cam, const uint4* tile_info, float4* normals, cudaStream_t stream);
-// dL_ddepth [H,W]: depth variant, dL/dz of every Gaussian lands in slot 11 of its packed sink row, or at sink.z (unpacked sink;
-// refused without either destination). det != null: the deterministic variant — slot stores, then the ordered gather, which WRITES the
-// sink rows (packed: gather_slots_kernel; unpacked: gather_slots_unpacked_kernel, dL/dz at sink.z with dL_ddepth). dL_dalpha [H,W]: opacity variant, the gradient of the accumulated opacity 1 - final_T joins dL/dalpha of every splat
 int launch_render_backward(const Camera& cam, const uint2* ranges, const uint32_t* point_list, const GaussRec* rec, const float* bg,
-                           const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, const GradSink& sink,
-                           cudaStream_t stream, const float* dL_ddepth = nullptr, const DetSlots* det = nullptr, const float* dL_dalpha = nullptr,
-                           const float4* normals = nullptr /* [P] n_i of the forward pass; with dL_dnormal only */,
-                           const float* dL_dnormal = nullptr /* [3,H,W]: normal variant, packed 16-float sink rows, 64-byte deterministic slots */,
-                           const float* dL_ddepth2 = nullptr /* [H,W]: moment variant (a depth variant; dL_ddepth may be null); its dL/dz
-                                                                (slot 11 of a packed sink, sink.z of an unpacked one) includes 2 z dL/dM */,
-                           float* dL_dn = nullptr /* [P,3] (unpacked sink with dL_dnormal, operator path): receives dL/dn; the
-                                                     operator's normal variant (render_bwd_op_normal_kernel; deterministic: 64-byte
-                                                     slots and gather_slots_unpacked_normal_kernel) */);
+                           const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, const GradSink& sink, const BwdPlanes& planes,
+                           cudaStream_t stream);
 // dL_dz [P] (non-null: depth variant): dL/dmean3D += dL/dz (V[2], V[6], V[10]) for every visible Gaussian
 // aa_dL_dopacity [P] (non-null: AA variant, after an anti-aliased forward): holds dL/do' on entry, dL/do on return
 // dL_dn [P,3] (non-null: normal variant, scales + rotations only): dL/drot += the rotation gradient of n_i (launch_op_normals' n_i)

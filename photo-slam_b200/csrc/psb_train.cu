@@ -45,7 +45,7 @@ constexpr int MODE_PUSH = 2;   // NVLink data-parallel step: 80-byte gradient re
 constexpr int MODE_ADAM_LIVE = 3;  // MODE_ADAM with the caller's per-row live byte (psb_model.adam_live): rows that are neither live nor
                                    // reached by a gradient are not read beyond that byte and the visibility word
 constexpr int MODE_DEPTH = 8;      // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE / MODE_PUSH: slot 11 of the sink row holds dL/dz (view-space depth,
-                                   // render_bwd_kernel<true, ...>) and joins dL/dxyz through the view matrix's z row
+                                   // render_bwd_kernel<F | BWD_DEPTH, Sink>) and joins dL/dxyz through the view matrix's z row
 constexpr int MODE_AA = 16;        // OR'd into any of the above: the forward was anti-aliased (o' = o h, preprocess_fwd_kernel<true, true>), slot 7
                                    // holds dL/do'; dL/dh joins the covariance gradient and the opacity gradient is h dL/do' sigma'
 constexpr int MODE_REG = 32;       // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE (each optionally | MODE_DEPTH | MODE_AA), not MODE_PUSH: the opacity
@@ -55,7 +55,7 @@ constexpr int MODE_F3D = 64;       // OR'd into MODE_GRADS / MODE_ADAM / MODE_AD
                                    // the forward applied the 3D smoothing filter f3d[idx] (preprocess_fwd_kernel<true, AA, true>): the covariance is
                                    // rebuilt from s' = sqrt(s^2 + f^2), and the filter's opacity factor c joins the scale and opacity gradients
 constexpr int MODE_NORMAL = 128;   // OR'd into MODE_GRADS / MODE_ADAM / MODE_ADAM_LIVE (each optionally | MODE_DEPTH | MODE_AA | MODE_REG | MODE_F3D)
-                                   // and into MODE_PUSH (optionally | MODE_DEPTH | MODE_AA): the sink rows are 16 floats (render_bwd_normal_kernel) and
+                                   // and into MODE_PUSH (optionally | MODE_DEPTH | MODE_AA): the sink rows are 16 floats (render_bwd_kernel<F | BWD_NORMAL, Sink>) and
                                    // slots 12..14 hold dL/dn; the rotation gradient takes dL/dq of n = sign V r_k(q) (normal_axis_backward)
 
 // torch::optim::Adam single-tensor update (LibTorch adam.cpp): exp_avg.mul_(b1).add_(g, 1-b1);

@@ -33,12 +33,12 @@ struct PassMode {
 	int D;       // SH degree of the pass; -1: no psb_trainer_backward_pixels may follow it
 	bool det;    // deterministic mode
 	bool aa;     // the forward was anti-aliased (launch_preprocess aa): slot 7 of the sink rows holds dL/do'
-	bool depth;  // the sink rows carry dL/dz in slot 11 (render_bwd_kernel<true, ...>)
+	bool depth;  // the sink rows carry dL/dz in slot 11 (render_bwd_kernel<F | BWD_DEPTH, GradSink>)
 	float reg_opacity, reg_scale;  // psb_trainer_set_regularizers: lambda_opacity, lambda_scale (both 0: the variants without MODE_REG)
 	const float* f3d;              // psb_trainer_set_filter3d: the 3D smoothing filter [P] the pass applies, or null (the variants without it)
 	bool normals = false;          // the forward wrote n_i of its visible rows (launch_normals): a normal gradient may follow it
-	bool normal = false;           // the sink rows are 16 floats and slots 12..14 hold dL/dn (render_bwd_normal_kernel, MODE_NORMAL)
-	bool moment = false;           // the forward wrote the second depth moment M (render_fwd_moment_kernel): a dL/dM may follow it
+	bool normal = false;           // the sink rows are 16 floats and slots 12..14 hold dL/dn (render_bwd_kernel<F | BWD_NORMAL, GradSink>, MODE_NORMAL)
+	bool moment = false;           // the forward wrote the second depth moment M (render_fwd_kernel<F | FWD_MOMENT>): a dL/dM may follow it
 };
 // lambda / P of the opacity and scale regularisers for the rows a per-Gaussian backward updates; both 0 = no regulariser
 struct RegCoef {

@@ -106,14 +106,20 @@ struct psb_trainer {
 
 namespace {
 
+// The context's own plane pairs a pass's loss terms use: depth_buf, normal_buf, alpha_buf, moment_buf ([2][H*W] each, [6][H*W] for the
+// normal plane): the rendered plane, when the caller passes none, then its gradient.
+struct OwnPlanes {
+	bool depth, normal, alpha, moment;
+};
+
 // The scratch of a pass of P Gaussians over W x H pixels, each buffer's need stated once (CudaBuffer::grow drains the stream before it
 // frees a buffer the last call's kernels may still use). Any failure leaves t->carved cleared: no call reads this scratch until an
 // ensure() succeeds.
-// normal: a normal pass (n_i, 16-float sink rows and 64-byte deterministic slots); normal_loss: the built-in normal term's planes;
-// dn_loss: the opacity planes of the consistency and distortion terms; dist_loss: the distortion term's moment planes.
-int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_loss, bool normal = false, bool normal_loss = false,
-           bool dn_loss = false, bool dist_loss = false)
+// mode.normals: a normal pass (n_i, 16-float sink rows and 64-byte deterministic slots); own: the context's plane pairs the pass's loss
+// terms use.
+int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, const PassMode& mode, const OwnPlanes& own)
 {
+	const bool normal = mode.normals;
 	const size_t N = (size_t)W * H;
 	// the binning arena grows to P * 6 + 64 Ki instances when it is empty, or when it is smaller and the last pass was over another P
 	const size_t bin_need = t->bin.count() == 0 || t->carved.P != P ? (size_t)P * 6 + (1u << 16) : 0;
@@ -123,11 +129,11 @@ int ensure(psb_trainer* t, int P, int W, int H, cudaStream_t stream, bool depth_
 	PSB_CUDA_OK(t->image.grow(3 * N, Fit::at_least, false, stream));
 	PSB_CUDA_OK(t->dL_dpix.grow(3 * N, Fit::at_least, false, stream));
 	PSB_CUDA_OK(t->dmap.grow(9 * N, Fit::at_least, false, stream));
-	if (depth_loss) PSB_CUDA_OK(t->depth_buf.grow(2 * N, Fit::at_least, false, stream));
+	if (own.depth) PSB_CUDA_OK(t->depth_buf.grow(2 * N, Fit::at_least, false, stream));
 	if (normal) PSB_CUDA_OK(t->normals.grow((size_t)P, Fit::at_least, false, stream));
-	if (normal_loss) PSB_CUDA_OK(t->normal_buf.grow(6 * N, Fit::at_least, false, stream));
-	if (dn_loss) PSB_CUDA_OK(t->alpha_buf.grow(2 * N, Fit::at_least, false, stream));
-	if (dist_loss) PSB_CUDA_OK(t->moment_buf.grow(2 * N, Fit::at_least, false, stream));
+	if (own.normal) PSB_CUDA_OK(t->normal_buf.grow(6 * N, Fit::at_least, false, stream));
+	if (own.alpha) PSB_CUDA_OK(t->alpha_buf.grow(2 * N, Fit::at_least, false, stream));
+	if (own.moment) PSB_CUDA_OK(t->moment_buf.grow(2 * N, Fit::at_least, false, stream));
 	PSB_CUDA_OK(t->sink.grow((size_t)P * (normal ? 16 : 12), Fit::at_least, true, stream));
 	PSB_CUDA_OK(t->seeds.grow((size_t)P * 20, Fit::at_least, false, stream));
 	if (!t->readback) {
@@ -338,19 +344,23 @@ int refuse_filter3d(const psb_trainer* t, const char* fn)
 	return 0;
 }
 
-// Stage 1 of every pass: forward of SH degree D from raw parameters into t->image (or out_color); out_depth != NULL: the depth variant
-// also writes the expected depth there; out_alpha != NULL: the opacity variant also writes 1 - final_T there. The pass is recorded as
-// `mode`, with D = -1 until it has been binned. score != NULL: the score variant also adds the contribution scores there (no depth or
-// opacity plane). mode.normals: n_i of the visible rows -> t->normals, and the normal variant writes the normal plane to out_normal.
-// out_depth2 != NULL (mode.moment): the moment variant also writes the second depth moment there (out_depth may then be NULL).
+// Stage 1 of every pass: forward of SH degree D from raw parameters into t->image (or out_color), with the planes of `planes`
+// (launch_render_forward). Each plane in `own` is the caller's where `planes` gives one, else the first half of the context's own pair:
+// `planes` returns the planes the pass rendered. mode.normals: n_i of the visible rows -> t->normals (planes.normals). The pass is
+// recorded as `mode`, with D = -1 until it has been binned.
 int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, const psb_camera* camera, const float* background,
-                float* out_color, int* radii, Scratch& sc, Camera& cam, cudaStream_t stream, float* out_depth, float* out_alpha, const PassMode& mode,
-                const ScoreSink* score = nullptr, float* out_normal = nullptr, float* out_depth2 = nullptr)
+                float* out_color, int* radii, Scratch& sc, Camera& cam, cudaStream_t stream, FwdPlanes& planes, const PassMode& mode,
+                const OwnPlanes& own)
 {
 	int rc;
 	t->pass = mode;
 	t->pass.D = -1;
-	if ((rc = ensure(t, P, camera->width, camera->height, stream, mode.depth, mode.normals))) return rc;
+	if ((rc = ensure(t, P, camera->width, camera->height, stream, mode, own))) return rc;
+	if (own.depth && !planes.out_depth) planes.out_depth = t->depth_buf.get();
+	if (own.normal && !planes.out_normal) planes.out_normal = t->normal_buf.get();
+	if (own.alpha && !planes.out_alpha) planes.out_alpha = t->alpha_buf.get();
+	if (own.moment && !planes.out_depth2) planes.out_depth2 = t->moment_buf.get();
+	planes.normals = mode.normals ? t->normals.get() : nullptr;
 	cam = to_camera(camera);
 	sc = carve_scratch(t, P, camera->width, camera->height);
 	GeomState& geom = sc.geom;
@@ -372,17 +382,17 @@ int forward_raw(psb_trainer* t, int P, int M, int D, const psb_model* model, con
 	PSB_CUDA_OK(cudaMemcpyAsync(t->h_count.get() + 1, t->ovf.get(), 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
 	PSB_CUDA_OK(cudaEventRecord(t->readback, stream));
 	rc = launch_render_forward(cam, img.ranges, bin.inst[sorted_slot(cam.W, cam.H)], geom.rec, background, out_color ? out_color : t->image.get(), img.final_T,
-	                           img.n_contrib, stream, out_depth, out_alpha, score, mode.normals ? t->normals.get() : nullptr, out_normal, out_depth2);
+	                           img.n_contrib, planes, stream);
 	t->mark(4, stream);
 	return rc;
 }
 
 // Stage 3 of every pass: the tile backward of the context's last forward pass (scratch sc, camera cam, mode t->pass) on per-pixel
-// gradients -> the packed sink rows (dL_ddepth: also dL/dz in slot 11; dL_dalpha: the opacity variant; dL_dnormal: the normal variant,
-// 16-float rows with dL/dn in slots 12..14, after a pass with mode.normals; dL_ddepth2: the moment variant, its 2 z dL/dM in slot 11, after
-// a pass with mode.moment). P > 0.
-int tile_backward(psb_trainer* t, int P, const Scratch& sc, const Camera& cam, const float* background, const float* dL_dpix, const float* dL_ddepth,
-                  const float* dL_dalpha, cudaStream_t stream, const float* dL_dnormal = nullptr, const float* dL_ddepth2 = nullptr)
+// gradients -> the packed sink rows (planes.dL_ddepth: also dL/dz in slot 11; dL_dalpha: the opacity variant; dL_dnormal: the normal
+// variant, 16-float rows with dL/dn in slots 12..14, after a pass with mode.normals; dL_ddepth2: the moment variant, its 2 z dL/dM in slot
+// 11, after a pass with mode.moment). The deterministic slots and n_i are the context's. P > 0.
+int tile_backward(psb_trainer* t, int P, const Scratch& sc, const Camera& cam, const float* background, const float* dL_dpix, BwdPlanes planes,
+                  cudaStream_t stream)
 {
 	float* const rows = t->sink.get();
 	GradSink sink;
@@ -400,11 +410,12 @@ int tile_backward(psb_trainer* t, int P, const Scratch& sc, const Camera& cam, c
 	det.seq = t->seq;
 	det.P = P;
 	det.tight = t->tight ? 1 : 0;
+	planes.det = t->pass.det ? &det : nullptr;
+	planes.normals = planes.dL_dnormal ? t->normals.get() : nullptr;
 	// (the deterministic gather runs inside this call: stage "render bwd" covers it)
 	int rc;
 	if ((rc = launch_render_backward(cam, sc.img.ranges, sc.bin.inst[sorted_slot(cam.W, cam.H)], sc.geom.rec, background, sc.img.final_T, sc.img.n_contrib,
-	                                 dL_dpix, sink, stream, dL_ddepth, t->pass.det ? &det : nullptr, dL_dalpha, dL_dnormal ? t->normals.get() : nullptr,
-	                                 dL_dnormal, dL_ddepth2)))
+	                                 dL_dpix, sink, planes, stream)))
 		return rc;
 	t->mark(6, stream);
 	return 0;
@@ -423,7 +434,7 @@ struct TileBackward {
 int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                          const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
                          bool moments, cudaStream_t stream, TileBackward& out, const psb_exposure* exposure, float* exposure_grad,
-                         const psb_normal* normal = nullptr, const psb_dn* dn = nullptr, const psb_dist* dist = nullptr)
+                         const psb_normal* normal, const psb_dn* dn, const psb_dist* dist)
 {
 	int rc;
 	if (!t || !camera || !step || !background || !gt_image) { set_error_msg("psb_trainer_step: null argument"); return PSB_ERR_ARG; }
@@ -435,50 +446,35 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	const bool dn_loss = dn != nullptr;
 	// the distortion term reads D, A and M of this pass, adds into dL/dD and dL/dA and writes dL/dM: it forces those three planes
 	const bool dist_loss = dist && dist->lambda_dist > 0.f;
-	// depth loss: the depth plane is the caller's out_depth or the context's own; dL/dD lives in the context
 	const bool depth_loss = depth && depth->gt_depth;
 	const bool depth_pass = depth_loss || dn_loss || dist_loss;
-	float* depth_plane = depth ? depth->out_depth : nullptr;
-	float* dL_ddepth = nullptr;
-	if (depth_pass) {
-		if ((rc = ensure(t, P, camera->width, camera->height, stream, true))) return rc;
-		if (!depth_plane) depth_plane = t->depth_buf.get();
-		dL_ddepth = t->depth_buf.get() + npix;
-	}
-	// normal term: the plane is the caller's out_normal or the context's own; dL/dN lives in the context. An out_normal alone renders the
-	// plane and leaves the backward that of the step without it.
 	const bool normal_loss = normal && normal->gt_normal;
 	const bool normal_grad = normal_loss || dn_loss;
-	float* normal_plane = normal ? normal->out_normal : nullptr;
-	float* dL_dnormal = nullptr;
-	if (normal_grad) {
-		if ((rc = ensure(t, P, camera->width, camera->height, stream, depth_pass, true, true, dn_loss))) return rc;
-		if (!normal_plane) normal_plane = t->normal_buf.get();
-		dL_dnormal = t->normal_buf.get() + 3 * npix;
-	}
-	// distortion term: the moment plane is the caller's out_depth2 or the context's own; dL/dM lives in the context. An out_depth2 alone
-	// renders the plane and leaves the backward that of the step without it.
-	float* depth2_plane = dist ? dist->out_depth2 : nullptr;
-	float* dL_ddepth2 = nullptr;
-	if (dist_loss) {
-		if ((rc = ensure(t, P, camera->width, camera->height, stream, true, normal_grad, normal_grad, true, true))) return rc;
-		if (!depth2_plane) depth2_plane = t->moment_buf.get();
-		dL_ddepth2 = t->moment_buf.get() + npix;
-	}
-	float* alpha_plane = dn_loss || dist_loss ? t->alpha_buf.get() : nullptr;
-	float* dL_dalpha = dn_loss || dist_loss ? t->alpha_buf.get() + npix : nullptr;
+	// each term's plane is the caller's or the context's own (forward_raw), and its gradient lives in the context. An out_normal or
+	// out_depth2 alone renders the plane and leaves the backward that of the step without it.
+	const OwnPlanes own{depth_pass, normal_grad, dn_loss || dist_loss, dist_loss};
+	FwdPlanes planes{};
+	planes.out_depth = depth ? depth->out_depth : nullptr;
+	planes.out_normal = normal ? normal->out_normal : nullptr;
+	planes.out_depth2 = dist ? dist->out_depth2 : nullptr;
 	if (exposure) PSB_CUDA_OK(t->exp_partials.grow(kExposurePartials, Fit::at_least, false, stream));
 	Scratch sc;
 	Camera cam;
 	PassMode mode = pass_mode(t, -1, depth_pass);
-	mode.normals = normal_plane != nullptr;
+	mode.normals = planes.out_normal || own.normal;
 	mode.normal = normal_grad;
-	mode.moment = depth2_plane != nullptr;
+	mode.moment = planes.out_depth2 || own.moment;
 	// this pass gets its own tile backward below and its sink rows belong to this call's per-Gaussian stage (or to the _slab calls
 	// that follow a _begin): psb_trainer_backward_pixels must not add a second backward of it (D = -1)
-	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, sc, cam, stream, depth_plane, alpha_plane, mode,
-	                      nullptr, normal_plane, depth2_plane)))
-		return rc;
+	if ((rc = forward_raw(t, P, M, step->sh_degree, model, camera, background, out_color, radii, sc, cam, stream, planes, mode, own))) return rc;
+	float* const depth_plane = planes.out_depth;
+	float* const normal_plane = planes.out_normal;
+	float* const alpha_plane = planes.out_alpha;
+	float* const depth2_plane = planes.out_depth2;
+	float* const dL_ddepth = own.depth ? t->depth_buf.get() + npix : nullptr;
+	float* const dL_dnormal = own.normal ? t->normal_buf.get() + 3 * npix : nullptr;
+	float* const dL_dalpha = own.alpha ? t->alpha_buf.get() + npix : nullptr;
+	float* const dL_ddepth2 = own.moment ? t->moment_buf.get() + npix : nullptr;
 	const float* image = out_color ? out_color : t->image.get();
 	double* partials = t->deterministic ? t->det_partials.get() : nullptr;
 	if ((rc = launch_loss(cam.H, cam.W, image, gt_image, mask, step->lambda_dssim, t->dmap.get(), t->sums.get(), t->dL_dpix.get(), stream, partials,
@@ -532,7 +528,9 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 	}
 	t->mark(5, stream);
 	if (P == 0) return 0;
-	if ((rc = tile_backward(t, P, sc, cam, background, t->dL_dpix.get(), dL_ddepth, dL_dalpha, stream, dL_dnormal, dL_ddepth2))) return rc;
+	if ((rc = tile_backward(t, P, sc, cam, background, t->dL_dpix.get(), BwdPlanes{dL_ddepth, nullptr, dL_dalpha, nullptr, dL_dnormal, dL_ddepth2, nullptr},
+	                        stream)))
+		return rc;
 	out.geom = sc.geom;
 	out.cam = cam;
 	return 0;
@@ -746,8 +744,7 @@ int psb_trainer_destroy(psb_trainer* t)
 }
 
 static int forward_impl(const char* fn, psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
-                        int sh_degree, float* out_color, int* radii, float* out_depth, float* out_alpha, unsigned* pass, cudaStream_t stream,
-                        float* out_normal = nullptr, float* out_depth2 = nullptr)
+                        int sh_degree, float* out_color, int* radii, FwdPlanes planes, unsigned* pass, cudaStream_t stream)
 {
 	int rc;
 	if (!t || !camera || !background || !out_color) { set_error_msg(std::string(fn).append(": null argument").c_str()); return PSB_ERR_ARG; }
@@ -757,11 +754,9 @@ static int forward_impl(const char* fn, psb_trainer* t, int P, int M, const psb_
 	Camera cam;
 	t->have_loss = false;
 	PassMode mode = pass_mode(t, sh_degree, false);
-	mode.normals = out_normal != nullptr;
-	mode.moment = out_depth2 != nullptr;
-	if ((rc = forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, sc, cam, stream, out_depth, out_alpha, mode, nullptr,
-	                      out_normal, out_depth2)))
-		return rc;
+	mode.normals = planes.out_normal != nullptr;
+	mode.moment = planes.out_depth2 != nullptr;
+	if ((rc = forward_raw(t, P, M, sh_degree, model, camera, background, out_color, radii, sc, cam, stream, planes, mode, OwnPlanes{}))) return rc;
 	if (pass) *pass = t->seq;
 	return 0;
 }
@@ -770,7 +765,7 @@ int psb_trainer_forward_normal(psb_trainer* t, int P, int M, const psb_model* mo
                                float* out_color, int* radii, float* out_depth, float* out_alpha, float* out_normal, unsigned* pass, void* stream_)
 {
 	return forward_impl(out_normal ? "psb_trainer_forward_normal" : "psb_trainer_forward", t, P, M, model, camera, background, sh_degree, out_color, radii,
-	                    out_depth, out_alpha, pass, (cudaStream_t)stream_, out_normal);
+	                    FwdPlanes{out_depth, out_alpha, nullptr, out_normal, nullptr}, pass, (cudaStream_t)stream_);
 }
 
 int psb_trainer_forward_moment(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
@@ -778,29 +773,28 @@ int psb_trainer_forward_moment(psb_trainer* t, int P, int M, const psb_model* mo
                                void* stream_)
 {
 	const char* fn = out_depth2 ? "psb_trainer_forward_moment" : out_normal ? "psb_trainer_forward_normal" : "psb_trainer_forward";
-	return forward_impl(fn, t, P, M, model, camera, background, sh_degree, out_color, radii, out_depth, out_alpha, pass, (cudaStream_t)stream_, out_normal,
-	                    out_depth2);
+	return forward_impl(fn, t, P, M, model, camera, background, sh_degree, out_color, radii, FwdPlanes{out_depth, out_alpha, nullptr, out_normal, out_depth2},
+	                    pass, (cudaStream_t)stream_);
 }
 
 int psb_trainer_forward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
                         float* out_color, int* radii, float* out_depth, float* out_alpha, unsigned* pass, void* stream_)
 {
-	return forward_impl("psb_trainer_forward", t, P, M, model, camera, background, sh_degree, out_color, radii, out_depth, out_alpha, pass,
-	                    (cudaStream_t)stream_);
+	return forward_impl("psb_trainer_forward", t, P, M, model, camera, background, sh_degree, out_color, radii,
+	                    FwdPlanes{out_depth, out_alpha, nullptr, nullptr, nullptr}, pass, (cudaStream_t)stream_);
 }
 
 int psb_trainer_render(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
                        float* out_color, int* radii, void* stream_)
 {
-	return forward_impl("psb_trainer_render", t, P, M, model, camera, background, sh_degree, out_color, radii, nullptr, nullptr, nullptr,
-	                    (cudaStream_t)stream_);
+	return forward_impl("psb_trainer_render", t, P, M, model, camera, background, sh_degree, out_color, radii, FwdPlanes{}, nullptr, (cudaStream_t)stream_);
 }
 
 int psb_trainer_render_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
                              float* out_color, int* radii, float* out_depth, void* stream_)
 {
-	return forward_impl("psb_trainer_render_depth", t, P, M, model, camera, background, sh_degree, out_color, radii, out_depth, nullptr, nullptr,
-	                    (cudaStream_t)stream_);
+	return forward_impl("psb_trainer_render_depth", t, P, M, model, camera, background, sh_degree, out_color, radii,
+	                    FwdPlanes{out_depth, nullptr, nullptr, nullptr, nullptr}, nullptr, (cudaStream_t)stream_);
 }
 
 static_assert(kScoreFracBits == PSB_CONTRIB_SUM_FRAC_BITS, "the score kernel's fixed-point unit is the header's");
@@ -817,9 +811,10 @@ int psb_trainer_contribution(psb_trainer* t, int P, int M, const psb_model* mode
 	Scratch sc;
 	Camera cam;
 	t->have_loss = false;
-	const ScoreSink score{max_weight, reinterpret_cast<unsigned long long*>(sum_weight)};
-	return forward_raw(t, P, M, sh_degree, model, camera, background, out_color, nullptr, sc, cam, (cudaStream_t)stream_, nullptr, nullptr,
-	                   pass_mode(t, sh_degree, false), &score);
+	FwdPlanes planes{};
+	planes.score = {max_weight, reinterpret_cast<unsigned long long*>(sum_weight)};
+	return forward_raw(t, P, M, sh_degree, model, camera, background, out_color, nullptr, sc, cam, (cudaStream_t)stream_, planes,
+	                   pass_mode(t, sh_degree, false), OwnPlanes{});
 }
 
 int psb_trainer_backward_pixels(psb_trainer* t, unsigned pass, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
@@ -883,8 +878,8 @@ int psb_trainer_backward_pixels_moment(psb_trainer* t, unsigned pass, int P, int
 	// (a moment gradient leaves 2 z dL/dM in slot 11: the per-Gaussian stage consumes dL/dz)
 	t->pass.depth = pixel_grads->dL_ddepth != nullptr || dL_ddepth2 != nullptr;
 	t->pass.normal = dL_dnormal != nullptr;
-	if ((rc = tile_backward(t, P, sc, cam, background, pixel_grads->dL_dcolor, pixel_grads->dL_ddepth, pixel_grads->dL_dalpha, stream, dL_dnormal,
-	                        dL_ddepth2)))
+	if ((rc = tile_backward(t, P, sc, cam, background, pixel_grads->dL_dcolor,
+	                        BwdPlanes{pixel_grads->dL_ddepth, nullptr, pixel_grads->dL_dalpha, nullptr, dL_dnormal, dL_ddepth2, nullptr}, stream)))
 		return rc;
 	GradSegments gs{};
 	if (!adam)
