@@ -1,4 +1,5 @@
-"""Worker of tests/test_dp_terms_gpu.py (one process per GPU, launched with torch.distributed.run): K data-parallel steps through
+"""Worker of tests/test_dp_terms_gpu.py (one process per GPU, launched with torch.distributed.run; or K processes on one GPU, launched
+by tests/shared_device.py, p2p only): K data-parallel steps through
 DataParallelTrainer(mode=..., geometry_terms=True) on world ranks, rank r training with the terms TERMS[r % 4] (normal + consistency,
 distortion, none, all of depth, normal, consistency and distortion), then
   (1) every rank's parameter replica, and the Adam moments gathered from their owners, must be BIT-identical,
@@ -17,6 +18,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 
 import photo_slam_b200.synthetic as syn  # noqa: E402
+import shared_device  # noqa: E402
 from photo_slam_b200 import _lib, trainer  # noqa: E402
 
 LRS = [0.00032, 0.0025, 0.0025 / 20, 0.05, 0.005, 0.001]
@@ -64,10 +66,15 @@ def main():
     mode = sys.argv[1] if len(sys.argv) > 1 else "p2p"
     P = int(sys.argv[2]) if len(sys.argv) > 2 else 30_001
     steps = int(sys.argv[3]) if len(sys.argv) > 3 else 3
-    rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    torch.cuda.set_device(local)
-    dev = torch.device("cuda", local)
-    dist.init_process_group("nccl", device_id=dev)
+    shared = shared_device.init_rank()
+    if shared:      # every rank on device 0 (tests/shared_device.py): gloo, and the NVLink step only
+        assert mode == "p2p", "ranks sharing one device run the p2p step only: NCCL refuses two ranks on one device"
+        rank, world, dev = shared
+    else:
+        rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
+        torch.cuda.set_device(local)
+        dev = torch.device("cuda", local)
+        dist.init_process_group("nccl", device_id=dev)
     W, H, fx, fy = 320, 240, 260.0, 260.0
     sc = syn.make_scene(P, syn.make_camera(W, H, fx, fy), seed=11, scale_px=4.0)
     model = trainer.GaussianModel.from_numpy(sc, dev)

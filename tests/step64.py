@@ -222,16 +222,44 @@ def step64(state, cam, targets, flags, conv=STEP_CONV, stats=True):
     for i, k in enumerate(GROUPS):
         nxt["params"][k], nxt["m"][k], nxt["v"][k] = adam64(state["params"][k], r["grads"][k], state["m"][k], state["v"][k], state["lr"][i], t, conv)
     if stats:
-        vis = r["visible"]
-        nxt["denom"] = state["denom"] + vis.to(torch.float64)[:, None]
-        nxt["max_radii"] = torch.where(vis, torch.maximum(state["max_radii"], r["radii"].to(torch.float64)), state["max_radii"])
-        nxt["accum"] = state["accum"] + torch.where(vis, r["mean2D"].norm(dim=1), torch.zeros_like(vis, dtype=torch.float64))[:, None]
+        nxt.update(stats64(state, r))
     if state.get("E") is not None:
         te = state["E_step"] + 1
         nxt["E"], nxt["E_m"], nxt["E_v"] = adam64(state["E"], r["E"], state["E_m"], state["E_v"], state["E_lr"], te, conv)
         nxt["E_step"] = te
     r["state"] = nxt
     return r
+
+
+def stats64(state, r):
+    """the densification statistics after the pass r of grads64 -> dict(denom, max_radii, accum): the rows the pass draws count once,
+    keep the larger radius and add |dL/dmean2D|"""
+    vis = r["visible"]
+    return dict(denom=state["denom"] + vis.to(torch.float64)[:, None],
+                max_radii=torch.where(vis, torch.maximum(state["max_radii"], r["radii"].to(torch.float64)), state["max_radii"]),
+                accum=state["accum"] + torch.where(vis, r["mean2D"].norm(dim=1), torch.zeros_like(vis, dtype=torch.float64))[:, None])
+
+
+def dp_step64(state, views, world, dropped=(), conv=STEP_CONV, per_view=None, scale=None):
+    """One data-parallel optimizer step in float64: every rank r renders views[r] = (cam, targets, flags) of the same replica, and
+    g = (1 / world) sum_{r not in dropped} grads64(state, *views[r]) is applied by adam64 once. A dropped view (its binning arena
+    overflowed) adds nothing, and still counts in the 1 / world.
+    per_view: grads64 results of the views (None for a dropped one), computed once by a caller that also builds perturbed truths from
+    them; scale replaces 1 / world. -> dict(state = the next parameters and moments, grads = the g Adam took, views = the per-view results).
+    The densification statistics are each rank's own: stats64(state, views[r])."""
+    rs = per_view if per_view is not None else [None if i in dropped else grads64(state, *v, conv) for i, v in enumerate(views)]
+    s = 1.0 / world if scale is None else scale
+    t = state["step"] + 1
+    nxt = dict(state, params={}, m={}, v={}, step=t)
+    grads = {}
+    for i, k in enumerate(GROUPS):
+        g = torch.zeros_like(state["params"][k])
+        for j, r in enumerate(rs):
+            if j not in dropped:
+                g = g + r["grads"][k]
+        grads[k] = g * s
+        nxt["params"][k], nxt["m"][k], nxt["v"][k] = adam64(state["params"][k], grads[k], state["m"][k], state["v"][k], state["lr"][i], t, conv)
+    return dict(state=nxt, grads=grads, views=rs)
 
 
 # ---- margins ------------------------------------------------------------------------------------------------------------------------

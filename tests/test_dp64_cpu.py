@@ -161,3 +161,48 @@ def test_margins_report_the_consistency_decisions(world):
     pj = step64.margins(st, cam, dict(tg, dn_max_rel_jump=j), fl)["dn_jump"]
     hit = pj[1][pj[0] < 1e-9].tolist()
     assert int(last[yy, xx]) in hit and int(last[yy, xx + 1]) in hit
+
+
+# ---- dp_step64: the truth of the multi-rank step ------------------------------------------------------------------------------------
+def _same_update(a, b):
+    for part in ("params", "m", "v"):
+        for k in step64.GROUPS:
+            assert torch.equal(a[part][k], b[part][k]), (part, k)
+
+
+def test_dp_step_of_one_view_is_the_step(world):
+    """world 1, and world 2 with the same view on both ranks ((g + g) / 2 = g): the parameters and moments of step64, bit for bit"""
+    sc, cam, tg = world
+    fl = step64.Flags(normal=True, dn=True, dist=True)
+    ref = step64.step64(_state(sc), cam, tg, fl)["state"]
+    _same_update(step64.dp_step64(_state(sc), [(cam, tg, fl)], 1)["state"], ref)
+    _same_update(step64.dp_step64(_state(sc), [(cam, tg, fl)] * 2, 2)["state"], ref)
+
+
+def test_dp_step_is_the_mean_gradient_and_a_dropped_view_adds_nothing(world):
+    """two views with their own targets and terms: Adam takes (g_0 + g_1) / 2; with view 1 dropped g_0 / 2, and view 1 is not evaluated;
+    scale overrides 1 / world"""
+    sc, cam, tg = world
+    views = [(cam, tg, step64.Flags(depth=True)), (cam, _terms(_targets(seed=5)), step64.Flags(dist=True, aa=True))]
+    st = _state(sc)
+    g = [step64.grads64(st, *v)["grads"] for v in views]
+    both = step64.dp_step64(st, views, 2)
+    one = step64.dp_step64(st, [views[0], None], 2, dropped=(1,))
+    unscaled = step64.dp_step64(st, views, 2, per_view=both["views"], scale=1.0)
+    assert one["views"][1] is None
+    for i, k in enumerate(step64.GROUPS):
+        assert torch.equal(both["grads"][k], (g[0][k] + g[1][k]) * 0.5)
+        assert torch.equal(one["grads"][k], g[0][k] * 0.5)
+        assert torch.equal(unscaled["grads"][k], g[0][k] + g[1][k])
+        p, m, v = step64.adam64(st["params"][k], both["grads"][k], st["m"][k], st["v"][k], st["lr"][i], st["step"] + 1)
+        assert torch.equal(both["state"]["params"][k], p) and torch.equal(both["state"]["m"][k], m) and torch.equal(both["state"]["v"][k], v)
+    assert any(not torch.equal(g[0][k], g[1][k]) for k in step64.GROUPS)
+
+
+def test_stats64_is_the_step_statistics(world):
+    sc, cam, tg = world
+    fl = step64.Flags(depth=True)
+    st = _state(sc)
+    r = step64.step64(st, cam, tg, fl)
+    for k, t in step64.stats64(st, r).items():
+        assert torch.equal(t, r["state"][k]), k

@@ -1,5 +1,6 @@
-"""-m gpu: the NVLink data-parallel step (psb_dp_step) — single-GPU equivalence with the fused step, and (when the box has
->= 2 GPUs) K ranks over real peer memory: replicas bit-identical and equal to the 1-rank step on the summed gradients."""
+"""-m gpu: the NVLink data-parallel step (psb_dp_step) — single-GPU equivalence with the fused step, and K ranks over real peer memory
+(one per GPU when the box has >= 2, three processes sharing the GPU otherwise): replicas bit-identical and equal to the 1-rank step on
+the summed gradients."""
 import os
 import subprocess
 import sys
@@ -8,6 +9,7 @@ import pytest
 import torch
 
 import photo_slam_b200.synthetic as syn
+import shared_device
 from helpers import scene_tensors
 
 pytestmark = pytest.mark.gpu
@@ -60,9 +62,18 @@ def _launch(world, mode, P, steps=3, timeout=420):
 
 @pytest.mark.parametrize("mode", ["p2p", "nccl"])
 def test_multi_rank_replicas_identical_and_equal_summed_gradient_step(cuda, mode):
+    """One rank per GPU; on a single GPU, p2p runs three ranks sharing it (tests/shared_device.py)"""
     n = torch.cuda.device_count()
     if n < 2:
-        pytest.skip("needs >= 2 GPUs")
+        if mode != "p2p":
+            pytest.skip("NCCL needs one GPU per rank: >= 2 GPUs")
+        why = shared_device.unavailable()
+        if why:
+            pytest.skip(why)
+        codes, out, tails = shared_device.launch(os.path.join(ROOT, "tests", "dp_worker.py"), [mode, 30_001, 3], 3, timeout=600)
+        assert codes == [0, 0, 0] and "DP_WORKER_OK" in out, tails
+        print(out.strip().splitlines()[-1])
+        return
     world = 2 if n < 4 else (4 if n < 8 else 8)
     r = _launch(world, mode, 30_001)
     assert r.returncode == 0 and "DP_WORKER_OK" in r.stdout, (r.stdout[-3000:], r.stderr[-3000:])

@@ -1,7 +1,7 @@
 """-m gpu: the normal, depth-normal consistency and distortion terms on the data-parallel paths — the NVLink step (psb_dp_step_dist),
 the slab pipeline (psb_trainer_backward_begin_dist -> psb_trainer_backward_slab) and the flat split path (psb_trainer_backward_dist) —
-on a DataParallelTrainer(geometry_terms=True), against the fused step with the same terms on one GPU, and (when the box has >= 2 GPUs)
-ranks with different terms in one step against the 1-rank step on the summed gradients."""
+on a DataParallelTrainer(geometry_terms=True), against the fused step with the same terms on one GPU, and ranks with different terms in
+one step (one per GPU when the box has >= 2, four processes sharing the GPU otherwise) against the 1-rank step on the summed gradients."""
 import ctypes as C
 import os
 import subprocess
@@ -10,6 +10,7 @@ import sys
 import pytest
 import torch
 
+import shared_device
 from test_dist_gpu import _dist_planes32
 from test_dp_depth_gpu import LRS, SLABS, _assert_same_state, _finish, _inputs, _model, _render_target
 from test_normal_gpu import _grad_of_l1, _same, _settled, _state, _targets
@@ -329,10 +330,19 @@ def _launch(world, mode, P, steps=3, timeout=420):
 
 @pytest.mark.parametrize("mode", ["p2p", "nccl"])
 def test_multi_rank_mixed_terms_replicas_identical_and_equal_summed_gradient_step(cuda, mode):
-    """Ranks train with normal+dn, dist, no term and all terms in turn (mode="nccl" runs the slab pipeline at world > 1)."""
+    """Ranks train with normal+dn, dist, no term and all terms in turn (mode="nccl" runs the slab pipeline at world > 1). On a single GPU,
+    p2p runs four ranks sharing it (tests/shared_device.py), one for each set of terms."""
     n = torch.cuda.device_count()
     if n < 2:
-        pytest.skip("needs >= 2 GPUs")
+        if mode != "p2p":
+            pytest.skip("NCCL needs one GPU per rank: >= 2 GPUs")
+        why = shared_device.unavailable()
+        if why:
+            pytest.skip(why)
+        codes, out, tails = shared_device.launch(os.path.join(ROOT, "tests", "dp_terms_worker.py"), [mode, 30_001, 3], 4, timeout=600)
+        assert codes == [0] * 4 and "DP_TERMS_WORKER_OK" in out, tails
+        print(out.strip().splitlines()[-1])
+        return
     world = 2 if n < 4 else (4 if n < 8 else 8)
     r = _launch(world, mode, 30_001)
     assert r.returncode == 0 and "DP_TERMS_WORKER_OK" in r.stdout, (r.stdout[-3000:], r.stderr[-3000:])
