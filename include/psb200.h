@@ -426,7 +426,7 @@ int psb_trainer_backward_depth(psb_trainer* t, int P, int M, const psb_model* mo
  * raw render; psb_trainer_result reports the loss of X. Only the given row and its moments are read or written. The row's Adam step
  * uses step->beta1 / beta2 / eps, its own lr and its own step count, which the device advances (no host round trip). A pass that
  * overflows the binning arena leaves the row, its moments and its step count untouched (the repeated call then updates it once).
- * The data-parallel calls take no exposure; on the operator path a caller applies E in torch.
+ * The data-parallel calls take a replicated table instead (psb_exposure_table); on the operator path a caller applies E in torch.
  * ------------------------------------------------------------------------------------------------ */
 typedef struct psb_exposure {
 	float* param;       /* [3,4] device, the row E_k (gradient mode: read only) */
@@ -653,6 +653,27 @@ int psb_trainer_backward_begin_dist(psb_trainer* t, int P, int M, const psb_mode
                                     const float* background, const float* gt_image, const float* mask, const psb_step* step,
                                     float* out_color, int* radii, const psb_depth* depth, const psb_normal* normal, const psb_dn* dn,
                                     const psb_dist* dist, void* stream);
+/* Exposure on the slab and flat paths (the replicated table: see psb_exposure_table below). psb_trainer_backward_begin_table is
+ * psb_trainer_backward_begin_dist and psb_trainer_backward_table is psb_trainer_backward_dist without its single-row exposure, each plus
+ * the table (NULL: exactly the _dist call without exposure): this rank's view trains through row exposure->id, and its record (valid = 0
+ * without a row or for an overflowing pass) goes to exposure->record; the table does not move. After gathering every rank's record,
+ * psb_exposure_apply(world, records, table, step, 1/world) updates the table. PSB_ERR_ARG, before any CUDA call, for everything the
+ * _dist call rejects, the table values psb_dp_step_table rejects and a NULL record. */
+struct psb_exposure_table;
+int psb_trainer_backward_begin_table(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                                     const float* background, const float* gt_image, const float* mask, const psb_step* step,
+                                     float* out_color, int* radii, const psb_depth* depth, const psb_normal* normal, const psb_dn* dn,
+                                     const psb_dist* dist, const struct psb_exposure_table* exposure, void* stream);
+int psb_trainer_backward_table(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera,
+                               const float* background, const float* gt_image, const float* mask, const psb_step* step,
+                               float* out_color, int* radii, float* const* grads, const psb_depth* depth, const psb_normal* normal,
+                               const psb_dn* dn, const psb_dist* dist, const struct psb_exposure_table* exposure, void* stream);
+/* The table update of the data-parallel exposure rule from `world` records (device, rank-major [world][PSB_EXPOSURE_RECORD], as the
+ * gradient modes write them), with step->beta1 / beta2 / eps: one kernel, the one psb_dp_step_table runs. A record whose K or id does
+ * not fit the table is skipped. PSB_ERR_ARG, before any CUDA call, for a world outside 1..8, a NULL records, table or step, the table
+ * values psb_dp_step_table rejects and a non-finite grad_scale. Asynchronous. */
+int psb_exposure_apply(int world, const float* records, const struct psb_exposure_table* table, const psb_step* step, float grad_scale,
+                       void* stream);
 /* Same update on one flat range of n floats (any slice of a parameter tensor and the matching slices of its moments and
  * gradient) with an explicit learning rate: lets the caller pipeline chunked all-reduces with the optimizer. */
 int psb_adam_flat(size_t n, float* param, float* exp_avg, float* exp_avg_sq, const float* grad, float lr,
@@ -703,9 +724,47 @@ int psb_dp_step_dist(psb_trainer* t, psb_dp* dp, int P, int M, const psb_model* 
                      const float* background, const float* gt_image, const float* mask, const psb_step* step,
                      float* out_color, int* radii, const psb_depth* depth, const psb_normal* normal, const psb_dn* dn,
                      const psb_dist* dist, void* stream);
+/* ------------------------------------------------------------------------------------------------
+ * Exposure compensation on the data-parallel steps: every rank holds the same exposure table (K rows E_k, the layout of
+ * psb_exposure, their Adam moments and int32 step counts) and trains its view either without exposure (id = -1) or through row
+ * id with learning rate lr. Rank r's loss is exactly the one psb_trainer_step_exposure builds with row E_id; its Gaussian gradients
+ * travel as on the step without exposure. Then, for every id k that at least one rank with a valid record trained:
+ *   g_k = grad_scale * sum, in rank order, of dL_r/dE_k over those ranks (grad_scale = 1/world: a dropped view still counts in it);
+ *   row k takes one Adam step with step count step[k] + 1, step->beta1 / beta2 / eps and the lr of the lowest such rank; step[k]
+ *   advances by one, however many ranks trained k.
+ * Rows no valid record names keep their row, moments and step count bit for bit; a view that overflows its binning arena sends an
+ * invalid record (its row is untouched unless another rank trained it). Every rank applies the same records in the same order with
+ * the same kernel, so after the step every rank's table is bit-identical, in every mode. The table is never grown here: every rank
+ * must hold the same K (a record whose K differs from the local K, or whose id is outside [0, K), is skipped on the device and, on
+ * the NVLink step, sets psb_dp_status to 2).
+ * Exposure record (PSB_EXPOSURE_RECORD floats, device): id | lr | K | valid | the 12 sums dL/dE in the layout of E. On the NVLink step
+ *   it rides in each rank's meta row, beside the camera centre, with no extra flag or collective. The slab and flat paths write it to
+ *   table->record; the caller gathers the world records (rank-major, world * 16 floats: one all-gather) and calls psb_exposure_apply.
+ *   For the same per-rank gradients the three paths give bit-identical tables.
+ * ------------------------------------------------------------------------------------------------ */
+#define PSB_EXPOSURE_RECORD 16
+typedef struct psb_exposure_table {
+	float* param;       /* [K,3,4] device: row k = E_k */
+	float* exp_avg;     /* [K,3,4] device */
+	float* exp_avg_sq;  /* [K,3,4] device */
+	int*   step;        /* [K] device int32 step counts */
+	int    K;           /* >= 0, the same on every rank */
+	int    id;          /* the row this rank trains this step, or -1 for none */
+	float  lr;          /* this rank's learning rate: finite, >= 0 */
+	float* record;      /* [PSB_EXPOSURE_RECORD] device: the gradient modes' output (slab and flat paths); unused by psb_dp_step_table */
+} psb_exposure_table;
+/* psb_dp_step_dist plus this rank's exposure (exposure == NULL: exactly psb_dp_step_dist, and the table is not read). The record of this
+ * rank's view is published with its meta row; after the device-side wait for every rank's records, each rank updates its own table
+ * (one kernel, before the owner-side Adam). P = 0 exchanges nothing and leaves the table untouched. PSB_ERR_ARG, before any CUDA call,
+ * for everything psb_dp_step_dist rejects, an id outside [-1, K), K < 0, a NULL table array with K > 0, and a negative or non-finite lr. */
+int psb_dp_step_table(psb_trainer* t, psb_dp* dp, int P, int M, const psb_model* model, const psb_camera* camera,
+                      const float* background, const float* gt_image, const float* mask, const psb_step* step,
+                      float* out_color, int* radii, const psb_depth* depth, const psb_normal* normal, const psb_dn* dn,
+                      const psb_dist* dist, const psb_exposure_table* exposure, void* stream);
 /* Enqueues a device-side wait until every rank's rows of the last psb_dp_step have landed in this rank's tensors. */
 int psb_dp_sync(psb_dp* dp, void* stream);
-/* 0 = healthy, 1 = a cross-rank wait timed out (PSB_DP_TIMEOUT_MS, default 20 s). Synchronises the stream. */
+/* 0 = healthy, 1 = a cross-rank wait timed out (PSB_DP_TIMEOUT_MS, default 20 s), 2 = an exposure record was refused (a K or id that
+ * does not fit this rank's table). Synchronises the stream. */
 int psb_dp_status(psb_dp* dp, void* stream);
 int psb_dp_destroy(psb_dp* dp);
 

@@ -280,12 +280,32 @@ __global__ void __launch_bounds__(256) exposure_mix_kernel(int n, const float* _
 // as reduce_partials_kernel), so the gradient is the same every run. Then, unless the pass overflowed the binning arena
 // (counters[0] > capacity: the step is a no-op and is repeated, so the row must not move), either the Adam step of the row with its
 // own device step count (grad == null), or the gradient -> grad[12] (zeros for an overflowing pass, like the raw-parameter gradients).
+// rec.rec != null: the gradient goes to the data-parallel record instead (header id, lr, K, valid; valid = 0 for an overflowing pass).
+
+// One element of an exposure row's Adam step with step count t (the single-GPU update and exposure_apply_kernel share it).
+__device__ __forceinline__ void exposure_adam(float* __restrict__ param, float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq, int t, float g,
+                                              float lr, float beta1, float beta2, float eps)
+{
+	const double bc1 = 1.0 - pow((double)beta1, t), bc2 = 1.0 - pow((double)beta2, t);
+	float m = *exp_avg, v = *exp_avg_sq;
+	m = m * beta1 + (1.f - beta1) * g;
+	v = v * beta2 + (1.f - beta2) * g * g;
+	*exp_avg = m;
+	*exp_avg_sq = v;
+	const float denom = sqrtf(v) / (float)sqrt(bc2) + eps;
+	*param -= (float)(lr / bc1) * (m / denom);
+}
+
 __global__ void __launch_bounds__(256) exposure_update_kernel(int n, const double* __restrict__ partials, const uint32_t* __restrict__ counters,
-                                                              uint32_t capacity, ExposureUpdate u, float* __restrict__ grad)
+                                                              uint32_t capacity, ExposureUpdate u, float* __restrict__ grad, ExposureRecordOut rec)
 {
 	__shared__ double s[12][256];
 	const int tid = threadIdx.x;
 	const bool overflow = counters && counters[0] > capacity;   // (null: a pass without Gaussians, which cannot overflow)
+	if (rec.rec) {
+		grad = rec.rec + 4;
+		if (tid == 0) { rec.rec[0] = (float)rec.id; rec.rec[1] = rec.lr; rec.rec[2] = (float)rec.K; rec.rec[3] = overflow ? 0.f : 1.f; }
+	}
 	if (overflow && !grad) return;
 	double a[12];
 #pragma unroll
@@ -308,18 +328,45 @@ __global__ void __launch_bounds__(256) exposure_update_kernel(int n, const doubl
 	}
 	const int t = u.step[0] + 1;   // read by every thread before thread 0 stores it
 	__syncthreads();
-	if (tid < 12) {
-		const float g = (float)s[tid][0];
-		const double bc1 = 1.0 - pow((double)u.beta1, t), bc2 = 1.0 - pow((double)u.beta2, t);
-		float m = u.exp_avg[tid], v = u.exp_avg_sq[tid];
-		m = m * u.beta1 + (1.f - u.beta1) * g;
-		v = v * u.beta2 + (1.f - u.beta2) * g * g;
-		u.exp_avg[tid] = m;
-		u.exp_avg_sq[tid] = v;
-		const float denom = sqrtf(v) / (float)sqrt(bc2) + u.eps;
-		u.param[tid] -= (float)(u.lr / bc1) * (m / denom);
-	}
+	if (tid < 12) exposure_adam(u.param + tid, u.exp_avg + tid, u.exp_avg_sq + tid, t, (float)s[tid][0], u.lr, u.beta1, u.beta2, u.eps);
 	if (tid == 0) u.step[0] = t;
+}
+
+// The data-parallel exposure update (launch_exposure_apply): one block, thread 12 s + j handles element j of the row record s names,
+// when s leads its id (the lowest valid rank with that id). Every rank runs it on the same records, so every replica of the table ends
+// bit-identical.
+constexpr int EXP_APPLY_THREADS = 12 * DP_MAX_WORLD;
+__global__ void __launch_bounds__(EXP_APPLY_THREADS) exposure_apply_kernel(const float* __restrict__ recs, int stride, int world, ExposureTable tab,
+                                                                           float beta1, float beta2, float eps, float grad_scale,
+                                                                           uint32_t* __restrict__ status)
+{
+	__shared__ int s_id[DP_MAX_WORLD];   // the row record s updates, or -1 (not valid, or refused)
+	const int tid = threadIdx.x, s = tid / 12, j = tid - 12 * s;
+	if (tid < world) {
+		const float* r = recs + (size_t)tid * stride;
+		int id = -1;
+		if (r[3] != 0.f) {
+			const float k = r[0];
+			if (r[2] == (float)tab.K && k >= 0.f && k < (float)tab.K) id = (int)k;
+			else if (status) atomicCAS(status, 0u, 2u);
+		}
+		s_id[tid] = id;
+	}
+	__syncthreads();
+	const int k = s < world ? s_id[s] : -1;
+	bool lead = k >= 0;
+	for (int r = 0; r < s && lead; r++) lead = s_id[r] != k;
+	const int t = lead ? tab.step[k] + 1 : 0;   // read by the row's 12 threads before its thread 0 stores it
+	__syncthreads();
+	if (!lead) return;
+	const float* rs = recs + (size_t)s * stride;
+	float g = rs[4 + j];
+	for (int r = s + 1; r < world; r++)
+		if (s_id[r] == k) g += recs[(size_t)r * stride + 4 + j];
+	g *= grad_scale;
+	const size_t e = 12 * (size_t)k + j;
+	exposure_adam(tab.param + e, tab.exp_avg + e, tab.exp_avg_sq + e, t, g, rs[1], beta1, beta2, eps);
+	if (j == 0) tab.step[k] = t;
 }
 
 // Depth L1, pass 1 (grid-stride, 256 threads): per valid pixel |D - G| and sign(D - G) (-> dL_dD, scaled by pass 2); block sums of
@@ -649,7 +696,7 @@ int launch_loss(int H, int W, const float* img, const float* gt, const float* ma
 }
 
 int launch_exposure(int H, int W, const float* img, const float* E, float* dL_dpix, double* partials, const uint32_t* counters, uint32_t capacity,
-                    const ExposureUpdate* update, float* grad, cudaStream_t stream)
+                    const ExposureUpdate* update, float* grad, const ExposureRecordOut* record, cudaStream_t stream)
 {
 	const int n = H * W;
 	const int grid = exposure_blocks(H, W);
@@ -657,7 +704,18 @@ int launch_exposure(int H, int W, const float* img, const float* E, float* dL_dp
 	PSB_LAUNCH_OK();
 	ExposureUpdate u{};
 	if (update) u = *update;
-	exposure_update_kernel<<<1, 256, 0, stream>>>(grid, partials, counters, capacity, u, update ? nullptr : grad);
+	ExposureRecordOut rec{};
+	if (record && !update) rec = *record;
+	exposure_update_kernel<<<1, 256, 0, stream>>>(grid, partials, counters, capacity, u, update || rec.rec ? nullptr : grad, rec);
+	PSB_LAUNCH_OK();
+	return 0;
+}
+
+int launch_exposure_apply(const float* recs, int stride, int world, const ExposureTable& table, float beta1, float beta2, float eps, float grad_scale,
+                          uint32_t* status, cudaStream_t stream)
+{
+	if (world < 1 || world > DP_MAX_WORLD) { set_error_msg("launch_exposure_apply: world must lie in 1..8"); return -1; }
+	exposure_apply_kernel<<<1, EXP_APPLY_THREADS, 0, stream>>>(recs, stride, world, table, beta1, beta2, eps, grad_scale, status);
 	PSB_LAUNCH_OK();
 	return 0;
 }

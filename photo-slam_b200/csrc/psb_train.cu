@@ -683,7 +683,7 @@ __global__ void __launch_bounds__(TB) shard_adam_small_kernel(DpShard d, TrainTe
 			acc.sc[1] += r2.x; acc.sc[2] += r2.y; acc.rot.x += r2.z; acc.rot.y += r2.w;
 			acc.rot.z += r3.x; acc.rot.w += r3.y;
 			const float gm[3] = {r3.z, r3.w, tail[s].x};
-			const float* mt = d.meta + 8 * s;
+			const float* mt = d.meta + DP_META * s;
 			const int deg = (int)mt[3], ncoef = (deg + 1) * (deg + 1);
 			float w[16];
 			sh_basis(sh_dir(make_float3(pos.x - mt[0], pos.y - mt[1], pos.z - mt[2])), w);
@@ -769,10 +769,12 @@ __global__ void __launch_bounds__(256) shard_adam_frest_kernel(DpShard d, TrainT
 // raises this rank's epoch word on rank j. Stream order puts it after every store of the data kernel; the single system-scope fence
 // orders those stores (cumulativity) before the flag for an observer on another GPU. It replaces a fence in every block of the data
 // kernel because a system-scope fence per block costs microseconds while NVLink stores are in flight.
+// The meta row carries this rank's exposure record (written earlier on this stream by the exposure update), or valid = 0 without one.
 struct DpSignal {
 	uint32_t* flag[DP_MAX_WORLD];
 	float* meta[DP_MAX_WORLD];   // null: no meta row
 	const float* campos;
+	const float* exp_rec;        // [EXP_REC] local, or null
 	int world, rank, degree;
 	uint32_t epoch;
 };
@@ -780,8 +782,15 @@ __global__ void dp_signal_kernel(DpSignal s)
 {
 	const int j = threadIdx.x;
 	if (j < s.world && s.meta[j]) {
-		float* mt = s.meta[j] + 8 * s.rank;
+		float* mt = s.meta[j] + DP_META * s.rank;
 		mt[0] = s.campos[0]; mt[1] = s.campos[1]; mt[2] = s.campos[2]; mt[3] = (float)s.degree;
+		float* er = mt + DP_META_EXP;
+		if (s.exp_rec) {
+#pragma unroll
+			for (int q = 0; q < EXP_REC; q++) er[q] = s.exp_rec[q];
+		} else {
+			er[0] = -1.f; er[3] = 0.f;   // id -1, not valid
+		}
 	}
 	__threadfence_system();
 	__syncwarp();
@@ -867,14 +876,15 @@ int launch_gaussian_backward(int mode, int first, int P, const TrainTensors& t, 
 	return 0;
 }
 
-// dp_signal_kernel for `world` ranks: raises this rank's word in flag[j] of every rank j; with meta, first publishes campos and degree
+// dp_signal_kernel for `world` ranks: raises this rank's word in flag[j] of every rank j; with meta, first publishes campos, degree and
+// the exposure record exp_rec (null: none)
 int launch_signal(uint32_t* const* flag, float* const* meta, const float* campos, int degree, int world, int rank, uint32_t epoch,
-                  cudaStream_t stream)
+                  cudaStream_t stream, const float* exp_rec = nullptr)
 {
 	DpSignal s;
 	memset(&s, 0, sizeof(s));
 	for (int j = 0; j < world; j++) { s.flag[j] = flag[j]; s.meta[j] = meta ? meta[j] : nullptr; }
-	s.campos = campos; s.degree = degree; s.world = world; s.rank = rank; s.epoch = epoch;
+	s.campos = campos; s.exp_rec = exp_rec; s.degree = degree; s.world = world; s.rank = rank; s.epoch = epoch;
 	dp_signal_kernel<<<1, 32, 0, stream>>>(s);
 	PSB_LAUNCH_OK();
 	return 0;
@@ -929,7 +939,7 @@ int launch_adam_live_rebuild(int P, const TrainTensors& t, unsigned char* live, 
 
 int launch_push_backward(int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, const StepHyper& h,
                          const DensifyStats& st, const uint32_t* counters, uint32_t capacity, const DpPush& dp, cudaStream_t stream,
-                         const PassMode& mode)
+                         const PassMode& mode, const float* exp_rec)
 {
 	const GradSegments nog = {};
 	int rc;
@@ -937,7 +947,7 @@ int launch_push_backward(int P, const TrainTensors& t, const Camera& cam, const 
 	if ((rc = launch_gaussian_backward(MODE_PUSH | (mode.depth ? MODE_DEPTH : 0) | (mode.aa ? MODE_AA : 0) | (mode.normal ? MODE_NORMAL : 0), 0, P, t, cam, geom, sink, h, nog, st, counters, capacity, nullptr, dp,
 	                                   nullptr, stream, RegCoef{0.f, 0.f}, nullptr, MomentumList{})))
 		return rc;
-	return launch_signal(dp.grad_flag, dp.meta, cam.campos, h.D, dp.world, dp.rank, dp.epoch, stream);
+	return launch_signal(dp.grad_flag, dp.meta, cam.campos, h.D, dp.world, dp.rank, dp.epoch, stream, exp_rec);
 }
 
 int launch_shard_adam(const DpShard& d, const TrainTensors& t, const StepHyper& h, float grad_scale, cudaStream_t stream, cudaEvent_t between)

@@ -52,9 +52,15 @@ inline RegCoef reg_coef(const PassMode& m, int P) { return {P > 0 ? m.reg_opacit
 // CUDA IPC): the six parameter tensors, an inbox [world][nlocal_max][128][20 floats], per-rank meta rows and epoch flags.
 constexpr int DP_MAX_WORLD = 8;
 constexpr int DP_REC = 20;   // floats per gradient record: g_xyz 3 | g_dc 3 | g_opacity 1 | g_scaling 3 | g_rotation 4 | masked dL/dRGB 3 | pad 2 | epoch
+// The exposure record of one rank's step (psb_exposure_table): id | lr | K | valid | the 12 sums dL/dE (the layout of E). valid = 0: the
+// rank trained no exposure row, or its pass overflowed the binning arena; the record then counts for nothing.
+constexpr int EXP_REC = 16;
+// One meta row per rank and step: camera centre 3 | SH degree | the exposure record [4, 20) | unused [20, 32)
+constexpr int DP_META = 32;
+constexpr int DP_META_EXP = 4;
 struct DpPush {              // what the per-Gaussian backward needs to deliver its records
 	float* inbox[DP_MAX_WORLD];        // inbox base of every rank (own included), peer-mapped
-	float* meta[DP_MAX_WORLD];         // [world][8] floats on every rank: row r = camera centre + SH degree of rank r this step
+	float* meta[DP_MAX_WORLD];         // [world][DP_META] floats on every rank: row r = rank r's meta row of this step
 	uint32_t* grad_flag[DP_MAX_WORLD]; // [world] epoch words on every rank: word r = "rank r's records of this epoch have landed"
 	int world, rank, nlocal_max;
 	uint32_t epoch;
@@ -68,9 +74,11 @@ struct DpShard {             // what the owner-side Adam kernels need
 	int world, rank, nlocal_max, nlocal, P;   // nlocal: owned chunks of this rank
 	uint32_t epoch;
 };
+// exp_rec: this rank's exposure record of this step (local, EXP_REC floats), published in its meta row with the camera centre; null: the
+// meta row says valid = 0
 int launch_push_backward(int P, const TrainTensors& t, const Camera& cam, const GeomState& geom, float* sink, const StepHyper& h,
                          const DensifyStats& st, const uint32_t* counters, uint32_t capacity, const DpPush& dp, cudaStream_t stream,
-                         const PassMode& mode);
+                         const PassMode& mode, const float* exp_rec);
 int launch_shard_adam(const DpShard& d, const TrainTensors& t, const StepHyper& h, float grad_scale, cudaStream_t stream, cudaEvent_t between = nullptr);
 // spins (device side) until flags[0..world) >= epoch (world <= 32 words); after `timeout_ms` writes 1 to *status and gives up
 int launch_wait_flags(const uint32_t* flags, int world, uint32_t epoch, uint32_t* status, cudaStream_t stream);
@@ -107,8 +115,30 @@ struct ExposureUpdate {
 // After launch_loss with E: dL_dpix (g) -> dL/dI in place, and the 12 sums dL/dE added in a fixed order (no atomics: the same every run).
 // update != null: the Adam step of the row; else grad [12] device receives dL/dE. An overflowing pass (counters[0] > capacity) leaves
 // the row, its moments and its step count untouched (grad: zeros). partials: exposure_blocks(H, W) * 12 doubles. Two launches.
+// record != null (the data-parallel steps): the gradient mode writes the EXP_REC-float record instead of grad: id, lr and K as given,
+// valid = 0 for an overflowing pass (sums zero), else 1 and the 12 sums.
+struct ExposureRecordOut {
+	float* rec;   // [EXP_REC] device
+	int id, K;
+	float lr;
+};
 int launch_exposure(int H, int W, const float* img, const float* E, float* dL_dpix, double* partials, const uint32_t* counters, uint32_t capacity,
-                    const ExposureUpdate* update, float* grad, cudaStream_t stream);
+                    const ExposureUpdate* update, float* grad, const ExposureRecordOut* record, cudaStream_t stream);
+// A replicated exposure table [K][3][4] (+ moments, int32 step counts [K]) on one rank.
+struct ExposureTable {
+	float* param;
+	float* exp_avg;
+	float* exp_avg_sq;
+	int* step;
+	int K;
+};
+// One block: the world exposure records recs[r * stride .. + EXP_REC) (rank order) -> the table. For every id k of at least one valid
+// record: g = grad_scale * the sum, in rank order, of the valid records' sums with that id; row k takes one Adam step (step count
+// step[k] + 1, the lr of the lowest such rank, the betas and eps given), exactly the arithmetic of the single-GPU step's exposure update.
+// Rows no valid record names are not touched. A valid record whose K differs from table.K or whose id is outside [0, K) is skipped and
+// sets *status to 2 if it was 0 (status may be null).
+int launch_exposure_apply(const float* recs, int stride, int world, const ExposureTable& table, float beta1, float beta2, float eps, float grad_scale,
+                          uint32_t* status, cudaStream_t stream);
 inline int exposure_blocks(int H, int W) { return min(cdiv(H * W, 256), kNumSMs * 8); }
 constexpr size_t kExposurePartials = 12 * (size_t)kNumSMs * 8;   // doubles: enough for any image
 // Depth L1 over the valid pixels (gt > 0 and, with a mask, mask[0, p] != 0): sums[0] = sum |D - G|, sums[1] = N_valid (zeroed here);

@@ -304,6 +304,52 @@ int check_exposure(const psb_exposure* e, bool adam, const float* grad, const ch
 	return 0;
 }
 
+// NULL: no table. Otherwise K >= 0, id in [-1, K), a finite lr >= 0, the row, moment and step arrays when K > 0 and, for the gradient
+// modes (`record`), a record output.
+int check_table(const psb_exposure_table* e, bool record, const char* fn)
+{
+	if (!e) return 0;
+	if (e->K < 0 || e->id < -1 || e->id >= e->K) {
+		set_error_msg(std::string(fn).append(": exposure id must be -1 or lie in [0, K), and K >= 0").c_str());
+		return PSB_ERR_ARG;
+	}
+	if (e->K > 0 && (!e->param || !e->exp_avg || !e->exp_avg_sq || !e->step)) {
+		set_error_msg(std::string(fn).append(": the exposure table needs param, exp_avg, exp_avg_sq and step").c_str());
+		return PSB_ERR_ARG;
+	}
+	if (!std::isfinite(e->lr) || e->lr < 0.f) {
+		set_error_msg(std::string(fn).append(": exposure lr must be finite and >= 0").c_str());
+		return PSB_ERR_ARG;
+	}
+	if (record && !e->record) {
+		set_error_msg(std::string(fn).append(": the exposure table needs a record output on this path").c_str());
+		return PSB_ERR_ARG;
+	}
+	return 0;
+}
+
+// The row a table trains this step, as a gradient-mode psb_exposure (param only), and where its record goes.
+struct TableRow {
+	psb_exposure row;
+	ExposureRecordOut rec;
+	bool any;   // the rank trains a row (id >= 0)
+};
+TableRow table_row(const psb_exposure_table* e, float* rec)
+{
+	TableRow r{};
+	if (!e || e->id < 0) return r;
+	r.row.param = e->param + 12 * (size_t)e->id;
+	r.row.lr = e->lr;
+	r.rec = {rec, e->id, e->K, e->lr};
+	r.any = true;
+	return r;
+}
+
+ExposureTable exposure_table(const psb_exposure_table* e)
+{
+	return {e->param, e->exp_avg, e->exp_avg_sq, e->step, e->K};
+}
+
 // Gradient segments of P rows: six non-null pointers, features_rest and rotation 16-byte aligned (written with float4 stores).
 int check_grads(float* const* grads, int P, const char* fn)
 {
@@ -430,11 +476,12 @@ struct TileBackward {
 
 // The built-in loss around the shared stages: forward -> loss (+ depth loss) -> pinned read-back of the loss sums -> (exposure) -> tile
 // backward. `moments`: the caller's per-Gaussian stage updates the Adam moments of the model. exposure != NULL: the loss is that of the
-// image through the row; exposure_grad == NULL: the row takes its Adam step (with step's betas and eps), else dL/dE -> exposure_grad.
+// image through the row; exposure_grad == NULL: the row takes its Adam step (with step's betas and eps), else dL/dE -> exposure_grad;
+// exposure_record != NULL: dL/dE goes to that data-parallel record instead (the row does not move).
 int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                          const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
                          bool moments, cudaStream_t stream, TileBackward& out, const psb_exposure* exposure, float* exposure_grad,
-                         const psb_normal* normal, const psb_dn* dn, const psb_dist* dist)
+                         const psb_normal* normal, const psb_dn* dn, const psb_dist* dist, const ExposureRecordOut* exposure_record = nullptr)
 {
 	int rc;
 	if (!t || !camera || !step || !background || !gt_image) { set_error_msg("psb_trainer_step: null argument"); return PSB_ERR_ARG; }
@@ -523,7 +570,7 @@ int render_loss_backward(psb_trainer* t, int P, int M, const psb_model* model, c
 		// dL/dI for the tile backward and the row's update (or gradient), inside stage "loss"; the row moves only after every read of it
 		ExposureUpdate u{exposure->param, exposure->exp_avg, exposure->exp_avg_sq, exposure->step, exposure->lr, step->beta1, step->beta2, step->eps};
 		if ((rc = launch_exposure(cam.H, cam.W, image, exposure->param, t->dL_dpix.get(), t->exp_partials.get(), P > 0 ? sc.geom.counters : nullptr,
-		                          (uint32_t)t->bin.count(), exposure_grad ? nullptr : &u, exposure_grad, stream)))
+		                          (uint32_t)t->bin.count(), exposure_grad || exposure_record ? nullptr : &u, exposure_grad, exposure_record, stream)))
 			return rc;
 	}
 	t->mark(5, stream);
@@ -548,7 +595,8 @@ struct psb_dp {
 	char* peer[DP_MAX_WORLD] = {};              // arena of every rank in this process' address space (peer[rank] == base)
 	size_t off_param[6] = {}, off_inbox = 0, off_meta = 0, off_gflag = 0, off_pflag = 0, bytes = 0;
 	CudaBuffer<float> g_rest;                   // local scratch
-	CudaBuffer<uint32_t> status;                // local word: 1 = a cross-rank wait timed out
+	CudaBuffer<uint32_t> status;                // local word: 1 = a cross-rank wait timed out, 2 = an exposure record was refused
+	CudaBuffer<float> exp_rec;                  // local [EXP_REC]: this rank's exposure record of the step, published in its meta row
 	uint32_t epoch = 0;
 	bool connected = false;
 	cudaIpcMemHandle_t handle;
@@ -560,7 +608,7 @@ void dp_layout(psb_dp* d)
 	size_t o = 0;
 	for (int i = 0; i < 6; i++) { d->off_param[i] = o; o = align_up(o + (size_t)d->P * row_floats(i) * sizeof(float), 256); }
 	d->off_inbox = o; o = align_up(o + (size_t)d->world * d->nlocal_max * 128 * DP_REC * sizeof(float), 256);
-	d->off_meta = o; o += 256;
+	d->off_meta = o; o += DP_MAX_WORLD * DP_META * sizeof(float);
 	d->off_gflag = o; o += 256;
 	d->off_pflag = o; o += 256;
 	d->bytes = o;
@@ -582,6 +630,7 @@ int psb_dp_create(psb_dp** out, int rank, int world, int P)
 	cudaError_t e = d->base.grow(d->bytes, Fit::exact, true, nullptr);
 	if (e == cudaSuccess) e = d->g_rest.grow((size_t)d->nlocal_max * 128 * kRestFloats + 64, Fit::exact, false, nullptr);
 	if (e == cudaSuccess) e = d->status.grow(1, Fit::exact, true, nullptr);
+	if (e == cudaSuccess) e = d->exp_rec.grow(EXP_REC, Fit::exact, true, nullptr);
 	if (e == cudaSuccess && world > 1) e = cudaIpcGetMemHandle(&d->handle, d->base.get());
 	if (e != cudaSuccess) {
 		set_error("psb_dp_create", e, __FILE__, __LINE__);
@@ -665,13 +714,21 @@ int psb_dp_step_dist(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* m
                      const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
                      const psb_normal* normal, const psb_dn* dn, const psb_dist* dist, void* stream_)
 {
+	return psb_dp_step_table(t, d, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, normal, dn, dist, nullptr, stream_);
+}
+
+int psb_dp_step_table(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                      const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, const psb_depth* depth,
+                      const psb_normal* normal, const psb_dn* dn, const psb_dist* dist, const psb_exposure_table* exposure, void* stream_)
+{
 	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
-	const char* fn = normal || dn || dist ? "psb_dp_step_dist" : "psb_dp_step_depth";
+	const char* fn = exposure ? "psb_dp_step_table" : normal || dn || dist ? "psb_dp_step_dist" : "psb_dp_step_depth";
 	if ((rc = check_depth(depth, fn))) return rc;
 	if ((rc = check_normal(normal, fn))) return rc;
 	if ((rc = check_dn(dn, fn))) return rc;
 	if ((rc = check_dist(dist, fn))) return rc;
+	if ((rc = check_table(exposure, false, fn))) return rc;
 	if ((rc = refuse_filter3d(t, fn))) return rc;
 	if (!d || !d->connected || P != d->P || !model) { set_error_msg("psb_dp_step: context not connected or built for a different P"); return PSB_ERR_ARG; }
 	if ((rc = check_model(P, M, model, true))) return rc;
@@ -688,9 +745,12 @@ int psb_dp_step_dist(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* m
 	// render, loss, tile backward (the 9 screen-space sums per Gaussian; with a depth, consistency or distortion term also dL/dz in slot 11,
 	// with a normal or consistency term 16-float rows with dL/dn in slots 12..14: the push backward below runs the variant t->pass names and
 	// consumes them, where a plain one would leave them in the sink for the next step)
+	// with a row: its 12 sums dL/dE and the valid flag go to the local record, which the signal behind the push backward publishes in this
+	// rank's meta row (every rank's row updates only after every rank's records have landed, in exposure_apply_kernel below)
+	const TableRow tr = table_row(exposure, d->exp_rec.get());
 	TileBackward tb;
-	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, stream, tb, nullptr,
-	                               nullptr, normal, dn, dist)) ||
+	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, stream, tb,
+	                               tr.any ? &tr.row : nullptr, nullptr, normal, dn, dist, tr.any ? &tr.rec : nullptr)) ||
 	    P == 0)
 		return rc;
 	const TrainTensors tt = train_tensors(model, true);
@@ -714,11 +774,18 @@ int psb_dp_step_dist(psb_trainer* t, psb_dp* d, int P, int M, const psb_model* m
 	// push backward (records go straight into the owners' inboxes) + signal; wait until every rank's records have landed -> Adam of
 	// the owned rows, updated rows stored to every replica + signal
 	if ((rc = launch_push_backward(P, tt, tb.cam, tb.geom, t->sink.get(), h, densify_stats(model, step), tb.geom.counters, (uint32_t)t->bin.count(), push, stream,
-	                               t->pass)))
+	                               t->pass, tr.any ? d->exp_rec.get() : nullptr)))
 		return rc;
 	t->mark(7, stream);
 	t->mark(8, stream);
 	if ((rc = launch_wait_flags(reinterpret_cast<const uint32_t*>(d->base.get() + d->off_gflag), d->world, epoch, d->status.get(), stream))) return rc;
+	// every rank's meta row of this step has landed: each rank applies the same exposure records to its own copy of the table. It runs
+	// before the shard Adam's "rows landed" signal, and a peer writes its next step's meta row only after it has seen that signal (the
+	// wait at the top of its next step), so no meta row is overwritten while this kernel reads it.
+	if (exposure &&
+	    (rc = launch_exposure_apply(reinterpret_cast<const float*>(d->base.get() + d->off_meta) + DP_META_EXP, DP_META, d->world, exposure_table(exposure),
+	                                step->beta1, step->beta2, step->eps, 1.0f / (float)d->world, d->status.get(), stream)))
+		return rc;
 	if ((rc = launch_shard_adam(sh, tt, h, 1.0f / (float)d->world, stream, t->event(10)))) return rc;
 	t->end_stages(9, stream);
 	return 0;
@@ -797,6 +864,7 @@ int psb_trainer_render_depth(psb_trainer* t, int P, int M, const psb_model* mode
 	                    FwdPlanes{out_depth, nullptr, nullptr, nullptr, nullptr}, nullptr, (cudaStream_t)stream_);
 }
 
+static_assert(EXP_REC == PSB_EXPOSURE_RECORD, "the exposure record of the kernels is the header's");
 static_assert(kScoreFracBits == PSB_CONTRIB_SUM_FRAC_BITS, "the score kernel's fixed-point unit is the header's");
 
 int psb_trainer_contribution(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, int sh_degree,
@@ -957,6 +1025,34 @@ int psb_adam_live_rebuild(int P, const psb_model* model, void* stream_)
 	return launch_adam_live_rebuild(P, train_tensors(model, true), model->adam_live, (cudaStream_t)stream_);
 }
 
+// The gradient-mode built-in step behind psb_trainer_backward_dist and psb_trainer_backward_table, its arguments checked: the raw-parameter
+// gradients -> grads, dL/dE -> exposure_grad or the record.
+static int backward_flat(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background, const float* gt_image,
+                         const float* mask, const psb_step* step, float* out_color, int* radii, float* const* grads, const psb_depth* depth,
+                         const psb_exposure* exposure, float* exposure_grad, const psb_normal* normal, const psb_dn* dn, const psb_dist* dist,
+                         const ExposureRecordOut* record, cudaStream_t stream)
+{
+	int rc;
+	TileBackward tb;
+	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, stream, tb, exposure,
+	                               exposure_grad, normal, dn, dist, record)) ||
+	    P == 0)
+		return rc;
+	GradSegments gs;
+	for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
+	rc = launch_fused_backward(false, 0, P, train_tensors(model, false), tb.cam, tb.geom, t->sink.get(), t->seeds.get(), to_hyper(step), gs, densify_stats(model, step),
+	                           tb.geom.counters, (uint32_t)t->bin.count(), stream, t->event(7), nullptr, t->pass, reg_coef(t->pass, P));
+	t->end_stages(8, stream);
+	return rc;
+}
+
+// A table whose rank trains no row this step still writes its record, with valid = 0 (all zeros), for the hosts' gather.
+static int clear_record(const psb_exposure_table* e, const TableRow& tr, cudaStream_t stream)
+{
+	if (e && !tr.any) PSB_CUDA_OK(cudaMemsetAsync(e->record, 0, EXP_REC * sizeof(float), stream));
+	return 0;
+}
+
 int psb_trainer_backward_depth(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
                                const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, float* const* grads,
                                const psb_depth* depth, void* stream_)
@@ -978,7 +1074,6 @@ int psb_trainer_backward_dist(psb_trainer* t, int P, int M, const psb_model* mod
                               const psb_depth* depth, const psb_exposure* exposure, float* exposure_grad, const psb_normal* normal, const psb_dn* dn,
                               const psb_dist* dist, void* stream_)
 {
-	cudaStream_t stream = (cudaStream_t)stream_;
 	int rc;
 	const bool terms = normal || dn || dist;
 	if ((rc = check_depth(depth, terms ? "psb_trainer_backward_dist" : exposure ? "psb_trainer_backward_exposure" : "psb_trainer_backward_depth"))) return rc;
@@ -987,17 +1082,28 @@ int psb_trainer_backward_dist(psb_trainer* t, int P, int M, const psb_model* mod
 	if ((rc = check_dn(dn, "psb_trainer_backward_dist"))) return rc;
 	if ((rc = check_dist(dist, "psb_trainer_backward_dist"))) return rc;
 	if ((rc = check_grads(grads, P, terms ? "psb_trainer_backward_dist" : "psb_trainer_backward"))) return rc;
-	TileBackward tb;
-	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, stream, tb, exposure,
-	                               exposure ? exposure_grad : nullptr, normal, dn, dist)) ||
-	    P == 0)
+	return backward_flat(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, grads, depth, exposure, exposure ? exposure_grad : nullptr,
+	                     normal, dn, dist, nullptr, (cudaStream_t)stream_);
+}
+
+int psb_trainer_backward_table(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                               const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii, float* const* grads,
+                               const psb_depth* depth, const psb_normal* normal, const psb_dn* dn, const psb_dist* dist,
+                               const psb_exposure_table* exposure, void* stream_)
+{
+	int rc;
+	const char* fn = "psb_trainer_backward_table";
+	if ((rc = check_depth(depth, fn))) return rc;
+	if ((rc = check_normal(normal, fn))) return rc;
+	if ((rc = check_dn(dn, fn))) return rc;
+	if ((rc = check_dist(dist, fn))) return rc;
+	if ((rc = check_table(exposure, true, fn))) return rc;
+	if ((rc = check_grads(grads, P, fn))) return rc;
+	const TableRow tr = table_row(exposure, exposure ? exposure->record : nullptr);
+	if ((rc = backward_flat(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, grads, depth, tr.any ? &tr.row : nullptr, nullptr,
+	                        normal, dn, dist, tr.any ? &tr.rec : nullptr, (cudaStream_t)stream_)))
 		return rc;
-	GradSegments gs;
-	for (int i = 0; i < 6; i++) gs.g[i] = grads[i];
-	rc = launch_fused_backward(false, 0, P, train_tensors(model, false), tb.cam, tb.geom, t->sink.get(), t->seeds.get(), to_hyper(step), gs, densify_stats(model, step),
-	                           tb.geom.counters, (uint32_t)t->bin.count(), stream, t->event(7), nullptr, t->pass, reg_coef(t->pass, P));
-	t->end_stages(8, stream);
-	return rc;
+	return clear_record(exposure, tr, (cudaStream_t)stream_);
 }
 
 int psb_trainer_backward(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
@@ -1019,12 +1125,22 @@ int psb_trainer_backward_begin_dist(psb_trainer* t, int P, int M, const psb_mode
                                     const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii,
                                     const psb_depth* depth, const psb_normal* normal, const psb_dn* dn, const psb_dist* dist, void* stream_)
 {
+	return psb_trainer_backward_begin_table(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, normal, dn, dist, nullptr,
+	                                        stream_);
+}
+
+int psb_trainer_backward_begin_table(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,
+                                     const float* gt_image, const float* mask, const psb_step* step, float* out_color, int* radii,
+                                     const psb_depth* depth, const psb_normal* normal, const psb_dn* dn, const psb_dist* dist,
+                                     const psb_exposure_table* exposure, void* stream_)
+{
 	int rc;
-	const char* fn = normal || dn || dist ? "psb_trainer_backward_begin_dist" : "psb_trainer_backward_begin_depth";
+	const char* fn = exposure ? "psb_trainer_backward_begin_table" : normal || dn || dist ? "psb_trainer_backward_begin_dist" : "psb_trainer_backward_begin_depth";
 	if ((rc = check_depth(depth, fn))) return rc;
 	if ((rc = check_normal(normal, fn))) return rc;
 	if ((rc = check_dn(dn, fn))) return rc;
 	if ((rc = check_dist(dist, fn))) return rc;
+	if ((rc = check_table(exposure, true, fn))) return rc;
 	if ((rc = refuse_filter3d(t, fn))) return rc;
 	// recorded whether or not the call below succeeds (render_loss_backward records the same rows again): dL/dz in slot 11 with a depth,
 	// consistency or distortion term, 16-float rows with dL/dn with a normal or consistency term. The variants that read them give the
@@ -1033,9 +1149,25 @@ int psb_trainer_backward_begin_dist(psb_trainer* t, int P, int M, const psb_mode
 		t->pass = pass_mode(t, -1, (depth && depth->gt_depth) || dn || (dist && dist->lambda_dist > 0.f));
 		t->pass.normal = (normal && normal->gt_normal) || dn;
 	}
+	const TableRow tr = table_row(exposure, exposure ? exposure->record : nullptr);
 	TileBackward tb;
-	return render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, (cudaStream_t)stream_, tb,
-	                            nullptr, nullptr, normal, dn, dist);
+	if ((rc = render_loss_backward(t, P, M, model, camera, background, gt_image, mask, step, out_color, radii, depth, false, (cudaStream_t)stream_, tb,
+	                               tr.any ? &tr.row : nullptr, nullptr, normal, dn, dist, tr.any ? &tr.rec : nullptr)))
+		return rc;
+	return clear_record(exposure, tr, (cudaStream_t)stream_);
+}
+
+int psb_exposure_apply(int world, const float* records, const psb_exposure_table* table, const psb_step* step, float grad_scale, void* stream_)
+{
+	int rc;
+	if (world < 1 || world > DP_MAX_WORLD || !records || !table || !step) {
+		set_error_msg("psb_exposure_apply: need 1 <= world <= 8, records, a table and a step");
+		return PSB_ERR_ARG;
+	}
+	if ((rc = check_table(table, false, "psb_exposure_apply"))) return rc;
+	if (!std::isfinite(grad_scale)) { set_error_msg("psb_exposure_apply: grad_scale must be finite"); return PSB_ERR_ARG; }
+	return launch_exposure_apply(records, EXP_REC, world, exposure_table(table), step->beta1, step->beta2, step->eps, grad_scale, nullptr,
+	                             (cudaStream_t)stream_);
 }
 
 int psb_trainer_backward_begin(psb_trainer* t, int P, int M, const psb_model* model, const psb_camera* camera, const float* background,

@@ -110,6 +110,15 @@ class _Exposure(C.Structure):
     _fields_ = [("param", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p), ("step", C.c_void_p), ("lr", C.c_float)]
 
 
+class _ExposureTable(C.Structure):
+    """psb_exposure_table: the replicated table of the data-parallel steps, this rank's row (-1: none) and the gradient modes' record."""
+    _fields_ = [("param", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p), ("step", C.c_void_p), ("K", C.c_int),
+                ("id", C.c_int), ("lr", C.c_float), ("record", C.c_void_p)]
+
+
+EXPOSURE_RECORD = 16   # floats of one rank's exposure record (PSB_EXPOSURE_RECORD)
+
+
 class _PixelGrads(C.Structure):
     _fields_ = [("dL_dcolor", C.c_void_p), ("dL_ddepth", C.c_void_p), ("dL_dalpha", C.c_void_p)]
 
@@ -216,6 +225,9 @@ def _bind():
         "psb_trainer_backward_begin": call + [vp],
         "psb_trainer_backward_begin_depth": call + [Depth, vp],
         "psb_trainer_backward_begin_dist": call + [Depth, P(_Normal), P(_Dn), P(_Dist), vp],
+        "psb_trainer_backward_begin_table": call + [Depth, P(_Normal), P(_Dn), P(_Dist), P(_ExposureTable), vp],
+        "psb_trainer_backward_table": call + [P(vp), Depth, P(_Normal), P(_Dn), P(_Dist), P(_ExposureTable), vp],
+        "psb_exposure_apply": [i, vp, P(_ExposureTable), Step, f, vp],
         "psb_trainer_backward_slab": [vp, i, i, Model, Cam, Step, i, i, P(vp), vp],
         "psb_trainer_result": [vp, P(f), P(i), vp],
         "psb_trainer_result_depth": [vp, P(f), P(i), vp],
@@ -247,6 +259,7 @@ def _bind():
         "psb_dp_step": [vp] + call + [vp],
         "psb_dp_step_depth": [vp] + call + [Depth, vp],
         "psb_dp_step_dist": [vp] + call + [Depth, P(_Normal), P(_Dn), P(_Dist), vp],
+        "psb_dp_step_table": [vp] + call + [Depth, P(_Normal), P(_Dn), P(_Dist), P(_ExposureTable), vp],
         "psb_dp_sync": [vp, vp],
         "psb_dp_status": [vp, vp],
         "psb_dp_destroy": [vp],
@@ -1378,12 +1391,19 @@ class DataParallelTrainer(GaussianTrainer):
     geometry_terms=True: trainForOneIteration takes the normal, depth-normal consistency and distortion arguments in every mode
         (psb_dp_step_dist, psb_trainer_backward_begin_dist, psb_trainer_backward_dist); each rank passes its own view's terms or none.
         Off (the default), those arguments raise NotImplementedError, as they always have, and every step makes the calls it made
-        before the terms existed."""
+        before the terms existed.
+    exposure=True: trainForOneIteration takes exposure_id in every mode (psb_dp_step_table, psb_trainer_backward_begin_table,
+        psb_trainer_backward_table + psb_exposure_apply). Every rank holds a replica of the model's exposure table; each step, every row
+        that some rank trained takes one Adam step from the mean of the ranks' gradients (the ranks' own exposure_lr_; the lowest rank's
+        where several trained one row), and the replicas stay bit-identical. The table is never grown here: call
+        model.ensureExposures(K) on every rank first; K is checked across the ranks when the trainer is built and on rebuild().
+        Off (the default), exposure_id raises NotImplementedError as it always has."""
 
     geometry_terms = False
+    exposure = False
 
     def __init__(self, model, opt=None, background=None, group=None, pipeline=None, nslabs=4, mode=None, deterministic=None,
-                 antialiasing=False, filter3d=False, geometry_terms=False):
+                 antialiasing=False, filter3d=False, geometry_terms=False, exposure=False):
         if filter3d:
             raise NotImplementedError("DataParallelTrainer: the 3D filter is not wired into the data-parallel steps (the NVLink push backward and "
                                       "the slab pipeline have no filtered variant); train with it on one GPU through GaussianTrainer(filter3d=True)")
@@ -1393,6 +1413,7 @@ class DataParallelTrainer(GaussianTrainer):
                                       "through GaussianTrainer")
         super().__init__(model, opt, background, deterministic=deterministic, antialiasing=antialiasing)
         self.geometry_terms = bool(geometry_terms)
+        self.exposure = bool(exposure)
         import os
         import torch.distributed as dist
         self.dist = dist
@@ -1422,6 +1443,23 @@ class DataParallelTrainer(GaussianTrainer):
                 self.mode = "nccl"
         if self.mode == "nccl":
             self._setup_nccl(pipeline, nslabs)
+        self._check_exposures()
+
+    def _check_exposures(self):
+        """exposure=True: every rank's table must have the same number of rows (a row id means the same keyframe on every rank)."""
+        if not self.exposure:
+            return
+        K = self.model.numExposures()
+        if self.world > 1:
+            t = torch.tensor([K, -K], device=self.model.device, dtype=torch.int64)
+            self.dist.all_reduce(t, op=self.dist.ReduceOp.MAX, group=self.group)
+            if int(t[0]) != -int(t[1]):
+                raise ValueError(f"DataParallelTrainer: the ranks' exposure tables differ in size (from {-int(t[1])} to {int(t[0])} rows): call "
+                                 "model.ensureExposures(K) with the same K on every rank")
+        self._exp_K = K
+        dev = self.model.device
+        self._exp_rec = torch.zeros(EXPOSURE_RECORD, device=dev)                       # this rank's record (slab and flat paths)
+        self._exp_recs = torch.zeros(self.world, EXPOSURE_RECORD, device=dev)          # every rank's, gathered
 
     # ---- p2p -----------------------------------------------------------------------------------------------------------
     def _setup_p2p(self):
@@ -1520,6 +1558,31 @@ class DataParallelTrainer(GaussianTrainer):
             self._setup_p2p()
         else:
             self._setup_nccl(self.pipeline, len(self.grads.slabs) if self.pipeline else 4)
+        self._check_exposures()
+
+    def _exposure_table(self, exposure_id):
+        """The psb_exposure_table of this rank's step (id -1 without exposure_id)."""
+        m = self.model
+        K = m.numExposures()
+        if K != self._exp_K:
+            raise ValueError(f"DataParallelTrainer: the exposure table has {K} rows, the trainer checked {self._exp_K} across the ranks: after "
+                             "model.ensureExposures(K) on every rank, call rebuild()")
+        k = -1
+        if exposure_id is not None:
+            k = int(exposure_id)
+            if k < 0 or k >= K:
+                raise ValueError(f"exposure_id must lie in [0, {K}), got {exposure_id}: the data-parallel table is not grown on demand; call "
+                                 "model.ensureExposures(K) on every rank first")
+        return _ExposureTable(m.exposure_.data_ptr(), m.exposure_exp_avg_.data_ptr(), m.exposure_exp_avg_sq_.data_ptr(), m.exposure_step_.data_ptr(),
+                              K, k, float(m.exposure_lr_), self._exp_rec.data_ptr())
+
+    def _apply_exposures(self, table, cs, stream):
+        """Slab and flat paths: every rank's record (one all-gather of world x 16 floats) -> the same table update on every rank."""
+        recs = self._exp_rec
+        if self.world > 1:
+            self.dist.all_gather_into_tensor(self._exp_recs, self._exp_rec, group=self.group)
+            recs = self._exp_recs
+        _lib.check(self.L.psb_exposure_apply(self.world, recs.data_ptr(), C.byref(table), C.byref(cs), 1.0 / self.world, stream), "psb_exposure_apply")
 
     # ---- nccl (round-1 path) -------------------------------------------------------------------------------------------
     def _setup_nccl(self, pipeline, nslabs):
@@ -1545,7 +1608,9 @@ class DataParallelTrainer(GaussianTrainer):
         (psb_trainer_backward_begin_depth) and the flat "nccl" path (psb_trainer_backward_depth). With geometry_terms=True also the normal,
         depth-normal consistency and distortion arguments, on every path: "p2p" (psb_dp_step_dist), the slab pipeline
         (psb_trainer_backward_begin_dist) and the flat "nccl" path (psb_trainer_backward_dist). Each rank passes its own view's terms or
-        none: ranks with different terms may train in the same step. exposure_id must be None."""
+        none: ranks with different terms may train in the same step. exposure_id needs exposure=True (psb_dp_step_table,
+        psb_trainer_backward_begin_table, psb_trainer_backward_table): the keyframe id k of gt_image, < model.numExposures(), or None for
+        a view without exposure; the row trains as in GaussianTrainer, from the mean of every rank's gradient."""
         if not self.geometry_terms:
             how = "; construct DataParallelTrainer(..., geometry_terms=True) to train it on the data-parallel steps"
             if gt_normal is not None or out_normal is not None or lambda_normal:
@@ -1554,10 +1619,10 @@ class DataParallelTrainer(GaussianTrainer):
                 raise NotImplementedError("DataParallelTrainer: the depth-normal consistency term is off on this trainer" + how)
             if lambda_dist or out_depth2 is not None:
                 raise NotImplementedError("DataParallelTrainer: the depth distortion term is off on this trainer" + how)
-        if exposure_id is not None:
-            raise NotImplementedError("DataParallelTrainer: exposure compensation is not wired into the data-parallel steps: the per-keyframe "
-                                      "exposure table would have to be replicated across the ranks (each rank's row updates gathered to "
-                                      "every rank every step); train with exposure on one GPU through GaussianTrainer")
+        if exposure_id is not None and not self.exposure:
+            raise NotImplementedError("DataParallelTrainer: exposure compensation is off on this trainer: the per-keyframe exposure table is "
+                                      "replicated across the ranks only with DataParallelTrainer(..., exposure=True) (or train with exposure "
+                                      "on one GPU through GaussianTrainer)")
         m = self.model
         built = self._dp_P if self.mode == "p2p" else self.grads.P
         if built != m.num_points():
@@ -1568,6 +1633,7 @@ class DataParallelTrainer(GaussianTrainer):
         normal = _cnormal(gt_normal, lambda_normal, out_normal, H, W)
         dn = _cdn(lambda_dn, dn_alpha_min, dn_max_rel_jump, out_depth_normal, H, W)
         dist = _cdist(lambda_dist, out_depth2, H, W)
+        table = self._exposure_table(exposure_id) if self.exposure else None
         self._apply_deterministic()
         self.iteration += 1
         if densify_stats is None:
@@ -1582,20 +1648,28 @@ class DataParallelTrainer(GaussianTrainer):
         terms = (byref(normal), byref(dn), byref(dist))
         geo = self.geometry_terms
         if self.mode == "p2p":
-            if geo:
+            if table is not None:
+                _lib.check(self.L.psb_dp_step_table(self.h, self.dp, *args[1:], cdepth, *terms, C.byref(table), stream), "psb_dp_step_table")
+            elif geo:
                 _lib.check(self.L.psb_dp_step_dist(self.h, self.dp, *args[1:], cdepth, *terms, stream), "psb_dp_step_dist")
             else:
                 _lib.check(self.L.psb_dp_step_depth(self.h, self.dp, *args[1:], cdepth, stream), "psb_dp_step_depth")
         elif not self.pipeline:
             ptrs = (C.c_void_p * 6)(*[s.data_ptr() for s in self.segs])
-            if geo:
+            if table is not None:
+                _lib.check(self.L.psb_trainer_backward_table(*args, ptrs, cdepth, *terms, C.byref(table), stream), "psb_trainer_backward_table")
+            elif geo:
                 _lib.check(self.L.psb_trainer_backward_dist(*args, ptrs, cdepth, None, None, *terms, stream), "psb_trainer_backward_dist")
             else:
                 _lib.check(self.L.psb_trainer_backward_depth(*args, ptrs, cdepth, stream), "psb_trainer_backward_depth")
             scale = self.grads.all_reduce(self.group)   # ONE collective per step: 59 floats per Gaussian
             _lib.check(self.L.psb_adam_update(P, 16, C.byref(cm), ptrs, C.byref(cs), scale, stream), "psb_adam_update")
+            if table is not None:
+                self._apply_exposures(table, cs, stream)
         else:
-            if geo:
+            if table is not None:
+                _lib.check(self.L.psb_trainer_backward_begin_table(*args, cdepth, *terms, C.byref(table), stream), "psb_trainer_backward_begin_table")
+            elif geo:
                 _lib.check(self.L.psb_trainer_backward_begin_dist(*args, cdepth, *terms, stream), "psb_trainer_backward_begin_dist")
             else:
                 _lib.check(self.L.psb_trainer_backward_begin_depth(*args, cdepth, stream), "psb_trainer_backward_begin_depth")
@@ -1618,6 +1692,8 @@ class DataParallelTrainer(GaussianTrainer):
                     o = first * k
                     _lib.check(self.L.psb_adam_flat(count * k, p[o:].data_ptr(), a[o:].data_ptr(), b[o:].data_ptr(), blk.data_ptr(), m.lr_[i],
                                                     C.byref(cs), scale, stream), "psb_adam_flat")
+            if table is not None:
+                self._apply_exposures(table, cs, stream)
         m.step_ += 1
         m.invalidateAdamLive()   # these steps write moments without maintaining the live bytes (and p2p: only on the owner rank)
 
